@@ -2,10 +2,11 @@
 """bench.py -- headline benchmark: Mpixels/s for thumbnail(4K -> 512, lanczos3).
 
 Workload = BASELINE.json configs[1]: vips_thumbnail 4096x4096 uchar RGBA -> 512x512,
-a batch of 1024 synthetic frames per GPU (64 GiB resident in HBM, >> the 126 MB L2).  A "step" is
-one pass of the fused thumbnail kernel over the whole batch, frames resident in HBM.
+a batch of 512 synthetic frames per GPU (32 GiB resident in the H100's 80 GB of HBM, >> the 50 MB L2).  A "step"
+is one pass of the fused thumbnail kernel over the whole batch, frames resident in HBM.
 
   python bench.py --gpus N --steps K --warmup W            (torchrun for N > 1)
+  python bench.py ... --dump-outputs DIR                    also write the last timed step's outputs as DIR/<name>.npy
   python bench.py --impl reference ...                      CPU arm (the oracle port
                                                             of the reference algorithm)
 
@@ -30,10 +31,6 @@ TARGET = 512
 MPIX_PER_FRAME = W * H / 1e6
 METRIC = "Mpixels/s for thumbnail(4K->512,lanczos3)"
 METRIC_PIPELINE = "Mpixels/s for thumbnail(4K->512,lanczos3) + sharpen + sRGB (BASELINE config 5 stream)"
-# dram__bytes_read.sum + dram__bytes_write.sum of the fused kernel per 4096x4096 frame, from the
-# committed `ncu --set full` capture (a launch of 148 frames: 10.1220 GB read, 159.4 MB written)
-DRAM_BYTES_PER_FRAME = (10.124448e9 + 161.176576e6) / 148
-DRAM_SOURCE = "profiles/r2/headline_random_alpha_ncu_summary.txt (ncu --set full, 148 frames: per frame x frames in the launch)"
 WORKLOAD = "vips_thumbnail 4K->512 uchar RGBA (premultiply,shrinkv4,reducev13,shrinkh4,reduceh13,unpremultiply), synthetic frames, device-resident"
 WORKLOAD_PIPELINE = ("vips_thumbnail 4K->512 uchar RGBA then vips_sharpen (sRGB->LabS, 3-tap integer blur of L, LUT, LabS->sRGB) on the 512x512 "
                      "result, synthetic frames, device-resident")
@@ -47,7 +44,30 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
+
+
+DUMP_BYTES = 64 * 10**6  # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(d, arrays):
+    """Write each output as d/<name>.npy in float32 (float64 stays float64).  An array larger than its share of
+    DUMP_BYTES is sampled along its first axis (frames, or rows of one image) at indices fixed by a seed, and those
+    indices go beside it as d/<name>_index.npy, so that two builds run with the same arguments compare entry for entry."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    share = DUMP_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        t = t if torch.is_tensor(t) else torch.from_numpy(np.ascontiguousarray(t))
+        dt = torch.float64 if t.dtype == torch.float64 else torch.float32
+        per = t[0].numel() * (8 if dt == torch.float64 else 4) if t.dim() else 4
+        if t.dim() and per * t.shape[0] > share:
+            keep = max(1, share // per)
+            idx = np.sort(np.random.default_rng(20240601).choice(t.shape[0], keep, replace=False))
+            np.save(os.path.join(d, name + "_index.npy"), idx.astype(np.float64))
+            t = t[torch.from_numpy(idx).to(t.device)]
+        np.save(os.path.join(d, name + ".npy"), t.to(dt).cpu().numpy())
 
 
 class ClockSampler:
@@ -134,7 +154,7 @@ class CpuArm:
         if os.environ.get("VB200_CPU_ARM") != "port":
             try:
                 from oracle import pyref
-                if pyref.available():
+                if pyref.live():
                     import multiprocessing as mp
                     _REF_FRAMES = self.a                      # inherited by fork: no copies, no pickling
                     self.pool = mp.get_context("fork").Pool(threads)
@@ -281,6 +301,7 @@ def side_workload(args):
 
     vb.init(0)
     dev = torch.device("cuda", 0)
+    torch.manual_seed(1234)  # the same inputs on every run: --dump-outputs of two builds compare
     stream = torch.cuda.current_stream()
     vb.set_stream(stream.cuda_stream)
     L = vb.lib()
@@ -301,7 +322,7 @@ def side_workload(args):
         dt = time.perf_counter() - t
         return {"value": units / dt, "unit": "Mpixels/s", "cores": 1, "kind": "port", "sample": "%s, %.1f s" % (sample, dt)}
 
-    def run(fn, alg_bytes, label, units, unit_name, cpu=None):
+    def run(fn, alg_bytes, label, units, unit_name, cpu=None, outputs=None):
         for _ in range(args.warmup):
             fn()
         torch.cuda.synchronize()
@@ -312,6 +333,8 @@ def side_workload(args):
             fn()
         e1.record(stream)
         torch.cuda.synchronize()
+        if args.dump_outputs and outputs:
+            dump_outputs(args.dump_outputs, outputs)
         ms = e0.elapsed_time(e1) / args.steps
         ach = alg_bytes / (ms / 1e3) / 1e9
         print(json.dumps({"metric": label, "value": units / (ms / 1e3), "unit": unit_name, "n_gpus": 1,
@@ -337,7 +360,8 @@ def side_workload(args):
         from oracle import pyconv
         ca = (np.random.default_rng(1234).random((2048, 2048, 3), dtype=np.float32) * 255)
         cpu = cpu_side(lambda: pyconv.convsep(ca, m, scale, off, "float"), 2048 * 2048 / 1e6, "2048x2048x3 float32")
-        run(fn, 2 * a.numel() * 4, "vips_convsep 15-tap Gaussian float on 8192x8192 RGB float32", n * n / 1e6, "Mpixels/s", cpu)
+        run(fn, 2 * a.numel() * 4, "vips_convsep 15-tap Gaussian float on 8192x8192 RGB float32", n * n / 1e6, "Mpixels/s", cpu,
+            {"convsep": out})
     elif args.workload == "colour":
         n = 16384
         a = torch.randint(0, 256, (n, n, 3), dtype=torch.uint8, device=dev)
@@ -359,7 +383,7 @@ def side_workload(args):
         cpu = cpu_side(lambda: pyoracle.colourspace(pyoracle.colourspace(ca, "lab", "srgb"), "srgb", "lab"),
                        2 * 2048 * 2048 / 1e6, "2048x2048x3 uint8, both directions")
         run(fn, 2 * (a.numel() + lab.numel() * 4), "vips_colourspace sRGB->Lab->sRGB round trip on 16384x16384",
-            2 * n * n / 1e6, "Mpixels/s", cpu)
+            2 * n * n / 1e6, "Mpixels/s", cpu, {"lab": lab, "srgb": back})
     elif args.workload == "reduce49":
         n = 4096
         a = torch.randint(0, 256, (n, n, 4), dtype=torch.uint8, device=dev)
@@ -374,7 +398,7 @@ def side_workload(args):
         cpu = cpu_side(lambda: pyoracle.reduceh(pyoracle.reducev(ca, 8.0, "lanczos3", 0.0), 8.0, "lanczos3", 0.0),
                        n * n / 1e6, "one 4096x4096 RGBA frame")
         run(fn, a.numel() + out.numel(), "vips_reduce(8, 8) Lanczos3 gap 0 (49 taps) on one 4096x4096 uchar RGBA",
-            n * n / 1e6, "Mpixels/s", cpu)
+            n * n / 1e6, "Mpixels/s", cpu, {"reduce": out})
     elif args.workload == "upsize":
         # SURVEY 8(a) a7: vips_resize x2 = vips_affine + bicubic (resize.c:235-305)
         n = 4096
@@ -389,7 +413,7 @@ def side_workload(args):
         ca = np.random.default_rng(1234).integers(0, 256, (1024, 1024, 4), dtype=np.uint8)
         cpu = cpu_side(lambda: pyoracle.resize(ca, 2.0), 4 * 1024 * 1024 / 1e6, "1024x1024 RGBA -> 2048x2048")
         run(fn, a.numel() + out.numel(), "vips_resize x2 (affine + bicubic) 4096x4096 uchar RGBA -> 8192x8192",
-            4 * n * n / 1e6, "output Mpixels/s", cpu)
+            4 * n * n / 1e6, "output Mpixels/s", cpu, {"resize": out})
     elif args.workload == "sharpen":
         # SURVEY 8(a) a11: vips_sharpen defaults on an sRGB image (sRGB -> LabS, L blur + LUT, LabS -> sRGB)
         n = 4096
@@ -403,7 +427,7 @@ def side_workload(args):
         from oracle import pyconv
         ca = np.random.default_rng(1234).integers(0, 256, (1024, 1024, 3), dtype=np.uint8)
         cpu = cpu_side(lambda: pyconv.sharpen(ca, "srgb"), 1024 * 1024 / 1e6, "1024x1024 RGB")
-        run(fn, 2 * a.numel(), "vips_sharpen defaults on 4096x4096 sRGB uchar", n * n / 1e6, "Mpixels/s", cpu)
+        run(fn, 2 * a.numel(), "vips_sharpen defaults on 4096x4096 sRGB uchar", n * n / 1e6, "Mpixels/s", cpu, {"sharpen": out})
     elif args.workload == "thumbnail_linear":
         # north_star's "fused Lanczos3-reduce -> sRGB -> linear" path: vips_thumbnail_image(linear=TRUE), SURVEY 3.1b
         F = max(1, min(args.frames, 128))
@@ -426,7 +450,7 @@ def side_workload(args):
         ca = np.random.default_rng(7).integers(0, 256, (H, W, BANDS), dtype=np.uint8)
         cpu = cpu_side(lambda: pyoracle.thumbnail_image(ca, TARGET, linear=True), W * H / 1e6, "one 4096x4096 RGBA frame")
         run(fn, plan.bytes_per_frame * F, "vips_thumbnail_image(linear=TRUE) 4K->512 uchar RGBA, %d frames (%s)" % (F, plan.kernel),
-            F * W * H / 1e6, "Mpixels/s", cpu)
+            F * W * H / 1e6, "Mpixels/s", cpu, {"thumbnails": outs})
     elif args.workload == "icc":
         # SURVEY 8(a) a20: vips_icc_import then vips_icc_export through an sRGB-like v4 matrix/TRC profile
         sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -455,9 +479,9 @@ def side_workload(args):
                            "2048x2048x3 uint8 through lcms2 2.18 itself, both directions")
             cpu["kind"] = "reference"
         run(fn, 2 * (a.numel() + lab.numel() * 4), "vips_icc_import + vips_icc_export (sRGB-like v4 profile) on 8192x8192",
-            2 * n * n / 1e6, "Mpixels/s", cpu)
+            2 * n * n / 1e6, "Mpixels/s", cpu, {"lab": lab, "srgb": back})
     elif args.workload in ("rank", "flatten", "greyscale"):
-        # SURVEY 8f ranks 3 / 4 (DESIGN 4.10-4.12): parity-green in round 2, never timed there (the GPU budget was spent)
+        # SURVEY 8f ranks 3 / 4 (DESIGN 4.10-4.12): vips_median, vips_flatten and sRGB -> B_W, device-resident
         n = 4096
         from oracle import pyconv
         rng = np.random.default_rng(1234)
@@ -471,7 +495,7 @@ def side_workload(args):
                 vb._check(L.vb200_rank(C.byref(cin), C.byref(cout), 3, 3, 4))
             ca = rng.integers(0, 256, (1024, 1024, 3), dtype=np.uint8)
             cpu = cpu_side(lambda: pyconv.median(ca, 3), 1024 * 1024 / 1e6, "1024x1024 RGB")
-            run(fn, 2 * a.numel(), "vips_median 3x3 on 4096x4096 sRGB uchar", n * n / 1e6, "Mpixels/s", cpu)
+            run(fn, 2 * a.numel(), "vips_median 3x3 on 4096x4096 sRGB uchar", n * n / 1e6, "Mpixels/s", cpu, {"median": out})
         elif args.workload == "flatten":
             a = torch.randint(0, 256, (n, n, 4), dtype=torch.uint8, device=dev)
             out = torch.empty((n, n, 3), dtype=torch.uint8, device=dev)
@@ -483,7 +507,8 @@ def side_workload(args):
                 vb._check(L.vb200_flatten(C.byref(cin), C.byref(cout), bg, 3, 0.0))
             ca = rng.integers(0, 256, (1024, 1024, 4), dtype=np.uint8)
             cpu = cpu_side(lambda: pyconv.flatten(ca, (255, 255, 255)), 1024 * 1024 / 1e6, "1024x1024 RGBA")
-            run(fn, a.numel() + out.numel(), "vips_flatten (white background) on 4096x4096 RGBA uchar", n * n / 1e6, "Mpixels/s", cpu)
+            run(fn, a.numel() + out.numel(), "vips_flatten (white background) on 4096x4096 RGBA uchar", n * n / 1e6, "Mpixels/s", cpu,
+                {"flatten": out})
         else:
             from oracle import pyoracle
             a = torch.randint(0, 256, (n, n, 3), dtype=torch.uint8, device=dev)
@@ -495,7 +520,8 @@ def side_workload(args):
                 vb._check(L.vb200_colourspace(C.byref(cin), C.byref(cout), 1))
             ca = rng.integers(0, 256, (1024, 1024, 3), dtype=np.uint8)
             cpu = cpu_side(lambda: pyoracle.colourspace(ca, "b-w", "srgb"), 1024 * 1024 / 1e6, "1024x1024 RGB")
-            run(fn, a.numel() + out.numel(), "vips_colourspace sRGB -> B_W on 4096x4096 uchar", n * n / 1e6, "Mpixels/s", cpu)
+            run(fn, a.numel() + out.numel(), "vips_colourspace sRGB -> B_W on 4096x4096 uchar", n * n / 1e6, "Mpixels/s", cpu,
+                {"greyscale": out})
     elif args.workload in ("thumbnail_jpeg", "thumbnail_jpeg_norestart", "thumbnail_jpeg_progressive"):
         # SURVEY 8(f) rank 1: vips_thumbnail_buffer() of JPEG streams.  Host memory holds only the COMPRESSED frames; the
         # shrink-on-load decode (thumbnail.c:489-517 picks 1/4 for 4K -> 512) and the thumbnail run on the device.
@@ -559,6 +585,8 @@ def side_workload(args):
             fn()
         torch.cuda.synchronize()
         dt = (time.perf_counter() - t0) / args.steps
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"thumbnails": outs})
         cpu = None
         if not args.no_cpu:
             import multiprocessing as mp
@@ -596,7 +624,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
-    ap.add_argument("--frames", type=int, default=1024, help="synthetic frames resident per GPU")
+    ap.add_argument("--frames", type=int, default=512, help="synthetic frames resident per GPU")
     ap.add_argument("--e2e-frames", type=int, default=24, help="host frames per end-to-end step")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--save", action="store_true",
@@ -609,6 +637,11 @@ def main():
                     help="thumbnail (the headline, default) | pipeline (BASELINE config 5: thumbnail + sharpen + sRGB, runs under "
                          "--gpus N like the headline) | thumbnail_jpeg | thumbnail_jpeg_norestart | thumbnail_jpeg_progressive (decode staging, SURVEY 8f; --save adds the encoder) | thumbnail_linear | convsep | colour | reduce49 | upsize | sharpen | icc | rank | flatten | greyscale: the other BASELINE.json "
                          "configs, one device-resident JSON line each (1 GPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32, at most 64 MB in "
+                         "all: a seeded sample of frames or rows of a larger output, its indices in DIR/<name>_index.npy).  "
+                         "thumbnail_jpeg workloads write the thumbnail pixels, also under --save, where a caller receives "
+                         "the JPEG streams encoded from them")
     args = ap.parse_args()
 
     global PIPELINE
@@ -716,6 +749,8 @@ def main():
     barrier()
     ev_mid[:] = []
     launches = vb.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"thumbnails": outs})
     clocks = sampler.stop() if rank == 0 else None
     total_ms = evs[0].elapsed_time(evs[-1])
     per_step = [evs[i].elapsed_time(evs[i + 1]) for i in range(args.steps)]
@@ -768,7 +803,7 @@ def main():
         for _ in range(2):
             plan.run_host_ptr(hin, hout, E)
         barrier()
-        n_e2e = max(3, min(args.steps, 10))
+        n_e2e = args.steps
         t0 = time.perf_counter()
         for _ in range(n_e2e):
             plan.run_host_ptr(hin, hout, E)
@@ -811,7 +846,7 @@ def main():
                        "output": "512x512x4 u8", "l2": "inputs (%.1f GiB per GPU) larger than L2" % (F * plan.in_frame_bytes / 2**30),
                        "sharding": "independent frames per rank, no data-path collective"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": DRAM_BYTES_PER_FRAME * F, "traffic_source": DRAM_SOURCE, "peak_source": peak_src,
+                         "traffic": None, "peak_source": peak_src,
                          "kernel": plan.kernel, "bytes_per_launch": bytes_per_launch, "kernel_ms": kern_ms, "kernels": kernels},
             "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
         }

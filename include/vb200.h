@@ -1,4 +1,4 @@
-/* vb200.h -- C ABI of libvb200.so, the sm_100a replacement for libvips'
+/* vb200.h -- C ABI of libvb200.so, the sm_90a (H100) replacement for libvips'
  * per-tile pixel hot path (resample / convolution / colour generate callbacks).
  *
  * Plain C, plain pointers and sizes.  Every entry point returns 0 on success

@@ -1,5 +1,5 @@
 """libvips_b200 -- Python mirror of the libvips operator interface for the
-B200-native pixel hot path, bound over the C ABI of libvb200.so (include/vb200.h).
+H100-native pixel hot path, bound over the C ABI of libvb200.so (include/vb200.h).
 
 The class and method names follow pyvips / the libvips C API
 (vips_reducev, vips_resize, vips_thumbnail_image, vips_conv, vips_colourspace ...)

@@ -2142,7 +2142,7 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 	if (const char *e = getenv("VB200_JPEG_CHUNK"))
 		if (atoi(e) > 0)
 			chunk = atoi(e);
-	long long huff_cta_slots = 148 * 32; /* resident CTAs: 32 per SM */
+	long long huff_cta_slots = (long long) sm_count() * 32; /* resident CTAs: 32 per SM */
 	if (const char *e = getenv("VB200_JPEG_CTAS"))
 		if (atoll(e) > 0)
 			huff_cta_slots = atoll(e);

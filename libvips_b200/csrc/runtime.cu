@@ -26,6 +26,7 @@ static thread_local std::string g_error;
 static thread_local cudaStream_t g_stream = nullptr;
 static std::atomic<uint64_t> g_launches{0};
 static std::atomic<int> g_device{-1};
+static std::atomic<int> g_sm_count{132};
 static std::mutex g_init_lock;
 /* reference: VIPS__TILE_WIDTH/HEIGHT 128, FATSTRIP 16, THINSTRIP 1,
  * include/vips/private.h:147-153
@@ -68,6 +69,12 @@ void
 count_launch(int n)
 {
 	g_launches.fetch_add(n, std::memory_order_relaxed);
+}
+
+int
+sm_count()
+{
+	return g_sm_count.load(std::memory_order_relaxed);
 }
 
 TileGeometry
@@ -364,8 +371,8 @@ vb200_init(int device)
 	VB200_CUDA("vb200_init", cudaSetDevice(device));
 	cudaDeviceProp prop;
 	VB200_CUDA("vb200_init", cudaGetDeviceProperties(&prop, device));
-	if (prop.major < 10) {
-		error("vb200_init", "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major,
+	if (prop.major != 9 || prop.minor != 0) {
+		error("vb200_init", "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
 			prop.minor);
 		return -1;
 	}
@@ -375,6 +382,7 @@ vb200_init(int device)
 		uint64_t threshold = UINT64_MAX;
 		cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &threshold);
 	}
+	g_sm_count.store(prop.multiProcessorCount);
 	g_device.store(device);
 	t_bound_device = device;
 	return 0;

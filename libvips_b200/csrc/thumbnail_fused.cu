@@ -1829,7 +1829,7 @@ launch_mma(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is,
 	const int K = fp.mma_rows;
 	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
 	int rpc = ((pl->OH + K - 1) / K) * K;
-	const int ctas = pl->mma_cols > 448 ? 148 : 2 * 148;
+	const int ctas = pl->mma_cols > 448 ? sm_count() : 2 * sm_count();
 	while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < ctas && rpc > 4 * K)
 		rpc = ((rpc / 2 + K - 1) / K) * K;
 	fp.RPC = rpc;
@@ -1867,7 +1867,7 @@ launch_tma(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is,
 	const int K = kChunkRowsTma;
 	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
 	int rpc = ((pl->OH + K - 1) / K) * K;
-	while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * 148 && rpc > 4 * K)
+	while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * sm_count() && rpc > 4 * K)
 		rpc = ((rpc / 2 + K - 1) / K) * K;
 	fp.RPC = rpc;
 	const dim3 grid(bands_x, (pl->OH + rpc - 1) / rpc, 1);
@@ -2481,7 +2481,7 @@ thumbnail_plan_run_fused(const char *domain, ThumbnailPlanImpl *pl, const void *
 		FusedParams &fp = pl->fp;
 		const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
 		int rpc = ((pl->OH + kChunkRows - 1) / kChunkRows) * kChunkRows;
-		while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * 148 && rpc > 2 * kChunkRows)
+		while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * sm_count() && rpc > 2 * kChunkRows)
 			rpc = ((rpc / 2 + kChunkRows - 1) / kChunkRows) * kChunkRows;
 		fp.RPC = rpc;
 		pl->grid = dim3(bands_x, (pl->OH + rpc - 1) / rpc, 1);

@@ -684,7 +684,7 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		/* rows per CTA: the whole height when there are enough frames to fill the machine */
 		const int col_blocks = (lt->W + kVThreads - 1) / kVThreads;
 		int splits = 1;
-		while ((long) col_blocks * splits * nf < 4 * 148 && lt->OH / (splits * 2) >= 16)
+		while ((long) col_blocks * splits * nf < 4 * sm_count() && lt->OH / (splits * 2) >= 16)
 			splits *= 2;
 		v.RPC = (lt->OH + splits - 1) / splits;
 		const dim3 gv(col_blocks, (lt->OH + v.RPC - 1) / v.RPC, nf);

@@ -33,6 +33,7 @@ int cuda_fail(const char *domain, cudaError_t e, const char *what);
 
 cudaStream_t current_stream();
 void count_launch(int n = 1);
+int sm_count(); /* SMs of the device vb200_init selected: grid sizing fills the machine */
 int ensure_init(const char *domain);
 
 struct TileGeometry {

@@ -117,6 +117,7 @@ def _rl():
     return L
 
 
+@pyref.recorded
 def ref_conv(a, mask, scale=1.0, offset=0.0, precision="float", vector=False, tile=(0, 0)):
     L = _rl()
     mask = np.ascontiguousarray(mask, np.float64)
@@ -128,6 +129,7 @@ def ref_conv(a, mask, scale=1.0, offset=0.0, precision="float", vector=False, ti
     return out.numpy(tile)
 
 
+@pyref.recorded
 def ref_gaussmat(sigma, min_ampl, separable=False, precision="integer"):
     L = _rl()
     m = L.ref_gaussmat(sigma, min_ampl, int(separable), _prec(precision))
@@ -138,6 +140,7 @@ def ref_gaussmat(sigma, min_ampl, separable=False, precision="integer"):
     return data.reshape(h, w).copy(), L.ref_matrix_scale(m), L.ref_matrix_offset(m)
 
 
+@pyref.recorded
 def ref_convsep(a, mask, scale=1.0, offset=0.0, precision="float", tile=(0, 0)):
     """vips_convsep through the reference's own convsep.c / conv.c / rot.c / convf.c / convi.c"""
     L = _rl()
@@ -151,6 +154,7 @@ def ref_convsep(a, mask, scale=1.0, offset=0.0, precision="float", tile=(0, 0)):
     return pyref.RefImage(L.ref_convsep(im.h, m, _prec(precision)), (im, mask)).numpy(tile)
 
 
+@pyref.recorded
 def ref_sharpen(a, interpretation, sigma=0.5, x1=2.0, y2=10.0, y3=20.0, m1=0.0, m2=3.0, tile=(0, 0)):
     """vips_sharpen through the reference's own sharpen.c (build + generate), 3-band images"""
     L = _rl()
@@ -160,6 +164,7 @@ def ref_sharpen(a, interpretation, sigma=0.5, x1=2.0, y2=10.0, y3=20.0, m1=0.0, 
     return pyref.RefImage(L.ref_sharpen(im.h, sigma, x1, y2, y3, m1, m2), (im,)).numpy(tile)
 
 
+@pyref.recorded
 def ref_sharpen_lut(sigma=0.5, x1=2.0, y2=10.0, y3=20.0, m1=0.0, m2=3.0):
     L = _rl()
     L.ref_sharpen_lut.argtypes = [C.c_double] * 6 + [C.c_void_p]
@@ -192,6 +197,7 @@ def morph(a, mask, op):
     return out
 
 
+@pyref.recorded
 def ref_morph(a, mask, op, tile=(0, 0)):
     """vips_morph through the reference's own morph.c (C generate functions)"""
     L = _rl()
@@ -219,6 +225,7 @@ def median(a, size):
     return rank(a, size, size, (size * size) // 2)
 
 
+@pyref.recorded
 def ref_rank(a, width, height, index, tile=(0, 0)):
     """vips_rank through the reference's own morphology/rank.c"""
     L = _rl()
@@ -228,6 +235,7 @@ def ref_rank(a, width, height, index, tile=(0, 0)):
     return pyref.RefImage(L.ref_rank(im.h, width, height, index), (im,)).numpy(tile)
 
 
+@pyref.recorded
 def ref_flatten(a, background=(0.0,), max_alpha=0.0, interpretation=None, tile=(0, 0)):
     """vips_flatten through the reference's own conversion/flatten.c (+ cast.c for the ink and the double detour)"""
     L = _rl()

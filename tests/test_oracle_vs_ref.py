@@ -32,7 +32,7 @@ def rand_image(rng, h, w, b, dt):
 
 def same(a, b):
     assert a.shape == b.shape and a.dtype == b.dtype, (a.shape, b.shape, a.dtype, b.dtype)
-    assert np.array_equal(a, b), "max diff %g" % np.abs(a.astype(np.float64) - b.astype(np.float64)).max()
+    assert np.array_equal(a, b), pyref.difference(a, b)
 
 
 @pytest.mark.parametrize("kernel", KERNELS)
@@ -151,21 +151,17 @@ def test_thumbnail_size_arithmetic():
     dims += [tuple(int(v) for v in rng.integers(1, 9000, 2)) for _ in range(300)]
     targets = [(512, None), (1, None), (7, 9000), (9000, 7), (300, 300), (1024, 1025), (100000, 2)]
     targets += [tuple(int(v) for v in rng.integers(1, 5000, 2)) for _ in range(40)]
-    n = 0
-    for (w, h) in dims:
-        for (tw, th) in targets:
-            for size in ("both", "up", "down", "force"):
-                hs, vs = pyref.thumbnail_calculate_shrink(w, h, tw, th, size)
-                # the shrinks are written before the resize geometry is worked out (which declines mixed up / down sizes)
-                ohs, ovs, ow, oh = C.c_double(), C.c_double(), C.c_int(), C.c_int()
-                orc.lib().orc_thumbnail_size(w, h, tw, tw if th is None else th, orc.SIZES[size], C.byref(ohs), C.byref(ovs),
-                                             C.byref(ow), C.byref(oh))
-                assert (hs, vs) == (ohs.value, ovs.value), (w, h, tw, th, size)
-                want = pyref.thumbnail_find_jpegshrink(w, h, tw, th, size)
-                assert vb.thumbnail_jpegshrink(w, h, tw, th, size) == want, (w, h, tw, th, size)
-                assert pyref.thumbnail_find_jpegshrink(w, h, tw, th, size, linear=True) == 1
-                n += 1
-    assert n > 50000
+    cases = [(w, h, tw, th, size) for (w, h) in dims for (tw, th) in targets for size in ("both", "up", "down", "force")]
+    got = []
+    for (w, h, tw, th, size) in cases:
+        # the shrinks are written before the resize geometry is worked out (which declines mixed up / down sizes)
+        ohs, ovs, ow, oh = C.c_double(), C.c_double(), C.c_int(), C.c_int()
+        orc.lib().orc_thumbnail_size(w, h, tw, tw if th is None else th, orc.SIZES[size], C.byref(ohs), C.byref(ovs),
+                                     C.byref(ow), C.byref(oh))
+        got.append((ohs.value, ovs.value, vb.thumbnail_jpegshrink(w, h, tw, th, size), 1))
+    # columns: hshrink, vshrink, jpegshrink, jpegshrink with linear (always 1)
+    assert np.array_equal(np.array(got, np.float64), pyref.thumbnail_size_table(cases))
+    assert len(cases) > 50000
 
 
 def test_thumbnail_chain_tile_geometries():

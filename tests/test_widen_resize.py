@@ -31,11 +31,7 @@ def test_oracle_nearest_resize_subsamples_like_the_reference():
         want = pyref.RefImage.from_array(a).resize(0.2, 0.3, "nearest", gap).numpy()
         assert np.array_equal(orc.resize(a, 0.2, 0.3, "nearest", gap), want), gap
     # subsample.c itself: out(x, y) = in(x * xfac, y * yfac), size rounded down
-    L = pyref.lib()
-    L.ref_subsample.restype = __import__("ctypes").c_void_p
-    L.ref_subsample.argtypes = [__import__("ctypes").c_void_p, __import__("ctypes").c_int, __import__("ctypes").c_int]
-    im = pyref.RefImage.from_array(a)
-    sub = pyref.RefImage(L.ref_subsample(im.h, 7, 4), (im,)).numpy()
+    sub = pyref.RefImage.from_array(a).subsample(7, 4).numpy()
     assert np.array_equal(sub, a[:88:4, :119:7][:90 // 4, :120 // 7])
 
 

@@ -1,4 +1,4 @@
-"""tools/kernel_resources.py -- profiles/r2/kernel_resources.txt: `cuobjdump -res-usage` of the shipped libvb200.so, demangled,
+"""tools/kernel_resources.py -- `cuobjdump -res-usage` of the shipped libvb200.so, demangled,
 one line per kernel instantiation (registers, per-thread stack, static shared memory, local-memory spills)."""
 import re
 import subprocess
@@ -16,7 +16,7 @@ for name, r in zip(names, rows):
     name = re.sub(r"^void ", "", name)
     name = re.sub(r"\(.*$", "", name)
     out.append("%-100s REG %3d  STACK %5d  SHARED %6d  LOCAL %d" % (name, r[1], r[2], r[3], r[4]))
-print("# cuobjdump -res-usage %s (sm_100a), demangled, one line per kernel instantiation (tools/kernel_resources.py)." % so)
+print("# cuobjdump -res-usage %s (sm_90a), demangled, one line per kernel instantiation (tools/kernel_resources.py)." % so)
 print("# LOCAL 0 everywhere: no register spills; STACK > 0 is a per-thread array the kernel declares (the 8x8 DCT workspaces, the ICC")
 print("# evaluator's stage buffer) or the frame of a called slow path (double division), not a spill.")
 print("\n".join(sorted(set(out))))

@@ -3,7 +3,7 @@
  * band of COLS pixel columns of one 4096x4096 RGBA frame and streams it top to bottom,
  * ROWS rows per stage through an S-deep mbarrier ring; consumer warps only touch one word
  * per row and release the stage.  Prints GB/s for a sweep of (COLS, ROWS, S, CTAs/SM).
- *   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tma_feed_bench tma_feed_bench.cu
+ *   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tma_feed_bench tma_feed_bench.cu
  */
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -20,7 +20,7 @@ __global__ void k(int *out, int spin)
 }
 int main()
 {
-	int n = 148 * 2 * 3;
+	int n = 132 * 2 * 3; /* H100: 132 SMs */
 	int *d, *h = new int[n * 16];
 	cudaMalloc(&d, n * 16 * 4);
 	cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 107 * 1024);
