@@ -71,15 +71,18 @@ sfr(int v)
  */
 /* vips_zoom: out(x, y) = in(x / xfac, y / yfac), pixels of ps bytes */
 __global__ void __launch_bounds__(256)
-zoom_kernel(const char *__restrict__ in, size_t in_bpl, char *__restrict__ out, size_t out_bpl, int ow, int ps, int xf, int yf)
+zoom_kernel(const char *__restrict__ in, size_t in_bpl, char *__restrict__ out, size_t out_bpl, int ow, int oh, int ps, int xf,
+	int yf)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= ow)
 		return;
-	const char *p = in + (size_t) (blockIdx.y / yf) * in_bpl + (size_t) (x / xf) * ps;
-	char *q = out + (size_t) blockIdx.y * out_bpl + (size_t) x * ps;
-	for (int i = 0; i < ps; i++)
-		q[i] = p[i];
+	for (int y = blockIdx.y; y < oh; y += gridDim.y) {
+		const char *p = in + (size_t) (y / yf) * in_bpl + (size_t) (x / xf) * ps;
+		char *q = out + (size_t) y * out_bpl + (size_t) x * ps;
+		for (int i = 0; i < ps; i++)
+			q[i] = p[i];
+	}
 }
 
 __device__ __forceinline__ int
@@ -97,13 +100,9 @@ dp2a_hi_s(unsigned coef, unsigned bytes, int acc)
 	return d;
 }
 
-__global__ void __launch_bounds__(256)
-affine_bicubic_u8x4_kernel(const __grid_constant__ AffineDev P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out)
+__device__ __forceinline__ void
+affine_bicubic_u8x4_px(const AffineDev &P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out, int x, int y)
 {
-	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
-	if (x >= P.OW)
-		return;
 	const double ix = P.ixs[x];
 	const double iy = P.iys[y];
 	unsigned *q = (unsigned *) ((char *) out + (size_t) y * P.out_bpl) + x;
@@ -153,6 +152,16 @@ affine_bicubic_u8x4_kernel(const __grid_constant__ AffineDev P, const uint8_t *_
 	*q = v;
 }
 
+__global__ void __launch_bounds__(256)
+affine_bicubic_u8x4_kernel(const __grid_constant__ AffineDev P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out)
+{
+	const int x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= P.OW)
+		return;
+	for (int y = blockIdx.y; y < P.OH; y += gridDim.y)
+		affine_bicubic_u8x4_px(P, in, out, x, y);
+}
+
 /* The same pixels, separably.  vips_interpolate_bicubic's integer path is two-stage -- four horizontal sums
  * rounded to integers, then the vertical sum of those (bicubic_unsigned_int_tab, bicubic.cpp:106-166) -- so
  * the horizontal stage of an input row is shared by every output row that samples it (two of them at x2).
@@ -162,15 +171,15 @@ affine_bicubic_u8x4_kernel(const __grid_constant__ AffineDev P, const uint8_t *_
  */
 constexpr int kSepTW = 64, kSepTH = 32, kSepRows = kSepTH + 4;
 
+template <bool LOOP>
 __global__ void __launch_bounds__(256)
 affine_bicubic_u8x4_sep_kernel(const __grid_constant__ AffineDev P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out)
 {
 	__shared__ short4 sh[kSepRows][kSepTW];
 	const int t = threadIdx.x;
 	const int lx = t & (kSepTW - 1), ly = t >> 6; /* 64 columns x 4 row phases */
-	const int x0 = blockIdx.x * kSepTW, y0 = blockIdx.y * kSepTH;
+	const int x0 = blockIdx.x * kSepTW;
 	const int x = min(x0 + lx, P.OW - 1);
-	const int y_last = min(y0 + kSepTH, P.OH) - 1;
 
 	/* this thread's column: the horizontal coordinates never change down the tile */
 	const double ix = P.ixs[x];
@@ -187,67 +196,71 @@ affine_bicubic_u8x4_sep_kernel(const __grid_constant__ AffineDev P, const uint8_
 	for (int i = 0; i < 4; i++)
 		col[i] = max(0, min(xi - 1 + i - P.pad, P.w - 1));
 
-	/* the input rows this tile samples */
-	const int r_lo = (int) P.iys[y0] - 1;
-	const int nrows = min((int) P.iys[y_last] + 2 - r_lo + 1, kSepRows);
-	for (int rr = ly; rr < nrows; rr += 4) {
-		const int sy2 = max(0, min(r_lo + rr - P.pad, P.h - 1));
-		const unsigned *row = (const unsigned *) (in + (size_t) sy2 * P.in_bpl);
-		const unsigned p0 = __ldg(row + col[0]), p1 = __ldg(row + col[1]), p2 = __ldg(row + col[2]), p3 = __ldg(row + col[3]);
-		const unsigned a01 = __byte_perm(p0, p1, 0x5140); /* [p0.c0 p1.c0 p0.c1 p1.c1] */
-		const unsigned b01 = __byte_perm(p0, p1, 0x7362); /* [p0.c2 p1.c2 p0.c3 p1.c3] */
-		const unsigned a23 = __byte_perm(p2, p3, 0x5140);
-		const unsigned b23 = __byte_perm(p2, p3, 0x7362);
-		short4 r;
-		r.x = (short) ufr(dp2a_lo_s(cx23, a23, dp2a_lo_s(cx01, a01, 0)));
-		r.y = (short) ufr(dp2a_hi_s(cx23, a23, dp2a_hi_s(cx01, a01, 0)));
-		r.z = (short) ufr(dp2a_lo_s(cx23, b23, dp2a_lo_s(cx01, b01, 0)));
-		r.w = (short) ufr(dp2a_hi_s(cx23, b23, dp2a_hi_s(cx01, b01, 0)));
-		sh[rr][lx] = r;
-	}
-	__syncthreads();
+	/* the whole CTA walks its tiles down the image together through the staged rows */
+	int y0 = blockIdx.y * kSepTH;
+	do {
+		if (y0 != (int) blockIdx.y * kSepTH)
+			__syncthreads(); /* the previous tile's rows have been read */
+		const int y_last = min(y0 + kSepTH, P.OH) - 1;
 
-	if (x0 + lx >= P.OW)
-		return;
-	for (int y = y0 + ly; y <= y_last; y += 4) {
-		unsigned *q = (unsigned *) ((char *) out + (size_t) y * P.out_bpl) + x;
-		const double iy = P.iys[y];
-		const int fy = (int) floor(iy);
-		if (!(x_in && fy >= P.ito && fy <= P.ibo)) {
-			*q = 0;
+		/* the input rows this tile samples */
+		const int r_lo = (int) P.iys[y0] - 1;
+		const int nrows = min((int) P.iys[y_last] + 2 - r_lo + 1, kSepRows);
+		for (int rr = ly; rr < nrows; rr += 4) {
+			const int sy2 = max(0, min(r_lo + rr - P.pad, P.h - 1));
+			const unsigned *row = (const unsigned *) (in + (size_t) sy2 * P.in_bpl);
+			const unsigned p0 = __ldg(row + col[0]), p1 = __ldg(row + col[1]), p2 = __ldg(row + col[2]), p3 = __ldg(row + col[3]);
+			const unsigned a01 = __byte_perm(p0, p1, 0x5140); /* [p0.c0 p1.c0 p0.c1 p1.c1] */
+			const unsigned b01 = __byte_perm(p0, p1, 0x7362); /* [p0.c2 p1.c2 p0.c3 p1.c3] */
+			const unsigned a23 = __byte_perm(p2, p3, 0x5140);
+			const unsigned b23 = __byte_perm(p2, p3, 0x7362);
+			short4 r;
+			r.x = (short) ufr(dp2a_lo_s(cx23, a23, dp2a_lo_s(cx01, a01, 0)));
+			r.y = (short) ufr(dp2a_hi_s(cx23, a23, dp2a_hi_s(cx01, a01, 0)));
+			r.z = (short) ufr(dp2a_lo_s(cx23, b23, dp2a_lo_s(cx01, b01, 0)));
+			r.w = (short) ufr(dp2a_hi_s(cx23, b23, dp2a_hi_s(cx01, b01, 0)));
+			sh[rr][lx] = r;
+		}
+		__syncthreads();
+
+		if (x0 + lx >= P.OW)
 			continue;
-		}
-		const int yi = (int) iy;
-		const int sy = (int) __dmul_rn(__dmul_rn(iy, (double) VB200_TRANSFORM_SCALE), 2.0);
-		const int ty = ((sy & (VB200_TRANSFORM_SCALE * 2 - 1)) + 1) >> 1;
-		const int4 cy = __ldg((const int4 *) (P.ci + ty * 4));
-		const int cyv[4] = {cy.x, cy.y, cy.z, cy.w};
-		const int base = yi - 1 - r_lo;
-		int acc[4] = {0, 0, 0, 0};
+		for (int y = y0 + ly; y <= y_last; y += 4) {
+			unsigned *q = (unsigned *) ((char *) out + (size_t) y * P.out_bpl) + x;
+			const double iy = P.iys[y];
+			const int fy = (int) floor(iy);
+			if (!(x_in && fy >= P.ito && fy <= P.ibo)) {
+				*q = 0;
+				continue;
+			}
+			const int yi = (int) iy;
+			const int sy = (int) __dmul_rn(__dmul_rn(iy, (double) VB200_TRANSFORM_SCALE), 2.0);
+			const int ty = ((sy & (VB200_TRANSFORM_SCALE * 2 - 1)) + 1) >> 1;
+			const int4 cy = __ldg((const int4 *) (P.ci + ty * 4));
+			const int cyv[4] = {cy.x, cy.y, cy.z, cy.w};
+			const int base = yi - 1 - r_lo;
+			int acc[4] = {0, 0, 0, 0};
 #pragma unroll
-		for (int j = 0; j < 4; j++) {
-			const short4 r = sh[base + j][lx];
-			acc[0] += cyv[j] * r.x;
-			acc[1] += cyv[j] * r.y;
-			acc[2] += cyv[j] * r.z;
-			acc[3] += cyv[j] * r.w;
-		}
-		unsigned v = 0;
+			for (int j = 0; j < 4; j++) {
+				const short4 r = sh[base + j][lx];
+				acc[0] += cyv[j] * r.x;
+				acc[1] += cyv[j] * r.y;
+				acc[2] += cyv[j] * r.z;
+				acc[3] += cyv[j] * r.w;
+			}
+			unsigned v = 0;
 #pragma unroll
-		for (int c = 0; c < 4; c++)
-			v |= (unsigned) max(0, min(ufr(acc[c]), 255)) << (8 * c);
-		*q = v;
-	}
+			for (int c = 0; c < 4; c++)
+				v |= (unsigned) max(0, min(ufr(acc[c]), 255)) << (8 * c);
+			*q = v;
+		}
+	} while (LOOP && (y0 += gridDim.y * kSepTH) < P.OH);
 }
 
 template <typename T>
-__global__ void __launch_bounds__(256)
-affine_scale_kernel(const __grid_constant__ AffineDev P, const T *__restrict__ in, T *__restrict__ out)
+__device__ __forceinline__ void
+affine_scale_px(const AffineDev &P, const T *__restrict__ in, T *__restrict__ out, int x, int y)
 {
-	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
-	if (x >= P.OW)
-		return;
 	const double ix = P.ixs[x];
 	const double iy = P.iys[y];
 	T *q = (T *) ((char *) out + (size_t) y * P.out_bpl) + (size_t) x * P.bands;
@@ -350,6 +363,19 @@ affine_scale_kernel(const __grid_constant__ AffineDev P, const T *__restrict__ i
 			}
 		}
 	}
+}
+
+template <typename T, bool LOOP>
+__global__ void __launch_bounds__(256)
+affine_scale_kernel(const __grid_constant__ AffineDev P, const T *__restrict__ in, T *__restrict__ out)
+{
+	const int x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= P.OW)
+		return;
+	int y = blockIdx.y;
+	do
+		affine_scale_px<T>(P, in, out, x, y);
+	while (LOOP && (y += gridDim.y) < P.OH);
 }
 
 #define VB200_ROUND_INT(R) ((int) ((R) > 0 ? ((R) + 0.5) : ((R) -0.5)))
@@ -505,14 +531,16 @@ dev_affine_scale(const char *domain, const DevImage &in, DevImage *out, double a
 	P.iri = P.ile + in.w;
 	P.ibo = P.ito + in.h;
 	P.interp = interp;
-	const dim3 grid((OW + 255) / 256, OH);
-#define AF(T) affine_scale_kernel<T><<<grid, 256, 0, s>>>(P, (const T *) in.data, (T *) out->data)
+	const dim3 grid = row_grid(OW, OH);
+	const bool loop = rows_loop(OH);
+#define AF(T) (loop ? affine_scale_kernel<T, true> : affine_scale_kernel<T, false>)<<<grid, 256, 0, s>>>(P, (const T *) in.data, (T *) out->data)
 	const bool u8x4 = in.fmt == VB200_FORMAT_UCHAR && in.bands == 4 && interp == INTERP_BICUBIC && (in.bpl & 3) == 0 &&
 		((uintptr_t) in.data & 3) == 0 && getenv("VB200_NO_AFFINE_X4") == nullptr;
 	/* vertical scale >= 1: a tile of 32 output rows touches at most 35 input rows (the separable kernel's budget) */
 	const bool sep = u8x4 && id <= 1.0 && getenv("VB200_NO_AFFINE_SEP") == nullptr;
 	if (sep)
-		affine_bicubic_u8x4_sep_kernel<<<dim3((OW + kSepTW - 1) / kSepTW, (OH + kSepTH - 1) / kSepTH), 256, 0, s>>>(P,
+		(rows_loop((OH + kSepTH - 1) / kSepTH) ? affine_bicubic_u8x4_sep_kernel<true> : affine_bicubic_u8x4_sep_kernel<false>)<<<
+			row_grid(OW, (OH + kSepTH - 1) / kSepTH, kSepTW), 256, 0, s>>>(P,
 			(const uint8_t *) in.data, (uint8_t *) out->data);
 	else if (u8x4)
 		affine_bicubic_u8x4_kernel<<<grid, 256, 0, s>>>(P, (const uint8_t *) in.data, (uint8_t *) out->data);
@@ -554,8 +582,8 @@ dev_resize_up(const char *domain, const DevImage &in, DevImage *out, double hsca
 		if (dev_image_new(domain, out, in.w * xf, in.h * yf, in.bands, in.fmt, in.type, s))
 			return -1;
 		const int ps = (int) (format_sizeof(in.fmt) * in.bands);
-		const dim3 grid((out->w + 255) / 256, out->h);
-		zoom_kernel<<<grid, 256, 0, s>>>((const char *) in.data, in.bpl, (char *) out->data, out->bpl, out->w, ps, xf, yf);
+		const dim3 grid = row_grid(out->w, out->h);
+		zoom_kernel<<<grid, 256, 0, s>>>((const char *) in.data, in.bpl, (char *) out->data, out->bpl, out->w, out->h, ps, xf, yf);
 		const cudaError_t e = cudaGetLastError();
 		if (e != cudaSuccess)
 			return cuda_fail(domain, e, "zoom_kernel");

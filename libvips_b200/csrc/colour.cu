@@ -117,8 +117,9 @@ get_tables(const char *domain, ColourTables *out)
 
 namespace {
 
+template <bool LOOP>
 __global__ void __launch_bounds__(256)
-colour_route_kernel(const __grid_constant__ RouteParams P, const void *__restrict__ in, void *__restrict__ out)
+colour_route_kernel(const __grid_constant__ RouteParams P, int h, const void *__restrict__ in, void *__restrict__ out)
 {
 	__shared__ float s_v2Y_8[256];
 	__shared__ float s_Y2v_8[257]; /* integers <= 255 held as floats: scRGB2sRGB_channel_f */
@@ -130,113 +131,115 @@ colour_route_kernel(const __grid_constant__ RouteParams P, const void *__restric
 	__syncthreads();
 
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= P.w)
 		return;
-	const char *pin = (const char *) in + (size_t) y * P.in_bpl;
-	char *pout = (char *) out + (size_t) y * P.out_bpl;
-	const int base = x * P.bands;
+	int y = blockIdx.y;
+	do {
+		const char *pin = (const char *) in + (size_t) y * P.in_bpl;
+		char *pout = (char *) out + (size_t) y * P.out_bpl;
+		const int base = x * P.bands;
 
-	/* the pixel: integer inputs are held exactly in float until their LUT step */
-	float a = (float) load_elem(pin, P.in_fmt, base);
-	float b = (float) load_elem(pin, P.in_fmt, base + 1);
-	float c = (float) load_elem(pin, P.in_fmt, base + 2);
-	int ia = 0, ib = 0, ic = 0; /* integer outputs (sRGB / RGB16 / LabS) */
+		/* the pixel: integer inputs are held exactly in float until their LUT step */
+		float a = (float) load_elem(pin, P.in_fmt, base);
+		float b = (float) load_elem(pin, P.in_fmt, base + 1);
+		float c = (float) load_elem(pin, P.in_fmt, base + 2);
+		int ia = 0, ib = 0, ic = 0; /* integer outputs (sRGB / RGB16 / LabS) */
 
-	for (int s = 0; s < P.n_steps; s++) {
-		switch (P.steps[s].step) {
-		case S_sRGB2scRGB:
-			a = s_v2Y_8[(int) a];
-			b = s_v2Y_8[(int) b];
-			c = s_v2Y_8[(int) c];
-			break;
-		case S_RGB162scRGB:
-			a = __ldg(P.t.v2Y_16 + (int) a);
-			b = __ldg(P.t.v2Y_16 + (int) b);
-			c = __ldg(P.t.v2Y_16 + (int) c);
-			break;
-		case S_scRGB2XYZ:
-			step_scRGB2XYZ(a, b, c);
-			break;
-		case S_XYZ2Lab:
-			step_XYZ2Lab(P.t.cbrt, a, b, c);
-			break;
-		case S_Lab2XYZ:
-			step_Lab2XYZ(a, b, c);
-			break;
-		case S_XYZ2scRGB:
-			step_XYZ2scRGB(a, b, c);
-			break;
-		case S_LabS2Lab:
-			a = (float) DIVC((double) a, 32767.0 / 100.0);
-			b = (float) DIVC((double) b, 32768.0 / 128.0);
-			c = (float) DIVC((double) c, 32768.0 / 128.0);
-			break;
-		case S_Lab2LabS:
-			ia = (int) (short) clipd(0, __dmul_rn((double) a, 32767.0 / 100.0), 32767);
-			ib = (int) (short) clipd(-32768, __dmul_rn((double) b, 32768.0 / 128.0), 32767);
-			ic = (int) (short) clipd(-32768, __dmul_rn((double) c, 32768.0 / 128.0), 32767);
-			break;
-		case S_scRGB2sRGB:
-			if (isnan(a) || isnan(b) || isnan(c))
-				ia = ib = ic = 0;
-			else {
-				ia = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, a);
-				ib = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, b);
-				ic = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, c);
+		for (int s = 0; s < P.n_steps; s++) {
+			switch (P.steps[s].step) {
+			case S_sRGB2scRGB:
+				a = s_v2Y_8[(int) a];
+				b = s_v2Y_8[(int) b];
+				c = s_v2Y_8[(int) c];
+				break;
+			case S_RGB162scRGB:
+				a = __ldg(P.t.v2Y_16 + (int) a);
+				b = __ldg(P.t.v2Y_16 + (int) b);
+				c = __ldg(P.t.v2Y_16 + (int) c);
+				break;
+			case S_scRGB2XYZ:
+				step_scRGB2XYZ(a, b, c);
+				break;
+			case S_XYZ2Lab:
+				step_XYZ2Lab(P.t.cbrt, a, b, c);
+				break;
+			case S_Lab2XYZ:
+				step_Lab2XYZ(a, b, c);
+				break;
+			case S_XYZ2scRGB:
+				step_XYZ2scRGB(a, b, c);
+				break;
+			case S_LabS2Lab:
+				a = (float) DIVC((double) a, 32767.0 / 100.0);
+				b = (float) DIVC((double) b, 32768.0 / 128.0);
+				c = (float) DIVC((double) c, 32768.0 / 128.0);
+				break;
+			case S_Lab2LabS:
+				ia = (int) (short) clipd(0, __dmul_rn((double) a, 32767.0 / 100.0), 32767);
+				ib = (int) (short) clipd(-32768, __dmul_rn((double) b, 32768.0 / 128.0), 32767);
+				ic = (int) (short) clipd(-32768, __dmul_rn((double) c, 32768.0 / 128.0), 32767);
+				break;
+			case S_scRGB2sRGB:
+				if (isnan(a) || isnan(b) || isnan(c))
+					ia = ib = ic = 0;
+				else {
+					ia = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, a);
+					ib = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, b);
+					ic = scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, c);
+				}
+				break;
+			case S_Lab2LCh:
+				step_Lab2LCh(a, b, c);
+				break;
+			case S_LCh2Lab:
+				step_LCh2Lab(a, b, c);
+				break;
+			case S_XYZ2Yxy:
+				step_XYZ2Yxy(a, b, c);
+				break;
+			case S_Yxy2XYZ:
+				step_Yxy2XYZ(a, b, c);
+				break;
+			case S_scRGB2RGB16:
+				if (isnan(a) || isnan(b) || isnan(c))
+					ia = ib = ic = 0;
+				else {
+					ia = scRGB2sRGB_channel(P.t.Y2v_16, 65535, a);
+					ib = scRGB2sRGB_channel(P.t.Y2v_16, 65535, b);
+					ic = scRGB2sRGB_channel(P.t.Y2v_16, 65535, c);
+				}
+				break;
 			}
+		}
+
+		switch (P.out_fmt) {
+		case VB200_FORMAT_UCHAR:
+			((uint8_t *) pout)[base] = (uint8_t) ia;
+			((uint8_t *) pout)[base + 1] = (uint8_t) ib;
+			((uint8_t *) pout)[base + 2] = (uint8_t) ic;
 			break;
-		case S_Lab2LCh:
-			step_Lab2LCh(a, b, c);
+		case VB200_FORMAT_USHORT:
+			((uint16_t *) pout)[base] = (uint16_t) ia;
+			((uint16_t *) pout)[base + 1] = (uint16_t) ib;
+			((uint16_t *) pout)[base + 2] = (uint16_t) ic;
 			break;
-		case S_LCh2Lab:
-			step_LCh2Lab(a, b, c);
+		case VB200_FORMAT_SHORT:
+			((int16_t *) pout)[base] = (int16_t) ia;
+			((int16_t *) pout)[base + 1] = (int16_t) ib;
+			((int16_t *) pout)[base + 2] = (int16_t) ic;
 			break;
-		case S_XYZ2Yxy:
-			step_XYZ2Yxy(a, b, c);
-			break;
-		case S_Yxy2XYZ:
-			step_Yxy2XYZ(a, b, c);
-			break;
-		case S_scRGB2RGB16:
-			if (isnan(a) || isnan(b) || isnan(c))
-				ia = ib = ic = 0;
-			else {
-				ia = scRGB2sRGB_channel(P.t.Y2v_16, 65535, a);
-				ib = scRGB2sRGB_channel(P.t.Y2v_16, 65535, b);
-				ic = scRGB2sRGB_channel(P.t.Y2v_16, 65535, c);
-			}
+		default:
+			((float *) pout)[base] = a;
+			((float *) pout)[base + 1] = b;
+			((float *) pout)[base + 2] = c;
 			break;
 		}
-	}
 
-	switch (P.out_fmt) {
-	case VB200_FORMAT_UCHAR:
-		((uint8_t *) pout)[base] = (uint8_t) ia;
-		((uint8_t *) pout)[base + 1] = (uint8_t) ib;
-		((uint8_t *) pout)[base + 2] = (uint8_t) ic;
-		break;
-	case VB200_FORMAT_USHORT:
-		((uint16_t *) pout)[base] = (uint16_t) ia;
-		((uint16_t *) pout)[base + 1] = (uint16_t) ib;
-		((uint16_t *) pout)[base + 2] = (uint16_t) ic;
-		break;
-	case VB200_FORMAT_SHORT:
-		((int16_t *) pout)[base] = (int16_t) ia;
-		((int16_t *) pout)[base + 1] = (int16_t) ib;
-		((int16_t *) pout)[base + 2] = (int16_t) ic;
-		break;
-	default:
-		((float *) pout)[base] = a;
-		((float *) pout)[base + 1] = b;
-		((float *) pout)[base + 2] = c;
-		break;
-	}
-
-	/* extra bands: colour.c:252-291 per step */
-	for (int e = 3; e < P.bands; e++) {
-		store_elem(pout, P.out_fmt, base + e, carry_extra_band(load_elem(pin, P.in_fmt, base + e), P.steps, P.n_steps));
-	}
+		/* extra bands: colour.c:252-291 per step */
+		for (int e = 3; e < P.bands; e++) {
+			store_elem(pout, P.out_fmt, base + e, carry_extra_band(load_elem(pin, P.in_fmt, base + e), P.steps, P.n_steps));
+		}
+	} while (LOOP && (y += gridDim.y) < h);
 }
 
 /* The two hot routes (BASELINE config 4), 3-band packed rows, four pixels per thread: sRGB bytes come
@@ -244,8 +247,9 @@ colour_route_kernel(const __grid_constant__ RouteParams P, const void *__restric
  * compiled in (no per-step switch) and the cbrt table is read as aligned (t[i], t[i + 1]) pairs.
  * Same steps, same roundings as colour_route_kernel.
  */
+template <bool LOOP>
 __global__ void __launch_bounds__(256)
-colour_srgb2lab_x4_kernel(const __grid_constant__ RouteParams P, const uint8_t *__restrict__ in, float *__restrict__ out)
+colour_srgb2lab_x4_kernel(const __grid_constant__ RouteParams P, int h, const uint8_t *__restrict__ in, float *__restrict__ out)
 {
 	__shared__ float s_v2Y_8[256];
 	for (int i = threadIdx.x; i < 256; i += blockDim.x)
@@ -254,33 +258,37 @@ colour_srgb2lab_x4_kernel(const __grid_constant__ RouteParams P, const uint8_t *
 	const int q = blockIdx.x * blockDim.x + threadIdx.x; /* group of 4 pixels */
 	if (q * 4 >= P.w)
 		return;
-	const uint32_t *pin = (const uint32_t *) (in + (size_t) blockIdx.y * P.in_bpl) + (size_t) q * 3;
-	float4 *pout = (float4 *) ((char *) out + (size_t) blockIdx.y * P.out_bpl) + (size_t) q * 3;
-	const uint32_t w0 = __ldg(pin), w1 = __ldg(pin + 1), w2 = __ldg(pin + 2);
-	const uint32_t bytes[12] = {w0 & 255, (w0 >> 8) & 255, (w0 >> 16) & 255, w0 >> 24, w1 & 255, (w1 >> 8) & 255,
-		(w1 >> 16) & 255, w1 >> 24, w2 & 255, (w2 >> 8) & 255, (w2 >> 16) & 255, w2 >> 24};
-	float r[12];
+	int y = blockIdx.y;
+	do {
+		const uint32_t *pin = (const uint32_t *) (in + (size_t) y * P.in_bpl) + (size_t) q * 3;
+		float4 *pout = (float4 *) ((char *) out + (size_t) y * P.out_bpl) + (size_t) q * 3;
+		const uint32_t w0 = __ldg(pin), w1 = __ldg(pin + 1), w2 = __ldg(pin + 2);
+		const uint32_t bytes[12] = {w0 & 255, (w0 >> 8) & 255, (w0 >> 16) & 255, w0 >> 24, w1 & 255, (w1 >> 8) & 255,
+			(w1 >> 16) & 255, w1 >> 24, w2 & 255, (w2 >> 8) & 255, (w2 >> 16) & 255, w2 >> 24};
+		float r[12];
 #pragma unroll
-	for (int k = 0; k < 4; k++) {
-		float a = s_v2Y_8[bytes[3 * k]], b = s_v2Y_8[bytes[3 * k + 1]], c = s_v2Y_8[bytes[3 * k + 2]];
-		step_scRGB2XYZ(a, b, c);
-		const float nX = (float) DIVC((double) __fmul_rn(100000.0f, a), 95.0470);
-		const float nY = (float) DIVC((double) __fmul_rn(100000.0f, b), 100.0);
-		const float nZ = (float) DIVC((double) __fmul_rn(100000.0f, c), 108.8827);
-		const float cbx = cbrt_lookup2(P.t.cbrt2, nX);
-		const float cby = cbrt_lookup2(P.t.cbrt2, nY);
-		const float cbz = cbrt_lookup2(P.t.cbrt2, nZ);
-		r[3 * k] = __fsub_rn(__fmul_rn(116.0F, cby), 16.0F);
-		r[3 * k + 1] = __fmul_rn(500.0F, __fsub_rn(cbx, cby));
-		r[3 * k + 2] = __fmul_rn(200.0F, __fsub_rn(cby, cbz));
-	}
-	pout[0] = make_float4(r[0], r[1], r[2], r[3]);
-	pout[1] = make_float4(r[4], r[5], r[6], r[7]);
-	pout[2] = make_float4(r[8], r[9], r[10], r[11]);
+		for (int k = 0; k < 4; k++) {
+			float a = s_v2Y_8[bytes[3 * k]], b = s_v2Y_8[bytes[3 * k + 1]], c = s_v2Y_8[bytes[3 * k + 2]];
+			step_scRGB2XYZ(a, b, c);
+			const float nX = (float) DIVC((double) __fmul_rn(100000.0f, a), 95.0470);
+			const float nY = (float) DIVC((double) __fmul_rn(100000.0f, b), 100.0);
+			const float nZ = (float) DIVC((double) __fmul_rn(100000.0f, c), 108.8827);
+			const float cbx = cbrt_lookup2(P.t.cbrt2, nX);
+			const float cby = cbrt_lookup2(P.t.cbrt2, nY);
+			const float cbz = cbrt_lookup2(P.t.cbrt2, nZ);
+			r[3 * k] = __fsub_rn(__fmul_rn(116.0F, cby), 16.0F);
+			r[3 * k + 1] = __fmul_rn(500.0F, __fsub_rn(cbx, cby));
+			r[3 * k + 2] = __fmul_rn(200.0F, __fsub_rn(cby, cbz));
+		}
+		pout[0] = make_float4(r[0], r[1], r[2], r[3]);
+		pout[1] = make_float4(r[4], r[5], r[6], r[7]);
+		pout[2] = make_float4(r[8], r[9], r[10], r[11]);
+	} while (LOOP && (y += gridDim.y) < h);
 }
 
+template <bool LOOP>
 __global__ void __launch_bounds__(256)
-colour_lab2srgb_x4_kernel(const __grid_constant__ RouteParams P, const float *__restrict__ in, uint8_t *__restrict__ out)
+colour_lab2srgb_x4_kernel(const __grid_constant__ RouteParams P, int h, const float *__restrict__ in, uint8_t *__restrict__ out)
 {
 	__shared__ float s_Y2v_8[257];
 	for (int i = threadIdx.x; i < 257; i += blockDim.x)
@@ -289,40 +297,45 @@ colour_lab2srgb_x4_kernel(const __grid_constant__ RouteParams P, const float *__
 	const int q = blockIdx.x * blockDim.x + threadIdx.x;
 	if (q * 4 >= P.w)
 		return;
-	const float4 *pin = (const float4 *) ((const char *) in + (size_t) blockIdx.y * P.in_bpl) + (size_t) q * 3;
-	uint32_t *pout = (uint32_t *) (out + (size_t) blockIdx.y * P.out_bpl) + (size_t) q * 3;
-	const float4 v0 = __ldg(pin), v1 = __ldg(pin + 1), v2 = __ldg(pin + 2);
-	const float f[12] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w};
-	uint32_t o[12];
+	int y = blockIdx.y;
+	do {
+		const float4 *pin = (const float4 *) ((const char *) in + (size_t) y * P.in_bpl) + (size_t) q * 3;
+		uint32_t *pout = (uint32_t *) (out + (size_t) y * P.out_bpl) + (size_t) q * 3;
+		const float4 v0 = __ldg(pin), v1 = __ldg(pin + 1), v2 = __ldg(pin + 2);
+		const float f[12] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w};
+		uint32_t o[12];
 #pragma unroll
-	for (int k = 0; k < 4; k++) {
-		float a = f[3 * k], b = f[3 * k + 1], c = f[3 * k + 2];
-		step_Lab2XYZ(a, b, c);
-		step_XYZ2scRGB(a, b, c);
-		if (isnan(a) || isnan(b) || isnan(c))
-			o[3 * k] = o[3 * k + 1] = o[3 * k + 2] = 0;
-		else {
-			o[3 * k] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, a) & 255u;
-			o[3 * k + 1] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, b) & 255u;
-			o[3 * k + 2] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, c) & 255u;
+		for (int k = 0; k < 4; k++) {
+			float a = f[3 * k], b = f[3 * k + 1], c = f[3 * k + 2];
+			step_Lab2XYZ(a, b, c);
+			step_XYZ2scRGB(a, b, c);
+			if (isnan(a) || isnan(b) || isnan(c))
+				o[3 * k] = o[3 * k + 1] = o[3 * k + 2] = 0;
+			else {
+				o[3 * k] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, a) & 255u;
+				o[3 * k + 1] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, b) & 255u;
+				o[3 * k + 2] = (uint32_t) scRGB2sRGB_channel_f(s_Y2v_8, 255.0f, c) & 255u;
+			}
 		}
-	}
-	pout[0] = o[0] | (o[1] << 8) | (o[2] << 16) | (o[3] << 24);
-	pout[1] = o[4] | (o[5] << 8) | (o[6] << 16) | (o[7] << 24);
-	pout[2] = o[8] | (o[9] << 8) | (o[10] << 16) | (o[11] << 24);
+		pout[0] = o[0] | (o[1] << 8) | (o[2] << 16) | (o[3] << 24);
+		pout[1] = o[4] | (o[5] << 8) | (o[6] << 16) | (o[7] << 24);
+		pout[2] = o[8] | (o[9] << 8) | (o[10] << 16) | (o[11] << 24);
+	} while (LOOP && (y += gridDim.y) < h);
 }
 
 /* identity routes: a cast to the space's format (colourspace.c rows X -> X) */
 __global__ void __launch_bounds__(256)
 cast_kernel(const void *__restrict__ in, size_t in_bpl, int in_fmt, void *__restrict__ out, size_t out_bpl, int out_fmt,
-	int ne)
+	int ne, int h)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= ne)
 		return;
-	const char *pin = (const char *) in + (size_t) blockIdx.y * in_bpl;
-	char *pout = (char *) out + (size_t) blockIdx.y * out_bpl;
-	store_elem(pout, out_fmt, x, cast_value(load_elem(pin, in_fmt, x), out_fmt));
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		const char *pin = (const char *) in + (size_t) y * in_bpl;
+		char *pout = (char *) out + (size_t) y * out_bpl;
+		store_elem(pout, out_fmt, x, cast_value(load_elem(pin, in_fmt, x), out_fmt));
+	}
 }
 
 /* sRGB <-> RGB16 are not colour conversions in the reference: vips_sRGB2RGB16 / vips_RGB162sRGB (colourspace.c:85-110)
@@ -330,19 +343,21 @@ cast_kernel(const void *__restrict__ in, size_t in_bpl, int in_fmt, void *__rest
  * right shift by the width difference; going up a left shift with the bottom bit copied into the new bits.
  */
 __global__ void __launch_bounds__(256)
-shift_cast_kernel(const void *__restrict__ in, size_t in_bpl, void *__restrict__ out, size_t out_bpl, int up, int ne)
+shift_cast_kernel(const void *__restrict__ in, size_t in_bpl, void *__restrict__ out, size_t out_bpl, int up, int ne, int h)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= ne)
 		return;
-	const char *pin = (const char *) in + (size_t) blockIdx.y * in_bpl;
-	char *pout = (char *) out + (size_t) blockIdx.y * out_bpl;
-	if (up) {
-		const unsigned v = ((const uint8_t *) pin)[x];
-		((uint16_t *) pout)[x] = (uint16_t) ((v << 8) | (((v & 1u) << 8) - (v & 1u)));
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		const char *pin = (const char *) in + (size_t) y * in_bpl;
+		char *pout = (char *) out + (size_t) y * out_bpl;
+		if (up) {
+			const unsigned v = ((const uint8_t *) pin)[x];
+			((uint16_t *) pout)[x] = (uint16_t) ((v << 8) | (((v & 1u) << 8) - (v & 1u)));
+		}
+		else
+			((uint8_t *) pout)[x] = (uint8_t) (((const uint16_t *) pin)[x] >> 8);
 	}
-	else
-		((uint8_t *) pout)[x] = (uint8_t) (((const uint16_t *) pin)[x] >> 8);
 }
 
 int
@@ -514,7 +529,7 @@ dev_colourspace(const char *domain, const DevImage &in, DevImage *out, int space
 		if (dev_image_new(domain, out, in.w, in.h, in.bands, up ? VB200_FORMAT_USHORT : VB200_FORMAT_UCHAR, space, s))
 			return -1;
 		const int ne = in.w * in.bands;
-		shift_cast_kernel<<<dim3((ne + 255) / 256, in.h), block, 0, s>>>(in.data, in.bpl, out->data, out->bpl, up ? 1 : 0, ne);
+		shift_cast_kernel<<<row_grid(ne, in.h), block, 0, s>>>(in.data, in.bpl, out->data, out->bpl, up ? 1 : 0, ne, in.h);
 		cudaError_t e = cudaGetLastError();
 		if (e != cudaSuccess)
 			return cuda_fail(domain, e, "shift_cast_kernel");
@@ -535,7 +550,10 @@ dev_colourspace(const char *domain, const DevImage &in, DevImage *out, int space
 		if (dev_image_new(domain, out, in.w, in.h, in.bands, ofmt, space, s))
 			return -1;
 		const int ne = in.w * in.bands;
-		cast_kernel<<<dim3((ne + 255) / 256, in.h), block, 0, s>>>(in.data, in.bpl, in.fmt, out->data, out->bpl, ofmt, ne);
+		cast_kernel<<<row_grid(ne, in.h), block, 0, s>>>(in.data, in.bpl, in.fmt, out->data, out->bpl, ofmt, ne, in.h);
+		cudaError_t e = cudaGetLastError();
+		if (e != cudaSuccess)
+			return cuda_fail(domain, e, "cast_kernel");
 		count_launch();
 		return 0;
 	}
@@ -563,13 +581,14 @@ dev_colourspace(const char *domain, const DevImage &in, DevImage *out, int space
 	P.out_bpl = out->bpl;
 	const bool x4 = in.bands == 3 && (in.w & 3) == 0 && ((uintptr_t) in.data & 15) == 0 && ((uintptr_t) out->data & 15) == 0 &&
 		(in.bpl & 15) == 0 && (out->bpl & 15) == 0 && getenv("VB200_NO_COLOUR_X4") == nullptr;
-	const dim3 grid4((in.w / 4 + 255) / 256, in.h);
+	const dim3 grid4 = row_grid(in.w / 4, in.h);
+	const bool loop = rows_loop(in.h);
 	if (x4 && n == 3 && steps[0] == S_sRGB2scRGB && steps[1] == S_scRGB2XYZ && steps[2] == S_XYZ2Lab)
-		colour_srgb2lab_x4_kernel<<<grid4, block, 0, s>>>(P, (const uint8_t *) in.data, (float *) out->data);
+		(loop ? colour_srgb2lab_x4_kernel<true> : colour_srgb2lab_x4_kernel<false>)<<<grid4, block, 0, s>>>(P, in.h, (const uint8_t *) in.data, (float *) out->data);
 	else if (x4 && n == 3 && steps[0] == S_Lab2XYZ && steps[1] == S_XYZ2scRGB && steps[2] == S_scRGB2sRGB)
-		colour_lab2srgb_x4_kernel<<<grid4, block, 0, s>>>(P, (const float *) in.data, (uint8_t *) out->data);
+		(loop ? colour_lab2srgb_x4_kernel<true> : colour_lab2srgb_x4_kernel<false>)<<<grid4, block, 0, s>>>(P, in.h, (const float *) in.data, (uint8_t *) out->data);
 	else
-		colour_route_kernel<<<dim3((in.w + 255) / 256, in.h), block, 0, s>>>(P, in.data, out->data);
+		(loop ? colour_route_kernel<true> : colour_route_kernel<false>)<<<row_grid(in.w, in.h), block, 0, s>>>(P, in.h, in.data, out->data);
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
 		return cuda_fail(domain, e, "colour_route_kernel");

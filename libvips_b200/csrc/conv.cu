@@ -54,20 +54,21 @@ __global__ void __launch_bounds__(256)
 convf_kernel(const __grid_constant__ ConvDev P, const T *__restrict__ in, float *__restrict__ out)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= P.w * P.bands)
 		return;
 	const int x = e / P.bands;
 	const int b = e - x * P.bands;
-	double sum = P.offset;
-	for (int i = 0; i < P.nnz; i++) {
-		const Tap t = P.taps[i];
-		const int sx = clampi(x + t.dx, 0, P.w - 1);
-		const int sy = clampi(y + t.dy, 0, P.h - 1);
-		const T v = ((const T *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
-		sum = __dadd_rn(sum, __dmul_rn(P.fcoeff[i], (double) v));
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		double sum = P.offset;
+		for (int i = 0; i < P.nnz; i++) {
+			const Tap t = P.taps[i];
+			const int sx = clampi(x + t.dx, 0, P.w - 1);
+			const int sy = clampi(y + t.dy, 0, P.h - 1);
+			const T v = ((const T *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
+			sum = __dadd_rn(sum, __dmul_rn(P.fcoeff[i], (double) v));
+		}
+		((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 	}
-	((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 }
 
 /* 1-D masks (the two passes of convsep / gaussblur): taps in shared memory, an
@@ -86,40 +87,41 @@ convf_line_kernel(const __grid_constant__ ConvDev P, const T *__restrict__ in, f
 	}
 	__syncthreads();
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= P.w * P.bands)
 		return;
 	const int nnz = P.nnz;
-	double sum = P.offset;
-	if (VERT) {
-		const size_t stride = P.in_bpl;
-		const char *col = (const char *) in + (size_t) e * sizeof(T);
-		if (y + sd[0] >= 0 && y + sd[nnz - 1] < P.h) {
-			const char *p = col + (size_t) y * stride;
-			for (int i = 0; i < nnz; i++)
-				sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) *(const T *) (p + (ptrdiff_t) sd[i] * (ptrdiff_t) stride)));
-		}
-		else
-			for (int i = 0; i < nnz; i++) {
-				const int sy = clampi(y + sd[i], 0, P.h - 1);
-				sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) *(const T *) (col + (size_t) sy * stride)));
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		double sum = P.offset;
+		if (VERT) {
+			const size_t stride = P.in_bpl;
+			const char *col = (const char *) in + (size_t) e * sizeof(T);
+			if (y + sd[0] >= 0 && y + sd[nnz - 1] < P.h) {
+				const char *p = col + (size_t) y * stride;
+				for (int i = 0; i < nnz; i++)
+					sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) *(const T *) (p + (ptrdiff_t) sd[i] * (ptrdiff_t) stride)));
 			}
-	}
-	else {
-		const T *row = (const T *) ((const char *) in + (size_t) y * P.in_bpl);
-		const int x = e / P.bands;
-		if (x + sd[0] >= 0 && x + sd[nnz - 1] < P.w) {
-			const T *p = row + e;
-			for (int i = 0; i < nnz; i++)
-				sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) p[sd[i] * P.bands]));
+			else
+				for (int i = 0; i < nnz; i++) {
+					const int sy = clampi(y + sd[i], 0, P.h - 1);
+					sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) *(const T *) (col + (size_t) sy * stride)));
+				}
 		}
 		else {
-			const int b = e - x * P.bands;
-			for (int i = 0; i < nnz; i++)
-				sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) row[clampi(x + sd[i], 0, P.w - 1) * P.bands + b]));
+			const T *row = (const T *) ((const char *) in + (size_t) y * P.in_bpl);
+			const int x = e / P.bands;
+			if (x + sd[0] >= 0 && x + sd[nnz - 1] < P.w) {
+				const T *p = row + e;
+				for (int i = 0; i < nnz; i++)
+					sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) p[sd[i] * P.bands]));
+			}
+			else {
+				const int b = e - x * P.bands;
+				for (int i = 0; i < nnz; i++)
+					sum = __dadd_rn(sum, __dmul_rn(sc[i], (double) row[clampi(x + sd[i], 0, P.w - 1) * P.bands + b]));
+			}
 		}
+		((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 	}
-	((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 }
 
 /* 1-D masks again, register-blocked: R outputs per thread along the mask axis, so each input
@@ -135,7 +137,7 @@ struct LineMask {
 	int n;					   /* mask length */
 };
 
-template <typename T, bool VERT, int R>
+template <typename T, bool VERT, int R, bool LOOP>
 __global__ void __launch_bounds__(128)
 convf_block_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ LineMask M, const T *__restrict__ in,
 	float *__restrict__ out)
@@ -143,12 +145,13 @@ convf_block_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ Li
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const int n = M.n;
 	const int d0 = -(n / 2);
-	int e, y0, x0 = 0, b = 0;
+	int e, y_first, y_step, x0 = 0, b = 0;
 	if (VERT) {
 		e = idx;
 		if (e >= P.w * P.bands)
 			return;
-		y0 = blockIdx.y * R;
+		y_first = blockIdx.y * R;
+		y_step = gridDim.y * R;
 	}
 	else {
 		const int groups = (P.w + R - 1) / R;
@@ -157,57 +160,61 @@ convf_block_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ Li
 		const int pg = idx / P.bands;
 		b = idx - pg * P.bands;
 		x0 = pg * R;
-		y0 = blockIdx.y;
+		y_first = blockIdx.y;
+		y_step = gridDim.y;
 		e = 0;
 	}
-	double acc[R];
+	int y0 = y_first;
+	do {
+		double acc[R];
 #pragma unroll
-	for (int r = 0; r < R; r++)
-		acc[r] = P.offset;
-	const char *base = (const char *) in;
-	const T *row = (const T *) (base + (size_t) y0 * P.in_bpl); /* HORIZ */
+		for (int r = 0; r < R; r++)
+			acc[r] = P.offset;
+		const char *base = (const char *) in;
+		const T *row = (const T *) (base + (size_t) y0 * P.in_bpl); /* HORIZ */
 
-	for (int j0 = 0; j0 < n + R - 1; j0 += R) {
-		double cc[2 * R - 1];
-		unsigned vm = 0;
+		for (int j0 = 0; j0 < n + R - 1; j0 += R) {
+			double cc[2 * R - 1];
+			unsigned vm = 0;
 #pragma unroll
-		for (int k = 0; k < 2 * R - 1; k++) {
-			const int i = j0 - (R - 1) + k;
-			const bool ok = (unsigned) i < (unsigned) n && ((M.present >> i) & 1ull);
-			cc[k] = ok ? M.c[i] : 0.0;
-			vm |= ok ? (1u << k) : 0u;
-		}
+			for (int k = 0; k < 2 * R - 1; k++) {
+				const int i = j0 - (R - 1) + k;
+				const bool ok = (unsigned) i < (unsigned) n && ((M.present >> i) & 1ull);
+				cc[k] = ok ? M.c[i] : 0.0;
+				vm |= ok ? (1u << k) : 0u;
+			}
 #pragma unroll
-		for (int jj = 0; jj < R; jj++) {
-			const int j = j0 + jj;
-			if (j < n + R - 1) {
-				double v;
-				if (VERT) {
-					const int sy = clampi(y0 + d0 + j, 0, P.h - 1);
-					v = (double) ((const T *) (base + (size_t) sy * P.in_bpl))[e];
-				}
-				else {
-					const int sx = clampi(x0 + d0 + j, 0, P.w - 1);
-					v = (double) row[sx * P.bands + b];
-				}
+			for (int jj = 0; jj < R; jj++) {
+				const int j = j0 + jj;
+				if (j < n + R - 1) {
+					double v;
+					if (VERT) {
+						const int sy = clampi(y0 + d0 + j, 0, P.h - 1);
+						v = (double) ((const T *) (base + (size_t) sy * P.in_bpl))[e];
+					}
+					else {
+						const int sx = clampi(x0 + d0 + j, 0, P.w - 1);
+						v = (double) row[sx * P.bands + b];
+					}
 #pragma unroll
-				for (int r = 0; r < R; r++) {
-					const int k = jj - r + R - 1;
-					if (vm & (1u << k))
-						acc[r] = __dadd_rn(acc[r], __dmul_rn(cc[k], v));
+					for (int r = 0; r < R; r++) {
+						const int k = jj - r + R - 1;
+						if (vm & (1u << k))
+							acc[r] = __dadd_rn(acc[r], __dmul_rn(cc[k], v));
+					}
 				}
 			}
 		}
-	}
 #pragma unroll
-	for (int r = 0; r < R; r++) {
-		if (VERT) {
-			if (y0 + r < P.h)
-				((float *) ((char *) out + (size_t) (y0 + r) * P.out_bpl))[e] = (float) acc[r];
+		for (int r = 0; r < R; r++) {
+			if (VERT) {
+				if (y0 + r < P.h)
+					((float *) ((char *) out + (size_t) (y0 + r) * P.out_bpl))[e] = (float) acc[r];
+			}
+			else if (x0 + r < P.w)
+				((float *) ((char *) out + (size_t) y0 * P.out_bpl))[(x0 + r) * P.bands + b] = (float) acc[r];
 		}
-		else if (x0 + r < P.w)
-			((float *) ((char *) out + (size_t) y0 * P.out_bpl))[(x0 + r) * P.bands + b] = (float) acc[r];
-	}
+	} while (LOOP && (y0 += y_step) < P.h);
 }
 
 /* The dense case of the above (every mask position is a tap, n >= R: Gaussians): the
@@ -215,7 +222,7 @@ convf_block_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ Li
  * triangle, so nothing is predicated and no multiply-add is issued for a tap that does
  * not exist.  Same arithmetic, same order.
  */
-template <typename T, bool VERT, int R>
+template <typename T, bool VERT, int R, bool LOOP>
 __global__ void __launch_bounds__(128)
 convf_dense_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ LineMask M, const T *__restrict__ in,
 	float *__restrict__ out)
@@ -223,12 +230,13 @@ convf_dense_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ Li
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const int n = M.n;
 	const int d0 = -(n / 2);
-	int e = 0, y0, x0 = 0, b = 0;
+	int e = 0, y_first, y_step, x0 = 0, b = 0;
 	if (VERT) {
 		e = idx;
 		if (e >= P.w * P.bands)
 			return;
-		y0 = blockIdx.y * R;
+		y_first = blockIdx.y * R;
+		y_step = gridDim.y * R;
 	}
 	else {
 		const int groups = (P.w + R - 1) / R;
@@ -237,79 +245,83 @@ convf_dense_kernel(const __grid_constant__ ConvDev P, const __grid_constant__ Li
 		const int pg = idx / P.bands;
 		b = idx - pg * P.bands;
 		x0 = pg * R;
-		y0 = blockIdx.y;
+		y_first = blockIdx.y;
+		y_step = gridDim.y;
 	}
-	const char *base = (const char *) in;
-	const T *row = (const T *) (base + (size_t) y0 * P.in_bpl); /* HORIZ */
-	const bool interior = VERT ? (y0 + d0 >= 0 && y0 + d0 + n + R - 2 < P.h) : (x0 + d0 >= 0 && x0 + d0 + n + R - 2 < P.w);
-	const T *p0 = VERT ? (const T *) (base + (size_t) (y0 + d0) * P.in_bpl) + e : row + (size_t) (x0 + d0) * P.bands + b;
-	const size_t step = VERT ? P.in_bpl / sizeof(T) : (size_t) P.bands;
-	double acc[R];
+	int y0 = y_first;
+	do {
+		const char *base = (const char *) in;
+		const T *row = (const T *) (base + (size_t) y0 * P.in_bpl); /* HORIZ */
+		const bool interior = VERT ? (y0 + d0 >= 0 && y0 + d0 + n + R - 2 < P.h) : (x0 + d0 >= 0 && x0 + d0 + n + R - 2 < P.w);
+		const T *p0 = VERT ? (const T *) (base + (size_t) (y0 + d0) * P.in_bpl) + e : row + (size_t) (x0 + d0) * P.bands + b;
+		const size_t step = VERT ? P.in_bpl / sizeof(T) : (size_t) P.bands;
+		double acc[R];
 #pragma unroll
-	for (int r = 0; r < R; r++)
-		acc[r] = P.offset;
+		for (int r = 0; r < R; r++)
+			acc[r] = P.offset;
 
-	/* the body twice: interior tiles read through one pointer + a constant step, so the loads of a
-	 * group of rows can be issued together; edge tiles clamp every coordinate (VIPS_EXTEND_COPY)
-	 */
-	auto body = [&](auto load) {
-		/* head: rows 0 .. R - 2, outputs r <= row */
+		/* the body twice: interior tiles read through one pointer + a constant step, so the loads of a
+		 * group of rows can be issued together; edge tiles clamp every coordinate (VIPS_EXTEND_COPY)
+		 */
+		auto body = [&](auto load) {
+			/* head: rows 0 .. R - 2, outputs r <= row */
 #pragma unroll
-		for (int j = 0; j < R - 1; j++) {
-			const double v = load(j);
+			for (int j = 0; j < R - 1; j++) {
+				const double v = load(j);
 #pragma unroll
-			for (int r = 0; r <= j; r++)
-				acc[r] = __dadd_rn(acc[r], __dmul_rn(M.c[j - r], v));
-		}
-		/* full rows R - 1 .. n - 1, R at a time with their 2R - 1 coefficients in registers */
-		int j = R - 1;
-		for (; j + R <= n; j += R) {
-			double cc[2 * R - 1];
+				for (int r = 0; r <= j; r++)
+					acc[r] = __dadd_rn(acc[r], __dmul_rn(M.c[j - r], v));
+			}
+			/* full rows R - 1 .. n - 1, R at a time with their 2R - 1 coefficients in registers */
+			int j = R - 1;
+			for (; j + R <= n; j += R) {
+				double cc[2 * R - 1];
 #pragma unroll
-			for (int k = 0; k < 2 * R - 1; k++)
-				cc[k] = M.c[j - (R - 1) + k];
+				for (int k = 0; k < 2 * R - 1; k++)
+					cc[k] = M.c[j - (R - 1) + k];
 #pragma unroll
-			for (int jj = 0; jj < R; jj++) {
-				const double v = load(j + jj);
+				for (int jj = 0; jj < R; jj++) {
+					const double v = load(j + jj);
+#pragma unroll
+					for (int r = 0; r < R; r++)
+						acc[r] = __dadd_rn(acc[r], __dmul_rn(cc[jj - r + R - 1], v));
+				}
+			}
+			for (; j < n; j++) {
+				const double v = load(j);
 #pragma unroll
 				for (int r = 0; r < R; r++)
-					acc[r] = __dadd_rn(acc[r], __dmul_rn(cc[jj - r + R - 1], v));
+					acc[r] = __dadd_rn(acc[r], __dmul_rn(M.c[j - r], v));
 			}
+			/* tail: rows n .. n + R - 2, outputs r > row - n */
+			double ct[R - 1];
+#pragma unroll
+			for (int k = 0; k < R - 1; k++)
+				ct[k] = M.c[n - R + 1 + k];
+#pragma unroll
+			for (int jt = 0; jt < R - 1; jt++) {
+				const double v = load(n + jt);
+#pragma unroll
+				for (int r = jt + 1; r < R; r++)
+					acc[r] = __dadd_rn(acc[r], __dmul_rn(ct[jt - r + R - 1], v));
+			}
+		};
+		if (interior)
+			body([&](int j) -> double { return (double) p0[(size_t) j * step]; });
+		else if (VERT)
+			body([&](int j) -> double { return (double) ((const T *) (base + (size_t) clampi(y0 + d0 + j, 0, P.h - 1) * P.in_bpl))[e]; });
+		else
+			body([&](int j) -> double { return (double) row[clampi(x0 + d0 + j, 0, P.w - 1) * P.bands + b]; });
+#pragma unroll
+		for (int r = 0; r < R; r++) {
+			if (VERT) {
+				if (y0 + r < P.h)
+					((float *) ((char *) out + (size_t) (y0 + r) * P.out_bpl))[e] = (float) acc[r];
+			}
+			else if (x0 + r < P.w)
+				((float *) ((char *) out + (size_t) y0 * P.out_bpl))[(x0 + r) * P.bands + b] = (float) acc[r];
 		}
-		for (; j < n; j++) {
-			const double v = load(j);
-#pragma unroll
-			for (int r = 0; r < R; r++)
-				acc[r] = __dadd_rn(acc[r], __dmul_rn(M.c[j - r], v));
-		}
-		/* tail: rows n .. n + R - 2, outputs r > row - n */
-		double ct[R - 1];
-#pragma unroll
-		for (int k = 0; k < R - 1; k++)
-			ct[k] = M.c[n - R + 1 + k];
-#pragma unroll
-		for (int jt = 0; jt < R - 1; jt++) {
-			const double v = load(n + jt);
-#pragma unroll
-			for (int r = jt + 1; r < R; r++)
-				acc[r] = __dadd_rn(acc[r], __dmul_rn(ct[jt - r + R - 1], v));
-		}
-	};
-	if (interior)
-		body([&](int j) -> double { return (double) p0[(size_t) j * step]; });
-	else if (VERT)
-		body([&](int j) -> double { return (double) ((const T *) (base + (size_t) clampi(y0 + d0 + j, 0, P.h - 1) * P.in_bpl))[e]; });
-	else
-		body([&](int j) -> double { return (double) row[clampi(x0 + d0 + j, 0, P.w - 1) * P.bands + b]; });
-#pragma unroll
-	for (int r = 0; r < R; r++) {
-		if (VERT) {
-			if (y0 + r < P.h)
-				((float *) ((char *) out + (size_t) (y0 + r) * P.out_bpl))[e] = (float) acc[r];
-		}
-		else if (x0 + r < P.w)
-			((float *) ((char *) out + (size_t) y0 * P.out_bpl))[(x0 + r) * P.bands + b] = (float) acc[r];
-	}
+	} while (LOOP && (y0 += y_step) < P.h);
 }
 
 template <typename T>
@@ -318,91 +330,96 @@ convi_kernel(const __grid_constant__ ConvDev P, const T *__restrict__ in, T *__r
 	long long hi, int clip)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= P.w * P.bands)
 		return;
 	const int x = e / P.bands;
 	const int b = e - x * P.bands;
-	long long sum = 0;
-	for (int i = 0; i < P.nnz; i++) {
-		const Tap t = P.taps[i];
-		const int sx = clampi(x + t.dx, 0, P.w - 1);
-		const int sy = clampi(y + t.dy, 0, P.h - 1);
-		const T v = ((const T *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
-		sum += (long long) P.icoeff[i] * (long long) v;
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		long long sum = 0;
+		for (int i = 0; i < P.nnz; i++) {
+			const Tap t = P.taps[i];
+			const int sx = clampi(x + t.dx, 0, P.w - 1);
+			const int sy = clampi(y + t.dy, 0, P.h - 1);
+			const T v = ((const T *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
+			sum += (long long) P.icoeff[i] * (long long) v;
+		}
+		sum = ((sum + P.iscale / 2) / P.iscale) + P.ioffset;
+		if (clip)
+			sum = sum < lo ? lo : (sum > hi ? hi : sum);
+		((T *) ((char *) out + (size_t) y * P.out_bpl))[e] = (T) sum;
 	}
-	sum = ((sum + P.iscale / 2) / P.iscale) + P.ioffset;
-	if (clip)
-		sum = sum < lo ? lo : (sum > hi ? hi : sum);
-	((T *) ((char *) out + (size_t) y * P.out_bpl))[e] = (T) sum;
 }
 
 __global__ void __launch_bounds__(256)
 convi_float_kernel(const __grid_constant__ ConvDev P, const float *__restrict__ in, float *__restrict__ out)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= P.w * P.bands)
 		return;
 	const int x = e / P.bands;
 	const int b = e - x * P.bands;
-	double sum = 0;
-	for (int i = 0; i < P.nnz; i++) {
-		const Tap t = P.taps[i];
-		const int sx = clampi(x + t.dx, 0, P.w - 1);
-		const int sy = clampi(y + t.dy, 0, P.h - 1);
-		const float v = ((const float *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
-		sum = __dadd_rn(sum, __dmul_rn((double) P.icoeff[i], (double) v));
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		double sum = 0;
+		for (int i = 0; i < P.nnz; i++) {
+			const Tap t = P.taps[i];
+			const int sx = clampi(x + t.dx, 0, P.w - 1);
+			const int sy = clampi(y + t.dy, 0, P.h - 1);
+			const float v = ((const float *) ((const char *) in + (size_t) sy * P.in_bpl))[sx * P.bands + b];
+			sum = __dadd_rn(sum, __dmul_rn((double) P.icoeff[i], (double) v));
+		}
+		sum = __dadd_rn(__ddiv_rn(sum, (double) P.iscale), (double) P.ioffset);
+		((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 	}
-	sum = __dadd_rn(__ddiv_rn(sum, (double) P.iscale), (double) P.ioffset);
-	((float *) ((char *) out + (size_t) y * P.out_bpl))[e] = (float) sum;
 }
 
 __global__ void __launch_bounds__(256)
 convi_vector_u8_kernel(const __grid_constant__ ConvDev P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= P.w * P.bands)
 		return;
 	const int x = e / P.bands;
 	const int b = e - x * P.bands;
-	int sum = 1 << (P.exp - 1);
-	for (int i = 0; i < P.nnz; i++) {
-		const Tap t = P.taps[i];
-		const int sx = clampi(x + t.dx, 0, P.w - 1);
-		const int sy = clampi(y + t.dy, 0, P.h - 1);
-		sum += (int) (in + (size_t) sy * P.in_bpl)[sx * P.bands + b] * P.icoeff[i];
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		int sum = 1 << (P.exp - 1);
+		for (int i = 0; i < P.nnz; i++) {
+			const Tap t = P.taps[i];
+			const int sx = clampi(x + t.dx, 0, P.w - 1);
+			const int sy = clampi(y + t.dy, 0, P.h - 1);
+			sum += (int) (in + (size_t) sy * P.in_bpl)[sx * P.bands + b] * P.icoeff[i];
+		}
+		(out + (size_t) y * P.out_bpl)[e] = (uint8_t) clampi((sum >> P.exp) + P.ioffset, 0, 255);
 	}
-	(out + (size_t) y * P.out_bpl)[e] = (uint8_t) clampi((sum >> P.exp) + P.ioffset, 0, 255);
 }
 
 /* band 0 of a short image -> packed 1-band image, and the sharpen merge */
 __global__ void __launch_bounds__(256)
 extract_band0_short_kernel(const short *__restrict__ in, size_t in_bpl, int bands, short *__restrict__ out,
-	size_t out_bpl, int w)
+	size_t out_bpl, int w, int h)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= w)
 		return;
-	((short *) ((char *) out + (size_t) blockIdx.y * out_bpl))[x] =
-		((const short *) ((const char *) in + (size_t) blockIdx.y * in_bpl))[x * bands];
+	for (int y = blockIdx.y; y < h; y += gridDim.y)
+		((short *) ((char *) out + (size_t) y * out_bpl))[x] = ((const short *) ((const char *) in + (size_t) y * in_bpl))[x * bands];
 }
 
 __global__ void __launch_bounds__(256)
 sharpen_kernel(short *__restrict__ labs, size_t labs_bpl, int bands, const short *__restrict__ blur, size_t blur_bpl,
-	const int *__restrict__ lut, int w)
+	const int *__restrict__ lut, int w, int h)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= w)
 		return;
-	short *p = (short *) ((char *) labs + (size_t) blockIdx.y * labs_bpl) + x * bands;
-	const int v1 = *p;
-	const int v2 = ((const short *) ((const char *) blur + (size_t) blockIdx.y * blur_bpl))[x];
-	const int diff = (v1 & 0x7fff) - (v2 & 0x7fff);
-	int o = v1 + __ldg(lut + diff + 32768);
-	o = max(0, min(o, 32767));
-	*p = (short) o;
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		short *p = (short *) ((char *) labs + (size_t) y * labs_bpl) + x * bands;
+		const int v1 = *p;
+		const int v2 = ((const short *) ((const char *) blur + (size_t) y * blur_bpl))[x];
+		const int diff = (v1 & 0x7fff) - (v2 & 0x7fff);
+		int o = v1 + __ldg(lut + diff + 32768);
+		o = max(0, min(o, 32767));
+		*p = (short) o;
+	}
 }
 
 /* vips__image_intize, convi.c:859-923 */
@@ -531,7 +548,7 @@ dev_conv(const char *domain, const DevImage &in, DevImage *out, const double *ma
 	P.bands = in.bands;
 	P.in_bpl = in.bpl;
 	Uploaded u;
-	const dim3 grid((in.w * in.bands + 255) / 256, in.h);
+	const dim3 grid = row_grid(in.w * in.bands, in.h);
 
 	if (precision == VB200_PRECISION_FLOAT) {
 		/* convf.c:303-331: bake the scale in, squeeze zeros */
@@ -577,18 +594,19 @@ dev_conv(const char *domain, const DevImage &in, DevImage *out, const double *ma
 		 */
 		if (!block_ok && upload_taps(domain, pos, mw, mh, &coeff, nullptr, &P, &u, s))
 			return -1;
-		const dim3 grid_h(((in.w + RB - 1) / RB * in.bands + 127) / 128, in.h);
-		const dim3 grid_v((in.w * in.bands + 127) / 128, (in.h + RB - 1) / RB);
+		const dim3 grid_h = row_grid((in.w + RB - 1) / RB * in.bands, in.h, 128);
+		const dim3 grid_v = row_grid(in.w * in.bands, (in.h + RB - 1) / RB, 128);
+		const bool loop_h = rows_loop(in.h), loop_v = rows_loop((in.h + RB - 1) / RB);
 #define CF(T) \
 	do { \
 		if (dense_ok && line_h) \
-			convf_dense_kernel<T, false, RB><<<grid_h, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
+			(loop_h ? convf_dense_kernel<T, false, RB, true> : convf_dense_kernel<T, false, RB, false>)<<<grid_h, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
 		else if (dense_ok && line_v) \
-			convf_dense_kernel<T, true, RB><<<grid_v, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
+			(loop_v ? convf_dense_kernel<T, true, RB, true> : convf_dense_kernel<T, true, RB, false>)<<<grid_v, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
 		else if (block_ok && line_h) \
-			convf_block_kernel<T, false, RB><<<grid_h, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
+			(loop_h ? convf_block_kernel<T, false, RB, true> : convf_block_kernel<T, false, RB, false>)<<<grid_h, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
 		else if (block_ok && line_v) \
-			convf_block_kernel<T, true, RB><<<grid_v, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
+			(loop_v ? convf_block_kernel<T, true, RB, true> : convf_block_kernel<T, true, RB, false>)<<<grid_v, 128, 0, s>>>(P, lm, (const T *) in.data, (float *) out->data); \
 		else if (line_h) \
 			convf_line_kernel<T, false><<<grid, 256, 0, s>>>(P, (const T *) in.data, (float *) out->data); \
 		else if (line_v) \
@@ -829,17 +847,17 @@ dev_sharpen(const char *domain, const DevImage &in, DevImage *out, double sigma,
 	DevImage L, blur;
 	if (!rc)
 		rc = dev_image_new(domain, &L, labs.w, labs.h, 1, VB200_FORMAT_SHORT, VB200_INTERPRETATION_B_W, s);
-	const dim3 grid((labs.w + 255) / 256, labs.h);
+	const dim3 grid = row_grid(labs.w, labs.h);
 	if (!rc) {
 		extract_band0_short_kernel<<<grid, 256, 0, s>>>((const short *) labs.data, labs.bpl, labs.bands, (short *) L.data,
-			L.bpl, labs.w);
+			L.bpl, labs.w, labs.h);
 		count_launch();
 		/* short input: always the exact C path, never the vector one */
 		rc = dev_convsep(domain, L, &blur, m.data(), mw, mh, scale, 0.0, VB200_PRECISION_INTEGER, s, false);
 	}
 	if (!rc) {
 		sharpen_kernel<<<grid, 256, 0, s>>>((short *) labs.data, labs.bpl, labs.bands, (const short *) blur.data, blur.bpl,
-			(const int *) dlut, labs.w);
+			(const int *) dlut, labs.w, labs.h);
 		count_launch();
 		rc = dev_colourspace(domain, labs, out, in.type, VB200_INTERPRETATION_LABS, s);
 		if (!rc && out->data == labs.data) {

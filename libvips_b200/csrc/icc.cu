@@ -1109,14 +1109,18 @@ icc_pixel(const IccJob &J, const void *pin, void *pout)
 
 static_assert(sizeof(IccJob) <= 4096, "IccJob travels as a kernel parameter");
 
+template <bool LOOP>
 __global__ void __launch_bounds__(256)
 icc_kernel(const __grid_constant__ IccJob J, const char *__restrict__ in, size_t in_bpl, size_t in_ps, char *__restrict__ out,
-	size_t out_bpl, size_t out_ps, int w)
+	size_t out_bpl, size_t out_ps, int w, int h)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= w)
 		return;
-	icc_pixel(J, in + (size_t) blockIdx.y * in_bpl + (size_t) x * in_ps, out + (size_t) blockIdx.y * out_bpl + (size_t) x * out_ps);
+	int y = blockIdx.y;
+	do
+		icc_pixel(J, in + (size_t) y * in_bpl + (size_t) x * in_ps, out + (size_t) y * out_bpl + (size_t) x * out_ps);
+	while (LOOP && (y += gridDim.y) < h);
 }
 
 struct JobSpec {
@@ -1252,9 +1256,9 @@ run_icc(const char *domain, const VB200Image *in, VB200Image *out, const JobSpec
 	if (!rc)
 		rc = dev_image_new(domain, &dout, din.w, din.h, ob, of, ot, s);
 	if (!rc) {
-		const dim3 grid((din.w + 255) / 256, din.h);
-		icc_kernel<<<grid, 256, 0, s>>>(J, (const char *) din.data, din.bpl, format_sizeof(din.fmt) * din.bands, (char *) dout.data,
-			dout.bpl, format_sizeof(of) * ob, din.w);
+		const dim3 grid = row_grid(din.w, din.h);
+		(rows_loop(din.h) ? icc_kernel<true> : icc_kernel<false>)<<<grid, 256, 0, s>>>(J, (const char *) din.data, din.bpl, format_sizeof(din.fmt) * din.bands, (char *) dout.data,
+			dout.bpl, format_sizeof(of) * ob, din.w, din.h);
 		const cudaError_t e = cudaGetLastError();
 		if (e != cudaSuccess)
 			rc = cuda_fail(domain, e, "icc_kernel");

@@ -2151,6 +2151,7 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 	auto since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count(); };
 	chunk = (int) std::max<size_t>(1, std::min<size_t>(chunk, coef_budget / std::max<size_t>(1, max_coef * sizeof(short))));
 	chunk = std::min(chunk, n);
+	chunk = std::min(chunk, kMaxBatchFrames); /* the frames of a chunk are gridDim.y / z of its kernels */
 
 	std::atomic<int> bad_frame(-1);
 	int *status = nullptr;

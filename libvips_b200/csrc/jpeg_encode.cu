@@ -708,22 +708,34 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 		unsigned long long *totals = (unsigned long long *) (scratch + o_tot), *lengths = (unsigned long long *) (scratch + o_len);
 		unsigned *counts = (unsigned *) (scratch + o_cnt);
 		const int mcus = G.mcus_x * G.mcus_y;
-		jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, n), 128, 0, s>>>(G, dT, (const unsigned char *) frames, bpl, frame_stride, coef);
-		jpeg_count_kernel<<<dim3((G.blocks + 127) / 128, n), 128, 0, s>>>(G, dT, coef, bits);
-		jpeg_bitscan_kernel<<<n, 1024, 0, s>>>(G.blocks, bits, totals);
-		jpeg_emit_kernel<<<dim3((G.blocks + 127) / 128, n), 128, 0, s>>>(G, dT, coef, bits, totals, (unsigned *) (scratch + o_raw), raw_bytes / 4);
-		jpeg_ffcount_kernel<<<dim3((max_chunks + 127) / 128, n), 128, 0, s>>>(totals, (const unsigned char *) (scratch + o_raw), raw_bytes, max_chunks,
-			counts);
-		jpeg_ffscan_kernel<<<n, 1024, 0, s>>>(totals, max_chunks, counts, (unsigned) header.size(), lengths);
-		jpeg_stuff_kernel<<<dim3((max_chunks + 127) / 128, n), 128, 0, s>>>(totals, (const unsigned char *) (scratch + o_raw), raw_bytes, max_chunks,
-			counts, (const unsigned char *) (scratch + o_hdr), (unsigned) header.size(), (unsigned char *) out, out_stride, lengths);
-		cudaError_t e = cudaGetLastError();
+		/* the frame is gridDim.y (or x) of every kernel: chunks of at most kMaxBatchFrames, each on its slice of the scratch */
+		cudaError_t e = cudaSuccess;
+		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
+			const int cn = std::min(kMaxBatchFrames, n - c0);
+			short *ccoef = coef + (size_t) c0 * G.blocks * 64;
+			unsigned *cbits = bits + (size_t) c0 * G.blocks;
+			unsigned long long *ctotals = totals + c0, *clengths = lengths + c0;
+			unsigned char *craw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
+			unsigned *ccounts = counts + (size_t) c0 * max_chunks;
+			jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, dT, (const unsigned char *) frames + (size_t) c0 * frame_stride, bpl,
+				frame_stride, ccoef);
+			jpeg_count_kernel<<<dim3((G.blocks + 127) / 128, cn), 128, 0, s>>>(G, dT, ccoef, cbits);
+			jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(G.blocks, cbits, ctotals);
+			jpeg_emit_kernel<<<dim3((G.blocks + 127) / 128, cn), 128, 0, s>>>(G, dT, ccoef, cbits, ctotals, (unsigned *) craw, raw_bytes / 4);
+			jpeg_ffcount_kernel<<<dim3((max_chunks + 127) / 128, cn), 128, 0, s>>>(ctotals, craw, raw_bytes, max_chunks, ccounts);
+			jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(ctotals, max_chunks, ccounts, (unsigned) header.size(), clengths);
+			jpeg_stuff_kernel<<<dim3((max_chunks + 127) / 128, cn), 128, 0, s>>>(ctotals, craw, raw_bytes, max_chunks, ccounts,
+				(const unsigned char *) (scratch + o_hdr), (unsigned) header.size(), (unsigned char *) out + (size_t) c0 * out_stride, out_stride,
+				clengths);
+			e = cudaGetLastError();
+			if (e == cudaSuccess)
+				for (int k = 0; k < 7; k++)
+					count_launch();
+		}
 		if (e != cudaSuccess) {
 			cuda_fail(domain, e, "jpeg encode kernels launch");
 			break;
 		}
-		for (int k = 0; k < 7; k++)
-			count_launch();
 		std::vector<unsigned long long> len(n);
 		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
 			cudaStreamSynchronize(s) != cudaSuccess) {

@@ -33,20 +33,21 @@ __global__ void __launch_bounds__(256)
 morph_kernel(const __grid_constant__ MorphDev P, const uint8_t *__restrict__ in, uint8_t *__restrict__ out)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x; /* element (byte) of the row */
-	const int y = blockIdx.y;
 	const int ne = P.w * P.bands;
 	if (e >= ne)
 		return;
 	const int x = e / P.bands, b = e - x * P.bands;
-	int result = DILATE ? 0 : 255;
-	for (int i = 0; i < P.n; i++) {
-		const int dx = __ldg(P.taps + 3 * i), dy = __ldg(P.taps + 3 * i + 1), co = __ldg(P.taps + 3 * i + 2);
-		const int sx = max(0, min(x + dx, P.w - 1)), sy = max(0, min(y + dy, P.h - 1));
-		const int p = in[(size_t) sy * P.in_bpl + (size_t) sx * P.bands + b];
-		const int v = co ? p : ~p;
-		result = DILATE ? (result | v) : (result & v);
+	for (int y = blockIdx.y; y < P.h; y += gridDim.y) {
+		int result = DILATE ? 0 : 255;
+		for (int i = 0; i < P.n; i++) {
+			const int dx = __ldg(P.taps + 3 * i), dy = __ldg(P.taps + 3 * i + 1), co = __ldg(P.taps + 3 * i + 2);
+			const int sx = max(0, min(x + dx, P.w - 1)), sy = max(0, min(y + dy, P.h - 1));
+			const int p = in[(size_t) sy * P.in_bpl + (size_t) sx * P.bands + b];
+			const int v = co ? p : ~p;
+			result = DILATE ? (result | v) : (result & v);
+		}
+		out[(size_t) y * P.out_bpl + e] = (uint8_t) result;
 	}
-	out[(size_t) y * P.out_bpl + e] = (uint8_t) result;
 }
 
 } // namespace
@@ -105,7 +106,7 @@ dev_morph(const char *domain, const DevImage &in, DevImage *out, const double *m
 	P.in_bpl = in.bpl;
 	P.out_bpl = out->bpl;
 	P.taps = (const int *) dt;
-	const dim3 grid((in.w * in.bands + 255) / 256, in.h);
+	const dim3 grid = row_grid(in.w * in.bands, in.h);
 	if (op)
 		morph_kernel<true><<<grid, 256, 0, s>>>(P, (const uint8_t *) in.data, (uint8_t *) out->data);
 	else

@@ -143,15 +143,21 @@ rank_select(const RankDev &P, const typename RankTraits<T>::Key *tile, T *__rest
 	}
 }
 
-template <typename T>
+template <typename T, bool LOOP>
 __global__ void __launch_bounds__(256)
 rank_kernel(const __grid_constant__ RankDev P, const T *__restrict__ in, T *__restrict__ out)
 {
 	extern __shared__ __align__(16) unsigned char rank_smem[];
 	typename RankTraits<T>::Key *tile = reinterpret_cast<typename RankTraits<T>::Key *>(rank_smem);
-	rank_stage<T>(P, in, tile, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x);
-	__syncthreads();
-	rank_select<T>(P, tile, out, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x);
+	/* the whole CTA walks its rows of tiles together through the staged window */
+	int by = blockIdx.y;
+	do {
+		if (by != (int) blockIdx.y)
+			__syncthreads(); /* the previous tile has been read */
+		rank_stage<T>(P, in, tile, blockIdx.x, by, threadIdx.x, blockDim.x);
+		__syncthreads();
+		rank_select<T>(P, tile, out, blockIdx.x, by, threadIdx.x, blockDim.x);
+	} while (LOOP && (by += gridDim.y) < (P.h + P.ty - 1) / P.ty);
 }
 
 constexpr size_t kRankMaxSmem = 200 * 1024;
@@ -202,10 +208,11 @@ template <typename T>
 int
 rank_launch(const char *domain, const RankDev &P, size_t smem, const void *in, void *out, cudaStream_t s)
 {
+	auto kern = rows_loop((P.h + P.ty - 1) / P.ty) ? rank_kernel<T, true> : rank_kernel<T, false>;
 	if (smem > 48 * 1024)
-		VB200_CUDA(domain, cudaFuncSetAttribute(rank_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-	const dim3 grid((P.w + P.tx - 1) / P.tx, (P.h + P.ty - 1) / P.ty);
-	rank_kernel<T><<<grid, 256, smem, s>>>(P, (const T *) in, (T *) out);
+		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+	const dim3 grid = row_grid(P.w, (P.h + P.ty - 1) / P.ty, P.tx);
+	kern<<<grid, 256, smem, s>>>(P, (const T *) in, (T *) out);
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
 		return cuda_fail(domain, e, "rank_kernel");

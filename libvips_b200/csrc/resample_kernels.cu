@@ -72,50 +72,52 @@ fixed_finalize(IT sum)
 
 template <typename T>
 __global__ void __launch_bounds__(256)
-shrinkv_kernel(const T *__restrict__ in, size_t in_bpl, int in_h, T *__restrict__ out, size_t out_bpl, int ne,
-	int vshrink, unsigned int mult8, unsigned long long mult16)
+shrinkv_kernel(const T *__restrict__ in, size_t in_bpl, int in_h, T *__restrict__ out, size_t out_bpl, int out_h,
+	int ne, int vshrink, unsigned int mult8, unsigned long long mult16)
 {
 	typedef typename Acc<T>::type ACC;
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= ne)
 		return;
 
 	const char *base = (const char *) in;
-	ACC sum = 0;
-	for (int k = 0; k < vshrink; k++) {
-		const int row = min(y * vshrink + k, in_h - 1);
-		const T v = ((const T *) (base + (size_t) row * in_bpl))[x];
-		sum += (ACC) v;
-	}
+	for (int y = blockIdx.y; y < out_h; y += gridDim.y) {
+		ACC sum = 0;
+		for (int k = 0; k < vshrink; k++) {
+			const int row = min(y * vshrink + k, in_h - 1);
+			const T v = ((const T *) (base + (size_t) row * in_bpl))[x];
+			sum += (ACC) v;
+		}
 
-	T *q = (T *) ((char *) out + (size_t) y * out_bpl) + x;
-	const int amend = vshrink / 2;
-	if constexpr (sizeof(T) == 1 && !Limits<T>::sgn)
-		*q = (T) ((((unsigned int) ((int) sum + amend)) * mult8) >> 24);
-	else if constexpr (sizeof(T) == 2 && !Limits<T>::sgn)
-		*q = (T) (((unsigned long long) ((int) sum + amend) * mult16) >> 32);
-	else
-		*q = (T) ((sum + (ACC) amend) / (ACC) vshrink);
+		T *q = (T *) ((char *) out + (size_t) y * out_bpl) + x;
+		const int amend = vshrink / 2;
+		if constexpr (sizeof(T) == 1 && !Limits<T>::sgn)
+			*q = (T) ((((unsigned int) ((int) sum + amend)) * mult8) >> 24);
+		else if constexpr (sizeof(T) == 2 && !Limits<T>::sgn)
+			*q = (T) (((unsigned long long) ((int) sum + amend) * mult16) >> 32);
+		else
+			*q = (T) ((sum + (ACC) amend) / (ACC) vshrink);
+	}
 }
 
 template <>
 __global__ void __launch_bounds__(256)
 shrinkv_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_h, float *__restrict__ out, size_t out_bpl,
-	int ne, int vshrink, unsigned int, unsigned long long)
+	int out_h, int ne, int vshrink, unsigned int, unsigned long long)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= ne)
 		return;
 	const char *base = (const char *) in;
-	double sum = 0.0;
-	for (int k = 0; k < vshrink; k++) {
-		const int row = min(y * vshrink + k, in_h - 1);
-		sum = __dadd_rn(sum, (double) ((const float *) (base + (size_t) row * in_bpl))[x]);
+	for (int y = blockIdx.y; y < out_h; y += gridDim.y) {
+		double sum = 0.0;
+		for (int k = 0; k < vshrink; k++) {
+			const int row = min(y * vshrink + k, in_h - 1);
+			sum = __dadd_rn(sum, (double) ((const float *) (base + (size_t) row * in_bpl))[x]);
+		}
+		const double inv = 1.0 / vshrink;
+		((float *) ((char *) out + (size_t) y * out_bpl))[x] = (float) __dmul_rn(sum, inv);
 	}
-	const double inv = 1.0 / vshrink;
-	((float *) ((char *) out + (size_t) y * out_bpl))[x] = (float) __dmul_rn(sum, inv);
 }
 
 /* uchar, 4 elements per thread: one 32-bit load per row, two 16-bit lanes per
@@ -123,25 +125,26 @@ shrinkv_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_h, flo
  */
 __global__ void __launch_bounds__(256)
 shrinkv_u8x4_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_h, uint8_t *__restrict__ out,
-	size_t out_bpl, int nwords, int vshrink, unsigned int mult8)
+	size_t out_bpl, int out_h, int nwords, int vshrink, unsigned int mult8)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= nwords)
 		return;
-	unsigned int lo = 0, hi = 0; /* bytes 0,2 and bytes 1,3 */
-	for (int k = 0; k < vshrink; k++) {
-		const int row = min(y * vshrink + k, in_h - 1);
-		const unsigned int v = __ldg((const unsigned int *) (in + (size_t) row * in_bpl) + x);
-		lo += v & 0x00ff00ffu;
-		hi += (v >> 8) & 0x00ff00ffu;
+	for (int y = blockIdx.y; y < out_h; y += gridDim.y) {
+		unsigned int lo = 0, hi = 0; /* bytes 0,2 and bytes 1,3 */
+		for (int k = 0; k < vshrink; k++) {
+			const int row = min(y * vshrink + k, in_h - 1);
+			const unsigned int v = __ldg((const unsigned int *) (in + (size_t) row * in_bpl) + x);
+			lo += v & 0x00ff00ffu;
+			hi += (v >> 8) & 0x00ff00ffu;
+		}
+		const unsigned int amend = vshrink / 2;
+		const unsigned int b0 = (((lo & 0xffffu) + amend) * mult8) >> 24;
+		const unsigned int b2 = (((lo >> 16) + amend) * mult8) >> 24;
+		const unsigned int b1 = (((hi & 0xffffu) + amend) * mult8) >> 24;
+		const unsigned int b3 = (((hi >> 16) + amend) * mult8) >> 24;
+		((unsigned int *) (out + (size_t) y * out_bpl))[x] = (b0 & 0xff) | ((b1 & 0xff) << 8) | ((b2 & 0xff) << 16) | (b3 << 24);
 	}
-	const unsigned int amend = vshrink / 2;
-	const unsigned int b0 = (((lo & 0xffffu) + amend) * mult8) >> 24;
-	const unsigned int b2 = (((lo >> 16) + amend) * mult8) >> 24;
-	const unsigned int b1 = (((hi & 0xffffu) + amend) * mult8) >> 24;
-	const unsigned int b3 = (((hi >> 16) + amend) * mult8) >> 24;
-	((unsigned int *) (out + (size_t) y * out_bpl))[x] = (b0 & 0xff) | ((b1 & 0xff) << 8) | ((b2 & 0xff) << 16) | (b3 << 24);
 }
 
 /* ------------------------------------------------------------------ shrinkh */
@@ -149,55 +152,57 @@ shrinkv_u8x4_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_h, uin
 template <typename T>
 __global__ void __launch_bounds__(256)
 shrinkh_kernel(const T *__restrict__ in, size_t in_bpl, int in_w, T *__restrict__ out, size_t out_bpl, int out_w,
-	int bands, int hshrink, unsigned int mult8, unsigned long long mult16)
+	int bands, int rows, int hshrink, unsigned int mult8, unsigned long long mult16)
 {
 	typedef typename Acc<T>::type ACC;
 	const int e = blockIdx.x * blockDim.x + threadIdx.x; /* output element on the row */
-	const int y = blockIdx.y;
 	if (e >= out_w * bands)
 		return;
 	const int x = e / bands;
 	const int b = e - x * bands;
-	const T *p = (const T *) ((const char *) in + (size_t) y * in_bpl);
-	T *q = (T *) ((char *) out + (size_t) y * out_bpl) + e;
 	const int amend = hshrink / 2;
+	for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+		const T *p = (const T *) ((const char *) in + (size_t) y * in_bpl);
+		T *q = (T *) ((char *) out + (size_t) y * out_bpl) + e;
 
-	if constexpr (sizeof(T) <= 2) {
-		int sum = amend;
-		for (int k = 0; k < hshrink; k++)
-			sum += p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b];
-		if constexpr (sizeof(T) == 1 && !Limits<T>::sgn)
-			*q = (T) (((unsigned int) sum * mult8) >> 24);
-		else if constexpr (sizeof(T) == 2 && !Limits<T>::sgn)
-			*q = (T) (((unsigned long long) sum * mult16) >> 32);
-		else
+		if constexpr (sizeof(T) <= 2) {
+			int sum = amend;
+			for (int k = 0; k < hshrink; k++)
+				sum += p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b];
+			if constexpr (sizeof(T) == 1 && !Limits<T>::sgn)
+				*q = (T) (((unsigned int) sum * mult8) >> 24);
+			else if constexpr (sizeof(T) == 2 && !Limits<T>::sgn)
+				*q = (T) (((unsigned long long) sum * mult16) >> 32);
+			else
+				*q = (T) (sum / hshrink);
+		}
+		else {
+			long long sum = amend;
+			for (int k = 0; k < hshrink; k++)
+				sum += p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b];
 			*q = (T) (sum / hshrink);
-	}
-	else {
-		long long sum = amend;
-		for (int k = 0; k < hshrink; k++)
-			sum += p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b];
-		*q = (T) (sum / hshrink);
+		}
 	}
 }
 
 template <>
 __global__ void __launch_bounds__(256)
 shrinkh_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_w, float *__restrict__ out, size_t out_bpl,
-	int out_w, int bands, int hshrink, unsigned int, unsigned long long)
+	int out_w, int bands, int rows, int hshrink, unsigned int, unsigned long long)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= out_w * bands)
 		return;
 	const int x = e / bands;
 	const int b = e - x * bands;
-	const float *p = (const float *) ((const char *) in + (size_t) y * in_bpl);
-	double sum = 0.0;
-	for (int k = 0; k < hshrink; k++)
-		sum = __dadd_rn(sum, (double) p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b]);
-	const double inv = 1.0 / hshrink;
-	((float *) ((char *) out + (size_t) y * out_bpl))[e] = (float) __dmul_rn(sum, inv);
+	for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+		const float *p = (const float *) ((const char *) in + (size_t) y * in_bpl);
+		double sum = 0.0;
+		for (int k = 0; k < hshrink; k++)
+			sum = __dadd_rn(sum, (double) p[(size_t) min(x * hshrink + k, in_w - 1) * bands + b]);
+		const double inv = 1.0 / hshrink;
+		((float *) ((char *) out + (size_t) y * out_bpl))[e] = (float) __dmul_rn(sum, inv);
+	}
 }
 
 /* ------------------------------------------------------------------ reducev */
@@ -231,85 +236,88 @@ dp2a_hi_(unsigned coef, unsigned bytes, int acc)
 
 template <typename T>
 __global__ void __launch_bounds__(256)
-reducev_kernel(const T *__restrict__ in, size_t in_bpl, int in_h, T *__restrict__ out, size_t out_bpl, int ne,
-	AxisDev t)
+reducev_kernel(const T *__restrict__ in, size_t in_bpl, int in_h, T *__restrict__ out, size_t out_bpl, int out_rows,
+	int ne, AxisDev t)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= ne)
 		return;
-	const int py = t.first[y] - t.embed;
 	const int n = t.n_point;
 	const char *base = (const char *) in;
-	T *q = (T *) ((char *) out + (size_t) y * out_bpl) + x;
+	for (int y = blockIdx.y; y < out_rows; y += gridDim.y) {
+		const int py = t.first[y] - t.embed;
+		T *q = (T *) ((char *) out + (size_t) y * out_bpl) + x;
 
-	if constexpr (sizeof(T) == 4) {
-		/* 32-bit ints: int64 sum */
-		const short *c = t.ms + (size_t) t.phase[y] * n;
-		long long sum = 0;
-		for (int i = 0; i < n; i++) {
-			const int row = clampi(py + i, 0, in_h - 1);
-			sum += (long long) c[i] * (long long) ((const T *) (base + (size_t) row * in_bpl))[x];
+		if constexpr (sizeof(T) == 4) {
+			/* 32-bit ints: int64 sum */
+			const short *c = t.ms + (size_t) t.phase[y] * n;
+			long long sum = 0;
+			for (int i = 0; i < n; i++) {
+				const int row = clampi(py + i, 0, in_h - 1);
+				sum += (long long) c[i] * (long long) ((const T *) (base + (size_t) row * in_bpl))[x];
+			}
+			*q = fixed_finalize<T, long long>(sum);
 		}
-		*q = fixed_finalize<T, long long>(sum);
-	}
-	else {
-		const short *c = t.ms + (size_t) t.phase[y] * n;
-		int sum = 0;
-		for (int i = 0; i < n; i++) {
-			const int row = clampi(py + i, 0, in_h - 1);
-			sum += (int) c[i] * (int) ((const T *) (base + (size_t) row * in_bpl))[x];
+		else {
+			const short *c = t.ms + (size_t) t.phase[y] * n;
+			int sum = 0;
+			for (int i = 0; i < n; i++) {
+				const int row = clampi(py + i, 0, in_h - 1);
+				sum += (int) c[i] * (int) ((const T *) (base + (size_t) row * in_bpl))[x];
+			}
+			*q = fixed_finalize<T, int>(sum);
 		}
-		*q = fixed_finalize<T, int>(sum);
 	}
 }
 
 template <>
 __global__ void __launch_bounds__(256)
 reducev_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_h, float *__restrict__ out, size_t out_bpl,
-	int ne, AxisDev t)
+	int out_rows, int ne, AxisDev t)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= ne)
 		return;
-	const int py = t.first[y] - t.embed;
 	const int n = t.n_point;
-	const double *c = t.mf + (size_t) t.phase[y] * n;
 	const char *base = (const char *) in;
-	double sum = 0.0;
-	for (int i = 0; i < n; i++) {
-		const int row = clampi(py + i, 0, in_h - 1);
-		sum = __dadd_rn(sum, __dmul_rn(c[i], (double) ((const float *) (base + (size_t) row * in_bpl))[x]));
+	for (int y = blockIdx.y; y < out_rows; y += gridDim.y) {
+		const int py = t.first[y] - t.embed;
+		const double *c = t.mf + (size_t) t.phase[y] * n;
+		double sum = 0.0;
+		for (int i = 0; i < n; i++) {
+			const int row = clampi(py + i, 0, in_h - 1);
+			sum = __dadd_rn(sum, __dmul_rn(c[i], (double) ((const float *) (base + (size_t) row * in_bpl))[x]));
+		}
+		((float *) ((char *) out + (size_t) y * out_bpl))[x] = (float) sum;
 	}
-	((float *) ((char *) out + (size_t) y * out_bpl))[x] = (float) sum;
 }
 
 /* uchar, 4 bytes per thread */
 __global__ void __launch_bounds__(256)
 reducev_u8x4_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_h, uint8_t *__restrict__ out,
-	size_t out_bpl, int nwords, AxisDev t)
+	size_t out_bpl, int out_rows, int nwords, AxisDev t)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= nwords)
 		return;
-	const int py = t.first[y] - t.embed;
 	const int n = t.n_point;
-	const short *c = t.ms + (size_t) t.phase[y] * n;
-	int s0 = 2048, s1 = 2048, s2 = 2048, s3 = 2048;
-	for (int i = 0; i < n; i++) {
-		const int row = clampi(py + i, 0, in_h - 1);
-		const unsigned int v = __ldg((const unsigned int *) (in + (size_t) row * in_bpl) + x);
-		const int ci = c[i];
-		s0 += ci * (int) (v & 0xff);
-		s1 += ci * (int) ((v >> 8) & 0xff);
-		s2 += ci * (int) ((v >> 16) & 0xff);
-		s3 += ci * (int) (v >> 24);
+	for (int y = blockIdx.y; y < out_rows; y += gridDim.y) {
+		const int py = t.first[y] - t.embed;
+		const short *c = t.ms + (size_t) t.phase[y] * n;
+		int s0 = 2048, s1 = 2048, s2 = 2048, s3 = 2048;
+		for (int i = 0; i < n; i++) {
+			const int row = clampi(py + i, 0, in_h - 1);
+			const unsigned int v = __ldg((const unsigned int *) (in + (size_t) row * in_bpl) + x);
+			const int ci = c[i];
+			s0 += ci * (int) (v & 0xff);
+			s1 += ci * (int) ((v >> 8) & 0xff);
+			s2 += ci * (int) ((v >> 16) & 0xff);
+			s3 += ci * (int) (v >> 24);
+		}
+		const unsigned int b0 = clampi(s0 >> 12, 0, 255), b1 = clampi(s1 >> 12, 0, 255);
+		const unsigned int b2 = clampi(s2 >> 12, 0, 255), b3 = clampi(s3 >> 12, 0, 255);
+		((unsigned int *) (out + (size_t) y * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
 	}
-	const unsigned int b0 = clampi(s0 >> 12, 0, 255), b1 = clampi(s1 >> 12, 0, 255);
-	const unsigned int b2 = clampi(s2 >> 12, 0, 255), b3 = clampi(s3 >> 12, 0, 255);
-	((unsigned int *) (out + (size_t) y * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
 }
 
 /* uchar, register-blocked: one thread owns a 4-byte column of kRvRows consecutive output rows and walks the
@@ -329,57 +337,61 @@ reducev_u8_dp2a_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_h, 
 {
 	extern __shared__ __align__(16) unsigned s_c2[]; /* [pairs][kRvRows] */
 	const int n = t.n_point;
-	const int y0 = blockIdx.y * kRvRows;
-	int u0 = 0x7fffffff, u1 = -0x7fffffff;
-#pragma unroll
-	for (int j = 0; j < kRvRows; j++) {
-		const int py = __ldg(t.first + min(y0 + j, out_rows - 1)) - t.embed;
-		u0 = min(u0, py);
-		u1 = max(u1, py + n - 1);
-	}
-	const int npairs = (u1 - u0 + 2) >> 1;
-	for (int idx = threadIdx.x; idx < npairs * kRvRows; idx += kRvThreads) {
-		const int k = idx / kRvRows, j = idx - k * kRvRows;
-		const int yj = min(y0 + j, out_rows - 1);
-		const short *c = t.ms + (size_t) __ldg(t.phase + yj) * n;
-		const int i0 = u0 + 2 * k - (__ldg(t.first + yj) - t.embed);
-		const unsigned lo = i0 >= 0 && i0 < n ? (unsigned short) c[i0] : 0u;
-		const unsigned hi = i0 + 1 >= 0 && i0 + 1 < n ? (unsigned short) c[i0 + 1] : 0u;
-		s_c2[idx] = lo | (hi << 16);
-	}
-	__syncthreads();
 	const int x = blockIdx.x * kRvThreads + threadIdx.x;
-	if (x >= nwords)
-		return;
-	int acc[kRvRows][4];
-#pragma unroll
-	for (int j = 0; j < kRvRows; j++)
-#pragma unroll
-		for (int c = 0; c < 4; c++)
-			acc[j][c] = VB200_INTERPOLATE_SCALE >> 1;
-#pragma unroll 8
-	for (int k = 0; k < npairs; k++) {
-		const int ra = clampi(u0 + 2 * k, 0, in_h - 1), rb = clampi(u0 + 2 * k + 1, 0, in_h - 1);
-		const unsigned va = __ldg((const unsigned *) (in + (size_t) ra * in_bpl) + x);
-		const unsigned vb = __ldg((const unsigned *) (in + (size_t) rb * in_bpl) + x);
-		const unsigned w0 = __byte_perm(va, vb, 0x5140), w1 = __byte_perm(va, vb, 0x7362);
-		const uint4 c4 = *(const uint4 *) (s_c2 + k * kRvRows);
-		const unsigned cj[4] = {c4.x, c4.y, c4.z, c4.w};
+	/* the whole CTA walks its groups of kRvRows output rows together: the pair table is shared */
+	for (int y0 = blockIdx.y * kRvRows; y0 < out_rows; y0 += gridDim.y * kRvRows) {
+		if (y0 != (int) blockIdx.y * kRvRows)
+			__syncthreads(); /* the previous group's pair table has been read */
+		int u0 = 0x7fffffff, u1 = -0x7fffffff;
 #pragma unroll
 		for (int j = 0; j < kRvRows; j++) {
-			acc[j][0] = dp2a_lo_(cj[j], w0, acc[j][0]);
-			acc[j][1] = dp2a_hi_(cj[j], w0, acc[j][1]);
-			acc[j][2] = dp2a_lo_(cj[j], w1, acc[j][2]);
-			acc[j][3] = dp2a_hi_(cj[j], w1, acc[j][3]);
+			const int py = __ldg(t.first + min(y0 + j, out_rows - 1)) - t.embed;
+			u0 = min(u0, py);
+			u1 = max(u1, py + n - 1);
 		}
-	}
+		const int npairs = (u1 - u0 + 2) >> 1;
+		for (int idx = threadIdx.x; idx < npairs * kRvRows; idx += kRvThreads) {
+			const int k = idx / kRvRows, j = idx - k * kRvRows;
+			const int yj = min(y0 + j, out_rows - 1);
+			const short *c = t.ms + (size_t) __ldg(t.phase + yj) * n;
+			const int i0 = u0 + 2 * k - (__ldg(t.first + yj) - t.embed);
+			const unsigned lo = i0 >= 0 && i0 < n ? (unsigned short) c[i0] : 0u;
+			const unsigned hi = i0 + 1 >= 0 && i0 + 1 < n ? (unsigned short) c[i0 + 1] : 0u;
+			s_c2[idx] = lo | (hi << 16);
+		}
+		__syncthreads();
+		if (x >= nwords)
+			continue;
+		int acc[kRvRows][4];
 #pragma unroll
-	for (int j = 0; j < kRvRows; j++)
-		if (y0 + j < out_rows) {
-			const unsigned b0 = clampi(acc[j][0] >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(acc[j][1] >> VB200_INTERPOLATE_SHIFT, 0, 255);
-			const unsigned b2 = clampi(acc[j][2] >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(acc[j][3] >> VB200_INTERPOLATE_SHIFT, 0, 255);
-			((unsigned *) (out + (size_t) (y0 + j) * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+		for (int j = 0; j < kRvRows; j++)
+#pragma unroll
+			for (int c = 0; c < 4; c++)
+				acc[j][c] = VB200_INTERPOLATE_SCALE >> 1;
+#pragma unroll 8
+		for (int k = 0; k < npairs; k++) {
+			const int ra = clampi(u0 + 2 * k, 0, in_h - 1), rb = clampi(u0 + 2 * k + 1, 0, in_h - 1);
+			const unsigned va = __ldg((const unsigned *) (in + (size_t) ra * in_bpl) + x);
+			const unsigned vb = __ldg((const unsigned *) (in + (size_t) rb * in_bpl) + x);
+			const unsigned w0 = __byte_perm(va, vb, 0x5140), w1 = __byte_perm(va, vb, 0x7362);
+			const uint4 c4 = *(const uint4 *) (s_c2 + k * kRvRows);
+			const unsigned cj[4] = {c4.x, c4.y, c4.z, c4.w};
+#pragma unroll
+			for (int j = 0; j < kRvRows; j++) {
+				acc[j][0] = dp2a_lo_(cj[j], w0, acc[j][0]);
+				acc[j][1] = dp2a_hi_(cj[j], w0, acc[j][1]);
+				acc[j][2] = dp2a_lo_(cj[j], w1, acc[j][2]);
+				acc[j][3] = dp2a_hi_(cj[j], w1, acc[j][3]);
+			}
 		}
+#pragma unroll
+		for (int j = 0; j < kRvRows; j++)
+			if (y0 + j < out_rows) {
+				const unsigned b0 = clampi(acc[j][0] >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(acc[j][1] >> VB200_INTERPOLATE_SHIFT, 0, 255);
+				const unsigned b2 = clampi(acc[j][2] >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(acc[j][3] >> VB200_INTERPOLATE_SHIFT, 0, 255);
+				((unsigned *) (out + (size_t) (y0 + j) * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+			}
+	}
 }
 
 /* The same kernel with the block's whole tap window staged in shared memory by bulk copies (cp.async.bulk, one per
@@ -395,6 +407,7 @@ rv_smem_addr(const void *p)
 	return (unsigned) __cvta_generic_to_shared(p);
 }
 
+template <bool LOOP>
 __global__ void __launch_bounds__(kRvThreads)
 reducev_u8_dp2a_staged_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_h, uint8_t *__restrict__ out, size_t out_bpl, int nwords,
 	int out_rows, AxisDev t, int max_pairs)
@@ -404,15 +417,6 @@ reducev_u8_dp2a_staged_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int
 	unsigned long long *bar = (unsigned long long *) (s_c2 + (size_t) max_pairs * kRvRows);
 	unsigned *s_rows = (unsigned *) (((uintptr_t) (bar + 1) + 127) & ~(uintptr_t) 127); /* [2 * npairs][kRvThreads] */
 	const int n = t.n_point;
-	const int y0 = blockIdx.y * kRvRows;
-	int u0 = 0x7fffffff, u1 = -0x7fffffff;
-#pragma unroll
-	for (int j = 0; j < kRvRows; j++) {
-		const int py = __ldg(t.first + min(y0 + j, out_rows - 1)) - t.embed;
-		u0 = min(u0, py);
-		u1 = max(u1, py + n - 1);
-	}
-	const int npairs = (u1 - u0 + 2) >> 1;
 	const int x0 = blockIdx.x * kRvThreads;
 	const unsigned row_bytes = (unsigned) min(kRvThreads, nwords - x0) * 4u;
 	const unsigned bar_s = rv_smem_addr(bar);
@@ -421,70 +425,88 @@ reducev_u8_dp2a_staged_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 	}
 	__syncthreads();
-	if (threadIdx.x == 0)
-		asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar_s),
-					 "r"(row_bytes * (unsigned) (2 * npairs))
-					 : "memory");
-	__syncthreads();
-	/* one bulk copy per window row, issued by as many threads as there are rows */
-	for (int r = threadIdx.x; r < 2 * npairs; r += kRvThreads) {
-		const int row = clampi(u0 + r, 0, in_h - 1);
-		asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-						 rv_smem_addr(s_rows + (size_t) r * kRvThreads)),
-					 "l"(in + (size_t) row * in_bpl + (size_t) x0 * 4), "r"(row_bytes), "r"(bar_s)
-					 : "memory");
-	}
-	/* the coefficient pairs of the block's rows, while the copies fly */
-	for (int idx = threadIdx.x; idx < npairs * kRvRows; idx += kRvThreads) {
-		const int k = idx / kRvRows, j = idx - k * kRvRows;
-		const int yj = min(y0 + j, out_rows - 1);
-		const short *c = t.ms + (size_t) __ldg(t.phase + yj) * n;
-		const int i0 = u0 + 2 * k - (__ldg(t.first + yj) - t.embed);
-		const unsigned lo = i0 >= 0 && i0 < n ? (unsigned short) c[i0] : 0u;
-		const unsigned hi = i0 + 1 >= 0 && i0 + 1 < n ? (unsigned short) c[i0 + 1] : 0u;
-		s_c2[idx] = lo | (hi << 16);
-	}
-	__syncthreads();
-	{
-		unsigned done;
-		do {
-			asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, 0x989680;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-						 : "=r"(done)
-						 : "r"(bar_s), "r"(0u)
-						 : "memory");
-		} while (!done);
-	}
-	const int x = x0 + threadIdx.x;
-	if (x >= nwords)
-		return;
-	int acc[kRvRows][4];
-#pragma unroll
-	for (int j = 0; j < kRvRows; j++)
-#pragma unroll
-		for (int c = 0; c < 4; c++)
-			acc[j][c] = VB200_INTERPOLATE_SCALE >> 1;
-	const unsigned *mine = s_rows + threadIdx.x;
-#pragma unroll 4
-	for (int k = 0; k < npairs; k++) {
-		const unsigned va = mine[(size_t) (2 * k) * kRvThreads], vb = mine[(size_t) (2 * k + 1) * kRvThreads];
-		const unsigned w0 = __byte_perm(va, vb, 0x5140), w1 = __byte_perm(va, vb, 0x7362);
-		const uint4 c4 = *(const uint4 *) (s_c2 + k * kRvRows);
-		const unsigned cj[4] = {c4.x, c4.y, c4.z, c4.w};
+	/* the whole CTA walks its groups of kRvRows output rows together; the barrier completes one phase per group */
+	unsigned parity = 0;
+	int y0 = blockIdx.y * kRvRows;
+	do {
+		if (y0 != (int) blockIdx.y * kRvRows) {
+			/* the previous group's rows and pair table have been read before the copies overwrite them */
+			asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+			__syncthreads();
+		}
+		int u0 = 0x7fffffff, u1 = -0x7fffffff;
 #pragma unroll
 		for (int j = 0; j < kRvRows; j++) {
-			acc[j][0] = dp2a_lo_(cj[j], w0, acc[j][0]);
-			acc[j][1] = dp2a_hi_(cj[j], w0, acc[j][1]);
-			acc[j][2] = dp2a_lo_(cj[j], w1, acc[j][2]);
-			acc[j][3] = dp2a_hi_(cj[j], w1, acc[j][3]);
+			const int py = __ldg(t.first + min(y0 + j, out_rows - 1)) - t.embed;
+			u0 = min(u0, py);
+			u1 = max(u1, py + n - 1);
 		}
-	}
+		const int npairs = (u1 - u0 + 2) >> 1;
+		if (threadIdx.x == 0)
+			asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar_s),
+						 "r"(row_bytes * (unsigned) (2 * npairs))
+						 : "memory");
+		__syncthreads();
+		/* one bulk copy per window row, issued by as many threads as there are rows */
+		for (int r = threadIdx.x; r < 2 * npairs; r += kRvThreads) {
+			const int row = clampi(u0 + r, 0, in_h - 1);
+			asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+							 rv_smem_addr(s_rows + (size_t) r * kRvThreads)),
+						 "l"(in + (size_t) row * in_bpl + (size_t) x0 * 4), "r"(row_bytes), "r"(bar_s)
+						 : "memory");
+		}
+		/* the coefficient pairs of the block's rows, while the copies fly */
+		for (int idx = threadIdx.x; idx < npairs * kRvRows; idx += kRvThreads) {
+			const int k = idx / kRvRows, j = idx - k * kRvRows;
+			const int yj = min(y0 + j, out_rows - 1);
+			const short *c = t.ms + (size_t) __ldg(t.phase + yj) * n;
+			const int i0 = u0 + 2 * k - (__ldg(t.first + yj) - t.embed);
+			const unsigned lo = i0 >= 0 && i0 < n ? (unsigned short) c[i0] : 0u;
+			const unsigned hi = i0 + 1 >= 0 && i0 + 1 < n ? (unsigned short) c[i0 + 1] : 0u;
+			s_c2[idx] = lo | (hi << 16);
+		}
+		__syncthreads();
+		{
+			unsigned done;
+			do {
+				asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, 0x989680;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+							 : "=r"(done)
+							 : "r"(bar_s), "r"(parity)
+							 : "memory");
+			} while (!done);
+		}
+		const int x = x0 + threadIdx.x;
+		if (x >= nwords)
+			continue;
+		int acc[kRvRows][4];
 #pragma unroll
-	for (int j = 0; j < kRvRows; j++)
-		if (y0 + j < out_rows) {
-			const unsigned b0 = clampi(acc[j][0] >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(acc[j][1] >> VB200_INTERPOLATE_SHIFT, 0, 255);
-			const unsigned b2 = clampi(acc[j][2] >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(acc[j][3] >> VB200_INTERPOLATE_SHIFT, 0, 255);
-			((unsigned *) (out + (size_t) (y0 + j) * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+		for (int j = 0; j < kRvRows; j++)
+#pragma unroll
+			for (int c = 0; c < 4; c++)
+				acc[j][c] = VB200_INTERPOLATE_SCALE >> 1;
+		const unsigned *mine = s_rows + threadIdx.x;
+#pragma unroll 4
+		for (int k = 0; k < npairs; k++) {
+			const unsigned va = mine[(size_t) (2 * k) * kRvThreads], vb = mine[(size_t) (2 * k + 1) * kRvThreads];
+			const unsigned w0 = __byte_perm(va, vb, 0x5140), w1 = __byte_perm(va, vb, 0x7362);
+			const uint4 c4 = *(const uint4 *) (s_c2 + k * kRvRows);
+			const unsigned cj[4] = {c4.x, c4.y, c4.z, c4.w};
+#pragma unroll
+			for (int j = 0; j < kRvRows; j++) {
+				acc[j][0] = dp2a_lo_(cj[j], w0, acc[j][0]);
+				acc[j][1] = dp2a_hi_(cj[j], w0, acc[j][1]);
+				acc[j][2] = dp2a_lo_(cj[j], w1, acc[j][2]);
+				acc[j][3] = dp2a_hi_(cj[j], w1, acc[j][3]);
+			}
 		}
+#pragma unroll
+		for (int j = 0; j < kRvRows; j++)
+			if (y0 + j < out_rows) {
+				const unsigned b0 = clampi(acc[j][0] >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(acc[j][1] >> VB200_INTERPOLATE_SHIFT, 0, 255);
+				const unsigned b2 = clampi(acc[j][2] >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(acc[j][3] >> VB200_INTERPOLATE_SHIFT, 0, 255);
+				((unsigned *) (out + (size_t) (y0 + j) * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+			}
+	} while (LOOP && (parity ^= 1u, y0 += gridDim.y * kRvRows) < out_rows);
 }
 
 /* uchar RGBA rows: a CTA stages the span of input pixels its kRhThreads output pixels read (clamp addressing =
@@ -500,14 +522,14 @@ rh_pad(int i)
 	return i + (i >> 3);
 }
 
+template <bool LOOP>
 __global__ void __launch_bounds__(kRhThreads)
 reduceh_u8x4_dp2a_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_w, uint8_t *__restrict__ out,
-	size_t out_bpl, int out_w, AxisDev t)
+	size_t out_bpl, int out_w, int rows, AxisDev t)
 {
 	extern __shared__ __align__(16) unsigned s_px[];
 	__shared__ int s_lo, s_hi;
 	const int x = blockIdx.x * kRhThreads + threadIdx.x;
-	const int y = blockIdx.y;
 	const bool live = x < out_w;
 	const int ix = __ldg(t.first + min(x, out_w - 1)) - t.embed;
 	if (threadIdx.x == 0) {
@@ -529,28 +551,34 @@ reduceh_u8x4_dp2a_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_w
 	}
 	__syncthreads();
 	const int p0 = s_lo, span = s_hi - s_lo + 2 * t.npairs; /* an odd tap count reads one word past its window (coefficient 0) */
-	const unsigned *row = (const unsigned *) (in + (size_t) y * in_bpl);
-	for (int i = threadIdx.x; i < span; i += kRhThreads)
-		s_px[rh_pad(i)] = __ldg(row + clampi(p0 + i, 0, in_w - 1));
-	__syncthreads();
-	if (!live)
-		return;
-	const unsigned *cp = t.mp + (size_t) __ldg(t.phase + x) * t.npairs;
 	const int rel = ix - p0;
-	int r = VB200_INTERPOLATE_SCALE >> 1, g = r, b = r, a = r;
+	/* the span depends on the columns only; the whole CTA walks its rows together through the staged row */
+	int y = blockIdx.y;
+	do {
+		if (y != (int) blockIdx.y)
+			__syncthreads(); /* the previous row has been read */
+		const unsigned *row = (const unsigned *) (in + (size_t) y * in_bpl);
+		for (int i = threadIdx.x; i < span; i += kRhThreads)
+			s_px[rh_pad(i)] = __ldg(row + clampi(p0 + i, 0, in_w - 1));
+		__syncthreads();
+		if (!live)
+			continue;
+		const unsigned *cp = t.mp + (size_t) __ldg(t.phase + x) * t.npairs;
+		int r = VB200_INTERPOLATE_SCALE >> 1, g = r, b = r, a = r;
 #pragma unroll 5
-	for (int k = 0; k < t.npairs; k++) {
-		const unsigned pa = s_px[rh_pad(rel + 2 * k)], pb = s_px[rh_pad(rel + 2 * k + 1)];
-		const unsigned w0 = __byte_perm(pa, pb, 0x5140), w1 = __byte_perm(pa, pb, 0x7362);
-		const unsigned c = __ldg(cp + k);
-		r = dp2a_lo_(c, w0, r);
-		g = dp2a_hi_(c, w0, g);
-		b = dp2a_lo_(c, w1, b);
-		a = dp2a_hi_(c, w1, a);
-	}
-	const unsigned b0 = clampi(r >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(g >> VB200_INTERPOLATE_SHIFT, 0, 255);
-	const unsigned b2 = clampi(b >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(a >> VB200_INTERPOLATE_SHIFT, 0, 255);
-	((unsigned *) (out + (size_t) y * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+		for (int k = 0; k < t.npairs; k++) {
+			const unsigned pa = s_px[rh_pad(rel + 2 * k)], pb = s_px[rh_pad(rel + 2 * k + 1)];
+			const unsigned w0 = __byte_perm(pa, pb, 0x5140), w1 = __byte_perm(pa, pb, 0x7362);
+			const unsigned c = __ldg(cp + k);
+			r = dp2a_lo_(c, w0, r);
+			g = dp2a_hi_(c, w0, g);
+			b = dp2a_lo_(c, w1, b);
+			a = dp2a_hi_(c, w1, a);
+		}
+		const unsigned b0 = clampi(r >> VB200_INTERPOLATE_SHIFT, 0, 255), b1 = clampi(g >> VB200_INTERPOLATE_SHIFT, 0, 255);
+		const unsigned b2 = clampi(b >> VB200_INTERPOLATE_SHIFT, 0, 255), b3 = clampi(a >> VB200_INTERPOLATE_SHIFT, 0, 255);
+		((unsigned *) (out + (size_t) y * out_bpl))[x] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
+	} while (LOOP && (y += gridDim.y) < rows);
 }
 
 /* ------------------------------------------------------------------ reduceh */
@@ -558,53 +586,55 @@ reduceh_u8x4_dp2a_kernel(const uint8_t *__restrict__ in, size_t in_bpl, int in_w
 template <typename T>
 __global__ void __launch_bounds__(256)
 reduceh_kernel(const T *__restrict__ in, size_t in_bpl, int in_w, T *__restrict__ out, size_t out_bpl, int out_w,
-	int bands, AxisDev t)
+	int bands, int rows, AxisDev t)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= out_w * bands)
 		return;
 	const int x = e / bands;
 	const int z = e - x * bands;
 	const int ix = t.first[x] - t.embed;
 	const int n = t.n_point;
-	const T *p = (const T *) ((const char *) in + (size_t) y * in_bpl) + z;
-	T *q = (T *) ((char *) out + (size_t) y * out_bpl) + e;
 	const short *c = t.ms + (size_t) t.phase[x] * n;
+	for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+		const T *p = (const T *) ((const char *) in + (size_t) y * in_bpl) + z;
+		T *q = (T *) ((char *) out + (size_t) y * out_bpl) + e;
 
-	if constexpr (sizeof(T) == 4) {
-		long long sum = 0;
-		for (int i = 0; i < n; i++)
-			sum += (long long) c[i] * (long long) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands];
-		*q = fixed_finalize<T, long long>(sum);
-	}
-	else {
-		int sum = 0;
-		for (int i = 0; i < n; i++)
-			sum += (int) c[i] * (int) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands];
-		*q = fixed_finalize<T, int>(sum);
+		if constexpr (sizeof(T) == 4) {
+			long long sum = 0;
+			for (int i = 0; i < n; i++)
+				sum += (long long) c[i] * (long long) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands];
+			*q = fixed_finalize<T, long long>(sum);
+		}
+		else {
+			int sum = 0;
+			for (int i = 0; i < n; i++)
+				sum += (int) c[i] * (int) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands];
+			*q = fixed_finalize<T, int>(sum);
+		}
 	}
 }
 
 template <>
 __global__ void __launch_bounds__(256)
 reduceh_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_w, float *__restrict__ out, size_t out_bpl,
-	int out_w, int bands, AxisDev t)
+	int out_w, int bands, int rows, AxisDev t)
 {
 	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (e >= out_w * bands)
 		return;
 	const int x = e / bands;
 	const int z = e - x * bands;
 	const int ix = t.first[x] - t.embed;
 	const int n = t.n_point;
-	const float *p = (const float *) ((const char *) in + (size_t) y * in_bpl) + z;
 	const double *c = t.mf + (size_t) t.phase[x] * n;
-	double sum = 0.0;
-	for (int i = 0; i < n; i++)
-		sum = __dadd_rn(sum, __dmul_rn(c[i], (double) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands]));
-	((float *) ((char *) out + (size_t) y * out_bpl))[e] = (float) sum;
+	for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+		const float *p = (const float *) ((const char *) in + (size_t) y * in_bpl) + z;
+		double sum = 0.0;
+		for (int i = 0; i < n; i++)
+			sum = __dadd_rn(sum, __dmul_rn(c[i], (double) p[(size_t) clampi(ix + i, 0, in_w - 1) * bands]));
+		((float *) ((char *) out + (size_t) y * out_bpl))[e] = (float) sum;
+	}
 }
 
 /* ------------------------------------------------- premultiply / unpremultiply */
@@ -618,7 +648,7 @@ reduceh_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_w, flo
 template <bool UNPRE>
 __global__ void __launch_bounds__(256)
 premul_u8_kernel(const uint8_t *__restrict__ in, size_t in_bpl, uint8_t *__restrict__ out, size_t out_bpl, int w,
-	int bands, double max_alpha)
+	int h, int bands, double max_alpha)
 {
 	__shared__ int scale[256];
 	{
@@ -631,77 +661,74 @@ premul_u8_kernel(const uint8_t *__restrict__ in, size_t in_bpl, uint8_t *__restr
 	}
 	__syncthreads();
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= w)
 		return;
-	const uint8_t *p = in + (size_t) y * in_bpl + (size_t) x * bands;
-	uint8_t *q = out + (size_t) y * out_bpl + (size_t) x * bands;
-	if (bands == 4) {
-		const unsigned int v = *(const unsigned int *) p;
-		const int s = scale[v >> 24];
-		const unsigned int r = (((v & 0xff) * s + 128) >> 8) & 0xff;
-		const unsigned int g = ((((v >> 8) & 0xff) * s + 128) >> 8) & 0xff;
-		const unsigned int b = ((((v >> 16) & 0xff) * s + 128) >> 8) & 0xff;
-		*(unsigned int *) q = r | (g << 8) | (b << 16) | (v & 0xff000000u);
-		return;
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		const uint8_t *p = in + (size_t) y * in_bpl + (size_t) x * bands;
+		uint8_t *q = out + (size_t) y * out_bpl + (size_t) x * bands;
+		if (bands == 4) {
+			const unsigned int v = *(const unsigned int *) p;
+			const int s = scale[v >> 24];
+			const unsigned int r = (((v & 0xff) * s + 128) >> 8) & 0xff;
+			const unsigned int g = ((((v >> 8) & 0xff) * s + 128) >> 8) & 0xff;
+			const unsigned int b = ((((v >> 16) & 0xff) * s + 128) >> 8) & 0xff;
+			*(unsigned int *) q = r | (g << 8) | (b << 16) | (v & 0xff000000u);
+			continue;
+		}
+		const uint8_t alpha = p[bands - 1];
+		const int s = scale[alpha];
+		int i;
+		for (i = 0; i < bands - 1; i++)
+			q[i] = (uint8_t) ((p[i] * s + 128) >> 8);
+		q[i] = alpha;
 	}
-	const uint8_t alpha = p[bands - 1];
-	const int s = scale[alpha];
-	int i;
-	for (i = 0; i < bands - 1; i++)
-		q[i] = (uint8_t) ((p[i] * s + 128) >> 8);
-	q[i] = alpha;
 }
 
 /* PRE_* : OUT nalpha = (OUT) clip_alpha / max_alpha; q = p * nalpha  (premultiply.c:86-122) */
 template <typename IN>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 8) /* the row loop must not cost occupancy */
 premul_float_kernel(const IN *__restrict__ in, size_t in_bpl, float *__restrict__ out, size_t out_bpl, int w,
-	int bands, double max_alpha)
+	int h, int bands, double max_alpha)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= w)
 		return;
-	const IN *p = (const IN *) ((const char *) in + (size_t) y * in_bpl) + (size_t) x * bands;
-	float *q = (float *) ((char *) out + (size_t) y * out_bpl) + (size_t) x * bands;
-	const IN alpha = p[bands - 1];
-	/* VIPS_CLIP(0, alpha, max_alpha) is evaluated in double, assigned to IN */
-	const IN clip_alpha = (IN) fmax(0.0, fmin(max_alpha, (double) alpha));
-	const float nalpha = (float) __ddiv_rn((double) (float) clip_alpha, max_alpha);
-	int i;
-	for (i = 0; i < bands - 1; i++)
-		q[i] = __fmul_rn((float) p[i], nalpha);
-	q[i] = (float) alpha;
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		const IN *p = (const IN *) ((const char *) in + (size_t) y * in_bpl) + (size_t) x * bands;
+		float *q = (float *) ((char *) out + (size_t) y * out_bpl) + (size_t) x * bands;
+		const IN alpha = p[bands - 1];
+		/* VIPS_CLIP(0, alpha, max_alpha) is evaluated in double, assigned to IN */
+		const IN clip_alpha = (IN) fmax(0.0, fmin(max_alpha, (double) alpha));
+		const float nalpha = (float) __ddiv_rn((double) (float) clip_alpha, max_alpha);
+		int i;
+		for (i = 0; i < bands - 1; i++)
+			q[i] = __fmul_rn((float) p[i], nalpha);
+		q[i] = (float) alpha;
+	}
 }
 
 /* UNPRE_* / FUNPRE_*  (unpremultiply.c:85-183), alpha_band = bands - 1 */
 template <typename IN, bool FP>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 8) /* the row loop must not cost occupancy */
 unpremul_float_kernel(const IN *__restrict__ in, size_t in_bpl, float *__restrict__ out, size_t out_bpl, int w,
-	int bands, double max_alpha)
+	int h, int bands, double max_alpha)
 {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x;
-	const int y = blockIdx.y;
 	if (x >= w)
 		return;
-	const IN *p = (const IN *) ((const char *) in + (size_t) y * in_bpl) + (size_t) x * bands;
-	float *q = (float *) ((char *) out + (size_t) y * out_bpl) + (size_t) x * bands;
-	const IN alpha = p[bands - 1];
-	float factor;
-	if (FP)
-		factor = fabs((double) alpha) < 0.01 ? 0.0f : (float) __ddiv_rn(max_alpha, (double) alpha);
-	else
-		factor = alpha == 0 ? 0.0f : (float) __ddiv_rn(max_alpha, (double) alpha);
-	for (int i = 0; i < bands - 1; i++)
-		q[i] = __fmul_rn(factor, (float) p[i]);
-	q[bands - 1] = (float) fmax(0.0, fmin(max_alpha, (double) alpha));
-}
-
-inline dim3
-row_grid(int elems, int rows, int threads = 256)
-{
-	return dim3((elems + threads - 1) / threads, rows);
+	for (int y = blockIdx.y; y < h; y += gridDim.y) {
+		const IN *p = (const IN *) ((const char *) in + (size_t) y * in_bpl) + (size_t) x * bands;
+		float *q = (float *) ((char *) out + (size_t) y * out_bpl) + (size_t) x * bands;
+		const IN alpha = p[bands - 1];
+		float factor;
+		if (FP)
+			factor = fabs((double) alpha) < 0.01 ? 0.0f : (float) __ddiv_rn(max_alpha, (double) alpha);
+		else
+			factor = alpha == 0 ? 0.0f : (float) __ddiv_rn(max_alpha, (double) alpha);
+		for (int i = 0; i < bands - 1; i++)
+			q[i] = __fmul_rn(factor, (float) p[i]);
+		q[bands - 1] = (float) fmax(0.0, fmin(max_alpha, (double) alpha));
+	}
 }
 
 bool
@@ -819,7 +846,7 @@ int
 run_reducev(const char *domain, const void *in, size_t in_bpl, int in_h, void *out, size_t out_bpl, int ne, int out_rows,
 	int fmt, const AxisDev &d, size_t dp2a_smem, cudaStream_t s)
 {
-#define RV(T) reducev_kernel<T><<<row_grid(ne, out_rows), 256, 0, s>>>((const T *) in, in_bpl, in_h, (T *) out, out_bpl, ne, d)
+#define RV(T) reducev_kernel<T><<<row_grid(ne, out_rows), 256, 0, s>>>((const T *) in, in_bpl, in_h, (T *) out, out_bpl, out_rows, ne, d)
 	switch (fmt) {
 	case VB200_FORMAT_UCHAR:
 		if ((ne & 3) == 0 && aligned4(in, in_bpl) && aligned4(out, out_bpl)) {
@@ -829,18 +856,19 @@ run_reducev(const char *domain, const void *in, size_t in_bpl, int in_h, void *o
 				const size_t smem = dp2a_smem + 8 + 128 + (size_t) 2 * max_pairs * kRvThreads * 4;
 				static bool attr_done = false;
 				if (!attr_done) {
-					cudaFuncSetAttribute(reducev_u8_dp2a_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+					cudaFuncSetAttribute(reducev_u8_dp2a_staged_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+					cudaFuncSetAttribute(reducev_u8_dp2a_staged_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
 					attr_done = true;
 				}
-				reducev_u8_dp2a_staged_kernel<<<dim3((ne / 4 + kRvThreads - 1) / kRvThreads, (out_rows + kRvRows - 1) / kRvRows), kRvThreads, smem,
+				(rows_loop((out_rows + kRvRows - 1) / kRvRows) ? reducev_u8_dp2a_staged_kernel<true> : reducev_u8_dp2a_staged_kernel<false>)<<<row_grid(ne / 4, (out_rows + kRvRows - 1) / kRvRows, kRvThreads), kRvThreads, smem,
 					s>>>((const uint8_t *) in, in_bpl, in_h, (uint8_t *) out, out_bpl, ne / 4, out_rows, d, max_pairs);
 			}
 			else if (dp2a_smem > 0 && dp2a_smem <= 40 * 1024 && out_rows >= 1)
-				reducev_u8_dp2a_kernel<<<dim3((ne / 4 + kRvThreads - 1) / kRvThreads, (out_rows + kRvRows - 1) / kRvRows), kRvThreads,
+				reducev_u8_dp2a_kernel<<<row_grid(ne / 4, (out_rows + kRvRows - 1) / kRvRows, kRvThreads), kRvThreads,
 					dp2a_smem, s>>>((const uint8_t *) in, in_bpl, in_h, (uint8_t *) out, out_bpl, ne / 4, out_rows, d);
 			else
 				reducev_u8x4_kernel<<<row_grid(ne / 4, out_rows), 256, 0, s>>>((const uint8_t *) in, in_bpl, in_h,
-					(uint8_t *) out, out_bpl, ne / 4, d);
+					(uint8_t *) out, out_bpl, out_rows, ne / 4, d);
 		}
 		else
 			RV(uint8_t);
@@ -863,12 +891,12 @@ int
 run_reduceh(const char *domain, const void *in, size_t in_bpl, int in_w, void *out, size_t out_bpl, int bands, int out_cols,
 	int rows, int fmt, const AxisDev &d, size_t dp2a_smem, cudaStream_t s)
 {
-#define RH(T) reduceh_kernel<T><<<row_grid(out_cols * bands, rows), 256, 0, s>>>((const T *) in, in_bpl, in_w, (T *) out, out_bpl, out_cols, bands, d)
+#define RH(T) reduceh_kernel<T><<<row_grid(out_cols * bands, rows), 256, 0, s>>>((const T *) in, in_bpl, in_w, (T *) out, out_bpl, out_cols, bands, rows, d)
 	switch (fmt) {
 	case VB200_FORMAT_UCHAR:
 		if (bands == 4 && aligned4(in, in_bpl) && aligned4(out, out_bpl) && dp2a_smem > 0 && dp2a_smem <= 40 * 1024)
-			reduceh_u8x4_dp2a_kernel<<<dim3((out_cols + kRhThreads - 1) / kRhThreads, rows), kRhThreads, dp2a_smem, s>>>(
-				(const uint8_t *) in, in_bpl, in_w, (uint8_t *) out, out_bpl, out_cols, d);
+			(rows_loop(rows) ? reduceh_u8x4_dp2a_kernel<true> : reduceh_u8x4_dp2a_kernel<false>)<<<row_grid(out_cols, rows, kRhThreads), kRhThreads, dp2a_smem, s>>>(
+				(const uint8_t *) in, in_bpl, in_w, (uint8_t *) out, out_bpl, out_cols, rows, d);
 		else
 			RH(uint8_t);
 		break;
@@ -1024,12 +1052,12 @@ dev_shrinkv(const char *domain, const DevImage &in, DevImage *out, int vshrink, 
 	const unsigned int mult8 = (unsigned int) ((1LL << 32) / ((1 << 8) * (long long) vshrink));
 	const unsigned long long mult16 = ((1ULL << 32) + vshrink - 1) / vshrink;
 
-#define SV(T) shrinkv_kernel<T><<<row_grid(ne, oh), 256, 0, s>>>((const T *) in.data, in.bpl, in.h, (T *) out->data, out->bpl, ne, vshrink, mult8, mult16)
+#define SV(T) shrinkv_kernel<T><<<row_grid(ne, oh), 256, 0, s>>>((const T *) in.data, in.bpl, in.h, (T *) out->data, out->bpl, oh, ne, vshrink, mult8, mult16)
 	switch (in.fmt) {
 	case VB200_FORMAT_UCHAR:
 		if ((ne & 3) == 0 && aligned4(in.data, in.bpl) && aligned4(out->data, out->bpl) && vshrink <= 257)
 			shrinkv_u8x4_kernel<<<row_grid(ne / 4, oh), 256, 0, s>>>((const uint8_t *) in.data, in.bpl, in.h,
-				(uint8_t *) out->data, out->bpl, ne / 4, vshrink, mult8);
+				(uint8_t *) out->data, out->bpl, oh, ne / 4, vshrink, mult8);
 		else
 			SV(uint8_t);
 		break;
@@ -1070,7 +1098,7 @@ dev_shrinkh(const char *domain, const DevImage &in, DevImage *out, int hshrink, 
 	const unsigned int mult8 = (unsigned int) ((1LL << 32) / ((1 << 8) * (long long) hshrink));
 	const unsigned long long mult16 = ((1ULL << 32) + hshrink - 1) / hshrink;
 
-#define SH(T) shrinkh_kernel<T><<<row_grid(ow * in.bands, in.h), 256, 0, s>>>((const T *) in.data, in.bpl, in.w, (T *) out->data, out->bpl, ow, in.bands, hshrink, mult8, mult16)
+#define SH(T) shrinkh_kernel<T><<<row_grid(ow * in.bands, in.h), 256, 0, s>>>((const T *) in.data, in.bpl, in.w, (T *) out->data, out->bpl, ow, in.bands, in.h, hshrink, mult8, mult16)
 	switch (in.fmt) {
 	case VB200_FORMAT_UCHAR: SH(uint8_t); break;
 	case VB200_FORMAT_CHAR: SH(int8_t); break;
@@ -1172,10 +1200,10 @@ dev_premultiply(const char *domain, const DevImage &in, DevImage *out, double ma
 	if (dev_image_new(domain, out, in.w, in.h, in.bands, lut ? VB200_FORMAT_UCHAR : VB200_FORMAT_FLOAT, in.type, s))
 		return -1;
 	const dim3 grid = row_grid(in.w, in.h);
-#define PM(T) premul_float_kernel<T><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.bands, max_alpha)
+#define PM(T) premul_float_kernel<T><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.h, in.bands, max_alpha)
 	if (lut)
 		premul_u8_kernel<false><<<grid, 256, 0, s>>>((const uint8_t *) in.data, in.bpl, (uint8_t *) out->data,
-			out->bpl, in.w, in.bands, max_alpha);
+			out->bpl, in.w, in.h, in.bands, max_alpha);
 	else
 		switch (in.fmt) {
 		case VB200_FORMAT_UCHAR: PM(uint8_t); break;
@@ -1209,10 +1237,10 @@ dev_unpremultiply(const char *domain, const DevImage &in, DevImage *out, double 
 	if (dev_image_new(domain, out, in.w, in.h, in.bands, lut ? VB200_FORMAT_UCHAR : VB200_FORMAT_FLOAT, in.type, s))
 		return -1;
 	const dim3 grid = row_grid(in.w, in.h);
-#define UPM(T, FP) unpremul_float_kernel<T, FP><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.bands, max_alpha)
+#define UPM(T, FP) unpremul_float_kernel<T, FP><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.h, in.bands, max_alpha)
 	if (lut)
 		premul_u8_kernel<true><<<grid, 256, 0, s>>>((const uint8_t *) in.data, in.bpl, (uint8_t *) out->data,
-			out->bpl, in.w, in.bands, max_alpha);
+			out->bpl, in.w, in.h, in.bands, max_alpha);
 	else
 		switch (in.fmt) {
 		case VB200_FORMAT_UCHAR: UPM(uint8_t, false); break;

@@ -2397,7 +2397,9 @@ thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const vo
 			return -1;
 		}
 		const size_t px_in = (size_t) pl->W * pl->H, px_out = (size_t) pl->OW * pl->OH;
-		const int sub = (int) std::max<size_t>(1, std::min<size_t>((size_t) n, ((size_t) 1 << 30) / (px_in * 4)));
+		/* the frames of a sub-batch are gridDim.y of the expand / compact kernels: at most kMaxBatchFrames */
+		const int sub = (int) std::max<size_t>(1,
+			std::min<size_t>(std::min<size_t>((size_t) n, kMaxBatchFrames), ((size_t) 1 << 30) / (px_in * 4)));
 		void *xin = nullptr, *xout = nullptr;
 		if (dev_alloc(domain, &xin, px_in * 4 * sub, s) || dev_alloc(domain, &xout, px_out * 4 * sub, s)) {
 			dev_free(xin, s);
@@ -2408,14 +2410,21 @@ thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const vo
 			const int nf = std::min(sub, n - f0);
 			rgb_expand_kernel<<<dim3((unsigned) ((px_in / 4 + 255) / 256), nf), 256, 0, s>>>(
 				(const uint8_t *) in + (size_t) f0 * in_stride, in_stride, (uint8_t *) xin, px_in * 4, px_in / 4);
+			cudaError_t e = cudaGetLastError();
+			if (e != cudaSuccess) {
+				rc = cuda_fail(domain, e, "rgb_expand_kernel");
+				break;
+			}
 			count_launch();
 			rc = thumbnail_plan_run_fused(domain, pl, xin, px_in * 4, xout, px_out * 4, nf, s);
 			if (!rc) {
 				rgbx_compact_kernel<<<dim3((unsigned) ((px_out + 255) / 256), nf), 256, 0, s>>>((const uint8_t *) xout, px_out * 4,
 					(uint8_t *) out + (size_t) f0 * out_stride, out_stride, px_out);
-				count_launch();
-				if (cudaGetLastError() != cudaSuccess)
-					rc = cuda_fail(domain, cudaGetLastError(), "rgb expand / compact");
+				e = cudaGetLastError();
+				if (e != cudaSuccess)
+					rc = cuda_fail(domain, e, "rgbx_compact_kernel");
+				else
+					count_launch();
 			}
 		}
 		dev_free(xin, s);

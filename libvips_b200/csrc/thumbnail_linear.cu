@@ -669,8 +669,11 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		return -1;
 	}
 	const size_t mid_frame = (size_t) lt->OH * lt->W * lt->bands; /* floats */
-	/* sub-batches keep the scratch near 2 GiB (33.5 MB per 4K frame) and, at small sizes, inside L2 */
-	const int sub = (int) std::max<size_t>(1, std::min<size_t>((size_t) n, ((size_t) 2 << 30) / (mid_frame * 4)));
+	/* sub-batches keep the scratch near 2 GiB (33.5 MB per 4K frame) and, at small sizes, inside L2; the frames of a
+	 * sub-batch are gridDim.z of the V pass and gridDim.y of the H pass, hence at most kMaxBatchFrames
+	 */
+	const int sub = (int) std::max<size_t>(1,
+		std::min<size_t>(std::min<size_t>((size_t) n, kMaxBatchFrames), ((size_t) 2 << 30) / (mid_frame * 4)));
 	float *mid = nullptr;
 	if (dev_alloc(domain, (void **) &mid, mid_frame * 4 * sub, s))
 		return -1;

@@ -31,6 +31,28 @@ int cuda_fail(const char *domain, cudaError_t e, const char *what);
 			return vb200::cuda_fail(domain, e_, #call); \
 	} while (0)
 
+/* CUDA refuses a launch whose gridDim.y or gridDim.z exceeds 65 535.  Whole-image kernels take one CTA row per
+ * `rows` unit (an image row, or a group of rows): row_grid() caps gridDim.y there and the kernels walk
+ * for (y = blockIdx.y; y < rows; y += gridDim.y), so the row count is limited only by memory, and an image of up
+ * to 65 535 units launches exactly one CTA row per unit.  Batches of frames in y / z go in chunks of kMaxBatchFrames.
+ */
+constexpr int kMaxGridY = 65535;
+constexpr int kMaxBatchFrames = 32768;
+inline dim3
+row_grid(int elems, int rows, int threads = 256)
+{
+	return dim3((elems + threads - 1) / threads, rows < kMaxGridY ? rows : kMaxGridY);
+}
+/* Whether row_grid(.., rows) caps the grid.  Kernels whose registers grow when the compiler sees a row loop take a
+ * template flag LOOP = rows_loop(rows): without it their loop advances straight to the end after one row, so an image of
+ * up to kMaxGridY units runs the code it ran with one CTA row per unit.
+ */
+inline bool
+rows_loop(int rows)
+{
+	return rows > kMaxGridY;
+}
+
 cudaStream_t current_stream();
 void count_launch(int n = 1);
 int sm_count(); /* SMs of the device vb200_init selected: grid sizing fills the machine */
