@@ -175,7 +175,7 @@ int vb200_resize(const VB200Image *in, VB200Image *out, double scale, double vsc
 int vb200_premultiply(const VB200Image *in, VB200Image *out, double max_alpha, int uchar_mode);
 int vb200_unpremultiply(const VB200Image *in, VB200Image *out, double max_alpha, int uchar_mode);
 /* reference: vips_thumbnail_image(), resample/thumbnail.c:2000 (image source,
- * no ICC, no crop/rotate).  height <= 0 = width.
+ * no colour management (see vb200_thumbnail_image_icc), no crop/rotate).  height <= 0 = width.
  */
 int vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear);
 
@@ -323,6 +323,58 @@ size_t vb200_thumbnail_plan_bytes_per_frame(const VB200ThumbnailPlan *plan);
  */
 const char *vb200_thumbnail_plan_kernel(const VB200ThumbnailPlan *plan);
 
+/* ------------------------------------------------ thumbnail: colour management
+ *
+ * vips_thumbnail's "input_profile" / "output_profile" / "intent" in non-linear mode (resample/thumbnail.c:733-735,
+ * 929-970).  With an output profile, each frame after the resize runs one of:
+ *   - vips_icc_transform(output_profile, input_profile, embedded = TRUE, depth 8) when the frame embeds a profile or
+ *     input_profile is set.  Its input profile is chosen as vips_icc_set_import does (colour/icc_transform.c:692-752):
+ *     the embedded profile, then input_profile, then the built-in one for the frame's interpretation (sRGB for 3+ bands,
+ *     grey below).  A profile lcms2 would not open, or whose colour space has the wrong band count, is skipped.
+ *   - vips_colourspace(XYZ) then vips_icc_export(output_profile, depth 8) when there is neither.
+ * Profiles are memory blobs (what vips_profile_load / vips_image_get_blob hand on).  The library ships no profile data:
+ * the caller passes the built-in "srgb" / "sgrey" profiles, needed only when selection reaches them.  A transform the
+ * device evaluator declines (see the ICC section) fails the call with -1, the error naming the frame: keep the host path.
+ * Output bands follow the output profile (grey -> 1, RGB -> 3, CMYK -> 4) plus the frame's extra bands (alpha).
+ * Frames are 8-bit sRGB (3+ bands) or B_W (1 / 2 bands), the thumbnail plan's interpretations: vb200_thumbnail_image_icc
+ * returns -1 for an image of any other interpretation (a CMYK image, say, which the reference imports with its CMYK profile).
+ */
+typedef struct {
+	const void *input_profile;	/* thumbnail "input_profile"; NULL = none */
+	size_t input_len;
+	const void *output_profile; /* thumbnail "output_profile"; NULL = colour management off */
+	size_t output_len;
+	const void *builtin_rgb; /* vips_profile_load("srgb"): last resort of the selection for 3+ band frames */
+	size_t builtin_rgb_len;
+	const void *builtin_grey; /* vips_profile_load("sgrey"): the same for 1 / 2 band frames */
+	size_t builtin_grey_len;
+	int intent; /* VB200_INTENT_*; vips_thumbnail's default is RELATIVE */
+} VB200ThumbnailIcc;
+
+/* The ICC stage runs after the thumbnail kernel and before the sharpen stage.  NULL, or a NULL output profile: off.
+ * The profiles are copied.  Not available with linear = 1 (-1).
+ */
+int vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc);
+/* bands of an output frame: the plan's bands, or what the output profile makes of them */
+int vb200_thumbnail_plan_output_bands(const VB200ThumbnailPlan *plan);
+/* the batch calls with each frame's embedded profile (arrays of n_frames; NULL arrays or a NULL / 0-length entry: none) */
+int vb200_thumbnail_batch_device_icc(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
+	size_t out_frame_stride, int n_frames, const void *const *embedded, const size_t *embedded_lens);
+int vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
+	size_t out_frame_stride, int n_frames, const void *const *embedded, const size_t *embedded_lens);
+/* vips_thumbnail_image with colour management; icc NULL = vb200_thumbnail_image.  embedded: the image's ICC blob */
+int vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	const void *embedded, size_t embedded_len);
+/* vips_thumbnail_buffer with colour management: the embedded profile comes from the stream's APP2 segments */
+int vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc);
+/* vips_image_get_blob(VIPS_META_ICC_NAME) of a JPEG stream (foreign/jpeg2vips.c:699-799): the APP2 "ICC_PROFILE" chunks
+ * before the first SOS, by sequence number 1 .. 100, concatenated up to the first missing one.  Host only, no GPU.
+ * 0 with *profile_len = 0: no profile; out = NULL only reports the length; -1 when cap is too small or the stream is
+ * not a JPEG.
+ */
+int vb200_jpeg_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len);
+
 /* test hook, host only: the sRGB <-> HSV per-pixel code of colour_ext.cu on the CPU; n pixels of 3 bytes */
 int vb200_debug_hsv_host(const void *in, size_t n, int to_hsv, void *out);
 
@@ -402,10 +454,22 @@ int vb200_icc_export(const VB200Image *in, VB200Image *out, const void *profile,
 int vb200_icc_transform(const VB200Image *in, VB200Image *out, const void *in_profile, size_t in_len,
 	const void *out_profile, size_t out_len, int intent, int depth);
 /* Test hook, host only: the evaluator's per-pixel code on the CPU over n packed pixels
- * (mode 0 import, 1 export, 2 transform; pa / pb = the profile(s)); returns the output band count.
+ * (mode 0 import, 1 export, 2 transform, 3 vips_colourspace(XYZ) of 8-bit sRGB (3+ bands) or B_W (1 / 2 bands) then
+ * export with the XYZ PCS -- the thumbnail's branch without an input profile; pa / pb = the profile(s));
+ * returns the output band count.
  */
 int vb200_debug_icc_eval(int mode, const void *in, int in_fmt, int in_bands, void *out, int n, const void *pa, size_t la,
 	const void *pb, size_t lb, int intent, int depth, int pcs);
+/* Test hooks, host only: the thumbnail's input-profile selection for one frame (0: transform with the profile *source names,
+ * 0 embedded / 1 input_profile / 2 built-in; 1: no input profile, the XYZ export; -1: error), and its per-profile check
+ * (0 usable, 1 skipped as the reference skips it, 2 kept by the reference with the header's intent instead).
+ */
+int vb200_debug_icc_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source);
+int vb200_debug_icc_classify(const void *profile, size_t len, int want_bands, int intent);
+/* with env VB200_ICC_TIMING set: CUDA-event milliseconds of the calling thread's last ICC stage of a thumbnail plan
+ * (its icc_frames_kernel launches, from the first to the last); -1 when none was timed
+ */
+float vb200_debug_icc_stage_ms(void);
 
 /* Test hook, host only (no GPU, no CUDA call): the reducev geometry, sampling table and
  * tensor-pipe tables of a vertical thumbnail shrink exactly as a plan builds them, so that the CPU

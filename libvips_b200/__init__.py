@@ -53,6 +53,47 @@ class CMask(C.Structure):
                 ("offset", C.c_double)]
 
 
+class CThumbnailIcc(C.Structure):
+    _fields_ = [("input_profile", C.c_char_p), ("input_len", C.c_size_t), ("output_profile", C.c_char_p), ("output_len", C.c_size_t),
+                ("builtin_rgb", C.c_char_p), ("builtin_rgb_len", C.c_size_t), ("builtin_grey", C.c_char_p),
+                ("builtin_grey_len", C.c_size_t), ("intent", C.c_int)]
+
+
+def thumbnail_icc(output_profile=None, input_profile=None, intent="relative", builtin_profiles=None):
+    """The VB200ThumbnailIcc of vips_thumbnail's output_profile / input_profile / intent (profiles are bytes);
+    builtin_profiles: {"srgb": bytes, "sgrey": bytes}, what vips_profile_load gives for those names.  None when
+    colour management is off."""
+    if output_profile is None:
+        return None
+    b = builtin_profiles or {}
+    blob = lambda p: (bytes(p), len(p)) if p is not None else (None, 0)
+    i, o, r, g = blob(input_profile), blob(output_profile), blob(b.get("srgb")), blob(b.get("sgrey"))
+    return CThumbnailIcc(i[0], i[1], o[0], o[1], r[0], r[1], g[0], g[1], INTENTS[intent] if isinstance(intent, str) else int(intent))
+
+
+def _embedded_arrays(embedded, n):
+    """per-frame embedded profiles (a list of bytes / None) as the pointer and length arrays the C ABI takes"""
+    if embedded is None:
+        return None, None, None
+    assert len(embedded) == n
+    keep = [C.create_string_buffer(bytes(e), len(e)) if e else None for e in embedded]
+    ptrs = (C.c_void_p * n)(*[C.cast(k, C.c_void_p) if k is not None else None for k in keep])
+    lens = (C.c_size_t * n)(*[len(e) if e else 0 for e in embedded])
+    return keep, ptrs, lens
+
+
+def jpeg_icc_profile(stream):
+    """vips_image_get_blob(VIPS_META_ICC_NAME) of a JPEG stream (its APP2 ICC_PROFILE chunks): bytes, or None; no GPU"""
+    stream = bytes(stream)
+    n = C.c_size_t()
+    _check(lib().vb200_jpeg_icc_profile(stream, len(stream), None, 0, C.byref(n)))
+    if n.value == 0:
+        return None
+    out = C.create_string_buffer(n.value)
+    _check(lib().vb200_jpeg_icc_profile(stream, len(stream), out, n.value, C.byref(n)))
+    return out.raw[:n.value]
+
+
 class CReduceParams(C.Structure):
     _fields_ = [("n_point", C.c_int), ("kernel", C.c_int), ("residual_shrink", C.c_double),
                 ("offset", C.c_double)]
@@ -120,6 +161,17 @@ def lib():
                                                    C.c_int]
         L.vb200_thumbnail_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                                  C.c_int]
+        TI = C.POINTER(CThumbnailIcc)
+        L.vb200_thumbnail_plan_set_icc.argtypes = [C.c_void_p, TI]
+        L.vb200_thumbnail_plan_output_bands.argtypes = [C.c_void_p]
+        L.vb200_thumbnail_batch_device_icc.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int,
+                                                       C.c_void_p, C.c_void_p]
+        L.vb200_thumbnail_batch_host_icc.argtypes = L.vb200_thumbnail_batch_device_icc.argtypes
+        L.vb200_thumbnail_image_icc.argtypes = [IP, IP, C.c_int, C.c_int, C.c_int, TI, C.c_char_p, C.c_size_t]
+        L.vb200_thumbnail_buffer_icc.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int, TI]
+        L.vb200_jpeg_icc_profile.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_icc_select.argtypes = [TI, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int)]
+        L.vb200_debug_icc_classify.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_int]
         RP = C.POINTER(CRegion)
         L.vb200_reducev_gen.argtypes = [RP, RP, C.POINTER(CReduceParams)]
         L.vb200_reduceh_gen.argtypes = [RP, RP, C.POINTER(CReduceParams)]
@@ -293,8 +345,18 @@ class Image:
     def unpremultiply(self, max_alpha=0.0, uchar=False):
         return self._call(lib().vb200_unpremultiply, float(max_alpha), int(uchar))
 
-    def thumbnail_image(self, width, height=None, size="both", linear=False):
-        return self._call(lib().vb200_thumbnail_image, int(width), int(height or 0), SIZES[size], int(linear))
+    def thumbnail_image(self, width, height=None, size="both", linear=False, output_profile=None, input_profile=None,
+                        intent="relative", embedded_profile=None, builtin_profiles=None):
+        """vips_thumbnail_image; with output_profile, colour-managed as vips_thumbnail does (embedded_profile: the image's
+        ICC blob; builtin_profiles: {"srgb": bytes, "sgrey": bytes})"""
+        icc = thumbnail_icc(output_profile, input_profile, intent, builtin_profiles)
+        if icc is None or linear:
+            if icc is not None:
+                raise Error("linear thumbnails with an output profile are not supported on the device path")
+            return self._call(lib().vb200_thumbnail_image, int(width), int(height or 0), SIZES[size], int(linear))
+        emb = bytes(embedded_profile) if embedded_profile else None
+        return self._call(lib().vb200_thumbnail_image_icc, int(width), int(height or 0), SIZES[size], C.byref(icc), emb,
+                          len(emb) if emb else 0)
 
     # ---- convolution
     @staticmethod
@@ -468,12 +530,19 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
     return [out[i, :lens[i]].tobytes() for i in range(n)]
 
 
-def thumbnail_buffer(stream, width, height=None, size="both"):
-    """vips_thumbnail_buffer() of a JPEG stream: shrink-on-load decode + thumbnail on the device -> uint8 array"""
+def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
+                     builtin_profiles=None):
+    """vips_thumbnail_buffer() of a JPEG stream: shrink-on-load decode + thumbnail on the device -> uint8 array; with
+    output_profile, colour-managed with the profile the stream embeds"""
     stream = bytes(stream)
     out = CImage()
     out.where = HOST
-    _check(lib().vb200_thumbnail_buffer(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size]))
+    icc = thumbnail_icc(output_profile, input_profile, intent, builtin_profiles)
+    if icc is None:
+        _check(lib().vb200_thumbnail_buffer(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size]))
+    else:
+        _check(lib().vb200_thumbnail_buffer_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
+                                                C.byref(icc)))
     n = out.Ysize * out.bpl
     a = np.frombuffer(C.string_at(out.data, n), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
     a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
@@ -503,6 +572,7 @@ class ThumbnailPlan:
         lib().vb200_thumbnail_plan_output(self._p, C.byref(ow), C.byref(oh))
         self.out_width, self.out_height = ow.value, oh.value
         self.in_frame_bytes = width * height * bands
+        self.out_bands = bands
         self.out_frame_bytes = self.out_width * self.out_height * bands
         self.bytes_per_frame = int(lib().vb200_thumbnail_plan_bytes_per_frame(self._p))
         self.fused = bool(lib().vb200_thumbnail_plan_is_fused(self._p))
@@ -512,6 +582,14 @@ class ThumbnailPlan:
         """vips_sharpen appended to every batch of this plan (sigma <= 0: off); BASELINE config 5"""
         _check(lib().vb200_thumbnail_plan_set_sharpen(self._p, float(sigma), float(x1), float(y2), float(y3), float(m1),
                                                       float(m2)))
+
+    def set_icc(self, output_profile=None, input_profile=None, intent="relative", builtin_profiles=None):
+        """vips_thumbnail's colour management for every batch of this plan (output_profile None: off); out_bands and
+        out_frame_bytes follow the output profile"""
+        icc = thumbnail_icc(output_profile, input_profile, intent, builtin_profiles)
+        _check(lib().vb200_thumbnail_plan_set_icc(self._p, C.byref(icc) if icc is not None else None))
+        self.out_bands = int(lib().vb200_thumbnail_plan_output_bands(self._p))
+        self.out_frame_bytes = self.out_width * self.out_height * self.out_bands
 
     def close(self):
         if self._p:
@@ -524,15 +602,27 @@ class ThumbnailPlan:
         except Exception:
             pass
 
-    def run_device(self, in_ptr, out_ptr, n_frames, in_stride=None, out_stride=None):
-        """Device pointers (ints); queued on the stream set with set_stream()."""
-        _check(lib().vb200_thumbnail_batch_device(self._p, C.c_void_p(in_ptr), in_stride or self.in_frame_bytes,
-                                                  C.c_void_p(out_ptr), out_stride or self.out_frame_bytes,
-                                                  n_frames))
+    def run_device(self, in_ptr, out_ptr, n_frames, in_stride=None, out_stride=None, embedded=None):
+        """Device pointers (ints); queued on the stream set with set_stream().  embedded: each frame's ICC profile
+        (bytes or None) for the colour-management stage"""
+        if embedded is None:
+            _check(lib().vb200_thumbnail_batch_device(self._p, C.c_void_p(in_ptr), in_stride or self.in_frame_bytes,
+                                                      C.c_void_p(out_ptr), out_stride or self.out_frame_bytes,
+                                                      n_frames))
+            return
+        keep, ptrs, lens = _embedded_arrays(embedded, n_frames)
+        _check(lib().vb200_thumbnail_batch_device_icc(self._p, C.c_void_p(in_ptr), in_stride or self.in_frame_bytes,
+                                                      C.c_void_p(out_ptr), out_stride or self.out_frame_bytes, n_frames,
+                                                      ptrs, lens))
 
-    def run_host_ptr(self, in_ptr, out_ptr, n_frames):
-        _check(lib().vb200_thumbnail_batch_host(self._p, C.c_void_p(in_ptr), self.in_frame_bytes,
-                                                C.c_void_p(out_ptr), self.out_frame_bytes, n_frames))
+    def run_host_ptr(self, in_ptr, out_ptr, n_frames, embedded=None):
+        if embedded is None:
+            _check(lib().vb200_thumbnail_batch_host(self._p, C.c_void_p(in_ptr), self.in_frame_bytes,
+                                                    C.c_void_p(out_ptr), self.out_frame_bytes, n_frames))
+            return
+        keep, ptrs, lens = _embedded_arrays(embedded, n_frames)
+        _check(lib().vb200_thumbnail_batch_host_icc(self._p, C.c_void_p(in_ptr), self.in_frame_bytes, C.c_void_p(out_ptr),
+                                                    self.out_frame_bytes, n_frames, ptrs, lens))
 
     def run_jpeg(self, streams, shrink, out_ptr=None):
         """JPEG streams decoded at `shrink` on the device and thumbnailed by this plan (made for the decoded
@@ -542,17 +632,17 @@ class ThumbnailPlan:
             _check(lib().vb200_thumbnail_plan_run_jpeg(self._p, b.ptrs, b.lens, b.n, int(shrink), C.c_void_p(out_ptr), DEVICE,
                                                        self.out_frame_bytes))
             return None
-        out = np.empty((b.n, self.out_height, self.out_width, self.bands), np.uint8)
+        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
         _check(lib().vb200_thumbnail_plan_run_jpeg(self._p, b.ptrs, b.lens, b.n, int(shrink), out.ctypes.data_as(C.c_void_p), HOST,
                                                    self.out_frame_bytes))
         return out
 
-    def run_host(self, frames):
-        """frames: uint8 array [n, H, W, bands] in host memory -> [n, OH, OW, bands]."""
+    def run_host(self, frames, embedded=None):
+        """frames: uint8 array [n, H, W, bands] in host memory -> [n, OH, OW, out_bands]."""
         frames = np.ascontiguousarray(frames)
         assert frames.dtype == np.uint8 and frames.shape[1:] == (self.height, self.width, self.bands)
-        out = np.empty((frames.shape[0], self.out_height, self.out_width, self.bands), np.uint8)
-        self.run_host_ptr(frames.ctypes.data, out.ctypes.data, frames.shape[0])
+        out = np.empty((frames.shape[0], self.out_height, self.out_width, self.out_bands), np.uint8)
+        self.run_host_ptr(frames.ctypes.data, out.ctypes.data, frames.shape[0], embedded)
         return out
 
 

@@ -25,9 +25,11 @@
  * One source, two targets: the per-pixel evaluation below is __host__ __device__, the kernels call it
  * per thread and vb200_debug_icc_eval calls it on the CPU, so the CPU test-suite exercises the same code.
  */
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "vb200_internal.h"
@@ -973,9 +975,23 @@ sat16(double v)
 	return v < 0.0 ? 0.0 : (v > 65535.0 ? 65535.0 : v);
 }
 
+/* float multiply / add without FMA contraction on either target (the reference's float steps round each operation) */
+#ifdef __CUDA_ARCH__
+#define FMUL_RN(a, b) __fmul_rn((a), (b))
+#define FADD_RN(a, b) __fadd_rn((a), (b))
+#else
+#define FMUL_RN(a, b) ((float) (a) * (float) (b))
+#define FADD_RN(a, b) ((float) (a) + (float) (b))
+#endif
+
+enum { MODE_IMPORT = 0, MODE_EXPORT = 1, MODE_TRANSFORM = 2, MODE_XYZ_EXPORT = 3 };
+
 struct IccJob {
 	IccSide in, out; /* whichever the mode uses */
-	int mode;		 /* 0 import, 1 export, 2 transform */
+	/* 0 import, 1 export, 2 transform, 3 vips_colourspace(sRGB or B_W -> XYZ) then export with XYZ PCS (thumbnail.c:957-970:
+	 * an 8-bit image without an input profile); in mode 3, in.bands is 3 (sRGB) or 1 (B_W) and in_tab the sRGB2scRGB table
+	 */
+	int mode;
 	int pcs_xyz;	 /* import / export: the vips PCS is XYZ (D65, Y = 100), else Lab */
 	int in_fmt, depth;
 	/* integer input / output through a matrix or grey profile: the TRCs tabulated once on the host
@@ -1039,8 +1055,22 @@ icc_colour(const IccJob &J, const void *pin, void *pout)
 		}
 		return;
 	}
-	if (J.mode == 1) {
-		const float *p = (const float *) pin;
+	float vxyz[3];
+	if (J.mode == MODE_XYZ_EXPORT) {
+		/* BW2sRGB (a grey pixel as three equal bands), vips_col_sRGB2scRGB_8 (sRGB2scRGB.c:71-107: the 8-bit table), then
+		 * scRGB2XYZ.c:58-79 in float -- the route kernel's steps, evaluated operation by operation
+		 */
+		const uint8_t *q = (const uint8_t *) pin;
+		float rgb[3];
+		for (int c = 0; c < 3; c++)
+			rgb[c] = J.in.pool[J.in_tab + q[J.in.bands == 1 ? 0 : c]];
+		const float R = FMUL_RN(rgb[0], 100.0F), G = FMUL_RN(rgb[1], 100.0F), B = FMUL_RN(rgb[2], 100.0F);
+		vxyz[0] = FADD_RN(FADD_RN(FMUL_RN(0.4124F, R), FMUL_RN(0.3576F, G)), FMUL_RN(0.1805F, B));
+		vxyz[1] = FADD_RN(FADD_RN(FMUL_RN(0.2126F, R), FMUL_RN(0.7152F, G)), FMUL_RN(0.0722F, B));
+		vxyz[2] = FADD_RN(FADD_RN(FMUL_RN(0.0193F, R), FMUL_RN(0.1192F, G)), FMUL_RN(0.9505F, B));
+	}
+	if (J.mode == MODE_EXPORT || J.mode == MODE_XYZ_EXPORT) {
+		const float *p = J.mode == MODE_XYZ_EXPORT ? vxyz : (const float *) pin;
 		if (!J.pcs_xyz) {
 			const double lab[3] = {p[0], p[1], p[2]};
 			lab2xyz(lab, xyz);
@@ -1090,6 +1120,11 @@ icc_pixel(const IccJob &J, const void *pin, void *pout)
 		double v = J.in_fmt == VB200_FORMAT_UCHAR ? (double) ((const uint8_t *) pin)[in_bands + e]
 			: J.in_fmt == VB200_FORMAT_USHORT	  ? (double) ((const uint16_t *) pin)[in_bands + e]
 												  : (double) ((const float *) pin)[in_bands + e];
+		if (J.mode == MODE_XYZ_EXPORT) {
+			/* vips_colour_build on the route's two float steps: sRGB (255) -> scRGB (1.0) -> XYZ (255) */
+			v = (double) FADD_RN(FMUL_RN((float) (1.0 / 255.0), (float) v), 0.0f);
+			v = (double) FADD_RN(FMUL_RN(255.0f, (float) v), 0.0f);
+		}
 		if (J.alpha_rescale) {
 			const float scaled = J.alpha_a * (float) v + 0.0f;
 			v = (double) scaled;
@@ -1157,9 +1192,26 @@ build_job(const char *domain, const JobSpec &sp, int in_fmt, int in_bands, int i
 		}
 		J->extra = in_bands - J->in.bands;
 	}
-	if (sp.mode == 1 || sp.mode == 2) {
-		const void *p = sp.mode == 1 ? sp.pa : sp.pb;
-		const size_t l = sp.mode == 1 ? sp.la : sp.lb;
+	if (sp.mode == MODE_XYZ_EXPORT) {
+		if (in_fmt != VB200_FORMAT_UCHAR || in_bands < 1) {
+			error(domain, "the XYZ export of a thumbnail wants an 8-bit image");
+			return -1;
+		}
+		J->pcs_xyz = 1;
+		J->in.bands = in_bands < 3 ? 1 : 3; /* B_W or sRGB, as the thumbnail's processing space */
+		J->extra = in_bands - J->in.bands;
+		/* the 8-bit sRGB2scRGB table, calcul_tables (LabQ2sRGB.c:130-159) as colour.cu builds it */
+		J->in_tab = (int) pool.size();
+		J->in_tab_n = 256;
+		for (int i = 0; i < 256; i++) {
+			const float f = (float) i / 255;
+			pool.push_back(f <= 0.04045 ? f / 12.92F : powf((f + 0.055F) / (1 + 0.055F), 2.4F));
+		}
+		in_type = VB200_INTERPRETATION_XYZ; /* the export's input; the route's own alpha steps are in icc_pixel */
+	}
+	if (sp.mode == 1 || sp.mode == 2 || sp.mode == MODE_XYZ_EXPORT) {
+		const void *p = sp.mode == 2 ? sp.pb : sp.pa;
+		const size_t l = sp.mode == 2 ? sp.lb : sp.la;
 		if (parse_side(domain, p, l, sp.intent, false, sp.mode == 1 && !sp.pcs_xyz, &J->out, pool))
 			return -1;
 	}
@@ -1192,7 +1244,9 @@ build_job(const char *domain, const JobSpec &sp, int in_fmt, int in_bands, int i
 		*out_bands += J->extra;
 	}
 	/* tabulate the TRCs for integer codes (the curves read `pool` themselves: evaluate against the host copy) */
-	J->in_tab = J->out_thr = -1;
+	J->out_thr = -1;
+	if (sp.mode != MODE_XYZ_EXPORT)
+		J->in_tab = -1;
 	const bool tabulate = getenv("VB200_NO_ICC_TABLES") == nullptr;
 	if (tabulate && (sp.mode == 0 || sp.mode == 2) && (J->in.model == MODEL_MATRIX || J->in.model == MODEL_GREY) &&
 		(in_fmt == VB200_FORMAT_UCHAR || in_fmt == VB200_FORMAT_USHORT)) {
@@ -1205,7 +1259,7 @@ build_job(const char *domain, const JobSpec &sp, int in_fmt, int in_bands, int i
 		J->in_tab_n = n;
 		pool.insert(pool.end(), tab.begin(), tab.end());
 	}
-	if (tabulate && (sp.mode == 1 || sp.mode == 2) && (J->out.model == MODEL_MATRIX || J->out.model == MODEL_GREY)) {
+	if (tabulate && sp.mode != MODE_IMPORT && (J->out.model == MODEL_MATRIX || J->out.model == MODEL_GREY)) {
 		const int n = sp.depth == 8 ? 256 : 65536;
 		std::vector<float> thr((size_t) J->out.bands * n);
 		bool monotone = true;
@@ -1275,7 +1329,488 @@ run_icc(const char *domain, const VB200Image *in, VB200Image *out, const JobSpec
 	return rc;
 }
 
+/* ------------------------------------------------------------------ the ICC stage of the thumbnail plan */
+
+/* What cmsOpenProfileFromMem (lcms2 2.18, cmsio0.c _cmsReadHeader) accepts: a 128-byte header with the 'acsp' magic, a
+ * version below 5.0 after _validatedVersion's clamp, a known device class (or 0), at most 100 tags whose directory can be read
+ * and no tag signature twice.  Tags whose offset + size fall outside the header's size (or the blob) are dropped from the
+ * directory, not refused.  *tags receives the signatures that stay.  No tag contents are read: lcms2 reads them lazily.
+ */
+bool
+lcms_would_open(const unsigned char *d, size_t n, std::vector<unsigned> *tags)
+{
+	tags->clear();
+	if (!d || n < 132)
+		return false;
+	const Blob b{d, n};
+	if (memcmp(d + 36, "acsp", 4) != 0)
+		return false;
+	unsigned char ver[4] = {d[8], d[9], 0, 0};
+	if (ver[0] > 0x09)
+		ver[0] = 0x09;
+	unsigned char hi = ver[1] & 0xf0, lo = ver[1] & 0x0f;
+	ver[1] = (unsigned char) ((hi > 0x90 ? 0x90 : hi) | (lo > 0x09 ? 0x09 : lo));
+	const unsigned version = ((unsigned) ver[0] << 24) | ((unsigned) ver[1] << 16);
+	if (version > 0x5000000u)
+		return false;
+	/* validDeviceClass: the ICC classes, or 0 (what older lcms versions wrote) */
+	static const char *classes[] = {"scnr", "mntr", "prtr", "link", "abst", "spac", "nmcl", "cenc", "mid ", "mlnk", "mvis", "\0\0\0\0"};
+	bool known = false;
+	for (const char *c : classes)
+		known = known || memcmp(d + 12, c, 4) == 0;
+	if (!known)
+		return false;
+	size_t header_size = b.u32(0);
+	if (header_size >= n)
+		header_size = n;
+	const unsigned count = b.u32(128);
+	if (count > 100 || !b.ok(132, 12 * (size_t) count))
+		return false;
+	for (unsigned i = 0; i < count; i++) {
+		const size_t e = 132 + 12 * (size_t) i;
+		const unsigned sig = b.u32(e), off = b.u32(e + 4), size = b.u32(e + 8);
+		if (size == 0 || off == 0)
+			continue;
+		if ((uint64_t) off + size > header_size || off + size < off) /* lcms2 adds in 32 bits */
+			continue;
+		for (unsigned t : *tags)
+			if (t == sig)
+				return false; /* "Duplicate tag found" */
+		tags->push_back(sig);
+	}
+	return true;
+}
+
+/* vips_icc_info (icc_transform.c:233-260): the profile colour spaces the reference handles, with their band counts */
+int
+icc_space_bands(const unsigned char *d)
+{
+	static const struct {
+		const char *sig;
+		int bands;
+	} table[] = {{"GRAY", 1}, {"RGB ", 3}, {"Lab ", 3}, {"XYZ ", 3}, {"CMYK", 4}, {"4CLR", 4}, {"5CLR", 5}, {"6CLR", 6}, {"7CLR", 7},
+		{"8CLR", 8}, {"9CLR", 9}, {"ACLR", 10}, {"BCLR", 11}, {"CCLR", 12}};
+	for (const auto &e : table)
+		if (memcmp(d + 16, e.sig, 4) == 0)
+			return e.bands;
+	return 0;
+}
+
+bool
+has_tag(const std::vector<unsigned> &tags, const char *sig)
+{
+	const unsigned s = ((unsigned) (unsigned char) sig[0] << 24) | ((unsigned char) sig[1] << 16) | ((unsigned char) sig[2] << 8) |
+		(unsigned char) sig[3];
+	for (unsigned t : tags)
+		if (t == s)
+			return true;
+	return false;
+}
+
+/* cmsIsIntentSupported (cmsio1.c): a lut tag for the intent in that direction, or a matrix / shaper profile */
+bool
+intent_supported(const unsigned char *d, const std::vector<unsigned> &tags, int intent, bool input)
+{
+	static const char *a2b[4] = {"A2B0", "A2B1", "A2B2", "A2B1"}, *b2a[4] = {"B2A0", "B2A1", "B2A2", "B2A1"};
+	if (memcmp(d + 12, "link", 4) == 0) {
+		if ((int) Blob{d, 128}.u32(64) == intent) /* cmsIsCLUT: a device link supports its header's intent */
+			return true;
+	}
+	else if (intent >= 0 && intent <= 3 && has_tag(tags, (input ? a2b : b2a)[intent]))
+		return true;
+	if (memcmp(d + 16, "GRAY", 4) == 0)
+		return has_tag(tags, "kTRC");
+	if (memcmp(d + 16, "RGB ", 4) == 0)
+		return has_tag(tags, "rXYZ") && has_tag(tags, "gXYZ") && has_tag(tags, "bXYZ") && has_tag(tags, "rTRC") && has_tag(tags, "gTRC") &&
+			has_tag(tags, "bTRC");
+	return false;
+}
+
+enum { PROFILE_USABLE = 0, PROFILE_UNUSABLE = 1, PROFILE_OTHER_INTENT = 2 };
+
+/* vips_icc_load_profile_blob (icc_transform.c:581-652) for an input profile of an image whose interpretation wants
+ * `want_bands`: PROFILE_UNUSABLE where the reference drops the profile and tries the next one; PROFILE_OTHER_INTENT where
+ * it would keep the profile with the header's intent in place of the one asked for
+ */
+int
+classify_input_profile(const void *p, size_t len, int want_bands, int intent)
+{
+	const unsigned char *d = (const unsigned char *) p;
+	std::vector<unsigned> tags;
+	if (!lcms_would_open(d, len, &tags))
+		return PROFILE_UNUSABLE;
+	int selected = intent;
+	if (!intent_supported(d, tags, intent, true)) {
+		const unsigned header_intent = Blob{d, len}.u32(64);
+		if (header_intent > 3)
+			return PROFILE_UNUSABLE;
+		selected = (int) header_intent;
+	}
+	const int bands = icc_space_bands(d);
+	if (bands == 0 || bands != want_bands)
+		return PROFILE_UNUSABLE;
+	if (!intent_supported(d, tags, selected, true))
+		return PROFILE_UNUSABLE;
+	return selected == intent ? PROFILE_USABLE : PROFILE_OTHER_INTENT;
+}
+
+struct IccProfileRef {
+	const void *data;
+	size_t len;
+};
+
+/* vips_icc_set_import (icc_transform.c:692-752) for one frame of a thumbnail: the embedded profile, then input_profile,
+ * then the built-in profile for the frame's interpretation.  Returns MODE_TRANSFORM with *use = the profile, MODE_XYZ_EXPORT
+ * when the frame has neither an embedded profile nor input_profile (thumbnail.c:957-970), or -1.  *source: 0 embedded,
+ * 1 input_profile, 2 built-in.
+ */
+int
+select_input_profile(const char *domain, int frame, const VB200ThumbnailIcc &icc, int bands, const void *embedded, size_t embedded_len,
+	IccProfileRef *use, int *source)
+{
+	const bool has_embedded = embedded && embedded_len > 0;
+	if (!has_embedded && !icc.input_profile)
+		return MODE_XYZ_EXPORT;
+	const bool grey = bands < 3;
+	const IccProfileRef candidates[3] = {{has_embedded ? embedded : nullptr, embedded_len}, {icc.input_profile, icc.input_len},
+		{grey ? icc.builtin_grey : icc.builtin_rgb, grey ? icc.builtin_grey_len : icc.builtin_rgb_len}};
+	for (int k = 0; k < 3; k++) {
+		if (!candidates[k].data) {
+			if (k == 2) {
+				error(domain, "frame %d: no usable embedded or input profile, and no built-in %s profile was passed", frame,
+					grey ? "grey" : "RGB");
+				return -1;
+			}
+			continue;
+		}
+		const int c = classify_input_profile(candidates[k].data, candidates[k].len, grey ? 1 : 3, icc.intent);
+		if (c == PROFILE_UNUSABLE)
+			continue;
+		if (c == PROFILE_OTHER_INTENT) {
+			error(domain, "frame %d: the input profile does not support rendering intent %d: its header intent is not supported on the "
+				"device path", frame, icc.intent);
+			return -1;
+		}
+		*use = candidates[k];
+		*source = k;
+		return MODE_TRANSFORM;
+	}
+	error(domain, "frame %d: unable to load or find any compatible input profile", frame);
+	return -1;
+}
+
+/* One launch per chunk of frames, whatever profiles they carry: frame f runs jobs[job_of[f]].  A CTA serves one frame,
+ * copies that frame's job into shared memory once and walks the frame's pixels.
+ */
+__global__ void __launch_bounds__(256)
+icc_frames_kernel(const IccJob *__restrict__ jobs, const int *__restrict__ job_of, const uint8_t *__restrict__ in, size_t in_stride,
+	int in_ps, uint8_t *__restrict__ out, size_t out_stride, int out_ps, size_t pixels)
+{
+	__shared__ __align__(16) unsigned char smem[sizeof(IccJob)];
+	const int f = blockIdx.y;
+	const unsigned *src = (const unsigned *) (jobs + job_of[f]);
+	for (int i = threadIdx.x; i < (int) (sizeof(IccJob) / 4); i += blockDim.x)
+		((unsigned *) smem)[i] = src[i];
+	__syncthreads();
+	const IccJob &J = *(const IccJob *) smem;
+	const uint8_t *fin = in + (size_t) f * in_stride;
+	uint8_t *fout = out + (size_t) f * out_stride;
+	for (size_t p = (size_t) blockIdx.x * blockDim.x + threadIdx.x; p < pixels; p += (size_t) gridDim.x * blockDim.x)
+		icc_pixel(J, fin + p * in_ps, fout + p * out_ps);
+}
+static_assert(sizeof(IccJob) % 4 == 0, "IccJob is copied to shared memory in words");
+
+uint64_t
+fnv1a64(const void *p, size_t n)
+{
+	const unsigned char *d = (const unsigned char *) p;
+	uint64_t h = 1469598103934665603ull;
+	for (size_t i = 0; i < n; i++)
+		h = (h ^ d[i]) * 1099511628211ull;
+	return h;
+}
+
 } // namespace
+
+/* A parsed and tabulated job on the device, keyed by the input profile's bytes (none: branch X) */
+struct IccCacheEntry {
+	int mode = 0;
+	uint64_t hash = 0;
+	std::vector<unsigned char> bytes;
+	IccJob job;
+	float *dpool = nullptr;
+	/* one event per stream that launched a kernel reading dpool, recorded after its latest such launch: the host pump runs
+	 * its slices on several streams, and an eviction waits for all of them
+	 */
+	std::vector<std::pair<cudaStream_t, cudaEvent_t>> used;
+	uint64_t tick = 0;
+};
+
+struct IccStage {
+	static constexpr size_t kCacheEntries = 16;
+	std::mutex lock;
+	std::vector<unsigned char> input, output, builtin_rgb, builtin_grey;
+	VB200ThumbnailIcc icc{}; /* pointers into the copies above */
+	int bands = 0, out_bands = 0;
+	std::vector<IccCacheEntry *> cache;
+	uint64_t tick = 0;
+};
+
+namespace {
+
+void
+entry_free(IccCacheEntry *e)
+{
+	for (auto &u : e->used)
+		cudaEventSynchronize(u.second);
+	if (e->dpool)
+		cudaFree(e->dpool);
+	for (auto &u : e->used)
+		cudaEventDestroy(u.second);
+	delete e;
+}
+
+int
+stage_job_spec(const IccStage &st, int mode, const IccProfileRef &in, JobSpec *sp)
+{
+	*sp = JobSpec{mode, st.icc.intent, mode == MODE_XYZ_EXPORT, 8, mode == MODE_XYZ_EXPORT ? st.icc.output_profile : in.data,
+		mode == MODE_XYZ_EXPORT ? st.icc.output_len : in.len, st.icc.output_profile, st.icc.output_len};
+	return 0;
+}
+
+/* the cached job for (mode, profile), built and uploaded on a miss; entries used by the current batch are never evicted */
+IccCacheEntry *
+stage_entry(const char *domain, IccStage &st, int frame, int mode, const IccProfileRef &in, const std::vector<IccCacheEntry *> &pinned)
+{
+	const uint64_t h = mode == MODE_TRANSFORM ? fnv1a64(in.data, in.len) : 0;
+	for (IccCacheEntry *e : st.cache)
+		if (e->mode == mode && (mode != MODE_TRANSFORM || (e->hash == h && e->bytes.size() == in.len && memcmp(e->bytes.data(), in.data, in.len) == 0))) {
+			e->tick = ++st.tick;
+			return e;
+		}
+	auto *e = new IccCacheEntry();
+	e->mode = mode;
+	e->hash = h;
+	if (mode == MODE_TRANSFORM)
+		e->bytes.assign((const unsigned char *) in.data, (const unsigned char *) in.data + in.len);
+	JobSpec sp;
+	stage_job_spec(st, mode, in, &sp);
+	std::vector<float> pool;
+	int ob, of, ot;
+	const int in_type = st.bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB;
+	if (build_job(domain, sp, VB200_FORMAT_UCHAR, st.bands, in_type, &e->job, pool, &ob, &of, &ot)) {
+		error(domain, "frame %d: its colour transform is not supported on the device path", frame);
+		delete e;
+		return nullptr;
+	}
+	if (ob != st.out_bands) {
+		error(domain, "frame %d: the transform gives %d bands, the plan expects %d", frame, ob, st.out_bands);
+		delete e;
+		return nullptr;
+	}
+	if (cudaMalloc(&e->dpool, std::max<size_t>(1, pool.size()) * sizeof(float)) != cudaSuccess ||
+		cudaMemcpy(e->dpool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+		cuda_fail(domain, cudaGetLastError(), "ICC job upload");
+		entry_free(e);
+		return nullptr;
+	}
+	e->job.in.pool = e->job.out.pool = e->dpool;
+	e->tick = ++st.tick;
+	/* a small LRU: evict the least recently used entry the batch in flight does not hold */
+	if (st.cache.size() >= IccStage::kCacheEntries) {
+		int victim = -1;
+		for (int i = 0; i < (int) st.cache.size(); i++) {
+			bool held = false;
+			for (IccCacheEntry *p : pinned)
+				held = held || p == st.cache[i];
+			if (!held && (victim < 0 || st.cache[i]->tick < st.cache[victim]->tick))
+				victim = i;
+		}
+		if (victim >= 0) {
+			entry_free(st.cache[victim]);
+			st.cache.erase(st.cache.begin() + victim);
+		}
+	}
+	st.cache.push_back(e);
+	return e;
+}
+
+} // namespace
+
+struct IccTiming {
+	cudaEvent_t start = nullptr, stop = nullptr;
+	bool pending = false;
+};
+thread_local IccTiming g_icc_timing;
+
+float
+icc_stage_last_ms()
+{
+	float ms = -1.0f;
+	if (g_icc_timing.pending && cudaEventSynchronize(g_icc_timing.stop) == cudaSuccess &&
+		cudaEventElapsedTime(&ms, g_icc_timing.start, g_icc_timing.stop) != cudaSuccess)
+		ms = -1.0f;
+	return ms;
+}
+
+IccStage *
+icc_stage_new()
+{
+	return new IccStage();
+}
+
+void
+icc_stage_free(IccStage *st)
+{
+	if (!st)
+		return;
+	for (IccCacheEntry *e : st->cache)
+		entry_free(e);
+	delete st;
+}
+
+int
+icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands)
+{
+	std::lock_guard<std::mutex> lock(st->lock);
+	for (IccCacheEntry *e : st->cache)
+		entry_free(e);
+	st->cache.clear();
+	auto copy = [](std::vector<unsigned char> &v, const void *p, size_t n) -> const void * {
+		v.assign((const unsigned char *) p, (const unsigned char *) p + (p ? n : 0));
+		return p ? v.data() : nullptr;
+	};
+	st->icc = *icc;
+	st->icc.input_profile = copy(st->input, icc->input_profile, icc->input_len);
+	st->icc.output_profile = copy(st->output, icc->output_profile, icc->output_len);
+	st->icc.builtin_rgb = copy(st->builtin_rgb, icc->builtin_rgb, icc->builtin_rgb_len);
+	st->icc.builtin_grey = copy(st->builtin_grey, icc->builtin_grey, icc->builtin_grey_len);
+	st->bands = bands;
+	/* vips_icc_transform / vips_icc_export fail outright when the output profile does not load (icc_transform.c:1032-1037) */
+	std::vector<unsigned> tags;
+	if (!lcms_would_open((const unsigned char *) st->icc.output_profile, st->icc.output_len, &tags)) {
+		error(domain, "no output profile: corrupt profile");
+		return -1;
+	}
+	const int ob = icc_space_bands((const unsigned char *) st->icc.output_profile);
+	if (ob != 1 && ob != 3 && ob != 4) {
+		error(domain, "output profile colour space %.4s not supported on the device path", (const char *) st->icc.output_profile + 16);
+		return -1;
+	}
+	if (!intent_supported((const unsigned char *) st->icc.output_profile, tags, icc->intent, false)) {
+		error(domain, "the output profile does not support rendering intent %d: its header intent is not supported on the device path",
+			icc->intent);
+		return -1;
+	}
+	st->out_bands = ob + bands - (bands < 3 ? 1 : 3);
+	/* parse the output side once now, so that a profile the evaluator declines fails here rather than per batch */
+	JobSpec sp;
+	stage_job_spec(*st, MODE_XYZ_EXPORT, IccProfileRef{nullptr, 0}, &sp);
+	IccJob J;
+	std::vector<float> pool;
+	int b, f, t;
+	if (build_job(domain, sp, VB200_FORMAT_UCHAR, bands, bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, &J, pool, &b, &f, &t))
+		return -1;
+	*out_bands = st->out_bands;
+	return 0;
+}
+
+int
+icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
+	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s)
+{
+	if (n <= 0)
+		return 0;
+	std::lock_guard<std::mutex> lock(st->lock);
+	std::vector<IccCacheEntry *> used; /* distinct entries of this batch, in first-use order */
+	std::vector<int> job_of(n);
+	for (int f = 0; f < n; f++) {
+		IccProfileRef ref{nullptr, 0};
+		int source = 0;
+		const int mode = select_input_profile(domain, f, st->icc, st->bands, embedded ? embedded[f] : nullptr,
+			embedded && embedded_lens ? embedded_lens[f] : 0, &ref, &source);
+		if (mode < 0)
+			return -1;
+		IccCacheEntry *e = stage_entry(domain, *st, f, mode, ref, used);
+		if (!e)
+			return -1;
+		int k = 0;
+		while (k < (int) used.size() && used[k] != e)
+			k++;
+		if (k == (int) used.size())
+			used.push_back(e);
+		job_of[f] = k;
+	}
+	std::vector<IccJob> jobs(used.size());
+	for (size_t k = 0; k < used.size(); k++)
+		jobs[k] = used[k]->job;
+	const size_t jobs_bytes = jobs.size() * sizeof(IccJob);
+	void *table = nullptr;
+	if (dev_alloc(domain, &table, jobs_bytes + (size_t) n * sizeof(int), s))
+		return -1;
+	int rc = 0;
+	if (cudaMemcpyAsync(table, jobs.data(), jobs_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+		cudaMemcpyAsync((char *) table + jobs_bytes, job_of.data(), (size_t) n * sizeof(int), cudaMemcpyHostToDevice, s) != cudaSuccess)
+		rc = cuda_fail(domain, cudaGetLastError(), "ICC job table upload");
+	const int in_ps = st->bands, out_ps = st->out_bands;
+	/* a few CTAs per frame, each walking its share of the pixels; frames on gridDim.y, at most kMaxBatchFrames a launch */
+	const unsigned per_frame = (unsigned) std::min<size_t>((pixels + 255) / 256, 64);
+	/* VB200_ICC_TIMING: CUDA events around this call's launches, read back by vb200_debug_icc_stage_ms */
+	const bool timing = getenv("VB200_ICC_TIMING") != nullptr;
+	if (timing) {
+		for (cudaEvent_t *ev : {&g_icc_timing.start, &g_icc_timing.stop})
+			if (!*ev && cudaEventCreate(ev) != cudaSuccess)
+				rc = cuda_fail(domain, cudaGetLastError(), "ICC timing event");
+		if (!rc)
+			cudaEventRecord(g_icc_timing.start, s);
+		g_icc_timing.pending = !rc;
+	}
+	for (int f0 = 0; f0 < n && !rc; f0 += kMaxBatchFrames) {
+		const int nf = std::min(n - f0, (int) kMaxBatchFrames);
+		icc_frames_kernel<<<dim3(per_frame, nf), 256, 0, s>>>((const IccJob *) table, (const int *) ((char *) table + jobs_bytes) + f0,
+			(const uint8_t *) in + (size_t) f0 * in_stride, in_stride, in_ps, (uint8_t *) out + (size_t) f0 * out_stride, out_stride,
+			out_ps, pixels);
+		const cudaError_t e = cudaGetLastError();
+		if (e != cudaSuccess)
+			rc = cuda_fail(domain, e, "icc_frames_kernel");
+		else
+			count_launch();
+	}
+	if (timing && g_icc_timing.pending)
+		cudaEventRecord(g_icc_timing.stop, s);
+	for (IccCacheEntry *e : used) {
+		size_t k = 0;
+		while (k < e->used.size() && e->used[k].first != s)
+			k++;
+		if (k == e->used.size()) {
+			cudaEvent_t ev = nullptr;
+			if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+				rc = cuda_fail(domain, cudaGetLastError(), "ICC job event");
+				continue;
+			}
+			e->used.emplace_back(s, ev);
+		}
+		cudaEventRecord(e->used[k].second, s);
+	}
+	dev_free(table, s);
+	return rc;
+}
+
+/* test hook: the selection of one frame, as the stage makes it */
+int
+icc_debug_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source)
+{
+	IccProfileRef ref{nullptr, 0};
+	*source = -1;
+	const int mode = select_input_profile("icc_select", 0, *icc, bands, embedded, embedded_len, &ref, source);
+	return mode < 0 ? -1 : mode == MODE_XYZ_EXPORT ? 1 : 0;
+}
+
+int
+icc_debug_classify(const void *profile, size_t len, int want_bands, int intent)
+{
+	return classify_input_profile(profile, len, want_bands, intent);
+}
 
 } // namespace vb200
 
@@ -1321,4 +1856,30 @@ vb200_debug_icc_eval(int mode, const void *in, int in_fmt, int in_bands, void *o
 	for (int i = 0; i < n; i++)
 		icc_pixel(J, (const char *) in + (size_t) i * ips, (char *) out + (size_t) i * ops);
 	return ob;
+}
+
+/* Test hooks, host only: the input-profile selection of one thumbnail frame (0: transform, *source = 0 embedded / 1 input_profile /
+ * 2 built-in; 1: no input profile, the XYZ export; -1: error), and the open / compatibility / intent check behind it.
+ */
+extern "C" int
+vb200_debug_icc_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source)
+{
+	if (!icc || !source) {
+		error("icc_select", "null argument");
+		return -1;
+	}
+	return icc_debug_select(icc, bands, embedded, embedded_len, source);
+}
+
+extern "C" int
+vb200_debug_icc_classify(const void *profile, size_t len, int want_bands, int intent)
+{
+	return icc_debug_classify(profile, len, want_bands, intent);
+}
+
+/* with env VB200_ICC_TIMING set: CUDA-event time of the calling thread's last ICC stage (its icc_frames_kernel launches); -1 if none */
+extern "C" float
+vb200_debug_icc_stage_ms(void)
+{
+	return icc_stage_last_ms();
 }

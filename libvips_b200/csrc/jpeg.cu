@@ -2803,3 +2803,89 @@ vb200_debug_jpeg_decode_sync(const void *buf, size_t len, int shrink, int sub_by
 		(unsigned) std::max(0, sub_bytes), max_passes, passes_used);
 }
 
+
+namespace vb200 {
+
+/* read_jpeg_header, foreign/jpeg2vips.c:699-799, over the markers jpeg_read_header sees (those before the first SOS):
+ * an APP2 segment of more than 14 bytes that starts "ICC_PROFILE" stores its bytes from 14 on in slot data[12] - 1 (slots
+ * 0 .. 99, a later duplicate wins; data[13], the chunk count, is not read); the profile is slots 0, 1, 2 ... concatenated
+ * up to the first empty one.  Marker walking as parse_jpeg (libjpeg's next_marker: garbage, then fill bytes, skipped).
+ */
+int
+jpeg_icc_profile(const char *domain, const unsigned char *d, size_t len, std::vector<unsigned char> *profile)
+{
+	profile->clear();
+	if (!d || len < 4 || d[0] != 0xFF || d[1] != 0xD8) {
+		error(domain, "not a JPEG stream");
+		return -1;
+	}
+	const unsigned char *slot[100] = {nullptr};
+	size_t slot_len[100] = {0};
+	size_t p = 2;
+	for (;;) {
+		while (p < len && d[p] != 0xFF)
+			p++;
+		while (p < len && d[p] == 0xFF)
+			p++;
+		if (p >= len) {
+			error(domain, "JPEG stream ends before the scan");
+			return -1;
+		}
+		const int m = d[p++];
+		if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01)
+			continue;
+		if (m == 0xD9) {
+			error(domain, "JPEG stream has no scan");
+			return -1;
+		}
+		if (p + 2 > len) {
+			error(domain, "truncated JPEG marker segment");
+			return -1;
+		}
+		const size_t L = be16(d + p);
+		if (L < 2 || p + L > len) {
+			error(domain, "truncated JPEG marker segment");
+			return -1;
+		}
+		if (m == 0xDA)
+			break;
+		const unsigned char *s = d + p + 2;
+		const size_t n = L - 2;
+		if (m == 0xE2 && n > 14 && memcmp(s, "ICC_PROFILE", 11) == 0) {
+			const int k = s[12] - 1;
+			if (k >= 0 && k < 100) {
+				slot[k] = s + 14;
+				slot_len[k] = n - 14;
+			}
+		}
+		p += L;
+	}
+	for (int k = 0; k < 100 && slot[k]; k++)
+		profile->insert(profile->end(), slot[k], slot[k] + slot_len[k]);
+	return 0;
+}
+
+} // namespace vb200
+
+extern "C" int
+vb200_jpeg_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len)
+{
+	const char *domain = "jpeg_icc_profile";
+	if (!profile_len) {
+		error(domain, "null argument");
+		return -1;
+	}
+	std::vector<unsigned char> prof;
+	if (jpeg_icc_profile(domain, (const unsigned char *) buf, len, &prof))
+		return -1;
+	*profile_len = prof.size();
+	if (!out)
+		return 0;
+	if (cap < prof.size()) {
+		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
+		return -1;
+	}
+	if (!prof.empty())
+		memcpy(out, prof.data(), prof.size());
+	return 0;
+}

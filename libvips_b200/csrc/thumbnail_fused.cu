@@ -1455,6 +1455,11 @@ struct ThumbnailPlanImpl {
 	/* vips_sharpen appended to every batch (vb200_thumbnail_plan_set_sharpen) */
 	bool sharpen = false;
 	double sh_sigma = 0.5, sh_x1 = 2.0, sh_y2 = 10.0, sh_y3 = 20.0, sh_m1 = 0.0, sh_m2 = 3.0;
+	/* colour management between the thumbnail and the sharpen stage (vb200_thumbnail_plan_set_icc); null = off */
+	IccStage *icc = nullptr;
+	int icc_bands = 0;			 /* output bands with the stage on */
+	size_t stage_out_frame = 0; /* the host pump's output slots are sized for frames of this many bytes */
+	int out_bands() const { return icc ? icc_bands : bands; }
 };
 
 /* sharpen_fused.cu */
@@ -2307,29 +2312,51 @@ thumbnail_common_shrink(int w, int h, int tw, int th, int size)
 	return std::min(hs, vs);
 }
 
+/* The plan's stages over a device batch: thumbnail kernel -> ICC stage (if set) -> sharpen stage (if set).  Every stage but
+ * the last writes a scratch batch from the stream-ordered pool; the last writes `out`.  embedded / embedded_lens: each
+ * frame's embedded ICC profile for the ICC stage (NULL: none).
+ */
 int
 thumbnail_plan_run_device(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s)
+	size_t out_stride, int n, cudaStream_t s, const void *const *embedded = nullptr, const size_t *embedded_lens = nullptr)
 {
 	if (n <= 0)
 		return 0;
-	if (!pl->sharpen)
+	if (!pl->sharpen && !pl->icc)
 		return thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, out, out_stride, n, s);
-	/* thumbnail -> scratch batch (stream-ordered pool) -> sharpen -> out */
 	const size_t frame = (size_t) pl->OW * pl->OH * pl->bands;
-	void *mid = nullptr;
+	const int sb = pl->out_bands(); /* bands the sharpen stage sees */
+	const size_t sframe = (size_t) pl->OW * pl->OH * sb;
+	void *mid = nullptr, *mid2 = nullptr;
 	if (dev_alloc(domain, &mid, frame * n, s))
 		return -1;
+	if (pl->icc && pl->sharpen && dev_alloc(domain, &mid2, sframe * n, s)) {
+		dev_free(mid, s);
+		return -1;
+	}
 	int rc = thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, mid, frame, n, s);
-	if (!rc) {
-		rc = dev_sharpen_fused(domain, mid, (size_t) pl->OW * pl->bands, frame, out, (size_t) pl->OW * pl->bands, out_stride, n,
-			pl->OW, pl->OH, pl->bands, pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
+	const void *sin = mid;
+	if (!rc && pl->icc) {
+		rc = icc_stage_run(domain, pl->icc, mid, frame, pl->sharpen ? mid2 : out, pl->sharpen ? sframe : out_stride, n,
+			(size_t) pl->OW * pl->OH, embedded, embedded_lens, s);
+		sin = mid2;
+	}
+	if (!rc && pl->sharpen) {
+		if (sb != 3 && sb != 4) {
+			error(domain, "the sharpen stage needs 3- or 4-band frames, the output profile gives %d bands", sb);
+			rc = -1;
+		}
+		else
+			rc = dev_sharpen_fused(domain, sin, (size_t) pl->OW * sb, sframe, out, (size_t) pl->OW * sb, out_stride, n, pl->OW, pl->OH, sb,
+				pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
 		if (rc == 1) {
 			error(domain, "sharpen parameters are not on the fused path (mask too wide)");
 			rc = -1;
 		}
 	}
 	dev_free(mid, s);
+	if (mid2)
+		dev_free(mid2, s);
 	return rc;
 }
 
@@ -2509,6 +2536,8 @@ thumbnail_plan_destroy(ThumbnailPlanImpl *pl)
 	if (pl->lin)
 		linear_thumb_free(pl->lin);
 	pl->lin = nullptr;
+	icc_stage_free(pl->icc);
+	pl->icc = nullptr;
 	for (int i = 0; i < ThumbnailPlanImpl::kHintSlots; i++)
 		if (pl->hint_done[i]) {
 			cudaEventSynchronize(pl->hint_done[i]);
@@ -2661,6 +2690,13 @@ extern "C" int
 vb200_thumbnail_batch_device(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
 	size_t out_frame_stride, int n_frames)
 {
+	return vb200_thumbnail_batch_device_icc(plan, in, in_frame_stride, out, out_frame_stride, n_frames, nullptr, nullptr);
+}
+
+extern "C" int
+vb200_thumbnail_batch_device_icc(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
+	size_t out_frame_stride, int n_frames, const void *const *embedded, const size_t *embedded_lens)
+{
 	const char *domain = "thumbnail_batch_device";
 	if (!plan || !in || !out) {
 		error(domain, "null argument");
@@ -2669,7 +2705,48 @@ vb200_thumbnail_batch_device(VB200ThumbnailPlan *plan, const void *in, size_t in
 	if (ensure_init(domain))
 		return -1;
 	return thumbnail_plan_run_device(domain, &plan->impl, in, in_frame_stride, out, out_frame_stride, n_frames,
-		current_stream());
+		current_stream(), embedded, embedded_lens);
+}
+
+extern "C" int
+vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc)
+{
+	const char *domain = "thumbnail_plan_set_icc";
+	if (!plan) {
+		error(domain, "null plan");
+		return -1;
+	}
+	ThumbnailPlanImpl &pl = plan->impl;
+	if (!icc || !icc->output_profile) {
+		icc_stage_free(pl.icc);
+		pl.icc = nullptr;
+		return 0;
+	}
+	if (pl.linear) {
+		/* thumbnail.c:766-806, 957-970: an ICC import into the linear V kernel and an export from the H kernel, not built */
+		error(domain, "linear thumbnails with an output profile are not supported on the device path");
+		return -1;
+	}
+	if (pl.fmt != VB200_FORMAT_UCHAR) {
+		error(domain, "colour-managed thumbnails need 8-bit frames");
+		return -1;
+	}
+	IccStage *st = icc_stage_new();
+	int ob = 0;
+	if (icc_stage_set(domain, st, icc, pl.bands, &ob)) {
+		icc_stage_free(st);
+		return -1;
+	}
+	icc_stage_free(pl.icc);
+	pl.icc = st;
+	pl.icc_bands = ob;
+	return 0;
+}
+
+extern "C" int
+vb200_thumbnail_plan_output_bands(const VB200ThumbnailPlan *plan)
+{
+	return plan ? plan->impl.out_bands() : -1;
 }
 
 /* reference: vips_thumbnail_buffer(buf, len, &out, width, "height", height, "size", size, NULL), resample/thumbnail.c:
@@ -2679,12 +2756,21 @@ vb200_thumbnail_batch_device(VB200ThumbnailPlan *plan, const void *in, size_t in
 extern "C" int
 vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size)
 {
+	return vb200_thumbnail_buffer_icc(buf, len, out, width, height, size, nullptr);
+}
+
+extern "C" int
+vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc)
+{
 	const char *domain = "thumbnail_buffer";
 	if (!buf || !out) {
 		error(domain, "null argument");
 		return -1;
 	}
 	if (ensure_init(domain))
+		return -1;
+	std::vector<unsigned char> embedded;
+	if (icc && icc->output_profile && jpeg_icc_profile(domain, (const unsigned char *) buf, len, &embedded))
 		return -1;
 	cudaStream_t s = current_stream();
 	int w0, h0, b0;
@@ -2713,7 +2799,7 @@ vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, 
 		VB200Image tmp;
 		memset(&tmp, 0, sizeof(tmp));
 		tmp.where = VB200_DEVICE;
-		rc = vb200_thumbnail_image(&din, &tmp, width, height, size, 0);
+		rc = vb200_thumbnail_image_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size());
 		if (!rc) {
 			/* deliver where the caller asked (allocate-or-fill) */
 			DevImage dt;
@@ -2751,9 +2837,23 @@ vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs,
 		return -1;
 	ThumbnailPlanImpl &pl = plan->impl;
 	cudaStream_t s = current_stream();
-	const size_t in_frame = (size_t) pl.W * pl.H * pl.bands, out_frame = (size_t) pl.OW * pl.OH * pl.bands;
+	const size_t in_frame = (size_t) pl.W * pl.H * pl.bands, out_frame = (size_t) pl.OW * pl.OH * pl.out_bands();
 	if (out_frame_stride == 0)
 		out_frame_stride = out_frame;
+	/* with colour management on, each stream's embedded profile (jpeg2vips.c:699-799) goes to the ICC stage */
+	std::vector<std::vector<unsigned char>> profiles(pl.icc ? n : 0);
+	std::vector<const void *> emb(profiles.size());
+	std::vector<size_t> emb_len(profiles.size());
+	for (size_t i = 0; i < profiles.size(); i++) {
+		if (jpeg_icc_profile(domain, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
+			error(domain, "stream %d", (int) i);
+			return -1;
+		}
+		emb[i] = profiles[i].empty() ? nullptr : profiles[i].data();
+		emb_len[i] = profiles[i].size();
+	}
+	const void *const *embedded = pl.icc ? emb.data() : nullptr;
+	const size_t *embedded_lens = pl.icc ? emb_len.data() : nullptr;
 	void *dec = nullptr, *res = nullptr;
 	if (dev_alloc(domain, &dec, in_frame * n, s))
 		return -1;
@@ -2767,12 +2867,12 @@ vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs,
 			break;
 		}
 		if (out_location == VB200_DEVICE) {
-			rc = thumbnail_plan_run_device(domain, &pl, dec, in_frame, out, out_frame_stride, n, s);
+			rc = thumbnail_plan_run_device(domain, &pl, dec, in_frame, out, out_frame_stride, n, s, embedded, embedded_lens);
 			break;
 		}
 		if (dev_alloc(domain, &res, out_frame * n, s))
 			break;
-		if (thumbnail_plan_run_device(domain, &pl, dec, in_frame, res, out_frame, n, s))
+		if (thumbnail_plan_run_device(domain, &pl, dec, in_frame, res, out_frame, n, s, embedded, embedded_lens))
 			break;
 		if (cudaMemcpy2DAsync(out, out_frame_stride, res, out_frame, out_frame, n, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
 			cudaStreamSynchronize(s) != cudaSuccess) {
@@ -2797,6 +2897,13 @@ extern "C" int
 vb200_thumbnail_batch_host(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
 	size_t out_frame_stride, int n_frames)
 {
+	return vb200_thumbnail_batch_host_icc(plan, in, in_frame_stride, out, out_frame_stride, n_frames, nullptr, nullptr);
+}
+
+extern "C" int
+vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t in_frame_stride, void *out,
+	size_t out_frame_stride, int n_frames, const void *const *embedded, const size_t *embedded_lens)
+{
 	const char *domain = "thumbnail_batch_host";
 	if (!plan || !in || !out) {
 		error(domain, "null argument");
@@ -2807,13 +2914,13 @@ vb200_thumbnail_batch_host(VB200ThumbnailPlan *plan, const void *in, size_t in_f
 	ThumbnailPlanImpl &pl = plan->impl;
 	std::lock_guard<std::mutex> lock(pl.pump_lock); /* one pump per plan at a time: the staging ring is the plan's */
 	const size_t in_frame = (size_t) pl.W * pl.H * pl.bands;
-	const size_t out_frame = (size_t) pl.OW * pl.OH * pl.bands;
+	const size_t out_frame = (size_t) pl.OW * pl.OH * pl.out_bands();
 	/* Slice size: ~64 MiB of input per slot (one 4K RGBA frame).  The pump is bound by the H2D copy
 	 * (one such frame is 1.2 ms of PCIe against 14 us of kernel), so small slices cost nothing and
 	 * shorten the pipeline fill; small frames are batched up to the same byte budget.
 	 */
 	const int per_slice = (int) std::max<size_t>(1, std::min<size_t>(n_frames, (64u << 20) / in_frame));
-	if (pl.stage_frames < per_slice) {
+	if (pl.stage_frames < per_slice || pl.stage_out_frame != out_frame) { /* the ICC stage may change the output bands */
 		for (int i = 0; i < ThumbnailPlanImpl::kStreams; i++) {
 			if (pl.streams[i])
 				cudaStreamSynchronize(pl.streams[i]);
@@ -2822,14 +2929,15 @@ vb200_thumbnail_batch_host(VB200ThumbnailPlan *plan, const void *in, size_t in_f
 			if (pl.stage_out[i])
 				cudaFree(pl.stage_out[i]);
 			pl.stage_in[i] = pl.stage_out[i] = nullptr;
-			VB200_CUDA(domain, cudaMalloc(&pl.stage_in[i], in_frame * per_slice));
-			VB200_CUDA(domain, cudaMalloc(&pl.stage_out[i], out_frame * per_slice));
+			VB200_CUDA(domain, cudaMalloc(&pl.stage_in[i], in_frame * std::max(per_slice, pl.stage_frames)));
+			VB200_CUDA(domain, cudaMalloc(&pl.stage_out[i], out_frame * std::max(per_slice, pl.stage_frames)));
 			if (!pl.streams[i])
 				VB200_CUDA(domain, cudaStreamCreateWithFlags(&pl.streams[i], cudaStreamNonBlocking));
 			if (!pl.drained[i])
 				VB200_CUDA(domain, cudaEventCreateWithFlags(&pl.drained[i], cudaEventDisableTiming | cudaEventBlockingSync));
 		}
-		pl.stage_frames = per_slice;
+		pl.stage_frames = std::max(per_slice, pl.stage_frames);
+		pl.stage_out_frame = out_frame;
 	}
 
 	bool used[ThumbnailPlanImpl::kStreams] = {false, false, false};
@@ -2844,7 +2952,8 @@ vb200_thumbnail_batch_host(VB200ThumbnailPlan *plan, const void *in, size_t in_f
 			VB200_CUDA(domain, cudaEventSynchronize(pl.drained[slot]));
 		VB200_CUDA(domain, cudaMemcpy2DAsync(pl.stage_in[slot], in_frame, (const char *) in + (size_t) f * in_frame_stride,
 							   in_frame_stride, in_frame, n, cudaMemcpyHostToDevice, s));
-		if (thumbnail_plan_run_device(domain, &pl, pl.stage_in[slot], in_frame, pl.stage_out[slot], out_frame, n, s))
+		if (thumbnail_plan_run_device(domain, &pl, pl.stage_in[slot], in_frame, pl.stage_out[slot], out_frame, n, s,
+				embedded ? embedded + f : nullptr, embedded_lens ? embedded_lens + f : nullptr))
 			return -1;
 		VB200_CUDA(domain, cudaMemcpy2DAsync((char *) out + (size_t) f * out_frame_stride, out_frame_stride,
 							   pl.stage_out[slot], out_frame, out_frame, n, cudaMemcpyDeviceToHost, s));
@@ -2857,13 +2966,23 @@ vb200_thumbnail_batch_host(VB200ThumbnailPlan *plan, const void *in, size_t in_f
 	return 0;
 }
 
-/* reference: vips_thumbnail_image(), resample/thumbnail.c:2000 */
-extern "C" int
-vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear)
+/* vips_thumbnail_image, with colour management when icc sets an output profile */
+static int
+thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear, const VB200ThumbnailIcc *icc,
+	const void *embedded, size_t embedded_len)
 {
 	const char *domain = "thumbnail";
 	if (!in || !out) {
 		error(domain, "null argument");
+		return -1;
+	}
+	if (icc && icc->output_profile &&
+		!((in->Type == VB200_INTERPRETATION_sRGB && in->Bands >= 3) || (in->Type == VB200_INTERPRETATION_B_W && in->Bands < 3))) {
+		/* with a profile pair the reference keeps the image's own interpretation (thumbnail.c:807-823) and imports with a
+		 * profile of that space (icc_transform.c:565-577, e.g. CMYK); the device stage takes 8-bit sRGB / B_W frames only
+		 */
+		error(domain, "colour-managed thumbnails of interpretation %d with %d bands are not supported on the device path", in->Type,
+			in->Bands);
 		return -1;
 	}
 	if (ensure_init(domain))
@@ -2878,6 +2997,17 @@ vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int heig
 		height, size, linear);
 	if (!plan)
 		return -1;
+	if (icc && vb200_thumbnail_plan_set_icc(plan, icc)) {
+		vb200_thumbnail_plan_free(plan);
+		return -1;
+	}
+	const int ob = plan->impl.out_bands();
+	/* icc_transform.c:374-433: the output interpretation follows the output profile's colour bands */
+	const int colour = ob - (in->Bands - (in->Bands < 3 ? 1 : 3));
+	const int otype = !plan->impl.icc ? in->Type
+		: colour == 1				  ? VB200_INTERPRETATION_B_W
+		: colour == 3				  ? VB200_INTERPRETATION_sRGB
+									  : VB200_INTERPRETATION_CMYK;
 	cudaStream_t s = current_stream();
 	DevImage din, dout;
 	int rc = to_device(domain, in, &din, s);
@@ -2886,9 +3016,12 @@ vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int heig
 		rc = -1;
 	}
 	if (!rc)
-		rc = dev_image_new(domain, &dout, plan->impl.OW, plan->impl.OH, in->Bands, in->BandFmt, in->Type, s);
-	if (!rc)
-		rc = thumbnail_plan_run_device(domain, &plan->impl, din.data, 0, dout.data, 0, 1, s);
+		rc = dev_image_new(domain, &dout, plan->impl.OW, plan->impl.OH, ob, in->BandFmt, otype, s);
+	if (!rc) {
+		const void *emb[1] = {embedded};
+		const size_t emb_len[1] = {embedded ? embedded_len : 0};
+		rc = thumbnail_plan_run_device(domain, &plan->impl, din.data, 0, dout.data, 0, 1, s, emb, emb_len);
+	}
 	if (!rc)
 		rc = deliver(domain, &dout, in, out, s);
 	if (!rc && in->where == VB200_DEVICE)
@@ -2896,4 +3029,19 @@ vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int heig
 	dev_image_release(&din, s);
 	vb200_thumbnail_plan_free(plan);
 	return rc;
+}
+
+/* reference: vips_thumbnail_image(), resample/thumbnail.c:2000 */
+extern "C" int
+vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear)
+{
+	return thumbnail_image_run(in, out, width, height, size, linear, nullptr, nullptr, 0);
+}
+
+/* vips_thumbnail_image with "input_profile" / "output_profile" / "intent"; `embedded`: the image's ICC blob */
+extern "C" int
+vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	const void *embedded, size_t embedded_len)
+{
+	return thumbnail_image_run(in, out, width, height, size, 0, icc, embedded, embedded_len);
 }

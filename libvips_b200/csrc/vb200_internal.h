@@ -197,6 +197,21 @@ int host_jpeg_decode(const char *domain, const void *buf, size_t len, int shrink
 double thumbnail_common_shrink(int w, int h, int tw, int th, int size);
 void jpeg_pump_release(); /* the JPEG pump's pinned / device slots (jpeg.cu); vb200_shutdown */
 void resample_cache_clear(); /* cached axis tables (resample_kernels.cu); vb200_shutdown */
+/* jpeg.cu: the ICC profile a JPEG stream embeds, as jpeg2vips.c:699-799 reassembles it (*len = 0: none) */
+int jpeg_icc_profile(const char *domain, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
+
+/* icc.cu: the colour-management stage of the thumbnail plan (vb200_thumbnail_plan_set_icc).  Frames are 8-bit, `bands`
+ * bands in, *out_bands out; each frame's input profile is chosen as vips_icc_set_import does, and one launch runs a batch.
+ */
+struct IccStage;
+IccStage *icc_stage_new();
+void icc_stage_free(IccStage *st);
+int icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands);
+int icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
+	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s);
+int icc_debug_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source);
+int icc_debug_classify(const void *profile, size_t len, int want_bands, int intent);
+
 int launch_reducev(const char *domain, const void *in, size_t in_bpl, int in_h, void *out, size_t out_bpl, int ne,
 	int out_rows, int fmt, const AxisTable &t, cudaStream_t s);
 int launch_reduceh(const char *domain, const void *in, size_t in_bpl, int in_w, void *out, size_t out_bpl, int bands,

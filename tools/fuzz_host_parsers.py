@@ -1,5 +1,5 @@
 """tools/fuzz_host_parsers.py -- mutation fuzzing of the host-side parsers that read untrusted bytes (the JPEG marker
-parser + the decoder's host twin, the ICC profile parser), meant to run against an AddressSanitizer build:
+parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser), meant to run against an AddressSanitizer build:
 
     VB200_LIB=/tmp/asan/libvb200_asan.so LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \
         python tools/fuzz_host_parsers.py [seconds]
@@ -60,6 +60,19 @@ def mutate(rng, s):
     return bytes(s)
 
 
+def app2_mutant(rng, s):
+    """a JPEG with APP2 ICC_PROFILE segments in any order: sequence numbers 0 / 1 / 100 / 101 / 255 and random, duplicates,
+    gaps, segment lengths 13 .. 16, and segments after the first SOS"""
+    segs = []
+    for _ in range(rng.integers(0, 6)):
+        seq = int(rng.choice([0, 1, 2, 3, 100, 101, 255, rng.integers(0, 256)]))
+        body = b"ICC_PROFILE\0" + bytes([seq, int(rng.integers(0, 256))]) + bytes(rng.integers(0, 256, rng.integers(0, 300), dtype=np.uint8))
+        body = body[:int(rng.choice([13, 14, 15, 16, len(body)]))]
+        segs.append(b"\xff\xe2" + (len(body) + 2).to_bytes(2, "big") + body)
+    cut = 2 if rng.integers(0, 2) else max(2, s.find(b"\xff\xda") + 4 + int(rng.integers(0, 40)))
+    return s[:cut] + b"".join(segs) + s[cut:]
+
+
 def main():
     budget = float(sys.argv[1]) if len(sys.argv) > 1 else 60.0
     rng = np.random.default_rng(int(time.time()))
@@ -77,6 +90,12 @@ def main():
         for shrink in (1, 2, 8):
             try:
                 vb.jpeg_decode_host_twin(s, shrink)
+                ok += 1
+            except vb.Error:
+                fails += 1
+        for t in (s, app2_mutant(rng, good[rng.integers(0, len(good))])):
+            try:
+                vb.jpeg_icc_profile(t)
                 ok += 1
             except vb.Error:
                 fails += 1
