@@ -352,7 +352,7 @@ typedef struct {
 } VB200ThumbnailIcc;
 
 /* The ICC stage runs after the thumbnail kernel and before the sharpen stage.  NULL, or a NULL output profile: off.
- * The profiles are copied.  Not available with linear = 1 (-1).
+ * The profiles are copied.  Not available with linear = 1 (-1): see vb200_thumbnail_plan_set_linear_icc.
  */
 int vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc);
 /* bands of an output frame: the plan's bands, or what the output profile makes of them */
@@ -368,6 +368,38 @@ int vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, 
 /* vips_thumbnail_buffer with colour management: the embedded profile comes from the stream's APP2 segments */
 int vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size,
 	const VB200ThumbnailIcc *icc);
+/* ------------------------------------------------ thumbnail: colour-managed linear-light thumbnails
+ *
+ * vips_thumbnail(..., linear = TRUE) with "input_profile" / "output_profile" / "intent" (resample/thumbnail.c:766-805, 929-987)
+ * for 8-bit sRGB frames of 3+ bands.  Unlike the non-linear mode, an embedded profile alone turns colour management on.  Per frame:
+ *   - a profile to import with (the embedded one, input_profile or the built-in sRGB profile, chosen as above): vips_icc_import
+ *     to float XYZ, float premultiply / resize / unpremultiply with max_alpha 255, vips_icc_export(depth 8) to output_profile --
+ *     or, with no output profile, to the profile the import used.  One that cannot serve as an output profile: -1, as the
+ *     reference's "no output profile".
+ *   - no embedded profile and no input_profile, but an output profile: the plain linear chain, vips_colourspace(scRGB -> XYZ),
+ *     then vips_icc_export(output_profile, depth 8).
+ *   - neither: the plain linear thumbnail, unchanged.
+ * The import runs inside the linear thumbnail's vertical kernel and the export inside its horizontal kernel.  Output bands
+ * follow the export's profile plus alpha.  1- / 2-band frames, 16-bit frames and other interpretations return -1.
+ */
+/* Linear plans only (-1 otherwise); NULL: off.  A struct with output_profile NULL: frames with a profile to import with export
+ * to that profile, the others run the plain path.  The profiles are copied and checked here.
+ */
+int vb200_thumbnail_plan_set_linear_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc);
+/* vips_thumbnail_image(..., linear = TRUE) with colour management; icc NULL = vb200_thumbnail_image(linear = 1) */
+int vb200_thumbnail_image_linear_icc(const VB200Image *in, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len);
+/* vips_thumbnail_buffer(..., linear = TRUE): decoded at full size (thumbnail.c:496-499), the embedded profile from the
+ * stream's APP2 segments
+ */
+int vb200_thumbnail_buffer_linear_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc);
+/* Test hook, host only: one frame's linear-mode choice.  *branch 0 plain, 1 import + export, 2 XYZ export; *source as
+ * vb200_debug_icc_select (-1: no import); *export_from 0 output_profile, 1 the import's profile, -1 no export.  -1: error.
+ */
+int vb200_debug_icc_select_linear(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len,
+	int *branch, int *source, int *export_from);
+
 /* vips_image_get_blob(VIPS_META_ICC_NAME) of a JPEG stream (foreign/jpeg2vips.c:699-799): the APP2 "ICC_PROFILE" chunks
  * before the first SOS, by sequence number 1 .. 100, concatenated up to the first missing one.  Host only, no GPU.
  * 0 with *profile_len = 0: no profile; out = NULL only reports the length; -1 when cap is too small or the stream is
@@ -470,6 +502,10 @@ int vb200_debug_icc_classify(const void *profile, size_t len, int want_bands, in
  * (its icc_frames_kernel launches, from the first to the last); -1 when none was timed
  */
 float vb200_debug_icc_stage_ms(void);
+/* with env VB200_LINEAR_TIMING set: CUDA-event milliseconds of the calling thread's last two-kernel linear thumbnail call
+ * (from before its first linear_v launch to after its last linear_h launch); -1 when none was timed
+ */
+float vb200_debug_linear_thumb_ms(void);
 
 /* Test hook, host only (no GPU, no CUDA call): the reducev geometry, sampling table and
  * tensor-pipe tables of a vertical thumbnail shrink exactly as a plan builds them, so that the CPU

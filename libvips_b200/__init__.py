@@ -59,16 +59,26 @@ class CThumbnailIcc(C.Structure):
                 ("builtin_grey_len", C.c_size_t), ("intent", C.c_int)]
 
 
+def _icc_struct(output_profile, input_profile, intent, builtin_profiles):
+    b = builtin_profiles or {}
+    blob = lambda p: (bytes(p), len(p)) if p is not None else (None, 0)
+    i, o, r, g = blob(input_profile), blob(output_profile), blob(b.get("srgb")), blob(b.get("sgrey"))
+    return CThumbnailIcc(i[0], i[1], o[0], o[1], r[0], r[1], g[0], g[1], INTENTS[intent] if isinstance(intent, str) else int(intent))
+
+
 def thumbnail_icc(output_profile=None, input_profile=None, intent="relative", builtin_profiles=None):
     """The VB200ThumbnailIcc of vips_thumbnail's output_profile / input_profile / intent (profiles are bytes);
     builtin_profiles: {"srgb": bytes, "sgrey": bytes}, what vips_profile_load gives for those names.  None when
     colour management is off."""
     if output_profile is None:
         return None
-    b = builtin_profiles or {}
-    blob = lambda p: (bytes(p), len(p)) if p is not None else (None, 0)
-    i, o, r, g = blob(input_profile), blob(output_profile), blob(b.get("srgb")), blob(b.get("sgrey"))
-    return CThumbnailIcc(i[0], i[1], o[0], o[1], r[0], r[1], g[0], g[1], INTENTS[intent] if isinstance(intent, str) else int(intent))
+    return _icc_struct(output_profile, input_profile, intent, builtin_profiles)
+
+
+def linear_icc(output_profile=None, input_profile=None, intent="relative", builtin_profiles=None):
+    """The VB200ThumbnailIcc of vips_thumbnail(linear=TRUE)'s output_profile / input_profile / intent: unlike thumbnail_icc it is
+    never None, since in linear mode an embedded profile alone turns colour management on"""
+    return _icc_struct(output_profile, input_profile, intent, builtin_profiles)
 
 
 def _embedded_arrays(embedded, n):
@@ -172,6 +182,10 @@ def lib():
         L.vb200_jpeg_icc_profile.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         L.vb200_debug_icc_select.argtypes = [TI, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int)]
         L.vb200_debug_icc_classify.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_int]
+        L.vb200_thumbnail_plan_set_linear_icc.argtypes = [C.c_void_p, TI]
+        L.vb200_thumbnail_image_linear_icc.argtypes = [IP, IP, C.c_int, C.c_int, C.c_int, TI, C.c_char_p, C.c_size_t]
+        L.vb200_thumbnail_buffer_linear_icc.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int, TI]
+        L.vb200_debug_icc_select_linear.argtypes = [TI, C.c_int, C.c_char_p, C.c_size_t, PI, PI, PI]
         RP = C.POINTER(CRegion)
         L.vb200_reducev_gen.argtypes = [RP, RP, C.POINTER(CReduceParams)]
         L.vb200_reduceh_gen.argtypes = [RP, RP, C.POINTER(CReduceParams)]
@@ -356,6 +370,15 @@ class Image:
             return self._call(lib().vb200_thumbnail_image, int(width), int(height or 0), SIZES[size], int(linear))
         emb = bytes(embedded_profile) if embedded_profile else None
         return self._call(lib().vb200_thumbnail_image_icc, int(width), int(height or 0), SIZES[size], C.byref(icc), emb,
+                          len(emb) if emb else 0)
+
+    def thumbnail_image_linear(self, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
+                               embedded_profile=None, builtin_profiles=None):
+        """vips_thumbnail_image(linear=TRUE) with colour management: an embedded profile alone turns it on; with no profiles
+        at all, the bytes of thumbnail_image(linear=True)"""
+        icc = linear_icc(output_profile, input_profile, intent, builtin_profiles)
+        emb = bytes(embedded_profile) if embedded_profile else None
+        return self._call(lib().vb200_thumbnail_image_linear_icc, int(width), int(height or 0), SIZES[size], C.byref(icc), emb,
                           len(emb) if emb else 0)
 
     # ---- convolution
@@ -550,6 +573,23 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
     return a
 
 
+def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
+                            builtin_profiles=None):
+    """vips_thumbnail_buffer(linear=TRUE) of a JPEG stream: full-size decode + linear-light thumbnail on the device, colour-managed
+    with the profile the stream embeds and / or the profiles given"""
+    stream = bytes(stream)
+    out = CImage()
+    out.where = HOST
+    icc = linear_icc(output_profile, input_profile, intent, builtin_profiles)
+    _check(lib().vb200_thumbnail_buffer_linear_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
+                                                   C.byref(icc)))
+    n = out.Ysize * out.bpl
+    a = np.frombuffer(C.string_at(out.data, n), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
+    a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
+    lib().vb200_image_free(C.byref(out))
+    return a
+
+
 def thumbnail_jpegshrink(width, height, target_width, target_height=None, size="both"):
     """vips_thumbnail_find_jpegshrink (thumbnail.c:489-517)"""
     return int(lib().vb200_thumbnail_jpegshrink(width, height, target_width, target_height or 0, SIZES[size]))
@@ -588,6 +628,15 @@ class ThumbnailPlan:
         out_frame_bytes follow the output profile"""
         icc = thumbnail_icc(output_profile, input_profile, intent, builtin_profiles)
         _check(lib().vb200_thumbnail_plan_set_icc(self._p, C.byref(icc) if icc is not None else None))
+        self.out_bands = int(lib().vb200_thumbnail_plan_output_bands(self._p))
+        self.out_frame_bytes = self.out_width * self.out_height * self.out_bands
+
+    def set_linear_icc(self, output_profile=None, input_profile=None, intent="relative", builtin_profiles=None, enabled=True):
+        """colour management of a linear plan (thumbnail.c:766-805, 929-987): frames with an embedded profile or input_profile
+        import to XYZ and export to output_profile (or to their own profile); others export to output_profile if set, else
+        run the plain path.  enabled=False: off"""
+        icc = linear_icc(output_profile, input_profile, intent, builtin_profiles) if enabled else None
+        _check(lib().vb200_thumbnail_plan_set_linear_icc(self._p, C.byref(icc) if icc is not None else None))
         self.out_bands = int(lib().vb200_thumbnail_plan_output_bands(self._p))
         self.out_frame_bytes = self.out_width * self.out_height * self.out_bands
 

@@ -1398,7 +1398,7 @@ struct LinearThumb;
 int linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const ReduceGeom &gv, const ReduceGeom &gh,
 	const AxisTable &tv, const AxisTable &th, LinearThumb **out);
 int linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_stride, void *out, size_t out_stride, int n,
-	cudaStream_t s);
+	cudaStream_t s, const LinIccBatch *icc = nullptr, int out_bands = 0);
 void linear_thumb_free(LinearThumb *lt);
 
 struct ThumbnailPlanImpl {
@@ -1458,8 +1458,11 @@ struct ThumbnailPlanImpl {
 	/* colour management between the thumbnail and the sharpen stage (vb200_thumbnail_plan_set_icc); null = off */
 	IccStage *icc = nullptr;
 	int icc_bands = 0;			 /* output bands with the stage on */
+	/* linear = TRUE with colour management (vb200_thumbnail_plan_set_linear_icc): import / export inside the linear thumbnail */
+	IccStage *licc = nullptr;
+	int licc_bands = 0;
 	size_t stage_out_frame = 0; /* the host pump's output slots are sized for frames of this many bytes */
-	int out_bands() const { return icc ? icc_bands : bands; }
+	int out_bands() const { return icc ? icc_bands : licc ? licc_bands : bands; }
 };
 
 /* sharpen_fused.cu */
@@ -2303,6 +2306,8 @@ static int thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *p
 	size_t out_stride, int n, cudaStream_t s);
 static int thumbnail_plan_run_fused(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
 	size_t out_stride, int n, cudaStream_t s);
+static int thumbnail_plan_run_linear_icc(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int n, cudaStream_t s, const void *const *embedded, const size_t *embedded_lens, int frame0);
 
 double
 thumbnail_common_shrink(int w, int h, int tw, int th, int size)
@@ -2318,10 +2323,13 @@ thumbnail_common_shrink(int w, int h, int tw, int th, int size)
  */
 int
 thumbnail_plan_run_device(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s, const void *const *embedded = nullptr, const size_t *embedded_lens = nullptr)
+	size_t out_stride, int n, cudaStream_t s, const void *const *embedded = nullptr, const size_t *embedded_lens = nullptr,
+	int frame0 = 0)
 {
 	if (n <= 0)
 		return 0;
+	if (pl->licc)
+		return thumbnail_plan_run_linear_icc(domain, pl, in, in_stride, out, out_stride, n, s, embedded, embedded_lens, frame0);
 	if (!pl->sharpen && !pl->icc)
 		return thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, out, out_stride, n, s);
 	const size_t frame = (size_t) pl->OW * pl->OH * pl->bands;
@@ -2338,7 +2346,7 @@ thumbnail_plan_run_device(const char *domain, ThumbnailPlanImpl *pl, const void 
 	const void *sin = mid;
 	if (!rc && pl->icc) {
 		rc = icc_stage_run(domain, pl->icc, mid, frame, pl->sharpen ? mid2 : out, pl->sharpen ? sframe : out_stride, n,
-			(size_t) pl->OW * pl->OH, embedded, embedded_lens, s);
+			(size_t) pl->OW * pl->OH, embedded, embedded_lens, s, frame0);
 		sin = mid2;
 	}
 	if (!rc && pl->sharpen) {
@@ -2400,6 +2408,97 @@ thumbnail_linear_chain(const char *domain, ThumbnailPlanImpl *pl, const void *in
 	dev_image_release(&res, s);
 	dev_image_release(&unpre, s);
 	dev_image_release(&fin, s);
+	return rc;
+}
+
+/* thumbnail.c:766-805, 848-902, 929-970 for one colour-managed frame of a linear plan, as the chain of leaf kernels (geometries the
+ * two-kernel path declines, and VB200_NO_LINEAR_FUSED): LIN_IMPORT runs the import job (icc_kernel) -> float premultiply (255) ->
+ * float resize -> float unpremultiply (255) -> the export job; LIN_XYZ the scRGB chain of thumbnail_linear_chain, then
+ * vips_colourspace(XYZ) and the export job.  `out` takes the export's bands.
+ */
+static int
+thumbnail_linear_icc_chain(const char *domain, ThumbnailPlanImpl *pl, const LinIccFrame &fr, const IccJob *jobs, const void *in,
+	void *out, cudaStream_t s)
+{
+	DevImage din, lin, pre, res, unpre, xyz, fin;
+	din.w = pl->W;
+	din.h = pl->H;
+	din.bands = pl->bands;
+	din.fmt = VB200_FORMAT_UCHAR;
+	din.type = VB200_INTERPRETATION_sRGB;
+	din.bpl = (size_t) pl->W * pl->bands;
+	din.data = const_cast<void *>(in);
+	const bool imp = fr.kind == LIN_IMPORT;
+	const double max_alpha = imp ? 255.0 : 1.0; /* XYZ after the import, scRGB otherwise (header.c:195-206) */
+	int rc = imp ? icc_job_apply(domain, jobs, fr.imp, din, &lin, s)
+				 : dev_colourspace(domain, din, &lin, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, s);
+	const DevImage *cur = &lin;
+	if (!rc && pl->premul) {
+		rc = dev_premultiply(domain, lin, &pre, max_alpha, 0, s);
+		cur = &pre;
+	}
+	if (!rc)
+		rc = dev_resize(domain, *cur, &res, 1.0 / pl->hshrink, 1.0 / pl->vshrink, VB200_KERNEL_LANCZOS3, 2.0, s);
+	cur = &res;
+	if (!rc && pl->premul) {
+		rc = dev_unpremultiply(domain, res, &unpre, max_alpha, 0, s);
+		cur = &unpre;
+	}
+	if (!rc && !imp) {
+		rc = dev_colourspace(domain, *cur, &xyz, VB200_INTERPRETATION_XYZ, VB200_INTERPRETATION_scRGB, s);
+		cur = &xyz;
+	}
+	if (!rc)
+		rc = icc_job_apply(domain, jobs, fr.exp, *cur, &fin, s);
+	if (!rc) {
+		const size_t line = (size_t) fin.w * fin.bands;
+		if (cudaMemcpy2DAsync(out, line, fin.data, fin.bpl, line, fin.h, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+			rc = cuda_fail(domain, cudaGetLastError(), "linear ICC thumbnail copy");
+	}
+	for (DevImage *d : {&lin, &pre, &res, &unpre, &xyz, &fin})
+		dev_image_release(d, s);
+	return rc;
+}
+
+/* A batch of a linear plan with colour management: each frame's branch and jobs from the stage, then the two-kernel path (one V and
+ * one H launch per chunk of frames, whatever their branches) or, where it declines, the leaf chains frame by frame; then sharpen.
+ */
+static int
+thumbnail_plan_run_linear_icc(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int n, cudaStream_t s, const void *const *embedded, const size_t *embedded_lens, int frame0)
+{
+	const int ob = pl->licc_bands;
+	const size_t sframe = (size_t) pl->OW * pl->OH * ob;
+	if (pl->sharpen && ob != 3 && ob != 4) {
+		error(domain, "the sharpen stage needs 3- or 4-band frames, the output profile gives %d bands", ob);
+		return -1;
+	}
+	void *mid = nullptr;
+	if (pl->sharpen && dev_alloc(domain, &mid, sframe * n, s))
+		return -1;
+	void *dst = pl->sharpen ? mid : out;
+	const size_t dst_stride = pl->sharpen ? sframe : out_stride;
+	int rc = icc_stage_run_linear(domain, pl->licc, n, embedded, embedded_lens, s, frame0, [&](const LinIccBatch &b) {
+		int r = pl->lin ? linear_thumb_run(domain, pl->lin, in, in_stride, dst, dst_stride, n, s, &b, ob) : 1;
+		for (int i = 0; r == 1 && i < n; i++) {
+			const void *fin = (const char *) in + (size_t) i * in_stride;
+			void *fout = (char *) dst + (size_t) i * dst_stride;
+			if (b.h_frames[i].kind == LIN_PLAIN ? thumbnail_linear_chain(domain, pl, fin, fout, s)
+												: thumbnail_linear_icc_chain(domain, pl, b.h_frames[i], b.h_jobs, fin, fout, s))
+				return -1;
+		}
+		return r == 1 ? 0 : r;
+	});
+	if (!rc && pl->sharpen) {
+		rc = dev_sharpen_fused(domain, mid, (size_t) pl->OW * ob, sframe, out, (size_t) pl->OW * ob, out_stride, n, pl->OW, pl->OH, ob,
+			pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
+		if (rc == 1) {
+			error(domain, "sharpen parameters are not on the fused path (mask too wide)");
+			rc = -1;
+		}
+	}
+	if (mid)
+		dev_free(mid, s);
 	return rc;
 }
 
@@ -2538,6 +2637,8 @@ thumbnail_plan_destroy(ThumbnailPlanImpl *pl)
 	pl->lin = nullptr;
 	icc_stage_free(pl->icc);
 	pl->icc = nullptr;
+	icc_stage_free(pl->licc);
+	pl->licc = nullptr;
 	for (int i = 0; i < ThumbnailPlanImpl::kHintSlots; i++)
 		if (pl->hint_done[i]) {
 			cudaEventSynchronize(pl->hint_done[i]);
@@ -2744,6 +2845,36 @@ vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *
 }
 
 extern "C" int
+vb200_thumbnail_plan_set_linear_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc)
+{
+	const char *domain = "thumbnail_plan_set_linear_icc";
+	if (!plan) {
+		error(domain, "null plan");
+		return -1;
+	}
+	ThumbnailPlanImpl &pl = plan->impl;
+	if (!pl.linear) {
+		error(domain, "the plan is not linear: use vb200_thumbnail_plan_set_icc");
+		return -1;
+	}
+	if (!icc) {
+		icc_stage_free(pl.licc);
+		pl.licc = nullptr;
+		return 0;
+	}
+	IccStage *st = icc_stage_new();
+	int ob = 0;
+	if (icc_stage_set_linear(domain, st, icc, pl.bands, &ob)) {
+		icc_stage_free(st);
+		return -1;
+	}
+	icc_stage_free(pl.licc);
+	pl.licc = st;
+	pl.licc_bands = ob;
+	return 0;
+}
+
+extern "C" int
 vb200_thumbnail_plan_output_bands(const VB200ThumbnailPlan *plan)
 {
 	return plan ? plan->impl.out_bands() : -1;
@@ -2759,8 +2890,10 @@ vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, 
 	return vb200_thumbnail_buffer_icc(buf, len, out, width, height, size, nullptr);
 }
 
-extern "C" int
-vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc)
+/* linear: decoded at full size (thumbnail.c:496-499) and thumbnailed by vb200_thumbnail_image_linear_icc */
+static int
+thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	bool linear)
 {
 	const char *domain = "thumbnail_buffer";
 	if (!buf || !out) {
@@ -2770,13 +2903,13 @@ vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int wid
 	if (ensure_init(domain))
 		return -1;
 	std::vector<unsigned char> embedded;
-	if (icc && icc->output_profile && jpeg_icc_profile(domain, (const unsigned char *) buf, len, &embedded))
+	if (icc && (icc->output_profile || linear) && jpeg_icc_profile(domain, (const unsigned char *) buf, len, &embedded))
 		return -1;
 	cudaStream_t s = current_stream();
 	int w0, h0, b0;
 	if (dev_jpeg_decode_batch(domain, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s))
 		return -1;
-	const int shrink = vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
+	const int shrink = linear ? 1 : vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
 	int w, h, b;
 	if (dev_jpeg_decode_batch(domain, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s))
 		return -1;
@@ -2799,7 +2932,8 @@ vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int wid
 		VB200Image tmp;
 		memset(&tmp, 0, sizeof(tmp));
 		tmp.where = VB200_DEVICE;
-		rc = vb200_thumbnail_image_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size());
+		rc = linear ? vb200_thumbnail_image_linear_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size())
+					: vb200_thumbnail_image_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size());
 		if (!rc) {
 			/* deliver where the caller asked (allocate-or-fill) */
 			DevImage dt;
@@ -2818,6 +2952,19 @@ vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int wid
 	}
 	dev_image_release(&dec, s);
 	return rc;
+}
+
+extern "C" int
+vb200_thumbnail_buffer_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc)
+{
+	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, false);
+}
+
+extern "C" int
+vb200_thumbnail_buffer_linear_icc(const void *buf, size_t len, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc)
+{
+	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, true);
 }
 
 /* Decode staging feeding the plan (SURVEY 8f rank 1): compressed JPEG bytes up, decoded at `shrink` on the device
@@ -2841,7 +2988,7 @@ vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs,
 	if (out_frame_stride == 0)
 		out_frame_stride = out_frame;
 	/* with colour management on, each stream's embedded profile (jpeg2vips.c:699-799) goes to the ICC stage */
-	std::vector<std::vector<unsigned char>> profiles(pl.icc ? n : 0);
+	std::vector<std::vector<unsigned char>> profiles(pl.icc || pl.licc ? n : 0);
 	std::vector<const void *> emb(profiles.size());
 	std::vector<size_t> emb_len(profiles.size());
 	for (size_t i = 0; i < profiles.size(); i++) {
@@ -2852,8 +2999,8 @@ vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs,
 		emb[i] = profiles[i].empty() ? nullptr : profiles[i].data();
 		emb_len[i] = profiles[i].size();
 	}
-	const void *const *embedded = pl.icc ? emb.data() : nullptr;
-	const size_t *embedded_lens = pl.icc ? emb_len.data() : nullptr;
+	const void *const *embedded = pl.icc || pl.licc ? emb.data() : nullptr;
+	const size_t *embedded_lens = pl.icc || pl.licc ? emb_len.data() : nullptr;
 	void *dec = nullptr, *res = nullptr;
 	if (dev_alloc(domain, &dec, in_frame * n, s))
 		return -1;
@@ -2953,7 +3100,7 @@ vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t 
 		VB200_CUDA(domain, cudaMemcpy2DAsync(pl.stage_in[slot], in_frame, (const char *) in + (size_t) f * in_frame_stride,
 							   in_frame_stride, in_frame, n, cudaMemcpyHostToDevice, s));
 		if (thumbnail_plan_run_device(domain, &pl, pl.stage_in[slot], in_frame, pl.stage_out[slot], out_frame, n, s,
-				embedded ? embedded + f : nullptr, embedded_lens ? embedded_lens + f : nullptr))
+				embedded ? embedded + f : nullptr, embedded_lens ? embedded_lens + f : nullptr, f))
 			return -1;
 		VB200_CUDA(domain, cudaMemcpy2DAsync((char *) out + (size_t) f * out_frame_stride, out_frame_stride,
 							   pl.stage_out[slot], out_frame, out_frame, n, cudaMemcpyDeviceToHost, s));
@@ -2966,15 +3113,34 @@ vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t 
 	return 0;
 }
 
-/* vips_thumbnail_image, with colour management when icc sets an output profile */
+/* vips_thumbnail_image, with colour management when icc sets an output profile; linear_icc: linear = TRUE with icc (may be NULL)
+ * through vb200_thumbnail_plan_set_linear_icc
+ */
 static int
 thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear, const VB200ThumbnailIcc *icc,
-	const void *embedded, size_t embedded_len)
+	const void *embedded, size_t embedded_len, bool linear_icc = false)
 {
 	const char *domain = "thumbnail";
 	if (!in || !out) {
 		error(domain, "null argument");
 		return -1;
+	}
+	if (linear_icc && icc && !(in->Type == VB200_INTERPRETATION_sRGB && in->Bands >= 3)) {
+		/* thumbnail.c:766-789 imports other interpretations with a profile of their space, and 1- / 2-band frames with sGrey:
+		 * not on the device path
+		 */
+		error(domain, "linear colour-managed thumbnails of interpretation %d with %d bands are not supported on the device path",
+			in->Type, in->Bands);
+		return -1;
+	}
+	if (linear_icc && icc) {
+		/* the profiles are checked before any pixel moves: the stage's own checks, on the host, on a stage of its own */
+		IccStage *st = icc_stage_new();
+		int ob = 0;
+		const int rc = icc_stage_set_linear(domain, st, icc, in->Bands, &ob);
+		icc_stage_free(st);
+		if (rc)
+			return -1;
 	}
 	if (icc && icc->output_profile &&
 		!((in->Type == VB200_INTERPRETATION_sRGB && in->Bands >= 3) || (in->Type == VB200_INTERPRETATION_B_W && in->Bands < 3))) {
@@ -2997,14 +3163,14 @@ thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height
 		height, size, linear);
 	if (!plan)
 		return -1;
-	if (icc && vb200_thumbnail_plan_set_icc(plan, icc)) {
+	if (icc && (linear_icc ? vb200_thumbnail_plan_set_linear_icc(plan, icc) : vb200_thumbnail_plan_set_icc(plan, icc))) {
 		vb200_thumbnail_plan_free(plan);
 		return -1;
 	}
 	const int ob = plan->impl.out_bands();
 	/* icc_transform.c:374-433: the output interpretation follows the output profile's colour bands */
 	const int colour = ob - (in->Bands - (in->Bands < 3 ? 1 : 3));
-	const int otype = !plan->impl.icc ? in->Type
+	const int otype = !plan->impl.icc && !plan->impl.licc ? in->Type
 		: colour == 1				  ? VB200_INTERPRETATION_B_W
 		: colour == 3				  ? VB200_INTERPRETATION_sRGB
 									  : VB200_INTERPRETATION_CMYK;
@@ -3044,4 +3210,14 @@ vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, int 
 	const void *embedded, size_t embedded_len)
 {
 	return thumbnail_image_run(in, out, width, height, size, 0, icc, embedded, embedded_len);
+}
+
+/* vips_thumbnail_image(..., linear = TRUE) with "input_profile" / "output_profile" / "intent" (thumbnail.c:766-805, 929-987):
+ * an embedded profile alone turns colour management on.  icc NULL: vb200_thumbnail_image(linear = 1).
+ */
+extern "C" int
+vb200_thumbnail_image_linear_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	const void *embedded, size_t embedded_len)
+{
+	return thumbnail_image_run(in, out, width, height, size, 1, icc, embedded, embedded_len, true);
 }

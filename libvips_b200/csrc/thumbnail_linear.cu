@@ -36,6 +36,7 @@
 #include <vector>
 
 #include "colour_steps.cuh"
+#include "icc_eval.cuh"
 #include "vb200_internal.h"
 
 namespace vb200 {
@@ -62,6 +63,12 @@ struct LinVParams {
 	/* the residual-2.0 schedule (linear_v2_kernel): first[y] = f0 + 2 y, one phase, 13 taps */
 	int f0;
 	double c2[13];
+	/* colour-managed instantiations: each frame's LinIccFrame (this launch's first frame at [0]) and the batch's job table; the
+	 * import job and its TRC tables are staged at byte icc_off of the dynamic shared memory
+	 */
+	const LinIccFrame *iframes;
+	const IccJob *ijobs;
+	int icc_off;
 };
 
 struct LinHParams {
@@ -75,9 +82,70 @@ struct LinHParams {
 	StepInfo bwd[2];
 	int n_bwd;
 	const int *Y2v_8;
+	/* colour-managed instantiations: as LinVParams; the export job at byte icc_off of the dynamic shared memory, out_bands
+	 * bands per output pixel, and the alpha steps of vips_colourspace(scRGB -> XYZ) for LIN_XYZ frames
+	 */
+	const LinIccFrame *iframes;
+	const IccJob *ijobs;
+	int icc_off, out_bands;
+	StepInfo xyz[2];
+	int n_xyz;
 };
 
-template <int NCH, bool PREMUL, int VST>
+/* ---- the colour-managed frames (LinIccFrame): import in kernel V, export in kernel H, the evaluator's own code (icc_eval.cuh) */
+
+/* kernel V's per-CTA setup of an LIN_IMPORT frame: the import job, and its tabulated TRCs (matrix / TRC profiles), into shared
+ * memory.  Uniform across the CTA (one frame per CTA).
+ */
+__device__ __forceinline__ const IccJob *
+stage_import(const LinVParams &P, int frame, unsigned char *smem_raw, const float **tab)
+{
+	const LinIccFrame fr = P.iframes[frame];
+	if (fr.kind != LIN_IMPORT)
+		return nullptr;
+	IccJob *sj = (IccJob *) (smem_raw + P.icc_off);
+	float *st = (float *) (sj + 1);
+	const unsigned *src = (const unsigned *) (P.ijobs + fr.imp);
+	for (int i = threadIdx.x; i < (int) (sizeof(IccJob) / 4); i += blockDim.x)
+		((unsigned *) sj)[i] = src[i];
+	__syncthreads();
+	if (sj->in_tab >= 0)
+		for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x)
+			st[i] = sj->in.pool[sj->in_tab + i];
+	*tab = st;
+	return sj;
+}
+
+/* profiles without tabulated TRCs (lut8 / lut16 / mAB): the evaluator's general path, out of line */
+__device__ __noinline__ void
+import_general(const IccJob &J, unsigned px, double *xyz)
+{
+	const double dev[4] = {(double) (px & 255u) / 255.0, (double) ((px >> 8) & 255u) / 255.0, (double) ((px >> 16) & 255u) / 255.0, 0.0};
+	side_to_xyz(J.in, dev, xyz);
+}
+
+/* vips_icc_import(pcs = XYZ) of one pixel's R, G, B bytes (px, low byte first) to float XYZ, icc_colour's mode 0 */
+__device__ __forceinline__ void
+import_pixel(const IccJob &J, const float *tab, unsigned px, float *q)
+{
+	double xyz[3];
+	if (J.in_tab >= 0) {
+		const int code[3] = {(int) (px & 255u), (int) ((px >> 8) & 255u), (int) ((px >> 16) & 255u)};
+		icc_tab_to_xyz(J, tab, code, xyz);
+	}
+	else
+		import_general(J, px, xyz);
+	icc_decode_xyz16(xyz, q);
+}
+
+/* vips_icc_export(depth 8) of one float XYZ pixel (+ alpha), icc_pixel's mode 1 */
+__device__ __noinline__ void
+export_pixel(const IccJob &J, const float *pix, uint8_t *o)
+{
+	icc_pixel(J, pix, o);
+}
+
+template <int NCH, bool PREMUL, int VST, bool ICC = false>
 __global__ void __launch_bounds__(kVThreads, 2)
 linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict__ in, int frame0)
 {
@@ -94,10 +162,22 @@ linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict_
 	unsigned *s_ring = (unsigned *) (s_nal + 256);
 
 	const int t = threadIdx.x;
+	const IccJob *J = nullptr; /* an LIN_IMPORT frame: its import job, in shared memory */
+	const float *s_tab = nullptr;
+	if (ICC)
+		J = stage_import(P, frame0 + blockIdx.z, smem_raw, &s_tab);
 	for (int i = t; i < 65 * P.nv; i += kVThreads)
 		s_vc[i] = P.vcoef[i];
 	for (int i = t; i < 256; i += kVThreads) {
 		s_lin[i] = P.v2Y_8[i];
+		if (ICC && J) {
+			/* vips_icc_import carries the alpha to float unscaled (sRGB and XYZ both max 255); PRE_RGBA with max_alpha 255
+			 * (XYZ is neither scRGB nor 16-bit, header.c:195-206)
+			 */
+			s_al[i] = (float) i;
+			s_nal[i] = (float) __ddiv_rn(fmax(0.0, fmin(255.0, (double) i)), 255.0);
+			continue;
+		}
 		/* the 4th band through sRGB -> scRGB as vips_colour_build carries it, then PRE_RGBA's
 		 * nalpha = (float) clip(alpha) / max_alpha with max_alpha = 1.0 (premultiply.c:104-111)
 		 */
@@ -165,7 +245,19 @@ linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict_
 				float q[NCH];
 				if (NCH == 4) {
 					const unsigned px = ring ? mine[(k + kk) * kVThreads] : __ldg((const unsigned *) p);
-					const float r = s_lin[px & 255], g = s_lin[(px >> 8) & 255], b = s_lin[(px >> 16) & 255];
+					float r, g, b;
+					if (ICC && J) {
+						float x3[3];
+						import_pixel(*J, s_tab, px, x3);
+						r = x3[0];
+						g = x3[1];
+						b = x3[2];
+					}
+					else {
+						r = s_lin[px & 255];
+						g = s_lin[(px >> 8) & 255];
+						b = s_lin[(px >> 16) & 255];
+					}
 					if (PREMUL) {
 						const float n = s_nal[px >> 24];
 						q[0] = __fmul_rn(r, n);
@@ -179,6 +271,8 @@ linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict_
 					}
 					q[NCH - 1] = s_al[px >> 24];
 				}
+				else if (ICC && J)
+					import_pixel(*J, s_tab, (unsigned) __ldg(p) | ((unsigned) __ldg(p + 1) << 8) | ((unsigned) __ldg(p + 2) << 16), q);
 				else {
 #pragma unroll
 					for (int c = 0; c < NCH; c++)
@@ -248,7 +342,7 @@ linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict_
  * accumulators rotate through registers by unrolling seven iterations; coefficients are kernel-parameter
  * constants.  Same sums in the same order as the general kernel -- 42 instead of 93 instructions per pixel.
  */
-template <bool PREMUL, int VST>
+template <bool PREMUL, int VST, bool ICC = false>
 __global__ void __launch_bounds__(kVThreads, 2)
 linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict__ in, int frame0)
 {
@@ -268,8 +362,16 @@ linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict
 	unsigned *s_ring = (unsigned *) (s_lin + 4 * 256);
 
 	const int t = threadIdx.x;
+	const IccJob *J = nullptr; /* an LIN_IMPORT frame: its import job, in shared memory (as linear_v_kernel) */
+	const float *s_tab = nullptr;
+	if (ICC)
+		J = stage_import(P, frame0 + blockIdx.z, smem_raw, &s_tab);
 	for (int i = t; i < 256; i += kVThreads) {
 		s_lin[i] = P.v2Y_8[i];
+		if (ICC && J) {
+			s_aln[i] = make_float2((float) __ddiv_rn(fmax(0.0, fmin(255.0, (double) i)), 255.0), (float) i);
+			continue;
+		}
 		const float A = (float) carry_extra_band((double) i, P.fwd, P.n_fwd);
 		const float clip_alpha = (float) fmax(0.0, fmin(1.0, (double) A));
 		s_aln[i] = make_float2((float) __ddiv_rn((double) clip_alpha, 1.0), A);
@@ -335,7 +437,19 @@ linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict
 #pragma unroll
 					for (int k = 0; k < VST; k++) {
 						const unsigned px = mine[(h * VST + k) * kVThreads];
-						const float r = s_lin[px & 255], g = s_lin[(px >> 8) & 255], b = s_lin[(px >> 16) & 255];
+						float r, g, b;
+						if (ICC && J) {
+							float x3[3];
+							import_pixel(*J, s_tab, px, x3);
+							r = x3[0];
+							g = x3[1];
+							b = x3[2];
+						}
+						else {
+							r = s_lin[px & 255];
+							g = s_lin[(px >> 8) & 255];
+							b = s_lin[(px >> 16) & 255];
+						}
 						const float2 an = s_aln[px >> 24];
 						float q0 = r, q1 = g, q2 = b;
 						if (PREMUL) {
@@ -382,7 +496,7 @@ linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict
 	}
 }
 
-template <int NCH, bool PREMUL>
+template <int NCH, bool PREMUL, bool ICC = false>
 __global__ void __launch_bounds__(256)
 linear_h_kernel(const __grid_constant__ LinHParams P, uint8_t *__restrict__ out, int frame0)
 {
@@ -401,6 +515,18 @@ linear_h_kernel(const __grid_constant__ LinHParams P, uint8_t *__restrict__ out,
 	const int y = blockIdx.x;
 	const int frame = frame0 + blockIdx.y;
 	const float *row = P.mid + (size_t) frame * P.mid_frame_stride + (size_t) y * P.W * NCH;
+	/* a colour-managed frame: its export job into shared memory (the barrier below publishes it) */
+	int kind = LIN_PLAIN;
+	IccJob *J = ICC ? (IccJob *) (smem_raw + P.icc_off) : nullptr;
+	if (ICC) {
+		const LinIccFrame fr = P.iframes[frame];
+		kind = fr.kind;
+		if (kind != LIN_PLAIN) {
+			const unsigned *src = (const unsigned *) (P.ijobs + fr.exp);
+			for (int i = t; i < (int) (sizeof(IccJob) / 4); i += 256)
+				((unsigned *) J)[i] = src[i];
+		}
+	}
 
 	/* ---- shrinkh (FSHRINK, shrinkh.c:134-152) over the embedded row: vips_embed(EXTEND_COPY) = clamp.
 	 * One (column, band) per thread straight from the intermediate image: the NCH lanes of a column read
@@ -432,6 +558,37 @@ linear_h_kernel(const __grid_constant__ LinHParams P, uint8_t *__restrict__ out,
 
 	/* ---- unpremultiply, scRGB -> sRGB: one pixel per thread */
 	uint8_t *orow = out + (size_t) frame * P.out_frame_stride + (size_t) y * P.out_bpl;
+	if (ICC && kind != LIN_PLAIN) {
+		/* unpremultiply with the space's max_alpha (XYZ 255 after the import, scRGB 1.0 otherwise), then the export: from XYZ
+		 * (LIN_IMPORT), or after vips_colourspace(scRGB -> XYZ) (LIN_XYZ)
+		 */
+		const double max_alpha = kind == LIN_IMPORT ? 255.0 : 1.0;
+		for (int x = t; x < P.OW; x += 256) {
+			float v[4] = {0, 0, 0, 0};
+#pragma unroll
+			for (int c = 0; c < NCH; c++)
+				v[c] = s_row[x * NCH + c];
+			if (PREMUL) {
+				const float alpha = v[NCH - 1];
+				const float factor = fabs((double) alpha) < 0.01 ? 0.0f : (float) __ddiv_rn(max_alpha, (double) alpha);
+				v[0] = __fmul_rn(factor, v[0]);
+				v[1] = __fmul_rn(factor, v[1]);
+				v[2] = __fmul_rn(factor, v[2]);
+				v[NCH - 1] = (float) fmax(0.0, fmin(max_alpha, (double) alpha));
+			}
+			if (kind == LIN_XYZ) {
+				step_scRGB2XYZ(v[0], v[1], v[2]);
+				if (NCH == 4)
+					v[3] = (float) carry_extra_band((double) v[3], P.xyz, P.n_xyz);
+			}
+			uint8_t o[8];
+			export_pixel(*J, v, o);
+			uint8_t *q = orow + (size_t) x * P.out_bands;
+			for (int c = 0; c < P.out_bands; c++)
+				q[c] = o[c];
+		}
+		return;
+	}
 	for (int x = t; x < P.OW; x += 256) {
 		float v[NCH];
 #pragma unroll
@@ -475,6 +632,9 @@ struct LinearThumb {
 	size_t smem_v = 0, smem_h = 0;
 	int vst = 0;
 	bool static2 = false; /* linear_v2_kernel: residual exactly 2.0, 13 taps, one phase */
+	/* the colour-managed instantiations: the ICC jobs (and the import's TRC tables) after the plain layout */
+	size_t smem_v_icc = 0, smem_h_icc = 0;
+	bool icc_ok = false;
 };
 
 /* 0 = ready, 1 = this geometry is not on the two-kernel path (the caller chains the leaf kernels), -1 = error */
@@ -508,9 +668,10 @@ linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const
 	if (smem_v > 100 * 1024 || smem_h > 200 * 1024)
 		return 1;
 
-	RouteParams fwd, bwd;
+	RouteParams fwd, bwd, xyz;
 	if (colour_route_params(domain, VB200_INTERPRETATION_sRGB, VB200_INTERPRETATION_scRGB, &fwd) ||
-		colour_route_params(domain, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, &bwd))
+		colour_route_params(domain, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, &bwd) ||
+		colour_route_params(domain, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_XYZ, &xyz))
 		return -1;
 	if (fwd.n_steps > 2 || bwd.n_steps > 2)
 		return 1;
@@ -524,6 +685,10 @@ linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const
 	lt->premul = premul;
 	lt->smem_v = smem_v;
 	lt->smem_h = smem_h;
+	lt->smem_v_icc = ((smem_v + 15) & ~(size_t) 15) + sizeof(IccJob) + 3 * 256 * 4;
+	lt->smem_h_icc = ((smem_h + 15) & ~(size_t) 15) + sizeof(IccJob);
+	/* two V CTAs per SM as the plain kernel, and no more than the H kernel's limit; otherwise the leaf chain */
+	lt->icc_ok = lt->smem_v_icc <= 110 * 1024 && lt->smem_h_icc <= 200 * 1024 && xyz.n_steps <= 2;
 	lt->vst = gv.int_shrink == 2 || gv.int_shrink == 4 || gv.int_shrink == 8 ? gv.int_shrink : 0;
 
 	/* one device block: vfirst | vphase | hfirst | hphase | vcoef | hcoef */
@@ -590,6 +755,10 @@ linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const
 	memcpy(h.bwd, bwd.steps, sizeof(h.bwd));
 	h.n_bwd = bwd.n_steps;
 	h.Y2v_8 = bwd.t.Y2v_8;
+	memcpy(h.xyz, xyz.steps, sizeof(h.xyz));
+	h.n_xyz = std::min(xyz.n_steps, 2);
+	v.icc_off = (int) ((smem_v + 15) & ~(size_t) 15);
+	h.icc_off = (int) ((smem_h + 15) & ~(size_t) 15);
 	*out = lt;
 	return 0;
 }
@@ -606,15 +775,16 @@ linear_thumb_free(LinearThumb *lt)
 
 namespace {
 
-template <int NCH, bool PREMUL>
+template <int NCH, bool PREMUL, bool ICC = false>
 int
 launch_v(const char *domain, const LinearThumb *lt, const LinVParams &v, const void *in, dim3 grid, int f0, cudaStream_t s)
 {
+	const size_t smem = ICC ? lt->smem_v_icc : lt->smem_v;
 #define LV(VST_) \
 	do { \
-		auto kern = linear_v_kernel<NCH, PREMUL, VST_>; \
-		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_v)); \
-		kern<<<grid, kVThreads, lt->smem_v, s>>>(v, (const uint8_t *) in, f0); \
+		auto kern = linear_v_kernel<NCH, PREMUL, VST_, ICC>; \
+		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); \
+		kern<<<grid, kVThreads, smem, s>>>(v, (const uint8_t *) in, f0); \
 	} while (0)
 	switch (lt->vst) {
 	case 2: LV(2); break;
@@ -653,18 +823,51 @@ launch_v2(const char *domain, const LinearThumb *lt, const LinVParams &v, const 
 	return 0;
 }
 
+/* the colour-managed linear_v2_kernel: a 4-band plan on the two-kernel path premultiplies */
+int
+launch_v2_icc(const char *domain, const LinearThumb *lt, const LinVParams &v, const void *in, dim3 grid, cudaStream_t s)
+{
+#define LV2(VST_) \
+	do { \
+		auto kern = linear_v2_kernel<true, VST_, true>; \
+		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_v_icc)); \
+		kern<<<grid, kVThreads, lt->smem_v_icc, s>>>(v, (const uint8_t *) in, 0); \
+	} while (0)
+	switch (lt->vst) {
+	case 2: LV2(2); break;
+	case 4: LV2(4); break;
+	default: LV2(8); break;
+	}
+#undef LV2
+	return 0;
+}
+
+struct LinearTiming {
+	cudaEvent_t start = nullptr, stop = nullptr;
+	bool pending = false;
+};
+thread_local LinearTiming g_linear_timing;
+
 } // namespace
 
 /* frames: packed uchar, `bands` per pixel; queued on s.  The float intermediate ([OH][W][bands] per frame)
- * comes from the stream-ordered pool, at most kSub frames of it at a time.
+ * comes from the stream-ordered pool, at most kSub frames of it at a time.  icc: the batch's colour-managed frames
+ * (vb200_thumbnail_plan_set_linear_icc), out_bands bands per output pixel; 1 when the plan's geometry leaves no room for
+ * the jobs in shared memory (the caller runs the leaf chain).
  */
 int
 linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_stride, void *out, size_t out_stride, int n,
-	cudaStream_t s)
+	cudaStream_t s, const LinIccBatch *icc, int out_bands)
 {
 	if (n <= 0)
 		return 0;
-	if (lt->bands == 4 && ((((uintptr_t) in) | in_stride | ((uintptr_t) out) | out_stride) & 3) != 0) {
+	if (icc && !lt->icc_ok)
+		return 1;
+	/* kernel V reads RGBA pixels as words; kernel H stores them as words when it writes 4 bands.  With colour management the
+	 * output has the export's bands (2 for grey + alpha, 5 for CMYK + alpha ...), stored byte by byte unless there are 4
+	 */
+	const bool out_words = icc ? out_bands == 4 : lt->bands == 4;
+	if ((lt->bands == 4 && ((((uintptr_t) in) | in_stride) & 3) != 0) || (out_words && ((((uintptr_t) out) | out_stride) & 3) != 0)) {
 		error(domain, "RGBA frames must be 4-byte aligned");
 		return -1;
 	}
@@ -678,12 +881,26 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 	if (dev_alloc(domain, (void **) &mid, mid_frame * 4 * sub, s))
 		return -1;
 	int rc = 0;
+	/* VB200_LINEAR_TIMING: CUDA events from before the first V launch to after the last H launch of this call, read back by
+	 * vb200_debug_linear_thumb_ms
+	 */
+	const bool timing = getenv("VB200_LINEAR_TIMING") != nullptr;
+	if (timing) {
+		for (cudaEvent_t *ev : {&g_linear_timing.start, &g_linear_timing.stop})
+			if (!*ev && cudaEventCreate(ev) != cudaSuccess)
+				rc = cuda_fail(domain, cudaGetLastError(), "linear thumbnail timing event");
+		if (!rc)
+			cudaEventRecord(g_linear_timing.start, s);
+		g_linear_timing.pending = !rc;
+	}
 	for (int f0 = 0; f0 < n && !rc; f0 += sub) {
 		const int nf = std::min(sub, n - f0);
 		LinVParams v = lt->v;
 		v.in_frame_stride = in_stride;
 		v.mid = mid;
 		v.mid_frame_stride = mid_frame;
+		v.iframes = icc ? icc->d_frames + f0 : nullptr;
+		v.ijobs = icc ? icc->d_jobs : nullptr;
 		/* rows per CTA: the whole height when there are enough frames to fill the machine */
 		const int col_blocks = (lt->W + kVThreads - 1) / kVThreads;
 		int splits = 1;
@@ -692,7 +909,11 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		v.RPC = (lt->OH + splits - 1) / splits;
 		const dim3 gv(col_blocks, (lt->OH + v.RPC - 1) / v.RPC, nf);
 		const char *fin = (const char *) in + (size_t) f0 * in_stride;
-		if (lt->static2)
+		if (icc)
+			rc = lt->static2 ? launch_v2_icc(domain, lt, v, fin, gv, s)
+				: lt->bands == 4 ? launch_v<4, true, true>(domain, lt, v, fin, gv, 0, s)
+								 : launch_v<3, false, true>(domain, lt, v, fin, gv, 0, s);
+		else if (lt->static2)
 			rc = launch_v2(domain, lt, v, fin, gv, s);
 		else if (lt->bands == 4)
 			rc = lt->premul ? launch_v<4, true>(domain, lt, v, fin, gv, 0, s) : launch_v<4, false>(domain, lt, v, fin, gv, 0, s);
@@ -711,7 +932,16 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		h.out_frame_stride = out_stride;
 		const dim3 gh(lt->OH, nf);
 		uint8_t *fout = (uint8_t *) out + (size_t) f0 * out_stride;
-		if (lt->bands == 4) {
+		if (icc) {
+			h.iframes = icc->d_frames + f0;
+			h.ijobs = icc->d_jobs;
+			h.out_bands = out_bands;
+			h.out_bpl = (size_t) lt->OW * out_bands;
+			auto kern = lt->bands == 4 ? linear_h_kernel<4, true, true> : linear_h_kernel<3, false, true>;
+			cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_h_icc);
+			kern<<<gh, 256, lt->smem_h_icc, s>>>(h, fout, 0);
+		}
+		else if (lt->bands == 4) {
 			auto kern = lt->premul ? linear_h_kernel<4, true> : linear_h_kernel<4, false>;
 			cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_h);
 			kern<<<gh, 256, lt->smem_h, s>>>(h, fout, 0);
@@ -727,8 +957,20 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		else
 			count_launch();
 	}
+	if (timing && g_linear_timing.pending)
+		cudaEventRecord(g_linear_timing.stop, s);
 	dev_free(mid, s);
 	return rc;
+}
+
+float
+linear_thumb_last_ms()
+{
+	float ms = -1.0f;
+	if (g_linear_timing.pending && cudaEventSynchronize(g_linear_timing.stop) == cudaSuccess &&
+		cudaEventElapsedTime(&ms, g_linear_timing.start, g_linear_timing.stop) != cudaSuccess)
+		ms = -1.0f;
+	return ms;
 }
 
 size_t
@@ -738,3 +980,12 @@ linear_thumb_scratch_bytes_per_frame(const LinearThumb *lt)
 }
 
 } // namespace vb200
+
+/* with env VB200_LINEAR_TIMING set: CUDA-event time of the calling thread's last two-kernel linear thumbnail call (its V and H
+ * launches); -1 if none
+ */
+extern "C" float
+vb200_debug_linear_thumb_ms(void)
+{
+	return vb200::linear_thumb_last_ms();
+}

@@ -7,6 +7,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <functional>
 #include <vector>
 
 #include "vb200.h"
@@ -208,9 +209,42 @@ IccStage *icc_stage_new();
 void icc_stage_free(IccStage *st);
 int icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands);
 int icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
-	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s);
+	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s, int frame0 = 0);
 int icc_debug_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source);
 int icc_debug_classify(const void *profile, size_t len, int want_bands, int intent);
+
+/* The linear mode of the stage (vb200_thumbnail_plan_set_linear_icc): the import runs inside the linear thumbnail's V kernel and
+ * the export inside its H kernel (thumbnail_linear.cu), or in the leaf chain around the float resize.  Each frame takes one of:
+ *   LIN_PLAIN   sRGB -> scRGB ... scRGB -> sRGB, today's linear thumbnail (no profile anywhere);
+ *   LIN_IMPORT  vips_icc_import(XYZ PCS) ... vips_icc_export from XYZ (thumbnail.c:766-789, 929-942: a profile to import with);
+ *   LIN_XYZ     sRGB -> scRGB ... scRGB -> XYZ, vips_icc_export from XYZ (:790-805, 957-970: only an output profile).
+ * imp / exp index the batch's job table.
+ */
+enum { LIN_PLAIN = 0, LIN_IMPORT = 1, LIN_XYZ = 2 };
+struct LinIccFrame {
+	int kind, imp, exp;
+};
+struct IccJob; /* icc_eval.cuh */
+/* one batch's resolved jobs: device copies for the kernels, host copies (device pool pointers) for the leaf chain */
+struct LinIccBatch {
+	const IccJob *d_jobs;
+	const LinIccFrame *d_frames;
+	const IccJob *h_jobs;
+	const LinIccFrame *h_frames;
+};
+int icc_stage_set_linear(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands);
+/* resolves the n frames' jobs (embedded / embedded_lens as icc_stage_run), uploads them on s and calls body with them, the
+ * stage locked and its cache entries held until the launches body queues have been recorded.  frame0: the index of the first
+ * frame in the caller's batch, for the errors that name a frame (the host pump runs a batch in slices)
+ */
+int icc_stage_run_linear(const char *domain, IccStage *st, int n, const void *const *embedded, const size_t *embedded_lens,
+	cudaStream_t s, int frame0, const std::function<int(const LinIccBatch &)> &body);
+/* the leaf chain's ICC steps: jobs[k] over a packed device image (icc_kernel, as vb200_icc_import / _export launch it) */
+int icc_job_apply(const char *domain, const IccJob *jobs, int k, const DevImage &in, DevImage *out, cudaStream_t s);
+/* test hook: one frame's linear-mode choice (*branch LIN_*, *source as icc_debug_select or -1, *export_from 0 output_profile,
+ * 1 the import's profile, -1 none) */
+int icc_debug_select_linear(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *branch,
+	int *source, int *export_from);
 
 int launch_reducev(const char *domain, const void *in, size_t in_bpl, int in_h, void *out, size_t out_bpl, int ne,
 	int out_rows, int fmt, const AxisTable &t, cudaStream_t s);
