@@ -560,10 +560,33 @@ int vb200_debug_jpeg_decode_sync(const void *buf, size_t len, int shrink, int su
  */
 int vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands,
 	int Q, int subsample_mode, void *out, int out_location, size_t out_stride, size_t *lengths);
+/* vips_jpegsave's options that the device encoder takes.  Q, subsample_mode: as above.  optimize_coding
+ * (jpegsave.c:227-232 -> vips2jpeg.c:590-591, cinfo.optimize_coding): non-zero builds each frame's Huffman tables from
+ * its own symbol counts (jchuff.c jpeg_gen_optimal_table), so every frame carries its own DHT segments.
+ * restart_interval (jpegsave.c:284-289 -> vips2jpeg.c:593-597, cinfo.restart_interval): an RSTn marker every that many
+ * MCUs and a DRI segment; 0 for none.  Values above 65535 are refused (-1): libjpeg would write DRI modulo 65536 and a
+ * stream no reader can follow.  With both 0 the streams are vb200_jpegsave_batch's.
+ */
+typedef struct {
+	int Q;
+	int subsample_mode;
+	int optimize_coding;
+	int restart_interval;
+} VB200JpegSaveOptions;
+/* vb200_jpegsave_batch with VB200JpegSaveOptions; the streams are libjpeg-turbo's byte for byte with the same options
+ * (tests/test_jpeg_encode_options.py) */
+int vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height,
+	int bands, const VB200JpegSaveOptions *options, void *out, int out_location, size_t out_stride, size_t *lengths);
 /* test hook, host only: vips_jpegsave_buffer's stream (csrc/jpeg_encode.cu) through the encoder's per-block code on the CPU.
  * subsample_mode: 0 auto (4:2:0 below Q 90, vips2jpeg.c:676-690), 1 on, 2 off.  *len = bytes written */
 int vb200_debug_jpeg_encode(const void *pixels, size_t bpl, int width, int height, int bands, int quality, int subsample_mode, void *out,
 	size_t cap, size_t *len);
+/* test hook, host only: vb200_debug_jpeg_encode with every option of VB200JpegSaveOptions */
+int vb200_debug_jpeg_encode_opts(const void *pixels, size_t bpl, int width, int height, int bands, const VB200JpegSaveOptions *options,
+	void *out, size_t cap, size_t *len);
+/* test hook, host only: the encoder's restatement of jpeg_gen_optimal_table on symbol counts freq[256] -> bits[17]
+ * (bits[0] unused) and huffval[256]; -1 when the counts add up to 10^9 or more */
+int vb200_debug_jpeg_optimal_table(const unsigned *freq, unsigned char *bits, unsigned char *huffval);
 /* with env VB200_JPEG_TIMING: CUDA-event times of jpeg_huffman_kernel / jpeg_idct_kernel over the calling thread's last decode */
 void vb200_debug_jpeg_times(float *huffman_ms, float *idct_ms);
 

@@ -157,6 +157,12 @@ def lib():
         L.vb200_thumbnail_jpegshrink.argtypes = [C.c_int] * 5
         L.vb200_jpegsave_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_void_p, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
+        SO = C.POINTER(JpegSaveOptions)
+        L.vb200_jpegsave_batch_opts.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, SO,
+                                                C.c_void_p, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_jpeg_encode_opts.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, SO, C.c_void_p, C.c_size_t,
+                                                   C.POINTER(C.c_size_t)]
+        L.vb200_debug_jpeg_optimal_table.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.vb200_thumbnail_buffer.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int]
         L.vb200_thumbnail_plan_run_jpeg.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int,
                                                     C.c_void_p, C.c_int, C.c_size_t]
@@ -529,10 +535,17 @@ def flatten_host_twin(a, background=None, max_alpha=0.0, interpretation=None, x4
 _SAVE_BUFFERS = {}
 
 
-def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None):
+class JpegSaveOptions(C.Structure):
+    """VB200JpegSaveOptions"""
+    _fields_ = [("Q", C.c_int), ("subsample_mode", C.c_int), ("optimize_coding", C.c_int), ("restart_interval", C.c_int)]
+
+
+def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0):
     """vips_jpegsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1 or 3) on the device -> list of bytes.
-    in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands)"""
+    in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  optimize_coding: per-frame Huffman
+    tables; restart_interval: an RSTn marker every that many MCUs (0..65535, 0 for none)"""
     mode = {"auto": 0, "on": 1, "off": 2}[subsample_mode]
+    opts = JpegSaveOptions(int(Q), mode, int(bool(optimize_coding)), int(restart_interval))
     if in_ptr is None:
         frames = np.ascontiguousarray(frames)
         if frames.ndim == 3:
@@ -548,8 +561,8 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
         _SAVE_BUFFERS.clear()          # one staging array, reused: a fresh quarter gigabyte per call is all page faults
         out = _SAVE_BUFFERS[(n, stride)] = np.empty((n, stride), np.uint8)
     lens = (C.c_size_t * n)()
-    _check(lib().vb200_jpegsave_batch(src, where, w * bands, w * h * bands, n, w, h, bands, int(Q), mode, out.ctypes.data_as(C.c_void_p), HOST,
-                                      stride, lens))
+    _check(lib().vb200_jpegsave_batch_opts(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), out.ctypes.data_as(C.c_void_p),
+                                           HOST, stride, lens))
     return [out[i, :lens[i]].tobytes() for i in range(n)]
 
 

@@ -22,6 +22,12 @@
  *   (prefix sum)           bit offset of every block
  *   jpeg_emit_kernel       one thread per block: its bits OR-ed into the frame's bit buffer
  *   jpeg_stuff_kernel      FF -> FF00 and the markers around the scan: per 256-byte span count, prefix sum, copy
+ * With vips_jpegsave's options (vips2jpeg.c:590-597):
+ *   optimize_coding        jpeg_stats_kernel (symbol counts per frame) and jpeg_huffopt_kernel (jchuff.c
+ *                          jpeg_gen_optimal_table per table, the frame's code tables and header) after the FDCT; the count,
+ *                          emit and stuffing kernels then take the frame's tables and header
+ *   restart_interval       jpeg_intervals_kernel after the bit prefix sum: every interval starts on a byte boundary, the
+ *                          stuffing kernels put FF Dn before each interval after the first
  */
 #include <algorithm>
 #include <cstdlib>
@@ -92,12 +98,14 @@ scaled_quant(int quality, const unsigned char *base, unsigned short *out)
 	}
 }
 
-/* jchuff.c jpeg_make_c_derived_tbl: canonical codes from (bits, values) */
-void
+/* jchuff.c jpeg_make_c_derived_tbl: canonical codes from (bits, values); bits[l - 1] codes of length l */
+HD void
 derive_codes(const unsigned char bits[16], const unsigned char *vals, unsigned *co, unsigned char *si)
 {
-	memset(co, 0, 256 * sizeof(unsigned));
-	memset(si, 0, 256);
+	for (int i = 0; i < 256; i++) {
+		co[i] = 0;
+		si[i] = 0;
+	}
 	unsigned code = 0;
 	int k = 0;
 	for (int l = 1; l <= 16; l++) {
@@ -319,13 +327,15 @@ block_comp(const EncodeGeom &G, int bi)
 	return bi < 4 ? 0 : bi - 3;
 }
 
-/* Walk one block's symbols: emit(code, length) for every Huffman code and its extra bits; returns the bit count */
-template <typename Emit>
-HD unsigned
-code_block(const EncodeTables &T, const short *blk, int comp, int prev_dc, Emit emit)
+/* Walk one block's symbols in jchuff.c's order (encode_one_block, and htest_one_block for the statistics): sym(table,
+ * symbol) for every Huffman-coded symbol -- table 0 DC, 1 AC, 2 / 3 the same for chroma --, extra(value, n) for the n
+ * magnitude bits that follow it
+ */
+template <typename Sym, typename Extra>
+HD void
+walk_block(const unsigned char *zz, const short *blk, int comp, int prev_dc, Sym sym, Extra extra)
 {
 	const int dt = comp ? 2 : 0, at = dt + 1;
-	unsigned bits = 0;
 	int diff = blk[0] - prev_dc;
 	int t2 = diff;
 	if (diff < 0) {
@@ -333,22 +343,18 @@ code_block(const EncodeTables &T, const short *blk, int comp, int prev_dc, Emit 
 		t2--; /* one's complement of the magnitude for negative values (F.1.2.1) */
 	}
 	int nb = bit_size(diff);
-	emit(T.ehufco[dt][nb], T.ehufsi[dt][nb]);
-	bits += T.ehufsi[dt][nb];
-	if (nb) {
-		emit((unsigned) t2 & ((1u << nb) - 1), nb);
-		bits += nb;
-	}
+	sym(dt, nb);
+	if (nb)
+		extra((unsigned) t2 & ((1u << nb) - 1), nb);
 	int run = 0;
 	for (int k = 1; k < 64; k++) {
-		int v = blk[T.zz[k]];
+		int v = blk[zz[k]];
 		if (v == 0) {
 			run++;
 			continue;
 		}
 		while (run > 15) {
-			emit(T.ehufco[at][0xF0], T.ehufsi[at][0xF0]);
-			bits += T.ehufsi[at][0xF0];
+			sym(at, 0xF0);
 			run -= 16;
 		}
 		t2 = v;
@@ -357,33 +363,179 @@ code_block(const EncodeTables &T, const short *blk, int comp, int prev_dc, Emit 
 			t2--;
 		}
 		nb = bit_size(v);
-		const int sym = (run << 4) + nb;
-		emit(T.ehufco[at][sym], T.ehufsi[at][sym]);
-		emit((unsigned) t2 & ((1u << nb) - 1), nb);
-		bits += T.ehufsi[at][sym] + nb;
+		sym(at, (run << 4) + nb);
+		extra((unsigned) t2 & ((1u << nb) - 1), nb);
 		run = 0;
 	}
-	if (run > 0) {
-		emit(T.ehufco[at][0], T.ehufsi[at][0]);
-		bits += T.ehufsi[at][0];
-	}
+	if (run > 0)
+		sym(at, 0);
+}
+
+/* Code one block: emit(code, length) for every Huffman code and its extra bits, with the code / length tables co / si
+ * (the batch's standard tables, or a frame's optimised ones); returns the bit count
+ */
+template <typename Emit>
+HD unsigned
+code_block(const unsigned (*co)[256], const unsigned char (*si)[256], const unsigned char *zz, const short *blk, int comp, int prev_dc, Emit emit)
+{
+	unsigned bits = 0;
+	walk_block(
+		zz, blk, comp, prev_dc,
+		[&](int t, int s) {
+			emit(co[t][s], si[t][s]);
+			bits += si[t][s];
+		},
+		[&](unsigned v, int n) {
+			emit(v, n);
+			bits += n;
+		});
 	return bits;
 }
 
-/* the DC value the block's difference is taken against: the previous block of its component in scan order */
+/* The DC value the block's difference is taken against: the previous block of its component in scan order.  restart:
+ * MCUs per restart interval (0: none); the first block of each component in an MCU that starts an interval predicts
+ * from 0 (jchuff.c: emit_restart, and encode_mcu_gather in the statistics pass, reset last_dc_val)
+ */
 HD int
-previous_dc(const EncodeGeom &G, const short *coef, unsigned blk)
+previous_dc(const EncodeGeom &G, const short *coef, unsigned blk, int restart)
 {
 	const int nb = G.blocks_per_mcu;
 	const unsigned mcu = blk / (unsigned) nb;
 	const int bi = (int) (blk - mcu * (unsigned) nb);
 	if (G.ncomp == 3 && G.sub && bi >= 1 && bi <= 3)
 		return coef[(size_t) (blk - 1) * 64]; /* luma blocks 1..3 follow luma block bi - 1 */
-	if (mcu == 0)
+	if (mcu == 0 || (restart > 0 && mcu % (unsigned) restart == 0))
 		return 0;
 	/* the last block of the component in the previous MCU */
 	const int last = (G.ncomp == 3 && G.sub && bi == 0) ? 3 : bi;
 	return coef[((size_t) (mcu - 1) * nb + last) * 64];
+}
+
+/* ------------------------------------------------------------------ optimised Huffman tables (host + device) */
+
+constexpr unsigned kFreqSentinel = 1000000000u; /* jchuff.c jpeg_gen_optimal_table: v = 1000000000L */
+constexpr int kMaxCodeLen = 32;					/* MAX_CLEN: the longest code before the 16-bit limit */
+
+/* Huffman tables of one frame when it is coded with its own: code / length per symbol, tables as in EncodeTables */
+struct FrameHuff {
+	unsigned ehufco[4][256];
+	unsigned char ehufsi[4][256];
+};
+
+/* jchuff.c jpeg_gen_optimal_table, restated.  freq[257] holds the symbol counts and is consumed (freq[256], the reserved
+ * all-ones code, is set to 1 here); codesize / others [257] are scratch; bits[17] (bits[l]: codes of length l, bits[0]
+ * unused) and huffval[256] receive the table.
+ * pick(exclude) returns the LARGEST index i != exclude whose freq[i] is the smallest in (0, kFreqSentinel], or -1 (libjpeg
+ * scans upwards with freq[i] <= v, so a tie goes to the larger index): a serial scan on the host, a warp reduction on the
+ * device.  All other work runs on the lead thread; the other lanes take part in pick only.
+ * huffval is ordered by code size BEFORE the 16-bit limit, then by symbol, as libjpeg orders it: after the limit it need
+ * not be ordered by final length.  Returns -1 when a code would be longer than 32 bits (JERR_HUFF_CLEN_OVERFLOW).
+ */
+template <typename Pick>
+HD int
+gen_optimal_table(unsigned *freq, int *codesize, int *others, unsigned char *bits, unsigned char *huffval, bool lead, Pick pick)
+{
+	if (lead) {
+		for (int i = 0; i < 257; i++) {
+			codesize[i] = 0;
+			others[i] = -1;
+		}
+		freq[256] = 1;
+	}
+	for (;;) {
+		int c1 = pick(-1);
+		int c2 = pick(c1);
+		if (c2 < 0)
+			break;
+		if (lead) {
+			freq[c1] += freq[c2];
+			freq[c2] = 0;
+			codesize[c1]++;
+			while (others[c1] >= 0) {
+				c1 = others[c1];
+				codesize[c1]++;
+			}
+			others[c1] = c2;
+			codesize[c2]++;
+			while (others[c2] >= 0) {
+				c2 = others[c2];
+				codesize[c2]++;
+			}
+		}
+	}
+	if (!lead)
+		return 0;
+	unsigned char b[kMaxCodeLen + 1]; /* UINT8, as libjpeg counts them */
+	for (int i = 0; i <= kMaxCodeLen; i++)
+		b[i] = 0;
+	for (int i = 0; i <= 256; i++)
+		if (codesize[i]) {
+			if (codesize[i] > kMaxCodeLen)
+				return -1;
+			b[codesize[i]]++;
+		}
+	/* JPEG codes are at most 16 bits: move pairs of the longest codes up (T.81 Annex K.3 Figure K.3) */
+	for (int i = kMaxCodeLen; i > 16; i--)
+		while (b[i] > 0) {
+			int j = i - 2;
+			while (b[j] == 0)
+				j--;
+			b[i] -= 2;
+			b[i - 1]++;
+			b[j + 1] += 2;
+			b[j]--;
+		}
+	/* drop the reserved symbol's code: one of the longest */
+	int i = 16;
+	while (b[i] == 0)
+		i--;
+	b[i]--;
+	for (int l = 0; l <= 16; l++)
+		bits[l] = b[l];
+	/* symbols 0..255 by pre-limit code size, then by value: a counting sort of libjpeg's size-major double loop */
+	int start[kMaxCodeLen + 1];
+	for (int l = 0; l <= kMaxCodeLen; l++)
+		start[l] = 0;
+	for (int j = 0; j < 256; j++)
+		if (codesize[j])
+			start[codesize[j]]++;
+	for (int l = 1, p = 0; l <= kMaxCodeLen; l++) {
+		const int c = start[l];
+		start[l] = p;
+		p += c;
+	}
+	for (int j = 0; j < 256; j++)
+		if (codesize[j])
+			huffval[start[codesize[j]]++] = (unsigned char) j;
+	return 0;
+}
+
+/* the symbols a table holds: the sum of bits[1..16] */
+HD int
+table_values(const unsigned char *bits)
+{
+	int n = 0;
+	for (int l = 1; l <= 16; l++)
+		n += bits[l];
+	return n;
+}
+
+/* jcmarker.c emit_dht: table t (0 DC lum, 1 AC lum, 2 DC chr, 3 AC chr) with bits[1..16] / huffval; returns its bytes */
+HD int
+put_dht(unsigned char *o, int t, const unsigned char *bits, const unsigned char *huffval)
+{
+	const int nv = table_values(bits);
+	const int len = 19 + nv;
+	o[0] = 0xFF;
+	o[1] = 0xC4;
+	o[2] = (unsigned char) (len >> 8);
+	o[3] = (unsigned char) len;
+	o[4] = (unsigned char) (((t & 1) << 4) | (t >> 1));
+	for (int l = 1; l <= 16; l++)
+		o[4 + l] = bits[l];
+	for (int k = 0; k < nv; k++)
+		o[21 + k] = huffval[k];
+	return 2 + len;
 }
 
 /* ------------------------------------------------------------------ stream assembly (host) */
@@ -395,9 +547,9 @@ put16(std::vector<unsigned char> &o, unsigned v)
 	o.push_back((unsigned char) v);
 }
 
-/* everything up to and including SOS, in libjpeg's order: SOI, JFIF APP0, DQT per table, SOF0, DHT per table, SOS */
+/* the markers before the Huffman tables, in libjpeg's order: SOI, JFIF APP0, DQT per table, SOF0 */
 void
-write_headers(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned char> &o)
+header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned char> &o)
 {
 	o.clear();
 	put16(o, 0xFFD8);
@@ -423,15 +575,18 @@ write_headers(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned c
 		o.push_back((unsigned char) (c == 0 && G.sub && G.ncomp == 3 ? 0x22 : 0x11));
 		o.push_back((unsigned char) (c ? 1 : 0));
 	}
-	const unsigned char *bits[4] = {kBitsDcLum, kBitsAcLum, kBitsDcChr, kBitsAcChr};
-	const unsigned char *vals[4] = {kValDc, kValAcLum, kValDc, kValAcChr};
-	const int nvals[4] = {12, 162, 12, 162};
-	for (int t = 0; t < (G.ncomp == 1 ? 2 : 4); t++) {
-		put16(o, 0xFFC4);
-		put16(o, 19 + nvals[t]);
-		o.push_back((unsigned char) (((t & 1) << 4) | (t >> 1)));
-		o.insert(o.end(), bits[t], bits[t] + 16);
-		o.insert(o.end(), vals[t], vals[t] + nvals[t]);
+}
+
+/* the markers after the Huffman tables: DRI when there are restart intervals (jcmarker.c write_scan_header: after the
+ * DHTs, before SOS, also when the interval covers the whole frame), then SOS
+ */
+void
+header_suffix(const EncodeGeom &G, int restart, std::vector<unsigned char> &o)
+{
+	if (restart > 0) {
+		put16(o, 0xFFDD);
+		put16(o, 4);
+		put16(o, (unsigned) restart);
 	}
 	put16(o, 0xFFDA);
 	put16(o, 6 + 2 * G.ncomp);
@@ -443,6 +598,57 @@ write_headers(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned c
 	o.push_back(0);
 	o.push_back(63);
 	o.push_back(0);
+}
+
+/* one frame's DHT segments: tables 0..3 (0 and 1 only for greyscale), bits[t][1..16] / huffval[t] */
+void
+put_dhts(const EncodeGeom &G, const unsigned char (*bits)[17], const unsigned char (*huffval)[256], std::vector<unsigned char> &o)
+{
+	for (int t = 0; t < (G.ncomp == 1 ? 2 : 4); t++) {
+		unsigned char seg[4 + 17 + 256];
+		const int n = put_dht(seg, t, bits[t], huffval[t]);
+		o.insert(o.end(), seg, seg + n);
+	}
+}
+
+/* the standard tables (T.81 Annex K.3) in put_dhts' form */
+void
+standard_tables(unsigned char (*bits)[17], unsigned char (*huffval)[256])
+{
+	const unsigned char *b[4] = {kBitsDcLum, kBitsAcLum, kBitsDcChr, kBitsAcChr};
+	const unsigned char *v[4] = {kValDc, kValAcLum, kValDc, kValAcChr};
+	for (int t = 0; t < 4; t++) {
+		bits[t][0] = 0;
+		memcpy(bits[t] + 1, b[t], 16);
+		memcpy(huffval[t], v[t], (size_t) table_values(bits[t]));
+	}
+}
+
+/* everything up to and including SOS with the standard Huffman tables, in libjpeg's order: SOI, JFIF APP0, DQT per
+ * table, SOF0, DHT per table, DRI when restart > 0, SOS
+ */
+void
+write_headers(const EncodeGeom &G, const EncodeTables &T, int restart, std::vector<unsigned char> &o)
+{
+	unsigned char bits[4][17], huffval[4][256];
+	standard_tables(bits, huffval);
+	header_prefix(G, T, o);
+	put_dhts(G, bits, huffval, o);
+	header_suffix(G, restart, o);
+}
+
+/* restart_interval as vips_jpegsave takes it (jpegsave.c:284-289): 0 for none.  The reference passes larger values
+ * on to libjpeg, which writes DRI modulo 65536 but spaces the markers by the full value: a stream no reader can follow,
+ * so they are refused here.
+ */
+int
+check_restart(const char *domain, int restart)
+{
+	if (restart < 0 || restart > 65535) {
+		error(domain, "restart_interval %d outside 0..65535", restart);
+		return -1;
+	}
+	return 0;
 }
 
 int
@@ -474,6 +680,14 @@ make_geom(const char *domain, int w, int h, int bands, int quality, int subsampl
 
 constexpr int kStuffChunk = 256; /* bytes of raw scan per thread of the stuffing kernels */
 constexpr int kMaxBlockBytes = 208; /* 64 coefficients x (16-bit code + 10 bits): the bit buffer's bound per block */
+/* a table counts at most 64 symbols per block (a DC category, or 63 AC symbols + EOB), and frames are refused from
+ * 2^29 / kMaxBlockBytes blocks on: every count, and every sum of counts, stays below libjpeg's search sentinel
+ */
+static_assert(((1u << 29) / kMaxBlockBytes) * 64u + 1u < kFreqSentinel, "symbol counts must stay below the sentinel");
+/* a frame's header with its own tables: SOI + APP0 + 2 DQT + SOF0 (177 bytes for 3 components) + 4 DHT (84 bytes + at
+ * most 12 DC and 162 AC symbols per table pair) + DRI + SOS (20) = 629 bytes at most; a larger one fails the frame
+ */
+constexpr int kHeaderSlot = 640;
 
 /* one thread per MCU; blockIdx.y = frame */
 __global__ void __launch_bounds__(128)
@@ -495,16 +709,134 @@ jpeg_fdct_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const u
 		*(uint4 *) (dst + j) = *(const uint4 *) (local + j);
 }
 
-/* one thread per block: how many bits its code takes */
+/* the Huffman tables a block of frame f is coded with: the batch's standard ones, or the frame's own */
+template <bool kFrameHuff>
+__device__ __forceinline__ void
+frame_tables(const EncodeTables *T, const FrameHuff *huff, unsigned f, const unsigned (**co)[256], const unsigned char (**si)[256])
+{
+	if (kFrameHuff) {
+		*co = huff[f].ehufco;
+		*si = huff[f].ehufsi;
+	}
+	else {
+		*co = T->ehufco;
+		*si = T->ehufsi;
+	}
+}
+
+/* optimise_coding, pass 1 (jchuff.c encode_mcu_gather): one thread per block walks its symbols into the CTA's
+ * histograms (4 tables x 256 symbols; Cb and Cr share tables 2 / 3), then the non-zero bins are added to the frame's
+ * counts[frame][4][256]
+ */
 __global__ void __launch_bounds__(128)
-jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const short *__restrict__ coef, unsigned *__restrict__ bits)
+jpeg_stats_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const short *__restrict__ coef, int restart, unsigned *__restrict__ counts)
+{
+	__shared__ unsigned s_hist[4 * 256];
+	for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x)
+		s_hist[i] = 0;
+	__syncthreads();
+	const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
+	if (b < (unsigned) G.blocks) {
+		const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
+		walk_block(
+			T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)), previous_dc(G, fc, b, restart),
+			[&](int t, int s) { atomicAdd(&s_hist[t * 256 + s], 1u); }, [](unsigned, int) {});
+	}
+	__syncthreads();
+	unsigned *dst = counts + (size_t) blockIdx.y * 4 * 256;
+	for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x)
+		if (s_hist[i])
+			atomicAdd(dst + i, s_hist[i]);
+}
+
+/* optimise_coding, pass 2: one CTA per frame, one warp per table (tables 0, 1 for greyscale).  Each warp runs
+ * gen_optimal_table on its counts with a warp-wide minimum search, writes the frame's code / length table, and the CTA
+ * then writes the frame's header -- prefix (SOI .. SOF0), its own DHTs, suffix (DRI, SOS) -- into its kHeaderSlot-byte
+ * slot and the header's length into header_lens[frame].  A frame whose tables cannot be built sets *bad.
+ */
+__global__ void __launch_bounds__(128)
+jpeg_huffopt_kernel(int ntab, const unsigned *__restrict__ counts, FrameHuff *__restrict__ huff, const unsigned char *__restrict__ prefix,
+	unsigned prefix_len, const unsigned char *__restrict__ suffix, unsigned suffix_len, unsigned char *__restrict__ headers,
+	unsigned *__restrict__ header_lens, int *__restrict__ bad)
+{
+	__shared__ unsigned s_freq[4][257];
+	__shared__ int s_size[4][257], s_others[4][257];
+	__shared__ unsigned char s_bits[4][17], s_val[4][256];
+	__shared__ int s_fail;
+	const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const unsigned *cnt = counts + (size_t) blockIdx.x * 4 * 256;
+	if (threadIdx.x == 0)
+		s_fail = 0;
+	for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x)
+		s_freq[i >> 8][i & 255] = cnt[i];
+	__syncthreads();
+	FrameHuff *fh = huff + blockIdx.x;
+	if (w < ntab) {
+		unsigned *freq = s_freq[w];
+		auto pick = [&](int exclude) {
+			__syncwarp();
+			/* key: frequency, then the larger index first */
+			unsigned long long best = ~0ull;
+			for (int i = lane; i <= 256; i += 32) {
+				const unsigned f = freq[i];
+				if (f && f <= kFreqSentinel && i != exclude) {
+					const unsigned long long key = ((unsigned long long) f << 9) | (unsigned) (511 - i);
+					best = key < best ? key : best;
+				}
+			}
+			for (int o = 16; o; o >>= 1) {
+				const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
+				best = v < best ? v : best;
+			}
+			return best == ~0ull ? -1 : 511 - (int) (best & 511u);
+		};
+		if (gen_optimal_table(freq, s_size[w], s_others[w], s_bits[w], s_val[w], lane == 0, pick))
+			s_fail = 1;
+		__syncwarp();
+		if (lane == 0)
+			derive_codes(s_bits[w] + 1, s_val[w], fh->ehufco[w], fh->ehufsi[w]);
+	}
+	__syncthreads();
+	unsigned len = prefix_len + suffix_len;
+	for (int t = 0; t < ntab; t++)
+		len += 21 + table_values(s_bits[t]);
+	if (s_fail || len > kHeaderSlot) {
+		if (threadIdx.x == 0) {
+			header_lens[blockIdx.x] = 0;
+			atomicExch(bad, 1);
+		}
+		return;
+	}
+	unsigned char *o = headers + (size_t) blockIdx.x * kHeaderSlot;
+	for (unsigned i = threadIdx.x; i < prefix_len; i += blockDim.x)
+		o[i] = prefix[i];
+	for (unsigned i = threadIdx.x; i < suffix_len; i += blockDim.x)
+		o[len - suffix_len + i] = suffix[i];
+	if (w < ntab && lane == 0) {
+		unsigned at = prefix_len;
+		for (int t = 0; t < w; t++)
+			at += 21 + table_values(s_bits[t]);
+		put_dht(o + at, w, s_bits[w], s_val[w]);
+	}
+	if (threadIdx.x == 0)
+		header_lens[blockIdx.x] = len;
+}
+
+/* one thread per block: how many bits its code takes */
+template <bool kFrameHuff, bool kRestart>
+__global__ void __launch_bounds__(128)
+jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const FrameHuff *__restrict__ huff, int restart,
+	const short *__restrict__ coef, unsigned *__restrict__ bits)
 {
 	const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
 	if (b >= (unsigned) G.blocks)
 		return;
 	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
-	bits[(size_t) blockIdx.y * G.blocks + b] = code_block(*T, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)),
-		previous_dc(G, fc, b), [](unsigned, int) {});
+	const unsigned (*co)[256];
+	const unsigned char (*si)[256];
+	frame_tables<kFrameHuff>(T, huff, blockIdx.y, &co, &si);
+	bits[(size_t) blockIdx.y * G.blocks + b] = code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)),
+		previous_dc(G, fc, b, kRestart ? restart : 0), [](unsigned, int) {});
 }
 
 /* exclusive prefix sum of a frame's per-block bit counts (in place), total into totals[frame]: one CTA per frame */
@@ -536,19 +868,84 @@ jpeg_bitscan_kernel(int blocks, unsigned *__restrict__ bits, unsigned long long 
 		totals[blockIdx.x] = s_part[threadIdx.x];
 }
 
-/* one thread per block: its bits into the frame's (zeroed) raw bit buffer, whole bytes OR-ed in (neighbouring blocks share
- * their boundary bytes); the thread that ends the frame also pads the last byte with 1-bits
+/* restart intervals, one CTA per frame: each interval takes its blocks' bits rounded up to a whole byte (the 1-padding
+ * before each RSTn), istart[frame][k] = the byte where interval k starts in the raw scan (an exclusive prefix sum over
+ * intervals), and totals[frame] becomes the padded scan's length in bits (whole bytes)
  */
+__global__ void __launch_bounds__(1024)
+jpeg_intervals_kernel(int blocks, int blocks_per_interval, int nint, const unsigned *__restrict__ offs, unsigned long long *__restrict__ totals,
+	unsigned *__restrict__ istart)
+{
+	__shared__ unsigned long long s_part[1024];
+	const unsigned *o = offs + (size_t) blockIdx.x * blocks;
+	unsigned *st = istart + (size_t) blockIdx.x * nint;
+	const unsigned long long total = totals[blockIdx.x];
+	auto ibytes = [&](unsigned k) {
+		const unsigned long long b0 = o[(size_t) k * blocks_per_interval];
+		const unsigned long long b1 = k + 1 < (unsigned) nint ? o[(size_t) (k + 1) * blocks_per_interval] : total;
+		return (b1 - b0 + 7) >> 3;
+	};
+	const unsigned per = ((unsigned) nint + blockDim.x - 1) / blockDim.x;
+	const unsigned a = min((unsigned) nint, threadIdx.x * per), e = min((unsigned) nint, a + per);
+	unsigned long long sum = 0;
+	for (unsigned k = a; k < e; k++)
+		sum += ibytes(k);
+	s_part[threadIdx.x] = sum;
+	__syncthreads();
+	for (unsigned d = 1; d < blockDim.x; d <<= 1) {
+		const unsigned long long v = threadIdx.x >= d ? s_part[threadIdx.x - d] : 0;
+		__syncthreads();
+		s_part[threadIdx.x] += v;
+		__syncthreads();
+	}
+	unsigned long long run = s_part[threadIdx.x] - sum;
+	for (unsigned k = a; k < e; k++) {
+		st[k] = (unsigned) run;
+		run += ibytes(k);
+	}
+	if (threadIdx.x == blockDim.x - 1)
+		totals[blockIdx.x] = s_part[threadIdx.x] * 8;
+}
+
+/* the number of the n ascending values p[] below v */
+__device__ __forceinline__ int
+count_below(const unsigned *p, int n, unsigned long long v)
+{
+	int lo = 0, hi = n;
+	while (lo < hi) {
+		const int mid = (lo + hi) >> 1;
+		if (p[mid] < v)
+			lo = mid + 1;
+		else
+			hi = mid;
+	}
+	return lo;
+}
+
+/* one thread per block: its bits into the frame's (zeroed) raw bit buffer, whole bytes OR-ed in (neighbouring blocks share
+ * their boundary bytes); the thread that ends the frame -- with restart intervals, each interval -- also pads the last
+ * byte with 1-bits.  With restart intervals a block's bit offset is relative to its interval, which starts at byte
+ * istart[frame][k].
+ */
+template <bool kFrameHuff, bool kRestart>
 __global__ void __launch_bounds__(128)
-jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const short *__restrict__ coef, const unsigned *__restrict__ offs,
-	const unsigned long long *__restrict__ totals, unsigned *__restrict__ raw, size_t raw_words)
+jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const FrameHuff *__restrict__ huff, int restart, int nint,
+	const unsigned *__restrict__ istart, const short *__restrict__ coef, const unsigned *__restrict__ offs, unsigned *__restrict__ raw,
+	size_t raw_words)
 {
 	const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
 	if (b >= (unsigned) G.blocks)
 		return;
 	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
 	unsigned *out = raw + (size_t) blockIdx.y * raw_words;
-	unsigned pos = offs[(size_t) blockIdx.y * G.blocks + b]; /* bit index */
+	const unsigned *fo = offs + (size_t) blockIdx.y * G.blocks;
+	unsigned pos = fo[b]; /* bit index */
+	bool last = b == (unsigned) G.blocks - 1;
+	if (kRestart) {
+		const unsigned bpm = (unsigned) G.blocks_per_mcu, mcu = b / bpm, k = mcu / (unsigned) restart;
+		pos += istart[(size_t) blockIdx.y * nint + k] * 8 - fo[k * (unsigned) restart * bpm];
+		last = last || (b - mcu * bpm == bpm - 1 && (mcu + 1) % (unsigned) restart == 0);
+	}
 	unsigned long long acc = 0;
 	int nacc = (int) (pos & 7u); /* the bits of the first byte that belong to the block before: zeros here, OR-ed there */
 	unsigned byte = pos >> 3;
@@ -563,21 +960,27 @@ jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const s
 			nacc -= 8;
 		}
 	};
-	code_block(*T, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)), previous_dc(G, fc, b), put);
+	const unsigned (*co)[256];
+	const unsigned char (*si)[256];
+	frame_tables<kFrameHuff>(T, huff, blockIdx.y, &co, &si);
+	code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)), previous_dc(G, fc, b, kRestart ? restart : 0),
+		put);
 	if (nacc > 0) {
 		unsigned v = (unsigned) (acc << (8 - nacc)) & 0xffu;
-		if (b == (unsigned) G.blocks - 1)
+		if (last)
 			v |= (1u << (8 - nacc)) - 1; /* jchuff.c flush_bits: pad the last byte with ones */
 		if (v)
 			atomicOr(out + (byte >> 2), v << (8 * (byte & 3u)));
 	}
-	(void) totals;
 }
 
-/* stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw scan */
+/* stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw scan; with restart intervals, plus 2 bytes
+ * for every RSTn marker that goes before a byte of the span (interval starts 1 .. nint - 1)
+ */
+template <bool kRestart>
 __global__ void __launch_bounds__(128)
 jpeg_ffcount_kernel(const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw, size_t raw_bytes, int max_chunks,
-	unsigned *__restrict__ counts)
+	int nint, const unsigned *__restrict__ istart, unsigned *__restrict__ counts)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	if (c >= max_chunks)
@@ -588,14 +991,23 @@ jpeg_ffcount_kernel(const unsigned long long *__restrict__ totals, const unsigne
 	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
 	for (unsigned long long i = a; i < e; i++)
 		n += p[i] == 0xFF;
+	if (kRestart && a < e) {
+		const unsigned *st = istart + (size_t) blockIdx.y * nint + 1;
+		n += 2 * (unsigned) (count_below(st, nint - 1, e) - count_below(st, nint - 1, a));
+	}
 	counts[(size_t) blockIdx.y * max_chunks + c] = n;
 }
 
-/* stuffing, pass 2: prefix sum of the spans' counts, one CTA per frame; lengths[frame] = header + scan + stuffed zeros + EOI */
+/* stuffing, pass 2: prefix sum of the spans' counts, one CTA per frame; lengths[frame] = header + scan + stuffed zeros +
+ * markers + EOI.  The header is the batch's (header_len) or, with optimised tables, the frame's (header_lens[frame]).
+ */
+template <bool kFrameHeader>
 __global__ void __launch_bounds__(1024)
 jpeg_ffscan_kernel(const unsigned long long *__restrict__ totals, int max_chunks, unsigned *__restrict__ counts, unsigned header_len,
-	unsigned long long *__restrict__ lengths)
+	const unsigned *__restrict__ header_lens, unsigned long long *__restrict__ lengths)
 {
+	if (kFrameHeader)
+		header_len = header_lens[blockIdx.x];
 	__shared__ unsigned s_part[1024];
 	unsigned *cnt = counts + (size_t) blockIdx.x * max_chunks;
 	const unsigned per = ((unsigned) max_chunks + blockDim.x - 1) / blockDim.x;
@@ -622,18 +1034,25 @@ jpeg_ffscan_kernel(const unsigned long long *__restrict__ totals, int max_chunks
 }
 
 /* stuffing, pass 3: header, stuffed scan, EOI into the caller's stream (a stream that does not fit is cut: the host
- * compares lengths[frame] with the stride and reports it)
+ * compares lengths[frame] with the stride and reports it).  With optimised tables the header is the frame's slot of
+ * kHeaderSlot bytes; with restart intervals FF D0+((k - 1) & 7) goes before the first byte of interval k >= 1 (padding
+ * bytes are stuffed, markers are not).
  */
+template <bool kFrameHeader, bool kRestart>
 __global__ void __launch_bounds__(128)
 jpeg_stuff_kernel(const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw, size_t raw_bytes, int max_chunks,
-	const unsigned *__restrict__ counts, const unsigned char *__restrict__ header, unsigned header_len, unsigned char *__restrict__ out,
-	size_t out_stride, const unsigned long long *__restrict__ lengths)
+	const unsigned *__restrict__ counts, const unsigned char *__restrict__ header, unsigned header_len, const unsigned *__restrict__ header_lens,
+	int nint, const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride, const unsigned long long *__restrict__ lengths)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	unsigned char *o = out + (size_t) blockIdx.y * out_stride;
 	const unsigned long long len = lengths[blockIdx.y];
 	if (len > out_stride)
 		return;
+	if (kFrameHeader) {
+		header += (size_t) blockIdx.y * kHeaderSlot;
+		header_len = header_lens[blockIdx.y];
+	}
 	if (c < (int) ((header_len + kStuffChunk - 1) / kStuffChunk)) {
 		/* the first spans' threads also copy the header */
 		for (unsigned i = (unsigned) c * kStuffChunk; i < min(header_len, (unsigned) (c + 1) * kStuffChunk); i++)
@@ -645,8 +1064,15 @@ jpeg_stuff_kernel(const unsigned long long *__restrict__ totals, const unsigned 
 	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
 	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
 	unsigned char *d = o + header_len + a + counts[(size_t) blockIdx.y * max_chunks + c];
+	const unsigned *st = istart + (size_t) blockIdx.y * nint;
+	int k = kRestart && a < e ? 1 + count_below(st + 1, nint - 1, a) : 0; /* the next interval starting in the span */
 	for (unsigned long long i = a; i < e; i++) {
 		const unsigned char v = p[i];
+		if (kRestart && k < nint && st[k] == i) {
+			*d++ = 0xFF;
+			*d++ = (unsigned char) (0xD0 + ((k - 1) & 7));
+			k++;
+		}
 		*d++ = v;
 		if (v == 0xFF)
 			*d++ = 0;
@@ -657,29 +1083,106 @@ jpeg_stuff_kernel(const unsigned long long *__restrict__ totals, const unsigned 
 	}
 }
 
+/* the device buffers of one chunk of frames */
+struct ChunkArgs {
+	EncodeGeom G;
+	const EncodeTables *T;
+	const unsigned char *frames;
+	size_t bpl, frame_stride;
+	int cn, restart, nint, max_chunks;
+	short *coef;
+	unsigned *bits, *counts, *istart, *freq, *header_lens;
+	unsigned long long *totals, *lengths;
+	unsigned char *raw;
+	size_t raw_bytes;
+	FrameHuff *huff;
+	const unsigned char *header; /* the batch's header, or with optimised tables the prefix and suffix around the DHTs */
+	unsigned header_len, prefix_len, suffix_len;
+	unsigned char *headers; /* per-frame header slots */
+	int *bad;
+	unsigned char *out;
+	size_t out_stride;
+};
+
+/* the kernels of one chunk: 7 launches with the standard tables and no restart intervals, +1 with restart intervals
+ * (jpeg_intervals_kernel), +2 with optimised tables (jpeg_stats_kernel, jpeg_huffopt_kernel); returns the launch count,
+ * -1 when the counts could not be cleared
+ */
+template <bool kOpt, bool kRestart>
+int
+launch_chunk(const ChunkArgs &A, cudaStream_t s)
+{
+	const EncodeGeom &G = A.G;
+	const int mcus = G.mcus_x * G.mcus_y, cn = A.cn;
+	const dim3 per_block((G.blocks + 127) / 128, cn), per_span((A.max_chunks + 127) / 128, cn);
+	int launches = 7;
+	jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, A.T, A.frames, A.bpl, A.frame_stride, A.coef);
+	if (kOpt) {
+		if (cudaMemsetAsync(A.freq, 0, (size_t) cn * 4 * 256 * sizeof(unsigned), s) != cudaSuccess)
+			return -1;
+		jpeg_stats_kernel<<<per_block, 128, 0, s>>>(G, A.T, A.coef, A.restart, A.freq);
+		jpeg_huffopt_kernel<<<cn, 128, 0, s>>>(G.ncomp == 1 ? 2 : 4, A.freq, A.huff, A.header, A.prefix_len, A.header + A.prefix_len, A.suffix_len,
+			A.headers, A.header_lens, A.bad);
+		launches += 2;
+	}
+	jpeg_count_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, A.huff, A.restart, A.coef, A.bits);
+	jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(G.blocks, A.bits, A.totals);
+	if (kRestart) {
+		jpeg_intervals_kernel<<<cn, 1024, 0, s>>>(G.blocks, A.restart * G.blocks_per_mcu, A.nint, A.bits, A.totals, A.istart);
+		launches++;
+	}
+	jpeg_emit_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, A.huff, A.restart, A.nint, A.istart, A.coef, A.bits, (unsigned *) A.raw,
+		A.raw_bytes / 4);
+	jpeg_ffcount_kernel<kRestart><<<per_span, 128, 0, s>>>(A.totals, A.raw, A.raw_bytes, A.max_chunks, A.nint, A.istart, A.counts);
+	jpeg_ffscan_kernel<kOpt><<<cn, 1024, 0, s>>>(A.totals, A.max_chunks, A.counts, A.header_len, A.header_lens, A.lengths);
+	jpeg_stuff_kernel<kOpt, kRestart><<<per_span, 128, 0, s>>>(A.totals, A.raw, A.raw_bytes, A.max_chunks, A.counts, kOpt ? A.headers : A.header,
+		A.header_len, A.header_lens, A.nint, A.istart, A.out, A.out_stride, A.lengths);
+	return launches;
+}
+
 } // namespace
 
 /* n equally sized 8-bit frames (1 or 3 bands) on the device -> n JPEG streams at out + i * out_stride (device), their
- * lengths to lengths_host[n].  Stream-ordered on s; returns after the lengths are known.
+ * lengths to lengths_host[n].  optimize: per-frame Huffman tables from the frame's symbol counts; restart: MCUs per
+ * restart interval (0: none).  Stream-ordered on s; returns after the lengths are known.
  */
 int
 dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, int quality,
-	int subsample_mode, void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
+	int subsample_mode, int optimize, int restart, void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
 {
 	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G))
+	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
 		return -1;
-	if ((size_t) G.blocks * kMaxBlockBytes >= (size_t) 1 << 29) {
+	const int mcus = G.mcus_x * G.mcus_y;
+	const int nint = restart ? (mcus + restart - 1) / restart : 1;
+	/* every interval may end with one byte of padding */
+	const size_t scan_bound = (size_t) G.blocks * kMaxBlockBytes + (restart ? (size_t) nint : 0);
+	if (scan_bound >= (size_t) 1 << 29) {
 		error(domain, "frame too large for the device encoder");
 		return -1;
 	}
 	EncodeTables T;
 	make_tables(quality, &T);
-	std::vector<unsigned char> header;
-	write_headers(G, T, header);
-	const size_t raw_bytes = (((size_t) G.blocks * kMaxBlockBytes + 3) & ~(size_t) 3) + 4;
+	/* standard tables: the whole header; optimised tables: the markers before and after the DHTs (prefix_len bytes, then
+	 * the suffix), which jpeg_huffopt_kernel puts around each frame's own tables
+	 */
+	std::vector<unsigned char> header, suffix;
+	unsigned prefix_len = 0;
+	if (optimize) {
+		header_prefix(G, T, header);
+		prefix_len = (unsigned) header.size();
+		header_suffix(G, restart, suffix);
+		header.insert(header.end(), suffix.begin(), suffix.end());
+	}
+	else
+		write_headers(G, T, restart, header);
+	const size_t raw_bytes = ((scan_bound + 3) & ~(size_t) 3) + 4;
 	const int max_chunks = (int) ((raw_bytes + kStuffChunk - 1) / kStuffChunk);
-	/* one block of device scratch: tables | header | coefficients | bit counts / offsets | totals | lengths | raw | span counts */
+	/* per-frame tables and header slots (about 10 KB a frame) for one chunk of frames, reused by the next */
+	const size_t nopt = optimize ? (size_t) std::min(n, kMaxBatchFrames) : 0;
+	/* one block of device scratch: tables | header | coefficients | bit counts / offsets | totals | lengths | raw | span counts
+	 * | interval starts | symbol counts | frame tables | header slots | header lengths | failure flag
+	 */
 	size_t off = 0;
 	auto take = [&](size_t bytes) {
 		const size_t o = off;
@@ -689,7 +1192,9 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 	const size_t o_tab = take(sizeof(T)), o_hdr = take(header.size()), o_coef = take((size_t) n * G.blocks * 64 * sizeof(short)),
 				 o_bits = take((size_t) n * G.blocks * sizeof(unsigned)), o_tot = take((size_t) n * sizeof(unsigned long long)),
 				 o_len = take((size_t) n * sizeof(unsigned long long)), o_raw = take((size_t) n * raw_bytes),
-				 o_cnt = take((size_t) n * max_chunks * sizeof(unsigned));
+				 o_cnt = take((size_t) n * max_chunks * sizeof(unsigned)), o_ist = take(restart ? (size_t) n * nint * sizeof(unsigned) : 0),
+				 o_freq = take(nopt * 4 * 256 * sizeof(unsigned)), o_huff = take(nopt * sizeof(FrameHuff)), o_slots = take(nopt * kHeaderSlot),
+				 o_hlen = take(nopt * sizeof(unsigned)), o_bad = take(sizeof(int));
 	char *scratch = nullptr;
 	if (dev_alloc(domain, (void **) &scratch, off, s))
 		return -1;
@@ -698,38 +1203,51 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 		/* tables and header from pageable memory: small, staged by the driver before the call returns */
 		if (cudaMemcpyAsync(scratch + o_tab, &T, sizeof(T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
 			cudaMemcpyAsync(scratch + o_hdr, header.data(), header.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-			cudaMemsetAsync(scratch + o_raw, 0, (size_t) n * raw_bytes, s) != cudaSuccess) {
+			cudaMemsetAsync(scratch + o_raw, 0, (size_t) n * raw_bytes, s) != cudaSuccess ||
+			cudaMemsetAsync(scratch + o_bad, 0, sizeof(int), s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode setup");
 			break;
 		}
-		const EncodeTables *dT = (const EncodeTables *) (scratch + o_tab);
-		short *coef = (short *) (scratch + o_coef);
-		unsigned *bits = (unsigned *) (scratch + o_bits);
-		unsigned long long *totals = (unsigned long long *) (scratch + o_tot), *lengths = (unsigned long long *) (scratch + o_len);
-		unsigned *counts = (unsigned *) (scratch + o_cnt);
-		const int mcus = G.mcus_x * G.mcus_y;
+		ChunkArgs A;
+		A.G = G;
+		A.T = (const EncodeTables *) (scratch + o_tab);
+		A.bpl = bpl;
+		A.frame_stride = frame_stride;
+		A.restart = restart;
+		A.nint = nint;
+		A.max_chunks = max_chunks;
+		A.raw_bytes = raw_bytes;
+		A.freq = (unsigned *) (scratch + o_freq);
+		A.huff = (FrameHuff *) (scratch + o_huff);
+		A.header = (const unsigned char *) (scratch + o_hdr);
+		A.header_len = (unsigned) header.size();
+		A.prefix_len = prefix_len;
+		A.suffix_len = (unsigned) suffix.size();
+		A.headers = (unsigned char *) (scratch + o_slots);
+		A.header_lens = (unsigned *) (scratch + o_hlen);
+		A.bad = (int *) (scratch + o_bad);
+		A.out_stride = out_stride;
+		unsigned long long *lengths = (unsigned long long *) (scratch + o_len);
 		/* the frame is gridDim.y (or x) of every kernel: chunks of at most kMaxBatchFrames, each on its slice of the scratch */
 		cudaError_t e = cudaSuccess;
 		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
-			const int cn = std::min(kMaxBatchFrames, n - c0);
-			short *ccoef = coef + (size_t) c0 * G.blocks * 64;
-			unsigned *cbits = bits + (size_t) c0 * G.blocks;
-			unsigned long long *ctotals = totals + c0, *clengths = lengths + c0;
-			unsigned char *craw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
-			unsigned *ccounts = counts + (size_t) c0 * max_chunks;
-			jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, dT, (const unsigned char *) frames + (size_t) c0 * frame_stride, bpl,
-				frame_stride, ccoef);
-			jpeg_count_kernel<<<dim3((G.blocks + 127) / 128, cn), 128, 0, s>>>(G, dT, ccoef, cbits);
-			jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(G.blocks, cbits, ctotals);
-			jpeg_emit_kernel<<<dim3((G.blocks + 127) / 128, cn), 128, 0, s>>>(G, dT, ccoef, cbits, ctotals, (unsigned *) craw, raw_bytes / 4);
-			jpeg_ffcount_kernel<<<dim3((max_chunks + 127) / 128, cn), 128, 0, s>>>(ctotals, craw, raw_bytes, max_chunks, ccounts);
-			jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(ctotals, max_chunks, ccounts, (unsigned) header.size(), clengths);
-			jpeg_stuff_kernel<<<dim3((max_chunks + 127) / 128, cn), 128, 0, s>>>(ctotals, craw, raw_bytes, max_chunks, ccounts,
-				(const unsigned char *) (scratch + o_hdr), (unsigned) header.size(), (unsigned char *) out + (size_t) c0 * out_stride, out_stride,
-				clengths);
+			A.cn = std::min(kMaxBatchFrames, n - c0);
+			A.frames = (const unsigned char *) frames + (size_t) c0 * frame_stride;
+			A.coef = (short *) (scratch + o_coef) + (size_t) c0 * G.blocks * 64;
+			A.bits = (unsigned *) (scratch + o_bits) + (size_t) c0 * G.blocks;
+			A.totals = (unsigned long long *) (scratch + o_tot) + c0;
+			A.lengths = lengths + c0;
+			A.raw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
+			A.counts = (unsigned *) (scratch + o_cnt) + (size_t) c0 * max_chunks;
+			A.istart = (unsigned *) (scratch + o_ist) + (size_t) c0 * nint;
+			A.out = (unsigned char *) out + (size_t) c0 * out_stride;
+			const int launches = optimize ? (restart ? launch_chunk<true, true>(A, s) : launch_chunk<true, false>(A, s))
+										  : (restart ? launch_chunk<false, true>(A, s) : launch_chunk<false, false>(A, s));
 			e = cudaGetLastError();
+			if (e == cudaSuccess && launches < 0)
+				e = cudaErrorUnknown;
 			if (e == cudaSuccess)
-				for (int k = 0; k < 7; k++)
+				for (int k = 0; k < launches; k++)
 					count_launch();
 		}
 		if (e != cudaSuccess) {
@@ -737,9 +1255,15 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 			break;
 		}
 		std::vector<unsigned long long> len(n);
+		int bad = 0;
 		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-			cudaStreamSynchronize(s) != cudaSuccess) {
+			cudaMemcpyAsync(&bad, scratch + o_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode");
+			break;
+		}
+		if (bad) {
+			/* libjpeg's JERR_HUFF_CLEN_OVERFLOW: a symbol distribution no image of the sizes taken here produces */
+			error(domain, "optimised Huffman table: a code longer than 32 bits");
 			break;
 		}
 		rc = 0;
@@ -756,13 +1280,33 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 	return rc;
 }
 
-/* the whole encoder on the CPU through the same per-block code: test hook */
+/* jpeg_gen_optimal_table on the host (libjpeg's own serial minimum search), for the host twin and its test hook */
 int
-host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
-	std::vector<unsigned char> &out)
+host_optimal_table(unsigned *freq, unsigned char *bits, unsigned char *huffval)
+{
+	int codesize[257], others[257];
+	auto pick = [&](int exclude) {
+		int c = -1;
+		unsigned v = kFreqSentinel;
+		for (int i = 0; i <= 256; i++)
+			if (freq[i] && freq[i] <= v && i != exclude) {
+				v = freq[i];
+				c = i;
+			}
+		return c;
+	};
+	return gen_optimal_table(freq, codesize, others, bits, huffval, true, pick);
+}
+
+/* the whole encoder on the CPU through the same per-block code, in the order libjpeg runs it: statistics and table
+ * generation when optimising, then the scan with its restart markers (test hook)
+ */
+int
+host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode, int optimize,
+	int restart, std::vector<unsigned char> &out)
 {
 	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G))
+	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
 		return -1;
 	EncodeTables T;
 	make_tables(quality, &T);
@@ -770,7 +1314,32 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
 	for (int my = 0; my < G.mcus_y; my++)
 		for (int mx = 0; mx < G.mcus_x; mx++)
 			encode_mcu(G, T.q, img, bpl, mx, my, coef.data() + ((size_t) my * G.mcus_x + mx) * G.blocks_per_mcu * 64);
-	write_headers(G, T, out);
+	const unsigned bpm = (unsigned) G.blocks_per_mcu;
+	unsigned char bits[4][17], huffval[4][256];
+	FrameHuff fh;
+	const unsigned (*co)[256] = T.ehufco;
+	const unsigned char (*si)[256] = T.ehufsi;
+	if (optimize) {
+		std::vector<unsigned> freq(4 * 257, 0);
+		for (unsigned b = 0; b < (unsigned) G.blocks; b++)
+			walk_block(
+				T.zz, coef.data() + (size_t) b * 64, block_comp(G, (int) (b % bpm)), previous_dc(G, coef.data(), b, restart),
+				[&](int t, int s) { freq[t * 257 + s]++; }, [](unsigned, int) {});
+		for (int t = 0; t < (G.ncomp == 1 ? 2 : 4); t++) {
+			if (host_optimal_table(freq.data() + t * 257, bits[t], huffval[t])) {
+				error(domain, "optimised Huffman table: a code longer than 32 bits");
+				return -1;
+			}
+			derive_codes(bits[t] + 1, huffval[t], fh.ehufco[t], fh.ehufsi[t]);
+		}
+		co = fh.ehufco;
+		si = fh.ehufsi;
+	}
+	else
+		standard_tables(bits, huffval);
+	header_prefix(G, T, out);
+	put_dhts(G, bits, huffval, out);
+	header_suffix(G, restart, out);
 	unsigned long long acc = 0;
 	int nacc = 0;
 	auto flush_byte = [&](unsigned char b) {
@@ -786,10 +1355,23 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
 			nacc -= 8;
 		}
 	};
-	for (unsigned b = 0; b < (unsigned) G.blocks; b++)
-		code_block(T, coef.data() + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)), previous_dc(G, coef.data(), b), emit);
-	if (nacc > 0)
-		flush_byte((unsigned char) (((acc << (8 - nacc)) | ((1u << (8 - nacc)) - 1)) & 0xFF));
+	/* jchuff.c flush_bits: the partial byte padded with 1-bits (and stuffed) */
+	auto pad = [&]() {
+		if (nacc > 0)
+			flush_byte((unsigned char) (((acc << (8 - nacc)) | ((1u << (8 - nacc)) - 1)) & 0xFF));
+		nacc = 0;
+	};
+	for (unsigned b = 0; b < (unsigned) G.blocks; b++) {
+		const unsigned mcu = b / bpm;
+		if (restart > 0 && b % bpm == 0 && mcu > 0 && mcu % (unsigned) restart == 0) {
+			/* jchuff.c emit_restart: before MCU k * restart, RST((k - 1) mod 8), not stuffed */
+			pad();
+			out.push_back(0xFF);
+			out.push_back((unsigned char) (0xD0 + ((mcu / (unsigned) restart - 1) & 7)));
+		}
+		code_block(co, si, T.zz, coef.data() + (size_t) b * 64, block_comp(G, (int) (b % bpm)), previous_dc(G, coef.data(), b, restart), emit);
+	}
+	pad();
 	put16(out, 0xFFD9);
 	return 0;
 }
@@ -806,8 +1388,22 @@ extern "C" int
 vb200_debug_jpeg_encode(const void *pixels, size_t bpl, int width, int height, int bands, int quality, int subsample_mode, void *out, size_t cap,
 	size_t *len)
 {
+	const VB200JpegSaveOptions opt = {quality, subsample_mode, 0, 0};
+	return vb200_debug_jpeg_encode_opts(pixels, bpl, width, height, bands, &opt, out, cap, len);
+}
+
+/* Test hook, host only: vb200_debug_jpeg_encode with every option of VB200JpegSaveOptions */
+extern "C" int
+vb200_debug_jpeg_encode_opts(const void *pixels, size_t bpl, int width, int height, int bands, const VB200JpegSaveOptions *opt, void *out, size_t cap,
+	size_t *len)
+{
+	if (!opt) {
+		error("jpeg_encode (host twin)", "null options");
+		return -1;
+	}
 	std::vector<unsigned char> o;
-	if (host_jpeg_encode("jpeg_encode (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, quality, subsample_mode, o))
+	if (host_jpeg_encode("jpeg_encode (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, opt->Q, opt->subsample_mode,
+			opt->optimize_coding, opt->restart_interval, o))
 		return -1;
 	if (len)
 		*len = o.size();
@@ -819,20 +1415,57 @@ vb200_debug_jpeg_encode(const void *pixels, size_t bpl, int width, int height, i
 	return 0;
 }
 
+/* Test hook, host only: jpeg_gen_optimal_table (jchuff.c) on the symbol counts freq[256] -> bits[17] (bits[0] unused),
+ * huffval[256] (sum of bits[1..16] entries used).  -1 when the counts add up to 10^9 or more (the frames the encoder takes
+ * stay far below) or a code would be longer than 32 bits.
+ */
+extern "C" int
+vb200_debug_jpeg_optimal_table(const unsigned *freq, unsigned char *bits, unsigned char *huffval)
+{
+	unsigned f[257];
+	unsigned long long total = 0;
+	for (int i = 0; i < 256; i++)
+		total += f[i] = freq[i];
+	if (total + 1 >= kFreqSentinel) {
+		error("jpeg_optimal_table", "symbol counts add up to %llu, the table generator takes less than %u", total, kFreqSentinel - 1);
+		return -1;
+	}
+	if (host_optimal_table(f, bits, huffval)) {
+		error("jpeg_optimal_table", "a code longer than 32 bits");
+		return -1;
+	}
+	return 0;
+}
+
 /* vips_jpegsave_buffer (foreign/vips2jpeg.c) for a batch of equally sized 8-bit frames (1 or 3 bands), on the device:
  * frames in host or device memory (frames_location), n streams to out + i * out_stride in host or device memory
  * (out_location), lengths[n] on the host.  Q and subsample_mode as the reference's arguments (0 auto, 1 on, 2 off);
- * everything else is the reference's default (baseline, standard Huffman tables, JFIF header).
+ * everything else is the reference's default (baseline, standard Huffman tables, no restart markers, JFIF header).
  */
 extern "C" int
 vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands, int Q,
 	int subsample_mode, void *out, int out_location, size_t out_stride, size_t *lengths)
 {
+	const VB200JpegSaveOptions opt = {Q, subsample_mode, 0, 0};
+	return vb200_jpegsave_batch_opts(frames, frames_location, bpl, frame_stride, n, width, height, bands, &opt, out, out_location, out_stride,
+		lengths);
+}
+
+/* vb200_jpegsave_batch with vips_jpegsave's entropy-coding options too: optimize_coding (per-frame Huffman tables) and
+ * restart_interval (RSTn every N MCUs, 0..65535)
+ */
+extern "C" int
+vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands,
+	const VB200JpegSaveOptions *opt, void *out, int out_location, size_t out_stride, size_t *lengths)
+{
 	const char *domain = "jpegsave_batch";
-	if (!frames || !out || n < 1) {
+	if (!frames || !out || !opt || n < 1) {
 		error(domain, "null argument");
 		return -1;
 	}
+	const int Q = opt->Q, subsample_mode = opt->subsample_mode;
+	if (check_restart(domain, opt->restart_interval))
+		return -1;
 	if (ensure_init(domain))
 		return -1;
 	cudaStream_t s = current_stream();
@@ -868,7 +1501,8 @@ vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, size_t
 			dst = dout;
 		}
 		std::vector<size_t> len(n);
-		if (dev_jpeg_encode_batch(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, dst, out_stride, len.data(), s))
+		if (dev_jpeg_encode_batch(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->optimize_coding != 0,
+				opt->restart_interval, dst, out_stride, len.data(), s))
 			break;
 		if (lengths)
 			memcpy(lengths, len.data(), n * sizeof(size_t));
