@@ -565,13 +565,19 @@ int vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, si
  * its own symbol counts (jchuff.c jpeg_gen_optimal_table), so every frame carries its own DHT segments.
  * restart_interval (jpegsave.c:284-289 -> vips2jpeg.c:593-597, cinfo.restart_interval): an RSTn marker every that many
  * MCUs and a DRI segment; 0 for none.  Values above 65535 are refused (-1): libjpeg would write DRI modulo 65536 and a
- * stream no reader can follow.  With both 0 the streams are vb200_jpegsave_batch's.
+ * stream no reader can follow.  interlace (jpegsave.c:234-238 -> vips2jpeg.c:670-673, jpeg_simple_progression):
+ * non-zero writes a progressive stream (SOF2, libjpeg's 10-scan script for colour, 6 scans for greyscale); libjpeg forces
+ * optimize_coding on in progressive mode, so every scan carries its own optimal Huffman table and optimize_coding makes
+ * no difference; restart_interval counts MCUs in the interleaved DC scans and single blocks in the others.  With all
+ * three 0 the streams are vb200_jpegsave_batch's.
+ * The struct grew by interlace, its last member: C callers rebuild against this header.
  */
 typedef struct {
 	int Q;
 	int subsample_mode;
 	int optimize_coding;
 	int restart_interval;
+	int interlace;
 } VB200JpegSaveOptions;
 /* vb200_jpegsave_batch with VB200JpegSaveOptions; the streams are libjpeg-turbo's byte for byte with the same options
  * (tests/test_jpeg_encode_options.py) */
@@ -584,6 +590,10 @@ int vb200_debug_jpeg_encode(const void *pixels, size_t bpl, int width, int heigh
 /* test hook, host only: vb200_debug_jpeg_encode with every option of VB200JpegSaveOptions */
 int vb200_debug_jpeg_encode_opts(const void *pixels, size_t bpl, int width, int height, int bands, const VB200JpegSaveOptions *options,
 	void *out, size_t cap, size_t *len);
+/* test hook, host only: what the host twin's progressive coder (jcphuff.c restated) reaches for an image: events[0] EOB runs
+ * forced out at 0x7FFF blocks, [1] EOB runs forced out by the correction-bit buffer, [2] ZRLs in refinement scans */
+int vb200_debug_jpeg_prog_events(const void *pixels, size_t bpl, int width, int height, int bands, const VB200JpegSaveOptions *options,
+	unsigned long long *events);
 /* test hook, host only: the encoder's restatement of jpeg_gen_optimal_table on symbol counts freq[256] -> bits[17]
  * (bits[0] unused) and huffval[256]; -1 when the counts add up to 10^9 or more */
 int vb200_debug_jpeg_optimal_table(const unsigned *freq, unsigned char *bits, unsigned char *huffval);

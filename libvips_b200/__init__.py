@@ -163,6 +163,7 @@ def lib():
         L.vb200_debug_jpeg_encode_opts.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, SO, C.c_void_p, C.c_size_t,
                                                    C.POINTER(C.c_size_t)]
         L.vb200_debug_jpeg_optimal_table.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.vb200_debug_jpeg_prog_events.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, SO, C.POINTER(C.c_ulonglong)]
         L.vb200_thumbnail_buffer.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int]
         L.vb200_thumbnail_plan_run_jpeg.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int,
                                                     C.c_void_p, C.c_int, C.c_size_t]
@@ -537,15 +538,18 @@ _SAVE_BUFFERS = {}
 
 class JpegSaveOptions(C.Structure):
     """VB200JpegSaveOptions"""
-    _fields_ = [("Q", C.c_int), ("subsample_mode", C.c_int), ("optimize_coding", C.c_int), ("restart_interval", C.c_int)]
+    _fields_ = [("Q", C.c_int), ("subsample_mode", C.c_int), ("optimize_coding", C.c_int), ("restart_interval", C.c_int),
+                ("interlace", C.c_int)]
 
 
-def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0):
+def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0,
+                   interlace=False):
     """vips_jpegsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1 or 3) on the device -> list of bytes.
     in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  optimize_coding: per-frame Huffman
-    tables; restart_interval: an RSTn marker every that many MCUs (0..65535, 0 for none)"""
+    tables; restart_interval: an RSTn marker every that many MCUs (0..65535, 0 for none); interlace: a progressive stream
+    (libjpeg's jpeg_simple_progression script, every scan with its own optimal tables)"""
     mode = {"auto": 0, "on": 1, "off": 2}[subsample_mode]
-    opts = JpegSaveOptions(int(Q), mode, int(bool(optimize_coding)), int(restart_interval))
+    opts = JpegSaveOptions(int(Q), mode, int(bool(optimize_coding)), int(restart_interval), int(bool(interlace)))
     if in_ptr is None:
         frames = np.ascontiguousarray(frames)
         if frames.ndim == 3:

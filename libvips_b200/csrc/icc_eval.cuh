@@ -625,7 +625,7 @@ icc_colour(const IccJob &J, const void *pin, void *pout)
 			lab2xyz(lab, xyz);
 		}
 		else {
-			/* encode_xyz (:1050-1076), then lcms2's XYZ float (1.0 = 1.0) */
+			/* encode_xyz (icc_transform.c:1050-1076), then lcms2's XYZ float (1.0 = 1.0) */
 			const float X = p[0] / 100.0f, Y = p[1] / 100.0f, Z = p[2] / 100.0f;
 			xyz[0] = 1.047886F * X + 0.022919F * Y + -0.050216F * Z;
 			xyz[1] = 0.029582F * X + 0.990484F * Y + -0.017079F * Z;

@@ -547,9 +547,11 @@ put16(std::vector<unsigned char> &o, unsigned v)
 	o.push_back((unsigned char) v);
 }
 
-/* the markers before the Huffman tables, in libjpeg's order: SOI, JFIF APP0, DQT per table, SOF0 */
+/* the markers before the Huffman tables, in libjpeg's order: SOI, JFIF APP0, DQT per table, SOF0 (sof: SOF2 for a
+ * progressive stream)
+ */
 void
-header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned char> &o)
+header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned char> &o, unsigned sof = 0xFFC0)
 {
 	o.clear();
 	put16(o, 0xFFD8);
@@ -564,7 +566,7 @@ header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned c
 		for (int i = 0; i < 64; i++)
 			o.push_back((unsigned char) T.q[t][kZz[i]]);
 	}
-	put16(o, 0xFFC0);
+	put16(o, sof);
 	put16(o, 8 + 3 * G.ncomp);
 	o.push_back(8);
 	put16(o, (unsigned) G.h);
@@ -674,6 +676,225 @@ make_geom(const char *domain, int w, int h, int bands, int quality, int subsampl
 	G->blocks_per_mcu = bands == 1 ? 1 : (G->sub ? 6 : 3);
 	G->blocks = G->mcus_x * G->mcus_y * G->blocks_per_mcu;
 	return 0;
+}
+
+/* ------------------------------------------------------------------ progressive save: the scan script (host + device) */
+
+constexpr int kMaxProgScans = 10;  /* jcparam.c jpeg_simple_progression: 10 scans for YCbCr, 6 for greyscale */
+constexpr int kMaxProgTables = 10; /* one table per DC-first component table and per AC scan: 10 for YCbCr, 5 for greyscale */
+constexpr int kMaxCorrBits = 1000; /* jcphuff.c MAX_CORR_BITS: the correction bits an EOB run may hold */
+
+/* One scan of the script.  A unit is what a restart interval counts: an MCU of the interleaved DC scans, one block of
+ * the component's own grid (ceil(comp_w / 8) x ceil(comp_h / 8), no dummy blocks; T.81 A.2.2) in the others.
+ */
+struct ProgScan {
+	int comp;			/* the scan's component, -1 for the interleaved DC scans */
+	int ss, se, ah, al; /* spectral band and successive-approximation bits */
+	int ux, units;		/* units per row, units */
+	int unit_base;		/* the scan's first unit in the frame's list of units */
+	int seg_base, nseg; /* its restart intervals (segments) in the frame's list of segments; 1 without restart markers */
+	int tab, nt;		/* its first table in the frame's list of tables and their number (0 for DC refinement) */
+};
+
+struct ProgScript {
+	int nscans, ntab, units, nseg, restart;
+	ProgScan s[kMaxProgScans];
+	int tab_class[kMaxProgTables]; /* put_dht's t: 0 DC lum, 1 AC lum, 2 DC chr, 3 AC chr */
+	/* the device's header template: the frame's markers before the first scan (prefix_len bytes), then each scan's DRI / SOS
+	 * at sfx_at[s] .. sfx_at[s + 1]
+	 */
+	int prefix_len, sfx_at[kMaxProgScans + 1];
+};
+
+/* the component's own block grid */
+HD void
+comp_grid(const EncodeGeom &G, int c, int *bw, int *bh)
+{
+	if (G.ncomp == 3 && G.sub && c == 0) {
+		*bw = (G.w + 7) / 8;
+		*bh = (G.h + 7) / 8;
+	}
+	else {
+		*bw = G.mcus_x;
+		*bh = G.mcus_y;
+	}
+}
+
+/* block (bx, by) of component c's grid -> its index in the MCU-ordered coefficients */
+HD unsigned
+comp_block_index(const EncodeGeom &G, int c, int bx, int by)
+{
+	if (G.ncomp == 3 && G.sub) {
+		if (c == 0)
+			return ((unsigned) (by >> 1) * G.mcus_x + (unsigned) (bx >> 1)) * 6 + (unsigned) ((by & 1) * 2 + (bx & 1));
+		return ((unsigned) by * G.mcus_x + (unsigned) bx) * 6 + 3 + (unsigned) c;
+	}
+	return ((unsigned) by * G.mcus_x + (unsigned) bx) * G.blocks_per_mcu + (unsigned) c;
+}
+
+/* jcparam.c jpeg_simple_progression (fill_dc_scans, fill_a_scan / fill_scans), laid out for one geometry: YCbCr
+ *   DC 0-0 Al 1 (interleaved); Y 1-5 Al 2; Cr 1-63 Al 1; Cb 1-63 Al 1; Y 6-63 Al 2; Y 1-63 Ah 2 Al 1;
+ *   DC Ah 1 Al 0 (interleaved); Cr 1-63 Ah 1 Al 0; Cb 1-63 Ah 1 Al 0; Y 1-63 Ah 1 Al 0
+ * and greyscale the same without the chroma scans.  Tables: the DC-first scan one per dc_tbl_no (Y 0, Cb and Cr 1), every
+ * AC scan its own (finish_pass_gather_phuff builds a table per scan), DC refinement none.
+ */
+void
+prog_script(const EncodeGeom &G, int restart, ProgScript *P)
+{
+	static const int colour[10][5] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2}, {2, 1, 63, 0, 1}, {1, 1, 63, 0, 1}, {0, 6, 63, 0, 2}, {0, 1, 63, 2, 1},
+		{-1, 0, 0, 1, 0}, {2, 1, 63, 1, 0}, {1, 1, 63, 1, 0}, {0, 1, 63, 1, 0}};
+	static const int grey[6][5] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2}, {0, 6, 63, 0, 2}, {0, 1, 63, 2, 1}, {-1, 0, 0, 1, 0}, {0, 1, 63, 1, 0}};
+	const int(*script)[5] = G.ncomp == 3 ? colour : grey;
+	memset(P, 0, sizeof(*P));
+	P->nscans = G.ncomp == 3 ? 10 : 6;
+	P->restart = restart;
+	for (int i = 0; i < P->nscans; i++) {
+		ProgScan &S = P->s[i];
+		S.comp = script[i][0];
+		S.ss = script[i][1];
+		S.se = script[i][2];
+		S.ah = script[i][3];
+		S.al = script[i][4];
+		int bw = G.mcus_x, bh = G.mcus_y;
+		if (S.comp >= 0)
+			comp_grid(G, S.comp, &bw, &bh);
+		S.ux = bw;
+		S.units = bw * bh;
+		S.unit_base = P->units;
+		P->units += S.units;
+		S.nseg = restart ? (S.units + restart - 1) / restart : 1;
+		S.seg_base = P->nseg;
+		P->nseg += S.nseg;
+		S.tab = P->ntab;
+		if (S.ss == 0 && S.ah == 0) {
+			P->tab_class[P->ntab++] = 0;
+			if (G.ncomp == 3)
+				P->tab_class[P->ntab++] = 2;
+		}
+		else if (S.ss > 0)
+			P->tab_class[P->ntab++] = S.comp ? 3 : 1;
+		S.nt = P->ntab - S.tab;
+	}
+}
+
+/* jcmarker.c write_scan_header after the DHTs: DRI before the first scan when there are restart intervals (emitted when
+ * the interval differs from the last one written), then emit_sos with 0 for the table selectors a scan does not use
+ */
+void
+prog_scan_suffix(const EncodeGeom &G, const ProgScan &S, bool first, int restart, std::vector<unsigned char> &o)
+{
+	if (first && restart > 0) {
+		put16(o, 0xFFDD);
+		put16(o, 4);
+		put16(o, (unsigned) restart);
+	}
+	const int nc = S.comp < 0 ? G.ncomp : 1;
+	put16(o, 0xFFDA);
+	put16(o, 6 + 2 * nc);
+	o.push_back((unsigned char) nc);
+	for (int i = 0; i < nc; i++) {
+		const int c = S.comp < 0 ? i : S.comp;
+		o.push_back((unsigned char) (c + 1));
+		int sel = 0;
+		if (S.ss == 0)
+			sel = S.ah == 0 && c ? 0x10 : 0; /* DC scan: dc_tbl_no, none in a refinement scan */
+		else
+			sel = c ? 1 : 0; /* AC scan: ac_tbl_no */
+		o.push_back((unsigned char) sel);
+	}
+	o.push_back((unsigned char) S.ss);
+	o.push_back((unsigned char) S.se);
+	o.push_back((unsigned char) ((S.ah << 4) | S.al));
+}
+
+/* The symbols and bits of one block in an AC scan of the script, without its EOB run (jcphuff.c encode_mcu_AC_first,
+ * encode_mcu_AC_refine; sym(symbol) for every Huffman symbol, bits(value, n) for the bits that follow it: the magnitude,
+ * or the sign of a newly non-zero coefficient followed by the correction bits buffered since the previous symbol (BR)).
+ * Returns the block's place in the EOB run structure: kEmits when it codes a symbol -- a pending EOB run is flushed just
+ * before its first one --, kTail when it ends in an EOB (it joins the run), and << 2 the correction bits it leaves to the
+ * run (BE), which tail(bit) receives in order.  None of this depends on the Huffman tables.
+ */
+constexpr unsigned kEmits = 1, kTail = 2;
+
+HD int
+ac_abs(const short *blk, const unsigned char *zz, int k, int al)
+{
+	const int v = blk[zz[k]];
+	return (v < 0 ? -v : v) >> al;
+}
+
+template <typename Sym, typename Bits, typename Tail>
+HD unsigned
+walk_ac_block(const unsigned char *zz, const short *blk, int ss, int se, int ah, int al, Sym sym, Bits bits, Tail tail)
+{
+	unsigned flags = 0;
+	int r = 0;
+	if (ah == 0) {
+		for (int k = ss; k <= se; k++) {
+			const int t = ac_abs(blk, zz, k, al); /* the point transform: |v| >> Al, the sign put back after */
+			if (t == 0) {
+				r++;
+				continue;
+			}
+			flags |= kEmits;
+			while (r > 15) {
+				sym(0xF0);
+				r -= 16;
+			}
+			const int nb = bit_size(t);
+			sym((r << 4) + nb);
+			bits((unsigned) (blk[zz[k]] < 0 ? ~t : t) & ((1u << nb) - 1), nb);
+			r = 0;
+		}
+		return r > 0 ? flags | kTail : flags;
+	}
+	int eob = 0; /* the last newly non-zero coefficient */
+	for (int k = ss; k <= se; k++)
+		if (ac_abs(blk, zz, k, al) == 1)
+			eob = k;
+	int kbr = ss, nbr = 0; /* BR: coefficients kbr .. k - 1 with |value| > 1, nbr of them */
+	auto put_br = [&](int k) {
+		for (int j = kbr; j < k; j++) {
+			const int t = ac_abs(blk, zz, j, al);
+			if (t > 1)
+				bits((unsigned) t & 1u, 1);
+		}
+		nbr = 0;
+	};
+	for (int k = ss; k <= se; k++) {
+		const int t = ac_abs(blk, zz, k, al);
+		if (t == 0) {
+			r++;
+			continue;
+		}
+		/* ZRLs, but not where they fold into the EOB */
+		while (r > 15 && k <= eob) {
+			flags |= kEmits;
+			sym(0xF0);
+			r -= 16;
+			put_br(k);
+			kbr = k;
+		}
+		if (t > 1) {
+			nbr++; /* a coefficient already non-zero: one correction bit, buffered */
+			continue;
+		}
+		flags |= kEmits;
+		sym((r << 4) + 1);
+		bits(blk[zz[k]] < 0 ? 0u : 1u, 1);
+		put_br(k);
+		kbr = k + 1;
+		r = 0;
+	}
+	if (r > 0 || nbr > 0) {
+		flags |= kTail | (unsigned) nbr << 2;
+		for (int j = kbr; j <= se; j++) {
+			const int t = ac_abs(blk, zz, j, al);
+			if (t > 1)
+				tail((unsigned) t & 1u);
+		}
+	}
+	return flags;
 }
 
 /* ------------------------------------------------------------------ kernels */
@@ -1083,6 +1304,554 @@ jpeg_stuff_kernel(const unsigned long long *__restrict__ totals, const unsigned 
 	}
 }
 
+/* ------------------------------------------------------------------ progressive save (interlace) on the device
+ *
+ * Every scan of the script is coded in the same launches: a frame's units (ProgScan) of all scans form one list, each
+ * unit owns two bit slots -- [the EOB run flushed before it + its own symbols] and [the run flushed after it] -- and a
+ * final empty slot makes the frame's total.  A segment is a restart interval of a scan (the whole scan without them);
+ * every segment starts on a byte boundary and ends padded with 1-bits, and the stuffing stage puts the next scan's
+ * header (DHTs, SOS) or FF Dn between segments.
+ */
+
+/* a unit's bit slots and a frame's bit slot count */
+constexpr int kProgSlotsPerUnit = 2;
+/* the bits one block takes over all the scans of the script, at most: DC first (a 16-bit code + 11 bits), DC refinement
+ * (1), the first AC scans over 63 positions (a 16-bit code + 10 bits each, ZRLs at most a bit per zero), the refinement
+ * scans over 63 positions twice (a 16-bit code + sign for a newly non-zero coefficient, else at most a correction bit or a
+ * bit of ZRL), and two EOB-run flushes (EOBn code 16 bits + 14 run bits; their correction bits are the blocks' own,
+ * counted above) per unit in each of the 4 AC scans of a luma block (chroma blocks take 2)
+ */
+constexpr int kProgBlockBits = (16 + 11) + 1 + 63 * (16 + 10) + 2 * 63 * (16 + 1) + 4 * 2 * (16 + 14);
+constexpr int kProgBlockBytes = (kProgBlockBits + 7) / 8;
+/* a table counts at most 65 symbols per block (63 AC symbols and two EOBn, or one DC category) */
+static_assert(((1u << 29) / kProgBlockBytes) * 65u + 1u < kFreqSentinel, "symbol counts must stay below the sentinel");
+/* a frame's headers: SOI + APP0 + 2 DQT + SOF2 (177 bytes for 3 components), a DHT per table (21 bytes + at most 256
+ * symbols), one DRI (6), an SOS per scan (at most 14)
+ */
+constexpr int kProgHeaderBound = 177 + kMaxProgTables * (21 + 256) + 6 + kMaxProgScans * 14;
+constexpr int kProgHeaderSlot = 3200;
+static_assert(kProgHeaderBound <= kProgHeaderSlot, "a frame's progressive headers must fit their slot");
+/* EOB runs: jcphuff.c flushes at 0x7FFF blocks, or when the buffered correction bits pass MAX_CORR_BITS - DCTSIZE2 + 1 */
+constexpr unsigned kMaxEobRun = 0x7FFF;
+static_assert(kMaxEobRun < (1u << 16) && kMaxCorrBits < (1 << 16), "a flush packs its run and its correction bits in 16 bits each");
+
+/* a frame's code tables, one per table of the script */
+struct ProgHuff {
+	unsigned ehufco[kMaxProgTables][256];
+	unsigned char ehufsi[kMaxProgTables][256];
+};
+
+__device__ __forceinline__ int
+prog_scan_of_unit(const ProgScript &P, unsigned u)
+{
+	int s = 0;
+	while (s + 1 < P.nscans && u >= (unsigned) P.s[s + 1].unit_base)
+		s++;
+	return s;
+}
+
+__device__ __forceinline__ int
+prog_scan_of_seg(const ProgScript &P, unsigned g)
+{
+	int s = 0;
+	while (s + 1 < P.nscans && g >= (unsigned) P.s[s + 1].seg_base)
+		s++;
+	return s;
+}
+
+/* the first bit slot of segment g (g == nseg: the frame's final slot) */
+__device__ __forceinline__ unsigned
+prog_seg_slot(const ProgScript &P, unsigned g)
+{
+	if (g >= (unsigned) P.nseg)
+		return kProgSlotsPerUnit * (unsigned) P.units;
+	const ProgScan &S = P.s[prog_scan_of_seg(P, g)];
+	const unsigned per = P.restart ? (unsigned) P.restart : (unsigned) S.units;
+	return kProgSlotsPerUnit * ((unsigned) S.unit_base + (g - (unsigned) S.seg_base) * per);
+}
+
+/* the block of unit i of a single-component scan */
+__device__ __forceinline__ unsigned
+prog_block(const EncodeGeom &G, const ProgScan &S, unsigned i)
+{
+	return comp_block_index(G, S.comp, (int) (i % (unsigned) S.ux), (int) (i / (unsigned) S.ux));
+}
+
+/* one MCU of the interleaved DC-first scan (jcphuff.c encode_mcu_DC_first): the point-transformed DC (arithmetic shift by
+ * Al) against the previous block of its component, reset at each restart interval; sym(table 0 / 1, category), bits
+ */
+template <typename Sym, typename Bits>
+__device__ __forceinline__ void
+walk_dc_first(const EncodeGeom &G, const short *fc, unsigned mcu, int al, int restart, Sym sym, Bits bits)
+{
+	for (int j = 0; j < G.blocks_per_mcu; j++) {
+		const unsigned b = mcu * (unsigned) G.blocks_per_mcu + (unsigned) j;
+		const int comp = block_comp(G, j);
+		int diff = (fc[(size_t) b * 64] >> al) - (previous_dc(G, fc, b, restart) >> al);
+		int t2 = diff;
+		if (diff < 0) {
+			diff = -diff;
+			t2--;
+		}
+		const int nb = bit_size(diff);
+		sym(comp ? 1 : 0, nb);
+		if (nb)
+			bits((unsigned) t2 & ((1u << nb) - 1), nb);
+	}
+}
+
+/* the EOBn symbol of a run of r blocks (emit_eobrun): n = floor(log2 r), then n bits of r */
+__device__ __forceinline__ int
+eobrun_n(unsigned r)
+{
+	return 31 - __clz((int) r);
+}
+
+/* bits written OR-ed into a zeroed bit buffer from bit pos on (neighbours share their boundary bytes) */
+struct BitSink {
+	unsigned *out;
+	unsigned byte;
+	unsigned long long acc;
+	int nacc;
+	__device__ BitSink(unsigned *o, unsigned pos) : out(o), byte(pos >> 3), acc(0), nacc((int) (pos & 7u)) {}
+	__device__ __forceinline__ void or_byte(unsigned at, unsigned v)
+	{
+		if (v)
+			atomicOr(out + (at >> 2), v << (8 * (at & 3u)));
+	}
+	__device__ __forceinline__ void put(unsigned code, int len)
+	{
+		acc = (acc << len) | code;
+		nacc += len;
+		while (nacc >= 8) {
+			or_byte(byte, (unsigned) (acc >> (nacc - 8)) & 0xffu);
+			byte++;
+			nacc -= 8;
+		}
+	}
+	/* n bits left to other threads */
+	__device__ __forceinline__ void skip(unsigned n)
+	{
+		for (; n > 16; n -= 16)
+			put(0, 16);
+		put(0, (int) n);
+	}
+	__device__ __forceinline__ void finish()
+	{
+		if (nacc > 0)
+			or_byte(byte, (unsigned) (acc << (8 - nacc)) & 0xffu);
+	}
+};
+
+/* 1. block summaries and statistics, one thread per unit (all scans): each AC unit's place in the EOB run structure
+ * (walk_ac_block's flags, a byte) into summ, and the symbols of its own -- everything but the EOBn of the runs -- into the
+ * CTA's histograms (a table per scan), added to the frame's counts[kMaxProgTables][256]
+ */
+__global__ void __launch_bounds__(128)
+jpeg_prog_summary_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const short *__restrict__ coef,
+	unsigned char *__restrict__ summ, unsigned *__restrict__ counts)
+{
+	__shared__ unsigned s_hist[kMaxProgTables * 256];
+	for (int i = threadIdx.x; i < kMaxProgTables * 256; i += blockDim.x)
+		s_hist[i] = 0;
+	__syncthreads();
+	const unsigned u = blockIdx.x * blockDim.x + threadIdx.x;
+	if (u < (unsigned) P.units) {
+		const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+		const unsigned i = u - (unsigned) S.unit_base;
+		const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
+		unsigned *h = s_hist + S.tab * 256;
+		if (S.ss == 0) {
+			if (S.ah == 0)
+				walk_dc_first(G, fc, i, S.al, P.restart, [&](int t, int sym) { atomicAdd(&h[t * 256 + sym], 1u); }, [](unsigned, int) {});
+		}
+		else
+			summ[(size_t) blockIdx.y * P.units + u] = (unsigned char) walk_ac_block(
+				T->zz, fc + (size_t) prog_block(G, S, i) * 64, S.ss, S.se, S.ah, S.al, [&](int sym) { atomicAdd(&h[sym], 1u); }, [](unsigned, int) {},
+				[](unsigned) {});
+	}
+	__syncthreads();
+	unsigned *dst = counts + (size_t) blockIdx.y * kMaxProgTables * 256;
+	for (int i = threadIdx.x; i < P.ntab * 256; i += blockDim.x)
+		if (s_hist[i])
+			atomicAdd(dst + i, s_hist[i]);
+}
+
+/* 2. the chain walk, one thread per segment of an AC scan: jcphuff.c's EOB run state (EOBRUN, BE) over the segment's
+ * summaries.  A run is flushed before the first unit that codes a symbol, after the unit that takes it to 0x7FFF blocks
+ * or past MAX_CORR_BITS - 63 correction bits, and after the segment's last unit (emit_restart / finish_pass).  Each
+ * flush goes into its slot of runs[] as (run << 16) | correction bits, its EOBn into the counts; each run member with
+ * correction bits gets the flush's slot (defer_slot) and the offset of its bits among the flush's (defer_off).
+ */
+__global__ void __launch_bounds__(128)
+jpeg_prog_walk_kernel(const __grid_constant__ ProgScript P, const unsigned char *__restrict__ summ, unsigned *__restrict__ runs,
+	unsigned *__restrict__ defer_slot, unsigned short *__restrict__ defer_off, unsigned *__restrict__ counts)
+{
+	const unsigned g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= (unsigned) P.nseg)
+		return;
+	const ProgScan &S = P.s[prog_scan_of_seg(P, g)];
+	if (S.ss == 0)
+		return;
+	const size_t f = blockIdx.y;
+	const unsigned char *sm = summ + f * P.units;
+	unsigned *rn = runs + f * kProgSlotsPerUnit * P.units, *ds = defer_slot + f * P.units;
+	unsigned short *dof = defer_off + f * P.units;
+	unsigned *cnt = counts + f * kMaxProgTables * 256 + (size_t) S.tab * 256;
+	const unsigned u0 = prog_seg_slot(P, g) / kProgSlotsPerUnit;
+	const unsigned u1 = min(u0 + (P.restart ? (unsigned) P.restart : (unsigned) S.units), (unsigned) (S.unit_base + S.units));
+	unsigned run = 0, be = 0, start = 0;
+	auto flush = [&](unsigned slot, unsigned last) {
+		rn[slot] = run << 16 | be;
+		for (unsigned v = start; v <= last; v++)
+			if (sm[v] >> 2)
+				ds[v] = slot;
+		atomicAdd(cnt + (eobrun_n(run) << 4), 1u);
+		run = be = 0;
+	};
+	for (unsigned u = u0; u < u1; u++) {
+		const unsigned fl = sm[u];
+		rn[kProgSlotsPerUnit * u] = 0;
+		rn[kProgSlotsPerUnit * u + 1] = 0;
+		if ((fl & kEmits) && run)
+			flush(kProgSlotsPerUnit * u, u - 1);
+		if (fl & kTail) {
+			if (!run)
+				start = u;
+			dof[u] = (unsigned short) be;
+			run++;
+			be += fl >> 2;
+			if (run == kMaxEobRun || be > (unsigned) (kMaxCorrBits - 64 + 1))
+				flush(kProgSlotsPerUnit * u + 1, u);
+		}
+	}
+	if (run)
+		flush(kProgSlotsPerUnit * (u1 - 1) + 1, u1 - 1);
+}
+
+/* 3. tables and headers, one CTA per frame, one warp per table of the script: gen_optimal_table on the table's counts,
+ * the frame's code tables, then its headers into its kProgHeaderSlot-byte slot -- the markers before the first scan, and
+ * per scan its DHTs and DRI / SOS from the template --; hdr_at[frame][s] = where scan s's header starts (0 for the first,
+ * which comes with the frame's markers; [nscans] = the end), header_lens[frame] = the bytes before the first scan's data
+ * (the stuffing passes count the later headers and the RSTn markers).  A frame whose tables cannot be built sets *bad.
+ */
+__global__ void __launch_bounds__(32 * kMaxProgTables)
+jpeg_prog_huffopt_kernel(const __grid_constant__ ProgScript P, const unsigned *__restrict__ counts, ProgHuff *__restrict__ huff,
+	const unsigned char *__restrict__ tmpl, unsigned char *__restrict__ headers, unsigned *__restrict__ hdr_at, unsigned *__restrict__ header_lens,
+	int *__restrict__ bad)
+{
+	__shared__ unsigned s_freq[kMaxProgTables][257];
+	__shared__ int s_size[kMaxProgTables][257], s_others[kMaxProgTables][257];
+	__shared__ unsigned char s_bits[kMaxProgTables][17], s_val[kMaxProgTables][256];
+	__shared__ unsigned s_dht_at[kMaxProgTables], s_sfx_dst[kMaxProgScans], s_len;
+	__shared__ int s_fail;
+	const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const unsigned *cnt = counts + (size_t) blockIdx.x * kMaxProgTables * 256;
+	if (threadIdx.x == 0)
+		s_fail = 0;
+	for (int i = threadIdx.x; i < kMaxProgTables * 256; i += blockDim.x)
+		s_freq[i >> 8][i & 255] = cnt[i];
+	__syncthreads();
+	ProgHuff *fh = huff + blockIdx.x;
+	if (w < P.ntab) {
+		unsigned *freq = s_freq[w];
+		auto pick = [&](int exclude) {
+			__syncwarp();
+			/* key: frequency, then the larger index first */
+			unsigned long long best = ~0ull;
+			for (int i = lane; i <= 256; i += 32) {
+				const unsigned f = freq[i];
+				if (f && f <= kFreqSentinel && i != exclude) {
+					const unsigned long long key = ((unsigned long long) f << 9) | (unsigned) (511 - i);
+					best = key < best ? key : best;
+				}
+			}
+			for (int o = 16; o; o >>= 1) {
+				const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
+				best = v < best ? v : best;
+			}
+			return best == ~0ull ? -1 : 511 - (int) (best & 511u);
+		};
+		if (gen_optimal_table(freq, s_size[w], s_others[w], s_bits[w], s_val[w], lane == 0, pick))
+			s_fail = 1;
+		__syncwarp();
+		if (lane == 0)
+			derive_codes(s_bits[w] + 1, s_val[w], fh->ehufco[w], fh->ehufsi[w]);
+	}
+	__syncthreads();
+	unsigned *at = hdr_at + (size_t) blockIdx.x * (kMaxProgScans + 1);
+	if (threadIdx.x == 0) {
+		unsigned len = (unsigned) P.prefix_len;
+		for (int s = 0; s < P.nscans; s++) {
+			at[s] = s ? len : 0;
+			for (int t = P.s[s].tab; t < P.s[s].tab + P.s[s].nt; t++) {
+				s_dht_at[t] = len;
+				len += 21 + table_values(s_bits[t]);
+			}
+			s_sfx_dst[s] = len;
+			len += (unsigned) (P.sfx_at[s + 1] - P.sfx_at[s]);
+		}
+		at[P.nscans] = len;
+		s_len = len;
+		header_lens[blockIdx.x] = at[1];
+		if (s_fail || len > kProgHeaderSlot) {
+			header_lens[blockIdx.x] = 0;
+			atomicExch(bad, 1);
+		}
+	}
+	__syncthreads();
+	if (s_fail || s_len > kProgHeaderSlot)
+		return;
+	unsigned char *o = headers + (size_t) blockIdx.x * kProgHeaderSlot;
+	for (int i = threadIdx.x; i < P.prefix_len; i += blockDim.x)
+		o[i] = tmpl[i];
+	for (int s = 0; s < P.nscans; s++)
+		for (int i = P.sfx_at[s] + threadIdx.x; i < P.sfx_at[s + 1]; i += blockDim.x)
+			o[s_sfx_dst[s] + (unsigned) (i - P.sfx_at[s])] = tmpl[i];
+	if (w < P.ntab && lane == 0)
+		put_dht(o + s_dht_at[w], P.tab_class[w], s_bits[w], s_val[w]);
+}
+
+/* the bits of a flushed EOB run: EOBn code, n bits of the run, its correction bits */
+__device__ __forceinline__ unsigned
+flush_bits(const unsigned char *si, unsigned r)
+{
+	if (!r)
+		return 0;
+	const int n = eobrun_n(r >> 16);
+	return si[n << 4] + (unsigned) n + (r & 0xffffu);
+}
+
+/* 4. one thread per unit: the bits of its two slots with the frame's tables */
+__global__ void __launch_bounds__(128)
+jpeg_prog_count_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const ProgHuff *__restrict__ huff,
+	const short *__restrict__ coef, const unsigned *__restrict__ runs, unsigned *__restrict__ bits)
+{
+	const unsigned u = blockIdx.x * blockDim.x + threadIdx.x;
+	const size_t nslots = (size_t) kProgSlotsPerUnit * P.units + 1;
+	unsigned *fb = bits + blockIdx.y * nslots;
+	if (u == 0)
+		fb[nslots - 1] = 0;
+	if (u >= (unsigned) P.units)
+		return;
+	const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+	const unsigned i = u - (unsigned) S.unit_base;
+	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
+	const ProgHuff &H = huff[blockIdx.y];
+	unsigned body = 0, post = 0;
+	if (S.ss == 0) {
+		if (S.ah == 0)
+			walk_dc_first(G, fc, i, S.al, P.restart, [&](int t, int sym) { body += H.ehufsi[S.tab + t][sym]; }, [&](unsigned, int n) { body += n; });
+		else
+			body = (unsigned) G.blocks_per_mcu; /* encode_mcu_DC_refine: a bit per block */
+	}
+	else {
+		const unsigned char *si = H.ehufsi[S.tab];
+		const unsigned *rn = runs + blockIdx.y * (nslots - 1) + kProgSlotsPerUnit * u;
+		walk_ac_block(
+			T->zz, fc + (size_t) prog_block(G, S, i) * 64, S.ss, S.se, S.ah, S.al, [&](int sym) { body += si[sym]; }, [&](unsigned, int n) { body += n; },
+			[](unsigned) {});
+		body += flush_bits(si, rn[0]);
+		post = flush_bits(si, rn[1]);
+	}
+	fb[kProgSlotsPerUnit * u] = body;
+	fb[kProgSlotsPerUnit * u + 1] = post;
+}
+
+/* 5. after the bit prefix sum: segments, one CTA per frame.  Each takes its slots' bits rounded up to a whole byte,
+ * istart[frame][g] = the byte where segment g starts in the raw scan data, totals[frame] = their length in bits
+ */
+__global__ void __launch_bounds__(1024)
+jpeg_prog_segments_kernel(const __grid_constant__ ProgScript P, const unsigned *__restrict__ offs, unsigned long long *__restrict__ totals,
+	unsigned *__restrict__ istart)
+{
+	__shared__ unsigned long long s_part[1024];
+	const unsigned nseg = (unsigned) P.nseg;
+	const unsigned *o = offs + (size_t) blockIdx.x * ((size_t) kProgSlotsPerUnit * P.units + 1);
+	unsigned *st = istart + (size_t) blockIdx.x * nseg;
+	auto ibytes = [&](unsigned g) { return ((unsigned long long) o[prog_seg_slot(P, g + 1)] - o[prog_seg_slot(P, g)] + 7) >> 3; };
+	const unsigned per = (nseg + blockDim.x - 1) / blockDim.x;
+	const unsigned a = min(nseg, threadIdx.x * per), e = min(nseg, a + per);
+	unsigned long long sum = 0;
+	for (unsigned k = a; k < e; k++)
+		sum += ibytes(k);
+	s_part[threadIdx.x] = sum;
+	__syncthreads();
+	for (unsigned d = 1; d < blockDim.x; d <<= 1) {
+		const unsigned long long v = threadIdx.x >= d ? s_part[threadIdx.x - d] : 0;
+		__syncthreads();
+		s_part[threadIdx.x] += v;
+		__syncthreads();
+	}
+	unsigned long long run = s_part[threadIdx.x] - sum;
+	for (unsigned k = a; k < e; k++) {
+		st[k] = (unsigned) run;
+		run += ibytes(k);
+	}
+	if (threadIdx.x == blockDim.x - 1)
+		totals[blockIdx.x] = s_part[threadIdx.x] * 8;
+}
+
+/* 6. one thread per unit: its symbols and the runs flushed around them OR-ed into the frame's raw bit buffer at its
+ * slots, its deferred correction bits at the offset the walk gave them behind their flush's EOBn and run bits; the
+ * segment's last unit pads the segment's last byte with 1-bits
+ */
+__global__ void __launch_bounds__(128)
+jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const ProgHuff *__restrict__ huff,
+	const unsigned *__restrict__ istart, const short *__restrict__ coef, const unsigned *__restrict__ offs, const unsigned char *__restrict__ summ,
+	const unsigned *__restrict__ runs, const unsigned *__restrict__ defer_slot, const unsigned short *__restrict__ defer_off, unsigned *__restrict__ raw,
+	size_t raw_words)
+{
+	const unsigned u = blockIdx.x * blockDim.x + threadIdx.x;
+	if (u >= (unsigned) P.units)
+		return;
+	const size_t f = blockIdx.y, nslots = (size_t) kProgSlotsPerUnit * P.units + 1;
+	const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+	const unsigned i = u - (unsigned) S.unit_base;
+	const unsigned g = (unsigned) S.seg_base + (P.restart ? i / (unsigned) P.restart : 0);
+	const unsigned *fo = offs + f * nslots;
+	/* bit positions in the raw buffer: slot offset - the segment's first slot offset + the segment's start */
+	const unsigned base = istart[f * P.nseg + g] * 8 - fo[prog_seg_slot(P, g)];
+	unsigned *out = raw + f * raw_words;
+	const short *fc = coef + f * G.blocks * 64;
+	const ProgHuff &H = huff[f];
+	BitSink w(out, base + fo[kProgSlotsPerUnit * u]);
+	if (S.ss == 0) {
+		if (S.ah == 0)
+			walk_dc_first(
+				G, fc, i, S.al, P.restart, [&](int t, int sym) { w.put(H.ehufco[S.tab + t][sym], H.ehufsi[S.tab + t][sym]); },
+				[&](unsigned v, int n) { w.put(v, n); });
+		else
+			for (int j = 0; j < G.blocks_per_mcu; j++)
+				w.put((unsigned) (fc[((size_t) i * G.blocks_per_mcu + j) * 64] >> S.al) & 1u, 1);
+	}
+	else {
+		const unsigned *co = H.ehufco[S.tab];
+		const unsigned char *si = H.ehufsi[S.tab];
+		const unsigned *rn = runs + f * (nslots - 1);
+		/* a flushed run: EOBn and the run's bits, then room for its members' correction bits, which they write */
+		auto put_flush = [&](BitSink &b, unsigned r) {
+			if (r) {
+				const unsigned run = r >> 16;
+				const int n = eobrun_n(run);
+				b.put(co[n << 4], si[n << 4]);
+				if (n)
+					b.put(run & ((1u << n) - 1), n);
+				b.skip(r & 0xffffu);
+			}
+		};
+		put_flush(w, rn[kProgSlotsPerUnit * u]);
+		/* this unit's correction bits for the run it joins, if any */
+		const bool deferred = summ[f * P.units + u] >> 2;
+		unsigned dpos = 0;
+		if (deferred) {
+			const unsigned slot = defer_slot[f * P.units + u], r = rn[slot];
+			const int n = eobrun_n(r >> 16);
+			dpos = base + fo[slot] + si[n << 4] + (unsigned) n + defer_off[f * P.units + u];
+		}
+		BitSink d(out, dpos);
+		walk_ac_block(
+			T->zz, fc + (size_t) prog_block(G, S, i) * 64, S.ss, S.se, S.ah, S.al, [&](int sym) { w.put(co[sym], si[sym]); },
+			[&](unsigned v, int n) { w.put(v, n); }, [&](unsigned bit) { d.put(bit, 1); });
+		put_flush(w, rn[kProgSlotsPerUnit * u + 1]);
+		if (deferred)
+			d.finish();
+	}
+	w.finish();
+	const bool last = i + 1 == (unsigned) S.units || (P.restart && (i + 1) % (unsigned) P.restart == 0);
+	if (last) {
+		const unsigned end = base + fo[prog_seg_slot(P, g + 1)];
+		if (end & 7u)
+			w.or_byte(end >> 3, (1u << (8 - (end & 7u))) - 1); /* flush_bits: pad with ones */
+	}
+}
+
+/* insertion bytes before segments 1 .. j: the header of each scan that starts there (hdr_at), FF Dn before the others */
+__device__ __forceinline__ unsigned
+prog_inserts(const ProgScript &P, const unsigned *hat, unsigned j)
+{
+	unsigned n = 2 * j;
+	for (int s = 1; s < P.nscans && (unsigned) P.s[s].seg_base <= j; s++)
+		n += hat[s + 1] - hat[s] - 2;
+	return n;
+}
+
+/* 7. stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw data, plus the bytes inserted before the
+ * segments that start in the span
+ */
+__global__ void __launch_bounds__(128)
+jpeg_prog_ffcount_kernel(const __grid_constant__ ProgScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
+	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ istart, const unsigned *__restrict__ hdr_at, unsigned *__restrict__ counts)
+{
+	const int c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= max_chunks)
+		return;
+	const unsigned long long nbytes = totals[blockIdx.y] >> 3;
+	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
+	unsigned n = 0;
+	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
+	for (unsigned long long i = a; i < e; i++)
+		n += p[i] == 0xFF;
+	if (a < e) {
+		const unsigned *st = istart + (size_t) blockIdx.y * P.nseg + 1;
+		const unsigned *hat = hdr_at + (size_t) blockIdx.y * (kMaxProgScans + 1);
+		n += prog_inserts(P, hat, (unsigned) count_below(st, P.nseg - 1, e)) - prog_inserts(P, hat, (unsigned) count_below(st, P.nseg - 1, a));
+	}
+	counts[(size_t) blockIdx.y * max_chunks + c] = n;
+}
+
+/* 8. stuffing, pass 3 (pass 2 is jpeg_ffscan_kernel): the frame's markers and first scan header, the stuffed data with
+ * the next scan's header or FF D0+((k - 1) & 7) before interval k >= 1 of a scan (RSTn numbering restarts with every
+ * scan), EOI
+ */
+__global__ void __launch_bounds__(128)
+jpeg_prog_stuff_kernel(const __grid_constant__ ProgScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
+	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ counts, const unsigned char *__restrict__ headers, const unsigned *__restrict__ hdr_at,
+	const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride, const unsigned long long *__restrict__ lengths)
+{
+	const int c = blockIdx.x * blockDim.x + threadIdx.x;
+	unsigned char *o = out + (size_t) blockIdx.y * out_stride;
+	const unsigned long long len = lengths[blockIdx.y];
+	if (len > out_stride)
+		return;
+	const unsigned char *hdr = headers + (size_t) blockIdx.y * kProgHeaderSlot;
+	const unsigned *hat = hdr_at + (size_t) blockIdx.y * (kMaxProgScans + 1);
+	const unsigned h0 = hat[1];
+	if (c < (int) ((h0 + kStuffChunk - 1) / kStuffChunk))
+		for (unsigned i = (unsigned) c * kStuffChunk; i < min(h0, (unsigned) (c + 1) * kStuffChunk); i++)
+			o[i] = hdr[i];
+	if (c >= max_chunks)
+		return;
+	const unsigned long long nbytes = totals[blockIdx.y] >> 3;
+	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
+	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
+	unsigned char *d = o + h0 + a + counts[(size_t) blockIdx.y * max_chunks + c];
+	const unsigned *st = istart + (size_t) blockIdx.y * P.nseg;
+	const unsigned nseg = (unsigned) P.nseg;
+	unsigned k = a < e ? 1 + (unsigned) count_below(st + 1, (int) nseg - 1, a) : nseg; /* the next segment starting in the span */
+	for (unsigned long long i = a; i < e; i++) {
+		if (k < nseg && st[k] == i) {
+			const int s = prog_scan_of_seg(P, k);
+			if (k == (unsigned) P.s[s].seg_base)
+				for (unsigned j = hat[s]; j < hat[s + 1]; j++)
+					*d++ = hdr[j];
+			else {
+				*d++ = 0xFF;
+				*d++ = (unsigned char) (0xD0 + ((k - (unsigned) P.s[s].seg_base - 1) & 7));
+			}
+			k++;
+		}
+		const unsigned char v = p[i];
+		*d++ = v;
+		if (v == 0xFF)
+			*d++ = 0;
+	}
+	if (c == 0) {
+		o[len - 2] = 0xFF;
+		o[len - 1] = 0xD9;
+	}
+}
+
 /* the device buffers of one chunk of frames */
 struct ChunkArgs {
 	EncodeGeom G;
@@ -1280,6 +2049,137 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 	return rc;
 }
 
+/* dev_jpeg_encode_batch for a progressive stream (interlace): the scan script of jpeg_simple_progression, every scan with
+ * its own optimal tables (libjpeg forces optimize_coding on).  11 launches per chunk of frames whatever the frame count,
+ * scan count or restart interval: FDCT, summaries, chain walk, tables and headers, bit counts, bit prefix sum, segments,
+ * emit, and the three stuffing passes.
+ */
+int
+dev_jpeg_encode_progressive(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, int quality,
+	int subsample_mode, int restart, void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
+{
+	EncodeGeom G;
+	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
+		return -1;
+	ProgScript P;
+	prog_script(G, restart, &P);
+	/* every segment may end with one byte of padding */
+	const size_t scan_bound = (size_t) G.blocks * kProgBlockBytes + (size_t) P.nseg;
+	if (scan_bound >= (size_t) 1 << 29) {
+		error(domain, "frame too large for the device encoder");
+		return -1;
+	}
+	EncodeTables T;
+	make_tables(quality, &T);
+	/* the header template: the frame's markers up to SOF2, then each scan's DRI / SOS */
+	std::vector<unsigned char> tmpl;
+	header_prefix(G, T, tmpl, 0xFFC2);
+	P.prefix_len = (int) tmpl.size();
+	for (int i = 0; i < P.nscans; i++) {
+		P.sfx_at[i] = (int) tmpl.size();
+		prog_scan_suffix(G, P.s[i], i == 0, restart, tmpl);
+	}
+	P.sfx_at[P.nscans] = (int) tmpl.size();
+	const size_t units = (size_t) P.units, nslots = kProgSlotsPerUnit * units + 1;
+	const size_t raw_bytes = ((scan_bound + 3) & ~(size_t) 3) + 4;
+	const int max_chunks = (int) ((raw_bytes + kStuffChunk - 1) / kStuffChunk);
+	/* per-frame counts, tables and header slots (about 26 KB a frame) for one chunk of frames, reused by the next */
+	const size_t nc = (size_t) std::min(n, kMaxBatchFrames);
+	size_t off = 0;
+	auto take = [&](size_t bytes) {
+		const size_t o = off;
+		off += (bytes + 255) & ~(size_t) 255;
+		return o;
+	};
+	const size_t o_tab = take(sizeof(T)), o_tmpl = take(tmpl.size()), o_coef = take((size_t) n * G.blocks * 64 * sizeof(short)),
+				 o_summ = take((size_t) n * units), o_runs = take((size_t) n * kProgSlotsPerUnit * units * sizeof(unsigned)),
+				 o_dslot = take((size_t) n * units * sizeof(unsigned)), o_doff = take((size_t) n * units * sizeof(unsigned short)),
+				 o_bits = take((size_t) n * nslots * sizeof(unsigned)), o_tot = take((size_t) n * sizeof(unsigned long long)),
+				 o_len = take((size_t) n * sizeof(unsigned long long)), o_raw = take((size_t) n * raw_bytes),
+				 o_cnt = take((size_t) n * max_chunks * sizeof(unsigned)), o_ist = take((size_t) n * P.nseg * sizeof(unsigned)),
+				 o_freq = take(nc * kMaxProgTables * 256 * sizeof(unsigned)), o_huff = take(nc * sizeof(ProgHuff)), o_slots = take(nc * kProgHeaderSlot),
+				 o_hat = take(nc * (kMaxProgScans + 1) * sizeof(unsigned)), o_hlen = take(nc * sizeof(unsigned)), o_bad = take(sizeof(int));
+	char *scratch = nullptr;
+	if (dev_alloc(domain, (void **) &scratch, off, s))
+		return -1;
+	int rc = -1;
+	do {
+		if (cudaMemcpyAsync(scratch + o_tab, &T, sizeof(T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+			cudaMemcpyAsync(scratch + o_tmpl, tmpl.data(), tmpl.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+			cudaMemsetAsync(scratch + o_raw, 0, (size_t) n * raw_bytes, s) != cudaSuccess ||
+			cudaMemsetAsync(scratch + o_bad, 0, sizeof(int), s) != cudaSuccess) {
+			cuda_fail(domain, cudaGetLastError(), "jpeg encode setup");
+			break;
+		}
+		const EncodeTables *dT = (const EncodeTables *) (scratch + o_tab);
+		unsigned *freq = (unsigned *) (scratch + o_freq), *hat = (unsigned *) (scratch + o_hat), *hlen = (unsigned *) (scratch + o_hlen);
+		ProgHuff *huff = (ProgHuff *) (scratch + o_huff);
+		unsigned char *slots = (unsigned char *) (scratch + o_slots);
+		unsigned long long *lengths = (unsigned long long *) (scratch + o_len);
+		const int mcus = G.mcus_x * G.mcus_y;
+		cudaError_t e = cudaSuccess;
+		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
+			const int cn = std::min(kMaxBatchFrames, n - c0);
+			const unsigned char *fr = (const unsigned char *) frames + (size_t) c0 * frame_stride;
+			short *coef = (short *) (scratch + o_coef) + (size_t) c0 * G.blocks * 64;
+			unsigned char *summ = (unsigned char *) (scratch + o_summ) + (size_t) c0 * units;
+			unsigned *runs = (unsigned *) (scratch + o_runs) + (size_t) c0 * kProgSlotsPerUnit * units;
+			unsigned *dslot = (unsigned *) (scratch + o_dslot) + (size_t) c0 * units;
+			unsigned short *doff = (unsigned short *) (scratch + o_doff) + (size_t) c0 * units;
+			unsigned *bits = (unsigned *) (scratch + o_bits) + (size_t) c0 * nslots;
+			unsigned long long *totals = (unsigned long long *) (scratch + o_tot) + c0;
+			unsigned char *raw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
+			unsigned *counts = (unsigned *) (scratch + o_cnt) + (size_t) c0 * max_chunks;
+			unsigned *ist = (unsigned *) (scratch + o_ist) + (size_t) c0 * P.nseg;
+			unsigned char *dst = (unsigned char *) out + (size_t) c0 * out_stride;
+			const dim3 per_unit((unsigned) ((units + 127) / 128), cn), per_span((max_chunks + 127) / 128, cn);
+			jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, dT, fr, bpl, frame_stride, coef);
+			if ((e = cudaMemsetAsync(freq, 0, (size_t) cn * kMaxProgTables * 256 * sizeof(unsigned), s)) != cudaSuccess)
+				break;
+			jpeg_prog_summary_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, coef, summ, freq);
+			jpeg_prog_walk_kernel<<<dim3((P.nseg + 127) / 128, cn), 128, 0, s>>>(P, summ, runs, dslot, doff, freq);
+			jpeg_prog_huffopt_kernel<<<cn, 32 * kMaxProgTables, 0, s>>>(P, freq, huff, (const unsigned char *) (scratch + o_tmpl), slots, hat, hlen,
+				(int *) (scratch + o_bad));
+			jpeg_prog_count_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, huff, coef, runs, bits);
+			jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>((int) nslots, bits, totals);
+			jpeg_prog_segments_kernel<<<cn, 1024, 0, s>>>(P, bits, totals, ist);
+			jpeg_prog_emit_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, huff, ist, coef, bits, summ, runs, dslot, doff, (unsigned *) raw, raw_bytes / 4);
+			jpeg_prog_ffcount_kernel<<<per_span, 128, 0, s>>>(P, totals, raw, raw_bytes, max_chunks, ist, hat, counts);
+			jpeg_ffscan_kernel<true><<<cn, 1024, 0, s>>>(totals, max_chunks, counts, 0, hlen, lengths + c0);
+			jpeg_prog_stuff_kernel<<<per_span, 128, 0, s>>>(P, totals, raw, raw_bytes, max_chunks, counts, slots, hat, ist, dst, out_stride, lengths + c0);
+			e = cudaGetLastError();
+			if (e == cudaSuccess)
+				count_launch(11);
+		}
+		if (e != cudaSuccess) {
+			cuda_fail(domain, e, "jpeg encode kernels launch");
+			break;
+		}
+		std::vector<unsigned long long> len(n);
+		int bad = 0;
+		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+			cudaMemcpyAsync(&bad, scratch + o_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
+			cuda_fail(domain, cudaGetLastError(), "jpeg encode");
+			break;
+		}
+		if (bad) {
+			error(domain, "optimised Huffman table: a code longer than 32 bits");
+			break;
+		}
+		rc = 0;
+		for (int i = 0; i < n; i++) {
+			if (lengths_host)
+				lengths_host[i] = (size_t) len[i];
+			if (len[i] > out_stride) {
+				error(domain, "frame %d: the stream takes %llu bytes, the output stride is %zu", i, len[i], out_stride);
+				rc = -1;
+			}
+		}
+	} while (0);
+	dev_free(scratch, s);
+	return rc;
+}
+
 /* jpeg_gen_optimal_table on the host (libjpeg's own serial minimum search), for the host twin and its test hook */
 int
 host_optimal_table(unsigned *freq, unsigned char *bits, unsigned char *huffval)
@@ -1376,6 +2276,262 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
 	return 0;
 }
 
+/* jcphuff.c on the CPU, serially and in libjpeg's order, for one scan of the progressive script: encode_mcu_DC_first,
+ * encode_mcu_DC_refine, encode_mcu_AC_first, encode_mcu_AC_refine with emit_eobrun inline and emit_restart between
+ * restart intervals.  counts != null: the statistics pass (gather_statistics; finish_pass_gather_phuff's last
+ * emit_eobrun), counts[table of the scan][symbol]; else the output pass with the scan's tables co / si into out (stuffed,
+ * RSTn between intervals, finish_pass_phuff's flush).  Deliberately not the device's decomposition, which it checks.
+ */
+void
+host_prog_scan(const EncodeGeom &G, const ProgScan &S, const short *coef, int restart, unsigned (*counts)[257], const unsigned (*co)[256],
+	const unsigned char (*si)[256], std::vector<unsigned char> &out, unsigned long long *events)
+{
+	const bool gather = counts != nullptr;
+	unsigned long long put_buffer = 0;
+	int put_bits = 0;
+	auto emit_bits = [&](unsigned code, int size) {
+		if (gather)
+			return;
+		put_buffer = (put_buffer << size) | (code & ((1u << size) - 1));
+		put_bits += size;
+		while (put_bits >= 8) {
+			const unsigned char c = (unsigned char) (put_buffer >> (put_bits - 8));
+			out.push_back(c);
+			if (c == 0xFF)
+				out.push_back(0);
+			put_bits -= 8;
+		}
+	};
+	auto flush_bits = [&]() {
+		emit_bits(0x7F, 7); /* fill any partial byte with ones */
+		put_buffer = 0;
+		put_bits = 0;
+	};
+	auto emit_symbol = [&](int tbl, int symbol) {
+		if (gather)
+			counts[tbl][symbol]++;
+		else
+			emit_bits(co[tbl][symbol], si[tbl][symbol]);
+	};
+	int EOBRUN = 0, BE = 0;
+	char bit_buffer[kMaxCorrBits];
+	int last_dc_val[3] = {0, 0, 0};
+	auto emit_eobrun = [&]() {
+		if (EOBRUN > 0) {
+			int temp = EOBRUN, nbits = 0;
+			while ((temp >>= 1))
+				nbits++;
+			emit_symbol(0, nbits << 4);
+			if (nbits)
+				emit_bits((unsigned) EOBRUN, nbits);
+			EOBRUN = 0;
+			for (int i = 0; i < BE; i++)
+				emit_bits((unsigned) bit_buffer[i], 1);
+			BE = 0;
+		}
+	};
+	auto emit_restart = [&](int restart_num) {
+		emit_eobrun();
+		if (!gather) {
+			flush_bits();
+			out.push_back(0xFF);
+			out.push_back((unsigned char) (0xD0 + restart_num));
+		}
+		if (S.ss == 0)
+			last_dc_val[0] = last_dc_val[1] = last_dc_val[2] = 0;
+		else
+			EOBRUN = BE = 0;
+	};
+	auto nbits_of = [](int temp) {
+		int nbits = 0;
+		while (temp) {
+			nbits++;
+			temp >>= 1;
+		}
+		return nbits;
+	};
+	int restarts_to_go = restart, next_restart_num = 0;
+	for (int unit = 0; unit < S.units; unit++) {
+		if (restart) {
+			if (restarts_to_go == 0) {
+				emit_restart(next_restart_num);
+				restarts_to_go = restart;
+				next_restart_num = (next_restart_num + 1) & 7;
+			}
+			restarts_to_go--;
+		}
+		if (S.ss == 0) {
+			/* an interleaved MCU (a single block for greyscale) */
+			for (int blkn = 0; blkn < G.blocks_per_mcu; blkn++) {
+				const short *block = coef + ((size_t) unit * G.blocks_per_mcu + blkn) * 64;
+				const int ci = block_comp(G, blkn);
+				if (S.ah == 0) {
+					const int temp2 = block[0] >> S.al; /* IRIGHT_SHIFT: arithmetic */
+					int temp = temp2 - last_dc_val[ci];
+					last_dc_val[ci] = temp2;
+					int t2 = temp;
+					if (temp < 0) {
+						temp = -temp;
+						t2--;
+					}
+					const int nbits = nbits_of(temp);
+					emit_symbol(ci ? 1 : 0, nbits);
+					if (nbits)
+						emit_bits((unsigned) t2, nbits);
+				}
+				else
+					emit_bits((unsigned) (block[0] >> S.al), 1);
+			}
+			continue;
+		}
+		const short *block = coef + (size_t) comp_block_index(G, S.comp, unit % S.ux, unit / S.ux) * 64;
+		if (S.ah == 0) {
+			int r = 0;
+			for (int k = S.ss; k <= S.se; k++) {
+				int temp = block[kZz[k]], temp2;
+				if (temp == 0) {
+					r++;
+					continue;
+				}
+				if (temp < 0) {
+					temp = -temp;
+					temp >>= S.al;
+					temp2 = ~temp;
+				}
+				else {
+					temp >>= S.al;
+					temp2 = temp;
+				}
+				if (temp == 0) {
+					r++;
+					continue;
+				}
+				if (EOBRUN > 0)
+					emit_eobrun();
+				while (r > 15) {
+					emit_symbol(0, 0xF0);
+					r -= 16;
+				}
+				const int nbits = nbits_of(temp);
+				emit_symbol(0, (r << 4) + nbits);
+				emit_bits((unsigned) temp2, nbits);
+				r = 0;
+			}
+			if (r > 0) {
+				EOBRUN++;
+				if (EOBRUN == 0x7FFF) {
+					if (!gather)
+						events[0]++;
+					emit_eobrun();
+				}
+			}
+			continue;
+		}
+		int absvalues[64];
+		int EOB = 0;
+		for (int k = S.ss; k <= S.se; k++) {
+			int temp = block[kZz[k]];
+			if (temp < 0)
+				temp = -temp;
+			temp >>= S.al;
+			absvalues[k] = temp;
+			if (temp == 1)
+				EOB = k;
+		}
+		int r = 0, BR = 0;
+		char *BR_buffer = bit_buffer + BE;
+		for (int k = S.ss; k <= S.se; k++) {
+			int temp = absvalues[k];
+			if (temp == 0) {
+				r++;
+				continue;
+			}
+			while (r > 15 && k <= EOB) {
+				emit_eobrun();
+				if (!gather)
+					events[2]++;
+				emit_symbol(0, 0xF0);
+				r -= 16;
+				for (int i = 0; i < BR; i++)
+					emit_bits((unsigned) BR_buffer[i], 1);
+				BR_buffer = bit_buffer;
+				BR = 0;
+			}
+			if (temp > 1) {
+				BR_buffer[BR++] = (char) (temp & 1);
+				continue;
+			}
+			emit_eobrun();
+			emit_symbol(0, (r << 4) + 1);
+			emit_bits(block[kZz[k]] < 0 ? 0u : 1u, 1);
+			for (int i = 0; i < BR; i++)
+				emit_bits((unsigned) BR_buffer[i], 1);
+			BR_buffer = bit_buffer;
+			BR = 0;
+			r = 0;
+		}
+		if (r > 0 || BR > 0) {
+			EOBRUN++;
+			BE += BR;
+			if (EOBRUN == 0x7FFF || BE > kMaxCorrBits - 64 + 1) {
+				if (!gather)
+					events[EOBRUN == 0x7FFF ? 0 : 1]++;
+				emit_eobrun();
+			}
+		}
+	}
+	emit_eobrun();
+	if (!gather)
+		flush_bits();
+}
+
+/* the progressive stream on the CPU (test hook): libjpeg's multi-pass order, scan by scan a statistics pass, the scan's
+ * tables (jpeg_gen_optimal_table), its header (DHTs, DRI before the first scan, SOS) and the output pass.  events[3]
+ * counts what the output passes reach: EOB runs forced out at 0x7FFF blocks, EOB runs forced out by the correction-bit
+ * buffer, ZRLs in refinement scans.
+ */
+int
+host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
+	int restart, std::vector<unsigned char> &out, unsigned long long *events)
+{
+	EncodeGeom G;
+	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
+		return -1;
+	EncodeTables T;
+	make_tables(quality, &T);
+	std::vector<short> coef((size_t) G.blocks * 64);
+	for (int my = 0; my < G.mcus_y; my++)
+		for (int mx = 0; mx < G.mcus_x; mx++)
+			encode_mcu(G, T.q, img, bpl, mx, my, coef.data() + ((size_t) my * G.mcus_x + mx) * G.blocks_per_mcu * 64);
+	ProgScript P;
+	prog_script(G, restart, &P);
+	header_prefix(G, T, out, 0xFFC2);
+	for (int s = 0; s < P.nscans; s++) {
+		const ProgScan &S = P.s[s];
+		FrameHuff fh; /* tables 0, 1 of the scan */
+		if (S.nt) {
+			unsigned counts[2][257];
+			memset(counts, 0, sizeof(counts));
+			host_prog_scan(G, S, coef.data(), restart, counts, nullptr, nullptr, out, events);
+			for (int t = 0; t < S.nt; t++) {
+				unsigned char bits[17], huffval[256];
+				if (host_optimal_table(counts[t], bits, huffval)) {
+					error(domain, "optimised Huffman table: a code longer than 32 bits");
+					return -1;
+				}
+				derive_codes(bits + 1, huffval, fh.ehufco[t], fh.ehufsi[t]);
+				unsigned char seg[4 + 17 + 256];
+				const int n = put_dht(seg, P.tab_class[S.tab + t], bits, huffval);
+				out.insert(out.end(), seg, seg + n);
+			}
+		}
+		prog_scan_suffix(G, S, s == 0, restart, out);
+		host_prog_scan(G, S, coef.data(), restart, nullptr, fh.ehufco, fh.ehufsi, out, events);
+	}
+	put16(out, 0xFFD9);
+	return 0;
+}
+
 } // namespace vb200
 
 using namespace vb200;
@@ -1388,7 +2544,7 @@ extern "C" int
 vb200_debug_jpeg_encode(const void *pixels, size_t bpl, int width, int height, int bands, int quality, int subsample_mode, void *out, size_t cap,
 	size_t *len)
 {
-	const VB200JpegSaveOptions opt = {quality, subsample_mode, 0, 0};
+	const VB200JpegSaveOptions opt = {quality, subsample_mode, 0, 0, 0};
 	return vb200_debug_jpeg_encode_opts(pixels, bpl, width, height, bands, &opt, out, cap, len);
 }
 
@@ -1402,8 +2558,11 @@ vb200_debug_jpeg_encode_opts(const void *pixels, size_t bpl, int width, int heig
 		return -1;
 	}
 	std::vector<unsigned char> o;
-	if (host_jpeg_encode("jpeg_encode (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, opt->Q, opt->subsample_mode,
-			opt->optimize_coding, opt->restart_interval, o))
+	unsigned long long events[3] = {0, 0, 0};
+	if (opt->interlace ? host_jpeg_encode_progressive("jpeg_encode (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, opt->Q,
+							 opt->subsample_mode, opt->restart_interval, o, events)
+					   : host_jpeg_encode("jpeg_encode (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, opt->Q,
+							 opt->subsample_mode, opt->optimize_coding, opt->restart_interval, o))
 		return -1;
 	if (len)
 		*len = o.size();
@@ -1413,6 +2572,24 @@ vb200_debug_jpeg_encode_opts(const void *pixels, size_t bpl, int width, int heig
 	}
 	memcpy(out, o.data(), o.size());
 	return 0;
+}
+
+/* Test hook, host only: what the host twin's progressive coder reached for an image (options as
+ * vb200_debug_jpeg_encode_opts, interlace implied): events[0] EOB runs forced out at 0x7FFF blocks, [1] EOB runs forced out
+ * by the correction-bit buffer (BE > MAX_CORR_BITS - 63), [2] ZRLs in refinement scans
+ */
+extern "C" int
+vb200_debug_jpeg_prog_events(const void *pixels, size_t bpl, int width, int height, int bands, const VB200JpegSaveOptions *opt,
+	unsigned long long *events)
+{
+	if (!opt || !events) {
+		error("jpeg_prog_events (host twin)", "null argument");
+		return -1;
+	}
+	std::vector<unsigned char> o;
+	events[0] = events[1] = events[2] = 0;
+	return host_jpeg_encode_progressive("jpeg_prog_events (host twin)", (const unsigned char *) pixels, bpl, width, height, bands, opt->Q,
+		opt->subsample_mode, opt->restart_interval, o, events);
 }
 
 /* Test hook, host only: jpeg_gen_optimal_table (jchuff.c) on the symbol counts freq[256] -> bits[17] (bits[0] unused),
@@ -1446,7 +2623,7 @@ extern "C" int
 vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands, int Q,
 	int subsample_mode, void *out, int out_location, size_t out_stride, size_t *lengths)
 {
-	const VB200JpegSaveOptions opt = {Q, subsample_mode, 0, 0};
+	const VB200JpegSaveOptions opt = {Q, subsample_mode, 0, 0, 0};
 	return vb200_jpegsave_batch_opts(frames, frames_location, bpl, frame_stride, n, width, height, bands, &opt, out, out_location, out_stride,
 		lengths);
 }
@@ -1501,8 +2678,10 @@ vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, s
 			dst = dout;
 		}
 		std::vector<size_t> len(n);
-		if (dev_jpeg_encode_batch(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->optimize_coding != 0,
-				opt->restart_interval, dst, out_stride, len.data(), s))
+		if (opt->interlace ? dev_jpeg_encode_progressive(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->restart_interval,
+								 dst, out_stride, len.data(), s)
+						   : dev_jpeg_encode_batch(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->optimize_coding != 0,
+								 opt->restart_interval, dst, out_stride, len.data(), s))
 			break;
 		if (lengths)
 			memcpy(lengths, len.data(), n * sizeof(size_t));

@@ -2,8 +2,9 @@
 
     python tools/bench_jpegsave.py [--frames 512] [--size 512] [--steps 10] [--cpu-frames 64]
 
-512 seeded, photo-like 512 x 512 RGB frames resident on the device, encoded into device memory at Q 75 and Q 90 in four
-configurations: default, optimize_coding, restart_interval = one MCU row, and both.  Each batch call is timed with CUDA
+512 seeded, photo-like 512 x 512 RGB frames resident on the device, encoded into device memory at Q 75 and Q 90 in six
+configurations: default, optimize_coding, restart_interval = one MCU row, both, and progressive (interlace) without and
+with restart_interval = one MCU row.  Each batch call is timed with CUDA
 events after a warm-up call; ms is the median over --steps calls.  Per configuration it prints ms per batch, frames/s,
 the kernel launches one call makes (vb.launch_count) and the mean stream size relative to the default configuration.
 Beside it, Pillow (libjpeg-turbo) with the same options over the host's cores, one frame per task, as the CPU
@@ -40,11 +41,13 @@ def card():
 
 def pil_one(args):
     from PIL import Image
-    a, q, opt, r = args
+    a, q, opt, r, il = args
     b = io.BytesIO()
     kw = {"optimize": True} if opt else {}
     if r:
         kw["restart_marker_blocks"] = r
+    if il:
+        kw["progressive"] = True
     Image.fromarray(a).save(b, "JPEG", quality=q, subsampling=2 if q < 90 else 0, **kw)
     return len(b.getvalue())
 
@@ -77,8 +80,9 @@ def main():
         mcu = 16 if q < 90 else 8
         row = (s + mcu - 1) // mcu
         base_bytes = None
-        for name, opt, r in (("default", 0, 0), ("optimize", 1, 0), ("restart_row", 0, row), ("optimize+restart_row", 1, row)):
-            opts = vb.JpegSaveOptions(q, 0, opt, r)
+        for name, opt, r, il in (("default", 0, 0, 0), ("optimize", 1, 0, 0), ("restart_row", 0, row, 0), ("optimize+restart_row", 1, row, 0),
+                                 ("interlace", 0, 0, 1), ("interlace+restart_row", 0, row, 1)):
+            opts = vb.JpegSaveOptions(q, 0, opt, r, il)
             call(opts)                                   # warm-up
             torch.cuda.synchronize()
             before = vb.launch_count()
@@ -97,13 +101,13 @@ def main():
                 times.append(a.elapsed_time(b))
             ms = float(np.median(times))
             cpu_n = min(args.cpu_frames, n)
-            work = [(host[i], q, opt, r) for i in range(cpu_n)]
+            work = [(host[i], q, opt, r, il) for i in range(cpu_n)]
             list(pool.map(pil_one, work[:4]))            # start the workers
             t0 = time.perf_counter()
             list(pool.map(pil_one, work))
             cpu_fps = cpu_n / (time.perf_counter() - t0)
             print(json.dumps(dict(info, workload="jpegsave %d x %dx%d RGB, device in/out" % (n, s, s), Q=q, config=name,
-                                  optimize_coding=opt, restart_interval=r, ms_per_batch=round(ms, 3), frames_per_s=round(n / ms * 1e3, 1),
+                                  optimize_coding=opt, restart_interval=r, interlace=il, ms_per_batch=round(ms, 3), frames_per_s=round(n / ms * 1e3, 1),
                                   launches_per_call=launches, mean_bytes=round(mean_bytes, 1),
                                   bytes_vs_default=round(mean_bytes / base_bytes, 4), pillow_frames_per_s=round(cpu_fps, 1),
                                   pillow_workers=os.cpu_count())), flush=True)

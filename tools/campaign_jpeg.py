@@ -89,10 +89,11 @@ def main():
             if got.shape != want.shape or not np.array_equal(got, want):
                 bad += 1
                 print("DECODE MISMATCH", (h, w, grey, q, sub, kw, shrink), got.shape, want.shape, flush=True)
-        # the encoder: baseline, 4:2:0 or 4:4:4, standard or optimised tables, restart intervals of 0, 1, 2, a few MCUs,
-        # or at least the MCU count
+        # the encoder: baseline or progressive, 4:2:0 or 4:4:4, standard or optimised tables, restart intervals of 0, 1, 2,
+        # a few MCUs, or at least the MCU count
         cap = w * h * 8 + 3 * w * h // 16 + 8192
         opt = int(rng.random() < 0.5)
+        interlace = int(rng.random() < 0.5)
         rmode = int(rng.integers(0, 5))
         mcus = ((w + 7) // 8) * ((h + 7) // 8)      # at least the MCU count of every sampling
         restart = [0, 1, 2, int(rng.integers(3, 12)), mcus + int(rng.integers(0, 3))][rmode]
@@ -101,11 +102,13 @@ def main():
             ekw["optimize"] = True
         if restart:
             ekw["restart_marker_blocks"] = restart
+        if interlace:
+            ekw["progressive"] = True
         buf = (C.c_ubyte * cap)()
         n = C.c_size_t()
         bands = 1 if grey else 3
         for mode, pil_sub in ((1, 2), (2, 0)) if not grey else ((0, None),):
-            opts = vb.JpegSaveOptions(q, mode, opt, restart)
+            opts = vb.JpegSaveOptions(q, mode, opt, restart, interlace)
             rc = L.vb200_debug_jpeg_encode_opts(a.ctypes.data_as(C.c_void_p), w * bands, w, h, bands, C.byref(opts), buf, cap, C.byref(n))
             if rc:
                 declined += 1
@@ -120,7 +123,7 @@ def main():
             enc += 1
             if ours != t.getvalue():
                 bad += 1
-                print("ENCODE MISMATCH", (h, w, grey, q, mode, opt, restart), len(ours), len(t.getvalue()), flush=True)
+                print("ENCODE MISMATCH", (h, w, grey, q, mode, opt, restart, interlace), len(ours), len(t.getvalue()), flush=True)
     print("jpeg campaign: %d decodes, %d encodes, %d declined, %d mismatches" % (dec, enc, declined, bad))
 
 
