@@ -523,11 +523,17 @@ int vb200_debug_mma_tables(int in_size, double shrink, int rect_size, int *int_s
  * bytes are all that crosses PCIe.  libjpeg(-turbo) itself is a third-party dependency outside the reference
  * tree; its algorithm for the reference's configuration (JDCT_ISLOW, 8-bit Huffman, sequential and progressive)
  * is restated in csrc/jpeg.cu and pinned bit for bit to the libjpeg-turbo inside this image's Pillow
- * (tests/test_jpeg.py).  Decoded: 8-bit Huffman streams, baseline / extended sequential and progressive, greyscale or
- * YCbCr at 4:4:4, 4:2:2 and 4:2:0, at shrink 1 / 2 / 4 / 8 (where libjpeg's upsampler has work left -- 4:2:0 at full
- * size, 4:2:2 -- its h2v2 / h2v1 "fancy" triangle filters, jdsample.c).  Arithmetic-coded, 12-bit, CMYK / RGB-coded and
- * 4:4:0 / 4:1:1 streams return -1 (host loader).  Baseline streams with restart markers decode one interval per GPU
- * thread, those without by self-synchronising subsequences; progressive streams one scan after the other.
+ * (tests/test_jpeg.py, tests/test_jpeg_layouts.py).  Decoded: 8-bit Huffman streams, baseline / extended sequential (one
+ * interleaved scan) and progressive, greyscale (whatever sampling its frame header declares) or YCbCr with sampling
+ * factors 1 or 2 in which Y has the largest factor both ways and each chroma component is at Y's resolution, halved
+ * across, or halved both ways: 4:4:4, 4:2:2, 4:2:0, every component 2x1, every component 1x2, Y 2x2 over chroma 1x2 --
+ * at shrink 1 / 2 / 4 / 8 (where libjpeg's upsampler has work left, its h2v2 / h2v1 "fancy" triangle filters,
+ * jdsample.c).  At shrink 2 / 4 / 8 also Y 1x1 under 2x2 chroma, which libjpeg's scaled IDCT brings to Y's size.
+ * Everything else returns -1 (host loader): arithmetic-coded, 12-bit, CMYK / RGB-coded streams, sequential streams with
+ * a scan per component, factors above 2 (4:1:1), chroma halved only vertically (4:4:0: libjpeg's h1v2 upsampler), Y
+ * that would need upsampling, and interleaved scans of more than 10 blocks per MCU (2x2 in all three components:
+ * T.81 B.2.3, libjpeg refuses them too).  Baseline streams with restart markers decode one interval per GPU thread,
+ * those without by self-synchronising subsequences; progressive streams one scan after the other.
  *
  * vb200_jpeg_decode_batch: n streams of ONE output geometry -> out[n][height][width][bands] uchar (bands 1 or 3),
  *   out in host or device memory (out_location VB200_HOST / VB200_DEVICE); out = NULL only reports the geometry.

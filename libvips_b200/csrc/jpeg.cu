@@ -122,7 +122,8 @@ struct JpegFrameDev {
 	int out_w, out_h, tile_w, tile_h; /* cropped output, and the MCU's footprint in output pixels */
 	int blocks_per_mcu;				  /* T.81 A.2.3: component by component, rows of blocks, left to right */
 	unsigned char blk_comp[12], blk_dx[12], blk_dy[12];
-	/* frames that need libjpeg's upsampler (4:2:0 at full size, 4:2:2): components are reconstructed into planes first */
+	/* frames that need libjpeg's upsampler (4:2:0 at full size, 4:2:2), or whose MCU is larger than reconstruct_mcu's tile:
+	 * components are reconstructed into planes first */
 	int planar;								 /* 1: jpeg_idct_planes_kernel + jpeg_upsample_kernel instead of jpeg_idct_kernel */
 	int fancy;								 /* jinit_upsampler: do_fancy_upsampling && min_DCT_scaled_size > 1 */
 	int ux[kMaxComp], uy[kMaxComp];			 /* upsampling factors 1 / 2 */
@@ -477,6 +478,24 @@ plan_frame(const char *domain, const JpegHeader &H, int shrink, int dct[kMaxComp
 		}
 		up[c][0] = ux;
 		up[c][1] = uy;
+	}
+	/* T.81 B.2.3: the MCU of an interleaved scan holds at most 10 blocks, and libjpeg refuses a frame with more ("Sampling
+	 * factors too large for interleaved scan"): 2x2 in all three components is 12
+	 */
+	int mcu_blocks = 0;
+	if (!H.progressive && H.ncomp > 1)
+		for (int c = 0; c < H.ncomp; c++)
+			mcu_blocks += H.comp[c].h * H.comp[c].v;
+	for (const JpegScan &sc : H.scans)
+		if (sc.ns > 1) {
+			int n = 0;
+			for (int i = 0; i < sc.ns; i++)
+				n += H.comp[sc.ci[i]].h * H.comp[sc.ci[i]].v;
+			mcu_blocks = std::max(mcu_blocks, n);
+		}
+	if (mcu_blocks > 10) {
+		error(domain, "JPEG interleaved scan of %d blocks per MCU: T.81 allows 10", mcu_blocks);
+		return -1;
 	}
 	return 0;
 }
@@ -1355,13 +1374,16 @@ ycc_to_rgb(int y, int cb, int cr, unsigned char *rgb)
 }
 
 /* One MCU: IDCT of every block of every component into a tile of tile_w x tile_h samples per component (the
- * upsampler is the identity in every supported case), colour conversion, store of the part inside the crop.
+ * upsampler is the identity, and the tile at most kTileSamples: frame_prep sends every other frame to the planar path),
+ * colour conversion, store of the part inside the crop.
  */
+constexpr int kTileSamples = 64;
+
 HD void
 reconstruct_mcu(const JpegFrameDev &F, const unsigned short (*qt)[64], const short *coef_pool, int mx, int my, unsigned char *out,
 	size_t out_bpl)
 {
-	unsigned char tile[kMaxComp][64];
+	unsigned char tile[kMaxComp][kTileSamples];
 	const int tw = F.tile_w, th = F.tile_h;
 	for (int c = 0; c < F.ncomp; c++)
 		for (int by = 0; by < F.v[c]; by++)
@@ -1781,6 +1803,11 @@ frame_prep(const char *domain, const unsigned char *d, size_t len, int shrink, F
 		F.plane_off[c] = P->plane_bytes;
 		P->plane_bytes += ((size_t) F.pw[c] * F.ph[c] + 15) & ~(size_t) 15;
 	}
+	/* reconstruct_mcu holds an MCU in tile[kMaxComp][kTileSamples]: a larger one (every component 2x1, 1x2 or 2x2 at full
+	 * size, where the upsampler is the identity) goes through the planes, in which an identity upsampler is a copy
+	 */
+	if (F.tile_w * F.tile_h > kTileSamples)
+		F.planar = 1;
 	if (!F.planar)
 		P->plane_bytes = 0;
 	F.blocks_per_mcu = 0;
