@@ -517,6 +517,15 @@ int vb200_debug_mma_tables(int in_size, double shrink, int rect_size, int *int_s
 	int *n_point, int *embed, int *first, int *phase, short *mask65, int *vchunk, unsigned *bfrag, int cap_rows,
 	int *rows_per_chunk);
 
+/* Test hook, host only (no GPU, no CUDA call): the bands of the tensor-pipe thumbnail kernel for a width x height
+ * RGBA uchar frame thumbnailed to target_width (VB200_SIZE_BOTH), exactly as a plan lays them out.  Band b writes
+ * output columns [xa[b], xb[b]) and reads input columns [c_lo[b], c_hi[b]); seam[b] (b < n_bands - 1) is how many input
+ * columns bands b and b + 1 both read.  A TMA stage row is *n_box boxes of *box_width pixels.  Caller-sized arrays
+ * [cap].  0 = ok, 1 = the plan does not use the tensor-pipe kernel, -1 = bad arguments.
+ */
+int vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_width, int *n_bands, int *xa, int *xb,
+	int *c_lo, int *c_hi, int *seam, int cap, int *box_width, int *n_box);
+
 /* ------------------------------------------------------------------ JPEG decode staging (SURVEY 8f rank 1)
  * vips_jpegload_buffer(buf, len, &out, "shrink", shrink) (foreign/jpeg2vips.c:532-538, 631-640: scale_num = 1,
  * scale_denom = shrink, output cropped to floor(size / shrink)) with the decoder on the device: the compressed

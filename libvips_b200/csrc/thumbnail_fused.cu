@@ -91,6 +91,14 @@ struct FusedParams {
 	double max_alpha; /* LUTs are derived from it in the prologue */
 };
 
+/* One band of the tensor-pipe kernel: output columns [xa, xb), ne embedded shrinkh columns, and the input columns
+ * [c_lo, c_hi) its stage rows load (c_lo on the layout's box alignment, c_hi on 16 bytes) -- what
+ * thumbnail_fused_mma.cuh derives from column_of
+ */
+struct MmaBand {
+	int xa, xb, ne, c_lo, c_hi;
+};
+
 __device__ __forceinline__ int
 dp2a_lo(unsigned coef, unsigned bytes, int acc)
 {
@@ -1426,7 +1434,10 @@ struct ThumbnailPlanImpl {
 	/* v4: reducev on the integer tensor pipe */
 	bool mma_ok = false;
 	int mma_cols = 0, mma_cpt = 1, mma_tw = 0, mma_nt = 0, mma_nemax = 0;
+	std::vector<MmaBand> mma_bands; /* the bands of mma_tw over a frame row */
 	size_t smem_mma = 0;
+	/* plan the geometry only: no device tables (vb200_debug_thumbnail_bands) */
+	bool geometry_only = false;
 	void *tables_mma = nullptr;
 	/* host pump */
 	static constexpr int kStreams = 3;
@@ -1608,7 +1619,7 @@ launch_tma3(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, co
 }
 
 /* A tiled tensor map over the batch: u64 elements (2 pixels), dims {W / 2, H, frames}, box
- * {(WCOLS + 8) / 2, rows, 1}: one cp.async.bulk.tensor per TMA stage.  Returns false when
+ * {v4_boxw(WCOLS, HS) / 2, rows, 1}: one cp.async.bulk.tensor per TMA stage.  Returns false when
  * the driver entry point or the geometry is not usable; the kernel then copies row by row.
  */
 bool
@@ -1775,7 +1786,7 @@ launch_mma_t(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, c
 {
 	CUtensorMap tm;
 	memset(&tm, 0, sizeof(tm));
-	const int use_tmap = make_stage_tensor_map(&tm, in, fp.W, fp.H, fp.in_bpl, in_stride, n, (WCOLS + 8) / (WCOLS + 8 > 512 ? 2 : 1), 2 * VS) ? 1 : 0;
+	const int use_tmap = make_stage_tensor_map(&tm, in, fp.W, fp.H, fp.in_bpl, in_stride, n, v4_boxw(WCOLS, HSQ), 2 * VS) ? 1 : 0;
 	/* the opaque-stage vote exists for the configuration real batches run: premultiplied, 768-column bands */
 	constexpr bool CAN_OPQ = PREMUL && CPT == 2 && WCOLS > 448;
 	for (int f0 = 0; f0 < n; f0 += 32768) {
@@ -1919,6 +1930,32 @@ plan_axis_tables(const ThumbnailPlanImpl *pl, AxisTable &tv, AxisTable &th)
 		rect_h = std::min(rect_h, tg.fatstrip_height);
 	build_axis_table(tv, pl->OH, pl->gv.residual, pl->gv.offset, pl->gv.n_point, VB200_KERNEL_LANCZOS3, rect_h);
 	build_axis_table(th, pl->OW, pl->gh.residual, pl->gh.offset, pl->gh.n_point, VB200_KERNEL_LANCZOS3, tile_w);
+}
+
+/* The tensor-pipe kernel's bands at band width tw (the last one shorter), with the input columns each loads in the
+ * wcols-column layout
+ */
+std::vector<MmaBand>
+mma_bands_of(const FusedParams &fp, const std::vector<int2> &hcol, int tw, int wcols)
+{
+	auto column_of = [&](int E0, int tt) {
+		const int e = E0 + tt / fp.HS;
+		const int k = tt % fp.HS;
+		const int sc = std::max(0, std::min(e - fp.hembed, fp.Ws - 1));
+		return std::min(sc * fp.HS + k, fp.W - 1);
+	};
+	std::vector<MmaBand> bands;
+	for (int xa = 0; xa < fp.OW; xa += tw) {
+		MmaBand b;
+		b.xa = xa;
+		b.xb = std::min(xa + tw, fp.OW);
+		const int E0 = 2 * hcol[xa].x + fp.hgrid;
+		b.ne = 2 * (hcol[b.xb - 1].x + fp.NPh - hcol[xa].x);
+		b.c_lo = column_of(E0, 0) & ~(v4_clo_align(wcols, fp.HS) - 1);
+		b.c_hi = std::min(fp.W, (column_of(E0, b.ne * fp.HS - 1) + 4) & ~3);
+		bands.push_back(b);
+	}
+	return bands;
 }
 
 int
@@ -2113,13 +2150,7 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 		 */
 		const int warp_cols = hpow2 ? 0 : 2 * (32 / fp.HS) * fp.HS;
 		pl->mma_cpt = wcols > 448 || (getenv("VB200_V4_CPT") && atoi(getenv("VB200_V4_CPT")) == 2) ? 2 : 1; /* columns per V thread */
-		const int pitch = (wcols + 8) * 4;
-		auto column_of = [&](int E0, int tt) {
-			const int e = E0 + tt / fp.HS;
-			const int k = tt % fp.HS;
-			const int sc = std::max(0, std::min(e - fp.hembed, fp.Ws - 1));
-			return std::min(sc * fp.HS + k, fp.W - 1);
-		};
+		const int pitch = v4_nbox(wcols, fp.HS) * v4_boxw(wcols, fp.HS) * 4;
 		/* band width: the one that needs the fewest V warps over a frame row (warps past a band's last
 		 * column exit at once, so a narrow last band is cheap); ties go to the wider band
 		 */
@@ -2130,15 +2161,10 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 		for (int tw = std::min(pl->OW, 256); tw >= 2 && ok; tw--) {
 			int worst = 0, max_cols = 0;
 			long cost = 0;
-			for (int xa = 0; xa < pl->OW; xa += tw) {
-				const int xb = std::min(xa + tw, pl->OW);
-				const int E0 = 2 * hcol[xa].x + hgrid;
-				const int ne = 2 * (hcol[xb - 1].x + fp.NPh - hcol[xa].x);
-				const int c_lo = column_of(E0, 0) & ~3;
-				const int c_hi = std::min(fp.W, (column_of(E0, ne * fp.HS - 1) + 4) & ~3);
-				worst = std::max(worst, ne);
-				max_cols = std::max(max_cols, c_hi - c_lo);
-				cost += (ne * fp.HS + cols_per_warp - 1) / cols_per_warp + 1; /* + the H / P warps' share */
+			for (const MmaBand &b : mma_bands_of(fp, hcol, tw, wcols)) {
+				worst = std::max(worst, b.ne);
+				max_cols = std::max(max_cols, b.c_hi - b.c_lo);
+				cost += (b.ne * fp.HS + cols_per_warp - 1) / cols_per_warp + 1; /* + the H / P warps' share */
 			}
 			if (worst * fp.HS <= col_budget && max_cols * 4 <= pitch && cost < best_cost) {
 				best_cost = cost;
@@ -2155,7 +2181,8 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 			const int stages = fp.VS <= 2 ? 2 * VB200_V4_STAGES
 				: (fp.VS >= 7 ? VB200_V4_STAGES / 2 : (fp.VS >= 5 ? (3 * VB200_V4_STAGES) / 4 : VB200_V4_STAGES));
 			const int logical_cols = warp_cols ? (pl->mma_nt / 32) * warp_cols : pl->mma_nt * pl->mma_cpt;
-			const int nbox = wcols + 8 > 512 ? 2 : 1;
+			pl->mma_bands = mma_bands_of(fp, hcol, tw4, wcols);
+			const int nbox = v4_nbox(wcols, fp.HS);
 			const size_t box_bytes = ((size_t) 2 * fp.VS * (pitch / nbox) + 127) & ~(size_t) 127;
 			pl->smem_mma = (size_t) stages * nbox * box_bytes + (2 * stages + 4) * 8 +
 				(size_t) kV4Quads * ((size_t) pl->mma_nt * pl->mma_cpt * 16 + 16) +
@@ -2163,15 +2190,19 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 				(size_t) (fp.nhsets * fp.NPh + 256) * 4;
 			const size_t n_ch = vchunk.size() * sizeof(int2), n_bf = bfrag.size() * sizeof(uint4);
 			if (pl->smem_mma <= (wcols > 448 ? 226 : 113) * 1024) {
-				VB200_CUDA(domain, cudaMalloc(&pl->tables_mma, n_bf + n_ch));
-				VB200_CUDA(domain, cudaMemcpy(pl->tables_mma, bfrag.data(), n_bf, cudaMemcpyHostToDevice));
-				VB200_CUDA(domain, cudaMemcpy((char *) pl->tables_mma + n_bf, vchunk.data(), n_ch, cudaMemcpyHostToDevice));
-				fp.vbfrag = (const uint4 *) pl->tables_mma;
-				fp.vchunk = (const int2 *) ((char *) pl->tables_mma + n_bf);
+				if (!pl->geometry_only) {
+					VB200_CUDA(domain, cudaMalloc(&pl->tables_mma, n_bf + n_ch));
+					VB200_CUDA(domain, cudaMemcpy(pl->tables_mma, bfrag.data(), n_bf, cudaMemcpyHostToDevice));
+					VB200_CUDA(domain, cudaMemcpy((char *) pl->tables_mma + n_bf, vchunk.data(), n_ch, cudaMemcpyHostToDevice));
+					fp.vbfrag = (const uint4 *) pl->tables_mma;
+					fp.vchunk = (const int2 *) ((char *) pl->tables_mma + n_bf);
+				}
 				pl->mma_ok = true;
 			}
 		}
 	}
+	if (pl->geometry_only)
+		return 0;
 
 	/* upload tables as one block */
 	const size_t n_vrow = vrow.size() * sizeof(int2), n_hcol = hcol.size() * sizeof(int2);
@@ -3220,4 +3251,44 @@ vb200_thumbnail_image_linear_icc(const VB200Image *in, VB200Image *out, int widt
 	const void *embedded, size_t embedded_len)
 {
 	return thumbnail_image_run(in, out, width, height, size, 1, icc, embedded, embedded_len, true);
+}
+
+/* Test hook (tests/test_thumbnail_bands.py, CPU): the tensor-pipe kernel's bands of an RGBA thumbnail plan, planned
+ * without a device.  See vb200.h.
+ */
+extern "C" int
+vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_width, int *n_bands, int *xa, int *xb,
+	int *c_lo, int *c_hi, int *seam, int cap, int *box_width, int *n_box)
+{
+	if (width <= 0 || height <= 0 || target_width <= 0 || cap <= 0)
+		return -1;
+	ThumbnailPlanImpl pl;
+	pl.W = width;
+	pl.H = height;
+	pl.bands = 4;
+	pl.fmt = VB200_FORMAT_UCHAR;
+	pl.has_alpha = 1;
+	pl.target_w = pl.target_h = target_width;
+	pl.size = VB200_SIZE_BOTH;
+	pl.geometry_only = true;
+	if (thumbnail_plan_init("debug_thumbnail_bands", &pl))
+		return -1;
+	if (!pl.fused || !pl.mma_ok)
+		return 1;
+	const int nb = (int) pl.mma_bands.size();
+	if (nb > cap)
+		return -1;
+	*out_width = pl.OW;
+	*n_bands = nb;
+	for (int b = 0; b < nb; b++) {
+		const MmaBand &m = pl.mma_bands[b];
+		xa[b] = m.xa;
+		xb[b] = m.xb;
+		c_lo[b] = m.c_lo;
+		c_hi[b] = m.c_hi;
+		seam[b] = b + 1 < nb ? std::max(0, m.c_hi - pl.mma_bands[b + 1].c_lo) : 0;
+	}
+	*n_box = v4_nbox(pl.mma_cols, pl.fp.HS); /* the boxes launch_mma_t gives the stage tensor map */
+	*box_width = v4_boxw(pl.mma_cols, pl.fp.HS);
+	return 0;
 }

@@ -108,6 +108,41 @@ struct V4HWarpsW {
 	static constexpr int value = WCOLS > 448 ? VB200_V4_NH768 : V4HWarps<CPT>::value;
 };
 
+/* A stage row is loaded as v4_nbox tiled-TMA boxes of v4_boxw pixels (a box is at most 256 u64 = 512 pixels wide),
+ * from the band's first input column rounded down to v4_clo_align pixels.  In the 768-column layout a row starts on a
+ * 128-byte line and is 13 whole lines per box (2 x 416 pixels): the same bands fed from 16-byte-aligned columns in
+ * 2 x 388-pixel boxes ran 2.8% slower on an H100 (12.54 against 12.19 ms per 512 4K frames), because rows that start
+ * or end inside a line cost the L2 and DRAM partial lines.  Where the shared memory has no room for that -- the
+ * 384-column layout (2 CTAs per SM) and a horizontal box of 2 (sh buffers twice as large) -- rows stay 392 / 776
+ * pixels from 16-byte columns.
+ */
+#ifndef VB200_V4_BOXPAD
+#define VB200_V4_BOXPAD 64 /* pixels of a line-aligned stage row beyond the band's column budget */
+#endif
+#ifndef VB200_V4_CLO_ALIGN
+#define VB200_V4_CLO_ALIGN 32 /* pixels, a power of two: 32 = one 128-byte line */
+#endif
+constexpr bool
+v4_lines(int wcols, int hs)
+{
+	return wcols > 448 && hs > 2;
+}
+constexpr int
+v4_clo_align(int wcols, int hs)
+{
+	return v4_lines(wcols, hs) ? VB200_V4_CLO_ALIGN : 4;
+}
+constexpr int
+v4_nbox(int wcols, int hs)
+{
+	return wcols + (v4_lines(wcols, hs) ? VB200_V4_BOXPAD : 8) > 512 ? 2 : 1;
+}
+constexpr int
+v4_boxw(int wcols, int hs)
+{
+	return (wcols + (v4_lines(wcols, hs) ? VB200_V4_BOXPAD : 8)) / v4_nbox(wcols, hs);
+}
+
 template <int VS>
 struct V4Stages {
 	/* a stage is 2 VS input rows: 8 stages of 4 rows, 4 of 6 / 8, 3 of 10 / 12, 2 of 14 / 16 keep the ring near 100 KB */
@@ -169,8 +204,9 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	constexpr int NH = V4HWarpsW<WCOLS, CPT>::value;
 	constexpr int kMmaUnroll = VB200_V4_MMA_UNROLL;
 	/* a stage row is held as NBOX column boxes (a tiled-TMA box is at most 256 elements = 512 pixels wide) */
-	constexpr int NBOX = WCOLS + 8 > 512 ? 2 : 1;
-	constexpr int BOXW = (WCOLS + 8) / NBOX; /* pixels; even, a multiple of 4 */
+	constexpr int NBOX = v4_nbox(WCOLS, HSQ);
+	constexpr int BOXW = v4_boxw(WCOLS, HSQ); /* pixels */
+	static_assert(BOXW % 4 == 0 && BOXW <= 512, "a box row is whole 16-byte units, at most 256 u64 elements");
 	constexpr int PITCH = BOXW * 4;			 /* bytes between rows of a box */
 	constexpr int NPR = NP > 0 ? NP : 1;
 	constexpr int HSHIFT = HSQ == 2 ? 1 : HSQ == 4 ? 2 : 3;
@@ -227,7 +263,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 		const int sc = max(0, min(e - P.hembed, P.Ws - 1));
 		return min(sc * HSQ + k, P.W - 1);
 	};
-	const int c_lo = column_of(0) & ~3;
+	const int c_lo = column_of(0) & ~(v4_clo_align(WCOLS, HSQ) - 1);
 	const int c_hi = min(P.W, (column_of(NE * HSQ - 1) + 4) & ~3);
 	const unsigned row_bytes = (unsigned) (c_hi - c_lo) * 4u;
 	const int chunk0 = y_begin / K; /* RPC is a multiple of K: chunk c of this CTA is table entry chunk0 + c */
