@@ -318,8 +318,10 @@ int vb200_thumbnail_plan_is_fused(const VB200ThumbnailPlan *plan);
 /* Algorithmic HBM bytes one frame moves through the fused kernel. */
 size_t vb200_thumbnail_plan_bytes_per_frame(const VB200ThumbnailPlan *plan);
 /* Which kernel a batch call of this plan launches (for bench / profile labels): a
- * static string such as "thumbnail_fused_mma_kernel<VS=4,NP=6,premul,HS=4,cols=384,cpt=1>",
- * or "leaf kernels" for an unfused plan.
+ * static string such as "thumbnail_fused_mma_kernel<VS=4,NP=6,premul,HS=4,cols=768,cpt=2>",
+ * or "leaf kernels" for an unfused plan.  The plan chooses the kernel once; the one exception is a
+ * batch whose base pointer, or whose frame stride (with more than one frame), is not a multiple of
+ * 16 bytes: it runs thumbnail_fused_kernel (the ld.global kernel) with the same pixels.
  */
 const char *vb200_thumbnail_plan_kernel(const VB200ThumbnailPlan *plan);
 
@@ -525,6 +527,13 @@ int vb200_debug_mma_tables(int in_size, double shrink, int rect_size, int *int_s
  */
 int vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_width, int *n_bands, int *xa, int *xb,
 	int *c_lo, int *c_hi, int *seam, int cap, int *box_width, int *n_box);
+/* Test hook, host only (no GPU, no CUDA call): the name vb200_thumbnail_plan_kernel gives the plan
+ * vb200_thumbnail_plan_new(width, height, bands, VB200_FORMAT_UCHAR, has_alpha, target_width, target_height, size, 0) would
+ * build, written to name[cap] with its terminating NUL ("leaf kernels" for an unfused plan).  0 = ok, -1 = bad arguments,
+ * a plan that fails, or a name longer than cap - 1.
+ */
+int vb200_debug_thumbnail_kernel(int width, int height, int bands, int has_alpha, int target_width, int target_height, int size,
+	char *name, int cap);
 
 /* ------------------------------------------------------------------ JPEG decode staging (SURVEY 8f rank 1)
  * vips_jpegload_buffer(buf, len, &out, "shrink", shrink) (foreign/jpeg2vips.c:532-538, 631-640: scale_num = 1,

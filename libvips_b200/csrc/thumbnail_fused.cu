@@ -60,7 +60,7 @@ struct FusedParams {
 	int NPv;	  /* coefficient pairs per vertical set */
 	unsigned vmul8; /* ((1 << 32) / (256 * VS)) << 8, for umulhi */
 	int vshift;	  /* log2(VS) if VS is a power of two, else -1 */
-	unsigned accmul; /* v3: 256 / VS when VS is a power of two (box sums kept pre-scaled), else 1 */
+	unsigned accmul; /* v4: 256 / VS when VS is a power of two (box sums scaled by it before the byte pick), else 1 */
 	/* horizontal */
 	int HS, Ws, hembed, NPh;
 	unsigned hmul8;
@@ -439,30 +439,6 @@ mbar_wait(unsigned bar, unsigned parity)
 	} while (!done);
 }
 
-/* The same wait for a warp that will wait LONG (the H warps on a chunk of reducev output, the producer on a
- * stage's release).  try_wait parks the warp on NANOSLEEP.SYNCS, which the hardware ends at EVERY mbarrier
- * event of the CTA -- the r1q capture has the three H warps re-checking 222 times per wait (one TMA
- * transaction or V-warp arrival at a time), 6% of all issued instructions, on the sub-partitions whose
- * issue slots bound the kernel.  Here the warp polls test_wait on a plain timer instead: a handful of
- * instructions per wait, at the price of up to `ns` of latency the double-buffered hand-offs absorb.
- */
-__device__ __forceinline__ void
-mbar_wait_poll(unsigned bar, unsigned parity, unsigned ns)
-{
-	for (;;) {
-		unsigned done;
-		asm volatile("{\n\t.reg .pred p;\n\t"
-					 "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-					 "selp.u32 %0, 1, 0, p;\n\t}"
-					 : "=r"(done)
-					 : "r"(bar), "r"(parity)
-					 : "memory");
-		if (done)
-			return;
-		asm volatile("nanosleep.u32 %0;" ::"r"(ns));
-	}
-}
-
 __device__ __forceinline__ void
 mbar_arrive(unsigned bar)
 {
@@ -534,37 +510,7 @@ average_pair(unsigned lanesA, unsigned lanesB, unsigned mul8, int shift)
 	return __byte_perm(a, b, 0x6240);
 }
 
-/* v3 forms.  The integer pipes of an SM sub-partition are two half-rate units: IMAD
- * (fma pipe) and everything else -- SHF, LOP3, PRMT, IADD3, IDP -- on the alu pipe,
- * which is what bounds this kernel.  So the per-pixel work is phrased to put as
- * much as possible on IMAD: the lane sums are accumulated by a multiply-add with a
- * run-time multiplier m = 256 / VS, which also leaves the box average
- * ((sum + VS / 2) * m) >> 8 sitting in bytes 1 and 3 (one PRMT, no shifts), and
- * scale[alpha] comes from one LOP3 + one IMAD.HI.
- */
-template <bool PREMUL>
-__device__ __forceinline__ void
-accumulate_pixel_m(unsigned x, unsigned m, unsigned k16, unsigned &rb, unsigned &ga)
-{
-	if (PREMUL) {
-		/* s = (a * 257 + 1) >> 8 = hi32((a << 24 | 1 << 16) * 257); k16 = 1 << 16 held in a
-		 * register so that the mask-and-or is ONE LOP3 (it encodes a single immediate)
-		 */
-		unsigned t0;
-		asm("lop3.b32 %0, %1, 0xff000000, %2, 0xea;" : "=r"(t0) : "r"(x), "r"(k16)); /* (x & 0xff000000) | k16 */
-		const unsigned s = __umulhi(t0, 257u);
-		const unsigned trb = (x & 0x00ff00ffu) * s + 0x00800080u; /* 16-bit lanes r * s + 128, b * s + 128 */
-		const unsigned tg = (x & 0x0000ff00u) * s + 0x00008000u;	  /* (g * s + 128) << 8: byte 2 = g', byte 3 = 0 */
-		rb = __byte_perm(trb, 0, 0x4341) * m + rb;				  /* [r', 0, b', 0] */
-		ga = __byte_perm(tg, x, 0x3732) * m + ga;				  /* [g', 0, a, 0] */
-	}
-	else {
-		rb = (x & 0x00ff00ffu) * m + rb;
-		ga = __byte_perm(x, 0, 0x4341) * m + ga;
-	}
-}
-
-/* The same sums on the half2 adder.  A 16-bit lane holding an integer below 1024 IS an fp16
+/* Box sums on the half2 adder.  A 16-bit lane holding an integer below 1024 IS an fp16
  * denormal (value n * 2^-24), denormals and the first normal binade share one spacing, so
  * add.f16x2 (no .ftz) adds the lanes as integers, exactly, while a lane stays below 2048 --
  * and a box of up to 8 bytes + its rounding amend does.  HADD2 keeps the accumulation off
@@ -583,11 +529,14 @@ __device__ __forceinline__ void
 accumulate_pixel_h(unsigned x, unsigned k16, unsigned &rb, unsigned &ga)
 {
 	if (PREMUL) {
+		/* s = (a * 257 + 1) >> 8 = hi32((a << 24 | 1 << 16) * 257); k16 = 1 << 16 held in a register so that the
+		 * mask-and-or is ONE LOP3 (it encodes a single immediate)
+		 */
 		unsigned t0;
-		asm("lop3.b32 %0, %1, 0xff000000, %2, 0xea;" : "=r"(t0) : "r"(x), "r"(k16));
+		asm("lop3.b32 %0, %1, 0xff000000, %2, 0xea;" : "=r"(t0) : "r"(x), "r"(k16)); /* (x & 0xff000000) | k16 */
 		const unsigned s = __umulhi(t0, 257u);
-		const unsigned trb = (x & 0x00ff00ffu) * s + 0x00800080u;
-		const unsigned tg = (x & 0x0000ff00u) * s + 0x00008000u;
+		const unsigned trb = (x & 0x00ff00ffu) * s + 0x00800080u; /* 16-bit lanes r * s + 128, b * s + 128 */
+		const unsigned tg = (x & 0x0000ff00u) * s + 0x00008000u;	  /* (g * s + 128) << 8: byte 2 = g', byte 3 = 0 */
 		rb = hadd2_lanes(rb, __byte_perm(trb, 0, 0x4341));
 		ga = hadd2_lanes(ga, __byte_perm(tg, x, 0x3732));
 	}
@@ -595,13 +544,6 @@ accumulate_pixel_h(unsigned x, unsigned k16, unsigned &rb, unsigned &ga)
 		rb = hadd2_lanes(rb, x & 0x00ff00ffu);
 		ga = hadd2_lanes(ga, __byte_perm(x, 0, 0x4341));
 	}
-}
-
-/* lanes hold (sum + VS / 2) * 256 / VS: the averages are bytes 1 and 3 */
-__device__ __forceinline__ unsigned
-average_pair_m(unsigned lanesA, unsigned lanesB)
-{
-	return __byte_perm(lanesA, lanesB, 0x7351);
 }
 
 __device__ __forceinline__ unsigned
@@ -974,377 +916,32 @@ thumbnail_fused_tma_kernel(const __grid_constant__ FusedParams P, const uint8_t 
 	}
 }
 
-/* ======================================================================
- * v3: v2 with the horizontal box done inside the warp and the reduceh pass on its
- * own warp.  Two adjacent input columns per thread (CPT 2), HS in {2, 4, 8}: the
- * HS columns of one box-shrunk pixel sit in HS / 2 adjacent lanes, so the box sum
- * is a shuffle reduction and the column PAIR is one more shuffle; the lane that
- * owns a pair stores it straight to sh[].  No rv[] round trip, no H1 stage and
- * -- because sh[] is double buffered and handed over with mbarriers -- no
- * block-wide barrier anywhere in the main loop:
- *     warps 0 .. NT/32-1   V: premultiply, box, reducev, shrinkh    -> sh[buf]
- *     warp  NT/32          H: reduceh, unpremultiply, store          <- sh[buf]
- *     warp  NT/32 + 1      P: cp.async.bulk producer
- * ====================================================================== */
-template <int VS, int NP, bool PREMUL, int HSQ>
-__global__ void __launch_bounds__(kMaxThreads / 2 + 64, 2)
-thumbnail_fused_tma3_kernel(const __grid_constant__ FusedParams P, const uint8_t *__restrict__ in, size_t in_frame_stride,
-	uint8_t *__restrict__ out, size_t out_frame_stride, int frame0)
-{
-	extern __shared__ __align__(128) unsigned char smem_raw[];
-
-	constexpr int K = kChunkRowsTma;
-	constexpr int CPT = 2;
-	constexpr int G = HSQ / CPT; /* lanes per box-shrunk column */
-	constexpr int HSHIFT = HSQ == 2 ? 1 : HSQ == 4 ? 2 : 3;
-	constexpr int NPR = NP > 0 ? NP : 1;
-	constexpr int VSR = VS > 0 ? VS : 1;
-	const int NT = P.NT;	   /* V threads */
-	const int NC = NT * CPT; /* columns: the stride of pairbuf */
-	const int t = threadIdx.x;
-	const int vs = VS > 0 ? VS : P.VS;
-	const int NPv = NP > 0 ? NP : P.NPv;
-	const int NPh = NP > 0 ? NP : P.NPh;
-	const int rows_per_stage = 2 * vs;
-	const unsigned stage_bytes = (unsigned) rows_per_stage * kStagePitch;
-	const int shs = P.NEmax / 2; /* pairs per sh row */
-
-	unsigned char *stages = smem_raw; /* [kStages][2 * vs][kStagePitch] */
-	uint64_t *bars = (uint64_t *) (smem_raw + kStages * stage_bytes); /* full[kStages] empty[kStages] shfull[2] shempty[2] */
-	uint2 *pairbuf = (uint2 *) (bars + 2 * kStages + 4);			  /* [slots][NC] */
-	uint2 *sh = pairbuf + (size_t) P.slots * NC;					  /* [2][K][shs] */
-	int *vcoef = (int *) (sh + (size_t) 2 * K * shs);
-	int *hcoef = vcoef + P.nvsets * P.NPv;
-	int *uscale = hcoef + P.nhsets * P.NPh; /* [256] unpremultiply LUT */
-
-	const unsigned stages_s = smem_addr(stages);
-	const unsigned full_s = smem_addr(bars);
-	const unsigned empty_s = full_s + 8u * kStages;
-	const unsigned shfull_s = empty_s + 8u * kStages;
-	const unsigned shempty_s = shfull_s + 16u;
-
-	if (t == 0) {
-		for (int i = 0; i < kStages; i++) {
-			mbar_init(full_s + 8u * i, 1);
-			mbar_init(empty_s + 8u * i, NT / 32);
-		}
-		for (int i = 0; i < 2; i++) {
-			mbar_init(shfull_s + 8u * i, NT / 32);
-			mbar_init(shempty_s + 8u * i, 1);
-		}
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	for (int i = t; i < P.nvsets * P.NPv; i += blockDim.x)
-		vcoef[i] = P.vcoef[i];
-	for (int i = t; i < P.nhsets * P.NPh; i += blockDim.x)
-		hcoef[i] = P.hcoef[i];
-	if (PREMUL)
-		for (int i = t; i < 256; i += blockDim.x)
-			uscale[i] = i == 0 ? 0 : (int) __ddiv_rn(__dmul_rn(256.0, 255.0), (double) i);
-
-	const int xa = blockIdx.x * P.TW;
-	const int xb = min(xa + P.TW, P.OW);
-	const int y_begin = blockIdx.y * P.RPC;
-	const int y_end = min(y_begin + P.RPC, P.OH);
-	const int frame = frame0 + blockIdx.z;
-	const uint8_t *fin = in + (size_t) frame * in_frame_stride;
-	uint8_t *fout = out + (size_t) frame * out_frame_stride;
-
-	const int pair_h0 = __ldg(&P.hcol[xa]).x;
-	const int E0 = 2 * pair_h0 + P.hgrid;
-	const int NE = 2 * (__ldg(&P.hcol[xb - 1]).x + P.NPh - pair_h0);
-	const int npairs = NE / 2;
-
-	auto column_of = [&](int tt) {
-		const int e = E0 + tt / HSQ;
-		const int k = tt - (tt / HSQ) * HSQ;
-		const int sc = max(0, min(e - P.hembed, P.Ws - 1));
-		return min(sc * HSQ + k, P.W - 1);
-	};
-	const int c_lo = column_of(0) & ~3;
-	const int c_hi = min(P.W, (column_of(NE * HSQ - 1) + 4) & ~3);
-	const unsigned row_bytes = (unsigned) (c_hi - c_lo) * 4u;
-
-	__syncthreads();
-
-	if (t >= NT + 32) {
-		/* ---------------- P: lane L copies row L of each stage */
-		const int lane = t - NT - 32;
-		const uint8_t *src0 = fin + (size_t) c_lo * 4;
-		const int j = lane / vs, k = lane - j * vs;
-		const bool copier = lane < rows_per_stage;
-		int s = 0;
-		unsigned phase = 0;
-		int pdone = INT_MIN;
-		for (int ya = y_begin; ya < y_end; ya += K) {
-			const int yb = min(ya + K, y_end);
-			const int P0 = __ldg(&P.vrow[ya]).x;
-			const int P1 = __ldg(&P.vrow[yb - 1]).x + P.NPv - 1;
-			for (int p = max(pdone, P0); p <= P1; p++) {
-				mbar_wait(empty_s + 8u * s, phase ^ 1u);
-				if (lane == 0)
-					mbar_expect_tx(full_s + 8u * s, (unsigned) rows_per_stage * row_bytes);
-				__syncwarp();
-				if (copier) {
-					const int sr = max(0, min(2 * p + P.vgrid + j - P.vembed, P.Hs - 1));
-					const int row = min(sr * vs + k, P.H - 1);
-					bulk_copy_g2s(stages_s + (unsigned) s * stage_bytes + (unsigned) lane * kStagePitch,
-						src0 + (size_t) row * P.in_bpl, row_bytes, full_s + 8u * s);
-				}
-				if (++s == kStages) {
-					s = 0;
-					phase ^= 1u;
-				}
-			}
-			pdone = P1 + 1;
-		}
-		return;
-	}
-
-	if (t >= NT) {
-		/* ---------------- H: reduceh + unpremultiply + store, one warp */
-		const int lane = t - NT;
-		const int bw = xb - xa;
-		int chunk = 0;
-		for (int ya = y_begin; ya < y_end; ya += K, chunk++) {
-			const int yb = min(ya + K, y_end);
-			const int rows = yb - ya;
-			const int buf = chunk & 1;
-			const uint2 *shb = sh + (size_t) buf * K * shs;
-			mbar_wait(shfull_s + 8u * buf, (unsigned) (chunk >> 1) & 1u);
-			for (int idx = lane; idx < rows * bw; idx += 32) {
-				const int k = fast_div(idx, bw);
-				const int x = xa + (idx - k * bw);
-				const int2 hc = __ldg(&P.hcol[x]);
-				const uint2 *win = shb + k * shs + (hc.x - pair_h0);
-				const int *cfp = hcoef + hc.y * NPh;
-				int r = VB200_INTERPOLATE_SCALE >> 1, g = r, b = r, a = r;
-				if (NP > 0) {
-#pragma unroll
-					for (int kk = 0; kk < NPR; kk++) {
-						const uint2 w = win[kk];
-						const unsigned c = (unsigned) cfp[kk];
-						r = dp2a_lo(c, w.x, r);
-						b = dp2a_hi(c, w.x, b);
-						g = dp2a_lo(c, w.y, g);
-						a = dp2a_hi(c, w.y, a);
-					}
-				}
-				else
-					for (int kk = 0; kk < NPh; kk++) {
-						const uint2 w = win[kk];
-						const unsigned c = (unsigned) cfp[kk];
-						r = dp2a_lo(c, w.x, r);
-						b = dp2a_hi(c, w.x, b);
-						g = dp2a_lo(c, w.y, g);
-						a = dp2a_hi(c, w.y, a);
-					}
-				r = max(0, min(r >> VB200_INTERPOLATE_SHIFT, 255));
-				g = max(0, min(g >> VB200_INTERPOLATE_SHIFT, 255));
-				b = max(0, min(b >> VB200_INTERPOLATE_SHIFT, 255));
-				a = max(0, min(a >> VB200_INTERPOLATE_SHIFT, 255));
-				if (PREMUL) {
-					const int sc = uscale[a];
-					r = ((r * sc + 128) >> 8) & 0xff;
-					g = ((g * sc + 128) >> 8) & 0xff;
-					b = ((b * sc + 128) >> 8) & 0xff;
-				}
-				*(unsigned *) (fout + (size_t) (ya + k) * P.out_bpl + (size_t) x * 4) =
-					(unsigned) r | ((unsigned) g << 8) | ((unsigned) b << 16) | ((unsigned) a << 24);
-			}
-			__syncwarp();
-			if (lane == 0)
-				mbar_arrive(shempty_s + 8u * buf);
-		}
-		return;
-	}
-
-	/* ---------------- V warps */
-	/* the thread's two columns are adjacent and start on an even column: one 64-bit LDS per row */
-	const unsigned char *my_cols = stages + (size_t) (column_of(min(t * CPT, NE * HSQ - 2)) - c_lo) * 4u;
-	const unsigned accm = P.accmul; /* run-time on purpose: keeps the accumulation on IMAD */
-	unsigned k16;
-	asm volatile("mov.u32 %0, 0x10000;" : "=r"(k16));
-	const unsigned amend2 = (unsigned) (vs / 2) * accm * 0x00010001u;
-	const unsigned hamend2 = (unsigned) (HSQ / 2) * 0x00010001u;
-	const bool lane0 = (t & 31) == 0;
-	const unsigned vmul8 = P.vmul8;
-	const int vshift = VS == 1 ? 0 : VS == 2 ? 1 : VS == 4 ? 2 : VS == 8 ? 3 : P.vshift;
-	const int tc = t * CPT;
-	/* this thread's column pair: lanes [2G m, 2G m + 2G) hold pair m; its first lane stores it */
-	const int my_pair = t / (2 * G);
-	const bool pair_writer = (t & (2 * G - 1)) == 0 && my_pair < npairs;
-	const bool is_B = (t & G) != 0; /* second column of the pair */
-
-	int s = 0;
-	unsigned phase = 0;
-	int pdone = INT_MIN;
-	int P0_prev = 0;
-	int cset = -1;
-	unsigned cf[NPR];
-	int chunk = 0;
-
-	for (int ya = y_begin; ya < y_end; ya += K, chunk++) {
-		const int yb = min(ya + K, y_end);
-		const int P0 = __ldg(&P.vrow[ya]).x;
-		const int P1 = __ldg(&P.vrow[yb - 1]).x + P.NPv - 1;
-
-		int pfirst = P0;
-		if (pdone > P0) {
-			const int shift = P0 - P0_prev;
-			if (shift > 0) {
-				const int cnt = pdone - P0;
-				uint2 *dstp = pairbuf + tc;
-				const uint2 *srcp = pairbuf + shift * NC + tc;
-#pragma unroll 4
-				for (int i = 0; i < cnt; i++)
-					*(uint4 *) (dstp + i * NC) = *(const uint4 *) (srcp + i * NC);
-			}
-			pfirst = pdone;
-		}
-
-		uint2 *pdst = pairbuf + (pfirst - P0) * NC + tc;
-		for (int p = pfirst; p <= P1; p++, pdst += NC) {
-			const unsigned soff = (unsigned) s * stage_bytes;
-			unsigned rbA[CPT], gaA[CPT], rbB[CPT], gaB[CPT];
-#pragma unroll
-			for (int i = 0; i < CPT; i++)
-				rbA[i] = gaA[i] = rbB[i] = gaB[i] = amend2;
-			mbar_wait(full_s + 8u * s, phase);
-			if (VS > 0) {
-				uint2 pa[VSR], pb[VSR];
-#pragma unroll
-				for (int k = 0; k < VSR; k++) {
-					pa[k] = *(const uint2 *) (my_cols + soff + k * kStagePitch);
-					pb[k] = *(const uint2 *) (my_cols + soff + (VSR + k) * kStagePitch);
-				}
-				__syncwarp();
-				if (lane0)
-					mbar_arrive(empty_s + 8u * s);
-#pragma unroll
-				for (int k = 0; k < VSR; k++) {
-					accumulate_pixel_m<PREMUL>(pa[k].x, accm, k16, rbA[0], gaA[0]);
-					accumulate_pixel_m<PREMUL>(pa[k].y, accm, k16, rbA[1], gaA[1]);
-					accumulate_pixel_m<PREMUL>(pb[k].x, accm, k16, rbB[0], gaB[0]);
-					accumulate_pixel_m<PREMUL>(pb[k].y, accm, k16, rbB[1], gaB[1]);
-				}
-			}
-			else {
-				for (int k = 0; k < vs; k++) {
-					const uint2 qa = *(const uint2 *) (my_cols + soff + k * kStagePitch);
-					const uint2 qb = *(const uint2 *) (my_cols + soff + (vs + k) * kStagePitch);
-					accumulate_pixel_m<PREMUL>(qa.x, accm, k16, rbA[0], gaA[0]);
-					accumulate_pixel_m<PREMUL>(qa.y, accm, k16, rbA[1], gaA[1]);
-					accumulate_pixel_m<PREMUL>(qb.x, accm, k16, rbB[0], gaB[0]);
-					accumulate_pixel_m<PREMUL>(qb.y, accm, k16, rbB[1], gaB[1]);
-				}
-				__syncwarp();
-				if (lane0)
-					mbar_arrive(empty_s + 8u * s);
-			}
-			if (++s == kStages) {
-				s = 0;
-				phase ^= 1u;
-			}
-			if (vshift >= 0)
-				*(uint4 *) pdst = make_uint4(average_pair_m(rbA[0], rbB[0]), average_pair_m(gaA[0], gaB[0]),
-					average_pair_m(rbA[1], rbB[1]), average_pair_m(gaA[1], gaB[1]));
-			else
-				*(uint4 *) pdst = make_uint4(average_pair(rbA[0], rbB[0], vmul8, -1), average_pair(gaA[0], gaB[0], vmul8, -1),
-					average_pair(rbA[1], rbB[1], vmul8, -1), average_pair(gaA[1], gaB[1], vmul8, -1));
-		}
-
-		/* reducev + in-warp shrinkh; rows go to sh[buf] once the H warp has released it */
-		const int buf = chunk & 1;
-		uint2 *shb = sh + (size_t) buf * K * shs + my_pair;
-		mbar_wait(shempty_s + 8u * buf, ((unsigned) (chunk >> 1) & 1u) ^ 1u);
-		for (int y = ya; y < yb; y++, shb += shs) {
-			const int2 vr = __ldg(&P.vrow[y]);
-			const uint2 *win = pairbuf + (vr.x - P0) * NC + tc;
-			int acc[CPT][4];
-#pragma unroll
-			for (int i = 0; i < CPT; i++)
-				acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = VB200_INTERPOLATE_SCALE >> 1;
-			if (NP > 0) {
-				if (vr.y != cset) {
-					cset = vr.y;
-#pragma unroll
-					for (int k = 0; k < NPR; k++)
-						cf[k] = (unsigned) vcoef[cset * NPR + k];
-				}
-#pragma unroll
-				for (int k = 0; k < NPR; k++) {
-					const uint4 q = *(const uint4 *) (win + k * NC);
-					acc[0][0] = dp2a_lo(cf[k], q.x, acc[0][0]);
-					acc[0][2] = dp2a_hi(cf[k], q.x, acc[0][2]);
-					acc[0][1] = dp2a_lo(cf[k], q.y, acc[0][1]);
-					acc[0][3] = dp2a_hi(cf[k], q.y, acc[0][3]);
-					acc[1][0] = dp2a_lo(cf[k], q.z, acc[1][0]);
-					acc[1][2] = dp2a_hi(cf[k], q.z, acc[1][2]);
-					acc[1][1] = dp2a_lo(cf[k], q.w, acc[1][1]);
-					acc[1][3] = dp2a_hi(cf[k], q.w, acc[1][3]);
-				}
-			}
-			else {
-				const int *cfp = vcoef + vr.y * NPv;
-				for (int k = 0; k < NPv; k++) {
-					const unsigned c = (unsigned) cfp[k];
-					const uint4 q = *(const uint4 *) (win + k * NC);
-					acc[0][0] = dp2a_lo(c, q.x, acc[0][0]);
-					acc[0][2] = dp2a_hi(c, q.x, acc[0][2]);
-					acc[0][1] = dp2a_lo(c, q.y, acc[0][1]);
-					acc[0][3] = dp2a_hi(c, q.y, acc[0][3]);
-					acc[1][0] = dp2a_lo(c, q.z, acc[1][0]);
-					acc[1][2] = dp2a_hi(c, q.z, acc[1][2]);
-					acc[1][1] = dp2a_lo(c, q.w, acc[1][1]);
-					acc[1][3] = dp2a_hi(c, q.w, acc[1][3]);
-				}
-			}
-			/* reducev results (clipped bytes) straight into the box-sum lanes:
-			 * rb = r | b << 16, ga = g | a << 16, this thread's two columns added
-			 */
-			unsigned rb = hamend2, ga = hamend2;
-#pragma unroll
-			for (int i = 0; i < CPT; i++) {
-				const int r = max(0, min(acc[i][0] >> VB200_INTERPOLATE_SHIFT, 255));
-				const int g = max(0, min(acc[i][1] >> VB200_INTERPOLATE_SHIFT, 255));
-				const int b = max(0, min(acc[i][2] >> VB200_INTERPOLATE_SHIFT, 255));
-				const int a = max(0, min(acc[i][3] >> VB200_INTERPOLATE_SHIFT, 255));
-				rb += (unsigned) r + (unsigned) b * 65536u;
-				ga += (unsigned) g + (unsigned) a * 65536u;
-			}
-			if (G > 1) {
-				/* the other lanes of this box-shrunk column; amend was added once per lane */
-#pragma unroll
-				for (int off = 1; off < G; off <<= 1) {
-					rb += __shfl_xor_sync(0xffffffffu, rb, off);
-					ga += __shfl_xor_sync(0xffffffffu, ga, off);
-				}
-				rb -= (unsigned) (G - 1) * hamend2;
-				ga -= (unsigned) (G - 1) * hamend2;
-			}
-			/* ((amend + sum) * multiplier) >> 24 with HS a power of two == >> log2(HS); bytes 0, 2 exact */
-			rb >>= HSHIFT;
-			ga >>= HSHIFT;
-			const unsigned orb = __shfl_xor_sync(0xffffffffu, rb, G);
-			const unsigned oga = __shfl_xor_sync(0xffffffffu, ga, G);
-			if (pair_writer) {
-				uint2 w;
-				w.x = __byte_perm(rb, orb, 0x6240); /* writer is the A column: [rA rB bA bB] */
-				w.y = __byte_perm(ga, oga, 0x6240);
-				*shb = w;
-			}
-			(void) is_B;
-		}
-		pdone = P1 + 1;
-		P0_prev = P0;
-		__syncwarp();
-		if (lane0)
-			mbar_arrive(shfull_s + 8u * buf);
-	}
-}
-
 #include "thumbnail_fused_mma.cuh"
+
+/* The tensor-pipe kernel's instantiations, (VS, NP, HS): boxes that are powers of two freely mixed but for (8, 2), and
+ * boxes 2 .. 8 that differ by at most one (what a uniform shrink gives).  The plan chooses the kernel only for a (VS, HS)
+ * pair listed here, and a launch dispatches on the same list.
+ */
+#define VB200_V4_LIST(X) \
+	X(4, 6, 4) X(4, 7, 4) X(2, 6, 2) X(2, 7, 2) X(8, 6, 8) X(8, 7, 8) \
+	X(4, 0, 4) X(2, 0, 2) X(4, 0, 2) X(2, 0, 4) X(4, 0, 8) X(2, 0, 8) X(8, 0, 8) X(8, 0, 4) \
+	X(3, 0, 3) X(5, 0, 5) X(6, 0, 6) X(7, 0, 7) X(2, 0, 3) X(3, 0, 2) X(3, 0, 4) X(4, 0, 3) \
+	X(4, 0, 5) X(5, 0, 4) X(5, 0, 6) X(6, 0, 5) X(6, 0, 7) X(7, 0, 6) X(7, 0, 8) X(8, 0, 7)
+
+/* The NP of the v4 instantiation that runs boxes (vs, hs) with nph horizontal coefficient pairs: nph where (vs, nph, hs)
+ * is listed, else 0 (the generic instantiation, which reads P.NPh at run time); -1 when (vs, hs) is not listed.
+ */
+int
+v4_np(int vs, int nph, int hs)
+{
+	int np = -1;
+#define X(VS_, NP_, HS_) \
+	if (vs == VS_ && hs == HS_ && (NP_ == nph || (NP_ == 0 && np < 0))) \
+		np = NP_;
+	VB200_V4_LIST(X)
+#undef X
+	return np;
+}
 
 /* Pack a 65 x n table of short coefficients into parity-aligned s16x2 pairs:
  * set (phase, parity) holds pairs k = 0..NP-1 = (c[2k - parity], c[2k + 1 - parity]).
@@ -1409,6 +1006,13 @@ int linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t
 	cudaStream_t s, const LinIccBatch *icc = nullptr, int out_bands = 0);
 void linear_thumb_free(LinearThumb *lt);
 
+/* The fused kernel a plan runs, chosen once by plan_build_fused */
+enum class FusedKernel {
+	Ldg, /* v1: thumbnail_fused_kernel */
+	Tma, /* v2: thumbnail_fused_tma_kernel */
+	Mma, /* v4: thumbnail_fused_mma_kernel */
+};
+
 struct ThumbnailPlanImpl {
 	/* request */
 	int W = 0, H = 0, bands = 0, fmt = 0, has_alpha = 0;
@@ -1420,20 +1024,16 @@ struct ThumbnailPlanImpl {
 	bool premul = false;
 	bool fused = false;
 	int device = -1;
-	/* fused path */
+	/* fused path: v1's parameters, which every fused plan can run */
+	FusedKernel kernel = FusedKernel::Ldg;
 	FusedParams fp{};
 	void *tables = nullptr; /* one device block */
 	size_t smem = 0;
-	dim3 grid;
 	/* v2 (TMA-fed) variant of the same kernel: its own chunking and smem */
-	bool tma_ok = false;
 	int slots_tma = 0;
 	size_t smem_tma = 0;
-	bool tma3_ok = false; /* v3: in-warp shrinkh + H warp (HS in {2,4,8}) */
-	size_t smem_tma3 = 0;
 	/* v4: reducev on the integer tensor pipe */
-	bool mma_ok = false;
-	int mma_cols = 0, mma_cpt = 1, mma_tw = 0, mma_nt = 0, mma_nemax = 0;
+	int mma_tw = 0, mma_nt = 0, mma_nemax = 0;
 	std::vector<MmaBand> mma_bands; /* the bands of mma_tw over a frame row */
 	size_t smem_mma = 0;
 	/* plan the geometry only: no device tables (vb200_debug_thumbnail_bands) */
@@ -1447,7 +1047,6 @@ struct ThumbnailPlanImpl {
 	cudaEvent_t drained[kStreams] = {nullptr, nullptr, nullptr};
 	int stage_frames = 0;
 	std::mutex pump_lock;
-	std::mutex launch_lock;
 	/* the opaque-stage vote of the tensor-pipe kernel (thumbnail_fused_mma.cuh): per-launch counts of hinted frames
 	 * come back through pinned memory, a few launches late; opaque_mode picks the instantiation of the NEXT launch
 	 */
@@ -1508,118 +1107,123 @@ thumbnail_shrink(int w, int h, int tw, int th, int size, double *hshrink, double
 	*vshrink = std::min(vs, (double) h);
 }
 
+/* The error check and launch count after a fused kernel's launch */
+int
+launch_status(const char *domain, const char *what)
+{
+	const cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess)
+		return cuda_fail(domain, e, what);
+	count_launch();
+	return 0;
+}
+
+/* Rows per CTA: the whole height in chunks of k rows, halved (on whole chunks, down to min_chunks of them) while the
+ * batch gives fewer than `ctas` CTAs
+ */
+int
+rows_per_cta(int OH, int k, int min_chunks, int bands_x, int n, int ctas)
+{
+	int rpc = ((OH + k - 1) / k) * k;
+	while ((long long) bands_x * ((OH + rpc - 1) / rpc) * n < ctas && rpc > min_chunks * k)
+		rpc = ((rpc / 2 + k - 1) / k) * k;
+	return rpc;
+}
+
+/* v1: frames f0 .. f0 + grid.z - 1 */
 template <int VS, bool PREMUL>
 int
-launch_fused_t(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s)
+launch_ldg_t(const char *domain, const FusedParams &fp, size_t smem, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int f0, dim3 grid, cudaStream_t s)
 {
 	auto kern = thumbnail_fused_kernel<VS, PREMUL>;
-	static thread_local int configured_for = -1;
-	(void) configured_for;
-	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) pl->smem));
-	for (int f0 = 0; f0 < n; f0 += 32768) {
-		dim3 grid = pl->grid;
-		grid.z = std::min(32768, n - f0);
-		kern<<<grid, pl->fp.NT, pl->smem, s>>>(pl->fp, (const uint8_t *) in, in_stride, (uint8_t *) out, out_stride, f0);
-		cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-			return cuda_fail(domain, e, "thumbnail_fused_kernel launch");
-		count_launch();
-	}
-	return 0;
+	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+	kern<<<grid, fp.NT, smem, s>>>(fp, (const uint8_t *) in, in_stride, (uint8_t *) out, out_stride, f0);
+	return launch_status(domain, "thumbnail_fused_kernel launch");
 }
 
 template <bool PREMUL>
 int
-launch_fused_vs(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n,
-	cudaStream_t s)
+launch_ldg_vs(const char *domain, const FusedParams &fp, size_t smem, const void *in, size_t is, void *out, size_t os, int f0,
+	dim3 grid, cudaStream_t s)
 {
-	switch (pl->fp.VS) {
-	case 1: return launch_fused_t<1, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 2: return launch_fused_t<2, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 3: return launch_fused_t<3, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 4: return launch_fused_t<4, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 5: return launch_fused_t<5, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 6: return launch_fused_t<6, PREMUL>(domain, pl, in, is, out, os, n, s);
-	case 8: return launch_fused_t<8, PREMUL>(domain, pl, in, is, out, os, n, s);
-	default: return launch_fused_t<0, PREMUL>(domain, pl, in, is, out, os, n, s);
+	switch (fp.VS) {
+	case 1: return launch_ldg_t<1, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 2: return launch_ldg_t<2, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 3: return launch_ldg_t<3, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 4: return launch_ldg_t<4, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 5: return launch_ldg_t<5, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 6: return launch_ldg_t<6, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 8: return launch_ldg_t<8, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	default: return launch_ldg_t<0, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
 	}
 }
 
-/* v2 launchers: same grid, one extra (producer) warp per CTA */
+/* v1 over frames f0 .. f0 + nf - 1 of an n-frame batch: enough CTAs to fill the machine, rows split when the batch is small */
+int
+launch_ldg(const char *domain, const ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n, int f0,
+	int nf, cudaStream_t s)
+{
+	FusedParams fp = pl->fp;
+	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
+	fp.RPC = rows_per_cta(pl->OH, kChunkRows, 2, bands_x, n, 2 * sm_count());
+	const dim3 grid(bands_x, (pl->OH + fp.RPC - 1) / fp.RPC, nf);
+	return pl->premul ? launch_ldg_vs<true>(domain, fp, pl->smem, in, is, out, os, f0, grid, s)
+					  : launch_ldg_vs<false>(domain, fp, pl->smem, in, is, out, os, f0, grid, s);
+}
+
+/* v2: the v1 grid, one extra (producer) warp per CTA */
 template <int VS, int NP, bool PREMUL>
 int
-launch_tma_t(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t in_stride,
-	void *out, size_t out_stride, int n, dim3 grid, cudaStream_t s)
+launch_tma_t(const char *domain, const FusedParams &fp, size_t smem, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int f0, dim3 grid, cudaStream_t s)
 {
 	auto kern = thumbnail_fused_tma_kernel<VS, NP, PREMUL, kColsPerThread>;
-	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) pl->smem_tma));
-	for (int f0 = 0; f0 < n; f0 += 32768) {
-		grid.z = std::min(32768, n - f0);
-		kern<<<grid, fp.NT + 32, pl->smem_tma, s>>>(fp, (const uint8_t *) in, in_stride, (uint8_t *) out, out_stride, f0);
-		cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-			return cuda_fail(domain, e, "thumbnail_fused_tma_kernel launch");
-		count_launch();
-	}
-	return 0;
+	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+	kern<<<grid, fp.NT + 32, smem, s>>>(fp, (const uint8_t *) in, in_stride, (uint8_t *) out, out_stride, f0);
+	return launch_status(domain, "thumbnail_fused_tma_kernel launch");
 }
 
 template <int NP, bool PREMUL>
 int
-launch_tma_vs(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t is, void *out,
-	size_t os, int n, dim3 grid, cudaStream_t s)
+launch_tma_vs(const char *domain, const FusedParams &fp, size_t smem, const void *in, size_t is, void *out, size_t os, int f0,
+	dim3 grid, cudaStream_t s)
 {
 	switch (fp.VS) {
-	case 1: return launch_tma_t<1, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
-	case 2: return launch_tma_t<2, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
-	case 3: return launch_tma_t<3, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
-	case 4: return launch_tma_t<4, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
-	case 8: return launch_tma_t<8, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
-	default: return launch_tma_t<0, NP, PREMUL>(domain, pl, fp, in, is, out, os, n, grid, s);
+	case 1: return launch_tma_t<1, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 2: return launch_tma_t<2, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 3: return launch_tma_t<3, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 4: return launch_tma_t<4, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	case 8: return launch_tma_t<8, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	default: return launch_tma_t<0, NP, PREMUL>(domain, fp, smem, in, is, out, os, f0, grid, s);
 	}
 }
 
-template <int VS, int NP, bool PREMUL, int HSQ>
 int
-launch_tma3_t(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t in_stride,
-	void *out, size_t out_stride, int n, dim3 grid, cudaStream_t s)
+launch_tma(const char *domain, const ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n, int f0,
+	int nf, cudaStream_t s)
 {
-	auto kern = thumbnail_fused_tma3_kernel<VS, NP, PREMUL, HSQ>;
-	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) pl->smem_tma3));
-	for (int f0 = 0; f0 < n; f0 += 32768) {
-		grid.z = std::min(32768, n - f0);
-		kern<<<grid, fp.NT + 64, pl->smem_tma3, s>>>(fp, (const uint8_t *) in, in_stride, (uint8_t *) out, out_stride, f0);
-		cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-			return cuda_fail(domain, e, "thumbnail_fused_tma3_kernel launch");
-		count_launch();
-	}
-	return 0;
-}
-
-/* the instantiated corner of v3: box 2 / 4 / 8 on both axes (what gap 2.0 gives for
- * shrinks 4..20) with 6 or 7 coefficient pairs; everything else runs v2
- */
-template <bool PREMUL>
-int
-launch_tma3(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t is, void *out,
-	size_t os, int n, dim3 grid, cudaStream_t s, bool *handled)
-{
-	*handled = true;
+	FusedParams fp = pl->fp;
+	fp.slots = pl->slots_tma;
+	/* consumer threads: kColsPerThread columns each (pl->fp.NT counts columns, rounded to 32) */
+	fp.NT = ((pl->fp.NT / kColsPerThread + 31) / 32) * 32;
+	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
+	fp.RPC = rows_per_cta(pl->OH, kChunkRowsTma, 4, bands_x, n, 2 * sm_count());
+	const dim3 grid(bands_x, (pl->OH + fp.RPC - 1) / fp.RPC, nf);
+	const size_t smem = pl->smem_tma;
 	const int np = fp.NPv == fp.NPh ? fp.NPv : 0;
-#define V3(VS_, NP_, HS_) \
-	if (fp.VS == VS_ && np == NP_ && fp.HS == HS_) \
-		return launch_tma3_t<VS_, NP_, PREMUL, HS_>(domain, pl, fp, in, is, out, os, n, grid, s);
-	V3(2, 6, 2) V3(2, 7, 2) V3(4, 6, 4) V3(4, 7, 4) V3(8, 6, 8) V3(8, 7, 8)
-	V3(2, 0, 2) V3(4, 0, 4) V3(8, 0, 8) V3(3, 0, 4) V3(4, 0, 2) V3(2, 0, 4)
-#undef V3
-	*handled = false;
-	return 0;
+	if (np == 6)
+		return pl->premul ? launch_tma_vs<6, true>(domain, fp, smem, in, is, out, os, f0, grid, s)
+						  : launch_tma_vs<6, false>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	if (np == 7)
+		return pl->premul ? launch_tma_vs<7, true>(domain, fp, smem, in, is, out, os, f0, grid, s)
+						  : launch_tma_vs<7, false>(domain, fp, smem, in, is, out, os, f0, grid, s);
+	return pl->premul ? launch_tma_vs<0, true>(domain, fp, smem, in, is, out, os, f0, grid, s)
+					  : launch_tma_vs<0, false>(domain, fp, smem, in, is, out, os, f0, grid, s);
 }
 
 /* A tiled tensor map over the batch: u64 elements (2 pixels), dims {W / 2, H, frames}, box
- * {v4_boxw(WCOLS, HS) / 2, rows, 1}: one cp.async.bulk.tensor per TMA stage.  Returns false when
+ * {v4_boxw(HS) / 2, rows, 1}: one cp.async.bulk.tensor per TMA stage.  Returns false when
  * the driver entry point or the geometry is not usable; the kernel then copies row by row.
  */
 bool
@@ -1700,7 +1304,7 @@ opaque_hint_begin(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &
 	*hint = nullptr;
 	*use_opq = false;
 	const char *probe_env = getenv("VB200_OPAQUE_PROBE"); /* 0: never (A/B timing); 2: always use the voting instantiation */
-	if (!VB200_V4_OPAQUE || !pl->premul || (probe_env && probe_env[0] == '0'))
+	if (!pl->premul || (probe_env && probe_env[0] == '0'))
 		return 0;
 	{
 		std::lock_guard<std::mutex> lock(pl->hint_lock);
@@ -1763,149 +1367,70 @@ opaque_hint_end(ThumbnailPlanImpl *pl, void *hint, int n, cudaStream_t s)
 	dev_free(hint, s);
 }
 
-template <int VS, int NP, bool PREMUL, int HSQ, int WCOLS, int CPT, bool OPQ>
+template <int VS, int NP, bool PREMUL, int HSQ, bool OPQ>
 int
-launch_mma_k(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const CUtensorMap &tm, int use_tmap, const void *in,
+launch_mma_k(const char *domain, const ThumbnailPlanImpl *pl, const FusedParams &fp, const CUtensorMap &tm, int use_tmap, const void *in,
 	size_t in_stride, void *out, size_t out_stride, int f0, dim3 grid, cudaStream_t s)
 {
-	auto kern = thumbnail_fused_mma_kernel<VS, NP, PREMUL, HSQ, WCOLS, CPT, OPQ>;
+	auto kern = thumbnail_fused_mma_kernel<VS, NP, PREMUL, HSQ, OPQ>;
 	VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) pl->smem_mma));
-	kern<<<grid, fp.NT + 32 * V4HWarpsW<WCOLS, CPT>::value + 32, pl->smem_mma, s>>>(fp, tm, use_tmap, (const uint8_t *) in, in_stride,
+	kern<<<grid, fp.NT + 32 * kV4HWarps + 32, pl->smem_mma, s>>>(fp, tm, use_tmap, (const uint8_t *) in, in_stride,
 		(uint8_t *) out, out_stride, f0);
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-		return cuda_fail(domain, e, "thumbnail_fused_mma_kernel launch");
-	count_launch();
-	return 0;
+	return launch_status(domain, "thumbnail_fused_mma_kernel launch");
 }
 
-template <int VS, int NP, bool PREMUL, int HSQ, int WCOLS, int CPT>
+/* v4 over frames f0 .. f0 + grid.z - 1 of an n-frame batch (the stage tensor map spans the batch) */
+template <int VS, int NP, bool PREMUL, int HSQ>
 int
-launch_mma_t(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, dim3 grid, cudaStream_t s)
+launch_mma_t(const char *domain, ThumbnailPlanImpl *pl, FusedParams fp, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int n, int f0, dim3 grid, cudaStream_t s)
 {
 	CUtensorMap tm;
 	memset(&tm, 0, sizeof(tm));
-	const int use_tmap = make_stage_tensor_map(&tm, in, fp.W, fp.H, fp.in_bpl, in_stride, n, v4_boxw(WCOLS, HSQ), 2 * VS) ? 1 : 0;
-	/* the opaque-stage vote exists for the configuration real batches run: premultiplied, 768-column bands */
-	constexpr bool CAN_OPQ = PREMUL && CPT == 2 && WCOLS > 448;
-	for (int f0 = 0; f0 < n; f0 += 32768) {
-		grid.z = std::min(32768, n - f0);
-		FusedParams fpl = fp;
-		void *hint = nullptr;
-		bool use_opq = false;
-		if (CAN_OPQ && opaque_hint_begin(domain, pl, fp, (const uint8_t *) in + (size_t) f0 * in_stride, in_stride, (int) grid.z, s, &hint, &use_opq))
-			return -1;
-		fpl.opaque_hint = (const unsigned char *) hint;
-		int rc;
-		if constexpr (CAN_OPQ)
-			rc = use_opq ? launch_mma_k<VS, NP, PREMUL, HSQ, WCOLS, CPT, true>(domain, pl, fpl, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s)
-						 : launch_mma_k<VS, NP, PREMUL, HSQ, WCOLS, CPT, false>(domain, pl, fpl, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s);
-		else
-			rc = launch_mma_k<VS, NP, PREMUL, HSQ, WCOLS, CPT, false>(domain, pl, fpl, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s);
-		opaque_hint_end(pl, hint, (int) grid.z, s);
-		if (rc)
-			return rc;
-	}
-	return 0;
+	const int use_tmap = make_stage_tensor_map(&tm, in, fp.W, fp.H, fp.in_bpl, in_stride, n, v4_boxw(HSQ), 2 * VS) ? 1 : 0;
+	void *hint = nullptr;
+	bool use_opq = false;
+	if (PREMUL && opaque_hint_begin(domain, pl, fp, (const uint8_t *) in + (size_t) f0 * in_stride, in_stride, (int) grid.z, s, &hint, &use_opq))
+		return -1;
+	fp.opaque_hint = (const unsigned char *) hint;
+	int rc;
+	if constexpr (PREMUL)
+		rc = use_opq ? launch_mma_k<VS, NP, PREMUL, HSQ, true>(domain, pl, fp, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s)
+					 : launch_mma_k<VS, NP, PREMUL, HSQ, false>(domain, pl, fp, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s);
+	else
+		rc = launch_mma_k<VS, NP, PREMUL, HSQ, false>(domain, pl, fp, tm, use_tmap, in, in_stride, out, out_stride, f0, grid, s);
+	opaque_hint_end(pl, hint, (int) grid.z, s);
+	return rc;
 }
 
-/* the instantiated corner of v4: box 2 / 4 vertically, 2 / 4 / 8 horizontally */
-template <bool PREMUL, int WCOLS, int CPT>
+template <bool PREMUL>
 int
-launch_mma_w(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t is, void *out,
-	size_t os, int n, dim3 grid, cudaStream_t s, bool *handled)
+launch_mma_list(const char *domain, ThumbnailPlanImpl *pl, const FusedParams &fp, const void *in, size_t is, void *out, size_t os,
+	int n, int f0, dim3 grid, cudaStream_t s)
 {
-	*handled = true;
-	const int np = fp.NPh == 6 || fp.NPh == 7 ? fp.NPh : 0;
-#define V4(VS_, NP_, HS_) \
+	const int np = v4_np(fp.VS, fp.NPh, fp.HS);
+#define X(VS_, NP_, HS_) \
 	if (fp.VS == VS_ && np == NP_ && fp.HS == HS_) \
-		return launch_mma_t<VS_, NP_, PREMUL, HS_, WCOLS, CPT>(domain, pl, fp, in, is, out, os, n, grid, s);
-	V4(4, 6, 4) V4(4, 7, 4) V4(2, 6, 2) V4(2, 7, 2)
-	V4(4, 0, 4) V4(2, 0, 2) V4(4, 0, 2) V4(2, 0, 4) V4(4, 0, 8) V4(2, 0, 8)
-	V4(8, 6, 8) V4(8, 7, 8) V4(8, 0, 8) V4(8, 0, 4)
-	/* boxes that are not powers of two: the pairs a uniform shrink produces (the two axes' boxes differ by at
-	 * most one), run-time tap counts, two columns per thread
-	 */
-	if constexpr (CPT == 2 && WCOLS > 448) {
-		V4(3, 0, 3) V4(5, 0, 5) V4(6, 0, 6) V4(7, 0, 7)
-		V4(2, 0, 3) V4(3, 0, 2) V4(3, 0, 4) V4(4, 0, 3) V4(4, 0, 5) V4(5, 0, 4) V4(5, 0, 6) V4(6, 0, 5)
-		V4(6, 0, 7) V4(7, 0, 6) V4(7, 0, 8) V4(8, 0, 7)
-	}
-#undef V4
-	*handled = false;
-	return 0;
+		return launch_mma_t<VS_, NP_, PREMUL, HS_>(domain, pl, fp, in, is, out, os, n, f0, grid, s);
+	VB200_V4_LIST(X)
+#undef X
+	error(domain, "the tensor-pipe kernel has no instantiation for VS %d, HS %d", fp.VS, fp.HS);
+	return -1;
 }
 
 int
-launch_mma(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n,
-	cudaStream_t s, bool *handled)
+launch_mma(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n, int f0, int nf,
+	cudaStream_t s)
 {
 	FusedParams fp = pl->fp;
 	fp.TW = pl->mma_tw;
 	fp.NT = pl->mma_nt;
 	fp.NEmax = pl->mma_nemax;
-	const int K = fp.mma_rows;
 	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
-	int rpc = ((pl->OH + K - 1) / K) * K;
-	const int ctas = pl->mma_cols > 448 ? sm_count() : 2 * sm_count();
-	while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < ctas && rpc > 4 * K)
-		rpc = ((rpc / 2 + K - 1) / K) * K;
-	fp.RPC = rpc;
-	const dim3 grid(bands_x, (pl->OH + rpc - 1) / rpc, 1);
-	if (pl->mma_cols > 448)
-		return pl->premul ? launch_mma_w<true, 768, 2>(domain, pl, fp, in, is, out, os, n, grid, s, handled)
-						  : launch_mma_w<false, 768, 2>(domain, pl, fp, in, is, out, os, n, grid, s, handled);
-	if (pl->mma_cpt == 1)
-		return pl->premul ? launch_mma_w<true, VB200_V4_COLS, 1>(domain, pl, fp, in, is, out, os, n, grid, s, handled)
-						  : launch_mma_w<false, VB200_V4_COLS, 1>(domain, pl, fp, in, is, out, os, n, grid, s, handled);
-	return pl->premul ? launch_mma_w<true, VB200_V4_COLS, 2>(domain, pl, fp, in, is, out, os, n, grid, s, handled)
-					  : launch_mma_w<false, VB200_V4_COLS, 2>(domain, pl, fp, in, is, out, os, n, grid, s, handled);
-}
-
-int
-launch_tma(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t is, void *out, size_t os, int n,
-	cudaStream_t s, bool *done)
-{
-	*done = true;
-	if (pl->mma_ok) {
-		bool handled = false;
-		const int rc = launch_mma(domain, pl, in, is, out, os, n, s, &handled);
-		if (handled)
-			return rc;
-	}
-	if (!pl->tma_ok) {
-		*done = false; /* the caller falls through to the ld.global kernel */
-		return 0;
-	}
-	FusedParams fp = pl->fp;
-	fp.slots = pl->slots_tma;
-	/* consumer threads: kColsPerThread columns each (pl->fp.NT counts columns, rounded to 32) */
-	fp.NT = ((pl->fp.NT / kColsPerThread + 31) / 32) * 32;
-	/* rows per CTA: whole height for big batches, split when there are few frames */
-	const int K = kChunkRowsTma;
-	const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
-	int rpc = ((pl->OH + K - 1) / K) * K;
-	while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * sm_count() && rpc > 4 * K)
-		rpc = ((rpc / 2 + K - 1) / K) * K;
-	fp.RPC = rpc;
-	const dim3 grid(bands_x, (pl->OH + rpc - 1) / rpc, 1);
-	if (pl->tma3_ok) {
-		bool handled = false;
-		const int rc = pl->premul ? launch_tma3<true>(domain, pl, fp, in, is, out, os, n, grid, s, &handled)
-								  : launch_tma3<false>(domain, pl, fp, in, is, out, os, n, grid, s, &handled);
-		if (handled)
-			return rc;
-	}
-	const int np = fp.NPv == fp.NPh ? fp.NPv : 0;
-	if (np == 6)
-		return pl->premul ? launch_tma_vs<6, true>(domain, pl, fp, in, is, out, os, n, grid, s)
-						  : launch_tma_vs<6, false>(domain, pl, fp, in, is, out, os, n, grid, s);
-	if (np == 7)
-		return pl->premul ? launch_tma_vs<7, true>(domain, pl, fp, in, is, out, os, n, grid, s)
-						  : launch_tma_vs<7, false>(domain, pl, fp, in, is, out, os, n, grid, s);
-	return pl->premul ? launch_tma_vs<0, true>(domain, pl, fp, in, is, out, os, n, grid, s)
-					  : launch_tma_vs<0, false>(domain, pl, fp, in, is, out, os, n, grid, s);
+	fp.RPC = rows_per_cta(pl->OH, fp.mma_rows, 4, bands_x, n, sm_count());
+	const dim3 grid(bands_x, (pl->OH + fp.RPC - 1) / fp.RPC, nf);
+	return pl->premul ? launch_mma_list<true>(domain, pl, fp, in, is, out, os, n, f0, grid, s)
+					  : launch_mma_list<false>(domain, pl, fp, in, is, out, os, n, f0, grid, s);
 }
 
 /* The per-row / per-column sampling tables of the plan's vips_resize, stepped per rect exactly as the
@@ -1932,11 +1457,11 @@ plan_axis_tables(const ThumbnailPlanImpl *pl, AxisTable &tv, AxisTable &th)
 	build_axis_table(th, pl->OW, pl->gh.residual, pl->gh.offset, pl->gh.n_point, VB200_KERNEL_LANCZOS3, tile_w);
 }
 
-/* The tensor-pipe kernel's bands at band width tw (the last one shorter), with the input columns each loads in the
- * wcols-column layout
+/* The bands of a fused kernel at band width tw (the last one shorter), with the input columns each loads: c_lo rounded
+ * down to clo_align pixels (v2: 4; v4: v4_clo_align)
  */
 std::vector<MmaBand>
-mma_bands_of(const FusedParams &fp, const std::vector<int2> &hcol, int tw, int wcols)
+mma_bands_of(const FusedParams &fp, const std::vector<int2> &hcol, int tw, int clo_align)
 {
 	auto column_of = [&](int E0, int tt) {
 		const int e = E0 + tt / fp.HS;
@@ -1951,7 +1476,7 @@ mma_bands_of(const FusedParams &fp, const std::vector<int2> &hcol, int tw, int w
 		b.xb = std::min(xa + tw, fp.OW);
 		const int E0 = 2 * hcol[xa].x + fp.hgrid;
 		b.ne = 2 * (hcol[b.xb - 1].x + fp.NPh - hcol[xa].x);
-		b.c_lo = column_of(E0, 0) & ~(v4_clo_align(wcols, fp.HS) - 1);
+		b.c_lo = column_of(E0, 0) & ~(clo_align - 1);
 		b.c_hi = std::min(fp.W, (column_of(E0, b.ne * fp.HS - 1) + 4) & ~3);
 		bands.push_back(b);
 	}
@@ -2062,11 +1587,6 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 	fp.NT = std::min(kMaxThreads, ((nemax * fp.HS + 31) / 32) * 32);
 	fp.NT = std::max(fp.NT, 64);
 
-	/* rows per CTA: whole height when there are many frames; the batch entry
-	 * point overrides this per launch if it needs more CTAs
-	 */
-	fp.RPC = ((pl->OH + kChunkRows - 1) / kChunkRows) * kChunkRows;
-
 	/* pair slots: worst chunk */
 	int slots = 0;
 	for (int ya = 0; ya < pl->OH; ya += kChunkRows) {
@@ -2080,8 +1600,10 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 	if (pl->smem > 200 * 1024)
 		return 1;
 
-	/* v2: rows arrive by cp.async.bulk, which wants 16-byte aligned rows */
-	pl->tma_ok = false;
+	/* The kernel: v4 where its tables, bands and shared memory fit and its (VS, HS) is instantiated, else v2 where the
+	 * rows are 16-byte aligned (cp.async.bulk) and the band fits a stage, else v1.
+	 */
+	pl->kernel = FusedKernel::Ldg;
 	if ((fp.in_bpl % 16) == 0 && fp.VS <= 16) {
 		int slots2 = 0;
 		for (int ya = 0; ya < pl->OH; ya += kChunkRowsTma) {
@@ -2089,47 +1611,28 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 			slots2 = std::max(slots2, vrow[yb - 1].x + fp.NPv - 1 - vrow[ya].x + 1);
 		}
 		/* widest band, in input columns rounded out to 4-pixel (16-byte) bounds */
-		auto column_of = [&](int E0, int tt) {
-			const int e = E0 + tt / fp.HS;
-			const int k = tt % fp.HS;
-			const int sc = std::max(0, std::min(e - fp.hembed, fp.Ws - 1));
-			return std::min(sc * fp.HS + k, fp.W - 1);
-		};
 		int max_cols = 0;
-		for (int xa = 0; xa < pl->OW; xa += TW) {
-			const int xb = std::min(xa + TW, pl->OW);
-			const int E0 = 2 * hcol[xa].x + hgrid;
-			const int ne = 2 * (hcol[xb - 1].x + fp.NPh - hcol[xa].x);
-			const int c_lo = column_of(E0, 0) & ~3;
-			const int c_hi = std::min(fp.W, (column_of(E0, ne * fp.HS - 1) + 4) & ~3);
-			max_cols = std::max(max_cols, c_hi - c_lo);
-		}
+		for (const MmaBand &b : mma_bands_of(fp, hcol, TW, 4))
+			max_cols = std::max(max_cols, b.c_hi - b.c_lo);
 		fp.stage_pitch = kStagePitch;
 		pl->slots_tma = slots2;
 		const int nc = ((fp.NT / kColsPerThread + 31) / 32) * 32 * kColsPerThread; /* buffer columns of the v2 kernel */
 		pl->smem_tma = (size_t) kStages * 2 * fp.VS * kStagePitch + 2 * kStages * 8 + (size_t) slots2 * nc * 8 +
 			(size_t) kChunkRowsTma * nc * 4 + (size_t) kChunkRowsTma * (nemax / 2) * 8 +
 			(size_t) (fp.nvsets * fp.NPv + fp.nhsets * fp.NPh + 256) * 4;
-		pl->smem_tma3 = (size_t) kStages * 2 * fp.VS * kStagePitch + (2 * kStages + 4) * 8 + (size_t) slots2 * nc * 8 +
-			(size_t) 2 * kChunkRowsTma * (nemax / 2) * 8 + (size_t) (fp.nvsets * fp.NPv + fp.nhsets * fp.NPh + 256) * 4;
-		pl->tma3_ok = (fp.HS == 2 || fp.HS == 4 || fp.HS == 8) && max_cols * 4 <= kStagePitch &&
-			pl->smem_tma3 <= 113 * 1024 && fp.max_alpha == 255.0 && getenv("VB200_NO_TMA3") == nullptr &&
-			getenv("VB200_NO_TMA") == nullptr;
-		pl->tma_ok = max_cols * 4 <= kStagePitch && pl->smem_tma <= 113 * 1024 && fp.max_alpha == 255.0 &&
-			getenv("VB200_NO_TMA") == nullptr;
+		if (max_cols * 4 <= kStagePitch && pl->smem_tma <= 113 * 1024 && fp.max_alpha == 255.0)
+			pl->kernel = FusedKernel::Tma;
 	}
 
-	/* v4: reducev as u8 x s8 MMAs over a ring of 8 quads (32 box-shrunk rows) per 8 output rows */
-	pl->mma_ok = false;
-	/* (not gated on tma_ok: the older TMA kernels' shared-memory bound fails for box 8, this kernel's does not) */
-	const bool vpow2 = fp.VS == 2 || fp.VS == 4 || fp.VS == 8, hpow2 = fp.HS == 2 || fp.HS == 4 || fp.HS == 8;
-	/* the (VS, HS) corners launch_mma_w instantiates: powers of two freely mixed; otherwise boxes 2 .. 8 that
-	 * differ by at most one (what a uniform shrink gives)
+	/* v4: reducev as u8 x s8 MMAs over a ring of 8 quads (32 box-shrunk rows) per 8 output rows.  Not gated on v2: v2's
+	 * shared-memory bound fails for box 8, this kernel's does not.
 	 */
-	const bool mma_pair = (vpow2 && hpow2) ||
-		(fp.VS >= 2 && fp.VS <= 8 && fp.HS >= 2 && fp.HS <= 8 && abs(fp.VS - fp.HS) <= 1 && getenv("VB200_NO_MMA_NPOT") == nullptr);
-	if ((fp.in_bpl % 16) == 0 && fp.max_alpha == 255.0 && getenv("VB200_NO_TMA") == nullptr && mma_pair &&
-		getenv("VB200_NO_MMA") == nullptr) {
+	const bool hpow2 = fp.HS == 2 || fp.HS == 4 || fp.HS == 8;
+	/* with a power-of-two horizontal box a V thread loads its two columns as one 8-byte word: not where the last box
+	 * runs past the frame's edge (W = 8k + 4 at box 8) and its columns replicate the odd last one
+	 */
+	const bool pairs_aligned = !hpow2 || fp.Ws * fp.HS <= fp.W;
+	if ((fp.in_bpl % 16) == 0 && fp.max_alpha == 255.0 && pairs_aligned && v4_np(fp.VS, fp.NPh, fp.HS) >= 0) {
 		std::vector<int> vchunk_flat;
 		std::vector<unsigned> bfrag_flat;
 		const int K = pick_mma_rows(tv, pl->OH, vchunk_flat, bfrag_flat); /* 0: no chunking fits the ring */
@@ -2142,26 +1645,22 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 			memcpy(vchunk.data(), vchunk_flat.data(), vchunk.size() * sizeof(int2));
 			memcpy(bfrag.data(), bfrag_flat.data(), bfrag.size() * sizeof(uint4));
 		}
-		/* band width: the fewest bands whose widest one fits the column budget */
-		const char *ev = getenv("VB200_V4_COLS");
-		const int wcols = ev && atoi(ev) <= 448 && vpow2 && hpow2 ? VB200_V4_COLS : 768; /* 768 (default): one CTA per SM, two columns per thread */
 		/* logical columns a V warp covers: 64, or 2 * floor(32 / HS) * HS when the horizontal box is not a
 		 * power of two (V4Group in thumbnail_fused_mma.cuh)
 		 */
 		const int warp_cols = hpow2 ? 0 : 2 * (32 / fp.HS) * fp.HS;
-		pl->mma_cpt = wcols > 448 || (getenv("VB200_V4_CPT") && atoi(getenv("VB200_V4_CPT")) == 2) ? 2 : 1; /* columns per V thread */
-		const int pitch = v4_nbox(wcols, fp.HS) * v4_boxw(wcols, fp.HS) * 4;
+		const int pitch = v4_nbox(fp.HS) * v4_boxw(fp.HS) * 4;
 		/* band width: the one that needs the fewest V warps over a frame row (warps past a band's last
 		 * column exit at once, so a narrow last band is cheap); ties go to the wider band
 		 */
 		int tw4 = 0, nemax4 = 0;
 		long best_cost = LONG_MAX;
-		const int cols_per_warp = warp_cols ? warp_cols : 32 * pl->mma_cpt;
-		const int col_budget = warp_cols ? (wcols / 64) * warp_cols : wcols;
+		const int cols_per_warp = warp_cols ? warp_cols : 32 * kV4Cpt;
+		const int col_budget = warp_cols ? (kV4Cols / (32 * kV4Cpt)) * warp_cols : kV4Cols;
 		for (int tw = std::min(pl->OW, 256); tw >= 2 && ok; tw--) {
 			int worst = 0, max_cols = 0;
 			long cost = 0;
-			for (const MmaBand &b : mma_bands_of(fp, hcol, tw, wcols)) {
+			for (const MmaBand &b : mma_bands_of(fp, hcol, tw, v4_clo_align(fp.HS))) {
 				worst = std::max(worst, b.ne);
 				max_cols = std::max(max_cols, b.c_hi - b.c_lo);
 				cost += (b.ne * fp.HS + cols_per_warp - 1) / cols_per_warp + 1; /* + the H / P warps' share */
@@ -2173,23 +1672,22 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 			}
 		}
 		if (ok && tw4 > 0) {
-			pl->mma_cols = wcols;
 			pl->mma_tw = tw4;
 			pl->mma_nemax = nemax4;
 			pl->mma_nt = warp_cols ? std::max(64, ((nemax4 * fp.HS + warp_cols - 1) / warp_cols) * 32)
-								   : std::max(64, ((nemax4 * fp.HS / pl->mma_cpt + 31) / 32) * 32);
+								   : std::max(64, ((nemax4 * fp.HS / kV4Cpt + 31) / 32) * 32);
 			const int stages = fp.VS <= 2 ? 2 * VB200_V4_STAGES
 				: (fp.VS >= 7 ? VB200_V4_STAGES / 2 : (fp.VS >= 5 ? (3 * VB200_V4_STAGES) / 4 : VB200_V4_STAGES));
-			const int logical_cols = warp_cols ? (pl->mma_nt / 32) * warp_cols : pl->mma_nt * pl->mma_cpt;
-			pl->mma_bands = mma_bands_of(fp, hcol, tw4, wcols);
-			const int nbox = v4_nbox(wcols, fp.HS);
+			const int logical_cols = warp_cols ? (pl->mma_nt / 32) * warp_cols : pl->mma_nt * kV4Cpt;
+			pl->mma_bands = mma_bands_of(fp, hcol, tw4, v4_clo_align(fp.HS));
+			const int nbox = v4_nbox(fp.HS);
 			const size_t box_bytes = ((size_t) 2 * fp.VS * (pitch / nbox) + 127) & ~(size_t) 127;
 			pl->smem_mma = (size_t) stages * nbox * box_bytes + (2 * stages + 4) * 8 +
-				(size_t) kV4Quads * ((size_t) pl->mma_nt * pl->mma_cpt * 16 + 16) +
+				(size_t) kV4Quads * ((size_t) pl->mma_nt * kV4Cpt * 16 + 16) +
 				(size_t) 2 * kV4Rows * ((logical_cols / fp.HS + 1) / 2) * 8 +
 				(size_t) (fp.nhsets * fp.NPh + 256) * 4;
 			const size_t n_ch = vchunk.size() * sizeof(int2), n_bf = bfrag.size() * sizeof(uint4);
-			if (pl->smem_mma <= (wcols > 448 ? 226 : 113) * 1024) {
+			if (pl->smem_mma <= 226 * 1024) {
 				if (!pl->geometry_only) {
 					VB200_CUDA(domain, cudaMalloc(&pl->tables_mma, n_bf + n_ch));
 					VB200_CUDA(domain, cudaMemcpy(pl->tables_mma, bfrag.data(), n_bf, cudaMemcpyHostToDevice));
@@ -2197,7 +1695,7 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 					fp.vbfrag = (const uint4 *) pl->tables_mma;
 					fp.vchunk = (const int2 *) ((char *) pl->tables_mma + n_bf);
 				}
-				pl->mma_ok = true;
+				pl->kernel = FusedKernel::Mma;
 			}
 		}
 	}
@@ -2219,8 +1717,6 @@ plan_build_fused(const char *domain, ThumbnailPlanImpl *pl)
 	fp.hcol = (const int2 *) (b + n_vrow);
 	fp.vcoef = (const int *) (b + n_vrow + n_hcol);
 	fp.hcoef = (const int *) (b + n_vrow + n_hcol + n_vc);
-
-	pl->grid = dim3((pl->OW + TW - 1) / TW, (pl->OH + fp.RPC - 1) / fp.RPC, 1);
 	return 0;
 }
 
@@ -2627,33 +2123,48 @@ thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const vo
 	return 0;
 }
 
-/* the fused kernels over RGBA frames */
+/* the fused kernels over RGBA frames: the plan's kernel, but v1 when the base pointer or the frame stride of a batch
+ * is off 16 bytes (the TMA-fed kernels copy whole 16-byte units); frames in chunks of at most kMaxBatchFrames (gridDim.z)
+ */
 static int
 thumbnail_plan_run_fused(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
 	size_t out_stride, int n, cudaStream_t s)
 {
-	{
-		/* the TMA-fed kernel when rows, frames and the base pointer are 16-byte aligned */
-		if ((pl->tma_ok || pl->mma_ok) && (((uintptr_t) in) & 15) == 0 && (n == 1 || (in_stride & 15) == 0)) {
-			bool handled = true;
-			const int rc = launch_tma(domain, pl, in, in_stride, out, out_stride, n, s, &handled);
-			if (handled)
-				return rc;
+	const bool aligned = (((uintptr_t) in) & 15) == 0 && (n == 1 || (in_stride & 15) == 0);
+	const FusedKernel kernel = aligned ? pl->kernel : FusedKernel::Ldg;
+	for (int f0 = 0; f0 < n; f0 += kMaxBatchFrames) {
+		const int nf = std::min(kMaxBatchFrames, n - f0);
+		int rc = 0;
+		switch (kernel) {
+		case FusedKernel::Ldg: rc = launch_ldg(domain, pl, in, in_stride, out, out_stride, n, f0, nf, s); break;
+		case FusedKernel::Tma: rc = launch_tma(domain, pl, in, in_stride, out, out_stride, n, f0, nf, s); break;
+		case FusedKernel::Mma: rc = launch_mma(domain, pl, in, in_stride, out, out_stride, n, f0, nf, s); break;
 		}
-		/* enough CTAs to fill the machine: split rows when the batch is small.  This (fallback) path
-		 * writes the per-launch geometry into the plan: serialise concurrent callers of one plan
-		 */
-		std::lock_guard<std::mutex> launch_lock(pl->launch_lock);
-		FusedParams &fp = pl->fp;
-		const int bands_x = (pl->OW + fp.TW - 1) / fp.TW;
-		int rpc = ((pl->OH + kChunkRows - 1) / kChunkRows) * kChunkRows;
-		while ((long long) bands_x * ((pl->OH + rpc - 1) / rpc) * n < 2 * sm_count() && rpc > 2 * kChunkRows)
-			rpc = ((rpc / 2 + kChunkRows - 1) / kChunkRows) * kChunkRows;
-		fp.RPC = rpc;
-		pl->grid = dim3(bands_x, (pl->OH + rpc - 1) / rpc, 1);
-		return pl->premul ? launch_fused_vs<true>(domain, pl, in, in_stride, out, out_stride, n, s)
-						  : launch_fused_vs<false>(domain, pl, in, in_stride, out, out_stride, n, s);
+		if (rc)
+			return rc;
 	}
+	return 0;
+}
+
+/* vb200_thumbnail_plan_kernel's name of the kernel a plan runs, in buf or a static string */
+static const char *
+plan_kernel_name(const ThumbnailPlanImpl &pl, char *buf, size_t cap)
+{
+	if (!pl.fused)
+		return "leaf kernels";
+	if (pl.linear)
+		return "linear_v_kernel + linear_h_kernel";
+	const FusedParams &fp = pl.fp;
+	const char *alpha = pl.premul ? "premul" : "plain";
+	switch (pl.kernel) {
+	case FusedKernel::Mma:
+		snprintf(buf, cap, "thumbnail_fused_mma_kernel<VS=%d,NP=%d,%s,HS=%d,cols=%d,cpt=%d>", fp.VS, v4_np(fp.VS, fp.NPh, fp.HS), alpha,
+			fp.HS, kV4Cols, kV4Cpt);
+		break;
+	case FusedKernel::Tma: snprintf(buf, cap, "thumbnail_fused_tma_kernel<VS=%d,%s>", fp.VS, alpha); break;
+	case FusedKernel::Ldg: snprintf(buf, cap, "thumbnail_fused_kernel<VS=%d,%s>", fp.VS, alpha); break;
+	}
+	return buf;
 }
 
 void
@@ -2794,28 +2305,14 @@ vb200_thumbnail_plan_is_fused(const VB200ThumbnailPlan *plan)
 	return plan && plan->impl.fused;
 }
 
+/* See vb200.h: the plan's kernel, which a batch call runs unless its frames are off 16 bytes */
 extern "C" const char *
 vb200_thumbnail_plan_kernel(const VB200ThumbnailPlan *plan)
 {
 	static thread_local char name[160];
-	if (!plan || !plan->impl.fused)
+	if (!plan)
 		return "leaf kernels";
-	const ThumbnailPlanImpl &pl = plan->impl;
-	if (pl.linear)
-		return "linear_v_kernel + linear_h_kernel";
-	const FusedParams &fp = pl.fp;
-	const int nph = fp.NPh == 6 || fp.NPh == 7 ? fp.NPh : 0;
-	const bool v4 = pl.mma_ok;
-	if (v4)
-		snprintf(name, sizeof(name), "thumbnail_fused_mma_kernel<VS=%d,NP=%d,%s,HS=%d,cols=%d,cpt=%d>", fp.VS, nph,
-			pl.premul ? "premul" : "plain", fp.HS, pl.mma_cols, pl.mma_cpt);
-	else if (pl.tma3_ok)
-		snprintf(name, sizeof(name), "thumbnail_fused_tma3_kernel<VS=%d,%s,HS=%d>", fp.VS, pl.premul ? "premul" : "plain", fp.HS);
-	else if (pl.tma_ok)
-		snprintf(name, sizeof(name), "thumbnail_fused_tma_kernel<VS=%d,%s>", fp.VS, pl.premul ? "premul" : "plain");
-	else
-		snprintf(name, sizeof(name), "thumbnail_fused_kernel<VS=%d,%s>", fp.VS, pl.premul ? "premul" : "plain");
-	return name;
+	return plan_kernel_name(plan->impl, name, sizeof(name));
 }
 
 extern "C" int
@@ -3273,7 +2770,7 @@ vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_wi
 	pl.geometry_only = true;
 	if (thumbnail_plan_init("debug_thumbnail_bands", &pl))
 		return -1;
-	if (!pl.fused || !pl.mma_ok)
+	if (!pl.fused || pl.kernel != FusedKernel::Mma)
 		return 1;
 	const int nb = (int) pl.mma_bands.size();
 	if (nb > cap)
@@ -3288,7 +2785,36 @@ vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_wi
 		c_hi[b] = m.c_hi;
 		seam[b] = b + 1 < nb ? std::max(0, m.c_hi - pl.mma_bands[b + 1].c_lo) : 0;
 	}
-	*n_box = v4_nbox(pl.mma_cols, pl.fp.HS); /* the boxes launch_mma_t gives the stage tensor map */
-	*box_width = v4_boxw(pl.mma_cols, pl.fp.HS);
+	*n_box = v4_nbox(pl.fp.HS); /* the boxes launch_mma_t gives the stage tensor map */
+	*box_width = v4_boxw(pl.fp.HS);
+	return 0;
+}
+
+/* Test hook (tests/test_thumbnail_kernel_choice.py, CPU): vb200_thumbnail_plan_kernel's name for the plan
+ * vb200_thumbnail_plan_new would build, planned without a device.  See vb200.h.
+ */
+extern "C" int
+vb200_debug_thumbnail_kernel(int width, int height, int bands, int has_alpha, int target_width, int target_height, int size,
+	char *name, int cap)
+{
+	if (width <= 0 || height <= 0 || bands <= 0 || target_width <= 0 || !name || cap <= 0)
+		return -1;
+	ThumbnailPlanImpl pl;
+	pl.W = width;
+	pl.H = height;
+	pl.bands = bands;
+	pl.fmt = VB200_FORMAT_UCHAR;
+	pl.has_alpha = has_alpha;
+	pl.target_w = target_width;
+	pl.target_h = target_height > 0 ? target_height : target_width;
+	pl.size = size;
+	pl.geometry_only = true;
+	if (thumbnail_plan_init("debug_thumbnail_kernel", &pl))
+		return -1;
+	char buf[160];
+	const char *k = plan_kernel_name(pl, buf, sizeof(buf));
+	if ((int) strlen(k) >= cap)
+		return -1;
+	strcpy(name, k);
 	return 0;
 }

@@ -1,8 +1,8 @@
 /* thumbnail_fused_mma.cuh -- v4 of the fused thumbnail kernel (included by
- * thumbnail_fused.cu inside its anonymous namespace, after v3).
+ * thumbnail_fused.cu inside its anonymous namespace).
  *
- * v3 is bound by the alu pipe, and 45% of its alu work is the reducev pass:
- * 48 IDP.2A per thread per output row.  v4 hands exactly that sum to the
+ * The dp2a form of this kernel is bound by the alu pipe, and 45% of its alu work is the
+ * reducev pass: 48 IDP.2A per thread per output row.  v4 hands exactly that sum to the
  * integer tensor-core path (legacy mma.sync m16n8k32, u8 x s8 -> s32, exact):
  *
  *     D[colchan][y] = sum_k  data[colchan][k] * coef[k][y]
@@ -16,69 +16,37 @@
  * This is not a GEMM reformulation for its own sake: the tensor pipe is ~3% busy; it is
  * used as a wide dot-product unit to take 3 alu instructions per input pixel off the
  * pipe that bounds the kernel.  Everything else (premultiply, box sums, shrinkh,
- * reduceh on the H warp, unpremultiply) is v3's arithmetic.
+ * reduceh on the H warps, unpremultiply) is the dp2a kernels' arithmetic.
  *
- * Warp roles:  12 V warps (COLS / (32 CPT); CPT = columns per thread) | NH H warps | 1 producer warp.
- * Each V warp owns 32 CPT columns end to end -- it writes the quads of its columns and runs the
- * MMAs over them -- so the only synchronisation inside the V side is __syncwarp().  NH (3 or 4) is
- * chosen so that each SM sub-partition (warp slot % 4) carries the same number of V warps and the
- * same share of the reduceh work: a TMA stage is refilled only when every V warp has read it, so
- * the V warp on the most loaded sub-partition sets the pace of the CTA.
+ * Warp roles:  12 V warps (768 columns, 2 per thread) | 3 H warps | 1 producer warp.
+ * Each V warp owns 64 columns end to end -- it writes the quads of its columns and runs the
+ * MMAs over them -- so the only synchronisation inside the V side is __syncwarp().  The H warp
+ * count is chosen so that each SM sub-partition (warp slot % 4) carries the same number of V warps
+ * and the same share of the reduceh work: a TMA stage is refilled only when every V warp has read
+ * it, so the V warp on the most loaded sub-partition sets the pace of the CTA.
  *
  * Shared memory:
  *   stages  [S][NBOX][2 VS][PITCH]  raw RGBA rows as NBOX tiled-TMA boxes (a stage = 2 shrunk rows)
  *   bars    full[S] empty[S] shfull[2] shempty[2]
  *   quadbuf [8][NC][4] u32 (+16 B per quad slot: conflict-free A-fragment loads)
- *   sh      [2][8][NC / HS / 2] uint2  reducev + shrinkh output, v3's pair layout
+ *   sh      [2][8][NC / HS / 2] uint2  reducev + shrinkh output, v1 / v2's pair layout
  *   hcoef, uscale
  */
 
 constexpr int kV4Rows = 8;	/* output rows per chunk: N of the MMA */
 constexpr int kV4Quads = 8; /* quad ring: K / 4 */
+constexpr int kV4Cols = 768; /* columns per CTA: one CTA per SM */
+constexpr int kV4Cpt = 2;	 /* adjacent columns per V thread */
 
-/* tuning knobs (compile time): columns per CTA and TMA stages for the VS 4 case */
-#ifndef VB200_V4_COLS
-#define VB200_V4_COLS 384
-#endif
+/* tuning knobs (compile time) */
 #ifndef VB200_V4_STAGES
-#define VB200_V4_STAGES 4
+#define VB200_V4_STAGES 4 /* TMA stages for the VS 4 case */
 #endif
 #ifndef VB200_V4_NH768
-#define VB200_V4_NH768 3 /* H warps of the 768-column configuration (3: 74.3%, 4: 73.2% of HBM at 296 frames) */
+#define VB200_V4_NH768 3 /* H warps (3: 74.3%, 4: 73.2% of HBM at 296 frames) */
 #endif
 #ifndef VB200_V4_MMA_UNROLL
 #define VB200_V4_MMA_UNROLL 2
-#endif
-/* long waits poll on a timer instead of parking on the barrier unit (mbar_wait_poll): 0 = try_wait */
-#ifndef VB200_V4_HPOLL_NS
-#define VB200_V4_HPOLL_NS 0 /* the H warps' wait for a chunk of reducev output */
-#endif
-#ifndef VB200_V4_PPOLL_NS
-#define VB200_V4_PPOLL_NS 0 /* the producer's wait for a stage to be released */
-#endif
-#ifndef VB200_V4_VPOLL_NS
-#define VB200_V4_VPOLL_NS 0 /* the V warps' wait for a TMA stage (latency-critical) */
-#endif
-#ifndef VB200_V4_EPOLL_NS
-#define VB200_V4_EPOLL_NS 0 /* the V warps' wait for the H warps to release an sh buffer */
-#endif
-
-/* timing experiment only: VB200_EXP_NOPREMUL drops the premultiply arithmetic (wrong pixels) */
-#ifndef VB200_V4_HADD2
-#define VB200_V4_HADD2 1 /* box sums on the half2 adder (hadd2_lanes) */
-#endif
-#ifdef VB200_EXP_NOPREMUL
-#define V4_ACC_PREMUL false
-#else
-#define V4_ACC_PREMUL PREMUL
-#endif
-
-#if VB200_V4_HADD2
-#define V4_ACC(x, rb, ga) accumulate_pixel_h<V4_ACC_PREMUL>(x, k16, rb, ga)
-#define V4_ACCO(x, rb, ga) accumulate_pixel_h<false>(x, k16, rb, ga)
-#else
-#define V4_ACC(x, rb, ga) accumulate_pixel_m<V4_ACC_PREMUL>(x, accm, k16, rb, ga)
-#define V4_ACCO(x, rb, ga) accumulate_pixel_m<false>(x, accm, k16, rb, ga)
 #endif
 
 /* Opaque stages.  scale[255] is 256 (premultiply.c:253-259), so a pixel whose alpha is 255 premultiplies to
@@ -92,29 +60,18 @@ constexpr int kV4Quads = 8; /* quad ring: K / 4 */
  * never waited for), and inside it only hinted frames vote.
  */
 constexpr int kV4OpaqueSkip = 7;
-#ifndef VB200_V4_OPAQUE
-#define VB200_V4_OPAQUE 1 /* 0: the OPQ instantiations are never used */
-#endif
 
 /* H warps per CTA: the reduceh work of a chunk is ~2/3 of a V warp's; one H warp overloads its SM
  * sub-partition (the V warps there set the pace for all), so it is spread over several
  */
-template <int CPT>
-struct V4HWarps {
-	static constexpr int value = CPT == 1 ? 3 : 2;
-};
-template <int WCOLS, int CPT>
-struct V4HWarpsW {
-	static constexpr int value = WCOLS > 448 ? VB200_V4_NH768 : V4HWarps<CPT>::value;
-};
+constexpr int kV4HWarps = VB200_V4_NH768;
 
 /* A stage row is loaded as v4_nbox tiled-TMA boxes of v4_boxw pixels (a box is at most 256 u64 = 512 pixels wide),
- * from the band's first input column rounded down to v4_clo_align pixels.  In the 768-column layout a row starts on a
- * 128-byte line and is 13 whole lines per box (2 x 416 pixels): the same bands fed from 16-byte-aligned columns in
- * 2 x 388-pixel boxes ran 2.8% slower on an H100 (12.54 against 12.19 ms per 512 4K frames), because rows that start
- * or end inside a line cost the L2 and DRAM partial lines.  Where the shared memory has no room for that -- the
- * 384-column layout (2 CTAs per SM) and a horizontal box of 2 (sh buffers twice as large) -- rows stay 392 / 776
- * pixels from 16-byte columns.
+ * from the band's first input column rounded down to v4_clo_align pixels.  A row starts on a 128-byte line and is 13
+ * whole lines per box (2 x 416 pixels): the same bands fed from 16-byte-aligned columns in 2 x 388-pixel boxes ran
+ * 2.8% slower on an H100 (12.54 against 12.19 ms per 512 4K frames), because rows that start or end inside a line
+ * cost the L2 and DRAM partial lines.  Where the shared memory has no room for that -- a horizontal box of 2 (sh
+ * buffers twice as large) -- rows stay 776 pixels from 16-byte columns.
  */
 #ifndef VB200_V4_BOXPAD
 #define VB200_V4_BOXPAD 64 /* pixels of a line-aligned stage row beyond the band's column budget */
@@ -123,24 +80,24 @@ struct V4HWarpsW {
 #define VB200_V4_CLO_ALIGN 32 /* pixels, a power of two: 32 = one 128-byte line */
 #endif
 constexpr bool
-v4_lines(int wcols, int hs)
+v4_lines(int hs)
 {
-	return wcols > 448 && hs > 2;
+	return hs > 2;
 }
 constexpr int
-v4_clo_align(int wcols, int hs)
+v4_clo_align(int hs)
 {
-	return v4_lines(wcols, hs) ? VB200_V4_CLO_ALIGN : 4;
+	return v4_lines(hs) ? VB200_V4_CLO_ALIGN : 4;
 }
 constexpr int
-v4_nbox(int wcols, int hs)
+v4_nbox(int hs)
 {
-	return wcols + (v4_lines(wcols, hs) ? VB200_V4_BOXPAD : 8) > 512 ? 2 : 1;
+	return kV4Cols + (v4_lines(hs) ? VB200_V4_BOXPAD : 8) > 512 ? 2 : 1;
 }
 constexpr int
-v4_boxw(int wcols, int hs)
+v4_boxw(int hs)
 {
-	return (wcols + (v4_lines(wcols, hs) ? VB200_V4_BOXPAD : 8)) / v4_nbox(wcols, hs);
+	return (kV4Cols + (v4_lines(hs) ? VB200_V4_BOXPAD : 8)) / v4_nbox(hs);
 }
 
 template <int VS>
@@ -191,8 +148,8 @@ v4_finish(int hi, int lo, int k20)
 	return max(0, min(v, 255));
 }
 
-template <int VS, int NP, bool PREMUL, int HSQ, int WCOLS, int CPT, bool OPQ = false>
-__global__ void __launch_bounds__(WCOLS / CPT + 32 * V4HWarpsW<WCOLS, CPT>::value + 32, WCOLS <= 448 ? 2 : 1)
+template <int VS, int NP, bool PREMUL, int HSQ, bool OPQ = false>
+__global__ void __launch_bounds__(kV4Cols / kV4Cpt + 32 * kV4HWarps + 32, 1)
 thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_constant__ CUtensorMap tmap, int use_tmap,
 	const uint8_t *__restrict__ in, size_t in_frame_stride, uint8_t *__restrict__ out, size_t out_frame_stride, int frame0)
 {
@@ -201,11 +158,12 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	constexpr int KM = kV4Rows; /* rows the sh buffers hold */
 	const int K = P.mma_rows;   /* output rows per chunk, 4 .. 8: as many as keep every chunk's tap window inside the 32-row ring */
 	constexpr int S = V4Stages<VS>::value;
-	constexpr int NH = V4HWarpsW<WCOLS, CPT>::value;
+	constexpr int NH = kV4HWarps;
+	constexpr int CPT = kV4Cpt;
 	constexpr int kMmaUnroll = VB200_V4_MMA_UNROLL;
 	/* a stage row is held as NBOX column boxes (a tiled-TMA box is at most 256 elements = 512 pixels wide) */
-	constexpr int NBOX = v4_nbox(WCOLS, HSQ);
-	constexpr int BOXW = v4_boxw(WCOLS, HSQ); /* pixels */
+	constexpr int NBOX = v4_nbox(HSQ);
+	constexpr int BOXW = v4_boxw(HSQ); /* pixels */
 	static_assert(BOXW % 4 == 0 && BOXW <= 512, "a box row is whole 16-byte units, at most 256 u64 elements");
 	constexpr int PITCH = BOXW * 4;			 /* bytes between rows of a box */
 	constexpr int NPR = NP > 0 ? NP : 1;
@@ -213,7 +171,6 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	constexpr bool VPOW2 = (VS & (VS - 1)) == 0;
 	constexpr bool HPOW2 = V4Group<HSQ>::pow2;
 	constexpr int G = V4Group<HSQ>::value; /* logical columns per jj group; 2 G per warp */
-	static_assert(HPOW2 || CPT == 2, "non-power-of-two horizontal boxes are built for two columns per thread");
 	constexpr int rows_per_stage = 2 * VS;
 	constexpr unsigned box_bytes = ((unsigned) rows_per_stage * PITCH + 127u) & ~127u; /* a tiled-TMA destination is 128-byte aligned */
 	constexpr unsigned stage_bytes = NBOX * box_bytes;
@@ -263,7 +220,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 		const int sc = max(0, min(e - P.hembed, P.Ws - 1));
 		return min(sc * HSQ + k, P.W - 1);
 	};
-	const int c_lo = column_of(0) & ~(v4_clo_align(WCOLS, HSQ) - 1);
+	const int c_lo = column_of(0) & ~(v4_clo_align(HSQ) - 1);
 	const int c_hi = min(P.W, (column_of(NE * HSQ - 1) + 4) & ~3);
 	const unsigned row_bytes = (unsigned) (c_hi - c_lo) * 4u;
 	const int chunk0 = y_begin / K; /* RPC is a multiple of K: chunk c of this CTA is table entry chunk0 + c */
@@ -296,10 +253,13 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 		for (int ya = y_begin, cc = chunk0; ya < y_end; ya += K, cc++) {
 			const int P1 = 2 * __ldg(&P.vchunk[cc]).y + 1; /* last pair of the chunk's last quad */
 			for (int p = pdone; p <= P1; p++) {
-				if (VB200_V4_PPOLL_NS)
-					mbar_wait_poll(empty_s + 8u * s, phase ^ 1u, VB200_V4_PPOLL_NS);
-				else
+				/* do .. while (0) keeps the block layout nvcc gives this loop's branch on `interior`: written as a plain
+				 * statement, the wait moved the TMA path and the headline ran 0.4% slower on an H100 (12.53 against
+				 * 12.48 ms per 512 4K frames)
+				 */
+				do
 					mbar_wait(empty_s + 8u * s, phase ^ 1u);
+				while (0);
 				/* interior stage: its 2 VS input rows are consecutive and none is an edge replica --
 				 * one tiled-TMA box {PITCH bytes, 2 VS rows} instead of 2 VS row copies
 				 */
@@ -343,7 +303,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	}
 
 	if (t >= NT) {
-		/* ---------------- H: reduceh + unpremultiply + store, one warp (v3's) */
+		/* ---------------- H: reduceh + unpremultiply + store, NH warps */
 		const int ht = t - NT; /* 0 .. 32 NH - 1 */
 		const int lane = ht & 31;
 		const int bw = xb - xa;
@@ -353,10 +313,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 			const int rows = yb - ya;
 			const int buf = chunk & 1;
 			const uint2 *shb = sh + (size_t) buf * KM * shs;
-			if (VB200_V4_HPOLL_NS)
-				mbar_wait_poll(shfull_s + 8u * buf, (unsigned) (chunk >> 1) & 1u, VB200_V4_HPOLL_NS);
-			else
-				mbar_wait(shfull_s + 8u * buf, (unsigned) (chunk >> 1) & 1u);
+			mbar_wait(shfull_s + 8u * buf, (unsigned) (chunk >> 1) & 1u);
 			for (int idx = ht; idx < rows * bw; idx += 32 * NH) {
 				const int k = fast_div(idx, bw);
 				const int x = xa + (idx - k * bw);
@@ -408,8 +365,9 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	if (t >= NTa)
 		return;
 	/* CPT 2: the thread's two columns are adjacent and start on an even column (one 64-bit LDS per row) when the
-	 * horizontal box is even; with an odd box a pair can straddle two boxes (or a replicated edge box) and the
-	 * two columns are addressed separately.  Logical column tt of the band: with G < 32 the last 32 - G slots of
+	 * horizontal box is a power of two (the plan keeps such boxes off frames whose last box is cut short, where a
+	 * column would be the replicated last one); with a box of 3, 5, 6 or 7 a pair can straddle two boxes (or be
+	 * replicated edge columns) and the two columns are addressed separately.  Logical column tt of the band: with G < 32 the last 32 - G slots of
 	 * each half-warp group idle (they repeat the group's last column).
 	 */
 	const int lane_ = t & 31;
@@ -417,15 +375,15 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 						  : (t >> 5) * 2 * G + (lane_ >> 4) * G + min((lane_ & 15) * 2, G - 2);
 	const int my_c = column_of(min(tt0, NE * HSQ - CPT)) - c_lo;
 	const unsigned char *my_cols = stages + (size_t) (my_c / BOXW) * box_bytes + (size_t) (my_c % BOXW) * 4u;
-	constexpr bool PAIR64 = (HSQ & 1) == 0;
+	constexpr bool PAIR64 = HPOW2;
 	const int my_c1 = column_of(min(tt0 + 1, NE * HSQ - 1)) - c_lo;
 	const unsigned char *my_cols1 = stages + (size_t) (my_c1 / BOXW) * box_bytes + (size_t) (my_c1 % BOXW) * 4u;
-	const unsigned accm = P.accmul; /* run-time on purpose: keeps the accumulation on IMAD */
+	const unsigned accm = P.accmul;
 	unsigned k16;
 	asm volatile("mov.u32 %0, 0x10000;" : "=r"(k16));
 	int k20;
 	asm volatile("mov.u32 %0, 0x100000;" : "=r"(k20));
-	const unsigned amend2 = (unsigned) (VS / 2) * (VB200_V4_HADD2 || !VPOW2 ? 1u : accm) * 0x00010001u;
+	const unsigned amend2 = (unsigned) (VS / 2) * 0x00010001u;
 	const unsigned vmul8 = P.vmul8, hmul8 = P.hmul8; /* ((1 << 32) / (256 * box)) << 8: umulhi gives ((sum) * mult) >> 24 */
 	const int lane = t & 31;
 	const bool lane0 = lane == 0;
@@ -437,7 +395,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 	 */
 	const unsigned char *a_base = quadbuf + (size_t) tig * QS + (size_t) (warp_col0 + (HPOW2 ? 4 : 32) * jj) * 16u + (unsigned) ch * 4u;
 	unsigned char *q_store = quadbuf + (size_t) (t * CPT) * 16u;
-	/* sh store: v3's pair layout, [rA rB bA bB gA gB aA aB] per column pair */
+	/* sh store: v1 / v2's pair layout, [rA rB bA bB gA gB aA aB] per column pair */
 	const int ch_off = ch == 0 ? 0 : ch == 1 ? 4 : ch == 2 ? 2 : 6;
 	const int warp_sx0 = HPOW2 ? warp_col0 / HSQ : (t >> 5) * (2 * G / HSQ) + jj * (G / HSQ);
 
@@ -462,98 +420,54 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 #pragma unroll
 			for (int half = 0; half < 2; half++) {
 				const unsigned soff = (unsigned) s * stage_bytes;
-				if (VB200_V4_VPOLL_NS)
-					mbar_wait_poll(full_s + 8u * s, phase, VB200_V4_VPOLL_NS);
-				else
-					mbar_wait(full_s + 8u * s, phase);
-				if (CPT == 2) {
-					uint2 pa[VS], pb[VS];
+				mbar_wait(full_s + 8u * s, phase);
+				uint2 pa[VS], pb[VS];
 #pragma unroll
-					for (int k = 0; k < VS; k++) {
-						if (PAIR64) {
-							pa[k] = *(const uint2 *) (my_cols + soff + k * PITCH);
-							pb[k] = *(const uint2 *) (my_cols + soff + (VS + k) * PITCH);
-						}
-						else {
-							pa[k].x = *(const unsigned *) (my_cols + soff + k * PITCH);
-							pa[k].y = *(const unsigned *) (my_cols1 + soff + k * PITCH);
-							pb[k].x = *(const unsigned *) (my_cols + soff + (VS + k) * PITCH);
-							pb[k].y = *(const unsigned *) (my_cols1 + soff + (VS + k) * PITCH);
-						}
-					}
-					__syncwarp();
-					if (lane0)
-						mbar_arrive(empty_s + 8u * s);
-					bool opaque = false;
-					if (OPQ && PREMUL && opq_on) {
-						if (opq_skip == 0) {
-							unsigned m = 0xffffffffu;
-#pragma unroll
-							for (int k = 0; k < VS; k++)
-								m &= pa[k].x & pa[k].y & pb[k].x & pb[k].y;
-							opaque = __all_sync(0xffffffffu, m >= 0xff000000u);
-							if (!opaque)
-								opq_skip = kV4OpaqueSkip;
-						}
-						else
-							opq_skip--;
-					}
-					if (opaque) {
-#pragma unroll
-						for (int k = 0; k < VS; k++) {
-							V4_ACCO(pa[k].x, rb[2 * half][0], ga[2 * half][0]);
-							V4_ACCO(pa[k].y, rb[2 * half][CPT - 1], ga[2 * half][CPT - 1]);
-							V4_ACCO(pb[k].x, rb[2 * half + 1][0], ga[2 * half + 1][0]);
-							V4_ACCO(pb[k].y, rb[2 * half + 1][CPT - 1], ga[2 * half + 1][CPT - 1]);
-						}
+				for (int k = 0; k < VS; k++) {
+					if (PAIR64) {
+						pa[k] = *(const uint2 *) (my_cols + soff + k * PITCH);
+						pb[k] = *(const uint2 *) (my_cols + soff + (VS + k) * PITCH);
 					}
 					else {
+						pa[k].x = *(const unsigned *) (my_cols + soff + k * PITCH);
+						pa[k].y = *(const unsigned *) (my_cols1 + soff + k * PITCH);
+						pb[k].x = *(const unsigned *) (my_cols + soff + (VS + k) * PITCH);
+						pb[k].y = *(const unsigned *) (my_cols1 + soff + (VS + k) * PITCH);
+					}
+				}
+				__syncwarp();
+				if (lane0)
+					mbar_arrive(empty_s + 8u * s);
+				bool opaque = false;
+				if (OPQ && PREMUL && opq_on) {
+					if (opq_skip == 0) {
+						unsigned m = 0xffffffffu;
 #pragma unroll
-						for (int k = 0; k < VS; k++) {
-							V4_ACC(pa[k].x, rb[2 * half][0], ga[2 * half][0]);
-							V4_ACC(pa[k].y, rb[2 * half][CPT - 1], ga[2 * half][CPT - 1]);
-							V4_ACC(pb[k].x, rb[2 * half + 1][0], ga[2 * half + 1][0]);
-							V4_ACC(pb[k].y, rb[2 * half + 1][CPT - 1], ga[2 * half + 1][CPT - 1]);
-						}
+						for (int k = 0; k < VS; k++)
+							m &= pa[k].x & pa[k].y & pb[k].x & pb[k].y;
+						opaque = __all_sync(0xffffffffu, m >= 0xff000000u);
+						if (!opaque)
+							opq_skip = kV4OpaqueSkip;
+					}
+					else
+						opq_skip--;
+				}
+				if (opaque) {
+#pragma unroll
+					for (int k = 0; k < VS; k++) {
+						accumulate_pixel_h<false>(pa[k].x, k16, rb[2 * half][0], ga[2 * half][0]);
+						accumulate_pixel_h<false>(pa[k].y, k16, rb[2 * half][CPT - 1], ga[2 * half][CPT - 1]);
+						accumulate_pixel_h<false>(pb[k].x, k16, rb[2 * half + 1][0], ga[2 * half + 1][0]);
+						accumulate_pixel_h<false>(pb[k].y, k16, rb[2 * half + 1][CPT - 1], ga[2 * half + 1][CPT - 1]);
 					}
 				}
 				else {
-					unsigned pa[VS], pb[VS];
 #pragma unroll
 					for (int k = 0; k < VS; k++) {
-						pa[k] = *(const unsigned *) (my_cols + soff + k * PITCH);
-						pb[k] = *(const unsigned *) (my_cols + soff + (VS + k) * PITCH);
-					}
-					__syncwarp();
-					if (lane0)
-						mbar_arrive(empty_s + 8u * s);
-					bool opaque = false;
-					if (OPQ && PREMUL && opq_on) {
-						if (opq_skip == 0) {
-							unsigned m = 0xffffffffu;
-#pragma unroll
-							for (int k = 0; k < VS; k++)
-								m &= pa[k] & pb[k];
-							opaque = __all_sync(0xffffffffu, m >= 0xff000000u);
-							if (!opaque)
-								opq_skip = kV4OpaqueSkip;
-						}
-						else
-							opq_skip--;
-					}
-					if (opaque) {
-#pragma unroll
-						for (int k = 0; k < VS; k++) {
-							V4_ACCO(pa[k], rb[2 * half][0], ga[2 * half][0]);
-							V4_ACCO(pb[k], rb[2 * half + 1][0], ga[2 * half + 1][0]);
-						}
-					}
-					else {
-#pragma unroll
-						for (int k = 0; k < VS; k++) {
-							V4_ACC(pa[k], rb[2 * half][0], ga[2 * half][0]);
-							V4_ACC(pb[k], rb[2 * half + 1][0], ga[2 * half + 1][0]);
-						}
+						accumulate_pixel_h<PREMUL>(pa[k].x, k16, rb[2 * half][0], ga[2 * half][0]);
+						accumulate_pixel_h<PREMUL>(pa[k].y, k16, rb[2 * half][CPT - 1], ga[2 * half][CPT - 1]);
+						accumulate_pixel_h<PREMUL>(pb[k].x, k16, rb[2 * half + 1][0], ga[2 * half + 1][0]);
+						accumulate_pixel_h<PREMUL>(pb[k].y, k16, rb[2 * half + 1][CPT - 1], ga[2 * half + 1][CPT - 1]);
 					}
 				}
 				if (++s == S) {
@@ -582,26 +496,25 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 					w.z = __byte_perm(__byte_perm(av[0][1], av[1][1], 0x0040), __byte_perm(av[2][1], av[3][1], 0x0040), 0x5410);
 					w.w = __byte_perm(__byte_perm(av[0][3], av[1][3], 0x0040), __byte_perm(av[2][3], av[3][3], 0x0040), 0x5410);
 					*(uint4 *) (q_store + (size_t) (q & (kV4Quads - 1)) * QS + i * 16) = w;
-					continue;
 				}
-				if (VB200_V4_HADD2) {
+				else {
 					/* plain sums (HADD2): scale them here, one IMAD per word instead of one per pixel */
 #pragma unroll
 					for (int r = 0; r < 4; r++) {
 						rb[r][i] *= accm;
 						ga[r][i] *= accm;
 					}
+					const unsigned rb01 = __byte_perm(rb[0][i], rb[1][i], 0x7351); /* [r0 r1 b0 b1] */
+					const unsigned rb23 = __byte_perm(rb[2][i], rb[3][i], 0x7351);
+					const unsigned ga01 = __byte_perm(ga[0][i], ga[1][i], 0x7351);
+					const unsigned ga23 = __byte_perm(ga[2][i], ga[3][i], 0x7351);
+					uint4 w;
+					w.x = __byte_perm(rb01, rb23, 0x5410); /* r rows 0..3 */
+					w.y = __byte_perm(ga01, ga23, 0x5410); /* g */
+					w.z = __byte_perm(rb01, rb23, 0x7632); /* b */
+					w.w = __byte_perm(ga01, ga23, 0x7632); /* a */
+					*(uint4 *) (q_store + (size_t) (q & (kV4Quads - 1)) * QS + i * 16) = w;
 				}
-				const unsigned rb01 = __byte_perm(rb[0][i], rb[1][i], 0x7351); /* [r0 r1 b0 b1] */
-				const unsigned rb23 = __byte_perm(rb[2][i], rb[3][i], 0x7351);
-				const unsigned ga01 = __byte_perm(ga[0][i], ga[1][i], 0x7351);
-				const unsigned ga23 = __byte_perm(ga[2][i], ga[3][i], 0x7351);
-				uint4 w;
-				w.x = __byte_perm(rb01, rb23, 0x5410); /* r rows 0..3 */
-				w.y = __byte_perm(ga01, ga23, 0x5410); /* g */
-				w.z = __byte_perm(rb01, rb23, 0x7632); /* b */
-				w.w = __byte_perm(ga01, ga23, 0x7632); /* a */
-				*(uint4 *) (q_store + (size_t) (q & (kV4Quads - 1)) * QS + i * 16) = w;
 			}
 		}
 		qdone = max(qdone, q1 + 1);
@@ -610,10 +523,7 @@ thumbnail_fused_mma_kernel(const __grid_constant__ FusedParams P, const __grid_c
 		/* reducev on the tensor pipe + in-thread shrinkh; rows go to sh[buf] once the H warp has released it */
 		const int buf = chunk & 1;
 		const uint4 bf = __ldg(&P.vbfrag[(size_t) (chunk0 + chunk) * 32 + lane]); /* {hi b0, hi b1, lo b0, lo b1} */
-		if (VB200_V4_EPOLL_NS)
-			mbar_wait_poll(shempty_s + 8u * buf, ((unsigned) (chunk >> 1) & 1u) ^ 1u, VB200_V4_EPOLL_NS);
-		else
-			mbar_wait(shempty_s + 8u * buf, ((unsigned) (chunk >> 1) & 1u) ^ 1u);
+		mbar_wait(shempty_s + 8u * buf, ((unsigned) (chunk >> 1) & 1u) ^ 1u);
 		unsigned char *shb = (unsigned char *) (sh + (size_t) buf * KM * shs) + (size_t) (2 * tig) * shs * 8 + ch_off;
 		int bsum[2] = {0, 0}; /* non-power-of-two boxes: running sums of the box in progress, output rows r = 0, 1 */
 		int bcnt = 0, bidx = 0;

@@ -305,6 +305,7 @@ V4_CASES = [
     # the older fused kernels with the same pixels
     (1003, 2057, 120, None, "both", True, 2, False),
     (2560, 1280, 256, 183, "force", True, 1, False),
+    (2052, 2052, 128, None, "both", True, 1, False),     # box 8 whose last box runs past the frame's right edge
 ]
 
 

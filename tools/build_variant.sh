@@ -1,5 +1,5 @@
 #!/bin/sh
-# tools/build_variant.sh NAME "-DVB200_V4_COLS=320 -DVB200_V4_STAGES=6"
+# tools/build_variant.sh NAME "-DVB200_V4_STAGES=6 -DVB200_V4_MMA_UNROLL=1"
 # A tuning build of libvb200.so with different compile-time knobs for the fused kernel:
 # libvips_b200/variants/libvb200_NAME.so, selected at run time with VB200_LIB=<path>.
 set -e
