@@ -624,6 +624,79 @@ int vb200_debug_jpeg_optimal_table(const unsigned *freq, unsigned char *bits, un
 /* with env VB200_JPEG_TIMING: CUDA-event times of jpeg_huffman_kernel / jpeg_idct_kernel over the calling thread's last decode */
 void vb200_debug_jpeg_times(float *huffman_ms, float *idct_ms);
 
+/* ------------------------------------------------------------------ Deep Zoom tile pyramids
+ * vips_dzsave (foreign/dzsave.c) in its "dz" and "zoomify" layouts with JPEG tiles, on the device (csrc/dzsave.cu):
+ * every level of the pyramid (strip_shrink :1761-1835 over region.c:1139-1156, each level the 2 x 2 rounded mean
+ * (a + b + c + d + 2) >> 2 of the level above with its last column / row repeated when its size is odd,
+ * level_generate_extras :1710-1754), every tile cut from it (image_strip_allocate :1106-1152) and every tile's
+ * vips_jpegsave stream (write_image :369-404 -- the bytes vb200_jpegsave_batch_opts writes) is produced by CUDA kernels;
+ * the finished streams and their index come back to the host.
+ *
+ * Options follow vips_foreign_save_dz_build (:2043-2113).  layout: the reference's VipsForeignDzLayout values; google,
+ * iiif and iiif3 return -1.  tile_size 0 and overlap -1 take the layout's defaults (254 and 1 for dz, 256 and 0 for
+ * zoomify); a tile_step (tile_size for dz, tile_size - overlap for zoomify) <= 0 is the reference's error "overlap too
+ * large".  depth 0 is the layout's default (onepixel for dz, onetile for zoomify).  region_shrink, skip_blanks and
+ * container are there to be refused: only the reference's defaults (mean, off, a directory tree) run here.  suffix NULL
+ * is the layout's default (".jpeg" / ".jpg"); any other suffix must name a JPEG tile without [options].
+ * Images are uchar with 1 or 3 bands, in host or device memory, any bpl; everything else returns -1 and keeps the host path.
+ */
+enum { VB200_DZ_LAYOUT_DZ = 0, VB200_DZ_LAYOUT_ZOOMIFY = 1, VB200_DZ_LAYOUT_GOOGLE = 2, VB200_DZ_LAYOUT_IIIF = 3, VB200_DZ_LAYOUT_IIIF3 = 4 };
+enum { VB200_DZ_DEPTH_DEFAULT = 0, VB200_DZ_DEPTH_ONEPIXEL = 1, VB200_DZ_DEPTH_ONETILE = 2, VB200_DZ_DEPTH_ONE = 3 };
+typedef struct {
+	int layout;
+	int tile_size;
+	int overlap;
+	int depth;
+	int region_shrink; /* VipsRegionShrink: 0 mean; the others return -1 */
+	int skip_blanks;   /* the reference's skip_blanks + 1, so that 0 is its default (off); anything else returns -1 */
+	int container;	   /* VipsForeignDzContainer: 0 a directory tree; zip and szi return -1 */
+	const char *suffix;
+	VB200JpegSaveOptions jpeg; /* Q 0 = 75; the rest as vb200_jpegsave_batch_opts */
+} VB200DzOptions;
+
+/* a finished pyramid: the tile streams and their index, on the host */
+typedef struct VB200DzPyramid VB200DzPyramid;
+
+/* The whole save.  options NULL = every default.  On any error *out is NULL and nothing is left allocated. */
+int vb200_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out);
+/* test hook, host only (no GPU, no CUDA call): the same pyramid, tiling and streams through the kernels' per-pixel code
+ * and the encoder's host twin
+ */
+int vb200_debug_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out);
+void vb200_dz_free(VB200DzPyramid *pyramid);
+/* levels are numbered as the reference numbers them (pyramid_build :441-577): n = 0 is the smallest */
+int vb200_dz_levels(const VB200DzPyramid *pyramid);
+int vb200_dz_level_geometry(const VB200DzPyramid *pyramid, int n, int *width, int *height, int *tiles_across, int *tiles_down);
+/* tiles in the order zoomify numbers them (tile_name :1182-1191): level 0 first, then down, then across.  left, top,
+ * width, height: the tile's rect in its level; stream: its JPEG, owned by the pyramid
+ */
+long vb200_dz_tiles(const VB200DzPyramid *pyramid);
+int vb200_dz_tile(const VB200DzPyramid *pyramid, long i, int *level, int *x, int *y, int *left, int *top, int *width, int *height,
+	const void **stream, size_t *len);
+/* tile i's path relative to the directory the save is written in (tile_name :1156-1297): <basename>_files/<n>/<x>_<y>.jpeg,
+ * or <basename>/TileGroup<N / 256>/<n>-<x>-<y>.jpg.  basename NULL = "untitled" (:2282)
+ */
+int vb200_dz_tile_name(const VB200DzPyramid *pyramid, long i, const char *basename, char *name, size_t cap);
+/* the file beside the tiles: <basename>.dzi (write_dzi :579-620) or <basename>/ImageProperties.xml (write_properties
+ * :622-655), byte for byte; *len = bytes of text (no terminating NUL is counted, one is written)
+ */
+int vb200_dz_sidecar(const VB200DzPyramid *pyramid, const char *basename, char *name, size_t ncap, char *text, size_t tcap, size_t *len);
+/* The pixel pyramid alone: level n_from_top of the image (0 = the image itself, 1 = half size ...) through the same
+ * kernels, into out (allocate-or-fill like every op).  -1 when the image has no such level (it stops at 1 x 1).
+ */
+int vb200_dz_pyramid_level(const VB200Image *in, int n_from_top, VB200Image *out);
+/* test hook, host only: vb200_dz_pyramid_level through the per-pixel code on the CPU; out: packed, caller-sized */
+int vb200_debug_dz_pyramid_level(const void *pixels, size_t bpl, int width, int height, int bands, int n_from_top, void *out);
+/* test hooks: the device memory one shape batch of tiles may take (pixels, encoder scratch and stream slots; 0 = the
+ * default, 1 GiB), and the bytes currently allocated from the device's stream-ordered pool
+ */
+void vb200_debug_dz_set_budget(size_t bytes);
+size_t vb200_debug_dz_pool_used(void);
+/* with env VB200_DZ_TIMING set: CUDA-event milliseconds of the calling thread's last vb200_dzsave, split into
+ * ms[0] pyramid kernels, [1] gather kernels, [2] encoder calls, [3] stream compaction and device-to-host copies
+ */
+void vb200_debug_dz_times(float *ms);
+
 /* Pinned host memory for the pump: page-locked and, on a multi-socket machine, placed on the NUMA
  * node the current device hangs off (falls back to cudaHostAlloc).  vb200_device_numa_node():
  * that node, or -1 (unknown / single node).

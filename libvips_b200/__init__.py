@@ -104,6 +104,18 @@ def jpeg_icc_profile(stream):
     return out.raw[:n.value]
 
 
+class JpegSaveOptions(C.Structure):
+    """VB200JpegSaveOptions"""
+    _fields_ = [("Q", C.c_int), ("subsample_mode", C.c_int), ("optimize_coding", C.c_int), ("restart_interval", C.c_int),
+                ("interlace", C.c_int)]
+
+
+class DzOptions(C.Structure):
+    """VB200DzOptions"""
+    _fields_ = [("layout", C.c_int), ("tile_size", C.c_int), ("overlap", C.c_int), ("depth", C.c_int), ("region_shrink", C.c_int),
+                ("skip_blanks", C.c_int), ("container", C.c_int), ("suffix", C.c_char_p), ("jpeg", JpegSaveOptions)]
+
+
 class CReduceParams(C.Structure):
     _fields_ = [("n_point", C.c_int), ("kernel", C.c_int), ("residual_shrink", C.c_double),
                 ("offset", C.c_double)]
@@ -230,6 +242,22 @@ def lib():
         L.vb200_chain_add_premultiply.argtypes = [C.c_void_p, C.c_double, C.c_int]
         L.vb200_chain_add_unpremultiply.argtypes = [C.c_void_p, C.c_double, C.c_int]
         L.vb200_chain_run_host.argtypes = [C.c_void_p, IP, IP, C.c_int]
+        DO, PP = C.POINTER(DzOptions), C.POINTER(C.c_void_p)
+        L.vb200_dzsave.argtypes = [IP, DO, PP]
+        L.vb200_debug_dzsave.argtypes = [IP, DO, PP]
+        L.vb200_dz_free.argtypes = [C.c_void_p]
+        L.vb200_dz_levels.argtypes = [C.c_void_p]
+        L.vb200_dz_level_geometry.argtypes = [C.c_void_p, C.c_int, PI, PI, PI, PI]
+        L.vb200_dz_tiles.argtypes = [C.c_void_p]
+        L.vb200_dz_tiles.restype = C.c_long
+        L.vb200_dz_tile.argtypes = [C.c_void_p, C.c_long] + [PI] * 7 + [PP, C.POINTER(C.c_size_t)]
+        L.vb200_dz_tile_name.argtypes = [C.c_void_p, C.c_long, C.c_char_p, C.c_char_p, C.c_size_t]
+        L.vb200_dz_sidecar.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_dz_pyramid_level.argtypes = [IP, C.c_int, IP]
+        L.vb200_debug_dz_pyramid_level.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+        L.vb200_debug_dz_set_budget.argtypes = [C.c_size_t]
+        L.vb200_debug_dz_pool_used.restype = C.c_size_t
+        L.vb200_debug_dz_times.argtypes = [C.POINTER(C.c_float)]
         _lib = L
     return _lib
 
@@ -435,6 +463,11 @@ class Image:
     def median(self, size):
         return self._call(lib().vb200_median, int(size))
 
+    # ---- savers
+    def dzsave(self, basename=None, **options):
+        """vips_dzsave: the Deep Zoom / Zoomify tile pyramid of this image -> DzPyramid (see dzsave())"""
+        return dzsave(self, basename, **options)
+
     # ---- colour
     def colourspace(self, space, source_space=None):
         src = self if source_space is None else Image(self.array, source_space)
@@ -536,12 +569,6 @@ def flatten_host_twin(a, background=None, max_alpha=0.0, interpretation=None, x4
 _SAVE_BUFFERS = {}
 
 
-class JpegSaveOptions(C.Structure):
-    """VB200JpegSaveOptions"""
-    _fields_ = [("Q", C.c_int), ("subsample_mode", C.c_int), ("optimize_coding", C.c_int), ("restart_interval", C.c_int),
-                ("interlace", C.c_int)]
-
-
 def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0,
                    interlace=False):
     """vips_jpegsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1 or 3) on the device -> list of bytes.
@@ -568,6 +595,138 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
     _check(lib().vb200_jpegsave_batch_opts(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), out.ctypes.data_as(C.c_void_p),
                                            HOST, stride, lens))
     return [out[i, :lens[i]].tobytes() for i in range(n)]
+
+
+DZ_LAYOUTS = {"dz": 0, "zoomify": 1, "google": 2, "iiif": 3, "iiif3": 4}
+DZ_DEPTHS = {None: 0, "onepixel": 1, "onetile": 2, "one": 3}
+DZ_CONTAINERS = {"fs": 0, "zip": 1, "szi": 2}
+REGION_SHRINKS = {"mean": 0, "median": 1, "mode": 2, "max": 3, "min": 4, "nearest": 5}
+
+
+class DzTile:
+    """one tile of a DzPyramid: name (path relative to the directory written in), level (0 = smallest), x, y,
+    rect = (left, top, width, height) in its level, bytes = its JPEG stream"""
+    __slots__ = ("name", "level", "x", "y", "rect", "bytes")
+
+    def __init__(self, name, level, x, y, rect, data):
+        self.name, self.level, self.x, self.y, self.rect, self.bytes = name, level, x, y, rect, data
+
+
+class DzPyramid:
+    """What vips_dzsave writes, in memory: .levels = [(width, height, tiles_across, tiles_down)] by the reference's level
+    number (0 = smallest), .tiles (DzTile, level 0 first, then down, then across), .sidecar = (name, text): the .dzi or
+    ImageProperties.xml.  .write(directory) makes the tree a viewer reads."""
+
+    def __init__(self, handle, basename):
+        L = lib()
+        try:
+            base = None if basename is None else os.fsencode(basename)
+            w, h, ta, td = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+            self.levels = []
+            for n in range(L.vb200_dz_levels(handle)):
+                _check(L.vb200_dz_level_geometry(handle, n, C.byref(w), C.byref(h), C.byref(ta), C.byref(td)))
+                self.levels.append((w.value, h.value, ta.value, td.value))
+            self.tiles = []
+            v = [C.c_int() for _ in range(7)]
+            p, n, name = C.c_void_p(), C.c_size_t(), C.create_string_buffer(4096)
+            for i in range(L.vb200_dz_tiles(handle)):
+                _check(L.vb200_dz_tile(handle, i, *[C.byref(x) for x in v], C.byref(p), C.byref(n)))
+                _check(L.vb200_dz_tile_name(handle, i, base, name, len(name)))
+                self.tiles.append(DzTile(os.fsdecode(name.value), v[0].value, v[1].value, v[2].value, tuple(x.value for x in v[3:]),
+                                         C.string_at(p.value, n.value)))
+            text = C.create_string_buffer(4096)
+            _check(L.vb200_dz_sidecar(handle, base, name, len(name), text, len(text), C.byref(n)))
+            self.sidecar = (os.fsdecode(name.value), text.raw[:n.value].decode())
+        finally:
+            L.vb200_dz_free(handle)
+
+    def write(self, directory):
+        """<directory>/<basename>.dzi + <basename>_files/<level>/<x>_<y>.jpeg, or the zoomify tree"""
+        for name, data in [(t.name, t.bytes) for t in self.tiles] + [(self.sidecar[0], self.sidecar[1].encode())]:
+            path = os.path.join(directory, name)
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            with open(path, "wb") as f:
+                f.write(data)
+
+
+def _dz_image(image, in_ptr, shape, bpl):
+    """(CImage, keep-alive) of a host array / Image, or of device memory in_ptr with shape = (height, width, bands)"""
+    if in_ptr is not None:
+        h, w, bands = shape
+        return CImage(w, h, bands, 0, 1 if bands < 3 else 22, DEVICE, C.c_void_p(in_ptr), int(bpl or w * bands)), None
+    a = image.array if isinstance(image, Image) else np.asarray(image)
+    if a.ndim == 2:
+        a = a[:, :, None]
+    if a.dtype not in FORMATS:
+        raise Error("unsupported dtype %s" % a.dtype)
+    if a.strides[1:] != (a.shape[2] * a.itemsize, a.itemsize) or a.strides[0] < a.shape[1] * a.shape[2] * a.itemsize:
+        a = np.ascontiguousarray(a)
+    return CImage(a.shape[1], a.shape[0], a.shape[2], FORMATS[a.dtype], 1 if a.shape[2] < 3 else 22, HOST, C.c_void_p(a.ctypes.data),
+                  a.strides[0]), a
+
+
+def _dzsave(fn, image, basename, layout, tile_size, overlap, depth, Q, suffix, region_shrink, skip_blanks, container, subsample_mode,
+            optimize_coding, restart_interval, interlace, in_ptr, shape, bpl):
+    pick = lambda table, v: table[v] if v in table else int(v)
+    jpeg = JpegSaveOptions(int(Q), {"auto": 0, "on": 1, "off": 2}[subsample_mode], int(bool(optimize_coding)), int(restart_interval),
+                           int(bool(interlace)))
+    opts = DzOptions(pick(DZ_LAYOUTS, layout), int(tile_size or 0), -1 if overlap is None else int(overlap), pick(DZ_DEPTHS, depth),
+                     pick(REGION_SHRINKS, region_shrink), int(skip_blanks) + 1, pick(DZ_CONTAINERS, container),
+                     None if suffix is None else suffix.encode(), jpeg)
+    cin, keep = _dz_image(image, in_ptr, shape, bpl)
+    handle = C.c_void_p()
+    _check(fn(C.byref(cin), C.byref(opts), C.byref(handle)))
+    return DzPyramid(handle, basename)
+
+
+def dzsave(image, basename=None, layout="dz", tile_size=None, overlap=None, depth=None, Q=75, suffix=None, region_shrink="mean",
+           skip_blanks=-1, container="fs", subsample_mode="auto", optimize_coding=False, restart_interval=0, interlace=False, in_ptr=None,
+           shape=None, bpl=None):
+    """vips_dzsave on the device: the Deep Zoom ("dz") or Zoomify pyramid of a uint8 image of 1 or 3 bands, every level and
+    every JPEG tile made by CUDA kernels -> DzPyramid.  image: an H x W x bands array or Image on the host, or None with
+    in_ptr / shape = (height, width, bands) / bpl for pixels already on the device.  tile_size / overlap / depth None: the
+    layout's defaults.  The remaining options are the reference's; what the device path does not take raises Error."""
+    return _dzsave(lib().vb200_dzsave, image, basename, layout, tile_size, overlap, depth, Q, suffix, region_shrink, skip_blanks, container,
+                   subsample_mode, optimize_coding, restart_interval, interlace, in_ptr, shape, bpl)
+
+
+def dzsave_host_twin(image, basename=None, layout="dz", tile_size=None, overlap=None, depth=None, Q=75, suffix=None, region_shrink="mean",
+                     skip_blanks=-1, container="fs", subsample_mode="auto", optimize_coding=False, restart_interval=0, interlace=False):
+    """dzsave through the kernels' per-pixel code and the encoder's host twin on the CPU (vb200_debug_dzsave): no GPU"""
+    return _dzsave(lib().vb200_debug_dzsave, image, basename, layout, tile_size, overlap, depth, Q, suffix, region_shrink, skip_blanks,
+                   container, subsample_mode, optimize_coding, restart_interval, interlace, None, None, None)
+
+
+def dz_pyramid_level(image, n_from_top, in_ptr=None, shape=None, bpl=None):
+    """level n_from_top of the pixel pyramid dzsave cuts its tiles from (0 = the image, 1 = half size ...), on the device ->
+    uint8 array [height, width, bands] on the host"""
+    cin, keep = _dz_image(image, in_ptr, shape, bpl)
+    cout = CImage()
+    if in_ptr is not None:
+        import torch
+        w, h = cin.Xsize, cin.Ysize
+        for _ in range(int(n_from_top)):
+            w, h = (w + 1) // 2, (h + 1) // 2
+        rows = torch.empty((h, w * cin.Bands), dtype=torch.uint8, device="cuda")     # the op fills the caller's buffer
+        cout.data, cout.bpl = rows.data_ptr(), w * cin.Bands
+        _check(lib().vb200_dz_pyramid_level(C.byref(cin), int(n_from_top), C.byref(cout)))
+        return rows.cpu().numpy().reshape(cout.Ysize, cout.Xsize, cout.Bands)
+    _check(lib().vb200_dz_pyramid_level(C.byref(cin), int(n_from_top), C.byref(cout)))
+    buf = (C.c_uint8 * (cout.Ysize * cout.bpl)).from_address(cout.data)
+    arr = np.frombuffer(buf, np.uint8).reshape(cout.Ysize, cout.Xsize, cout.Bands).copy()
+    lib().vb200_image_free(C.byref(cout))
+    return arr
+
+
+def dz_pyramid_level_host_twin(image, n_from_top):
+    """the same level through the kernel's per-pixel code on the CPU (vb200_debug_dz_pyramid_level): no GPU"""
+    cin, keep = _dz_image(image, None, None, None)
+    w, h = cin.Xsize, cin.Ysize
+    for _ in range(int(n_from_top)):
+        w, h = (w + 1) // 2, (h + 1) // 2
+    out = np.empty((h, w, cin.Bands), np.uint8)
+    _check(lib().vb200_debug_dz_pyramid_level(cin.data, cin.bpl, cin.Xsize, cin.Ysize, cin.Bands, int(n_from_top), out.ctypes.data_as(C.c_void_p)))
+    return out
 
 
 def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",

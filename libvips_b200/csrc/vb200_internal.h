@@ -194,6 +194,11 @@ int dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const siz
 	size_t out_frame_stride, int *out_w, int *out_h, int *bands, cudaStream_t s);
 int host_jpeg_decode(const char *domain, const void *buf, size_t len, int shrink, unsigned char *out, size_t out_bpl, int *out_w,
 	int *out_h, int *bands, unsigned sub_bytes, int max_passes, int *passes_used);
+/* jpeg_encode.cu: the encoder's host twins (the per-block code on the CPU), one stream appended to out */
+int host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode, int optimize,
+	int restart, std::vector<unsigned char> &out);
+int host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
+	int restart, std::vector<unsigned char> &out, unsigned long long *events);
 /* min(hshrink, vshrink) of vips_thumbnail_calculate_shrink, thumbnail.c:413-487 */
 double thumbnail_common_shrink(int w, int h, int tw, int th, int size);
 void jpeg_pump_release(); /* the JPEG pump's pinned / device slots (jpeg.cu); vb200_shutdown */
