@@ -402,15 +402,6 @@ dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options,
 	return 0;
 }
 
-/* blocks the encoder codes for one tile (jpeg_encode.cu make_geom) */
-size_t
-dz_blocks(int w, int h, int bands, const VB200JpegSaveOptions &j)
-{
-	const bool sub = bands == 3 && (j.subsample_mode == 1 || (j.subsample_mode == 0 && j.Q < 90));
-	const int ms = sub ? 16 : 8;
-	return (size_t) ((w + ms - 1) / ms) * ((h + ms - 1) / ms) * (bands == 1 ? 1 : (sub ? 6 : 3));
-}
-
 std::atomic<size_t> g_budget{0};
 constexpr size_t kDzBudget = (size_t) 1 << 30;
 
@@ -481,12 +472,12 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 		const int w = sh.first.first, h = sh.first.second;
 		const std::vector<long> &idx = sh.second;
 		const size_t frame_stride = ((size_t) w * h * bands + 15) & ~(size_t) 15;
-		/* a stream's slot, from the bound the encoder sizes its own bit buffers by (208 bytes a block, 506 over the scans of
-		 * a progressive stream) plus its headers; what the encoder takes beside: coefficients, bit counts and that buffer
-		 */
-		const size_t blocks = dz_blocks(w, h, bands, jpeg), per_block = jpeg.interlace ? 512 : 208;
-		const size_t slot = (blocks * (per_block + (jpeg.restart_interval ? 8 : 0)) + 4096 + 15) & ~(size_t) 15;
-		const size_t per_tile = frame_stride + slot + blocks * (64 * sizeof(short) + 8 + per_block) + 16384;
+		/* a stream's slot, from the bound the encoder sizes its scan data by, and the device scratch the encoder takes beside */
+		size_t stream_bytes = 0, scratch_bytes = 0;
+		if (jpeg_encode_room(domain, w, h, bands, jpeg, &stream_bytes, &scratch_bytes))
+			return -1;
+		const size_t slot = (stream_bytes + 15) & ~(size_t) 15;
+		const size_t per_tile = frame_stride + slot + scratch_bytes;
 		if (per_tile > budget) {
 			error(domain, "a %d x %d tile takes %zu bytes of device memory, more than the %zu allowed for a batch", w, h, per_tile, budget);
 			return -1;

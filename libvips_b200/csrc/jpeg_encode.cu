@@ -21,13 +21,16 @@
  *                          previous block of its component: the coefficients are all there, nothing is sequential)
  *   (prefix sum)           bit offset of every block
  *   jpeg_emit_kernel       one thread per block: its bits OR-ed into the frame's bit buffer
- *   jpeg_stuff_kernel      FF -> FF00 and the markers around the scan: per 256-byte span count, prefix sum, copy
+ *   (stuffing)             FF -> FF00 and the markers around the scan: per 256-byte span count (jpeg_stuffcount_kernel),
+ *                          prefix sum (jpeg_ffscan_kernel), copy (jpeg_stuffcopy_kernel)
  * With vips_jpegsave's options (vips2jpeg.c:590-597):
- *   optimize_coding        jpeg_stats_kernel (symbol counts per frame) and jpeg_huffopt_kernel (jchuff.c
+ *   optimize_coding        jpeg_stats_kernel (symbol counts per frame) and jpeg_tables_kernel (jchuff.c
  *                          jpeg_gen_optimal_table per table, the frame's code tables and header) after the FDCT; the count,
  *                          emit and stuffing kernels then take the frame's tables and header
- *   restart_interval       jpeg_intervals_kernel after the bit prefix sum: every interval starts on a byte boundary, the
+ *   restart_interval       jpeg_segments_kernel after the bit prefix sum: every interval starts on a byte boundary, the
  *                          stuffing kernels put FF Dn before each interval after the first
+ * A sequential stream is the one-scan case of the progressive script (ScanScript): the table, segment and stuffing kernels
+ * serve both; only the coders differ.
  */
 #include <algorithm>
 #include <cstdlib>
@@ -416,12 +419,6 @@ previous_dc(const EncodeGeom &G, const short *coef, unsigned blk, int restart)
 constexpr unsigned kFreqSentinel = 1000000000u; /* jchuff.c jpeg_gen_optimal_table: v = 1000000000L */
 constexpr int kMaxCodeLen = 32;					/* MAX_CLEN: the longest code before the 16-bit limit */
 
-/* Huffman tables of one frame when it is coded with its own: code / length per symbol, tables as in EncodeTables */
-struct FrameHuff {
-	unsigned ehufco[4][256];
-	unsigned char ehufsi[4][256];
-};
-
 /* jchuff.c jpeg_gen_optimal_table, restated.  freq[257] holds the symbol counts and is consumed (freq[256], the reserved
  * all-ones code, is set to 1 here); codesize / others [257] are scratch; bits[17] (bits[l]: codes of length l, bits[0]
  * unused) and huffval[256] receive the table.
@@ -579,29 +576,6 @@ header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned c
 	}
 }
 
-/* the markers after the Huffman tables: DRI when there are restart intervals (jcmarker.c write_scan_header: after the
- * DHTs, before SOS, also when the interval covers the whole frame), then SOS
- */
-void
-header_suffix(const EncodeGeom &G, int restart, std::vector<unsigned char> &o)
-{
-	if (restart > 0) {
-		put16(o, 0xFFDD);
-		put16(o, 4);
-		put16(o, (unsigned) restart);
-	}
-	put16(o, 0xFFDA);
-	put16(o, 6 + 2 * G.ncomp);
-	o.push_back((unsigned char) G.ncomp);
-	for (int c = 0; c < G.ncomp; c++) {
-		o.push_back((unsigned char) (c + 1));
-		o.push_back((unsigned char) (c ? 0x11 : 0x00));
-	}
-	o.push_back(0);
-	o.push_back(63);
-	o.push_back(0);
-}
-
 /* one frame's DHT segments: tables 0..3 (0 and 1 only for greyscale), bits[t][1..16] / huffval[t] */
 void
 put_dhts(const EncodeGeom &G, const unsigned char (*bits)[17], const unsigned char (*huffval)[256], std::vector<unsigned char> &o)
@@ -624,19 +598,6 @@ standard_tables(unsigned char (*bits)[17], unsigned char (*huffval)[256])
 		memcpy(bits[t] + 1, b[t], 16);
 		memcpy(huffval[t], v[t], (size_t) table_values(bits[t]));
 	}
-}
-
-/* everything up to and including SOS with the standard Huffman tables, in libjpeg's order: SOI, JFIF APP0, DQT per
- * table, SOF0, DHT per table, DRI when restart > 0, SOS
- */
-void
-write_headers(const EncodeGeom &G, const EncodeTables &T, int restart, std::vector<unsigned char> &o)
-{
-	unsigned char bits[4][17], huffval[4][256];
-	standard_tables(bits, huffval);
-	header_prefix(G, T, o);
-	put_dhts(G, bits, huffval, o);
-	header_suffix(G, restart, o);
 }
 
 /* restart_interval as vips_jpegsave takes it (jpegsave.c:284-289): 0 for none.  The reference passes larger values
@@ -678,17 +639,18 @@ make_geom(const char *domain, int w, int h, int bands, int quality, int subsampl
 	return 0;
 }
 
-/* ------------------------------------------------------------------ progressive save: the scan script (host + device) */
+/* ------------------------------------------------------------------ the scan script (host + device) */
 
 constexpr int kMaxProgScans = 10;  /* jcparam.c jpeg_simple_progression: 10 scans for YCbCr, 6 for greyscale */
 constexpr int kMaxProgTables = 10; /* one table per DC-first component table and per AC scan: 10 for YCbCr, 5 for greyscale */
 constexpr int kMaxCorrBits = 1000; /* jcphuff.c MAX_CORR_BITS: the correction bits an EOB run may hold */
 
-/* One scan of the script.  A unit is what a restart interval counts: an MCU of the interleaved DC scans, one block of
- * the component's own grid (ceil(comp_w / 8) x ceil(comp_h / 8), no dummy blocks; T.81 A.2.2) in the others.
+/* One scan of the script.  A unit is what a restart interval counts: an MCU of the interleaved scans (the sequential
+ * scan, the progressive DC scans), one block of the component's own grid (ceil(comp_w / 8) x ceil(comp_h / 8), no dummy
+ * blocks; T.81 A.2.2) in the others.
  */
-struct ProgScan {
-	int comp;			/* the scan's component, -1 for the interleaved DC scans */
+struct Scan {
+	int comp;			/* the scan's component, -1 for an interleaved scan */
 	int ss, se, ah, al; /* spectral band and successive-approximation bits */
 	int ux, units;		/* units per row, units */
 	int unit_base;		/* the scan's first unit in the frame's list of units */
@@ -696,9 +658,10 @@ struct ProgScan {
 	int tab, nt;		/* its first table in the frame's list of tables and their number (0 for DC refinement) */
 };
 
-struct ProgScript {
+/* A stream's scans: the progressive script, or the sequential stream's one scan (Ss 0, Se 63, Ah Al 0) */
+struct ScanScript {
 	int nscans, ntab, units, nseg, restart;
-	ProgScan s[kMaxProgScans];
+	Scan s[kMaxProgScans];
 	int tab_class[kMaxProgTables]; /* put_dht's t: 0 DC lum, 1 AC lum, 2 DC chr, 3 AC chr */
 	/* the device's header template: the frame's markers before the first scan (prefix_len bytes), then each scan's DRI / SOS
 	 * at sfx_at[s] .. sfx_at[s + 1]
@@ -732,24 +695,27 @@ comp_block_index(const EncodeGeom &G, int c, int bx, int by)
 	return ((unsigned) by * G.mcus_x + (unsigned) bx) * G.blocks_per_mcu + (unsigned) c;
 }
 
-/* jcparam.c jpeg_simple_progression (fill_dc_scans, fill_a_scan / fill_scans), laid out for one geometry: YCbCr
+/* The scans of one geometry.  Sequential: one interleaved scan, Ss 0, Se 63, with tables DC and AC per component class
+ * (0 DC lum, 1 AC lum, 2 DC chr, 3 AC chr).  Progressive: jcparam.c jpeg_simple_progression (fill_dc_scans, fill_a_scan /
+ * fill_scans), YCbCr
  *   DC 0-0 Al 1 (interleaved); Y 1-5 Al 2; Cr 1-63 Al 1; Cb 1-63 Al 1; Y 6-63 Al 2; Y 1-63 Ah 2 Al 1;
  *   DC Ah 1 Al 0 (interleaved); Cr 1-63 Ah 1 Al 0; Cb 1-63 Ah 1 Al 0; Y 1-63 Ah 1 Al 0
  * and greyscale the same without the chroma scans.  Tables: the DC-first scan one per dc_tbl_no (Y 0, Cb and Cr 1), every
  * AC scan its own (finish_pass_gather_phuff builds a table per scan), DC refinement none.
  */
 void
-prog_script(const EncodeGeom &G, int restart, ProgScript *P)
+scan_script(const EncodeGeom &G, int restart, bool progressive, ScanScript *P)
 {
+	static const int sequential[1][5] = {{-1, 0, 63, 0, 0}};
 	static const int colour[10][5] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2}, {2, 1, 63, 0, 1}, {1, 1, 63, 0, 1}, {0, 6, 63, 0, 2}, {0, 1, 63, 2, 1},
 		{-1, 0, 0, 1, 0}, {2, 1, 63, 1, 0}, {1, 1, 63, 1, 0}, {0, 1, 63, 1, 0}};
 	static const int grey[6][5] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2}, {0, 6, 63, 0, 2}, {0, 1, 63, 2, 1}, {-1, 0, 0, 1, 0}, {0, 1, 63, 1, 0}};
-	const int(*script)[5] = G.ncomp == 3 ? colour : grey;
+	const int(*script)[5] = !progressive ? sequential : G.ncomp == 3 ? colour : grey;
 	memset(P, 0, sizeof(*P));
-	P->nscans = G.ncomp == 3 ? 10 : 6;
+	P->nscans = !progressive ? 1 : G.ncomp == 3 ? 10 : 6;
 	P->restart = restart;
 	for (int i = 0; i < P->nscans; i++) {
-		ProgScan &S = P->s[i];
+		Scan &S = P->s[i];
 		S.comp = script[i][0];
 		S.ss = script[i][1];
 		S.se = script[i][2];
@@ -765,23 +731,25 @@ prog_script(const EncodeGeom &G, int restart, ProgScript *P)
 		S.nseg = restart ? (S.units + restart - 1) / restart : 1;
 		S.seg_base = P->nseg;
 		P->nseg += S.nseg;
+		/* per component class of the scan (luma, chroma): a DC table unless it refines DC, an AC table unless Se is 0 */
 		S.tab = P->ntab;
-		if (S.ss == 0 && S.ah == 0) {
-			P->tab_class[P->ntab++] = 0;
-			if (G.ncomp == 3)
-				P->tab_class[P->ntab++] = 2;
+		for (int k = 0; k < (S.comp < 0 && G.ncomp == 3 ? 2 : 1); k++) {
+			const int chr = S.comp < 0 ? k : S.comp > 0;
+			if (S.ss == 0 && S.ah == 0)
+				P->tab_class[P->ntab++] = 2 * chr;
+			if (S.se > 0)
+				P->tab_class[P->ntab++] = 2 * chr + 1;
 		}
-		else if (S.ss > 0)
-			P->tab_class[P->ntab++] = S.comp ? 3 : 1;
 		S.nt = P->ntab - S.tab;
 	}
 }
 
 /* jcmarker.c write_scan_header after the DHTs: DRI before the first scan when there are restart intervals (emitted when
- * the interval differs from the last one written), then emit_sos with 0 for the table selectors a scan does not use
+ * the interval differs from the last one written; also when it covers the whole frame), then emit_sos with 0 for the
+ * table selectors a scan does not use
  */
 void
-prog_scan_suffix(const EncodeGeom &G, const ProgScan &S, bool first, int restart, std::vector<unsigned char> &o)
+scan_suffix(const EncodeGeom &G, const Scan &S, bool first, int restart, std::vector<unsigned char> &o)
 {
 	if (first && restart > 0) {
 		put16(o, 0xFFDD);
@@ -795,12 +763,9 @@ prog_scan_suffix(const EncodeGeom &G, const ProgScan &S, bool first, int restart
 	for (int i = 0; i < nc; i++) {
 		const int c = S.comp < 0 ? i : S.comp;
 		o.push_back((unsigned char) (c + 1));
-		int sel = 0;
-		if (S.ss == 0)
-			sel = S.ah == 0 && c ? 0x10 : 0; /* DC scan: dc_tbl_no, none in a refinement scan */
-		else
-			sel = c ? 1 : 0; /* AC scan: ac_tbl_no */
-		o.push_back((unsigned char) sel);
+		/* dc_tbl_no when the scan codes a DC first pass, ac_tbl_no when it codes AC coefficients */
+		const int dc = S.ss == 0 && S.ah == 0 && c ? 0x10 : 0, ac = S.se > 0 && c ? 1 : 0;
+		o.push_back((unsigned char) (dc | ac));
 	}
 	o.push_back((unsigned char) S.ss);
 	o.push_back((unsigned char) S.se);
@@ -910,6 +875,15 @@ static_assert(((1u << 29) / kMaxBlockBytes) * 64u + 1u < kFreqSentinel, "symbol 
  */
 constexpr int kHeaderSlot = 640;
 
+/* a frame's own Huffman tables, code / length per symbol: N = 4 for a sequential frame (tables as in EncodeTables),
+ * kMaxProgTables for a progressive one (one per table of the script)
+ */
+template <int N>
+struct HuffSet {
+	unsigned ehufco[N][256];
+	unsigned char ehufsi[N][256];
+};
+
 /* one thread per MCU; blockIdx.y = frame */
 __global__ void __launch_bounds__(128)
 jpeg_fdct_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const unsigned char *__restrict__ img, size_t bpl, size_t frame_stride,
@@ -931,11 +905,11 @@ jpeg_fdct_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const u
 }
 
 /* the Huffman tables a block of frame f is coded with: the batch's standard ones, or the frame's own */
-template <bool kFrameHuff>
+template <bool kFrameTables>
 __device__ __forceinline__ void
-frame_tables(const EncodeTables *T, const FrameHuff *huff, unsigned f, const unsigned (**co)[256], const unsigned char (**si)[256])
+frame_tables(const EncodeTables *T, const HuffSet<4> *huff, unsigned f, const unsigned (**co)[256], const unsigned char (**si)[256])
 {
-	if (kFrameHuff) {
+	if (kFrameTables) {
 		*co = huff[f].ehufco;
 		*si = huff[f].ehufsi;
 	}
@@ -970,29 +944,34 @@ jpeg_stats_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const 
 			atomicAdd(dst + i, s_hist[i]);
 }
 
-/* optimise_coding, pass 2: one CTA per frame, one warp per table (tables 0, 1 for greyscale).  Each warp runs
- * gen_optimal_table on its counts with a warp-wide minimum search, writes the frame's code / length table, and the CTA
- * then writes the frame's header -- prefix (SOI .. SOF0), its own DHTs, suffix (DRI, SOS) -- into its kHeaderSlot-byte
- * slot and the header's length into header_lens[frame].  A frame whose tables cannot be built sets *bad.
+/* optimise_coding, pass 2: tables and headers, one CTA per frame, one warp per table of the script (N: the tables a
+ * frame can have, which sets the block size).  Each warp runs gen_optimal_table on its counts with a warp-wide minimum
+ * search and writes the frame's code / length table; the CTA then writes the frame's headers into its slot_bytes-byte
+ * slot -- the markers before the first scan (SOI .. SOF), and per scan its DHTs and DRI / SOS from the template.
+ * hdr_end[frame][s] = where scan s's header ends: the first scan's comes with the frame's markers, so hdr_end[frame][0] is
+ * the bytes before the scan data (with one scan, the whole header); the stuffing passes insert the later ones.  A frame
+ * whose tables cannot be built sets *bad.
  */
-__global__ void __launch_bounds__(128)
-jpeg_huffopt_kernel(int ntab, const unsigned *__restrict__ counts, FrameHuff *__restrict__ huff, const unsigned char *__restrict__ prefix,
-	unsigned prefix_len, const unsigned char *__restrict__ suffix, unsigned suffix_len, unsigned char *__restrict__ headers,
-	unsigned *__restrict__ header_lens, int *__restrict__ bad)
+template <int N>
+__global__ void __launch_bounds__(32 * N)
+jpeg_tables_kernel(const __grid_constant__ ScanScript P, const unsigned *__restrict__ counts, HuffSet<N> *__restrict__ huff,
+	const unsigned char *__restrict__ tmpl, unsigned char *__restrict__ headers, unsigned slot_bytes, unsigned *__restrict__ hdr_end,
+	int *__restrict__ bad)
 {
-	__shared__ unsigned s_freq[4][257];
-	__shared__ int s_size[4][257], s_others[4][257];
-	__shared__ unsigned char s_bits[4][17], s_val[4][256];
+	__shared__ unsigned s_freq[N][257];
+	__shared__ int s_size[N][257], s_others[N][257];
+	__shared__ unsigned char s_bits[N][17], s_val[N][256];
+	__shared__ unsigned s_dht_at[N], s_sfx_dst[kMaxProgScans], s_len;
 	__shared__ int s_fail;
 	const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const unsigned *cnt = counts + (size_t) blockIdx.x * 4 * 256;
+	const unsigned *cnt = counts + (size_t) blockIdx.x * N * 256;
 	if (threadIdx.x == 0)
 		s_fail = 0;
-	for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x)
+	for (int i = threadIdx.x; i < N * 256; i += blockDim.x)
 		s_freq[i >> 8][i & 255] = cnt[i];
 	__syncthreads();
-	FrameHuff *fh = huff + blockIdx.x;
-	if (w < ntab) {
+	HuffSet<N> *fh = huff + blockIdx.x;
+	if (w < P.ntab) {
 		unsigned *freq = s_freq[w];
 		auto pick = [&](int exclude) {
 			__syncwarp();
@@ -1018,35 +997,43 @@ jpeg_huffopt_kernel(int ntab, const unsigned *__restrict__ counts, FrameHuff *__
 			derive_codes(s_bits[w] + 1, s_val[w], fh->ehufco[w], fh->ehufsi[w]);
 	}
 	__syncthreads();
-	unsigned len = prefix_len + suffix_len;
-	for (int t = 0; t < ntab; t++)
-		len += 21 + table_values(s_bits[t]);
-	if (s_fail || len > kHeaderSlot) {
-		if (threadIdx.x == 0) {
-			header_lens[blockIdx.x] = 0;
+	unsigned *end = hdr_end + (size_t) blockIdx.x * P.nscans;
+	if (threadIdx.x == 0) {
+		unsigned len = (unsigned) P.prefix_len;
+		for (int s = 0; s < P.nscans; s++) {
+			for (int t = P.s[s].tab; t < P.s[s].tab + P.s[s].nt; t++) {
+				s_dht_at[t] = len;
+				len += 21 + table_values(s_bits[t]);
+			}
+			s_sfx_dst[s] = len;
+			len += (unsigned) (P.sfx_at[s + 1] - P.sfx_at[s]);
+			end[s] = len;
+		}
+		s_len = len;
+		if (s_fail || len > slot_bytes) {
+			end[0] = 0;
 			atomicExch(bad, 1);
 		}
+	}
+	__syncthreads();
+	if (s_fail || s_len > slot_bytes)
 		return;
-	}
-	unsigned char *o = headers + (size_t) blockIdx.x * kHeaderSlot;
-	for (unsigned i = threadIdx.x; i < prefix_len; i += blockDim.x)
-		o[i] = prefix[i];
-	for (unsigned i = threadIdx.x; i < suffix_len; i += blockDim.x)
-		o[len - suffix_len + i] = suffix[i];
-	if (w < ntab && lane == 0) {
-		unsigned at = prefix_len;
-		for (int t = 0; t < w; t++)
-			at += 21 + table_values(s_bits[t]);
-		put_dht(o + at, w, s_bits[w], s_val[w]);
-	}
-	if (threadIdx.x == 0)
-		header_lens[blockIdx.x] = len;
+	unsigned char *o = headers + (size_t) blockIdx.x * slot_bytes;
+	for (int i = threadIdx.x; i < P.prefix_len; i += blockDim.x)
+		o[i] = tmpl[i];
+	for (int s = 0; s < P.nscans; s++)
+		for (int i = P.sfx_at[s] + threadIdx.x; i < P.sfx_at[s + 1]; i += blockDim.x)
+			o[s_sfx_dst[s] + (unsigned) (i - P.sfx_at[s])] = tmpl[i];
+	if (w < P.ntab && lane == 0)
+		put_dht(o + s_dht_at[w], P.tab_class[w], s_bits[w], s_val[w]);
 }
 
-/* one thread per block: how many bits its code takes */
-template <bool kFrameHuff, bool kRestart>
+/* one thread per block: how many bits its code takes, into the frame's list of G.blocks + 1 slots (the last is the
+ * bit prefix sum's)
+ */
+template <bool kFrameTables, bool kRestart>
 __global__ void __launch_bounds__(128)
-jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const FrameHuff *__restrict__ huff, int restart,
+jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const HuffSet<4> *__restrict__ huff, int restart,
 	const short *__restrict__ coef, unsigned *__restrict__ bits)
 {
 	const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1055,77 +1042,82 @@ jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const 
 	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
 	const unsigned (*co)[256];
 	const unsigned char (*si)[256];
-	frame_tables<kFrameHuff>(T, huff, blockIdx.y, &co, &si);
-	bits[(size_t) blockIdx.y * G.blocks + b] = code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)),
+	frame_tables<kFrameTables>(T, huff, blockIdx.y, &co, &si);
+	bits[(size_t) blockIdx.y * (G.blocks + 1) + b] = code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)),
 		previous_dc(G, fc, b, kRestart ? restart : 0), [](unsigned, int) {});
 }
 
-/* exclusive prefix sum of a frame's per-block bit counts (in place), total into totals[frame]: one CTA per frame */
-__global__ void __launch_bounds__(1024)
-jpeg_bitscan_kernel(int blocks, unsigned *__restrict__ bits, unsigned long long *__restrict__ totals)
+/* Exclusive prefix sum over items 0 .. n - 1 in one CTA: each thread sums a contiguous chunk of val(i), the chunk sums
+ * are scanned in s_part[blockDim.x] (shared memory), then put(i, the sum of the items before i) is called for every item
+ * in order, each after its val(i).  Returns the sum of all items.
+ */
+template <typename T, typename Val, typename Put>
+__device__ __forceinline__ T
+cta_exclusive_scan(unsigned n, T *s_part, Val val, Put put)
 {
-	__shared__ unsigned long long s_part[1024];
-	unsigned *b = bits + (size_t) blockIdx.x * blocks;
-	const unsigned per = ((unsigned) blocks + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min((unsigned) blocks, threadIdx.x * per), e = min((unsigned) blocks, a + per);
-	unsigned long long sum = 0;
+	const unsigned per = (n + blockDim.x - 1) / blockDim.x;
+	const unsigned a = min(n, threadIdx.x * per), e = min(n, a + per);
+	T sum = 0;
 	for (unsigned i = a; i < e; i++)
-		sum += b[i];
+		sum += val(i);
 	s_part[threadIdx.x] = sum;
 	__syncthreads();
 	for (unsigned o = 1; o < blockDim.x; o <<= 1) {
-		const unsigned long long v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
+		const T v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
 		__syncthreads();
 		s_part[threadIdx.x] += v;
 		__syncthreads();
 	}
-	unsigned long long run = s_part[threadIdx.x] - sum;
+	T run = s_part[threadIdx.x] - sum;
 	for (unsigned i = a; i < e; i++) {
-		const unsigned n = b[i];
-		b[i] = (unsigned) run; /* a frame's scan stays far below 2^32 bits (65535 x 65535 would not, and is refused) */
-		run += n;
+		const T v = val(i);
+		put(i, run);
+		run += v;
 	}
-	if (threadIdx.x == blockDim.x - 1)
-		totals[blockIdx.x] = s_part[threadIdx.x];
+	return s_part[blockDim.x - 1];
 }
 
-/* restart intervals, one CTA per frame: each interval takes its blocks' bits rounded up to a whole byte (the 1-padding
- * before each RSTn), istart[frame][k] = the byte where interval k starts in the raw scan (an exclusive prefix sum over
- * intervals), and totals[frame] becomes the padded scan's length in bits (whole bytes)
+/* exclusive prefix sum of a frame's bit counts (in place) over its nslots slots, the last of which receives the total,
+ * as does totals[frame]: one CTA per frame
  */
 __global__ void __launch_bounds__(1024)
-jpeg_intervals_kernel(int blocks, int blocks_per_interval, int nint, const unsigned *__restrict__ offs, unsigned long long *__restrict__ totals,
+jpeg_bitscan_kernel(int nslots, unsigned *__restrict__ bits, unsigned long long *__restrict__ totals)
+{
+	__shared__ unsigned long long s_part[1024];
+	unsigned *b = bits + (size_t) blockIdx.x * nslots;
+	/* a frame's scan stays far below 2^32 bits (65535 x 65535 would not, and is refused) */
+	const unsigned long long total = cta_exclusive_scan(
+		(unsigned) nslots - 1, s_part, [&](unsigned i) { return b[i]; }, [&](unsigned i, unsigned long long run) { b[i] = (unsigned) run; });
+	if (threadIdx.x == blockDim.x - 1) {
+		b[nslots - 1] = (unsigned) total;
+		totals[blockIdx.x] = total;
+	}
+}
+
+/* a sequential frame's segments in its bit list: restart interval g starts at slot g * per, the final slot is end */
+struct IntervalSlots {
+	unsigned per, nseg, end;
+	__device__ __forceinline__ unsigned operator()(unsigned g) const { return g < nseg ? g * per : end; }
+};
+
+/* Segments after the bit prefix sum, one CTA per frame: segment g (a restart interval of a scan, or a whole scan without
+ * them) spans slots M(g) .. M(g + 1) of the frame's nslots and takes their bits rounded up to a whole byte (the 1-padding
+ * before each RSTn or scan header); istart[frame][g] = the byte where it starts in the raw scan data, totals[frame] =
+ * their length in bits (whole bytes)
+ */
+template <typename Slots>
+__global__ void __launch_bounds__(1024)
+jpeg_segments_kernel(const __grid_constant__ Slots M, int nseg, int nslots, const unsigned *__restrict__ offs, unsigned long long *__restrict__ totals,
 	unsigned *__restrict__ istart)
 {
 	__shared__ unsigned long long s_part[1024];
-	const unsigned *o = offs + (size_t) blockIdx.x * blocks;
-	unsigned *st = istart + (size_t) blockIdx.x * nint;
-	const unsigned long long total = totals[blockIdx.x];
-	auto ibytes = [&](unsigned k) {
-		const unsigned long long b0 = o[(size_t) k * blocks_per_interval];
-		const unsigned long long b1 = k + 1 < (unsigned) nint ? o[(size_t) (k + 1) * blocks_per_interval] : total;
-		return (b1 - b0 + 7) >> 3;
-	};
-	const unsigned per = ((unsigned) nint + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min((unsigned) nint, threadIdx.x * per), e = min((unsigned) nint, a + per);
-	unsigned long long sum = 0;
-	for (unsigned k = a; k < e; k++)
-		sum += ibytes(k);
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	for (unsigned d = 1; d < blockDim.x; d <<= 1) {
-		const unsigned long long v = threadIdx.x >= d ? s_part[threadIdx.x - d] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned long long run = s_part[threadIdx.x] - sum;
-	for (unsigned k = a; k < e; k++) {
-		st[k] = (unsigned) run;
-		run += ibytes(k);
-	}
+	const unsigned *o = offs + (size_t) blockIdx.x * nslots;
+	unsigned *st = istart + (size_t) blockIdx.x * nseg;
+	const unsigned long long bytes = cta_exclusive_scan(
+		(unsigned) nseg, s_part, [&](unsigned g) { return ((unsigned long long) o[M(g + 1)] - o[M(g)] + 7) >> 3; },
+		[&](unsigned g, unsigned long long run) { st[g] = (unsigned) run; });
 	if (threadIdx.x == blockDim.x - 1)
-		totals[blockIdx.x] = s_part[threadIdx.x] * 8;
+		totals[blockIdx.x] = bytes * 8;
 }
 
 /* the number of the n ascending values p[] below v */
@@ -1148,9 +1140,9 @@ count_below(const unsigned *p, int n, unsigned long long v)
  * byte with 1-bits.  With restart intervals a block's bit offset is relative to its interval, which starts at byte
  * istart[frame][k].
  */
-template <bool kFrameHuff, bool kRestart>
+template <bool kFrameTables, bool kRestart>
 __global__ void __launch_bounds__(128)
-jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const FrameHuff *__restrict__ huff, int restart, int nint,
+jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const HuffSet<4> *__restrict__ huff, int restart, int nint,
 	const unsigned *__restrict__ istart, const short *__restrict__ coef, const unsigned *__restrict__ offs, unsigned *__restrict__ raw,
 	size_t raw_words)
 {
@@ -1159,7 +1151,7 @@ jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const F
 		return;
 	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
 	unsigned *out = raw + (size_t) blockIdx.y * raw_words;
-	const unsigned *fo = offs + (size_t) blockIdx.y * G.blocks;
+	const unsigned *fo = offs + (size_t) blockIdx.y * G.blocks + blockIdx.y;
 	unsigned pos = fo[b]; /* bit index */
 	bool last = b == (unsigned) G.blocks - 1;
 	if (kRestart) {
@@ -1183,7 +1175,7 @@ jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const F
 	};
 	const unsigned (*co)[256];
 	const unsigned char (*si)[256];
-	frame_tables<kFrameHuff>(T, huff, blockIdx.y, &co, &si);
+	frame_tables<kFrameTables>(T, huff, blockIdx.y, &co, &si);
 	code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)), previous_dc(G, fc, b, kRestart ? restart : 0),
 		put);
 	if (nacc > 0) {
@@ -1195,122 +1187,14 @@ jpeg_emit_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const F
 	}
 }
 
-/* stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw scan; with restart intervals, plus 2 bytes
- * for every RSTn marker that goes before a byte of the span (interval starts 1 .. nint - 1)
- */
-template <bool kRestart>
-__global__ void __launch_bounds__(128)
-jpeg_ffcount_kernel(const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw, size_t raw_bytes, int max_chunks,
-	int nint, const unsigned *__restrict__ istart, unsigned *__restrict__ counts)
-{
-	const int c = blockIdx.x * blockDim.x + threadIdx.x;
-	if (c >= max_chunks)
-		return;
-	const unsigned long long nbytes = (totals[blockIdx.y] + 7) >> 3;
-	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
-	unsigned n = 0;
-	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
-	for (unsigned long long i = a; i < e; i++)
-		n += p[i] == 0xFF;
-	if (kRestart && a < e) {
-		const unsigned *st = istart + (size_t) blockIdx.y * nint + 1;
-		n += 2 * (unsigned) (count_below(st, nint - 1, e) - count_below(st, nint - 1, a));
-	}
-	counts[(size_t) blockIdx.y * max_chunks + c] = n;
-}
-
-/* stuffing, pass 2: prefix sum of the spans' counts, one CTA per frame; lengths[frame] = header + scan + stuffed zeros +
- * markers + EOI.  The header is the batch's (header_len) or, with optimised tables, the frame's (header_lens[frame]).
- */
-template <bool kFrameHeader>
-__global__ void __launch_bounds__(1024)
-jpeg_ffscan_kernel(const unsigned long long *__restrict__ totals, int max_chunks, unsigned *__restrict__ counts, unsigned header_len,
-	const unsigned *__restrict__ header_lens, unsigned long long *__restrict__ lengths)
-{
-	if (kFrameHeader)
-		header_len = header_lens[blockIdx.x];
-	__shared__ unsigned s_part[1024];
-	unsigned *cnt = counts + (size_t) blockIdx.x * max_chunks;
-	const unsigned per = ((unsigned) max_chunks + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min((unsigned) max_chunks, threadIdx.x * per), e = min((unsigned) max_chunks, a + per);
-	unsigned sum = 0;
-	for (unsigned i = a; i < e; i++)
-		sum += cnt[i];
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	for (unsigned o = 1; o < blockDim.x; o <<= 1) {
-		const unsigned v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned run = s_part[threadIdx.x] - sum;
-	for (unsigned i = a; i < e; i++) {
-		const unsigned n = cnt[i];
-		cnt[i] = run;
-		run += n;
-	}
-	if (threadIdx.x == blockDim.x - 1)
-		lengths[blockIdx.x] = (unsigned long long) header_len + ((totals[blockIdx.x] + 7) >> 3) + s_part[threadIdx.x] + 2;
-}
-
-/* stuffing, pass 3: header, stuffed scan, EOI into the caller's stream (a stream that does not fit is cut: the host
- * compares lengths[frame] with the stride and reports it).  With optimised tables the header is the frame's slot of
- * kHeaderSlot bytes; with restart intervals FF D0+((k - 1) & 7) goes before the first byte of interval k >= 1 (padding
- * bytes are stuffed, markers are not).
- */
-template <bool kFrameHeader, bool kRestart>
-__global__ void __launch_bounds__(128)
-jpeg_stuff_kernel(const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw, size_t raw_bytes, int max_chunks,
-	const unsigned *__restrict__ counts, const unsigned char *__restrict__ header, unsigned header_len, const unsigned *__restrict__ header_lens,
-	int nint, const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride, const unsigned long long *__restrict__ lengths)
-{
-	const int c = blockIdx.x * blockDim.x + threadIdx.x;
-	unsigned char *o = out + (size_t) blockIdx.y * out_stride;
-	const unsigned long long len = lengths[blockIdx.y];
-	if (len > out_stride)
-		return;
-	if (kFrameHeader) {
-		header += (size_t) blockIdx.y * kHeaderSlot;
-		header_len = header_lens[blockIdx.y];
-	}
-	if (c < (int) ((header_len + kStuffChunk - 1) / kStuffChunk)) {
-		/* the first spans' threads also copy the header */
-		for (unsigned i = (unsigned) c * kStuffChunk; i < min(header_len, (unsigned) (c + 1) * kStuffChunk); i++)
-			o[i] = header[i];
-	}
-	if (c >= max_chunks)
-		return;
-	const unsigned long long nbytes = (totals[blockIdx.y] + 7) >> 3;
-	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
-	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
-	unsigned char *d = o + header_len + a + counts[(size_t) blockIdx.y * max_chunks + c];
-	const unsigned *st = istart + (size_t) blockIdx.y * nint;
-	int k = kRestart && a < e ? 1 + count_below(st + 1, nint - 1, a) : 0; /* the next interval starting in the span */
-	for (unsigned long long i = a; i < e; i++) {
-		const unsigned char v = p[i];
-		if (kRestart && k < nint && st[k] == i) {
-			*d++ = 0xFF;
-			*d++ = (unsigned char) (0xD0 + ((k - 1) & 7));
-			k++;
-		}
-		*d++ = v;
-		if (v == 0xFF)
-			*d++ = 0;
-	}
-	if (c == 0) {
-		o[len - 2] = 0xFF;
-		o[len - 1] = 0xD9;
-	}
-}
-
 /* ------------------------------------------------------------------ progressive save (interlace) on the device
  *
- * Every scan of the script is coded in the same launches: a frame's units (ProgScan) of all scans form one list, each
+ * Every scan of the script is coded in the same launches: a frame's units (Scan) of all scans form one list, each
  * unit owns two bit slots -- [the EOB run flushed before it + its own symbols] and [the run flushed after it] -- and a
  * final empty slot makes the frame's total.  A segment is a restart interval of a scan (the whole scan without them);
  * every segment starts on a byte boundary and ends padded with 1-bits, and the stuffing stage puts the next scan's
- * header (DHTs, SOS) or FF Dn between segments.
+ * header (DHTs, SOS) or FF Dn between segments.  The coders are numbered in launch order; 3 (jpeg_tables_kernel),
+ * 5 (jpeg_segments_kernel) and the stuffing passes are the sequential stream's too.
  */
 
 /* a unit's bit slots and a frame's bit slot count */
@@ -1335,14 +1219,8 @@ static_assert(kProgHeaderBound <= kProgHeaderSlot, "a frame's progressive header
 constexpr unsigned kMaxEobRun = 0x7FFF;
 static_assert(kMaxEobRun < (1u << 16) && kMaxCorrBits < (1 << 16), "a flush packs its run and its correction bits in 16 bits each");
 
-/* a frame's code tables, one per table of the script */
-struct ProgHuff {
-	unsigned ehufco[kMaxProgTables][256];
-	unsigned char ehufsi[kMaxProgTables][256];
-};
-
 __device__ __forceinline__ int
-prog_scan_of_unit(const ProgScript &P, unsigned u)
+prog_scan_of_unit(const ScanScript &P, unsigned u)
 {
 	int s = 0;
 	while (s + 1 < P.nscans && u >= (unsigned) P.s[s + 1].unit_base)
@@ -1351,7 +1229,7 @@ prog_scan_of_unit(const ProgScript &P, unsigned u)
 }
 
 __device__ __forceinline__ int
-prog_scan_of_seg(const ProgScript &P, unsigned g)
+scan_of_seg(const ScanScript &P, unsigned g)
 {
 	int s = 0;
 	while (s + 1 < P.nscans && g >= (unsigned) P.s[s + 1].seg_base)
@@ -1361,18 +1239,24 @@ prog_scan_of_seg(const ProgScript &P, unsigned g)
 
 /* the first bit slot of segment g (g == nseg: the frame's final slot) */
 __device__ __forceinline__ unsigned
-prog_seg_slot(const ProgScript &P, unsigned g)
+prog_seg_slot(const ScanScript &P, unsigned g)
 {
 	if (g >= (unsigned) P.nseg)
 		return kProgSlotsPerUnit * (unsigned) P.units;
-	const ProgScan &S = P.s[prog_scan_of_seg(P, g)];
+	const Scan &S = P.s[scan_of_seg(P, g)];
 	const unsigned per = P.restart ? (unsigned) P.restart : (unsigned) S.units;
 	return kProgSlotsPerUnit * ((unsigned) S.unit_base + (g - (unsigned) S.seg_base) * per);
 }
 
+/* a progressive frame's segments in its bit list (jpeg_segments_kernel) */
+struct ScriptSlots {
+	ScanScript P;
+	__device__ __forceinline__ unsigned operator()(unsigned g) const { return prog_seg_slot(P, g); }
+};
+
 /* the block of unit i of a single-component scan */
 __device__ __forceinline__ unsigned
-prog_block(const EncodeGeom &G, const ProgScan &S, unsigned i)
+prog_block(const EncodeGeom &G, const Scan &S, unsigned i)
 {
 	return comp_block_index(G, S.comp, (int) (i % (unsigned) S.ux), (int) (i / (unsigned) S.ux));
 }
@@ -1448,7 +1332,7 @@ struct BitSink {
  * CTA's histograms (a table per scan), added to the frame's counts[kMaxProgTables][256]
  */
 __global__ void __launch_bounds__(128)
-jpeg_prog_summary_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const short *__restrict__ coef,
+jpeg_prog_summary_kernel(const EncodeGeom G, const __grid_constant__ ScanScript P, const EncodeTables *__restrict__ T, const short *__restrict__ coef,
 	unsigned char *__restrict__ summ, unsigned *__restrict__ counts)
 {
 	__shared__ unsigned s_hist[kMaxProgTables * 256];
@@ -1457,7 +1341,7 @@ jpeg_prog_summary_kernel(const EncodeGeom G, const __grid_constant__ ProgScript 
 	__syncthreads();
 	const unsigned u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u < (unsigned) P.units) {
-		const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+		const Scan &S = P.s[prog_scan_of_unit(P, u)];
 		const unsigned i = u - (unsigned) S.unit_base;
 		const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
 		unsigned *h = s_hist + S.tab * 256;
@@ -1484,13 +1368,13 @@ jpeg_prog_summary_kernel(const EncodeGeom G, const __grid_constant__ ProgScript 
  * correction bits gets the flush's slot (defer_slot) and the offset of its bits among the flush's (defer_off).
  */
 __global__ void __launch_bounds__(128)
-jpeg_prog_walk_kernel(const __grid_constant__ ProgScript P, const unsigned char *__restrict__ summ, unsigned *__restrict__ runs,
+jpeg_prog_walk_kernel(const __grid_constant__ ScanScript P, const unsigned char *__restrict__ summ, unsigned *__restrict__ runs,
 	unsigned *__restrict__ defer_slot, unsigned short *__restrict__ defer_off, unsigned *__restrict__ counts)
 {
 	const unsigned g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= (unsigned) P.nseg)
 		return;
-	const ProgScan &S = P.s[prog_scan_of_seg(P, g)];
+	const Scan &S = P.s[scan_of_seg(P, g)];
 	if (S.ss == 0)
 		return;
 	const size_t f = blockIdx.y;
@@ -1529,89 +1413,6 @@ jpeg_prog_walk_kernel(const __grid_constant__ ProgScript P, const unsigned char 
 		flush(kProgSlotsPerUnit * (u1 - 1) + 1, u1 - 1);
 }
 
-/* 3. tables and headers, one CTA per frame, one warp per table of the script: gen_optimal_table on the table's counts,
- * the frame's code tables, then its headers into its kProgHeaderSlot-byte slot -- the markers before the first scan, and
- * per scan its DHTs and DRI / SOS from the template --; hdr_at[frame][s] = where scan s's header starts (0 for the first,
- * which comes with the frame's markers; [nscans] = the end), header_lens[frame] = the bytes before the first scan's data
- * (the stuffing passes count the later headers and the RSTn markers).  A frame whose tables cannot be built sets *bad.
- */
-__global__ void __launch_bounds__(32 * kMaxProgTables)
-jpeg_prog_huffopt_kernel(const __grid_constant__ ProgScript P, const unsigned *__restrict__ counts, ProgHuff *__restrict__ huff,
-	const unsigned char *__restrict__ tmpl, unsigned char *__restrict__ headers, unsigned *__restrict__ hdr_at, unsigned *__restrict__ header_lens,
-	int *__restrict__ bad)
-{
-	__shared__ unsigned s_freq[kMaxProgTables][257];
-	__shared__ int s_size[kMaxProgTables][257], s_others[kMaxProgTables][257];
-	__shared__ unsigned char s_bits[kMaxProgTables][17], s_val[kMaxProgTables][256];
-	__shared__ unsigned s_dht_at[kMaxProgTables], s_sfx_dst[kMaxProgScans], s_len;
-	__shared__ int s_fail;
-	const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const unsigned *cnt = counts + (size_t) blockIdx.x * kMaxProgTables * 256;
-	if (threadIdx.x == 0)
-		s_fail = 0;
-	for (int i = threadIdx.x; i < kMaxProgTables * 256; i += blockDim.x)
-		s_freq[i >> 8][i & 255] = cnt[i];
-	__syncthreads();
-	ProgHuff *fh = huff + blockIdx.x;
-	if (w < P.ntab) {
-		unsigned *freq = s_freq[w];
-		auto pick = [&](int exclude) {
-			__syncwarp();
-			/* key: frequency, then the larger index first */
-			unsigned long long best = ~0ull;
-			for (int i = lane; i <= 256; i += 32) {
-				const unsigned f = freq[i];
-				if (f && f <= kFreqSentinel && i != exclude) {
-					const unsigned long long key = ((unsigned long long) f << 9) | (unsigned) (511 - i);
-					best = key < best ? key : best;
-				}
-			}
-			for (int o = 16; o; o >>= 1) {
-				const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
-				best = v < best ? v : best;
-			}
-			return best == ~0ull ? -1 : 511 - (int) (best & 511u);
-		};
-		if (gen_optimal_table(freq, s_size[w], s_others[w], s_bits[w], s_val[w], lane == 0, pick))
-			s_fail = 1;
-		__syncwarp();
-		if (lane == 0)
-			derive_codes(s_bits[w] + 1, s_val[w], fh->ehufco[w], fh->ehufsi[w]);
-	}
-	__syncthreads();
-	unsigned *at = hdr_at + (size_t) blockIdx.x * (kMaxProgScans + 1);
-	if (threadIdx.x == 0) {
-		unsigned len = (unsigned) P.prefix_len;
-		for (int s = 0; s < P.nscans; s++) {
-			at[s] = s ? len : 0;
-			for (int t = P.s[s].tab; t < P.s[s].tab + P.s[s].nt; t++) {
-				s_dht_at[t] = len;
-				len += 21 + table_values(s_bits[t]);
-			}
-			s_sfx_dst[s] = len;
-			len += (unsigned) (P.sfx_at[s + 1] - P.sfx_at[s]);
-		}
-		at[P.nscans] = len;
-		s_len = len;
-		header_lens[blockIdx.x] = at[1];
-		if (s_fail || len > kProgHeaderSlot) {
-			header_lens[blockIdx.x] = 0;
-			atomicExch(bad, 1);
-		}
-	}
-	__syncthreads();
-	if (s_fail || s_len > kProgHeaderSlot)
-		return;
-	unsigned char *o = headers + (size_t) blockIdx.x * kProgHeaderSlot;
-	for (int i = threadIdx.x; i < P.prefix_len; i += blockDim.x)
-		o[i] = tmpl[i];
-	for (int s = 0; s < P.nscans; s++)
-		for (int i = P.sfx_at[s] + threadIdx.x; i < P.sfx_at[s + 1]; i += blockDim.x)
-			o[s_sfx_dst[s] + (unsigned) (i - P.sfx_at[s])] = tmpl[i];
-	if (w < P.ntab && lane == 0)
-		put_dht(o + s_dht_at[w], P.tab_class[w], s_bits[w], s_val[w]);
-}
-
 /* the bits of a flushed EOB run: EOBn code, n bits of the run, its correction bits */
 __device__ __forceinline__ unsigned
 flush_bits(const unsigned char *si, unsigned r)
@@ -1624,20 +1425,18 @@ flush_bits(const unsigned char *si, unsigned r)
 
 /* 4. one thread per unit: the bits of its two slots with the frame's tables */
 __global__ void __launch_bounds__(128)
-jpeg_prog_count_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const ProgHuff *__restrict__ huff,
+jpeg_prog_count_kernel(const EncodeGeom G, const __grid_constant__ ScanScript P, const EncodeTables *__restrict__ T, const HuffSet<kMaxProgTables> *__restrict__ huff,
 	const short *__restrict__ coef, const unsigned *__restrict__ runs, unsigned *__restrict__ bits)
 {
 	const unsigned u = blockIdx.x * blockDim.x + threadIdx.x;
 	const size_t nslots = (size_t) kProgSlotsPerUnit * P.units + 1;
 	unsigned *fb = bits + blockIdx.y * nslots;
-	if (u == 0)
-		fb[nslots - 1] = 0;
 	if (u >= (unsigned) P.units)
 		return;
-	const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+	const Scan &S = P.s[prog_scan_of_unit(P, u)];
 	const unsigned i = u - (unsigned) S.unit_base;
 	const short *fc = coef + (size_t) blockIdx.y * G.blocks * 64;
-	const ProgHuff &H = huff[blockIdx.y];
+	const HuffSet<kMaxProgTables> &H = huff[blockIdx.y];
 	unsigned body = 0, post = 0;
 	if (S.ss == 0) {
 		if (S.ah == 0)
@@ -1658,46 +1457,12 @@ jpeg_prog_count_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P,
 	fb[kProgSlotsPerUnit * u + 1] = post;
 }
 
-/* 5. after the bit prefix sum: segments, one CTA per frame.  Each takes its slots' bits rounded up to a whole byte,
- * istart[frame][g] = the byte where segment g starts in the raw scan data, totals[frame] = their length in bits
- */
-__global__ void __launch_bounds__(1024)
-jpeg_prog_segments_kernel(const __grid_constant__ ProgScript P, const unsigned *__restrict__ offs, unsigned long long *__restrict__ totals,
-	unsigned *__restrict__ istart)
-{
-	__shared__ unsigned long long s_part[1024];
-	const unsigned nseg = (unsigned) P.nseg;
-	const unsigned *o = offs + (size_t) blockIdx.x * ((size_t) kProgSlotsPerUnit * P.units + 1);
-	unsigned *st = istart + (size_t) blockIdx.x * nseg;
-	auto ibytes = [&](unsigned g) { return ((unsigned long long) o[prog_seg_slot(P, g + 1)] - o[prog_seg_slot(P, g)] + 7) >> 3; };
-	const unsigned per = (nseg + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min(nseg, threadIdx.x * per), e = min(nseg, a + per);
-	unsigned long long sum = 0;
-	for (unsigned k = a; k < e; k++)
-		sum += ibytes(k);
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	for (unsigned d = 1; d < blockDim.x; d <<= 1) {
-		const unsigned long long v = threadIdx.x >= d ? s_part[threadIdx.x - d] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned long long run = s_part[threadIdx.x] - sum;
-	for (unsigned k = a; k < e; k++) {
-		st[k] = (unsigned) run;
-		run += ibytes(k);
-	}
-	if (threadIdx.x == blockDim.x - 1)
-		totals[blockIdx.x] = s_part[threadIdx.x] * 8;
-}
-
 /* 6. one thread per unit: its symbols and the runs flushed around them OR-ed into the frame's raw bit buffer at its
  * slots, its deferred correction bits at the offset the walk gave them behind their flush's EOBn and run bits; the
  * segment's last unit pads the segment's last byte with 1-bits
  */
 __global__ void __launch_bounds__(128)
-jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, const EncodeTables *__restrict__ T, const ProgHuff *__restrict__ huff,
+jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ScanScript P, const EncodeTables *__restrict__ T, const HuffSet<kMaxProgTables> *__restrict__ huff,
 	const unsigned *__restrict__ istart, const short *__restrict__ coef, const unsigned *__restrict__ offs, const unsigned char *__restrict__ summ,
 	const unsigned *__restrict__ runs, const unsigned *__restrict__ defer_slot, const unsigned short *__restrict__ defer_off, unsigned *__restrict__ raw,
 	size_t raw_words)
@@ -1706,7 +1471,7 @@ jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, 
 	if (u >= (unsigned) P.units)
 		return;
 	const size_t f = blockIdx.y, nslots = (size_t) kProgSlotsPerUnit * P.units + 1;
-	const ProgScan &S = P.s[prog_scan_of_unit(P, u)];
+	const Scan &S = P.s[prog_scan_of_unit(P, u)];
 	const unsigned i = u - (unsigned) S.unit_base;
 	const unsigned g = (unsigned) S.seg_base + (P.restart ? i / (unsigned) P.restart : 0);
 	const unsigned *fo = offs + f * nslots;
@@ -1714,7 +1479,7 @@ jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, 
 	const unsigned base = istart[f * P.nseg + g] * 8 - fo[prog_seg_slot(P, g)];
 	unsigned *out = raw + f * raw_words;
 	const short *fc = coef + f * G.blocks * 64;
-	const ProgHuff &H = huff[f];
+	const HuffSet<kMaxProgTables> &H = huff[f];
 	BitSink w(out, base + fo[kProgSlotsPerUnit * u]);
 	if (S.ss == 0) {
 		if (S.ah == 0)
@@ -1766,82 +1531,122 @@ jpeg_prog_emit_kernel(const EncodeGeom G, const __grid_constant__ ProgScript P, 
 	}
 }
 
-/* insertion bytes before segments 1 .. j: the header of each scan that starts there (hdr_at), FF Dn before the others */
+/* ------------------------------------------------------------------ stuffing (sequential and progressive)
+ *
+ * A frame's raw data is its segments, each starting on a byte.  The stream is the frame's header, the raw data with
+ * FF -> FF 00 and, before each segment after the first, the next scan's header (DHTs, SOS) where a scan starts, else
+ * FF Dn; then EOI.  The header is the frame's own (slots of hdr_stride bytes, hdr_end[frame][nscans] from
+ * jpeg_tables_kernel) or, with the standard tables, the batch's: hdr_stride and hend_stride 0.  What goes between
+ * segments is a compile-time choice, so that a sequential stream's byte loop carries no scan-header copy:
+ */
+enum {
+	kOneSegment,	 /* nothing: a sequential stream without restart markers */
+	kRestartMarkers, /* FF Dn: the restart intervals of a sequential stream */
+	kScanHeaders	 /* FF Dn, or the next scan's header where a scan starts: a progressive stream */
+};
+
+/* insertion bytes before segments 1 .. j: the header of each scan that starts there, FF Dn before the others */
+template <int kInserts>
 __device__ __forceinline__ unsigned
-prog_inserts(const ProgScript &P, const unsigned *hat, unsigned j)
+inserts_before(const ScanScript &P, const unsigned *hend, unsigned j)
 {
 	unsigned n = 2 * j;
-	for (int s = 1; s < P.nscans && (unsigned) P.s[s].seg_base <= j; s++)
-		n += hat[s + 1] - hat[s] - 2;
+	if (kInserts == kScanHeaders)
+		for (int s = 1; s < P.nscans && (unsigned) P.s[s].seg_base <= j; s++)
+			n += hend[s] - hend[s - 1] - 2;
 	return n;
 }
 
-/* 7. stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw data, plus the bytes inserted before the
+/* stuffing, pass 1: 0xFF bytes per kStuffChunk-byte span of each frame's raw data, plus the bytes inserted before the
  * segments that start in the span
  */
+template <int kInserts>
 __global__ void __launch_bounds__(128)
-jpeg_prog_ffcount_kernel(const __grid_constant__ ProgScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
-	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ istart, const unsigned *__restrict__ hdr_at, unsigned *__restrict__ counts)
+jpeg_stuffcount_kernel(const __grid_constant__ ScanScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
+	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ istart, const unsigned *__restrict__ hdr_end, int hend_stride,
+	unsigned *__restrict__ counts)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	if (c >= max_chunks)
 		return;
-	const unsigned long long nbytes = totals[blockIdx.y] >> 3;
+	const unsigned long long nbytes = (totals[blockIdx.y] + 7) >> 3;
 	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
 	unsigned n = 0;
 	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
 	for (unsigned long long i = a; i < e; i++)
 		n += p[i] == 0xFF;
-	if (a < e) {
+	if (kInserts != kOneSegment && a < e) {
 		const unsigned *st = istart + (size_t) blockIdx.y * P.nseg + 1;
-		const unsigned *hat = hdr_at + (size_t) blockIdx.y * (kMaxProgScans + 1);
-		n += prog_inserts(P, hat, (unsigned) count_below(st, P.nseg - 1, e)) - prog_inserts(P, hat, (unsigned) count_below(st, P.nseg - 1, a));
+		const unsigned *hend = hdr_end + (size_t) blockIdx.y * hend_stride;
+		n += inserts_before<kInserts>(P, hend, (unsigned) count_below(st, P.nseg - 1, e)) -
+			 inserts_before<kInserts>(P, hend, (unsigned) count_below(st, P.nseg - 1, a));
 	}
 	counts[(size_t) blockIdx.y * max_chunks + c] = n;
 }
 
-/* 8. stuffing, pass 3 (pass 2 is jpeg_ffscan_kernel): the frame's markers and first scan header, the stuffed data with
- * the next scan's header or FF D0+((k - 1) & 7) before interval k >= 1 of a scan (RSTn numbering restarts with every
- * scan), EOI
+/* stuffing, pass 2: prefix sum of the spans' counts, one CTA per frame; lengths[frame] = header (hdr_end[frame][0]) + raw
+ * data + stuffed zeros + inserted bytes + EOI
  */
+__global__ void __launch_bounds__(1024)
+jpeg_ffscan_kernel(const unsigned long long *__restrict__ totals, int max_chunks, unsigned *__restrict__ counts, const unsigned *__restrict__ hdr_end,
+	int hend_stride, unsigned long long *__restrict__ lengths)
+{
+	__shared__ unsigned s_part[1024];
+	unsigned *cnt = counts + (size_t) blockIdx.x * max_chunks;
+	const unsigned added = cta_exclusive_scan(
+		(unsigned) max_chunks, s_part, [&](unsigned i) { return cnt[i]; }, [&](unsigned i, unsigned run) { cnt[i] = run; });
+	if (threadIdx.x == blockDim.x - 1)
+		lengths[blockIdx.x] = (unsigned long long) hdr_end[(size_t) blockIdx.x * hend_stride] + ((totals[blockIdx.x] + 7) >> 3) + added + 2;
+}
+
+/* stuffing, pass 3: the header, the stuffed data with the next scan's header or FF D0+((k - 1) & 7) before segment k >= 1
+ * of a scan (RSTn numbering restarts with every scan; padding bytes are stuffed, markers are not), EOI, into the caller's
+ * stream (a stream that does not fit is cut: the host compares lengths[frame] with the stride and reports it)
+ */
+template <int kInserts>
 __global__ void __launch_bounds__(128)
-jpeg_prog_stuff_kernel(const __grid_constant__ ProgScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
-	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ counts, const unsigned char *__restrict__ headers, const unsigned *__restrict__ hdr_at,
-	const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride, const unsigned long long *__restrict__ lengths)
+jpeg_stuffcopy_kernel(const __grid_constant__ ScanScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
+	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ counts, const unsigned char *__restrict__ headers, size_t hdr_stride,
+	const unsigned *__restrict__ hdr_end, int hend_stride, const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride,
+	const unsigned long long *__restrict__ lengths)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	unsigned char *o = out + (size_t) blockIdx.y * out_stride;
 	const unsigned long long len = lengths[blockIdx.y];
 	if (len > out_stride)
 		return;
-	const unsigned char *hdr = headers + (size_t) blockIdx.y * kProgHeaderSlot;
-	const unsigned *hat = hdr_at + (size_t) blockIdx.y * (kMaxProgScans + 1);
-	const unsigned h0 = hat[1];
-	if (c < (int) ((h0 + kStuffChunk - 1) / kStuffChunk))
+	const unsigned char *hdr = headers + (size_t) blockIdx.y * hdr_stride;
+	const unsigned *hend = hdr_end + (size_t) blockIdx.y * hend_stride;
+	const unsigned h0 = hend[0];
+	if (c < (int) ((h0 + kStuffChunk - 1) / kStuffChunk)) {
+		/* the first spans' threads also copy the header */
 		for (unsigned i = (unsigned) c * kStuffChunk; i < min(h0, (unsigned) (c + 1) * kStuffChunk); i++)
 			o[i] = hdr[i];
+	}
 	if (c >= max_chunks)
 		return;
-	const unsigned long long nbytes = totals[blockIdx.y] >> 3;
+	const unsigned long long nbytes = (totals[blockIdx.y] + 7) >> 3;
 	const unsigned char *p = raw + (size_t) blockIdx.y * raw_bytes;
 	const unsigned long long a = (unsigned long long) c * kStuffChunk, e = min(nbytes, a + kStuffChunk);
 	unsigned char *d = o + h0 + a + counts[(size_t) blockIdx.y * max_chunks + c];
 	const unsigned *st = istart + (size_t) blockIdx.y * P.nseg;
 	const unsigned nseg = (unsigned) P.nseg;
-	unsigned k = a < e ? 1 + (unsigned) count_below(st + 1, (int) nseg - 1, a) : nseg; /* the next segment starting in the span */
+	/* the next segment starting in the span */
+	unsigned k = kInserts != kOneSegment && a < e ? 1 + (unsigned) count_below(st + 1, (int) nseg - 1, a) : nseg;
 	for (unsigned long long i = a; i < e; i++) {
-		if (k < nseg && st[k] == i) {
-			const int s = prog_scan_of_seg(P, k);
-			if (k == (unsigned) P.s[s].seg_base)
-				for (unsigned j = hat[s]; j < hat[s + 1]; j++)
+		const unsigned char v = p[i];
+		if (kInserts != kOneSegment && k < nseg && st[k] == i) {
+			const int s = kInserts == kScanHeaders ? scan_of_seg(P, k) : 0;
+			const unsigned base = kInserts == kScanHeaders ? (unsigned) P.s[s].seg_base : 0;
+			if (kInserts == kScanHeaders && k == base)
+				for (unsigned j = hend[s - 1]; j < hend[s]; j++)
 					*d++ = hdr[j];
 			else {
 				*d++ = 0xFF;
-				*d++ = (unsigned char) (0xD0 + ((k - (unsigned) P.s[s].seg_base - 1) & 7));
+				*d++ = (unsigned char) (0xD0 + ((k - base - 1) & 7));
 			}
 			k++;
 		}
-		const unsigned char v = p[i];
 		*d++ = v;
 		if (v == 0xFF)
 			*d++ = 0;
@@ -1852,172 +1657,276 @@ jpeg_prog_stuff_kernel(const __grid_constant__ ProgScript P, const unsigned long
 	}
 }
 
-/* the device buffers of one chunk of frames */
-struct ChunkArgs {
+/* What one call encodes with, from its options: the geometry, the quantisation and standard tables, the scan script, the
+ * header -- with the standard tables the whole of it, else the template the table kernel builds each frame's headers from
+ * (the markers before the Huffman tables, then each scan's DRI / SOS) -- and the sizes of the per-frame buffers
+ */
+struct EncodePlan {
 	EncodeGeom G;
-	const EncodeTables *T;
-	const unsigned char *frames;
-	size_t bpl, frame_stride;
-	int cn, restart, nint, max_chunks;
-	short *coef;
-	unsigned *bits, *counts, *istart, *freq, *header_lens;
-	unsigned long long *totals, *lengths;
-	unsigned char *raw;
-	size_t raw_bytes;
-	FrameHuff *huff;
-	const unsigned char *header; /* the batch's header, or with optimised tables the prefix and suffix around the DHTs */
-	unsigned header_len, prefix_len, suffix_len;
-	unsigned char *headers; /* per-frame header slots */
-	int *bad;
-	unsigned char *out;
-	size_t out_stride;
+	EncodeTables T;
+	ScanScript P;
+	std::vector<unsigned char> header;
+	bool prog, opt;			   /* progressive; the frame's own tables (libjpeg forces them for a progressive stream) */
+	size_t nslots;			   /* bit slots per frame: a block each, or two a unit of the progressive script; and the final one */
+	size_t scan_bound;		   /* the raw data's bound: every segment may end with one byte of padding */
+	size_t raw_bytes;		   /* a frame's raw data buffer */
+	int max_chunks;			   /* its kStuffChunk-byte spans */
+	int ntab;				   /* the tables a frame can have: HuffSet<ntab> */
+	unsigned slot;			   /* a frame's header slot */
 };
 
-/* the kernels of one chunk: 7 launches with the standard tables and no restart intervals, +1 with restart intervals
- * (jpeg_intervals_kernel), +2 with optimised tables (jpeg_stats_kernel, jpeg_huffopt_kernel); returns the launch count,
- * -1 when the counts could not be cleared
- */
-template <bool kOpt, bool kRestart>
 int
-launch_chunk(const ChunkArgs &A, cudaStream_t s)
+make_plan(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, EncodePlan *E)
 {
-	const EncodeGeom &G = A.G;
-	const int mcus = G.mcus_x * G.mcus_y, cn = A.cn;
-	const dim3 per_block((G.blocks + 127) / 128, cn), per_span((A.max_chunks + 127) / 128, cn);
-	int launches = 7;
-	jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, A.T, A.frames, A.bpl, A.frame_stride, A.coef);
-	if (kOpt) {
-		if (cudaMemsetAsync(A.freq, 0, (size_t) cn * 4 * 256 * sizeof(unsigned), s) != cudaSuccess)
-			return -1;
-		jpeg_stats_kernel<<<per_block, 128, 0, s>>>(G, A.T, A.coef, A.restart, A.freq);
-		jpeg_huffopt_kernel<<<cn, 128, 0, s>>>(G.ncomp == 1 ? 2 : 4, A.freq, A.huff, A.header, A.prefix_len, A.header + A.prefix_len, A.suffix_len,
-			A.headers, A.header_lens, A.bad);
-		launches += 2;
-	}
-	jpeg_count_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, A.huff, A.restart, A.coef, A.bits);
-	jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(G.blocks, A.bits, A.totals);
-	if (kRestart) {
-		jpeg_intervals_kernel<<<cn, 1024, 0, s>>>(G.blocks, A.restart * G.blocks_per_mcu, A.nint, A.bits, A.totals, A.istart);
-		launches++;
-	}
-	jpeg_emit_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, A.huff, A.restart, A.nint, A.istart, A.coef, A.bits, (unsigned *) A.raw,
-		A.raw_bytes / 4);
-	jpeg_ffcount_kernel<kRestart><<<per_span, 128, 0, s>>>(A.totals, A.raw, A.raw_bytes, A.max_chunks, A.nint, A.istart, A.counts);
-	jpeg_ffscan_kernel<kOpt><<<cn, 1024, 0, s>>>(A.totals, A.max_chunks, A.counts, A.header_len, A.header_lens, A.lengths);
-	jpeg_stuff_kernel<kOpt, kRestart><<<per_span, 128, 0, s>>>(A.totals, A.raw, A.raw_bytes, A.max_chunks, A.counts, kOpt ? A.headers : A.header,
-		A.header_len, A.header_lens, A.nint, A.istart, A.out, A.out_stride, A.lengths);
-	return launches;
-}
-
-} // namespace
-
-/* n equally sized 8-bit frames (1 or 3 bands) on the device -> n JPEG streams at out + i * out_stride (device), their
- * lengths to lengths_host[n].  optimize: per-frame Huffman tables from the frame's symbol counts; restart: MCUs per
- * restart interval (0: none).  Stream-ordered on s; returns after the lengths are known.
- */
-int
-dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, int quality,
-	int subsample_mode, int optimize, int restart, void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
-{
-	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
+	EncodeGeom &G = E->G;
+	ScanScript &P = E->P;
+	const int restart = o.restart_interval;
+	if (make_geom(domain, w, h, bands, o.Q, o.subsample_mode, &G) || check_restart(domain, restart))
 		return -1;
-	const int mcus = G.mcus_x * G.mcus_y;
-	const int nint = restart ? (mcus + restart - 1) / restart : 1;
-	/* every interval may end with one byte of padding */
-	const size_t scan_bound = (size_t) G.blocks * kMaxBlockBytes + (restart ? (size_t) nint : 0);
-	if (scan_bound >= (size_t) 1 << 29) {
+	E->prog = o.interlace != 0;
+	E->opt = E->prog || o.optimize_coding;
+	scan_script(G, restart, E->prog, &P);
+	E->nslots = (E->prog ? kProgSlotsPerUnit * (size_t) P.units : (size_t) G.blocks) + 1;
+	E->scan_bound = (size_t) G.blocks * (E->prog ? kProgBlockBytes : kMaxBlockBytes) + (size_t) P.nseg;
+	if (E->scan_bound >= (size_t) 1 << 29) {
 		error(domain, "frame too large for the device encoder");
 		return -1;
 	}
-	EncodeTables T;
-	make_tables(quality, &T);
-	/* standard tables: the whole header; optimised tables: the markers before and after the DHTs (prefix_len bytes, then
-	 * the suffix), which jpeg_huffopt_kernel puts around each frame's own tables
-	 */
-	std::vector<unsigned char> header, suffix;
-	unsigned prefix_len = 0;
-	if (optimize) {
-		header_prefix(G, T, header);
-		prefix_len = (unsigned) header.size();
-		header_suffix(G, restart, suffix);
-		header.insert(header.end(), suffix.begin(), suffix.end());
+	make_tables(o.Q, &E->T);
+	std::vector<unsigned char> &hd = E->header;
+	header_prefix(G, E->T, hd, E->prog ? 0xFFC2 : 0xFFC0);
+	if (!E->opt) {
+		unsigned char bits[4][17], huffval[4][256];
+		standard_tables(bits, huffval);
+		put_dhts(G, bits, huffval, hd);
 	}
-	else
-		write_headers(G, T, restart, header);
-	const size_t raw_bytes = ((scan_bound + 3) & ~(size_t) 3) + 4;
-	const int max_chunks = (int) ((raw_bytes + kStuffChunk - 1) / kStuffChunk);
-	/* per-frame tables and header slots (about 10 KB a frame) for one chunk of frames, reused by the next */
-	const size_t nopt = optimize ? (size_t) std::min(n, kMaxBatchFrames) : 0;
-	/* one block of device scratch: tables | header | coefficients | bit counts / offsets | totals | lengths | raw | span counts
-	 * | interval starts | symbol counts | frame tables | header slots | header lengths | failure flag
-	 */
+	P.prefix_len = (int) hd.size();
+	for (int i = 0; i < P.nscans; i++) {
+		P.sfx_at[i] = (int) hd.size();
+		scan_suffix(G, P.s[i], i == 0, restart, hd);
+	}
+	P.sfx_at[P.nscans] = (int) hd.size();
+	E->raw_bytes = ((E->scan_bound + 3) & ~(size_t) 3) + 4;
+	E->max_chunks = (int) ((E->raw_bytes + kStuffChunk - 1) / kStuffChunk);
+	E->ntab = E->prog ? kMaxProgTables : 4;
+	E->slot = E->prog ? kProgHeaderSlot : kHeaderSlot;
+	return 0;
+}
+
+/* The device scratch of a call of n frames, one allocation: the buffers' offsets and the total.  Per frame: coefficients,
+ * bit slots, totals, lengths, raw data, span counts, segment starts and the progressive coder's unit summaries, flushed
+ * runs and deferred correction bits.  Per chunk of frames, reused by the next: symbol counts, code tables, header slots
+ * and header ends (with the standard tables, the batch's header length).  Every buffer grows with n or is shared, so
+ * carve(n) takes at most n times carve(1).
+ */
+struct Scratch {
+	size_t tab, hdr, coef, bits, tot, len, raw, cnt, ist, summ, runs, dslot, doff, freq, huff, slots, hend, bad, bytes;
+};
+
+Scratch
+carve(const EncodePlan &E, int n)
+{
+	const size_t nf = (size_t) n, units = E.prog ? (size_t) E.P.units : 0, nopt = E.opt ? (size_t) std::min(n, kMaxBatchFrames) : 0;
 	size_t off = 0;
 	auto take = [&](size_t bytes) {
 		const size_t o = off;
 		off += (bytes + 255) & ~(size_t) 255;
 		return o;
 	};
-	const size_t o_tab = take(sizeof(T)), o_hdr = take(header.size()), o_coef = take((size_t) n * G.blocks * 64 * sizeof(short)),
-				 o_bits = take((size_t) n * G.blocks * sizeof(unsigned)), o_tot = take((size_t) n * sizeof(unsigned long long)),
-				 o_len = take((size_t) n * sizeof(unsigned long long)), o_raw = take((size_t) n * raw_bytes),
-				 o_cnt = take((size_t) n * max_chunks * sizeof(unsigned)), o_ist = take(restart ? (size_t) n * nint * sizeof(unsigned) : 0),
-				 o_freq = take(nopt * 4 * 256 * sizeof(unsigned)), o_huff = take(nopt * sizeof(FrameHuff)), o_slots = take(nopt * kHeaderSlot),
-				 o_hlen = take(nopt * sizeof(unsigned)), o_bad = take(sizeof(int));
-	char *scratch = nullptr;
-	if (dev_alloc(domain, (void **) &scratch, off, s))
+	Scratch S;
+	S.tab = take(sizeof(EncodeTables));
+	S.hdr = take(E.header.size());
+	S.coef = take(nf * E.G.blocks * 64 * sizeof(short));
+	S.bits = take(nf * E.nslots * sizeof(unsigned));
+	S.tot = take(nf * sizeof(unsigned long long));
+	S.len = take(nf * sizeof(unsigned long long));
+	S.raw = take(nf * E.raw_bytes);
+	S.cnt = take(nf * E.max_chunks * sizeof(unsigned));
+	S.ist = take(E.prog || E.P.restart ? nf * E.P.nseg * sizeof(unsigned) : 0);
+	S.summ = take(nf * units);
+	S.runs = take(nf * kProgSlotsPerUnit * units * sizeof(unsigned));
+	S.dslot = take(nf * units * sizeof(unsigned));
+	S.doff = take(nf * units * sizeof(unsigned short));
+	S.freq = take(nopt * E.ntab * 256 * sizeof(unsigned));
+	S.huff = take(nopt * (E.prog ? sizeof(HuffSet<kMaxProgTables>) : sizeof(HuffSet<4>)));
+	S.slots = take(nopt * E.slot);
+	S.hend = take((E.opt ? nopt * E.P.nscans : 1) * sizeof(unsigned));
+	S.bad = take(sizeof(int));
+	S.bytes = off;
+	return S;
+}
+
+/* the device buffers of one chunk of frames */
+struct ChunkArgs {
+	const EncodePlan *E;
+	const EncodeTables *T;
+	const unsigned char *frames;
+	size_t bpl, frame_stride;
+	int cn;
+	short *coef;
+	unsigned *bits, *counts, *istart, *freq, *hdr_end;
+	unsigned long long *totals, *lengths;
+	unsigned char *raw;
+	void *huff;				   /* the frames' HuffSet<E->ntab> */
+	const unsigned char *tmpl; /* the plan's header */
+	unsigned char *slots;	   /* the frames' header slots */
+	unsigned char *summ;	   /* progressive: unit summaries, flushed runs, deferred correction bits */
+	unsigned *runs, *dslot;
+	unsigned short *doff;
+	int *bad;
+	unsigned char *out;
+	size_t out_stride;
+};
+
+/* a sequential chunk: 7 launches with the standard tables and no restart intervals, +1 with restart intervals
+ * (jpeg_segments_kernel), +2 with optimised tables (jpeg_stats_kernel, jpeg_tables_kernel); returns the launch count, -1
+ * when the counts could not be cleared
+ */
+template <bool kOpt, bool kRestart>
+int
+launch_chunk(const ChunkArgs &A, cudaStream_t s)
+{
+	const EncodePlan &E = *A.E;
+	const EncodeGeom &G = E.G;
+	const ScanScript &P = E.P;
+	const int mcus = G.mcus_x * G.mcus_y, cn = A.cn, nslots = (int) E.nslots;
+	const dim3 per_block((G.blocks + 127) / 128, cn), per_span((E.max_chunks + 127) / 128, cn);
+	HuffSet<4> *huff = (HuffSet<4> *) A.huff;
+	/* the frames' own headers, or the batch's for every frame */
+	const unsigned char *hdr = kOpt ? A.slots : A.tmpl;
+	const size_t hdr_stride = kOpt ? kHeaderSlot : 0;
+	const int hend_stride = kOpt ? 1 : 0;
+	int launches = 7;
+	jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, A.T, A.frames, A.bpl, A.frame_stride, A.coef);
+	if (kOpt) {
+		if (cudaMemsetAsync(A.freq, 0, (size_t) cn * 4 * 256 * sizeof(unsigned), s) != cudaSuccess)
+			return -1;
+		jpeg_stats_kernel<<<per_block, 128, 0, s>>>(G, A.T, A.coef, P.restart, A.freq);
+		jpeg_tables_kernel<4><<<cn, 32 * 4, 0, s>>>(P, A.freq, huff, A.tmpl, A.slots, kHeaderSlot, A.hdr_end, A.bad);
+		launches += 2;
+	}
+	jpeg_count_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, huff, P.restart, A.coef, A.bits);
+	jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(nslots, A.bits, A.totals);
+	if (kRestart) {
+		const IntervalSlots M = {(unsigned) (P.restart * G.blocks_per_mcu), (unsigned) P.nseg, (unsigned) G.blocks};
+		jpeg_segments_kernel<<<cn, 1024, 0, s>>>(M, P.nseg, nslots, A.bits, A.totals, A.istart);
+		launches++;
+	}
+	jpeg_emit_kernel<kOpt, kRestart><<<per_block, 128, 0, s>>>(G, A.T, huff, P.restart, P.nseg, A.istart, A.coef, A.bits, (unsigned *) A.raw,
+		E.raw_bytes / 4);
+	constexpr int kInserts = kRestart ? kRestartMarkers : kOneSegment;
+	jpeg_stuffcount_kernel<kInserts><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.istart, A.hdr_end, hend_stride, A.counts);
+	jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(A.totals, E.max_chunks, A.counts, A.hdr_end, hend_stride, A.lengths);
+	jpeg_stuffcopy_kernel<kInserts><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.counts, hdr, hdr_stride, A.hdr_end,
+		hend_stride, A.istart, A.out, A.out_stride, A.lengths);
+	return launches;
+}
+
+/* a progressive chunk: 11 launches whatever the frame count, scan count or restart interval -- FDCT, summaries, chain
+ * walk, tables and headers, bit counts, bit prefix sum, segments, emit, and the three stuffing passes; -1 when the counts
+ * could not be cleared
+ */
+int
+launch_progressive(const ChunkArgs &A, cudaStream_t s)
+{
+	const EncodePlan &E = *A.E;
+	const EncodeGeom &G = E.G;
+	const ScanScript &P = E.P;
+	const int mcus = G.mcus_x * G.mcus_y, cn = A.cn, nslots = (int) E.nslots;
+	const dim3 per_unit((P.units + 127) / 128, cn), per_span((E.max_chunks + 127) / 128, cn);
+	HuffSet<kMaxProgTables> *huff = (HuffSet<kMaxProgTables> *) A.huff;
+	jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, A.T, A.frames, A.bpl, A.frame_stride, A.coef);
+	if (cudaMemsetAsync(A.freq, 0, (size_t) cn * kMaxProgTables * 256 * sizeof(unsigned), s) != cudaSuccess)
 		return -1;
+	jpeg_prog_summary_kernel<<<per_unit, 128, 0, s>>>(G, P, A.T, A.coef, A.summ, A.freq);
+	jpeg_prog_walk_kernel<<<dim3((P.nseg + 127) / 128, cn), 128, 0, s>>>(P, A.summ, A.runs, A.dslot, A.doff, A.freq);
+	jpeg_tables_kernel<kMaxProgTables><<<cn, 32 * kMaxProgTables, 0, s>>>(P, A.freq, huff, A.tmpl, A.slots, kProgHeaderSlot, A.hdr_end, A.bad);
+	jpeg_prog_count_kernel<<<per_unit, 128, 0, s>>>(G, P, A.T, huff, A.coef, A.runs, A.bits);
+	jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>(nslots, A.bits, A.totals);
+	jpeg_segments_kernel<<<cn, 1024, 0, s>>>(ScriptSlots{P}, P.nseg, nslots, A.bits, A.totals, A.istart);
+	jpeg_prog_emit_kernel<<<per_unit, 128, 0, s>>>(G, P, A.T, huff, A.istart, A.coef, A.bits, A.summ, A.runs, A.dslot, A.doff, (unsigned *) A.raw,
+		E.raw_bytes / 4);
+	jpeg_stuffcount_kernel<kScanHeaders><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.istart, A.hdr_end, P.nscans, A.counts);
+	jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(A.totals, E.max_chunks, A.counts, A.hdr_end, P.nscans, A.lengths);
+	jpeg_stuffcopy_kernel<kScanHeaders><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.counts, A.slots, kProgHeaderSlot, A.hdr_end,
+		P.nscans, A.istart, A.out, A.out_stride, A.lengths);
+	return 11;
+}
+
+} // namespace
+
+/* n equally sized 8-bit frames (1 or 3 bands) on the device -> n JPEG streams at out + i * out_stride (device), their
+ * lengths to lengths_host[n], with vips_jpegsave's options o: sequential with the standard tables or, optimize_coding,
+ * per-frame tables from the frame's symbol counts; interlace, progressive with the scan script of jpeg_simple_progression,
+ * every scan with its own optimal tables; restart_interval MCUs per restart interval (0: none).  Stream-ordered on s;
+ * returns after the lengths are known.
+ */
+int
+dev_jpeg_encode(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, const VB200JpegSaveOptions &o,
+	void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
+{
+	EncodePlan E;
+	if (make_plan(domain, w, h, bands, o, &E))
+		return -1;
+	const Scratch S = carve(E, n);
+	char *scratch = nullptr;
+	if (dev_alloc(domain, (void **) &scratch, S.bytes, s))
+		return -1;
+	const unsigned header_len = (unsigned) E.header.size();
 	int rc = -1;
 	do {
-		/* tables and header from pageable memory: small, staged by the driver before the call returns */
-		if (cudaMemcpyAsync(scratch + o_tab, &T, sizeof(T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-			cudaMemcpyAsync(scratch + o_hdr, header.data(), header.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-			cudaMemsetAsync(scratch + o_raw, 0, (size_t) n * raw_bytes, s) != cudaSuccess ||
-			cudaMemsetAsync(scratch + o_bad, 0, sizeof(int), s) != cudaSuccess) {
+		/* tables and header (with the standard tables, its length too) from pageable memory: small, staged by the driver
+		 * before the call returns
+		 */
+		if (cudaMemcpyAsync(scratch + S.tab, &E.T, sizeof(E.T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+			cudaMemcpyAsync(scratch + S.hdr, E.header.data(), E.header.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+			(!E.opt && cudaMemcpyAsync(scratch + S.hend, &header_len, sizeof(header_len), cudaMemcpyHostToDevice, s) != cudaSuccess) ||
+			cudaMemsetAsync(scratch + S.raw, 0, (size_t) n * E.raw_bytes, s) != cudaSuccess ||
+			cudaMemsetAsync(scratch + S.bad, 0, sizeof(int), s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode setup");
 			break;
 		}
 		ChunkArgs A;
-		A.G = G;
-		A.T = (const EncodeTables *) (scratch + o_tab);
+		A.E = &E;
+		A.T = (const EncodeTables *) (scratch + S.tab);
 		A.bpl = bpl;
 		A.frame_stride = frame_stride;
-		A.restart = restart;
-		A.nint = nint;
-		A.max_chunks = max_chunks;
-		A.raw_bytes = raw_bytes;
-		A.freq = (unsigned *) (scratch + o_freq);
-		A.huff = (FrameHuff *) (scratch + o_huff);
-		A.header = (const unsigned char *) (scratch + o_hdr);
-		A.header_len = (unsigned) header.size();
-		A.prefix_len = prefix_len;
-		A.suffix_len = (unsigned) suffix.size();
-		A.headers = (unsigned char *) (scratch + o_slots);
-		A.header_lens = (unsigned *) (scratch + o_hlen);
-		A.bad = (int *) (scratch + o_bad);
+		A.freq = (unsigned *) (scratch + S.freq);
+		A.hdr_end = (unsigned *) (scratch + S.hend);
+		A.huff = scratch + S.huff;
+		A.tmpl = (const unsigned char *) (scratch + S.hdr);
+		A.slots = (unsigned char *) (scratch + S.slots);
+		A.bad = (int *) (scratch + S.bad);
 		A.out_stride = out_stride;
-		unsigned long long *lengths = (unsigned long long *) (scratch + o_len);
+		unsigned long long *lengths = (unsigned long long *) (scratch + S.len);
+		const size_t units = E.prog ? (size_t) E.P.units : 0;
+		const bool restart = E.P.restart > 0;
 		/* the frame is gridDim.y (or x) of every kernel: chunks of at most kMaxBatchFrames, each on its slice of the scratch */
 		cudaError_t e = cudaSuccess;
 		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
+			const size_t f0 = (size_t) c0;
 			A.cn = std::min(kMaxBatchFrames, n - c0);
-			A.frames = (const unsigned char *) frames + (size_t) c0 * frame_stride;
-			A.coef = (short *) (scratch + o_coef) + (size_t) c0 * G.blocks * 64;
-			A.bits = (unsigned *) (scratch + o_bits) + (size_t) c0 * G.blocks;
-			A.totals = (unsigned long long *) (scratch + o_tot) + c0;
-			A.lengths = lengths + c0;
-			A.raw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
-			A.counts = (unsigned *) (scratch + o_cnt) + (size_t) c0 * max_chunks;
-			A.istart = (unsigned *) (scratch + o_ist) + (size_t) c0 * nint;
-			A.out = (unsigned char *) out + (size_t) c0 * out_stride;
-			const int launches = optimize ? (restart ? launch_chunk<true, true>(A, s) : launch_chunk<true, false>(A, s))
-										  : (restart ? launch_chunk<false, true>(A, s) : launch_chunk<false, false>(A, s));
+			A.frames = (const unsigned char *) frames + f0 * frame_stride;
+			A.coef = (short *) (scratch + S.coef) + f0 * E.G.blocks * 64;
+			A.bits = (unsigned *) (scratch + S.bits) + f0 * E.nslots;
+			A.totals = (unsigned long long *) (scratch + S.tot) + f0;
+			A.lengths = lengths + f0;
+			A.raw = (unsigned char *) (scratch + S.raw) + f0 * E.raw_bytes;
+			A.counts = (unsigned *) (scratch + S.cnt) + f0 * E.max_chunks;
+			A.istart = (unsigned *) (scratch + S.ist) + f0 * E.P.nseg;
+			A.summ = (unsigned char *) (scratch + S.summ) + f0 * units;
+			A.runs = (unsigned *) (scratch + S.runs) + f0 * kProgSlotsPerUnit * units;
+			A.dslot = (unsigned *) (scratch + S.dslot) + f0 * units;
+			A.doff = (unsigned short *) (scratch + S.doff) + f0 * units;
+			A.out = (unsigned char *) out + f0 * out_stride;
+			const int launches = E.prog ? launch_progressive(A, s)
+							   : E.opt	? (restart ? launch_chunk<true, true>(A, s) : launch_chunk<true, false>(A, s))
+										: (restart ? launch_chunk<false, true>(A, s) : launch_chunk<false, false>(A, s));
 			e = cudaGetLastError();
 			if (e == cudaSuccess && launches < 0)
 				e = cudaErrorUnknown;
 			if (e == cudaSuccess)
-				for (int k = 0; k < launches; k++)
-					count_launch();
+				count_launch(launches);
 		}
 		if (e != cudaSuccess) {
 			cuda_fail(domain, e, "jpeg encode kernels launch");
@@ -2026,7 +1935,7 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 		std::vector<unsigned long long> len(n);
 		int bad = 0;
 		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-			cudaMemcpyAsync(&bad, scratch + o_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
+			cudaMemcpyAsync(&bad, scratch + S.bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode");
 			break;
 		}
@@ -2049,135 +1958,16 @@ dev_jpeg_encode_batch(const char *domain, const void *frames, size_t bpl, size_t
 	return rc;
 }
 
-/* dev_jpeg_encode_batch for a progressive stream (interlace): the scan script of jpeg_simple_progression, every scan with
- * its own optimal tables (libjpeg forces optimize_coding on).  11 launches per chunk of frames whatever the frame count,
- * scan count or restart interval: FDCT, summaries, chain walk, tables and headers, bit counts, bit prefix sum, segments,
- * emit, and the three stuffing passes.
- */
 int
-dev_jpeg_encode_progressive(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, int quality,
-	int subsample_mode, int restart, void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
+jpeg_encode_room(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, size_t *stream_bytes, size_t *scratch_bytes)
 {
-	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
+	EncodePlan E;
+	if (make_plan(domain, w, h, bands, o, &E))
 		return -1;
-	ProgScript P;
-	prog_script(G, restart, &P);
-	/* every segment may end with one byte of padding */
-	const size_t scan_bound = (size_t) G.blocks * kProgBlockBytes + (size_t) P.nseg;
-	if (scan_bound >= (size_t) 1 << 29) {
-		error(domain, "frame too large for the device encoder");
-		return -1;
-	}
-	EncodeTables T;
-	make_tables(quality, &T);
-	/* the header template: the frame's markers up to SOF2, then each scan's DRI / SOS */
-	std::vector<unsigned char> tmpl;
-	header_prefix(G, T, tmpl, 0xFFC2);
-	P.prefix_len = (int) tmpl.size();
-	for (int i = 0; i < P.nscans; i++) {
-		P.sfx_at[i] = (int) tmpl.size();
-		prog_scan_suffix(G, P.s[i], i == 0, restart, tmpl);
-	}
-	P.sfx_at[P.nscans] = (int) tmpl.size();
-	const size_t units = (size_t) P.units, nslots = kProgSlotsPerUnit * units + 1;
-	const size_t raw_bytes = ((scan_bound + 3) & ~(size_t) 3) + 4;
-	const int max_chunks = (int) ((raw_bytes + kStuffChunk - 1) / kStuffChunk);
-	/* per-frame counts, tables and header slots (about 26 KB a frame) for one chunk of frames, reused by the next */
-	const size_t nc = (size_t) std::min(n, kMaxBatchFrames);
-	size_t off = 0;
-	auto take = [&](size_t bytes) {
-		const size_t o = off;
-		off += (bytes + 255) & ~(size_t) 255;
-		return o;
-	};
-	const size_t o_tab = take(sizeof(T)), o_tmpl = take(tmpl.size()), o_coef = take((size_t) n * G.blocks * 64 * sizeof(short)),
-				 o_summ = take((size_t) n * units), o_runs = take((size_t) n * kProgSlotsPerUnit * units * sizeof(unsigned)),
-				 o_dslot = take((size_t) n * units * sizeof(unsigned)), o_doff = take((size_t) n * units * sizeof(unsigned short)),
-				 o_bits = take((size_t) n * nslots * sizeof(unsigned)), o_tot = take((size_t) n * sizeof(unsigned long long)),
-				 o_len = take((size_t) n * sizeof(unsigned long long)), o_raw = take((size_t) n * raw_bytes),
-				 o_cnt = take((size_t) n * max_chunks * sizeof(unsigned)), o_ist = take((size_t) n * P.nseg * sizeof(unsigned)),
-				 o_freq = take(nc * kMaxProgTables * 256 * sizeof(unsigned)), o_huff = take(nc * sizeof(ProgHuff)), o_slots = take(nc * kProgHeaderSlot),
-				 o_hat = take(nc * (kMaxProgScans + 1) * sizeof(unsigned)), o_hlen = take(nc * sizeof(unsigned)), o_bad = take(sizeof(int));
-	char *scratch = nullptr;
-	if (dev_alloc(domain, (void **) &scratch, off, s))
-		return -1;
-	int rc = -1;
-	do {
-		if (cudaMemcpyAsync(scratch + o_tab, &T, sizeof(T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-			cudaMemcpyAsync(scratch + o_tmpl, tmpl.data(), tmpl.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-			cudaMemsetAsync(scratch + o_raw, 0, (size_t) n * raw_bytes, s) != cudaSuccess ||
-			cudaMemsetAsync(scratch + o_bad, 0, sizeof(int), s) != cudaSuccess) {
-			cuda_fail(domain, cudaGetLastError(), "jpeg encode setup");
-			break;
-		}
-		const EncodeTables *dT = (const EncodeTables *) (scratch + o_tab);
-		unsigned *freq = (unsigned *) (scratch + o_freq), *hat = (unsigned *) (scratch + o_hat), *hlen = (unsigned *) (scratch + o_hlen);
-		ProgHuff *huff = (ProgHuff *) (scratch + o_huff);
-		unsigned char *slots = (unsigned char *) (scratch + o_slots);
-		unsigned long long *lengths = (unsigned long long *) (scratch + o_len);
-		const int mcus = G.mcus_x * G.mcus_y;
-		cudaError_t e = cudaSuccess;
-		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
-			const int cn = std::min(kMaxBatchFrames, n - c0);
-			const unsigned char *fr = (const unsigned char *) frames + (size_t) c0 * frame_stride;
-			short *coef = (short *) (scratch + o_coef) + (size_t) c0 * G.blocks * 64;
-			unsigned char *summ = (unsigned char *) (scratch + o_summ) + (size_t) c0 * units;
-			unsigned *runs = (unsigned *) (scratch + o_runs) + (size_t) c0 * kProgSlotsPerUnit * units;
-			unsigned *dslot = (unsigned *) (scratch + o_dslot) + (size_t) c0 * units;
-			unsigned short *doff = (unsigned short *) (scratch + o_doff) + (size_t) c0 * units;
-			unsigned *bits = (unsigned *) (scratch + o_bits) + (size_t) c0 * nslots;
-			unsigned long long *totals = (unsigned long long *) (scratch + o_tot) + c0;
-			unsigned char *raw = (unsigned char *) (scratch + o_raw) + (size_t) c0 * raw_bytes;
-			unsigned *counts = (unsigned *) (scratch + o_cnt) + (size_t) c0 * max_chunks;
-			unsigned *ist = (unsigned *) (scratch + o_ist) + (size_t) c0 * P.nseg;
-			unsigned char *dst = (unsigned char *) out + (size_t) c0 * out_stride;
-			const dim3 per_unit((unsigned) ((units + 127) / 128), cn), per_span((max_chunks + 127) / 128, cn);
-			jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, dT, fr, bpl, frame_stride, coef);
-			if ((e = cudaMemsetAsync(freq, 0, (size_t) cn * kMaxProgTables * 256 * sizeof(unsigned), s)) != cudaSuccess)
-				break;
-			jpeg_prog_summary_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, coef, summ, freq);
-			jpeg_prog_walk_kernel<<<dim3((P.nseg + 127) / 128, cn), 128, 0, s>>>(P, summ, runs, dslot, doff, freq);
-			jpeg_prog_huffopt_kernel<<<cn, 32 * kMaxProgTables, 0, s>>>(P, freq, huff, (const unsigned char *) (scratch + o_tmpl), slots, hat, hlen,
-				(int *) (scratch + o_bad));
-			jpeg_prog_count_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, huff, coef, runs, bits);
-			jpeg_bitscan_kernel<<<cn, 1024, 0, s>>>((int) nslots, bits, totals);
-			jpeg_prog_segments_kernel<<<cn, 1024, 0, s>>>(P, bits, totals, ist);
-			jpeg_prog_emit_kernel<<<per_unit, 128, 0, s>>>(G, P, dT, huff, ist, coef, bits, summ, runs, dslot, doff, (unsigned *) raw, raw_bytes / 4);
-			jpeg_prog_ffcount_kernel<<<per_span, 128, 0, s>>>(P, totals, raw, raw_bytes, max_chunks, ist, hat, counts);
-			jpeg_ffscan_kernel<true><<<cn, 1024, 0, s>>>(totals, max_chunks, counts, 0, hlen, lengths + c0);
-			jpeg_prog_stuff_kernel<<<per_span, 128, 0, s>>>(P, totals, raw, raw_bytes, max_chunks, counts, slots, hat, ist, dst, out_stride, lengths + c0);
-			e = cudaGetLastError();
-			if (e == cudaSuccess)
-				count_launch(11);
-		}
-		if (e != cudaSuccess) {
-			cuda_fail(domain, e, "jpeg encode kernels launch");
-			break;
-		}
-		std::vector<unsigned long long> len(n);
-		int bad = 0;
-		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-			cudaMemcpyAsync(&bad, scratch + o_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
-			cuda_fail(domain, cudaGetLastError(), "jpeg encode");
-			break;
-		}
-		if (bad) {
-			error(domain, "optimised Huffman table: a code longer than 32 bits");
-			break;
-		}
-		rc = 0;
-		for (int i = 0; i < n; i++) {
-			if (lengths_host)
-				lengths_host[i] = (size_t) len[i];
-			if (len[i] > out_stride) {
-				error(domain, "frame %d: the stream takes %llu bytes, the output stride is %zu", i, len[i], out_stride);
-				rc = -1;
-			}
-		}
-	} while (0);
-	dev_free(scratch, s);
-	return rc;
+	/* the header slot, the raw data's bound, FF Dn or a scan header (counted in the slot) before each segment, EOI */
+	*stream_bytes = E.slot + E.scan_bound + 2 * (size_t) E.P.nseg + 2;
+	*scratch_bytes = carve(E, 1).bytes;
+	return 0;
 }
 
 /* jpeg_gen_optimal_table on the host (libjpeg's own serial minimum search), for the host twin and its test hook */
@@ -2198,6 +1988,37 @@ host_optimal_table(unsigned *freq, unsigned char *bits, unsigned char *huffval)
 	return gen_optimal_table(freq, codesize, others, bits, huffval, true, pick);
 }
 
+/* a host twin's set-up: the geometry, the tables and the frame's quantised coefficients, MCU by MCU through
+ * jpeg_fdct_kernel's code
+ */
+int
+host_coefficients(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode, int restart,
+	EncodeGeom *G, EncodeTables *T, std::vector<short> &coef)
+{
+	if (make_geom(domain, w, h, bands, quality, subsample_mode, G) || check_restart(domain, restart))
+		return -1;
+	make_tables(quality, T);
+	coef.assign((size_t) G->blocks * 64, 0);
+	for (int my = 0; my < G->mcus_y; my++)
+		for (int mx = 0; mx < G->mcus_x; mx++)
+			encode_mcu(*G, T->q, img, bpl, mx, my, coef.data() + ((size_t) my * G->mcus_x + mx) * G->blocks_per_mcu * 64);
+	return 0;
+}
+
+/* a host twin's optimal table from the symbol counts freq[257] (consumed): bits / huffval for its DHT, and the code /
+ * length per symbol co / si
+ */
+int
+host_table(const char *domain, unsigned *freq, unsigned char *bits, unsigned char *huffval, unsigned *co, unsigned char *si)
+{
+	if (host_optimal_table(freq, bits, huffval)) {
+		error(domain, "optimised Huffman table: a code longer than 32 bits");
+		return -1;
+	}
+	derive_codes(bits + 1, huffval, co, si);
+	return 0;
+}
+
 /* the whole encoder on the CPU through the same per-block code, in the order libjpeg runs it: statistics and table
  * generation when optimising, then the scan with its restart markers (test hook)
  */
@@ -2206,17 +2027,13 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
 	int restart, std::vector<unsigned char> &out)
 {
 	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
-		return -1;
 	EncodeTables T;
-	make_tables(quality, &T);
-	std::vector<short> coef((size_t) G.blocks * 64);
-	for (int my = 0; my < G.mcus_y; my++)
-		for (int mx = 0; mx < G.mcus_x; mx++)
-			encode_mcu(G, T.q, img, bpl, mx, my, coef.data() + ((size_t) my * G.mcus_x + mx) * G.blocks_per_mcu * 64);
+	std::vector<short> coef;
+	if (host_coefficients(domain, img, bpl, w, h, bands, quality, subsample_mode, restart, &G, &T, coef))
+		return -1;
 	const unsigned bpm = (unsigned) G.blocks_per_mcu;
 	unsigned char bits[4][17], huffval[4][256];
-	FrameHuff fh;
+	HuffSet<4> fh;
 	const unsigned (*co)[256] = T.ehufco;
 	const unsigned char (*si)[256] = T.ehufsi;
 	if (optimize) {
@@ -2225,21 +2042,19 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
 			walk_block(
 				T.zz, coef.data() + (size_t) b * 64, block_comp(G, (int) (b % bpm)), previous_dc(G, coef.data(), b, restart),
 				[&](int t, int s) { freq[t * 257 + s]++; }, [](unsigned, int) {});
-		for (int t = 0; t < (G.ncomp == 1 ? 2 : 4); t++) {
-			if (host_optimal_table(freq.data() + t * 257, bits[t], huffval[t])) {
-				error(domain, "optimised Huffman table: a code longer than 32 bits");
+		for (int t = 0; t < (G.ncomp == 1 ? 2 : 4); t++)
+			if (host_table(domain, freq.data() + t * 257, bits[t], huffval[t], fh.ehufco[t], fh.ehufsi[t]))
 				return -1;
-			}
-			derive_codes(bits[t] + 1, huffval[t], fh.ehufco[t], fh.ehufsi[t]);
-		}
 		co = fh.ehufco;
 		si = fh.ehufsi;
 	}
 	else
 		standard_tables(bits, huffval);
+	ScanScript P;
+	scan_script(G, restart, false, &P);
 	header_prefix(G, T, out);
 	put_dhts(G, bits, huffval, out);
-	header_suffix(G, restart, out);
+	scan_suffix(G, P.s[0], true, restart, out);
 	unsigned long long acc = 0;
 	int nacc = 0;
 	auto flush_byte = [&](unsigned char b) {
@@ -2283,7 +2098,7 @@ host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, int w
  * RSTn between intervals, finish_pass_phuff's flush).  Deliberately not the device's decomposition, which it checks.
  */
 void
-host_prog_scan(const EncodeGeom &G, const ProgScan &S, const short *coef, int restart, unsigned (*counts)[257], const unsigned (*co)[256],
+host_prog_scan(const EncodeGeom &G, const Scan &S, const short *coef, int restart, unsigned (*counts)[257], const unsigned (*co)[256],
 	const unsigned char (*si)[256], std::vector<unsigned char> &out, unsigned long long *events)
 {
 	const bool gather = counts != nullptr;
@@ -2495,37 +2310,30 @@ host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_
 	int restart, std::vector<unsigned char> &out, unsigned long long *events)
 {
 	EncodeGeom G;
-	if (make_geom(domain, w, h, bands, quality, subsample_mode, &G) || check_restart(domain, restart))
-		return -1;
 	EncodeTables T;
-	make_tables(quality, &T);
-	std::vector<short> coef((size_t) G.blocks * 64);
-	for (int my = 0; my < G.mcus_y; my++)
-		for (int mx = 0; mx < G.mcus_x; mx++)
-			encode_mcu(G, T.q, img, bpl, mx, my, coef.data() + ((size_t) my * G.mcus_x + mx) * G.blocks_per_mcu * 64);
-	ProgScript P;
-	prog_script(G, restart, &P);
+	std::vector<short> coef;
+	if (host_coefficients(domain, img, bpl, w, h, bands, quality, subsample_mode, restart, &G, &T, coef))
+		return -1;
+	ScanScript P;
+	scan_script(G, restart, true, &P);
 	header_prefix(G, T, out, 0xFFC2);
 	for (int s = 0; s < P.nscans; s++) {
-		const ProgScan &S = P.s[s];
-		FrameHuff fh; /* tables 0, 1 of the scan */
+		const Scan &S = P.s[s];
+		HuffSet<2> fh; /* tables 0, 1 of the scan */
 		if (S.nt) {
 			unsigned counts[2][257];
 			memset(counts, 0, sizeof(counts));
 			host_prog_scan(G, S, coef.data(), restart, counts, nullptr, nullptr, out, events);
 			for (int t = 0; t < S.nt; t++) {
 				unsigned char bits[17], huffval[256];
-				if (host_optimal_table(counts[t], bits, huffval)) {
-					error(domain, "optimised Huffman table: a code longer than 32 bits");
+				if (host_table(domain, counts[t], bits, huffval, fh.ehufco[t], fh.ehufsi[t]))
 					return -1;
-				}
-				derive_codes(bits + 1, huffval, fh.ehufco[t], fh.ehufsi[t]);
 				unsigned char seg[4 + 17 + 256];
 				const int n = put_dht(seg, P.tab_class[S.tab + t], bits, huffval);
 				out.insert(out.end(), seg, seg + n);
 			}
 		}
-		prog_scan_suffix(G, S, s == 0, restart, out);
+		scan_suffix(G, S, s == 0, restart, out);
 		host_prog_scan(G, S, coef.data(), restart, nullptr, fh.ehufco, fh.ehufsi, out, events);
 	}
 	put16(out, 0xFFD9);
@@ -2640,7 +2448,6 @@ vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, s
 		error(domain, "null argument");
 		return -1;
 	}
-	const int Q = opt->Q, subsample_mode = opt->subsample_mode;
 	if (check_restart(domain, opt->restart_interval))
 		return -1;
 	if (ensure_init(domain))
@@ -2678,10 +2485,7 @@ vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, s
 			dst = dout;
 		}
 		std::vector<size_t> len(n);
-		if (opt->interlace ? dev_jpeg_encode_progressive(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->restart_interval,
-								 dst, out_stride, len.data(), s)
-						   : dev_jpeg_encode_batch(domain, src, sbpl, sstride, n, width, height, bands, Q, subsample_mode, opt->optimize_coding != 0,
-								 opt->restart_interval, dst, out_stride, len.data(), s))
+		if (dev_jpeg_encode(domain, src, sbpl, sstride, n, width, height, bands, *opt, dst, out_stride, len.data(), s))
 			break;
 		if (lengths)
 			memcpy(lengths, len.data(), n * sizeof(size_t));

@@ -199,6 +199,11 @@ int host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, i
 	int restart, std::vector<unsigned char> &out);
 int host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
 	int restart, std::vector<unsigned char> &out, unsigned long long *events);
+/* jpeg_encode.cu: the room the device encoder needs for w x h x bands frames with options o: *stream_bytes, a stream's
+ * bound (its header slot, the bound its scan data is sized by, the markers between segments, EOI), and *scratch_bytes,
+ * the device scratch it takes per frame of a batch
+ */
+int jpeg_encode_room(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, size_t *stream_bytes, size_t *scratch_bytes);
 /* min(hshrink, vshrink) of vips_thumbnail_calculate_shrink, thumbnail.c:413-487 */
 double thumbnail_common_shrink(int w, int h, int tw, int th, int size);
 void jpeg_pump_release(); /* the JPEG pump's pinned / device slots (jpeg.cu); vb200_shutdown */
