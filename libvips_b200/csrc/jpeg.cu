@@ -39,6 +39,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <exception>
+#include <future>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -49,12 +50,11 @@
 
 #include "../../include/vb200.h"
 #include "vb200_internal.h"
+#include "jpeg_common.cuh"
 
 namespace vb200 {
 
 namespace {
-
-#define HD __host__ __device__ __forceinline__
 
 constexpr int kMaxComp = 3;
 constexpr int kLook = 9; /* lookahead bits of the fast Huffman table */
@@ -63,32 +63,28 @@ struct JpegComp {
 	int id, h, v, tq, td, ta;
 };
 
-/* one scan of a progressive frame (T.81 G): its components, spectral band and bit position, and the Huffman tables and
- * restart interval in force when its SOS arrived (both may be redefined between scans)
+/* one scan (T.81 G; a sequential frame's is all its components, Ss..Se 0..63): its components, band and bit position, and
+ * the Huffman tables and restart interval in force when its SOS arrived (both may be redefined between scans)
  */
 struct JpegScan {
-	int ns = 0, ci[3] = {0, 0, 0}, td[3] = {0, 0, 0}, ta[3] = {0, 0, 0};
+	int ns = 0, ci[4] = {0, 0, 0, 0}, td[4] = {0, 0, 0, 0}, ta[4] = {0, 0, 0, 0};
 	int Ss = 0, Se = 63, Ah = 0, Al = 0;
 	int restart_interval = 0;
 	size_t off = 0, end = 0;
 	unsigned char hcount[2][4][16];
 	unsigned char hsym[2][4][256];
-	bool hset[2][4];
+	bool hset[2][4] = {{false, false, false, false}, {false, false, false, false}};
 };
 
 struct JpegHeader {
-	std::vector<JpegScan> scans; /* progressive frames only */
+	std::vector<JpegScan> scans;
 	int width = 0, height = 0, ncomp = 0;
 	JpegComp comp[4];
 	bool progressive = false, arithmetic = false;
 	int precision = 8;
 	unsigned short qt[4][64]; /* natural (row-major) order */
 	bool qt_set[4] = {false, false, false, false};
-	unsigned char hcount[2][4][16];
-	unsigned char hsym[2][4][256];
-	bool hset[2][4] = {{false, false, false, false}, {false, false, false, false}};
-	int restart_interval = 0;
-	size_t scan_off = 0, scan_end = 0; /* entropy-coded segment: [scan_off, scan_end) */
+	JpegScan next; /* the Huffman tables and restart interval in force: what the next SOS starts from */
 	int adobe_transform = -1;
 	bool jfif = false;
 	int max_h = 1, max_v = 1;
@@ -111,13 +107,9 @@ struct JpegFrameDev {
 	int h[kMaxComp], v[kMaxComp]; /* sampling factors */
 	int dct[kMaxComp];			  /* scaled DCT size of the component: 1, 2, 4, 8 */
 	int td[kMaxComp], ta[kMaxComp];
-	int restart_interval;		   /* MCUs per interval; 0 = one interval */
-	int n_intervals;
 	size_t data_off;			   /* entropy-coded bytes of the frame in the batch's byte pool */
-	size_t interval_off;		   /* first of n_intervals + 1 offsets (relative to data_off) in the offsets pool */
 	size_t coef_off[kMaxComp];	   /* int16 coefficient planes in the batch's coefficient pool (elements) */
 	int blocks_x[kMaxComp], blocks_y[kMaxComp];
-	int huff_base;				   /* index of this frame's 8 HuffDev (dc 0..3, ac 0..3) */
 	unsigned short qt[kMaxComp][64];
 	int out_w, out_h, tile_w, tile_h; /* cropped output, and the MCU's footprint in output pixels */
 	int blocks_per_mcu;				  /* T.81 A.2.3: component by component, rows of blocks, left to right */
@@ -130,28 +122,27 @@ struct JpegFrameDev {
 	int pw[kMaxComp], ph[kMaxComp];			 /* plane size in samples (whole blocks) */
 	int dw[kMaxComp], dh[kMaxComp];			 /* the component's true size: jdmaster.c downsampled_width / height */
 	size_t plane_off[kMaxComp];				 /* in the chunk's plane pool (bytes) */
-	/* progressive frames: n_scans scan records from scan_base in the chunk's scan pool, decoded in order */
+	/* n_scans scan records from scan_base in the chunk's scan pool, decoded in order: one for a sequential frame */
 	int progressive, n_scans;
 	unsigned scan_base;
 	/* the self-synchronising path (frames with too few restart intervals to fill the machine) */
 	int sync;			 /* 1: decode by subsequences */
 	unsigned clean_len;	 /* bytes of the unstuffed scan (set while staging) */
 	unsigned sync_off;	 /* first of this frame's subsequence records in the chunk's arrays */
-	unsigned sync_cap;	 /* records reserved (from the stuffed length) */
 };
 
-/* one scan of a progressive frame, device layout: offsets are into the chunk's pools */
+/* one scan, device layout: offsets are into the chunk's pools.  A sequential frame's huff_base points at its 8 tables (DC
+ * 0..3, AC 0..3) and its blocks take theirs by the frame's td / ta: dc_tab / ac_tab are set for progressive scans only
+ */
 struct ScanDev {
 	int ns, comp[3], dc_tab[3], ac_tab; /* tables: indices from huff_base */
 	int Ss, Se, Ah, Al;
 	int restart_interval, n_intervals;
 	int units_x, units_y;	 /* MCUs (interleaved scans) or the component's own blocks (one-component scans, T.81 A.2.2) */
 	unsigned interval_off;	 /* first of n_intervals + 1 offsets (relative to the frame's data) */
-	int huff_base;			 /* the scan's four HuffDev */
+	int huff_base;			 /* the scan's HuffDev */
 };
 
-const unsigned char kZigzag[64] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14,
-	21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 __device__ unsigned char d_zigzag[64]; /* global, not __constant__: the lanes of a warp index it divergently */
 
 /* ------------------------------------------------------------------ host: marker parsing (T.81 B.2) */
@@ -160,6 +151,37 @@ inline unsigned
 be16(const unsigned char *p)
 {
 	return ((unsigned) p[0] << 8) | p[1];
+}
+
+/* The next marker from byte p on as libjpeg's next_marker finds it (garbage, fill bytes and standalone markers skipped), with
+ * its payload (*s, *n) and p moved past it; EOI (0xD9) has none.  -1 (error set): the stream ends first or is truncated.
+ */
+int
+next_segment(const char *domain, const unsigned char *d, size_t len, size_t &p, const unsigned char **s, size_t *n)
+{
+	for (;;) {
+		while (p < len && d[p] != 0xFF)
+			p++;
+		while (p < len && d[p] == 0xFF)
+			p++;
+		if (p >= len) {
+			error(domain, "JPEG stream ends before the scan");
+			return -1;
+		}
+		const int m = d[p++];
+		if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01)
+			continue; /* standalone markers */
+		if (m == 0xD9)
+			return m;
+		if (p + 2 > len || be16(d + p) < 2 || p + be16(d + p) > len) {
+			error(domain, "truncated JPEG marker segment");
+			return -1;
+		}
+		*s = d + p + 2;
+		*n = be16(d + p) - 2;
+		p += *n + 2;
+		return m;
+	}
 }
 
 int
@@ -172,35 +194,17 @@ parse_jpeg(const char *domain, const unsigned char *d, size_t len, JpegHeader *H
 	size_t p = 2;
 	bool have_sof = false;
 	for (;;) {
-		/* next marker: any number of fill bytes 0xFF */
-		while (p < len && d[p] != 0xFF)
-			p++;
-		while (p < len && d[p] == 0xFF)
-			p++;
-		if (p >= len) {
-			error(domain, "JPEG stream ends before the scan");
+		const unsigned char *s = nullptr;
+		size_t n = 0;
+		const int m = next_segment(domain, d, len, p, &s, &n);
+		if (m < 0)
 			return -1;
-		}
-		const int m = d[p++];
-		if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01)
-			continue; /* standalone markers */
 		if (m == 0xD9) {
 			if (!H->scans.empty())
 				return 0; /* a progressive frame: all its scans are in */
 			error(domain, "JPEG stream has no scan");
 			return -1;
 		}
-		if (p + 2 > len) {
-			error(domain, "truncated JPEG marker segment");
-			return -1;
-		}
-		const size_t L = be16(d + p);
-		if (L < 2 || p + L > len) {
-			error(domain, "truncated JPEG marker segment");
-			return -1;
-		}
-		const unsigned char *s = d + p + 2;
-		const size_t n = L - 2;
 		switch (m) {
 		case 0xE0:
 			if (n >= 5 && memcmp(s, "JFIF", 5) == 0)
@@ -230,33 +234,29 @@ parse_jpeg(const char *domain, const unsigned char *d, size_t len, JpegHeader *H
 		case 0xC4: { /* DHT */
 			size_t o = 0;
 			while (o < n) {
-				if (o + 17 > n) {
-					error(domain, "malformed DHT");
-					return -1;
-				}
 				const int tc = s[o] >> 4, th = s[o] & 15;
-				if (tc > 1 || th > 3) {
+				if (o + 17 > n || tc > 1 || th > 3) {
 					error(domain, "malformed DHT");
 					return -1;
 				}
 				int total = 0;
 				for (int i = 0; i < 16; i++) {
-					H->hcount[tc][th][i] = s[o + 1 + i];
+					H->next.hcount[tc][th][i] = s[o + 1 + i];
 					total += s[o + 1 + i];
 				}
 				if (total > 256 || o + 17 + total > n) {
 					error(domain, "malformed DHT");
 					return -1;
 				}
-				memcpy(H->hsym[tc][th], s + o + 17, total);
-				H->hset[tc][th] = true;
+				memcpy(H->next.hsym[tc][th], s + o + 17, total);
+				H->next.hset[tc][th] = true;
 				o += 17 + total;
 			}
 			break;
 		}
 		case 0xDD:
 			if (n >= 2)
-				H->restart_interval = be16(s);
+				H->next.restart_interval = be16(s);
 			break;
 		case 0xC0:
 		case 0xC1:
@@ -265,7 +265,7 @@ parse_jpeg(const char *domain, const unsigned char *d, size_t len, JpegHeader *H
 		case 0xCA: {
 			H->progressive = m == 0xC2 || m == 0xCA;
 			H->arithmetic = m == 0xC9 || m == 0xCA;
-			if (n < 6) {
+			if (n < 6 || s[5] < 1 || s[5] > 4 || n < (size_t) 6 + 3 * s[5]) {
 				error(domain, "malformed SOF");
 				return -1;
 			}
@@ -273,10 +273,6 @@ parse_jpeg(const char *domain, const unsigned char *d, size_t len, JpegHeader *H
 			H->height = be16(s + 1);
 			H->width = be16(s + 3);
 			H->ncomp = s[5];
-			if (H->ncomp < 1 || H->ncomp > 4 || n < (size_t) 6 + 3 * H->ncomp) {
-				error(domain, "malformed SOF");
-				return -1;
-			}
 			for (int i = 0; i < H->ncomp; i++) {
 				H->comp[i].id = s[6 + 3 * i];
 				H->comp[i].h = s[7 + 3 * i] >> 4;
@@ -307,95 +303,75 @@ parse_jpeg(const char *domain, const unsigned char *d, size_t len, JpegHeader *H
 				return -1;
 			}
 			const int ns = s[0];
-			if (H->progressive) {
-				/* T.81 G.1: a scan codes a band Ss..Se of one bit position of its components; what follows its header
-				 * runs to the next marker that is neither FF00 nor RSTn
-				 */
-				JpegScan sc;
-				if (ns < 1 || ns > 3 || ns > H->ncomp) {
-					error(domain, "malformed SOS");
+			if (H->progressive && (ns < 1 || ns > 3 || ns > H->ncomp)) {
+				error(domain, "malformed SOS");
+				return -1;
+			}
+			if (!H->progressive && ns != H->ncomp) {
+				error(domain, "non-interleaved scans are not supported on the device path");
+				return -1;
+			}
+			JpegScan sc = H->next;
+			sc.ns = ns;
+			for (int i = 0; i < ns; i++) {
+				int k = -1;
+				for (int j = 0; j < H->ncomp; j++)
+					if (H->comp[j].id == s[1 + 2 * i])
+						k = j;
+				if (k < 0 || (i && k <= sc.ci[i - 1])) {
+					error(domain, "scan components out of frame order");
 					return -1;
 				}
-				sc.ns = ns;
-				for (int i = 0; i < ns; i++) {
-					int k = -1;
-					for (int j = 0; j < H->ncomp; j++)
-						if (H->comp[j].id == s[1 + 2 * i])
-							k = j;
-					if (k < 0 || (i && k <= sc.ci[i - 1])) {
-						error(domain, "scan components out of frame order");
-						return -1;
-					}
-					sc.ci[i] = k;
-					sc.td[i] = s[2 + 2 * i] >> 4;
-					sc.ta[i] = s[2 + 2 * i] & 15;
+				sc.ci[i] = k;
+				sc.td[i] = s[2 + 2 * i] >> 4;
+				sc.ta[i] = s[2 + 2 * i] & 15;
+				if (!H->progressive) {
+					H->comp[k].td = sc.td[i];
+					H->comp[k].ta = sc.ta[i];
 				}
+			}
+			if (H->progressive) {
+				/* T.81 G.1: a scan codes a band Ss..Se of one bit position of its components */
 				sc.Ss = s[1 + 2 * ns];
 				sc.Se = s[2 + 2 * ns];
 				sc.Ah = s[3 + 2 * ns] >> 4;
 				sc.Al = s[3 + 2 * ns] & 15;
-				sc.restart_interval = H->restart_interval;
-				memcpy(sc.hcount, H->hcount, sizeof(sc.hcount));
-				memcpy(sc.hsym, H->hsym, sizeof(sc.hsym));
-				memcpy(sc.hset, H->hset, sizeof(sc.hset));
-				sc.off = p + L;
-				size_t e = sc.off;
-				while (e + 1 < len) {
-					const unsigned char *q = (const unsigned char *) memchr(d + e, 0xFF, len - 1 - e);
-					if (!q) {
-						e = len;
-						break;
-					}
-					e = q - d;
-					const int nx = d[e + 1];
-					if (nx == 0x00 || (nx >= 0xD0 && nx <= 0xD7) || nx == 0xFF) {
-						e += nx == 0xFF ? 1 : 2;
-						continue;
-					}
+			}
+			sc.off = p;
+			/* the segment runs to the next marker that is neither FF00 nor RSTn: for a sequential frame the staging copy (destuff_scan,
+			 * the host's only pass over the scan) finds it; a progressive scan's is found here, the next scan's header follows
+			 */
+			size_t e = H->progressive ? p : len;
+			while (e + 1 < len) {
+				const unsigned char *q = (const unsigned char *) memchr(d + e, 0xFF, len - 1 - e);
+				if (!q) {
+					e = len;
 					break;
 				}
-				if (e + 1 >= len)
-					e = len;
-				sc.end = e;
-				H->scans.push_back(sc);
-				if (H->scans.size() > 256) {
-					error(domain, "too many scans");
-					return -1;
+				e = q - d;
+				const int nx = d[e + 1];
+				if (nx == 0x00 || (nx >= 0xD0 && nx <= 0xD7) || nx == 0xFF) {
+					e += nx == 0xFF ? 1 : 2;
+					continue;
 				}
-				if (e >= len)
-					return 0; /* no EOI: take what is there, as jdinput.c does with a warning */
-				p = e;
-				continue;
+				break;
 			}
-			if (ns != H->ncomp) {
-				error(domain, "non-interleaved scans are not supported on the device path");
+			if (e + 1 >= len)
+				e = len;
+			sc.end = e;
+			H->scans.push_back(sc);
+			if (H->scans.size() > 256) {
+				error(domain, "too many scans");
 				return -1;
 			}
-			for (int i = 0; i < ns; i++) {
-				const int cs = s[1 + 2 * i];
-				int k = -1;
-				for (int j = 0; j < H->ncomp; j++)
-					if (H->comp[j].id == cs)
-						k = j;
-				if (k != i) {
-					error(domain, "scan components out of frame order");
-					return -1;
-				}
-				H->comp[k].td = s[2 + 2 * i] >> 4;
-				H->comp[k].ta = s[2 + 2 * i] & 15;
-			}
-			H->scan_off = p + L;
-			/* the entropy-coded segment runs to the next marker that is neither FF00 nor RSTn (normally EOI): found by
-			 * the staging copy (destuff_scan), the only pass over the scan the host makes
-			 */
-			const size_t e = len;
-			H->scan_end = std::min(e, len);
-			return 0;
+			if (e >= len)
+				return 0; /* a sequential scan, or a progressive frame without EOI: take what is there, as jdinput.c does */
+			p = e;
+			continue;
 		}
 		default:
 			break;
 		}
-		p += L;
 	}
 }
 
@@ -408,6 +384,8 @@ plan_frame(const char *domain, const JpegHeader &H, int shrink, int dct[kMaxComp
 		return -1;
 	}
 	for (const JpegScan &sc : H.scans) {
+		if (!H.progressive)
+			break;
 		/* T.81 G.1.1.1.1: DC scans (Ss = 0) have Se = 0 and may interleave; AC scans have one component */
 		const bool dc = sc.Ss == 0;
 		if (sc.Ss > sc.Se || sc.Se > 63 || (dc && sc.Se != 0) || (!dc && sc.ns != 1) || sc.Al > 13 || (sc.Ah && sc.Ah != sc.Al + 1)) {
@@ -459,7 +437,7 @@ plan_frame(const char *domain, const JpegHeader &H, int shrink, int dct[kMaxComp
 	for (int c = 0; c < H.ncomp; c++) {
 		const JpegComp &k = H.comp[c];
 		if (k.h < 1 || k.v < 1 || k.h > 2 || k.v > 2 || k.tq > 3 || !H.qt_set[k.tq] ||
-			(!H.progressive && (k.td > 3 || k.ta > 3 || !H.hset[0][k.td] || !H.hset[1][k.ta]))) {
+			(!H.progressive && (k.td > 3 || k.ta > 3 || !H.next.hset[0][k.td] || !H.next.hset[1][k.ta]))) {
 			error(domain, "JPEG component %d: unsupported sampling or missing table", c);
 			return -1;
 		}
@@ -483,9 +461,6 @@ plan_frame(const char *domain, const JpegHeader &H, int shrink, int dct[kMaxComp
 	 * factors too large for interleaved scan"): 2x2 in all three components is 12
 	 */
 	int mcu_blocks = 0;
-	if (!H.progressive && H.ncomp > 1)
-		for (int c = 0; c < H.ncomp; c++)
-			mcu_blocks += H.comp[c].h * H.comp[c].v;
 	for (const JpegScan &sc : H.scans)
 		if (sc.ns > 1) {
 			int n = 0;
@@ -662,6 +637,16 @@ mcu_layout(const JpegFrameDev &F, McuLayout &M)
 		M.dc[i] = (unsigned char) F.td[c];
 		M.ac[i] = (unsigned char) (4 + F.ta[c]);
 	}
+}
+
+/* the units (MCUs, or a one-component scan's blocks) [*u0, *u1) of restart interval i of a scan */
+HD void
+scan_interval(const ScanDev &S, int i, int *u0, int *u1)
+{
+	const int total = S.units_x * S.units_y;
+	const int per = S.restart_interval > 0 ? S.restart_interval : total;
+	*u0 = i * per;
+	*u1 = total < *u0 + per ? total : *u0 + per;
 }
 
 /* Decode the MCUs [mcu0, mcu1) of a frame from one restart interval's bytes into the coefficient planes.
@@ -1111,37 +1096,6 @@ dc_block(const McuLayout &M, const int *first, int per, unsigned i, short *coef_
 
 /* ------------------------------------------------------------------ inverse DCTs (jidctint.c, jidctred.c) */
 
-#define FIXC(name, v) constexpr int name = v
-FIXC(F_0_211164243, 1730);
-FIXC(F_0_298631336, 2446);
-FIXC(F_0_390180644, 3196);
-FIXC(F_0_509795579, 4176);
-FIXC(F_0_541196100, 4433);
-FIXC(F_0_601344887, 4926);
-FIXC(F_0_720959822, 5906);
-FIXC(F_0_765366865, 6270);
-FIXC(F_0_850430095, 6967);
-FIXC(F_0_899976223, 7373);
-FIXC(F_1_061594337, 8697);
-FIXC(F_1_175875602, 9633);
-FIXC(F_1_272758580, 10426);
-FIXC(F_1_451774981, 11893);
-FIXC(F_1_501321110, 12299);
-FIXC(F_1_847759065, 15137);
-FIXC(F_1_961570560, 16069);
-FIXC(F_2_053119869, 16819);
-FIXC(F_2_172734803, 17799);
-FIXC(F_2_562915447, 20995);
-FIXC(F_3_072711026, 25172);
-FIXC(F_3_624509785, 29692);
-constexpr int CB = 13, P1 = 2; /* CONST_BITS, PASS1_BITS */
-
-HD int
-descale(int x, int n)
-{
-	return (x + (1 << (n - 1))) >> n;
-}
-
 /* the post-IDCT half of libjpeg's range-limit table (jdmaster.c prepare_range_limit_table): + 128, clamp, and
  * the wrap-around that wild coefficients see (index & 1023)
  */
@@ -1493,8 +1447,8 @@ upsample_pixel(const JpegFrameDev &F, const unsigned char *planes, int x, int y,
 constexpr int kHuffThreads = 32;
 
 __global__ void __launch_bounds__(kHuffThreads)
-jpeg_huffman_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *__restrict__ huff, const unsigned char *__restrict__ bytes,
-	const unsigned *__restrict__ offsets, short *__restrict__ coef, int *__restrict__ status)
+jpeg_huffman_kernel(const JpegFrameDev *__restrict__ frames, const ScanDev *__restrict__ scans, const HuffDev *__restrict__ huff,
+	const unsigned char *__restrict__ bytes, const unsigned *__restrict__ offsets, short *__restrict__ coef, int *__restrict__ status)
 {
 	__shared__ McuLayout M;
 	const JpegFrameDev &F = frames[blockIdx.y];
@@ -1503,15 +1457,14 @@ jpeg_huffman_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *__re
 	if (threadIdx.x == 0)
 		mcu_layout(F, M);
 	__syncthreads();
+	const ScanDev &S = scans[F.scan_base];
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= F.n_intervals)
+	if (i >= S.n_intervals)
 		return;
-	const unsigned *off = offsets + F.interval_off;
-	const unsigned char *base = bytes + F.data_off;
-	const int total = F.mcus_x * F.mcus_y;
-	const int per = F.restart_interval > 0 ? F.restart_interval : total;
-	const int mcu0 = i * per, mcu1 = min(total, mcu0 + per);
-	if (decode_interval(M, huff + F.huff_base, d_zigzag, base, off[i], off[i + 1], mcu0, mcu1, coef))
+	const unsigned *off = offsets + S.interval_off;
+	int mcu0, mcu1;
+	scan_interval(S, i, &mcu0, &mcu1);
+	if (decode_interval(M, huff + S.huff_base, d_zigzag, bytes + F.data_off, off[i], off[i + 1], mcu0, mcu1, coef))
 		atomicOr(status + blockIdx.y, 1);
 }
 
@@ -1528,9 +1481,9 @@ jpeg_progressive_kernel(const JpegFrameDev *__restrict__ frames, const ScanDev *
 	if (i >= S.n_intervals)
 		return;
 	const unsigned *off = offsets + S.interval_off;
-	const int total = S.units_x * S.units_y;
-	const int per = S.restart_interval > 0 ? S.restart_interval : total;
-	if (decode_scan_interval(F, S, huff + S.huff_base, d_zigzag, bytes + F.data_off, off[i], off[i + 1], i * per, min(total, (i + 1) * per), coef))
+	int u0, u1;
+	scan_interval(S, i, &u0, &u1);
+	if (decode_scan_interval(F, S, huff + S.huff_base, d_zigzag, bytes + F.data_off, off[i], off[i + 1], u0, u1, coef))
 		atomicOr(status + blockIdx.y, 1);
 }
 
@@ -1538,9 +1491,9 @@ jpeg_progressive_kernel(const JpegFrameDev *__restrict__ frames, const ScanDev *
 constexpr int kSyncThreads = 64;
 
 __global__ void __launch_bounds__(kSyncThreads)
-jpeg_sync_pass_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *__restrict__ huff, const unsigned char *__restrict__ bytes,
-	int pass, unsigned sub_bytes, const SyncState *__restrict__ Ein, const unsigned *__restrict__ Nin, SyncState *__restrict__ Eout,
-	unsigned *__restrict__ Nout, SyncState *__restrict__ start_used, int *__restrict__ redo)
+jpeg_sync_pass_kernel(const JpegFrameDev *__restrict__ frames, const ScanDev *__restrict__ scans, const HuffDev *__restrict__ huff,
+	const unsigned char *__restrict__ bytes, int pass, unsigned sub_bytes, const SyncState *__restrict__ Ein, const unsigned *__restrict__ Nin,
+	SyncState *__restrict__ Eout, unsigned *__restrict__ Nout, SyncState *__restrict__ start_used, int *__restrict__ redo)
 {
 	__shared__ McuLayout M;
 	const JpegFrameDev &F = frames[blockIdx.y];
@@ -1553,7 +1506,7 @@ jpeg_sync_pass_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *__
 	const unsigned S = (F.clean_len + sub_bytes - 1) / sub_bytes;
 	if (s >= S)
 		return;
-	if (sync_pass(M, huff + F.huff_base, bytes + F.data_off, F.clean_len, sub_bytes, pass, s, Ein + F.sync_off, Nin + F.sync_off,
+	if (sync_pass(M, huff + scans[F.scan_base].huff_base, bytes + F.data_off, F.clean_len, sub_bytes, pass, s, Ein + F.sync_off, Nin + F.sync_off,
 			Eout + F.sync_off, Nout + F.sync_off, start_used + F.sync_off) &&
 		pass > 0)
 		*redo = 1; /* benign race: every writer stores 1 */
@@ -1567,34 +1520,16 @@ jpeg_sync_scan_kernel(const JpegFrameDev *__restrict__ frames, unsigned sub_byte
 	const JpegFrameDev &F = frames[blockIdx.x];
 	if (!F.sync)
 		return;
-	const unsigned S = (F.clean_len + sub_bytes - 1) / sub_bytes;
-	const unsigned per = (S + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min(S, threadIdx.x * per), b = min(S, a + per);
 	const unsigned *n = N + F.sync_off;
-	unsigned sum = 0;
-	for (unsigned i = a; i < b; i++)
-		sum += n[i];
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	/* Hillis-Steele over the 1024 partials */
-	for (unsigned o = 1; o < blockDim.x; o <<= 1) {
-		const unsigned v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned run = s_part[threadIdx.x] - sum; /* exclusive */
 	unsigned *base = Base + F.sync_off;
-	for (unsigned i = a; i < b; i++) {
-		base[i] = run;
-		run += n[i];
-	}
+	cta_exclusive_scan(
+		(F.clean_len + sub_bytes - 1) / sub_bytes, s_part, [&](unsigned i) { return n[i]; }, [&](unsigned i, unsigned run) { base[i] = run; });
 }
 
 __global__ void __launch_bounds__(kSyncThreads)
-jpeg_sync_write_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *__restrict__ huff, const unsigned char *__restrict__ bytes,
-	unsigned sub_bytes, const SyncState *__restrict__ E, const unsigned *__restrict__ Base, const SyncState *__restrict__ start_used,
-	short *__restrict__ coef, int *__restrict__ status)
+jpeg_sync_write_kernel(const JpegFrameDev *__restrict__ frames, const ScanDev *__restrict__ scans, const HuffDev *__restrict__ huff,
+	const unsigned char *__restrict__ bytes, unsigned sub_bytes, const SyncState *__restrict__ E, const unsigned *__restrict__ Base,
+	const SyncState *__restrict__ start_used, short *__restrict__ coef, int *__restrict__ status)
 {
 	__shared__ McuLayout M;
 	const JpegFrameDev &F = frames[blockIdx.y];
@@ -1607,8 +1542,8 @@ jpeg_sync_write_kernel(const JpegFrameDev *__restrict__ frames, const HuffDev *_
 	const unsigned S = (F.clean_len + sub_bytes - 1) / sub_bytes;
 	if (s >= S)
 		return;
-	const int rc = sync_write(M, huff + F.huff_base, d_zigzag, bytes + F.data_off, F.clean_len, sub_bytes, s, S, E + F.sync_off, Base + F.sync_off,
-		start_used + F.sync_off, (unsigned) (F.mcus_x * F.mcus_y * F.blocks_per_mcu), coef);
+	const int rc = sync_write(M, huff + scans[F.scan_base].huff_base, d_zigzag, bytes + F.data_off, F.clean_len, sub_bytes, s, S, E + F.sync_off,
+		Base + F.sync_off, start_used + F.sync_off, (unsigned) (F.mcus_x * F.mcus_y * F.blocks_per_mcu), coef);
 	if (rc)
 		atomicOr(status + blockIdx.y, rc);
 }
@@ -1630,26 +1565,13 @@ jpeg_dc_scan_kernel(const JpegFrameDev *__restrict__ frames, short *__restrict__
 	while (first < M.n && M.comp[first] != c)
 		first++;
 	const int per = F.h[c] * F.v[c];
-	const unsigned total = (unsigned) (F.mcus_x * F.mcus_y * per);
-	const unsigned seg = (total + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min(total, threadIdx.x * seg), b = min(total, a + seg);
-	int sum = 0;
-	for (unsigned i = a; i < b; i++)
-		sum += dc_block(M, &first, per, i, coef)[0];
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	for (unsigned o = 1; o < blockDim.x; o <<= 1) {
-		const int v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	int run = s_part[threadIdx.x] - sum;
-	for (unsigned i = a; i < b; i++) {
-		short *p = dc_block(M, &first, per, i, coef);
-		run += p[0];
-		p[0] = (short) run;
-	}
+	/* put runs after val(i) has read the difference: the value is the inclusive sum */
+	cta_exclusive_scan(
+		(unsigned) (F.mcus_x * F.mcus_y * per), s_part, [&](unsigned i) { return (int) dc_block(M, &first, per, i, coef)[0]; },
+		[&](unsigned i, int run) {
+			short *p = dc_block(M, &first, per, i, coef);
+			p[0] = (short) (run + p[0]);
+		});
 }
 
 /* one thread per MCU */
@@ -1712,22 +1634,28 @@ jpeg_upsample_kernel(const JpegFrameDev *__restrict__ frames, const unsigned cha
 
 /* ------------------------------------------------------------------ host: frame preparation and the pump */
 
+/* one entropy-coded segment: its scan record (offsets relative to the frame's), stuffed bytes, and place in the frame's data */
+struct Segment {
+	ScanDev S;
+	const unsigned char *src;
+	size_t len, at;
+};
+
+/* what a segment of len stuffed bytes takes of the byte pool: at most len clean bytes, 16-byte aligned, and the look-ahead */
+size_t
+staged_size(size_t len)
+{
+	return ((len + 15) & ~(size_t) 15) + 16;
+}
+
 /* one stream, parsed: everything relative to the frame (pool offsets are assigned when a chunk is assembled) */
 struct FramePrep {
 	JpegFrameDev F;
-	HuffDev huff[8];
-	const unsigned char *src = nullptr;
-	size_t src_len = 0, coef_count = 0, plane_bytes = 0;
+	std::vector<Segment> segs; /* one per scan: a sequential frame has one */
+	std::vector<HuffDev> huff; /* a sequential frame's 8 (DC 0..3, AC 0..3), or 4 per scan of a progressive one */
+	size_t coef_count = 0, plane_bytes = 0;
 	int bands = 0;
-	/* progressive frames: one record per scan */
-	struct ScanPrep {
-		ScanDev S;
-		HuffDev huff[4];
-		const unsigned char *src;
-		size_t len;
-	};
-	std::vector<ScanPrep> scans;
-	size_t stage_bytes = 0, stage_ints = 0, stage_huffs = 8; /* what the frame takes of the chunk's pools */
+	size_t stage_bytes = 0, stage_ints = 0; /* what the frame takes of the chunk's byte and offset pools */
 	std::string err;
 };
 
@@ -1736,8 +1664,8 @@ frame_prep(const char *domain, const unsigned char *d, size_t len, int shrink, F
 {
 	JpegHeader H;
 	memset(H.qt, 0, sizeof(H.qt));
-	memset(H.hcount, 0, sizeof(H.hcount));
-	memset(H.hsym, 0, sizeof(H.hsym));
+	memset(H.next.hcount, 0, sizeof(H.next.hcount));
+	memset(H.next.hsym, 0, sizeof(H.next.hsym));
 	if (parse_jpeg(domain, d, len, &H))
 		return -1;
 	if (H.ncomp == 1) {
@@ -1819,79 +1747,64 @@ frame_prep(const char *domain, const unsigned char *d, size_t len, int shrink, F
 				F.blk_dy[F.blocks_per_mcu] = (unsigned char) by;
 				F.blocks_per_mcu++;
 			}
-	memset(P->huff, 0, sizeof(P->huff));
-	for (int tc = 0; tc < 2; tc++)
-		for (int th = 0; th < 4; th++)
-			if (H.hset[tc][th])
-				build_huff(H.hcount[tc][th], H.hsym[tc][th], &P->huff[4 * tc + th]);
-	if (H.progressive) {
-		F.progressive = 1;
-		F.n_scans = (int) H.scans.size();
-		F.n_intervals = 0;
-		P->scans.resize(H.scans.size());
-		P->stage_bytes = P->stage_ints = 0;
-		P->stage_huffs = 4 * H.scans.size();
-		P->src = nullptr;
-		P->src_len = 0;
-		for (size_t j = 0; j < H.scans.size(); j++) {
-			const JpegScan &sc = H.scans[j];
-			FramePrep::ScanPrep &sp = P->scans[j];
-			memset(&sp.S, 0, sizeof(sp.S));
-			memset(sp.huff, 0, sizeof(sp.huff));
-			sp.S.ns = sc.ns;
-			for (int i = 0; i < sc.ns; i++) {
-				sp.S.comp[i] = sc.ci[i];
-				sp.S.dc_tab[i] = i; /* the scan's own tables: slots 0..2 DC per scan component, slot 3 AC */
-				if (sc.Ss == 0 && sc.Ah == 0)
-					build_huff(sc.hcount[0][sc.td[i]], sc.hsym[0][sc.td[i]], &sp.huff[i]);
-			}
-			sp.S.ac_tab = 3;
-			if (sc.Ss > 0)
-				build_huff(sc.hcount[1][sc.ta[0]], sc.hsym[1][sc.ta[0]], &sp.huff[3]);
-			sp.S.Ss = sc.Ss;
-			sp.S.Se = sc.Se;
-			sp.S.Ah = sc.Ah;
-			sp.S.Al = sc.Al;
-			sp.S.restart_interval = sc.restart_interval;
-			if (sc.ns > 1 || H.ncomp == 1) {
-				sp.S.units_x = F.mcus_x;
-				sp.S.units_y = F.mcus_y;
-			}
-			else {
-				/* a one-component scan of a multi-component frame walks the component's own block grid (T.81 A.2.2) */
-				const int c = sc.ci[0];
-				sp.S.units_x = (int) ((((long long) H.width * H.comp[c].h + H.max_h - 1) / H.max_h + 7) / 8);
-				sp.S.units_y = (int) ((((long long) H.height * H.comp[c].v + H.max_v - 1) / H.max_v + 7) / 8);
-			}
-			const int units = sp.S.units_x * sp.S.units_y;
-			sp.S.n_intervals = sc.restart_interval > 0 ? (units + sc.restart_interval - 1) / sc.restart_interval : 1;
-			sp.src = d + sc.off;
-			sp.len = sc.end - sc.off;
-			if (sp.len >= 0xffffff00u || P->stage_bytes >= 0xf0000000u) {
-				error(domain, "entropy-coded segment too large");
-				return -1;
-			}
-			P->stage_bytes += ((sp.len + 15) & ~(size_t) 15) + 16;
-			P->stage_ints += (size_t) sp.S.n_intervals + 1;
+	/* one segment per scan: a sequential frame's with 8 tables, a progressive one's with 4 (0..2 DC per component, 3 AC) */
+	F.progressive = H.progressive ? 1 : 0;
+	for (const JpegScan &sc : H.scans) {
+		Segment g = {};
+		g.S.huff_base = (int) P->huff.size();
+		g.S.ns = sc.ns;
+		for (int i = 0; i < sc.ns; i++)
+			g.S.comp[i] = sc.ci[i];
+		if (!H.progressive) {
+			P->huff.resize(8);
+			for (int tc = 0; tc < 2; tc++)
+				for (int th = 0; th < 4; th++)
+					if (sc.hset[tc][th])
+						build_huff(sc.hcount[tc][th], sc.hsym[tc][th], &P->huff[4 * tc + th]);
 		}
-		return 0;
+		else {
+			P->huff.resize(P->huff.size() + 4);
+			HuffDev *t = &P->huff[g.S.huff_base];
+			for (int i = 0; i < sc.ns; i++) {
+				g.S.dc_tab[i] = i;
+				if (sc.Ss == 0 && sc.Ah == 0)
+					build_huff(sc.hcount[0][sc.td[i]], sc.hsym[0][sc.td[i]], &t[i]);
+			}
+			g.S.ac_tab = 3;
+			if (sc.Ss > 0)
+				build_huff(sc.hcount[1][sc.ta[0]], sc.hsym[1][sc.ta[0]], &t[3]);
+		}
+		g.S.Ss = sc.Ss;
+		g.S.Se = sc.Se;
+		g.S.Ah = sc.Ah;
+		g.S.Al = sc.Al;
+		g.S.restart_interval = sc.restart_interval;
+		if (sc.ns > 1 || H.ncomp == 1) {
+			g.S.units_x = F.mcus_x;
+			g.S.units_y = F.mcus_y;
+		}
+		else {
+			/* a one-component scan of a multi-component frame walks the component's own block grid (T.81 A.2.2) */
+			const int c = sc.ci[0];
+			g.S.units_x = (int) ((((long long) H.width * H.comp[c].h + H.max_h - 1) / H.max_h + 7) / 8);
+			g.S.units_y = (int) ((((long long) H.height * H.comp[c].v + H.max_v - 1) / H.max_v + 7) / 8);
+		}
+		/* restart intervals: the RSTn markers themselves are found (and counted against this) while the segment is staged */
+		const int units = g.S.units_x * g.S.units_y;
+		g.S.n_intervals = sc.restart_interval > 0 ? (units + sc.restart_interval - 1) / sc.restart_interval : 1;
+		g.S.interval_off = (unsigned) P->stage_ints;
+		g.src = d + sc.off;
+		g.len = sc.end - sc.off;
+		g.at = P->stage_bytes;
+		if (g.len >= 0xffffff00u || P->stage_bytes >= 0xf0000000u) {
+			error(domain, "entropy-coded segment too large");
+			return -1;
+		}
+		P->stage_bytes += staged_size(g.len);
+		P->stage_ints += (size_t) g.S.n_intervals + 1;
+		P->segs.push_back(g);
 	}
-	/* restart intervals: RSTn markers are byte-aligned FFD0..FFD7 inside the entropy-coded segment */
-	const int total = F.mcus_x * F.mcus_y;
-	F.restart_interval = H.restart_interval;
-	const size_t seg = H.scan_end - H.scan_off;
-	if (seg >= 0xffffff00u) {
-		error(domain, "entropy-coded segment too large");
-		return -1;
-	}
-	/* the RSTn markers themselves are found (and counted against this) while the scan is staged */
-	const int n_int = H.restart_interval > 0 ? (total + H.restart_interval - 1) / H.restart_interval : 1;
-	F.n_intervals = n_int;
-	P->src = d + H.scan_off;
-	P->src_len = seg;
-	P->stage_bytes = ((seg + 15) & ~(size_t) 15) + 16;
-	P->stage_ints = (size_t) n_int + 1;
-	P->stage_huffs = 8;
+	F.n_scans = (int) P->segs.size();
 	return 0;
 }
 
@@ -1902,7 +1815,7 @@ frame_prep(const char *domain, const unsigned char *d, size_t len, int shrink, F
  * into pinned memory they had to do anyway.
  */
 size_t
-destuff_scan(const unsigned char *src, size_t len, unsigned char *dst, unsigned *offsets, int want, unsigned base = 0)
+destuff_scan(const unsigned char *src, size_t len, unsigned char *dst, unsigned *offsets, int want, unsigned base)
 {
 	size_t p = 0, o = 0;
 	int found = 1;
@@ -1940,6 +1853,23 @@ destuff_scan(const unsigned char *src, size_t len, unsigned char *dst, unsigned 
 		return (size_t) -1;
 	offsets[want] = base + (unsigned) o;
 	return o;
+}
+
+/* Stage one segment: its unstuffed bytes into the frame's data (zero through the look-ahead), its interval offsets into
+ * the frame's offsets and its scan record, with the frame's first offset and table in the chunk's pools added, to *rec.
+ * Returns the clean length, or (size_t) -1 when the restart markers found are not the ones the header promised.
+ */
+size_t
+stage_segment(const Segment &g, unsigned char *data, unsigned *ints, size_t int_base, size_t huff_base, ScanDev *rec)
+{
+	const size_t clean = destuff_scan(g.src, g.len, data + g.at, ints + g.S.interval_off, g.S.n_intervals, (unsigned) g.at);
+	if (clean == (size_t) -1)
+		return clean;
+	memset(data + g.at + clean, 0, staged_size(g.len) - clean);
+	*rec = g.S;
+	rec->interval_off += (unsigned) int_base;
+	rec->huff_base += (int) huff_base;
+	return clean;
 }
 
 /* run fn(i) for i in [0, n) on up to `threads` host threads */
@@ -2002,25 +1932,61 @@ struct JpegSlot {
 	cudaStream_t stream = nullptr;
 	cudaEvent_t done = nullptr;
 	bool busy = false;
+
+	/* the device buffer p of capacity cap, reallocated when it holds less than want bytes */
+	static bool grow(const char *domain, void *&p, size_t &cap, size_t want)
+	{
+		if (cap >= want)
+			return true;
+		if (p)
+			cudaFree(p); /* waits for the device: nothing of this slot is in flight (busy was waited for) */
+		p = nullptr;
+		cap = 0;
+		if (cudaMalloc(&p, want + want / 8) != cudaSuccess) {
+			cuda_fail(domain, cudaGetLastError(), "cudaMalloc (jpeg slot)");
+			return false;
+		}
+		cap = want + want / 8;
+		return true;
+	}
+
+	void release()
+	{
+		if (pinned)
+			cudaFreeHost(pinned);
+		for (void *p : {dev, coef, sync, planes})
+			if (p)
+				cudaFree(p);
+		pinned = dev = coef = sync = planes = nullptr;
+		cap = dev_cap = coef_cap = sync_cap = planes_cap = 0;
+	}
 };
 constexpr int kJpegSlots = 3;
 struct JpegPump {
 	JpegSlot slot[kJpegSlots];
 	cudaEvent_t fork = nullptr;
 	float huff_ms = 0, idct_ms = 0; /* VB200_JPEG_TIMING: the last call's kernel times */
+	std::chrono::steady_clock::time_point t0; /* VB200_JPEG_TIMING=2: when the call's chunks began */
+
+	double ms() const { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
+
+	/* the streams and events on first use; a new call's times */
+	int open(const char *domain)
+	{
+		for (auto &sl : slot)
+			if (!sl.stream) {
+				VB200_CUDA(domain, cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
+				VB200_CUDA(domain, cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
+			}
+		if (!fork)
+			VB200_CUDA(domain, cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+		huff_ms = idct_ms = 0;
+		return 0;
+	}
 	~JpegPump()
 	{
 		for (auto &sl : slot) {
-			if (sl.pinned)
-				cudaFreeHost(sl.pinned);
-			if (sl.dev)
-				cudaFree(sl.dev);
-			if (sl.coef)
-				cudaFree(sl.coef);
-			if (sl.sync)
-				cudaFree(sl.sync);
-			if (sl.planes)
-				cudaFree(sl.planes);
+			sl.release();
 			if (sl.done)
 				cudaEventDestroy(sl.done);
 			if (sl.stream)
@@ -2036,43 +2002,342 @@ struct JpegPump {
 JpegPump g_pump;
 std::mutex g_pump_lock;
 
+/* the decoder's switches, read from the environment once per call */
+struct DecodeOptions {
+	/* the subsequence path: VB200_JPEG_SYNC=0: never (one thread per frame), =N: subsequences of N bytes, any size of scan */
+	unsigned sub_bytes = 2048;
+	size_t sync_min_bytes = 64 * 1024;
+	int sync_passes = 256;	  /* VB200_JPEG_SYNC_PASSES */
+	int chunk = 0;			  /* VB200_JPEG_CHUNK: frames per chunk; 0 = chosen from the batch */
+	long long cta_slots = 0;  /* VB200_JPEG_CTAS: resident Huffman CTAs; 0 = 32 per SM */
+	char timing = 0;		  /* VB200_JPEG_TIMING: '1' = CUDA-event kernel times, '2' = host-side milestones on stderr */
+};
+
+DecodeOptions
+decode_options()
+{
+	DecodeOptions o;
+	if (const char *e = getenv("VB200_JPEG_SYNC")) {
+		o.sub_bytes = (unsigned) std::max(0, atoi(e));
+		o.sync_min_bytes = 0;
+	}
+	if (const char *e = getenv("VB200_JPEG_SYNC_PASSES"))
+		o.sync_passes = std::max(1, atoi(e));
+	if (const char *e = getenv("VB200_JPEG_CHUNK"))
+		o.chunk = std::max(0, atoi(e));
+	if (const char *e = getenv("VB200_JPEG_CTAS"))
+		o.cta_slots = std::max(0LL, atoll(e));
+	if (const char *e = getenv("VB200_JPEG_TIMING"))
+		o.timing = e[0];
+	return o;
+}
+
+/* one chunk: its frame records placed in its pools, each frame's first interval offset and table, the pinned block (frame
+ * records, then tables, scan records, offsets, bytes; total bytes), the device pools' sizes and the launches' extents
+ */
+struct ChunkLayout {
+	int c0 = 0, cn = 0;
+	std::vector<JpegFrameDev> F;
+	std::vector<size_t> ints, huffs;
+	size_t off_h = 0, off_s = 0, off_o = 0, off_b = 0, total = 0;
+	size_t coef_total = 0, plane_total = 0, sync_total = 0;
+	int max_intervals = 0, max_mcus = 0, max_blocks = 0, max_scans = 0, max_scan_intervals = 0;
+	unsigned max_subs = 0;
+	std::string err; /* staging failed */
+};
+
+/* Lay out frames c0 .. c0 + cn - 1 as chunk k, wait for its slot and stage them into its pinned block on the host workers.
+ * Runs on a helper thread for chunk k + 1 while the calling thread queues (and, on the subsequence path, waits on) chunk k.
+ */
+ChunkLayout
+stage_chunk(const std::vector<FramePrep> &prep, int k, int c0, int cn, JpegPump &P, const DecodeOptions &o)
+{
+	ChunkLayout L{c0, cn};
+	size_t n_bytes = 0, n_ints = 0, n_huffs = 0, n_scans = 0;
+	/* the next n units of a pool; the parts of the pinned block are 16-byte aligned */
+	auto take = [](size_t &pool, size_t n, size_t align = 1) {
+		const size_t o = pool;
+		pool += (n + align - 1) / align * align;
+		return o;
+	};
+	for (int i = 0; i < cn; i++) {
+		const FramePrep &fp = prep[c0 + i];
+		JpegFrameDev F = fp.F;
+		F.data_off = take(n_bytes, fp.stage_bytes);
+		F.scan_base = (unsigned) take(n_scans, fp.segs.size());
+		for (int c = 0; c < F.ncomp; c++) {
+			F.coef_off[c] += L.coef_total;
+			F.plane_off[c] += L.plane_total;
+		}
+		L.coef_total += fp.coef_count;
+		L.plane_total += fp.plane_bytes;
+		L.ints.push_back(take(n_ints, fp.stage_ints));
+		L.huffs.push_back(take(n_huffs, fp.huff.size()));
+		if (F.sync) {
+			const unsigned cap = (unsigned) ((fp.segs[0].len + o.sub_bytes - 1) / o.sub_bytes + 1);
+			F.sync_off = (unsigned) take(L.sync_total, cap);
+			L.max_subs = std::max(L.max_subs, cap);
+		}
+		L.max_mcus = std::max(L.max_mcus, F.mcus_x * F.mcus_y);
+		if (F.planar)
+			L.max_blocks = std::max(L.max_blocks, F.mcus_x * F.mcus_y * F.blocks_per_mcu);
+		if (F.progressive) {
+			L.max_scans = std::max(L.max_scans, F.n_scans);
+			for (const Segment &g : fp.segs)
+				L.max_scan_intervals = std::max(L.max_scan_intervals, g.S.n_intervals);
+		}
+		else
+			L.max_intervals = std::max(L.max_intervals, fp.segs[0].S.n_intervals);
+		L.F.push_back(F);
+	}
+	size_t off = 0;
+	take(off, (size_t) cn * sizeof(JpegFrameDev), 16);
+	L.off_h = take(off, n_huffs * sizeof(HuffDev), 16);
+	L.off_s = take(off, n_scans * sizeof(ScanDev), 16);
+	L.off_o = take(off, n_ints * sizeof(unsigned), 16);
+	L.off_b = take(off, n_bytes, 16);
+	L.total = off + 16; /* the last reader's look-ahead */
+	JpegSlot &sl = P.slot[k % kJpegSlots];
+	if (o.timing == '2')
+		fprintf(stderr, "[jpeg] chunk %d begins at %.2f ms\n", k, P.ms());
+	if (sl.busy) {
+		if (cudaEventSynchronize(sl.done) != cudaSuccess) {
+			L.err = std::string("jpeg decode: ") + cudaGetErrorString(cudaGetLastError());
+			return L;
+		}
+		sl.busy = false;
+	}
+	if (sl.cap < L.total) {
+		if (sl.pinned)
+			cudaFreeHost(sl.pinned);
+		sl.pinned = nullptr;
+		sl.cap = 0;
+		const size_t want = L.total + L.total / 4;
+		if (cudaMallocHost(&sl.pinned, want) != cudaSuccess) {
+			L.err = std::string("cudaMallocHost (jpeg staging): ") + cudaGetErrorString(cudaGetLastError());
+			return L;
+		}
+		sl.cap = want;
+	}
+	if (o.timing == '2')
+		fprintf(stderr, "[jpeg] chunk %d slot free at %.2f ms\n", k, P.ms());
+	char *hst = (char *) sl.pinned;
+	HuffDev *huffs = (HuffDev *) (hst + L.off_h);
+	ScanDev *scans = (ScanDev *) (hst + L.off_s);
+	unsigned *ints = (unsigned *) (hst + L.off_o);
+	unsigned char *bytes = (unsigned char *) hst + L.off_b;
+	std::atomic<int> bad_frame(-1);
+	parallel_for(cn, host_workers(), [&](int i) {
+		const FramePrep &fp = prep[c0 + i];
+		JpegFrameDev &F = L.F[i];
+		for (size_t j = 0; j < fp.segs.size(); j++) {
+			const size_t clean = stage_segment(fp.segs[j], bytes + F.data_off, ints + L.ints[i], L.ints[i], L.huffs[i], scans + F.scan_base + j);
+			if (clean == (size_t) -1) {
+				int none = -1;
+				bad_frame.compare_exchange_strong(none, c0 + i);
+				return;
+			}
+			F.clean_len = (unsigned) clean; /* read by the subsequence path, whose frames have one segment */
+		}
+		((JpegFrameDev *) hst)[i] = F;
+		memcpy(huffs + L.huffs[i], fp.huff.data(), fp.huff.size() * sizeof(HuffDev));
+	});
+	if (bad_frame.load() >= 0) {
+		L.err = "frame " + std::to_string(bad_frame.load()) + ": restart markers do not match the restart interval";
+		return L;
+	}
+	if (o.timing == '2')
+		fprintf(stderr, "[jpeg] chunk %d (%d frames) staged at %.2f ms\n", k, cn, P.ms());
+	return L;
+}
+
+/* Frames per chunk.  Frames with many restart intervals fill the machine with few frames; a stream decoded by one thread
+ * per frame wants everything up at once.  Bounded by the coefficient pool (128 bytes per block).
+ */
+int
+chunk_frames(const std::vector<FramePrep> &prep, const DecodeOptions &o)
+{
+	int max_int = 1;
+	size_t max_coef = 0;
+	bool one_thread_frames = false;
+	for (const FramePrep &fp : prep) {
+		const int intervals = fp.F.progressive ? 0 : fp.segs[0].S.n_intervals;
+		max_int = std::max(max_int, intervals);
+		max_coef = std::max(max_coef, fp.coef_count);
+		one_thread_frames |= intervals == 1 && !fp.F.sync;
+	}
+	size_t free_b = 0, total_b = 0;
+	cudaMemGetInfo(&free_b, &total_b);
+	/* the slots keep their pools: an eighth of the device per chunk, three chunks in flight */
+	const size_t coef_budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
+	/* more intervals in flight decode faster per frame (the kernel is latency-bound per thread), more chunks overlap
+	 * staging and copies better: a quarter of the batch, between 64 and 256 frames
+	 */
+	const int n = (int) prep.size();
+	int chunk = o.chunk > 0 ? o.chunk : (max_int >= 32 || !one_thread_frames) ? std::max(64, std::min(256, (n + 3) / 4)) : n;
+	chunk = (int) std::max<size_t>(1, std::min<size_t>(chunk, coef_budget / std::max<size_t>(1, max_coef * sizeof(short))));
+	chunk = std::min(chunk, n);
+	return std::min(chunk, kMaxBatchFrames); /* the frames of a chunk are gridDim.y / z of its kernels */
+}
+
+/* per subsequence: two (state, count) records, the start state last decoded from, the first block's index */
+constexpr size_t kSyncRecordBytes = 3 * sizeof(SyncState) + 3 * sizeof(unsigned);
+
+/* Queue a staged chunk on its slot's stream: the subsequence passes, prefix sum, write and DC passes; the progressive scans;
+ * the Huffman kernel; the IDCT; the planar pair.  ev (timing) marks the entropy decode's start and end and the chunk's end.
+ * Returns the launch count, or -1 (error set, launches counted) when the flags of a group of passes could not be read.
+ */
+int
+launch_chunk(const char *domain, const ChunkLayout &L, const JpegSlot &sl, const DecodeOptions &o, int *status, unsigned char *out, size_t out_bpl,
+	size_t out_frame_stride, int out_w, int out_h, cudaEvent_t *ev)
+{
+	const cudaStream_t st = sl.stream;
+	const char *dev = (const char *) sl.dev;
+	const JpegFrameDev *dF = (const JpegFrameDev *) dev;
+	const HuffDev *dH = (const HuffDev *) (dev + L.off_h);
+	const ScanDev *dS = (const ScanDev *) (dev + L.off_s);
+	const unsigned *dO = (const unsigned *) (dev + L.off_o);
+	const unsigned char *dB = (const unsigned char *) dev + L.off_b;
+	short *coef = (short *) sl.coef;
+	status += L.c0;
+	out += (size_t) L.c0 * out_frame_stride;
+	int launches = 0;
+	if (ev)
+		cudaEventRecord(ev[0], st);
+	if (L.sync_total) {
+		const size_t n = L.sync_total;
+		SyncState *Ea = (SyncState *) sl.sync, *Eb = Ea + n, *Su = Eb + n;
+		unsigned *Na = (unsigned *) (Su + n), *Nb = Na + n, *Bs = Nb + n;
+		int *redo = (int *) (Bs + n);
+		const dim3 sg((L.max_subs + kSyncThreads - 1) / kSyncThreads, L.cn);
+		/* passes until one in which no subsequence had to decode again: groups of four, each pass with its own flag word
+		 * (after the records), read back after the group -- this chunk's stream waits, the others run on
+		 */
+		int pass = 0;
+		bool settled = false;
+		while (!settled && pass < o.sync_passes) {
+			int flags[4] = {1, 1, 1, 1};
+			cudaMemsetAsync(redo, 0, sizeof(flags), st);
+			int g = 0;
+			for (; g < 4 && pass < o.sync_passes; g++, pass++) {
+				jpeg_sync_pass_kernel<<<sg, kSyncThreads, 0, st>>>(dF, dS, dH, dB, pass, o.sub_bytes, Ea, Na, Eb, Nb, Su, redo + g);
+				std::swap(Ea, Eb);
+				std::swap(Na, Nb);
+				launches++;
+			}
+			if (cudaMemcpyAsync(flags, redo, sizeof(flags), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+				count_launch(launches);
+				return cuda_fail(domain, cudaGetLastError(), "jpeg_sync_pass_kernel");
+			}
+			for (int j = pass - g == 0 ? 1 : 0; j < g; j++)
+				if (flags[j] == 0)
+					settled = true; /* later passes of the group only copied */
+		}
+		/* not settled: the write pass finds the inconsistency and fails the frame */
+		jpeg_sync_scan_kernel<<<L.cn, 1024, 0, st>>>(dF, o.sub_bytes, Na, Bs);
+		jpeg_sync_write_kernel<<<sg, kSyncThreads, 0, st>>>(dF, dS, dH, dB, o.sub_bytes, Ea, Bs, Su, coef, status);
+		jpeg_dc_scan_kernel<<<dim3(kMaxComp, L.cn), 1024, 0, st>>>(dF, coef);
+		launches += 3;
+	}
+	/* progressive frames: their scans in order, scan j of every frame in one launch */
+	for (int j = 0; j < L.max_scans; j++) {
+		jpeg_progressive_kernel<<<dim3((L.max_scan_intervals + kHuffThreads - 1) / kHuffThreads, L.cn), kHuffThreads, 0, st>>>(dF, dS, dH, dB, dO,
+			coef, status, j);
+		launches++;
+	}
+	/* CTA width: one interval per warp while the chunk has fewer intervals than the machine has CTA slots */
+	const long long cta_slots = o.cta_slots > 0 ? o.cta_slots : (long long) sm_count() * 32;
+	int ht = 1;
+	while (ht < kHuffThreads && (long long) L.cn * ((L.max_intervals + ht - 1) / ht) > cta_slots)
+		ht *= 2;
+	if (L.max_intervals > 0) /* a chunk of progressive frames only has no sequential interval */
+		jpeg_huffman_kernel<<<dim3((L.max_intervals + ht - 1) / ht, L.cn), ht, 0, st>>>(dF, dS, dH, dB, dO, coef, status);
+	launches++;
+	if (ev)
+		cudaEventRecord(ev[1], st);
+	jpeg_idct_kernel<<<dim3((L.max_mcus + 127) / 128, L.cn), 128, 0, st>>>(dF, coef, out, out_bpl, out_frame_stride);
+	launches++;
+	if (L.plane_total) {
+		jpeg_idct_planes_kernel<<<dim3((L.max_blocks + 127) / 128, L.cn), 128, 0, st>>>(dF, coef, (unsigned char *) sl.planes);
+		jpeg_upsample_kernel<<<dim3((out_w + 31) / 32, (out_h + 7) / 8, L.cn), 256, 0, st>>>(dF, (const unsigned char *) sl.planes, out, out_bpl,
+			out_frame_stride);
+		launches += 2;
+	}
+	if (ev)
+		cudaEventRecord(ev[2], st);
+	return launches;
+}
+
+/* the device's subsequence decode of a staged frame on the CPU, one "thread" after another; *passes_used = the last pass
+ * that changed a record
+ */
+int
+host_sync_decode(const char *domain, const JpegFrameDev &F, const McuLayout &M, const HuffDev *huff, const unsigned char *bytes, unsigned clean,
+	unsigned sub_bytes, int max_passes, int *passes_used, short *coef)
+{
+	const unsigned S = (clean + sub_bytes - 1) / sub_bytes;
+	std::vector<SyncState> Ea(S + 1), Eb(S + 1), Su(S + 1);
+	std::vector<unsigned> Na(S + 1, 0), Nb(S + 1, 0), Bs(S + 1, 0);
+	int used = 0;
+	for (int pass = 0; pass < max_passes; pass++) {
+		bool redo = false;
+		for (unsigned sx = 0; sx < S; sx++)
+			redo |= sync_pass(M, huff, bytes, clean, sub_bytes, pass, sx, Ea.data(), Na.data(), Eb.data(), Nb.data(), Su.data());
+		Ea.swap(Eb);
+		Na.swap(Nb);
+		if (pass > 0 && !redo)
+			break;
+		used = pass + 1;
+	}
+	if (passes_used)
+		*passes_used = used;
+	unsigned run = 0;
+	for (unsigned sx = 0; sx < S; sx++) {
+		Bs[sx] = run;
+		run += Na[sx];
+	}
+	const unsigned total = (unsigned) (F.mcus_x * F.mcus_y);
+	int bad = 0;
+	for (unsigned sx = 0; sx < S; sx++)
+		bad |= sync_write(M, huff, kZigzag, bytes, clean, sub_bytes, sx, S, Ea.data(), Bs.data(), Su.data(), total * F.blocks_per_mcu, coef);
+	if (bad) {
+		error(domain, (bad & 1) ? "corrupt JPEG data: bad Huffman code" : "the subsequence decode did not converge");
+		return -1;
+	}
+	for (int c = 0; c < F.ncomp; c++) {
+		int first = 0;
+		while (first < M.n && M.comp[first] != c)
+			first++;
+		const int pc = F.h[c] * F.v[c];
+		int runv = 0;
+		for (unsigned i = 0; i < total * pc; i++) {
+			short *p = dc_block(M, &first, pc, i, coef);
+			runv += p[0];
+			p[0] = (short) runv;
+		}
+	}
+	return 0;
+}
+
 } // namespace
 
 void
 jpeg_pump_release()
 {
 	std::lock_guard<std::mutex> lock(g_pump_lock);
-	for (auto &sl : g_pump.slot) {
-		if (sl.pinned)
-			cudaFreeHost(sl.pinned);
-		if (sl.dev)
-			cudaFree(sl.dev);
-		if (sl.coef)
-			cudaFree(sl.coef);
-		if (sl.sync)
-			cudaFree(sl.sync);
-		if (sl.planes)
-			cudaFree(sl.planes);
-		sl.pinned = sl.dev = sl.coef = sl.sync = sl.planes = nullptr;
-		sl.cap = sl.dev_cap = sl.coef_cap = sl.sync_cap = sl.planes_cap = 0;
-	}
-}
-
-static void
-jpeg_last_kernel_times(float *huff_ms, float *idct_ms)
-{
-	*huff_ms = g_pump.huff_ms;
-	*idct_ms = g_pump.idct_ms;
+	for (auto &sl : g_pump.slot)
+		sl.release();
 }
 
 /* Decode n JPEG streams (host memory) that share one output geometry into out[n][out_h][out_w][bands] on the
  * device (out = nullptr: only report the geometry).
  *
  * The pump: headers are parsed and restart markers located on the host workers; the frames go up in chunks, each
- * chunk = one pinned staging block (frame records, Huffman tables, interval offsets, compressed bytes) copied to the
- * device and decoded on one of three internal streams, so that staging chunk k + 1 overlaps copy and kernels of
- * chunk k (and the Huffman kernels of consecutive chunks share the machine).  The internal streams start after everything queued on s and s continues after them; the call returns when
- * the frames are decoded (a corrupt stream is an error, as jpeg2vips.c makes it one by default).
+ * chunk = one pinned staging block (frame records, Huffman tables, scan records, interval offsets, compressed bytes) copied
+ * to the device and decoded on one of three internal streams, so that staging chunk k + 1 overlaps copy and kernels of
+ * chunk k (and the Huffman kernels of consecutive chunks share the machine).  The internal streams start after everything
+ * queued on s and s continues after them; the call returns when the frames are decoded (a corrupt stream is an error, as
+ * jpeg2vips.c makes it one by default).
  */
 int
 dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
@@ -2082,13 +2347,16 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 		error(domain, "no frames");
 		return -1;
 	}
+	const DecodeOptions o = decode_options();
 	std::vector<FramePrep> prep(n);
-	std::atomic<int> failed(-1);
 	parallel_for(n, host_workers(), [&](int i) {
-		if (frame_prep(domain, (const unsigned char *) bufs[i], lens[i], shrink, &prep[i])) {
+		if (frame_prep(domain, (const unsigned char *) bufs[i], lens[i], shrink, &prep[i]))
 			prep[i].err = vb200_error_buffer(); /* the worker's thread-local text */
-			int none = -1;
-			failed.compare_exchange_strong(none, i);
+		else {
+			/* frames with one restart interval (no DRI) and a scan worth splitting decode by self-synchronising subsequences */
+			const Segment &g = prep[i].segs[0];
+			prep[i].F.sync =
+				!prep[i].F.progressive && g.S.n_intervals == 1 && o.sub_bytes > 0 && g.len >= o.sync_min_bytes && g.len / o.sub_bytes >= 8;
 		}
 	});
 	for (int i = 0; i < n; i++)
@@ -2096,7 +2364,7 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 			error(domain, "frame %d: %s", i, prep[i].err.c_str());
 			return -1;
 		}
-	if (getenv("VB200_JPEG_TIMING") && getenv("VB200_JPEG_TIMING")[0] == '2')
+	if (o.timing == '2')
 		fprintf(stderr, "[jpeg] %d headers parsed\n", n);
 	const int W = prep[0].F.out_w, Hh = prep[0].F.out_h, B = prep[0].bands;
 	for (int i = 1; i < n; i++)
@@ -2122,429 +2390,82 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 
 	std::lock_guard<std::mutex> pump_lock(g_pump_lock);
 	JpegPump &P = g_pump;
-	for (auto &sl : P.slot)
-		if (!sl.stream) {
-			VB200_CUDA(domain, cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
-			VB200_CUDA(domain, cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-		}
-	if (!P.fork)
-		VB200_CUDA(domain, cudaEventCreateWithFlags(&P.fork, cudaEventDisableTiming));
-	const bool timing = getenv("VB200_JPEG_TIMING") && getenv("VB200_JPEG_TIMING")[0] == '1'; /* 2 = host-side trace only */
-	P.huff_ms = P.idct_ms = 0;
+	if (P.open(domain))
+		return -1;
 
-	/* chunks: frames with many restart intervals fill the machine with few frames; a stream without them is one
-	 * thread per frame, so everything goes up at once.  Bounded by the coefficient pool (128 bytes per block).
-	 */
-	int max_int = 1;
-	size_t max_coef = 0;
-	for (int i = 0; i < n; i++) {
-		max_int = std::max(max_int, prep[i].F.n_intervals);
-		max_coef = std::max(max_coef, prep[i].coef_count);
-	}
-	size_t free_b = 0, total_b = 0;
-	cudaMemGetInfo(&free_b, &total_b);
-	/* the slots keep their pools: an eighth of the device per chunk, three chunks in flight */
-	const size_t coef_budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
-	/* frames with one restart interval (no DRI) and a scan worth splitting decode by self-synchronising subsequences;
-	 * VB200_JPEG_SYNC=0: never (one thread per frame), =N: subsequences of N bytes, any size of scan
-	 */
-	unsigned sub_bytes = 2048;
-	size_t sync_min_bytes = 64 * 1024;
-	if (const char *e = getenv("VB200_JPEG_SYNC")) {
-		sub_bytes = (unsigned) std::max(0, atoi(e));
-		sync_min_bytes = 0;
-	}
-	int sync_passes = 256;
-	if (const char *e = getenv("VB200_JPEG_SYNC_PASSES"))
-		sync_passes = std::max(1, atoi(e));
-	/* more intervals in flight decode faster per frame (the kernel is latency-bound per thread), more chunks overlap
-	 * staging and copies better: a quarter of the batch, between 64 and 256 frames
-	 */
-	bool any_plain_single = false;
-	for (int i = 0; i < n; i++)
-		if (!prep[i].F.progressive && prep[i].F.n_intervals == 1 &&
-			!(sub_bytes > 0 && prep[i].src_len >= sync_min_bytes && prep[i].src_len / sub_bytes >= 8))
-			any_plain_single = true;
-	int chunk = (max_int >= 32 || !any_plain_single) ? std::max(64, std::min(256, (n + 3) / 4)) : n;
-	if (const char *e = getenv("VB200_JPEG_CHUNK"))
-		if (atoi(e) > 0)
-			chunk = atoi(e);
-	long long huff_cta_slots = (long long) sm_count() * 32; /* resident CTAs: 32 per SM */
-	if (const char *e = getenv("VB200_JPEG_CTAS"))
-		if (atoll(e) > 0)
-			huff_cta_slots = atoll(e);
-	const bool trace = getenv("VB200_JPEG_TIMING") && getenv("VB200_JPEG_TIMING")[0] == '2';
-	const auto t_start = std::chrono::steady_clock::now();
-	auto since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count(); };
-	chunk = (int) std::max<size_t>(1, std::min<size_t>(chunk, coef_budget / std::max<size_t>(1, max_coef * sizeof(short))));
-	chunk = std::min(chunk, n);
-	chunk = std::min(chunk, kMaxBatchFrames); /* the frames of a chunk are gridDim.y / z of its kernels */
-
-	std::atomic<int> bad_frame(-1);
+	const int chunk = chunk_frames(prep, o);
+	P.t0 = std::chrono::steady_clock::now();
 	int *status = nullptr;
 	if (dev_alloc(domain, (void **) &status, (size_t) n * sizeof(int), s))
 		return -1;
 	int rc = 0;
 	if (cudaMemsetAsync(status, 0, (size_t) n * sizeof(int), s) != cudaSuccess || cudaEventRecord(P.fork, s) != cudaSuccess)
 		rc = cuda_fail(domain, cudaGetLastError(), "jpeg decode setup");
-	/* staging of a chunk: layout, the slot's pinned block, the unstuffing copies.  Runs on a helper thread for chunk
-	 * k + 1 while the calling thread queues (and, on the subsequence path, waits on) chunk k.
-	 */
-	struct Staged {
-		int rc = 0, c0 = 0, cn = 0, max_intervals = 0, max_mcus = 0;
-		unsigned max_subs = 0;
-		size_t total = 0, off_h = 0, off_o = 0, off_b = 0, coef_total = 0, sync_total = 0, plane_total = 0;
-		int max_blocks = 0, max_scans = 0, max_scan_intervals = 0;
-		size_t off_s = 0;
-		std::string err;
-	};
 	int device = 0;
 	cudaGetDevice(&device);
-	auto stage_chunk = [&](int k, bool helper) {
-		Staged R;
-		if (helper)
-			cudaSetDevice(device);
-		const int c0 = k * chunk;
-		const int cn = std::min(chunk, n - c0);
-		JpegSlot &sl = P.slot[k % kJpegSlots];
-		R.c0 = c0;
-		R.cn = cn;
-		/* layout of the chunk's block */
-		std::vector<size_t> data_off(cn), int_off(cn), coef_off(cn);
-		std::vector<unsigned> sync_off(cn, 0), sync_cap(cn, 0);
-		std::vector<size_t> plane_off(cn, 0), huff_off(cn, 0), scan_off(cn, 0);
-		size_t bytes_total = 0, ints_total = 0, coef_total = 0, sync_total = 0, plane_total = 0, huffs_total = 0, scans_total = 0;
-		int max_scans = 0, max_scan_intervals = 0;
-		int max_blocks = 0;
-		int max_intervals = 0, max_mcus = 0;
-		unsigned max_subs = 0;
-		for (int i = 0; i < cn; i++) {
-			const FramePrep &fp = prep[c0 + i];
-			data_off[i] = bytes_total;
-			bytes_total += fp.stage_bytes;
-			int_off[i] = ints_total;
-			ints_total += fp.stage_ints;
-			huff_off[i] = huffs_total;
-			huffs_total += fp.stage_huffs;
-			scan_off[i] = scans_total;
-			scans_total += fp.scans.size();
-			max_scans = std::max(max_scans, (int) fp.scans.size());
-			for (const auto &sp : fp.scans)
-				max_scan_intervals = std::max(max_scan_intervals, sp.S.n_intervals);
-			coef_off[i] = coef_total;
-			coef_total += fp.coef_count;
-			max_intervals = std::max(max_intervals, fp.F.n_intervals);
-			max_mcus = std::max(max_mcus, fp.F.mcus_x * fp.F.mcus_y);
-			plane_off[i] = plane_total;
-			plane_total += fp.plane_bytes;
-			if (fp.F.planar)
-				max_blocks = std::max(max_blocks, fp.F.mcus_x * fp.F.mcus_y * fp.F.blocks_per_mcu);
-			if (!fp.F.progressive && fp.F.n_intervals == 1 && sub_bytes > 0 && fp.src_len >= sync_min_bytes && fp.src_len / sub_bytes >= 8) {
-				sync_off[i] = (unsigned) sync_total;
-				sync_cap[i] = (unsigned) ((fp.src_len + sub_bytes - 1) / sub_bytes + 1);
-				sync_total += sync_cap[i];
-				max_subs = std::max(max_subs, sync_cap[i]);
-			}
-		}
-		const size_t sz_f = (size_t) cn * sizeof(JpegFrameDev), sz_h = huffs_total * sizeof(HuffDev), sz_s = scans_total * sizeof(ScanDev);
-		const size_t off_h = (sz_f + 15) & ~(size_t) 15, off_s = off_h + ((sz_h + 15) & ~(size_t) 15);
-		const size_t off_o = off_s + ((sz_s + 15) & ~(size_t) 15);
-		const size_t off_b = off_o + ((ints_total * sizeof(unsigned) + 15) & ~(size_t) 15);
-		const size_t total = off_b + bytes_total + 16;
-		if (trace)
-			fprintf(stderr, "[jpeg] chunk %d begins at %.2f ms\n", k, since());
-		if (sl.busy) {
-			if (cudaEventSynchronize(sl.done) != cudaSuccess) {
-				R.rc = -1;
-				R.err = std::string("jpeg decode: ") + cudaGetErrorString(cudaGetLastError());
-				return R;
-			}
-			sl.busy = false;
-		}
-		if (sl.cap < total) {
-			if (sl.pinned)
-				cudaFreeHost(sl.pinned);
-			sl.pinned = nullptr;
-			sl.cap = 0;
-			const size_t want = total + total / 4;
-			if (cudaMallocHost(&sl.pinned, want) != cudaSuccess) {
-				R.rc = -1;
-				R.err = std::string("cudaMallocHost (jpeg staging): ") + cudaGetErrorString(cudaGetLastError());
-				return R;
-			}
-			sl.cap = want;
-		}
-		char *hst = (char *) sl.pinned;
-		if (trace)
-			fprintf(stderr, "[jpeg] chunk %d slot free at %.2f ms\n", k, since());
-		parallel_for(cn, host_workers(), [&](int i) {
-			const FramePrep &fp = prep[c0 + i];
-			unsigned char *dst = (unsigned char *) hst + off_b + data_off[i];
-			if (fp.F.progressive) {
-				/* every scan's segment unstuffed one after the other; the scan records and their tables beside them */
-				JpegFrameDev F = fp.F;
-				F.data_off = data_off[i];
-				for (int c = 0; c < F.ncomp; c++)
-					F.coef_off[c] += coef_off[i];
-				F.huff_base = (int) huff_off[i];
-				F.scan_base = (unsigned) scan_off[i];
-				F.sync = 0;
-				for (int c = 0; c < F.ncomp; c++)
-					F.plane_off[c] += plane_off[i];
-				size_t pos = 0, ipos = int_off[i];
-				for (size_t j = 0; j < fp.scans.size(); j++) {
-					const FramePrep::ScanPrep &sp = fp.scans[j];
-					const size_t clean = destuff_scan(sp.src, sp.len, dst + pos, (unsigned *) (hst + off_o) + ipos, sp.S.n_intervals, (unsigned) pos);
-					if (clean == (size_t) -1) {
-						int none = -1;
-						bad_frame.compare_exchange_strong(none, c0 + i);
-						return;
-					}
-					const size_t room = ((sp.len + 15) & ~(size_t) 15) + 16;
-					memset(dst + pos + clean, 0, room - clean);
-					ScanDev S = sp.S;
-					S.interval_off = (unsigned) ipos;
-					S.huff_base = (int) (huff_off[i] + 4 * j);
-					memcpy(hst + off_s + (scan_off[i] + j) * sizeof(ScanDev), &S, sizeof(S));
-					memcpy(hst + off_h + (huff_off[i] + 4 * j) * sizeof(HuffDev), sp.huff, 4 * sizeof(HuffDev));
-					pos += room;
-					ipos += (size_t) sp.S.n_intervals + 1;
-				}
-				memcpy(hst + (size_t) i * sizeof(JpegFrameDev), &F, sizeof(F));
-				return;
-			}
-			const size_t clean = destuff_scan(fp.src, fp.src_len, dst, (unsigned *) (hst + off_o) + int_off[i], fp.F.n_intervals);
-			if (clean == (size_t) -1) {
-				int none = -1;
-				bad_frame.compare_exchange_strong(none, c0 + i);
-				return;
-			}
-			JpegFrameDev F = fp.F;
-			F.data_off = data_off[i];
-			F.interval_off = int_off[i];
-			for (int c = 0; c < F.ncomp; c++)
-				F.coef_off[c] += coef_off[i];
-			F.huff_base = (int) huff_off[i];
-			F.clean_len = (unsigned) clean;
-			F.sync = sync_cap[i] > 0;
-			F.sync_off = sync_off[i];
-			F.sync_cap = sync_cap[i];
-			for (int c = 0; c < F.ncomp; c++)
-				F.plane_off[c] += plane_off[i];
-			memcpy(hst + (size_t) i * sizeof(JpegFrameDev), &F, sizeof(F));
-			memcpy(hst + off_h + huff_off[i] * sizeof(HuffDev), fp.huff, 8 * sizeof(HuffDev));
-			memset(dst + clean, 0, (((fp.src_len + 15) & ~(size_t) 15) + 16) - clean); /* the reader's look-ahead past the end */
-		});
-		if (bad_frame.load() >= 0) {
-			R.rc = -1;
-			R.err = "frame " + std::to_string(bad_frame.load()) + ": restart markers do not match the restart interval";
-			return R;
-		}
-		if (trace)
-			fprintf(stderr, "[jpeg] chunk %d (%d frames) staged at %.2f ms\n", k, cn, since());
-		R.max_intervals = max_intervals;
-		R.max_mcus = max_mcus;
-		R.max_subs = max_subs;
-		R.total = total;
-		R.off_h = off_h;
-		R.off_o = off_o;
-		R.off_b = off_b;
-		R.coef_total = coef_total;
-		R.sync_total = sync_total;
-		R.plane_total = plane_total;
-		R.max_blocks = max_blocks;
-		R.max_scans = max_scans;
-		R.max_scan_intervals = max_scan_intervals;
-		R.off_s = off_s;
-		return R;
-	};
-
 	const int n_chunks = (n + chunk - 1) / chunk;
-	Staged cur = stage_chunk(0, false);
+	auto stage = [&](int k) { return stage_chunk(prep, k, k * chunk, std::min(chunk, n - k * chunk), P, o); };
+	ChunkLayout cur = stage(0);
 	for (int k = 0; k < n_chunks && !rc; k++) {
-		if (cur.rc) {
+		if (!cur.err.empty()) {
 			error(domain, "%s", cur.err.c_str());
 			rc = -1;
 			break;
 		}
-		/* the next chunk stages while this one is queued and decoded */
-		Staged next;
-		std::thread helper;
+		/* the next chunk stages while this one is queued and decoded (leaving the loop waits for it: see std::async) */
+		std::future<ChunkLayout> next;
 		if (k + 1 < n_chunks)
-			helper = std::thread([&, k] { next = stage_chunk(k + 1, true); });
-		struct Joiner {
-			std::thread &t;
-			~Joiner()
-			{
-				if (t.joinable())
-					t.join();
-			}
-		} joiner{helper};
-		const int c0 = cur.c0, cn = cur.cn, max_intervals = cur.max_intervals, max_mcus = cur.max_mcus;
-		const unsigned max_subs = cur.max_subs;
-		const size_t total = cur.total, off_h = cur.off_h, off_o = cur.off_o, off_b = cur.off_b, coef_total = cur.coef_total,
-					 sync_total = cur.sync_total, plane_total = cur.plane_total;
-		const int max_blocks = cur.max_blocks, max_scans = cur.max_scans, max_scan_intervals = cur.max_scan_intervals;
-		const size_t off_s = cur.off_s;
+			next = std::async(std::launch::async, [&, k] {
+				cudaSetDevice(device);
+				return stage(k + 1);
+			});
 		JpegSlot &sl = P.slot[k % kJpegSlots];
-		char *hst = (char *) sl.pinned;
-		cudaStream_t st = sl.stream;
-		if (k < kJpegSlots && cudaStreamWaitEvent(st, P.fork, 0) != cudaSuccess) {
+		if (k < kJpegSlots && cudaStreamWaitEvent(sl.stream, P.fork, 0) != cudaSuccess) {
 			rc = cuda_fail(domain, cudaGetLastError(), "jpeg decode");
 			break;
 		}
-		auto grow = [&](void **p, size_t *cap, size_t want) {
-			if (*cap >= want)
-				return true;
-			if (*p)
-				cudaFree(*p); /* waits for the device: nothing of this slot is in flight (sl.busy was waited for) */
-			*p = nullptr;
-			*cap = 0;
-			if (cudaMalloc(p, want + want / 8) != cudaSuccess) {
-				cuda_fail(domain, cudaGetLastError(), "cudaMalloc (jpeg slot)");
-				return false;
-			}
-			*cap = want + want / 8;
-			return true;
-		};
-		/* per subsequence: two (state, count) records, the start state last decoded from, the first block's index */
-		const size_t sync_rec = 2 * sizeof(SyncState) + 2 * sizeof(unsigned) + sizeof(SyncState) + sizeof(unsigned);
-		if (!grow(&sl.dev, &sl.dev_cap, total) || !grow(&sl.coef, &sl.coef_cap, coef_total * sizeof(short)) ||
-			(sync_total && !grow(&sl.sync, &sl.sync_cap, sync_total * sync_rec + 256)) ||
-			(plane_total && !grow(&sl.planes, &sl.planes_cap, plane_total))) {
+		if (!JpegSlot::grow(domain, sl.dev, sl.dev_cap, cur.total) || !JpegSlot::grow(domain, sl.coef, sl.coef_cap, cur.coef_total * sizeof(short)) ||
+			(cur.sync_total && !JpegSlot::grow(domain, sl.sync, sl.sync_cap, cur.sync_total * kSyncRecordBytes + 256)) ||
+			(cur.plane_total && !JpegSlot::grow(domain, sl.planes, sl.planes_cap, cur.plane_total))) {
 			rc = -1;
 			break;
 		}
-		void *dev = sl.dev, *coef = sl.coef;
 		cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-		do {
-			if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-				cudaMemsetAsync(coef, 0, coef_total * sizeof(short), st) != cudaSuccess) {
-				rc = cuda_fail(domain, cudaGetLastError(), "jpeg staging copy");
-				break;
-			}
-			const JpegFrameDev *dF = (const JpegFrameDev *) dev;
-			const HuffDev *dH = (const HuffDev *) ((char *) dev + off_h);
-			const unsigned *dO = (const unsigned *) ((char *) dev + off_o);
-			const unsigned char *dB = (const unsigned char *) dev + off_b;
-			if (timing) {
-				for (auto &e : ev)
-					cudaEventCreate(&e);
-				cudaEventRecord(ev[0], st);
-			}
-			if (sync_total) {
-				SyncState *Ea = (SyncState *) sl.sync, *Eb = Ea + sync_total, *Su = Eb + sync_total;
-				unsigned *Na = (unsigned *) (Su + sync_total), *Nb = Na + sync_total, *Bs = Nb + sync_total;
-				const dim3 sg((max_subs + kSyncThreads - 1) / kSyncThreads, cn);
-				/* passes until one in which no subsequence had to decode again: groups of four, each pass with its own flag
-				 * word (after the records), read back after the group -- this chunk's stream waits, the others run on
-				 */
-				int *redo = (int *) (Bs + sync_total);
-				int pass = 0;
-				bool settled = false;
-				while (!settled && pass < sync_passes) {
-					int flags[4] = {1, 1, 1, 1};
-					cudaMemsetAsync(redo, 0, sizeof(flags), st);
-					int g = 0;
-					for (; g < 4 && pass < sync_passes; g++, pass++) {
-						jpeg_sync_pass_kernel<<<sg, kSyncThreads, 0, st>>>(dF, dH, dB, pass, sub_bytes, Ea, Na, Eb, Nb, Su, redo + g);
-						std::swap(Ea, Eb);
-						std::swap(Na, Nb);
-						count_launch();
-					}
-					if (cudaMemcpyAsync(flags, redo, sizeof(flags), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-						cudaStreamSynchronize(st) != cudaSuccess) {
-						rc = cuda_fail(domain, cudaGetLastError(), "jpeg_sync_pass_kernel");
-						break;
-					}
-					for (int j = pass - g == 0 ? 1 : 0; j < g; j++)
-						if (flags[j] == 0)
-							settled = true; /* later passes of the group only copied */
-				}
-				if (rc)
-					break;
-				/* not settled: the write pass finds the inconsistency and fails the frame */
-				jpeg_sync_scan_kernel<<<cn, 1024, 0, st>>>(dF, sub_bytes, Na, Bs);
-				jpeg_sync_write_kernel<<<sg, kSyncThreads, 0, st>>>(dF, dH, dB, sub_bytes, Ea, Bs, Su, (short *) coef, status + c0);
-				jpeg_dc_scan_kernel<<<dim3(kMaxComp, cn), 1024, 0, st>>>(dF, (short *) coef);
-				cudaError_t es = cudaGetLastError();
-				if (es != cudaSuccess) {
-					rc = cuda_fail(domain, es, "jpeg_sync kernels launch");
-					break;
-				}
-				count_launch();
-				count_launch();
-				count_launch();
-			}
-			if (max_scans > 0) {
-				/* progressive frames: their scans in order, scan j of every frame in one launch */
-				const ScanDev *dS = (const ScanDev *) ((char *) dev + off_s);
-				for (int j = 0; j < max_scans; j++) {
-					jpeg_progressive_kernel<<<dim3((max_scan_intervals + kHuffThreads - 1) / kHuffThreads, cn), kHuffThreads, 0, st>>>(dF, dS, dH, dB, dO,
-						(short *) coef, status + c0, j);
-					count_launch();
-				}
-				cudaError_t ep = cudaGetLastError();
-				if (ep != cudaSuccess) {
-					rc = cuda_fail(domain, ep, "jpeg_progressive_kernel launch");
-					break;
-				}
-			}
-			/* CTA width: one interval per warp while the chunk has fewer intervals than the machine has CTA slots */
-			int ht = 1;
-			while (ht < kHuffThreads && (long long) cn * ((max_intervals + ht - 1) / ht) > huff_cta_slots)
-				ht *= 2;
-			if (max_intervals > 0) /* a chunk of progressive frames only has no baseline interval */
-				jpeg_huffman_kernel<<<dim3((max_intervals + ht - 1) / ht, cn), ht, 0, st>>>(dF, dH, dB, dO, (short *) coef, status + c0);
-			cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess) {
-				rc = cuda_fail(domain, e, "jpeg_huffman_kernel launch");
-				break;
-			}
-			count_launch();
-			if (timing)
-				cudaEventRecord(ev[1], st);
-			jpeg_idct_kernel<<<dim3((max_mcus + 127) / 128, cn), 128, 0, st>>>(dF, (const short *) coef,
-				(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
-			e = cudaGetLastError();
-			if (e != cudaSuccess) {
-				rc = cuda_fail(domain, e, "jpeg_idct_kernel launch");
-				break;
-			}
-			count_launch();
-			if (plane_total) {
-				jpeg_idct_planes_kernel<<<dim3((max_blocks + 127) / 128, cn), 128, 0, st>>>(dF, (const short *) coef, (unsigned char *) sl.planes);
-				jpeg_upsample_kernel<<<dim3((W + 31) / 32, (Hh + 7) / 8, cn), 256, 0, st>>>(dF, (const unsigned char *) sl.planes,
-					(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
-				e = cudaGetLastError();
-				if (e != cudaSuccess) {
-					rc = cuda_fail(domain, e, "jpeg planar kernels launch");
-					break;
-				}
-				count_launch();
-				count_launch();
-			}
-			if (timing) {
-				cudaEventRecord(ev[2], st);
-				cudaEventSynchronize(ev[2]);
-				float a = 0, b = 0;
-				cudaEventElapsedTime(&a, ev[0], ev[1]);
-				cudaEventElapsedTime(&b, ev[1], ev[2]);
-				P.huff_ms += a;
-				P.idct_ms += b;
-			}
-		} while (0);
+		if (o.timing == '1')
+			for (auto &e : ev)
+				cudaEventCreate(&e);
+		if (cudaMemcpyAsync(sl.dev, sl.pinned, cur.total, cudaMemcpyHostToDevice, sl.stream) != cudaSuccess ||
+			cudaMemsetAsync(sl.coef, 0, cur.coef_total * sizeof(short), sl.stream) != cudaSuccess)
+			rc = cuda_fail(domain, cudaGetLastError(), "jpeg staging copy");
+		else {
+			const int launches =
+				launch_chunk(domain, cur, sl, o, status, (unsigned char *) out, out_bpl, out_frame_stride, W, Hh, o.timing == '1' ? ev : nullptr);
+			const cudaError_t e = cudaGetLastError();
+			if (launches < 0)
+				rc = -1;
+			else if (e != cudaSuccess)
+				rc = cuda_fail(domain, e, "jpeg decode kernels launch");
+			else
+				count_launch(launches);
+		}
+		if (!rc && o.timing == '1') {
+			cudaEventSynchronize(ev[2]);
+			float a = 0, b = 0;
+			cudaEventElapsedTime(&a, ev[0], ev[1]);
+			cudaEventElapsedTime(&b, ev[1], ev[2]);
+			P.huff_ms += a;
+			P.idct_ms += b;
+		}
 		for (auto &e : ev)
 			if (e)
 				cudaEventDestroy(e);
-		if (!rc && cudaEventRecord(sl.done, st) == cudaSuccess)
+		if (!rc && cudaEventRecord(sl.done, sl.stream) == cudaSuccess)
 			sl.busy = true;
-		if (helper.joinable())
-			helper.join();
-		cur = next;
+		if (next.valid())
+			cur = next.get();
 	}
-	if (trace)
-		fprintf(stderr, "[jpeg] all chunks queued at %.2f ms\n", since());
+	if (o.timing == '2')
+		fprintf(stderr, "[jpeg] all chunks queued at %.2f ms\n", P.ms());
 	/* join: s continues after the internal streams; then wait for the verdict */
 	for (auto &sl : P.slot)
 		if (sl.busy) {
@@ -2557,8 +2478,8 @@ dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t 
 		rc = cuda_fail(domain, cudaGetLastError(), "jpeg decode");
 	if (rc)
 		cudaDeviceSynchronize();
-	if (trace)
-		fprintf(stderr, "[jpeg] decoded at %.2f ms\n", since());
+	if (o.timing == '2')
+		fprintf(stderr, "[jpeg] decoded at %.2f ms\n", P.ms());
 	dev_free(status, s);
 	for (int i = 0; i < n && !rc; i++)
 		if (st[i]) {
@@ -2588,90 +2509,36 @@ host_jpeg_decode(const char *domain, const void *buf, size_t len, int shrink, un
 	if (!out)
 		return 0;
 	const JpegFrameDev &F = P.F;
+	/* staged as the pump stages a chunk of this one frame: unstuffed, aligned, zero-padded */
+	std::vector<unsigned> bytes_w((P.stage_bytes + 16) / 4, 0), ints(P.stage_ints);
+	const unsigned char *bytes = (const unsigned char *) bytes_w.data();
+	std::vector<ScanDev> scans(P.segs.size());
+	size_t clean = 0;
+	for (size_t j = 0; j < P.segs.size(); j++)
+		if ((clean = stage_segment(P.segs[j], (unsigned char *) bytes_w.data(), ints.data(), 0, 0, &scans[j])) == (size_t) -1) {
+			error(domain, "restart markers do not match the restart interval");
+			return -1;
+		}
 	std::vector<short> coef(P.coef_count, 0);
-	if (F.progressive) {
-		for (const FramePrep::ScanPrep &sp : P.scans) {
-			std::vector<unsigned> pw((sp.len + 32) / 4 + 1, 0);
-			std::vector<unsigned> offs(sp.S.n_intervals + 1);
-			if (destuff_scan(sp.src, sp.len, (unsigned char *) pw.data(), offs.data(), sp.S.n_intervals) == (size_t) -1) {
-				error(domain, "restart markers do not match the restart interval");
-				return -1;
-			}
-			const int total = sp.S.units_x * sp.S.units_y;
-			const int per = sp.S.restart_interval > 0 ? sp.S.restart_interval : total;
-			for (int i = 0; i < sp.S.n_intervals; i++)
-				if (decode_scan_interval(F, sp.S, sp.huff, kZigzag, (const unsigned char *) pw.data(), offs[i], offs[i + 1], i * per,
-						std::min(total, (i + 1) * per), coef.data())) {
+	McuLayout M;
+	mcu_layout(F, M);
+	if (!F.progressive && sub_bytes > 0 && scans[0].n_intervals == 1) {
+		if (host_sync_decode(domain, F, M, P.huff.data(), bytes, (unsigned) clean, sub_bytes, max_passes, passes_used, coef.data()))
+			return -1;
+	}
+	else
+		for (const ScanDev &S : scans)
+			for (int i = 0; i < S.n_intervals; i++) {
+				const unsigned *off = ints.data() + S.interval_off;
+				const HuffDev *huff = P.huff.data() + S.huff_base;
+				int u0, u1;
+				scan_interval(S, i, &u0, &u1);
+				if (F.progressive ? decode_scan_interval(F, S, huff, kZigzag, bytes, off[i], off[i + 1], u0, u1, coef.data())
+								  : decode_interval(M, huff, kZigzag, bytes, off[i], off[i + 1], u0, u1, coef.data())) {
 					error(domain, "corrupt JPEG data: bad Huffman code");
 					return -1;
 				}
-		}
-	}
-	else {
-	/* unstuffed, aligned, zero-padded: as the pump stages it */
-	std::vector<unsigned> padded_w((P.src_len + 32) / 4 + 1, 0);
-	unsigned char *padded = (unsigned char *) padded_w.data();
-	std::vector<unsigned> offs(F.n_intervals + 1);
-	const size_t clean = destuff_scan(P.src, P.src_len, padded, offs.data(), F.n_intervals);
-	if (clean == (size_t) -1) {
-		error(domain, "restart markers do not match the restart interval");
-		return -1;
-	}
-	const int total = F.mcus_x * F.mcus_y;
-	const int per = F.restart_interval > 0 ? F.restart_interval : total;
-	McuLayout M;
-	mcu_layout(F, M);
-	if (sub_bytes > 0 && F.n_intervals == 1) {
-		const unsigned S = (unsigned) ((clean + sub_bytes - 1) / sub_bytes);
-		std::vector<SyncState> Ea(S + 1), Eb(S + 1), Su(S + 1);
-		std::vector<unsigned> Na(S + 1, 0), Nb(S + 1, 0), Bs(S + 1, 0);
-		int used = 0;
-		for (int pass = 0; pass < max_passes; pass++) {
-			bool redo = false;
-			for (unsigned sx = 0; sx < S; sx++)
-				redo |= sync_pass(M, P.huff, padded, (unsigned) clean, sub_bytes, pass, sx, Ea.data(), Na.data(), Eb.data(), Nb.data(), Su.data());
-			Ea.swap(Eb);
-			Na.swap(Nb);
-			if (pass > 0 && !redo)
-				break;
-			used = pass + 1;
-		}
-		if (passes_used)
-			*passes_used = used;
-		unsigned run = 0;
-		for (unsigned sx = 0; sx < S; sx++) {
-			Bs[sx] = run;
-			run += Na[sx];
-		}
-		const unsigned total_blocks = (unsigned) (total * F.blocks_per_mcu);
-		int bad = 0;
-		for (unsigned sx = 0; sx < S; sx++)
-			bad |= sync_write(M, P.huff, kZigzag, padded, (unsigned) clean, sub_bytes, sx, S, Ea.data(), Bs.data(), Su.data(), total_blocks,
-				coef.data());
-		if (bad) {
-			error(domain, (bad & 1) ? "corrupt JPEG data: bad Huffman code" : "the subsequence decode did not converge");
-			return -1;
-		}
-		for (int c = 0; c < F.ncomp; c++) {
-			int first = 0;
-			while (first < M.n && M.comp[first] != c)
-				first++;
-			const int pc = F.h[c] * F.v[c];
-			int runv = 0;
-			for (unsigned i = 0; i < (unsigned) (total * pc); i++) {
-				short *p = dc_block(M, &first, pc, i, coef.data());
-				runv += p[0];
-				p[0] = (short) runv;
 			}
-		}
-	}
-	else
-		for (int i = 0; i < F.n_intervals; i++)
-			if (decode_interval(M, P.huff, kZigzag, padded, offs[i], offs[i + 1], i * per, std::min(total, (i + 1) * per), coef.data())) {
-				error(domain, "corrupt JPEG data: bad Huffman code");
-				return -1;
-			}
-	}
 	if (F.planar) {
 		std::vector<unsigned char> planes(P.plane_bytes);
 		for (int c = 0; c < F.ncomp; c++)
@@ -2799,12 +2666,10 @@ vb200_thumbnail_jpegshrink(int width, int height, int target_width, int target_h
 extern "C" void
 vb200_debug_jpeg_times(float *huffman_ms, float *idct_ms)
 {
-	float a = 0, b = 0;
-	jpeg_last_kernel_times(&a, &b);
 	if (huffman_ms)
-		*huffman_ms = a;
+		*huffman_ms = g_pump.huff_ms;
 	if (idct_ms)
-		*idct_ms = b;
+		*idct_ms = g_pump.idct_ms;
 }
 
 extern "C" int
@@ -2836,7 +2701,7 @@ namespace vb200 {
 /* read_jpeg_header, foreign/jpeg2vips.c:699-799, over the markers jpeg_read_header sees (those before the first SOS):
  * an APP2 segment of more than 14 bytes that starts "ICC_PROFILE" stores its bytes from 14 on in slot data[12] - 1 (slots
  * 0 .. 99, a later duplicate wins; data[13], the chunk count, is not read); the profile is slots 0, 1, 2 ... concatenated
- * up to the first empty one.  Marker walking as parse_jpeg (libjpeg's next_marker: garbage, then fill bytes, skipped).
+ * up to the first empty one.  Markers are walked by next_segment, as parse_jpeg walks them.
  */
 int
 jpeg_icc_profile(const char *domain, const unsigned char *d, size_t len, std::vector<unsigned char> *profile)
@@ -2850,34 +2715,17 @@ jpeg_icc_profile(const char *domain, const unsigned char *d, size_t len, std::ve
 	size_t slot_len[100] = {0};
 	size_t p = 2;
 	for (;;) {
-		while (p < len && d[p] != 0xFF)
-			p++;
-		while (p < len && d[p] == 0xFF)
-			p++;
-		if (p >= len) {
-			error(domain, "JPEG stream ends before the scan");
+		const unsigned char *s = nullptr;
+		size_t n = 0;
+		const int m = next_segment(domain, d, len, p, &s, &n);
+		if (m < 0)
 			return -1;
-		}
-		const int m = d[p++];
-		if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01)
-			continue;
 		if (m == 0xD9) {
 			error(domain, "JPEG stream has no scan");
 			return -1;
 		}
-		if (p + 2 > len) {
-			error(domain, "truncated JPEG marker segment");
-			return -1;
-		}
-		const size_t L = be16(d + p);
-		if (L < 2 || p + L > len) {
-			error(domain, "truncated JPEG marker segment");
-			return -1;
-		}
 		if (m == 0xDA)
 			break;
-		const unsigned char *s = d + p + 2;
-		const size_t n = L - 2;
 		if (m == 0xE2 && n > 14 && memcmp(s, "ICC_PROFILE", 11) == 0) {
 			const int k = s[12] - 1;
 			if (k >= 0 && k < 100) {
@@ -2885,7 +2733,6 @@ jpeg_icc_profile(const char *domain, const unsigned char *d, size_t len, std::ve
 				slot_len[k] = n - 14;
 			}
 		}
-		p += L;
 	}
 	for (int k = 0; k < 100 && slot[k]; k++)
 		profile->insert(profile->end(), slot[k], slot[k] + slot_len[k]);

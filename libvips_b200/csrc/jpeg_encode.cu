@@ -39,12 +39,11 @@
 
 #include "../../include/vb200.h"
 #include "vb200_internal.h"
+#include "jpeg_common.cuh"
 
 namespace vb200 {
 
 namespace {
-
-#define HD __host__ __device__ __forceinline__
 
 /* ITU T.81 Annex K.1 / K.3, as jcparam.c holds them (natural order) */
 const unsigned char kStdLumQ[64] = {16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51,
@@ -70,8 +69,6 @@ const unsigned char kValAcChr[162] = {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 
 	0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3,
 	0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda,
 	0xe2, 0xe3, 0xe4, 0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa};
-const unsigned char kZz[64] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28, 35,
-	42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
 /* everything the kernels need about one geometry / quality */
 struct EncodeTables {
@@ -129,7 +126,7 @@ make_tables(int quality, EncodeTables *T)
 	derive_codes(kBitsAcLum, kValAcLum, T->ehufco[1], T->ehufsi[1]);
 	derive_codes(kBitsDcChr, kValDc, T->ehufco[2], T->ehufsi[2]);
 	derive_codes(kBitsAcChr, kValAcChr, T->ehufco[3], T->ehufsi[3]);
-	memcpy(T->zz, kZz, 64);
+	memcpy(T->zz, kZigzag, 64);
 }
 
 /* ------------------------------------------------------------------ pixels -> quantised blocks (host + device) */
@@ -155,20 +152,10 @@ min_(int a, int b)
 	return a < b ? a : b;
 }
 
-HD int
-fdescale(int x, int n)
-{
-	return (x + (1 << (n - 1))) >> n;
-}
-
 /* jfdctint.c jpeg_fdct_islow on d[64] (samples already centred on 0), in place */
 HD void
 fdct_islow(int *d)
 {
-	constexpr int CB = 13, P1 = 2;
-	constexpr int F_0_298631336 = 2446, F_0_390180644 = 3196, F_0_541196100 = 4433, F_0_765366865 = 6270, F_0_899976223 = 7373, F_1_175875602 = 9633,
-				  F_1_501321110 = 12299, F_1_847759065 = 15137, F_1_961570560 = 16069, F_2_053119869 = 16819, F_2_562915447 = 20995,
-				  F_3_072711026 = 25172;
 	for (int pass = 0; pass < 2; pass++) {
 		const int step = pass == 0 ? 1 : 8, next = pass == 0 ? 8 : 1;
 		for (int i = 0; i < 8; i++) {
@@ -183,13 +170,13 @@ fdct_islow(int *d)
 				p[4 * step] = (int) ((unsigned) (tmp10 - tmp11) << P1);
 			}
 			else {
-				p[0] = fdescale(tmp10 + tmp11, P1);
-				p[4 * step] = fdescale(tmp10 - tmp11, P1);
+				p[0] = descale(tmp10 + tmp11, P1);
+				p[4 * step] = descale(tmp10 - tmp11, P1);
 			}
 			const int sh = pass == 0 ? CB - P1 : CB + P1;
 			int z1 = (tmp12 + tmp13) * F_0_541196100;
-			p[2 * step] = fdescale(z1 + tmp13 * F_0_765366865, sh);
-			p[6 * step] = fdescale(z1 + tmp12 * (-F_1_847759065), sh);
+			p[2 * step] = descale(z1 + tmp13 * F_0_765366865, sh);
+			p[6 * step] = descale(z1 + tmp12 * (-F_1_847759065), sh);
 			z1 = tmp4 + tmp7;
 			int z2 = tmp5 + tmp6, z3 = tmp4 + tmp6, z4 = tmp5 + tmp7;
 			const int z5 = (z3 + z4) * F_1_175875602;
@@ -200,10 +187,10 @@ fdct_islow(int *d)
 			z4 *= -F_0_390180644;
 			z3 += z5;
 			z4 += z5;
-			p[7 * step] = fdescale(t4 + z1 + z3, sh);
-			p[5 * step] = fdescale(t5 + z2 + z4, sh);
-			p[3 * step] = fdescale(t6 + z2 + z3, sh);
-			p[1 * step] = fdescale(t7 + z1 + z4, sh);
+			p[7 * step] = descale(t4 + z1 + z3, sh);
+			p[5 * step] = descale(t5 + z2 + z4, sh);
+			p[3 * step] = descale(t6 + z2 + z3, sh);
+			p[1 * step] = descale(t7 + z1 + z4, sh);
 		}
 	}
 }
@@ -561,7 +548,7 @@ header_prefix(const EncodeGeom &G, const EncodeTables &T, std::vector<unsigned c
 		put16(o, 67);
 		o.push_back((unsigned char) t);
 		for (int i = 0; i < 64; i++)
-			o.push_back((unsigned char) T.q[t][kZz[i]]);
+			o.push_back((unsigned char) T.q[t][kZigzag[i]]);
 	}
 	put16(o, sof);
 	put16(o, 8 + 3 * G.ncomp);
@@ -1045,36 +1032,6 @@ jpeg_count_kernel(const EncodeGeom G, const EncodeTables *__restrict__ T, const 
 	frame_tables<kFrameTables>(T, huff, blockIdx.y, &co, &si);
 	bits[(size_t) blockIdx.y * (G.blocks + 1) + b] = code_block(co, si, T->zz, fc + (size_t) b * 64, block_comp(G, (int) (b % (unsigned) G.blocks_per_mcu)),
 		previous_dc(G, fc, b, kRestart ? restart : 0), [](unsigned, int) {});
-}
-
-/* Exclusive prefix sum over items 0 .. n - 1 in one CTA: each thread sums a contiguous chunk of val(i), the chunk sums
- * are scanned in s_part[blockDim.x] (shared memory), then put(i, the sum of the items before i) is called for every item
- * in order, each after its val(i).  Returns the sum of all items.
- */
-template <typename T, typename Val, typename Put>
-__device__ __forceinline__ T
-cta_exclusive_scan(unsigned n, T *s_part, Val val, Put put)
-{
-	const unsigned per = (n + blockDim.x - 1) / blockDim.x;
-	const unsigned a = min(n, threadIdx.x * per), e = min(n, a + per);
-	T sum = 0;
-	for (unsigned i = a; i < e; i++)
-		sum += val(i);
-	s_part[threadIdx.x] = sum;
-	__syncthreads();
-	for (unsigned o = 1; o < blockDim.x; o <<= 1) {
-		const T v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-		__syncthreads();
-		s_part[threadIdx.x] += v;
-		__syncthreads();
-	}
-	T run = s_part[threadIdx.x] - sum;
-	for (unsigned i = a; i < e; i++) {
-		const T v = val(i);
-		put(i, run);
-		run += v;
-	}
-	return s_part[blockDim.x - 1];
 }
 
 /* exclusive prefix sum of a frame's bit counts (in place) over its nslots slots, the last of which receives the total,
@@ -2203,7 +2160,7 @@ host_prog_scan(const EncodeGeom &G, const Scan &S, const short *coef, int restar
 		if (S.ah == 0) {
 			int r = 0;
 			for (int k = S.ss; k <= S.se; k++) {
-				int temp = block[kZz[k]], temp2;
+				int temp = block[kZigzag[k]], temp2;
 				if (temp == 0) {
 					r++;
 					continue;
@@ -2245,7 +2202,7 @@ host_prog_scan(const EncodeGeom &G, const Scan &S, const short *coef, int restar
 		int absvalues[64];
 		int EOB = 0;
 		for (int k = S.ss; k <= S.se; k++) {
-			int temp = block[kZz[k]];
+			int temp = block[kZigzag[k]];
 			if (temp < 0)
 				temp = -temp;
 			temp >>= S.al;
@@ -2278,7 +2235,7 @@ host_prog_scan(const EncodeGeom &G, const Scan &S, const short *coef, int restar
 			}
 			emit_eobrun();
 			emit_symbol(0, (r << 4) + 1);
-			emit_bits(block[kZz[k]] < 0 ? 0u : 1u, 1);
+			emit_bits(block[kZigzag[k]] < 0 ? 0u : 1u, 1);
 			for (int i = 0; i < BR; i++)
 				emit_bits((unsigned) BR_buffer[i], 1);
 			BR_buffer = bit_buffer;
