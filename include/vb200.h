@@ -566,7 +566,9 @@ int vb200_jpeg_decode_batch(const void *const *bufs, const size_t *lens, int n, 
 int vb200_jpegload_buffer(const void *buf, size_t len, int shrink, VB200Image *out);
 int vb200_thumbnail_jpegshrink(int width, int height, int target_width, int target_height, int size);
 /* vips_thumbnail_buffer(buf, len, &out, width, "height", height, "size", size, NULL) for a JPEG stream (thumbnail.c:583-613,
- * 848-902): load-time shrink by vb200_thumbnail_jpegshrink, decode and thumbnail on the device; out: allocate-or-fill */
+ * 848-902): load-time shrink by vb200_thumbnail_jpegshrink, decode and thumbnail on the device; out: allocate-or-fill.
+ * A PNG stream (by its signature) decodes at full size (no load-time shrink, thumbnail.c:609-660) with its iCCP profile as
+ * the embedded profile; PNGs with eXIf return -1 (their orientation would need vips_autorot). */
 int vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size);
 int vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink,
 	void *out, int out_location, size_t out_frame_stride);
@@ -576,6 +578,39 @@ int vb200_debug_jpeg_decode(const void *buf, size_t len, int shrink, void *out, 
  * max_passes passes), *passes_used = the last pass that changed a record */
 int vb200_debug_jpeg_decode_sync(const void *buf, size_t len, int shrink, int sub_bytes, int max_passes, void *out, size_t out_bpl,
 	int *width, int *height, int *bands, int *passes_used);
+
+/* ------------------------------------------------------------------ PNG decode on the device (SURVEY 8f rank 1)
+ * vips_pngload_buffer(buf, len, &out, NULL) (foreign/spngload.c, libspng over zlib, fail_on = none: CRCs and Adler-32 not
+ * checked, :346-352) with inflate and unfilter on the device (csrc/png.cu): the IDAT payloads are all that crosses PCIe.
+ * Decoded: non-interlaced 8-bit grey, grey + alpha, RGB and RGBA; palette at 1 / 2 / 4 / 8 bits, to RGB or, with tRNS,
+ * RGBA; grey at 1 / 2 / 4 bits scaled to 8; tRNS on 8-bit grey and RGB as an alpha band, 0 where the sample equals the
+ * key (SPNG_DECODE_TRNS, :592; formats :385-480).  Output is uchar [n][height][width][bands], bands 1 to 4, B_W below 3
+ * bands and sRGB from 3.  Everything else returns -1 with its reason (the host keeps its loader): 16-bit samples, Adam7,
+ * low-bit grey with tRNS, a missing PLTE or an index beyond it, IDAT chunks that are not consecutive, a zlib header with a
+ * preset dictionary, another method or a bad FCHECK, a deflate stream zlib refuses, one that inflates to more or fewer
+ * scanline bytes than IHDR implies, frames over 2^28 pixels.
+ *
+ * vb200_png_decode_batch: n streams of ONE output geometry; a stream that fails fails the batch with "frame i:" in the
+ *   error, and with out in host memory nothing is written (in device memory, frames of earlier chunks of a batch larger
+ *   than one chunk may be).  out = NULL only reports the geometry, without a device.
+ * vb200_pngload_buffer: one stream into a VB200Image (allocate-or-fill).
+ * vb200_png_icc_profile: the iCCP profile (spngload.c:244-246), inflated on the host; as vb200_jpeg_icc_profile.
+ * vb200_thumbnail_plan_run_png: decode + the plan's thumbnail chain, frames never leave the device; PNG has no load-time
+ *   shrink (thumbnail.c:609-660), so the plan is made for the full frame.  Streams with eXIf are declined, as by
+ *   vb200_thumbnail_buffer: their orientation would need vips_autorot (thumbnail.c:989-996).
+ * vb200_debug_png_decode / vb200_debug_inflate: test hooks, host only -- the same per-symbol, per-byte and per-pixel code
+ *   on the CPU; vb200_debug_inflate takes raw deflate data and sets *out_len = cap + 1 when the output does not fit.
+ * vb200_debug_png_set_budget: device bytes per chunk (0: an eighth of the device, at least 1 GiB).
+ */
+int vb200_png_decode_batch(const void *const *bufs, const size_t *lens, int n, void *out, int out_location, size_t out_bpl,
+	size_t out_frame_stride, int *width, int *height, int *bands);
+int vb200_pngload_buffer(const void *buf, size_t len, VB200Image *out);
+int vb200_png_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len);
+int vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out,
+	int out_location, size_t out_frame_stride);
+int vb200_debug_png_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
+int vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *out_len);
+void vb200_debug_png_set_budget(size_t bytes);
 /* vips_jpegsave_buffer (foreign/vips2jpeg.c:551-700: jpeg_set_quality(Q, TRUE), chroma subsampled 2 x 2 below Q 90 unless
  * subsample_mode says otherwise -- 0 auto, 1 on, 2 off --, baseline, standard Huffman tables, JFIF header) for n equally sized
  * 8-bit frames of 1 or 3 bands, encoded on the device (csrc/jpeg_encode.cu): the streams are libjpeg-turbo's byte for byte

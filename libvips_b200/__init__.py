@@ -92,16 +92,25 @@ def _embedded_arrays(embedded, n):
     return keep, ptrs, lens
 
 
-def jpeg_icc_profile(stream):
-    """vips_image_get_blob(VIPS_META_ICC_NAME) of a JPEG stream (its APP2 ICC_PROFILE chunks): bytes, or None; no GPU"""
+def _icc_blob(fn, stream):
     stream = bytes(stream)
     n = C.c_size_t()
-    _check(lib().vb200_jpeg_icc_profile(stream, len(stream), None, 0, C.byref(n)))
+    _check(fn(stream, len(stream), None, 0, C.byref(n)))
     if n.value == 0:
         return None
     out = C.create_string_buffer(n.value)
-    _check(lib().vb200_jpeg_icc_profile(stream, len(stream), out, n.value, C.byref(n)))
+    _check(fn(stream, len(stream), out, n.value, C.byref(n)))
     return out.raw[:n.value]
+
+
+def jpeg_icc_profile(stream):
+    """vips_image_get_blob(VIPS_META_ICC_NAME) of a JPEG stream (its APP2 ICC_PROFILE chunks): bytes, or None; no GPU"""
+    return _icc_blob(lib().vb200_jpeg_icc_profile, stream)
+
+
+def png_icc_profile(stream):
+    """vips_image_get_blob(VIPS_META_ICC_NAME) of a PNG stream (its iCCP chunk, inflated): bytes, or None; no GPU"""
+    return _icc_blob(lib().vb200_png_icc_profile, stream)
 
 
 class JpegSaveOptions(C.Structure):
@@ -258,6 +267,15 @@ def lib():
         L.vb200_debug_dz_set_budget.argtypes = [C.c_size_t]
         L.vb200_debug_dz_pool_used.restype = C.c_size_t
         L.vb200_debug_dz_times.argtypes = [C.POINTER(C.c_float)]
+        L.vb200_png_decode_batch.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t,
+                                             PI, PI, PI]
+        L.vb200_pngload_buffer.argtypes = [C.c_void_p, C.c_size_t, IP]
+        L.vb200_png_icc_profile.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_thumbnail_plan_run_png.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_void_p, C.c_int,
+                                                   C.c_size_t]
+        L.vb200_debug_png_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_debug_inflate.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_png_set_budget.argtypes = [C.c_size_t]
         _lib = L
     return _lib
 
@@ -485,8 +503,8 @@ class Image:
                           INTENTS[intent], int(depth))
 
 
-class JpegBatch:
-    """n JPEG streams (bytes objects) as the pointer / length arrays the C ABI takes; keeps them alive."""
+class StreamBatch:
+    """n compressed streams (bytes objects: JPEG or PNG) as the pointer / length arrays the C ABI takes; keeps them alive."""
 
     def __init__(self, streams):
         self.streams = [bytes(s) for s in streams]
@@ -495,6 +513,9 @@ class JpegBatch:
         self.ptrs = (C.c_void_p * self.n)(*[C.cast(b, C.c_void_p) for b in self._bufs])
         self.lens = (C.c_size_t * self.n)(*[len(s) for s in self.streams])
         self.nbytes = sum(len(s) for s in self.streams)
+
+
+JpegBatch = StreamBatch
 
 
 def jpeg_geometry(streams, shrink=1):
@@ -530,6 +551,53 @@ def jpeg_decode_host_twin(stream, shrink=1):
     _check(lib().vb200_debug_jpeg_decode(stream, len(stream), int(shrink), out.ctypes.data_as(C.c_void_p), w.value * bands.value,
                                          C.byref(w), C.byref(h), C.byref(bands)))
     return out
+
+
+def png_geometry(streams):
+    """(width, height, bands) the PNG streams decode to (they must agree); no GPU needed"""
+    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, None, HOST, 0, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    return w.value, h.value, bands.value
+
+
+def png_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None):
+    """vips_pngload_buffer() of every stream on the device -> uint8 [n, h, w, bands] (host), or into the device pointer out_ptr
+    (packed frames unless out_bpl / out_frame_stride say otherwise)"""
+    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+    w, h, bands = png_geometry(b)
+    ww, hh, bb = C.c_int(), C.c_int(), C.c_int()
+    if out_ptr is not None:
+        bpl = out_bpl or w * bands
+        _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, bpl, out_frame_stride or bpl * h,
+                                            C.byref(ww), C.byref(hh), C.byref(bb)))
+        return w, h, bands
+    out = np.empty((b.n, h, w, bands), np.uint8)
+    _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST, w * bands, w * h * bands,
+                                        C.byref(ww), C.byref(hh), C.byref(bb)))
+    return out
+
+
+def png_decode_host_twin(stream):
+    """the decoder's per-symbol / per-byte / per-pixel code compiled for the host (vb200_debug_png_decode): what the CPU tests
+    pin to Pillow and zlib"""
+    stream = bytes(stream)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_debug_png_decode(stream, len(stream), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    out = np.empty((h.value, w.value, bands.value), np.uint8)
+    _check(lib().vb200_debug_png_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
+                                        C.byref(h), C.byref(bands)))
+    return out
+
+
+def inflate_host_twin(data, cap=1 << 24):
+    """raw deflate data (RFC 1951, no zlib header) through the PNG decoder's inflate on the host -> bytes; vb.Error when it
+    refuses the stream or the output would exceed cap bytes"""
+    data = bytes(data)
+    out = C.create_string_buffer(max(1, cap))
+    n = C.c_size_t()
+    _check(lib().vb200_debug_inflate(data, len(data), out, cap, C.byref(n)))
+    return out.raw[:n.value]
 
 
 def rank_host_twin(a, width, height, index):
@@ -731,8 +799,9 @@ def dz_pyramid_level_host_twin(image, n_from_top):
 
 def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                      builtin_profiles=None):
-    """vips_thumbnail_buffer() of a JPEG stream: shrink-on-load decode + thumbnail on the device -> uint8 array; with
-    output_profile, colour-managed with the profile the stream embeds"""
+    """vips_thumbnail_buffer() of a JPEG or PNG stream: decode (JPEG with shrink-on-load) + thumbnail on the device -> uint8
+    array; with output_profile, colour-managed with the profile the stream embeds (APP2 ICC_PROFILE or iCCP).  PNG streams
+    with eXIf are refused: their orientation would need vips_autorot"""
     stream = bytes(stream)
     out = CImage()
     out.where = HOST
@@ -751,8 +820,8 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
 
 def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                             builtin_profiles=None):
-    """vips_thumbnail_buffer(linear=TRUE) of a JPEG stream: full-size decode + linear-light thumbnail on the device, colour-managed
-    with the profile the stream embeds and / or the profiles given"""
+    """vips_thumbnail_buffer(linear=TRUE) of a JPEG or PNG stream: full-size decode + linear-light thumbnail on the device,
+    colour-managed with the profile the stream embeds and / or the profiles given.  PNG streams with eXIf are refused"""
     stream = bytes(stream)
     out = CImage()
     out.where = HOST
@@ -860,6 +929,18 @@ class ThumbnailPlan:
         out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
         _check(lib().vb200_thumbnail_plan_run_jpeg(self._p, b.ptrs, b.lens, b.n, int(shrink), out.ctypes.data_as(C.c_void_p), HOST,
                                                    self.out_frame_bytes))
+        return out
+
+    def run_png(self, streams, out_ptr=None):
+        """PNG streams decoded on the device at full size and thumbnailed by this plan (made for the decoded geometry):
+        -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
+        b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+        if out_ptr is not None:
+            _check(lib().vb200_thumbnail_plan_run_png(self._p, b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, self.out_frame_bytes))
+            return None
+        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
+        _check(lib().vb200_thumbnail_plan_run_png(self._p, b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST,
+                                                  self.out_frame_bytes))
         return out
 
     def run_host(self, frames, embedded=None):

@@ -1872,31 +1872,7 @@ stage_segment(const Segment &g, unsigned char *data, unsigned *ints, size_t int_
 	return clean;
 }
 
-/* run fn(i) for i in [0, n) on up to `threads` host threads */
-template <typename Fn>
-void
-parallel_for(int n, int threads, Fn fn)
-{
-	threads = std::max(1, std::min(threads, n));
-	if (threads == 1) {
-		for (int i = 0; i < n; i++)
-			fn(i);
-		return;
-	}
-	std::atomic<int> next(0);
-	std::vector<std::thread> pool;
-	for (int t = 0; t < threads; t++)
-		pool.emplace_back([&] {
-			for (;;) {
-				const int i = next.fetch_add(1);
-				if (i >= n)
-					return;
-				fn(i);
-			}
-		});
-	for (auto &t : pool)
-		t.join();
-}
+} // namespace
 
 int
 host_workers()
@@ -1917,6 +1893,8 @@ host_workers()
 	}();
 	return n;
 }
+
+namespace {
 
 /* the pump's slots: pinned staging, device twins and a stream each (grow-only; vb200_shutdown releases them) */
 struct JpegSlot {

@@ -396,6 +396,7 @@ vb200_shutdown(void)
 		cudaDeviceSynchronize();
 		resample_cache_clear();
 		jpeg_pump_release();
+		png_staging_release();
 	}
 	g_device.store(-1);
 }

@@ -4,10 +4,13 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <atomic>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
 #include <functional>
+#include <thread>
 #include <vector>
 
 #include "vb200.h"
@@ -210,6 +213,42 @@ void jpeg_pump_release(); /* the JPEG pump's pinned / device slots (jpeg.cu); vb
 void resample_cache_clear(); /* cached axis tables (resample_kernels.cu); vb200_shutdown */
 /* jpeg.cu: the ICC profile a JPEG stream embeds, as jpeg2vips.c:699-799 reassembles it (*len = 0: none) */
 int jpeg_icc_profile(const char *domain, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
+/* png.cu: n PNG streams of one output geometry -> out[n][h][w][bands] on the device (out = nullptr: geometry only, no
+ * device call) */
+int dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
+	int *out_w, int *out_h, int *bands, cudaStream_t s);
+bool png_signature(const void *buf, size_t len);
+/* png.cu: the iCCP profile inflated (empty: none); *exif = whether the stream has an eXIf chunk (exif may be null) */
+int png_icc_profile(const char *domain, const unsigned char *d, size_t n, std::vector<unsigned char> *profile, bool *exif);
+void png_staging_release(); /* png.cu's pinned staging; vb200_shutdown */
+
+/* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
+int host_workers();
+/* run fn(i) for i in [0, n) on up to `threads` host threads */
+template <typename Fn>
+void
+parallel_for(int n, int threads, Fn fn)
+{
+	threads = std::max(1, std::min(threads, n));
+	if (threads == 1) {
+		for (int i = 0; i < n; i++)
+			fn(i);
+		return;
+	}
+	std::atomic<int> next(0);
+	std::vector<std::thread> pool;
+	for (int t = 0; t < threads; t++)
+		pool.emplace_back([&] {
+			for (;;) {
+				const int i = next.fetch_add(1);
+				if (i >= n)
+					return;
+				fn(i);
+			}
+		});
+	for (auto &t : pool)
+		t.join();
+}
 
 /* icc.cu: the colour-management stage of the thumbnail plan (vb200_thumbnail_plan_set_icc).  Frames are 8-bit, `bands`
  * bands in, *out_bands out; each frame's input profile is chosen as vips_icc_set_import does, and one launch runs a batch.

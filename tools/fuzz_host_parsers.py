@@ -1,5 +1,6 @@
 """tools/fuzz_host_parsers.py -- mutation fuzzing of the host-side parsers that read untrusted bytes (the JPEG marker
-parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser), meant to run against an AddressSanitizer build:
+parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser, the PNG chunk walker + the PNG
+decoder's host twin with its inflate, on PNG streams and on raw deflate data), meant to run against an AddressSanitizer build:
 
     VB200_LIB=/tmp/asan/libvb200_asan.so LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \
         python tools/fuzz_host_parsers.py [seconds]
@@ -8,6 +9,7 @@ Every call must either succeed or fail with vb.Error; a crash or an ASan report 
 import io
 import sys
 import time
+import zlib
 
 import numpy as np
 from PIL import Image as PIL
@@ -30,6 +32,19 @@ def jpegs(rng):
             b = io.BytesIO()
             PIL.fromarray(a).save(b, "JPEG", quality=int(rng.integers(30, 96)), **kw)
             out.append(b.getvalue())
+    return out
+
+
+def pngs(rng):
+    out = []
+    for mode, shape, kw in (("RGB", (33, 47, 3), {}), ("RGBA", (20, 9, 4), {}), ("L", (17, 90), {}), ("LA", (5, 31, 2), {}),
+                            ("P", (29, 13), {"bits": 2}), ("P", (40, 40), {"transparency": 1}), ("L", (8, 8), {"transparency": 3}),
+                            ("RGB", (9, 9, 3), {"icc_profile": bytes(range(256)) * 2})):
+        a = rng.integers(0, 4 if mode == "P" else 256, shape, dtype=np.uint8)
+        a[: shape[0] // 2] = a[:1]
+        b = io.BytesIO()
+        PIL.fromarray(a, mode).save(b, "PNG", compress_level=int(rng.integers(0, 10)), **kw)
+        out.append(b.getvalue())
     return out
 
 
@@ -77,6 +92,8 @@ def main():
     budget = float(sys.argv[1]) if len(sys.argv) > 1 else 60.0
     rng = np.random.default_rng(int(time.time()))
     good = jpegs(rng)
+    good_png = pngs(rng)
+    deflate = [zlib.compress(s, int(rng.integers(0, 10)))[2:-4] for s in good_png]
     import icc_fixtures as F
     import test_icc as T
     profiles = [F.rgb_profile(t) for t in ("srgb", "gamma", "para4", "table")] + [F.grey_profile(), F.ink_profile(),
@@ -99,6 +116,18 @@ def main():
                 ok += 1
             except vb.Error:
                 fails += 1
+        p = mutate(rng, good_png[rng.integers(0, len(good_png))])
+        for fn in (vb.png_decode_host_twin, vb.png_icc_profile, lambda t: vb.png_geometry([t])):
+            try:
+                fn(p)
+                ok += 1
+            except vb.Error:
+                fails += 1
+        try:
+            vb.inflate_host_twin(mutate(rng, deflate[rng.integers(0, len(deflate))]), 1 << 16)
+            ok += 1
+        except vb.Error:
+            fails += 1
         if profiles:
             p = mutate(rng, profiles[rng.integers(0, len(profiles))])
             for mode in (0, 1):
