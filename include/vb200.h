@@ -611,6 +611,43 @@ int vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bu
 int vb200_debug_png_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
 int vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *out_len);
 void vb200_debug_png_set_budget(size_t bytes);
+/* ------------------------------------------------------------------ PNG save on the device
+ * vips_pngsave_buffer (foreign/spngsave.c, libspng over zlib) for uchar frames of 1-4 bands (grey, grey + alpha, RGB,
+ * RGBA): bit depth 8 (:608-613), non-interlaced, filter NONE (:714-720, :769), IHDR from the bands (:405-439), pHYs of
+ * rint(xres * 1000) pixels per metre on both axes (:455-456 reads Xres twice), iCCP named "icc" when a profile is given
+ * (:176-230), compressed at the image's level (:447-448).  The frames are deflated on the device (csrc/png_encode.cu): the
+ * zlib stream -- the IDAT payloads concatenated -- is zlib 1.3's at window bits 15 and memLevel 8 byte for byte
+ * (tests/test_png_save.py).  Chunks: signature, IHDR, iCCP, pHYs, IDATs of at most 8192 payload bytes, IEND.  Whole-file
+ * equality with libspng is not claimed: its IDAT split, its chunk order and the strategy it picks cannot be checked here.
+ *
+ * compression: zlib level (:700-705, default 6); 4-9 are built, 0-3 return -1 with the reason.  strategy: 0
+ *   Z_DEFAULT_STRATEGY (libpng's choice for unfiltered images), 1 Z_FILTERED.  xres: pixels per millimetre (libvips' Xres,
+ *   default 1.0).
+ * Declined (-1 with the reason; the host keeps spngsave): compression 0-3, another strategy, bands outside 1-4, frames over
+ *   2^28 pixels, a format other than uchar (vb200_pngsave_buffer).  Filters other than NONE, interlace, palette and
+ *   metadata chunks other than iCCP are not written.
+ * vb200_pngsave_batch: n frames of one geometry in host or device memory (frames_location); stream i at out + i *
+ *   out_stride (out_location), lengths[i] bytes (host array).  A stream that does not fit out_stride returns -1 with its
+ *   frame; with out in host memory nothing is written then, in device memory the frames of earlier chunks of a batch larger
+ *   than one chunk (vb200_debug_png_set_budget) may be.
+ * vb200_pngsave_buffer: one image; *out is malloc()ed, free() it.
+ * vb200_debug_png_encode: test hook, host only -- the whole stream through the kernels' per-position, per-symbol and
+ *   per-block code compiled for the CPU.  out = NULL only reports *len.
+ * vb200_debug_deflate: test hook, host only -- the zlib stream (header, deflate data, Adler-32) of buf[0, n) at a level
+ *   and strategy, through the same code.  out = NULL only reports *len.
+ */
+typedef struct {
+	int compression;
+	int strategy;
+	double xres;
+} VB200PngSaveOptions;
+int vb200_pngsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands,
+	const VB200PngSaveOptions *options, const void *profile, size_t profile_len, void *out, int out_location, size_t out_stride, size_t *lengths);
+int vb200_pngsave_buffer(const VB200Image *in, const VB200PngSaveOptions *options, const void *profile, size_t profile_len, void **out,
+	size_t *len);
+int vb200_debug_png_encode(const void *pixels, size_t bpl, int width, int height, int bands, const VB200PngSaveOptions *options,
+	const void *profile, size_t profile_len, void *out, size_t cap, size_t *len);
+int vb200_debug_deflate(const void *buf, size_t n, int level, int strategy, void *out, size_t cap, size_t *len);
 /* vips_jpegsave_buffer (foreign/vips2jpeg.c:551-700: jpeg_set_quality(Q, TRUE), chroma subsampled 2 x 2 below Q 90 unless
  * subsample_mode says otherwise -- 0 auto, 1 on, 2 off --, baseline, standard Huffman tables, JFIF header) for n equally sized
  * 8-bit frames of 1 or 3 bands, encoded on the device (csrc/jpeg_encode.cu): the streams are libjpeg-turbo's byte for byte

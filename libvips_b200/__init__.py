@@ -119,6 +119,18 @@ class JpegSaveOptions(C.Structure):
                 ("interlace", C.c_int)]
 
 
+class PngSaveOptions(C.Structure):
+    """VB200PngSaveOptions"""
+    _fields_ = [("compression", C.c_int), ("strategy", C.c_int), ("xres", C.c_double)]
+
+
+PNG_STRATEGIES = {"default": 0, "filtered": 1}
+
+
+def _png_options(compression, strategy, xres):
+    return PngSaveOptions(int(compression), PNG_STRATEGIES.get(strategy, strategy), float(xres))
+
+
 class DzOptions(C.Structure):
     """VB200DzOptions"""
     _fields_ = [("layout", C.c_int), ("tile_size", C.c_int), ("overlap", C.c_int), ("depth", C.c_int), ("region_shrink", C.c_int),
@@ -276,6 +288,13 @@ def lib():
         L.vb200_debug_png_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_inflate.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         L.vb200_debug_png_set_budget.argtypes = [C.c_size_t]
+        PO = C.POINTER(PngSaveOptions)
+        L.vb200_pngsave_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, PO, C.c_char_p,
+                                          C.c_size_t, C.c_void_p, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_pngsave_buffer.argtypes = [IP, PO, C.c_char_p, C.c_size_t, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
+        L.vb200_debug_png_encode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, PO, C.c_char_p, C.c_size_t, C.c_void_p,
+                                             C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_deflate.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         _lib = L
     return _lib
 
@@ -486,6 +505,18 @@ class Image:
         """vips_dzsave: the Deep Zoom / Zoomify tile pyramid of this image -> DzPyramid (see dzsave())"""
         return dzsave(self, basename, **options)
 
+    def pngsave_buffer(self, compression=6, strategy="default", xres=1.0, profile=None):
+        """vips_pngsave_buffer: this uchar image (1-4 bands) as a PNG stream (bytes), deflated on the device"""
+        cin = self._c()
+        opts = _png_options(compression, strategy, xres)
+        prof = bytes(profile) if profile else None
+        p, n = C.c_void_p(), C.c_size_t()
+        _check(lib().vb200_pngsave_buffer(C.byref(cin), C.byref(opts), prof, len(prof) if prof else 0, C.byref(p), C.byref(n)))
+        try:
+            return C.string_at(p.value, n.value)
+        finally:
+            C.CDLL(None).free(p)
+
     # ---- colour
     def colourspace(self, space, source_space=None):
         src = self if source_space is None else Image(self.array, source_space)
@@ -663,6 +694,64 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
     _check(lib().vb200_jpegsave_batch_opts(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), out.ctypes.data_as(C.c_void_p),
                                            HOST, stride, lens))
     return [out[i, :lens[i]].tobytes() for i in range(n)]
+
+
+def _png_stride(w, h, bands, profile):
+    """a slot no stream of a w x h x bands frame can overflow: fixed codes cost at most 9 bits a byte"""
+    n = h * (w * bands + 1)
+    return n + n // 8 + 400 * (n // 16383 + 2) + 12 * (n // 8192 + 2) + 2 * len(profile or b"") + 4096
+
+
+def pngsave_batch(frames, compression=6, strategy="default", xres=1.0, profile=None, in_ptr=None, shape=None, stride=None):
+    """vips_pngsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1-4) on the device -> list of bytes.
+    in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  compression 4-9; strategy "default"
+    or "filtered"; xres in pixels per millimetre; profile: ICC bytes written as iCCP.  stride: bytes per output slot."""
+    opts = _png_options(compression, strategy, xres)
+    if in_ptr is None:
+        frames = np.ascontiguousarray(frames)
+        if frames.ndim == 3:
+            frames = frames[..., None]
+        n, h, w, bands = frames.shape
+        src, where = frames.ctypes.data_as(C.c_void_p), HOST
+    else:
+        n, h, w, bands = shape
+        src, where = C.c_void_p(in_ptr), DEVICE
+    prof = bytes(profile) if profile else None
+    stride = int(stride or _png_stride(w, h, bands, prof))
+    out = np.empty((n, stride), np.uint8)
+    lens = (C.c_size_t * n)()
+    _check(lib().vb200_pngsave_batch(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), prof, len(prof) if prof else 0,
+                                     out.ctypes.data_as(C.c_void_p), HOST, stride, lens))
+    return [out[i, :lens[i]].tobytes() for i in range(n)]
+
+
+def pngsave_host_twin(a, compression=6, strategy="default", xres=1.0, profile=None):
+    """the PNG stream of one uint8 frame [h, w, bands] through the encoder's per-position, per-symbol and per-block code
+    compiled for the host (vb200_debug_png_encode); no GPU"""
+    a = np.ascontiguousarray(a)
+    if a.ndim == 2:
+        a = a[:, :, None]
+    h, w, bands = a.shape
+    opts = _png_options(compression, strategy, xres)
+    prof = bytes(profile) if profile else None
+    n = C.c_size_t()
+    args = (a.ctypes.data_as(C.c_void_p), a.strides[0], w, h, bands, C.byref(opts), prof, len(prof) if prof else 0)
+    _check(lib().vb200_debug_png_encode(*args, None, 0, C.byref(n)))
+    out = C.create_string_buffer(max(1, n.value))
+    _check(lib().vb200_debug_png_encode(*args, out, n.value, C.byref(n)))
+    return out.raw[:n.value]
+
+
+def deflate_host_twin(data, level=6, strategy="default"):
+    """the zlib stream (header, deflate data, Adler-32) of data at a level (4-9) and strategy through the PNG encoder's code on
+    the host (vb200_debug_deflate): what zlib.compressobj(level, DEFLATED, 15, 8, strategy) gives; no GPU"""
+    data = bytes(data)
+    st = PNG_STRATEGIES.get(strategy, strategy)
+    n = C.c_size_t()
+    _check(lib().vb200_debug_deflate(data, len(data), int(level), st, None, 0, C.byref(n)))
+    out = C.create_string_buffer(max(1, n.value))
+    _check(lib().vb200_debug_deflate(data, len(data), int(level), st, out, n.value, C.byref(n)))
+    return out.raw[:n.value]
 
 
 DZ_LAYOUTS = {"dz": 0, "zoomify": 1, "google": 2, "iiif": 3, "iiif3": 4}

@@ -1003,12 +1003,7 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		error(domain, "output strides too small for %d x %d x %d", W, Hh, B);
 		return -1;
 	}
-	size_t budget = g_chunk_budget;
-	if (!budget) {
-		size_t free_b = 0, total_b = 0;
-		cudaMemGetInfo(&free_b, &total_b);
-		budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
-	}
+	const size_t budget = png_chunk_budget();
 	std::lock_guard<std::mutex> lock(g_staging_lock);
 	int rc = 0;
 	for (int c0 = 0; c0 < n && !rc;) {
@@ -1298,6 +1293,19 @@ vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *
 	if (rc)
 		error("inflate (host twin)", "%s", err == ERR_MORE ? "more output than the buffer holds" : "corrupt deflate stream");
 	return rc;
+}
+
+/* device bytes per chunk of the PNG decoder and encoder */
+size_t
+vb200::png_chunk_budget()
+{
+	size_t budget = g_chunk_budget;
+	if (!budget) {
+		size_t free_b = 0, total_b = 0;
+		cudaMemGetInfo(&free_b, &total_b);
+		budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
+	}
+	return budget;
 }
 
 extern "C" void

@@ -221,6 +221,9 @@ bool png_signature(const void *buf, size_t len);
 /* png.cu: the iCCP profile inflated (empty: none); *exif = whether the stream has an eXIf chunk (exif may be null) */
 int png_icc_profile(const char *domain, const unsigned char *d, size_t n, std::vector<unsigned char> *profile, bool *exif);
 void png_staging_release(); /* png.cu's pinned staging; vb200_shutdown */
+/* png.cu: device bytes per chunk of the PNG decoder and encoder (vb200_debug_png_set_budget; 0: an eighth of the device, at
+ * least 1 GiB) */
+size_t png_chunk_budget();
 
 /* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
 int host_workers();
