@@ -568,7 +568,9 @@ int vb200_thumbnail_jpegshrink(int width, int height, int target_width, int targ
 /* vips_thumbnail_buffer(buf, len, &out, width, "height", height, "size", size, NULL) for a JPEG stream (thumbnail.c:583-613,
  * 848-902): load-time shrink by vb200_thumbnail_jpegshrink, decode and thumbnail on the device; out: allocate-or-fill.
  * A PNG stream (by its signature) decodes at full size (no load-time shrink, thumbnail.c:609-660) with its iCCP profile as
- * the embedded profile; PNGs with eXIf return -1 (their orientation would need vips_autorot). */
+ * the embedded profile; PNGs with eXIf return -1 (their orientation would need vips_autorot).  A GIF stream (GIF87a /
+ * GIF89a) loads with nsgifload's defaults (page 0, n = 1) at full size and without a profile (nsgifload attaches none):
+ * its first frame, RGB or RGBA, is an untagged input to colour management. */
 int vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size);
 int vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink,
 	void *out, int out_location, size_t out_frame_stride);
@@ -611,6 +613,37 @@ int vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bu
 int vb200_debug_png_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
 int vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *out_len);
 void vb200_debug_png_set_budget(size_t bytes);
+/* ------------------------------------------------------------------ GIF decode on the device (SURVEY 8f rank 1)
+ * vips_gifload_buffer(buf, len, &out, "page", page, "n", n, NULL) (foreign/nsgifload.c over libnsgif, fail_on = none)
+ * with LZW and frame composition on the device (csrc/gif.cu): the LZW payloads, without their sub-block length bytes, and
+ * one colour table per frame are all that crosses PCIe.  Output is uchar sRGB [n_streams][height * pages][width][bands]:
+ * page k is the screen after frames 0 .. page + k composed by libnsgif's disposal rules, 4 bands if any frame of the
+ * stream has transparency and 3 otherwise (nsgifload.c:262-280, 480-540).  n_pages = -1: every page from `page` on.
+ * Declined (-1 with the reason; the host keeps nsgifload): a scan that is not NSGIF_OK, a truncated last frame (nsgifload
+ * loads those only with a warning), no frames, screens over 65 535 on a side ("bad image dimensions") or over 2^28
+ * pixels, page / n out of range ("bad page number").  A frame with a code libnsgif refuses fails the batch.
+ *
+ * vb200_gif_geometry: nsgif_get_info after the scan: screen width and height, bands, frame count; host only.
+ * vb200_gif_decode_batch: n streams of ONE geometry (screen, bands and pages); a stream that fails fails the batch with
+ *   "stream i:" in the error, and with out in host memory nothing is written (in device memory, streams of earlier chunks
+ *   of a batch larger than one chunk may be).  out = NULL only reports the geometry (*height: all pages), without a device.
+ * vb200_gifload_buffer: one stream into a VB200Image (allocate-or-fill), height * pages rows.
+ * vb200_thumbnail_plan_run_gif: page 0 of each stream + the plan's thumbnail chain, frames never leave the device; GIF has
+ *   no load-time shrink (thumbnail.c:609-660), so the plan is made for the full screen (3 or 4 bands).
+ * vb200_debug_gif_decode / vb200_debug_lzw: test hooks, host only -- the same per-code and per-pixel code on the CPU;
+ *   vb200_debug_lzw takes joined sub-block data and decodes at most `want` values (lenient: the complex path's rule that a
+ *   bad code at a multiple of 4096 values ends the frame quietly).
+ * Chunks are bounded by vb200_debug_png_set_budget, the PNG codecs' device budget.
+ */
+int vb200_gif_geometry(const void *buf, size_t len, int *width, int *height, int *bands, int *frames);
+int vb200_gif_decode_batch(const void *const *bufs, const size_t *lens, int n, int page, int n_pages, void *out, int out_location,
+	size_t out_bpl, size_t out_frame_stride, int *width, int *height, int *bands);
+int vb200_gifload_buffer(const void *buf, size_t len, int page, int n, VB200Image *out);
+int vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out,
+	int out_location, size_t out_frame_stride);
+int vb200_debug_gif_decode(const void *buf, size_t len, int page, int n, void *out, size_t out_bpl, int *width, int *height,
+	int *bands);
+int vb200_debug_lzw(const void *data, size_t len, int min_code_size, unsigned want, int lenient, void *out, size_t *out_len);
 /* ------------------------------------------------------------------ PNG save on the device
  * vips_pngsave_buffer (foreign/spngsave.c, libspng over zlib) for uchar frames of 1-4 bands (grey, grey + alpha, RGB,
  * RGBA): bit depth 8 (:608-613), non-interlaced, filter NONE (:714-720, :769), IHDR from the bands (:405-439), pHYs of

@@ -288,6 +288,14 @@ def lib():
         L.vb200_debug_png_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_inflate.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         L.vb200_debug_png_set_budget.argtypes = [C.c_size_t]
+        L.vb200_gif_geometry.argtypes = [C.c_void_p, C.c_size_t, PI, PI, PI, PI]
+        L.vb200_gif_decode_batch.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                             C.c_size_t, C.c_size_t, PI, PI, PI]
+        L.vb200_gifload_buffer.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, IP]
+        L.vb200_thumbnail_plan_run_gif.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_void_p, C.c_int,
+                                                   C.c_size_t]
+        L.vb200_debug_gif_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_debug_lzw.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.POINTER(C.c_size_t)]
         PO = C.POINTER(PngSaveOptions)
         L.vb200_pngsave_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, PO, C.c_char_p,
                                           C.c_size_t, C.c_void_p, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -518,6 +526,19 @@ class Image:
             C.CDLL(None).free(p)
 
     # ---- colour
+    @staticmethod
+    def gifload_buffer(stream, page=0, n=1):
+        """vips_gifload_buffer(stream, page=page, n=n): the pages decoded on the device (n = -1: every page from `page` on),
+        stacked vertically as libvips does -> Image (uint8, 3 or 4 bands)"""
+        stream = bytes(stream)
+        out = CImage()
+        out.where = HOST
+        _check(lib().vb200_gifload_buffer(stream, len(stream), int(page), int(n), C.byref(out)))
+        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
+        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
+        lib().vb200_image_free(C.byref(out))
+        return Image(a, "srgb")
+
     def colourspace(self, space, source_space=None):
         src = self if source_space is None else Image(self.array, source_space)
         return src._call(lib().vb200_colourspace, _interp(space))
@@ -535,7 +556,7 @@ class Image:
 
 
 class StreamBatch:
-    """n compressed streams (bytes objects: JPEG or PNG) as the pointer / length arrays the C ABI takes; keeps them alive."""
+    """n compressed streams (bytes objects: JPEG, PNG or GIF) as the pointer / length arrays the C ABI takes; keeps them alive."""
 
     def __init__(self, streams):
         self.streams = [bytes(s) for s in streams]
@@ -619,6 +640,61 @@ def png_decode_host_twin(stream):
     _check(lib().vb200_debug_png_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
                                         C.byref(h), C.byref(bands)))
     return out
+
+
+def gif_geometry(stream):
+    """(width, height, bands, frames) of a GIF stream after libnsgif's scan (the screen, not the pages); no GPU needed"""
+    stream = bytes(stream)
+    w, h, bands, frames = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_gif_geometry(stream, len(stream), C.byref(w), C.byref(h), C.byref(bands), C.byref(frames)))
+    return w.value, h.value, bands.value, frames.value
+
+
+def _gif_batch_geometry(b, page, n):
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), None, HOST, 0, 0, C.byref(w), C.byref(h),
+                                        C.byref(bands)))
+    return w.value, h.value, bands.value
+
+
+def gif_decode_batch(streams, page=0, n=1, out_ptr=None, out_bpl=None, out_frame_stride=None):
+    """vips_gifload_buffer(page=page, n=n) of every stream on the device -> uint8 [streams, h * pages, w, bands] (host), or
+    into the device pointer out_ptr (packed unless out_bpl / out_frame_stride say otherwise)"""
+    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+    w, h, bands = _gif_batch_geometry(b, page, n)
+    ww, hh, bb = C.c_int(), C.c_int(), C.c_int()
+    if out_ptr is not None:
+        bpl = out_bpl or w * bands
+        _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), C.c_void_p(out_ptr), DEVICE, bpl,
+                                            out_frame_stride or bpl * h, C.byref(ww), C.byref(hh), C.byref(bb)))
+        return w, h, bands
+    out = np.empty((b.n, h, w, bands), np.uint8)
+    _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), out.ctypes.data_as(C.c_void_p), HOST, w * bands,
+                                        w * h * bands, C.byref(ww), C.byref(hh), C.byref(bb)))
+    return out
+
+
+def gif_decode_host_twin(stream, page=0, n=1):
+    """the decoder's per-code / per-pixel code compiled for the host (vb200_debug_gif_decode): what the CPU tests pin to
+    libnsgif -> uint8 [h * pages, w, bands]"""
+    stream = bytes(stream)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_debug_gif_decode(stream, len(stream), int(page), int(n), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    out = np.empty((h.value, w.value, bands.value), np.uint8)
+    _check(lib().vb200_debug_gif_decode(stream, len(stream), int(page), int(n), out.ctypes.data_as(C.c_void_p), w.value * bands.value,
+                                        C.byref(w), C.byref(h), C.byref(bands)))
+    return out
+
+
+def lzw_host_twin(data, min_code_size, want, lenient=False):
+    """GIF LZW data (sub-blocks joined) through the GIF decoder's LZW on the host -> at most `want` index bytes; vb.Error
+    for a code libnsgif refuses (lenient: the rule of its complex path, which takes a bad code at a multiple of 4096 values
+    as the end)"""
+    data = bytes(data)
+    out = C.create_string_buffer(max(1, int(want)))
+    n = C.c_size_t()
+    _check(lib().vb200_debug_lzw(data, len(data), int(min_code_size), int(want), int(bool(lenient)), out, C.byref(n)))
+    return out.raw[:n.value]
 
 
 def inflate_host_twin(data, cap=1 << 24):
@@ -888,9 +964,9 @@ def dz_pyramid_level_host_twin(image, n_from_top):
 
 def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                      builtin_profiles=None):
-    """vips_thumbnail_buffer() of a JPEG or PNG stream: decode (JPEG with shrink-on-load) + thumbnail on the device -> uint8
-    array; with output_profile, colour-managed with the profile the stream embeds (APP2 ICC_PROFILE or iCCP).  PNG streams
-    with eXIf are refused: their orientation would need vips_autorot"""
+    """vips_thumbnail_buffer() of a JPEG, PNG or GIF stream: decode (JPEG with shrink-on-load, GIF's first page) + thumbnail
+    on the device -> uint8 array; with output_profile, colour-managed with the profile the stream embeds (APP2 ICC_PROFILE
+    or iCCP; GIF has none).  PNG streams with eXIf are refused: their orientation would need vips_autorot"""
     stream = bytes(stream)
     out = CImage()
     out.where = HOST
@@ -909,7 +985,7 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
 
 def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                             builtin_profiles=None):
-    """vips_thumbnail_buffer(linear=TRUE) of a JPEG or PNG stream: full-size decode + linear-light thumbnail on the device,
+    """vips_thumbnail_buffer(linear=TRUE) of a JPEG, PNG or GIF stream: full-size decode + linear-light thumbnail on the device,
     colour-managed with the profile the stream embeds and / or the profiles given.  PNG streams with eXIf are refused"""
     stream = bytes(stream)
     out = CImage()
@@ -1029,6 +1105,18 @@ class ThumbnailPlan:
             return None
         out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
         _check(lib().vb200_thumbnail_plan_run_png(self._p, b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST,
+                                                  self.out_frame_bytes))
+        return out
+
+    def run_gif(self, streams, out_ptr=None):
+        """GIF streams, page 0 of each decoded on the device at full size and thumbnailed by this plan (made for the screen,
+        3 or 4 bands): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
+        b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+        if out_ptr is not None:
+            _check(lib().vb200_thumbnail_plan_run_gif(self._p, b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, self.out_frame_bytes))
+            return None
+        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
+        _check(lib().vb200_thumbnail_plan_run_gif(self._p, b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST,
                                                   self.out_frame_bytes))
         return out
 

@@ -397,6 +397,7 @@ vb200_shutdown(void)
 		resample_cache_clear();
 		jpeg_pump_release();
 		png_staging_release();
+		gif_staging_release();
 	}
 	g_device.store(-1);
 }

@@ -2410,7 +2410,7 @@ vb200_thumbnail_plan_output_bands(const VB200ThumbnailPlan *plan)
 
 /* reference: vips_thumbnail_buffer(buf, len, &out, width, "height", height, "size", size, NULL), resample/thumbnail.c:
  * 583-613 (open with the load-time shrink vips_thumbnail_find_jpegshrink picks) then :848-902 on what was loaded.
- * JPEG or PNG streams; everything between the compressed bytes and the thumbnail stays on the device.
+ * JPEG, PNG or GIF streams; everything between the compressed bytes and the thumbnail stays on the device.
  */
 extern "C" int
 vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size)
@@ -2418,14 +2418,27 @@ vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, 
 	return vb200_thumbnail_buffer_icc(buf, len, out, width, height, size, nullptr);
 }
 
-/* The streams the thumbnail entry points take: JPEG, or PNG by its signature.  The decoder and where the embedded profile
- * comes from are all that differ.  PNG has no load-time shrink (thumbnail.c:609-660 lists the loaders that do), and a PNG
- * with eXIf is declined: its orientation would need vips_autorot (thumbnail.c:989-996), which is not built.
+/* The streams the thumbnail entry points take: JPEG, or PNG / GIF by their signatures.  The decoder and where the embedded
+ * profile comes from are all that differ.  PNG and GIF have no load-time shrink (thumbnail.c:609-660 lists the loaders
+ * that do), and a PNG with eXIf is declined: its orientation would need vips_autorot (thumbnail.c:989-996), which is not
+ * built.  A GIF loads with nsgifload's defaults, page 0 and n = 1, and carries no profile.
  */
-static int
-stream_profile(const char *domain, bool png, const unsigned char *d, size_t n, std::vector<unsigned char> *profile)
+enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF };
+
+static StreamKind
+stream_kind(const void *buf, size_t len)
 {
-	if (!png)
+	return png_signature(buf, len) ? STREAM_PNG : gif_signature(buf, len) ? STREAM_GIF : STREAM_JPEG;
+}
+
+static int
+stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size_t n, std::vector<unsigned char> *profile)
+{
+	if (kind == STREAM_GIF) {
+		profile->clear();
+		return 0;
+	}
+	if (kind == STREAM_JPEG)
 		return jpeg_icc_profile(domain, d, n, profile);
 	bool exif = false;
 	if (png_icc_profile(domain, d, n, profile, &exif))
@@ -2438,11 +2451,17 @@ stream_profile(const char *domain, bool png, const unsigned char *d, size_t n, s
 }
 
 static int
-stream_decode(const char *domain, bool png, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
+stream_decode(const char *domain, StreamKind kind, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
 	size_t out_frame_stride, int *w, int *h, int *b, cudaStream_t s)
 {
-	return png ? dev_png_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, w, h, b, s)
-			   : dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, out, out_bpl, out_frame_stride, w, h, b, s);
+	switch (kind) {
+	case STREAM_PNG:
+		return dev_png_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, w, h, b, s);
+	case STREAM_GIF:
+		return dev_gif_decode_batch(domain, bufs, lens, n, 0, 1, out, out_bpl, out_frame_stride, w, h, b, s);
+	default:
+		return dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, out, out_bpl, out_frame_stride, w, h, b, s);
+	}
 }
 
 /* linear: decoded at full size (thumbnail.c:496-499) and thumbnailed by vb200_thumbnail_image_linear_icc */
@@ -2457,25 +2476,25 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 	}
 	if (ensure_init(domain))
 		return -1;
-	const bool png = png_signature(buf, len);
+	const StreamKind kind = stream_kind(buf, len);
 	const bool want_profile = icc && (icc->output_profile || linear);
 	std::vector<unsigned char> embedded;
-	if ((png || want_profile) && stream_profile(domain, png, (const unsigned char *) buf, len, &embedded))
+	if ((kind == STREAM_PNG || want_profile) && stream_profile(domain, kind, (const unsigned char *) buf, len, &embedded))
 		return -1;
 	if (!want_profile)
 		embedded.clear();
 	cudaStream_t s = current_stream();
 	int w0, h0, b0;
-	if (stream_decode(domain, png, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s))
+	if (stream_decode(domain, kind, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s))
 		return -1;
-	const int shrink = linear || png ? 1 : vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
+	const int shrink = linear || kind != STREAM_JPEG ? 1 : vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
 	int w, h, b;
-	if (stream_decode(domain, png, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s))
+	if (stream_decode(domain, kind, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s))
 		return -1;
 	DevImage dec;
 	if (dev_image_new(domain, &dec, w, h, b, VB200_FORMAT_UCHAR, b <= 2 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, s))
 		return -1;
-	int rc = stream_decode(domain, png, &buf, &len, 1, shrink, dec.data, dec.bpl, dec.bpl * h, nullptr, nullptr, nullptr, s);
+	int rc = stream_decode(domain, kind, &buf, &len, 1, shrink, dec.data, dec.bpl, dec.bpl * h, nullptr, nullptr, nullptr, s);
 	if (!rc) {
 		VB200Image din;
 		memset(&din, 0, sizeof(din));
@@ -2527,11 +2546,11 @@ vb200_thumbnail_buffer_linear_icc(const void *buf, size_t len, VB200Image *out, 
 }
 
 /* Decode staging feeding the plan (SURVEY 8f rank 1): compressed bytes up, decoded on the device (jpeg.cu at `shrink`,
- * png.cu at full size), thumbnailed by the plan's kernels -- the decoded frames never exist in host memory.  What
+ * png.cu and gif.cu at full size), thumbnailed by the plan's kernels -- the decoded frames never exist in host memory.  What
  * vips_thumbnail_buffer() does with the loader + vips_thumbnail_image (thumbnail.c:583-613, 848-902).
  */
 static int
-plan_run_streams(const char *domain, bool png, VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
+plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
 	int out_location, size_t out_frame_stride)
 {
 	if (!plan || !bufs || !lens || !out || n < 1) {
@@ -2549,11 +2568,11 @@ plan_run_streams(const char *domain, bool png, VB200ThumbnailPlan *plan, const v
 	 * stage; PNG streams are read for eXIf either way
 	 */
 	const bool managed = pl.icc || pl.licc;
-	std::vector<std::vector<unsigned char>> profiles(managed || png ? n : 0);
+	std::vector<std::vector<unsigned char>> profiles(managed || kind == STREAM_PNG ? n : 0);
 	std::vector<const void *> emb(profiles.size());
 	std::vector<size_t> emb_len(profiles.size());
 	for (size_t i = 0; i < profiles.size(); i++) {
-		if (stream_profile(domain, png, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
+		if (stream_profile(domain, kind, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
 			error(domain, "stream %d", (int) i);
 			return -1;
 		}
@@ -2568,7 +2587,7 @@ plan_run_streams(const char *domain, bool png, VB200ThumbnailPlan *plan, const v
 	int rc = -1;
 	do {
 		int w, h, b;
-		if (stream_decode(domain, png, bufs, lens, n, shrink, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, s))
+		if (stream_decode(domain, kind, bufs, lens, n, shrink, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, s))
 			break;
 		if (w != pl.W || h != pl.H || b != pl.bands) {
 			error(domain, "the plan is for %d x %d x %d frames, the streams decode to %d x %d x %d", pl.W, pl.H, pl.bands, w, h, b);
@@ -2599,14 +2618,21 @@ extern "C" int
 vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
 	int out_location, size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_jpeg", false, plan, bufs, lens, n, shrink, out, out_location, out_frame_stride);
+	return plan_run_streams("thumbnail_plan_run_jpeg", STREAM_JPEG, plan, bufs, lens, n, shrink, out, out_location, out_frame_stride);
 }
 
 extern "C" int
 vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
 	size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_png", true, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
+	return plan_run_streams("thumbnail_plan_run_png", STREAM_PNG, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
+}
+
+extern "C" int
+vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
+	size_t out_frame_stride)
+{
+	return plan_run_streams("thumbnail_plan_run_gif", STREAM_GIF, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
 }
 
 /* The tile pump: a ring of kStreams device staging slots; for each slice of

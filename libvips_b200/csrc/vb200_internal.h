@@ -224,6 +224,12 @@ void png_staging_release(); /* png.cu's pinned staging; vb200_shutdown */
 /* png.cu: device bytes per chunk of the PNG decoder and encoder (vb200_debug_png_set_budget; 0: an eighth of the device, at
  * least 1 GiB) */
 size_t png_chunk_budget();
+/* gif.cu: n GIF streams of one geometry, pages page .. page + npages - 1 (npages -1: to the last) -> out[n][h][w][bands] on
+ * the device, h the height of all pages (out = nullptr: geometry only, no device call) */
+int dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int page, int npages, void *out, size_t out_bpl,
+	size_t out_frame_stride, int *out_w, int *out_h, int *bands, cudaStream_t s);
+bool gif_signature(const void *buf, size_t len); /* GIF87a or GIF89a */
+void gif_staging_release(); /* gif.cu's pinned staging; vb200_shutdown */
 
 /* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
 int host_workers();

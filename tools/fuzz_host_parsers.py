@@ -1,5 +1,6 @@
 """tools/fuzz_host_parsers.py -- mutation fuzzing of the host-side parsers that read untrusted bytes (the JPEG marker
-parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser, the PNG chunk walker + the PNG
+parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser, the GIF block walker + the GIF
+decoder's host twin with its LZW, the PNG chunk walker + the PNG
 decoder's host twin with its inflate, on PNG streams and on raw deflate data), meant to run against an AddressSanitizer build:
 
     VB200_LIB=/tmp/asan/libvb200_asan.so LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \
@@ -88,11 +89,26 @@ def app2_mutant(rng, s):
     return s[:cut] + b"".join(segs) + s[cut:]
 
 
+def gifs(rng):
+    """GIFs written by Pillow: static and animated, with and without transparency, interlaced or not"""
+    out = []
+    for i in range(6):
+        h, w = int(rng.integers(1, 60)), int(rng.integers(1, 60))
+        ims = [PIL.fromarray(rng.integers(0, 256, (h, w, 3), dtype=np.uint8)).quantize(int(rng.integers(2, 257))) for _ in range(1 + i % 3)]
+        b = io.BytesIO()
+        kw = {"transparency": 1} if i % 2 else {}
+        ims[0].save(b, "GIF", save_all=True, append_images=ims[1:], interlace=bool(i % 4 == 3), disposal=i % 4, **kw)
+        out.append(b.getvalue())
+    return out
+
+
 def main():
     budget = float(sys.argv[1]) if len(sys.argv) > 1 else 60.0
     rng = np.random.default_rng(int(time.time()))
     good = jpegs(rng)
     good_png = pngs(rng)
+    good_gif = gifs(rng)
+    lzw = [g[g.index(b"\x2c") + 11:] for g in good_gif]  # from the minimum code size on: sub-block framing fed to the LZW as data
     deflate = [zlib.compress(s, int(rng.integers(0, 10)))[2:-4] for s in good_png]
     import icc_fixtures as F
     import test_icc as T
@@ -123,6 +139,18 @@ def main():
                 ok += 1
             except vb.Error:
                 fails += 1
+        g = mutate(rng, good_gif[rng.integers(0, len(good_gif))])
+        for fn in (vb.gif_decode_host_twin, lambda t: vb.gif_decode_host_twin(t, 0, -1), vb.gif_geometry):
+            try:
+                fn(g)
+                ok += 1
+            except vb.Error:
+                fails += 1
+        try:
+            vb.lzw_host_twin(mutate(rng, lzw[rng.integers(0, len(lzw))]), int(rng.integers(0, 13)), 1 << 14, bool(rng.integers(0, 2)))
+            ok += 1
+        except vb.Error:
+            fails += 1
         try:
             vb.inflate_host_twin(mutate(rng, deflate[rng.integers(0, len(deflate))]), 1 << 16)
             ok += 1
