@@ -644,6 +644,52 @@ int vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bu
 int vb200_debug_gif_decode(const void *buf, size_t len, int page, int n, void *out, size_t out_bpl, int *width, int *height,
 	int *bands);
 int vb200_debug_lzw(const void *data, size_t len, int min_code_size, unsigned want, int lenient, void *out, size_t *out_len);
+/* ------------------------------------------------------------------ thumbnail: page strips (animated thumbnails)
+ * vips_thumbnail of a multi-page image held as a strip: pages of page_height rows stacked vertically, with libvips'
+ * "page-height" metadata (a GIF loaded with n = -1, a multi-page TIFF, an animated WebP).  As vips_thumbnail_build does
+ * (resample/thumbnail.c:825-839, 848-861, 904-917):
+ *   - the page height is read as vips_image_get_page_height does (iofuncs/header.c:889-901): <= 0, not less than the
+ *     height, or not dividing it means one page;
+ *   - hshrink / vshrink are vips_thumbnail_calculate_shrink's for one page (width x page_height), then, with more than one
+ *     page, vshrink = height / (rint(page_height / vshrink) * n_pages) so that every page lands on whole rows;
+ *   - premultiply when there is alpha and neither adjusted shrink is 1; vips_resize(1 / hshrink, vscale = 1 / vshrink)
+ *     runs over the whole strip as one image, so shrink boxes and reduce windows straddle the page seams as in libvips;
+ *   - the result's page height is rint(page_height / vshrink), reported as vips_image_get_page_height would read it back:
+ *     the output height when it does not divide it, and for one page.
+ * With one page every entry below computes what the single-image entry computes.  Strips over 2^31 - 1 input bytes are
+ * declined (-1 with the reason).
+ *
+ * vb200_thumbnail_plan_new_pages: vb200_thumbnail_plan_new for strips of n_pages pages of page_height rows (frames of
+ *   width x page_height * n_pages); vb200_thumbnail_plan_new is the n_pages = 1 case.
+ * vb200_thumbnail_plan_page_height: the page height of the plan's output frames (vips_image_get_page_height of the result).
+ * vb200_thumbnail_image_pages: vips_thumbnail_image of a strip with page_height (0: none); icc NULL = no colour
+ *   management; linear selects vb200_thumbnail_image_linear_icc's path, otherwise vb200_thumbnail_image_icc's.
+ *   *out_page_height (may be NULL): the result's page height.
+ * vb200_thumbnail_plan_run_gif_pages: vb200_thumbnail_plan_run_gif of pages page .. page + n_pages - 1 (n_pages = -1: every
+ *   page from `page` on).  The streams of a batch share screen, bands and page count (vb200_gif_decode_batch); the plan is
+ *   made with vb200_thumbnail_plan_new_pages(screen width, screen height, pages, ...).
+ * vb200_thumbnail_buffer_pages: vips_thumbnail_buffer(..., option_string = "page=..,n=..") (thumbnail.c:1486-1490,
+ *   1585-1590), with the ICC and linear variants as vb200_thumbnail_image_pages.  A GIF loads pages page .. page + n - 1,
+ *   with page-height set only when more than one page loaded (nsgifload.c:279-280).  JPEG and PNG streams with page != 0
+ *   or n != 1 return -1: jpegload and spngload have no such options.
+ * vb200_debug_thumbnail_pages_size: test hook, host only (no GPU, no CUDA call): the shrinks, output size and output page
+ *   height vb200_thumbnail_plan_new_pages would plan.  -1: bad arguments or a plan that declines (mixed up / down).
+ *   Each entry cites thumbnail.c where its rule comes from: :825-839 (shrink), :848-861 (premultiply), :904-917 (page-height).
+ */
+VB200ThumbnailPlan *vb200_thumbnail_plan_new_pages(int width, int page_height, int n_pages, int bands, int band_format, int has_alpha,
+	int target_width, int target_height, int size, int linear);
+int vb200_thumbnail_plan_page_height(const VB200ThumbnailPlan *plan);
+int vb200_thumbnail_image_pages(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, int linear, int *out_page_height);
+int vb200_thumbnail_plan_run_gif_pages(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int page,
+	int n_pages, void *out, int out_location, size_t out_frame_stride);
+int vb200_thumbnail_buffer_pages(const void *buf, size_t len, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc, int linear, int page, int n, int *out_page_height);
+int vb200_debug_thumbnail_pages_size(int width, int page_height, int n_pages, int target_width, int target_height, int size,
+	double *hshrink, double *vshrink, int *out_width, int *out_height, int *out_page_height);
+/* test hook, host only: vb200_debug_thumbnail_kernel's kernel name for the plan vb200_thumbnail_plan_new_pages would build */
+int vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, int bands, int has_alpha, int target_width,
+	int target_height, int size, char *name, int cap);
 /* ------------------------------------------------------------------ PNG save on the device
  * vips_pngsave_buffer (foreign/spngsave.c, libspng over zlib) for uchar frames of 1-4 bands (grey, grey + alpha, RGB,
  * RGBA): bit depth 8 (:608-613), non-interlaced, filter NONE (:714-720, :769), IHDR from the bands (:405-439), pHYs of

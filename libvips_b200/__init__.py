@@ -296,6 +296,16 @@ def lib():
                                                    C.c_size_t]
         L.vb200_debug_gif_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_lzw.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.POINTER(C.c_size_t)]
+        L.vb200_thumbnail_plan_new_pages.restype = C.c_void_p
+        L.vb200_thumbnail_plan_new_pages.argtypes = [C.c_int] * 10
+        L.vb200_thumbnail_plan_page_height.argtypes = [C.c_void_p]
+        L.vb200_thumbnail_image_pages.argtypes = [IP, C.c_int, IP, C.c_int, C.c_int, C.c_int, TI, C.c_char_p, C.c_size_t, C.c_int, PI]
+        L.vb200_thumbnail_plan_run_gif_pages.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int,
+                                                         C.c_void_p, C.c_int, C.c_size_t]
+        L.vb200_thumbnail_buffer_pages.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int, TI, C.c_int, C.c_int, C.c_int, PI]
+        PD = C.POINTER(C.c_double)
+        L.vb200_debug_thumbnail_pages_size.argtypes = [C.c_int] * 6 + [PD, PD, PI, PI, PI]
+        L.vb200_debug_thumbnail_pages_kernel.argtypes = [C.c_int] * 8 + [C.c_char_p, C.c_int]
         PO = C.POINTER(PngSaveOptions)
         L.vb200_pngsave_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, PO, C.c_char_p,
                                           C.c_size_t, C.c_void_p, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -359,7 +369,7 @@ def _interp(name):
 class Image:
     """A host image (numpy array, H x W x Bands) with libvips-style operators."""
 
-    def __init__(self, array, interpretation=None):
+    def __init__(self, array, interpretation=None, page_height=None):
         a = np.ascontiguousarray(array)
         if a.ndim == 2:
             a = a[:, :, None]
@@ -369,6 +379,8 @@ class Image:
         if interpretation is None:
             interpretation = "b-w" if a.shape[2] < 3 else "srgb"
         self.interpretation = _interp(interpretation)
+        # libvips' "page-height": pages of this many rows stacked vertically (a page strip); None = one page
+        self.page_height = page_height
 
     # pyvips-style constructors / accessors
     @staticmethod
@@ -406,6 +418,10 @@ class Image:
         cin = self._c()
         cout = CImage()
         _check(fn(C.byref(cin), C.byref(cout), *args))
+        return Image._take(cout)
+
+    @staticmethod
+    def _take(cout):
         n = cout.Ysize * cout.bpl
         buf = (C.c_uint8 * n).from_address(cout.data)
         dt = DTYPES[cout.BandFmt]
@@ -447,8 +463,12 @@ class Image:
         if icc is None or linear:
             if icc is not None:
                 raise Error("linear thumbnails with an output profile are not supported on the device path")
+            if self.page_height is not None:
+                return self._thumbnail_pages(width, height, size, None, None, linear)
             return self._call(lib().vb200_thumbnail_image, int(width), int(height or 0), SIZES[size], int(linear))
         emb = bytes(embedded_profile) if embedded_profile else None
+        if self.page_height is not None:
+            return self._thumbnail_pages(width, height, size, icc, emb, False)
         return self._call(lib().vb200_thumbnail_image_icc, int(width), int(height or 0), SIZES[size], C.byref(icc), emb,
                           len(emb) if emb else 0)
 
@@ -458,8 +478,21 @@ class Image:
         at all, the bytes of thumbnail_image(linear=True)"""
         icc = linear_icc(output_profile, input_profile, intent, builtin_profiles)
         emb = bytes(embedded_profile) if embedded_profile else None
+        if self.page_height is not None:
+            return self._thumbnail_pages(width, height, size, icc, emb, True)
         return self._call(lib().vb200_thumbnail_image_linear_icc, int(width), int(height or 0), SIZES[size], C.byref(icc), emb,
                           len(emb) if emb else 0)
+
+    def _thumbnail_pages(self, width, height, size, icc, emb, linear):
+        """vb200_thumbnail_image_pages: the strip thumbnailed as vips_thumbnail does (thumbnail.c:825-839), its page height
+        set on the result (None when the result is one page)"""
+        cin, cout, oph = self._c(), CImage(), C.c_int()
+        _check(lib().vb200_thumbnail_image_pages(C.byref(cin), int(self.page_height), C.byref(cout), int(width), int(height or 0),
+                                                 SIZES[size], C.byref(icc) if icc is not None else None, emb, len(emb) if emb else 0,
+                                                 int(linear), C.byref(oph)))
+        out = Image._take(cout)
+        out.page_height = oph.value if oph.value < out.height else None
+        return out
 
     # ---- convolution
     @staticmethod
@@ -529,7 +562,8 @@ class Image:
     @staticmethod
     def gifload_buffer(stream, page=0, n=1):
         """vips_gifload_buffer(stream, page=page, n=n): the pages decoded on the device (n = -1: every page from `page` on),
-        stacked vertically as libvips does -> Image (uint8, 3 or 4 bands)"""
+        stacked vertically as libvips does -> Image (uint8, 3 or 4 bands), with page_height the screen height when more than
+        one page loaded (nsgifload.c:279-280)"""
         stream = bytes(stream)
         out = CImage()
         out.where = HOST
@@ -537,7 +571,8 @@ class Image:
         a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
         a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
         lib().vb200_image_free(C.byref(out))
-        return Image(a, "srgb")
+        screen_h = gif_geometry(stream)[1]
+        return Image(a, "srgb", page_height=screen_h if a.shape[0] > screen_h else None)
 
     def colourspace(self, space, source_space=None):
         src = self if source_space is None else Image(self.array, source_space)
@@ -962,15 +997,31 @@ def dz_pyramid_level_host_twin(image, n_from_top):
     return out
 
 
-def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
-                     builtin_profiles=None):
-    """vips_thumbnail_buffer() of a JPEG, PNG or GIF stream: decode (JPEG with shrink-on-load, GIF's first page) + thumbnail
-    on the device -> uint8 array; with output_profile, colour-managed with the profile the stream embeds (APP2 ICC_PROFILE
-    or iCCP; GIF has none).  PNG streams with eXIf are refused: their orientation would need vips_autorot"""
-    stream = bytes(stream)
+def _thumbnail_buffer_pages(stream, width, height, size, icc, linear, page, n):
+    """vb200_thumbnail_buffer_pages -> (uint8 array, page height of the result or None for one page)"""
     out = CImage()
     out.where = HOST
+    oph = C.c_int()
+    _check(lib().vb200_thumbnail_buffer_pages(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
+                                              C.byref(icc) if icc is not None else None, int(linear), int(page), int(n), C.byref(oph)))
+    a = Image._take(out).array
+    return a, (oph.value if oph.value < a.shape[0] else None)
+
+
+def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
+                     builtin_profiles=None, page=0, n=1, return_page_height=False):
+    """vips_thumbnail_buffer() of a JPEG, PNG or GIF stream: decode (JPEG with shrink-on-load, GIF's pages page .. page + n - 1,
+    n = -1 for all from page on) + thumbnail on the device -> uint8 array; with output_profile, colour-managed with the profile
+    the stream embeds (APP2 ICC_PROFILE or iCCP; GIF has none).  PNG streams with eXIf are refused: their orientation would
+    need vips_autorot.  A GIF of several pages thumbnails as a page strip; return_page_height=True returns
+    (array, page height) with None for a result of one page"""
+    stream = bytes(stream)
     icc = thumbnail_icc(output_profile, input_profile, intent, builtin_profiles)
+    if return_page_height or page != 0 or n != 1:
+        a, ph = _thumbnail_buffer_pages(stream, width, height, size, icc, False, page, n)
+        return (a, ph) if return_page_height else a
+    out = CImage()
+    out.where = HOST
     if icc is None:
         _check(lib().vb200_thumbnail_buffer(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size]))
     else:
@@ -984,13 +1035,17 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
 
 
 def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
-                            builtin_profiles=None):
+                            builtin_profiles=None, page=0, n=1, return_page_height=False):
     """vips_thumbnail_buffer(linear=TRUE) of a JPEG, PNG or GIF stream: full-size decode + linear-light thumbnail on the device,
-    colour-managed with the profile the stream embeds and / or the profiles given.  PNG streams with eXIf are refused"""
+    colour-managed with the profile the stream embeds and / or the profiles given.  PNG streams with eXIf are refused.
+    page / n / return_page_height as thumbnail_buffer"""
     stream = bytes(stream)
+    icc = linear_icc(output_profile, input_profile, intent, builtin_profiles)
+    if return_page_height or page != 0 or n != 1:
+        a, ph = _thumbnail_buffer_pages(stream, width, height, size, icc, True, page, n)
+        return (a, ph) if return_page_height else a
     out = CImage()
     out.where = HOST
-    icc = linear_icc(output_profile, input_profile, intent, builtin_profiles)
     _check(lib().vb200_thumbnail_buffer_linear_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
                                                    C.byref(icc)))
     n = out.Ysize * out.bpl
@@ -1005,22 +1060,54 @@ def thumbnail_jpegshrink(width, height, target_width, target_height=None, size="
     return int(lib().vb200_thumbnail_jpegshrink(width, height, target_width, target_height or 0, SIZES[size]))
 
 
+def thumbnail_pages_size(width, page_height, n_pages, target_width, target_height=None, size="both"):
+    """(hshrink, vshrink, out_width, out_height, out_page_height) a plan for a strip of n_pages pages computes
+    (vb200_debug_thumbnail_pages_size, no GPU needed), or None where the plan declines"""
+    hs, vs, ow, oh, oph = C.c_double(), C.c_double(), C.c_int(), C.c_int(), C.c_int()
+    if lib().vb200_debug_thumbnail_pages_size(int(width), int(page_height), int(n_pages), int(target_width), int(target_height or 0),
+                                              SIZES[size], C.byref(hs), C.byref(vs), C.byref(ow), C.byref(oh), C.byref(oph)):
+        lib().vb200_error_clear()
+        return None
+    return hs.value, vs.value, ow.value, oh.value, oph.value
+
+
+def thumbnail_pages_kernel(width, page_height, n_pages, bands, target_width, target_height=None, size="both", has_alpha=None):
+    """the kernel name (ThumbnailPlan.kernel) of the plan for a strip of n_pages pages, planned without a GPU; None where the
+    plan declines"""
+    if has_alpha is None:
+        has_alpha = bands == 2 or bands >= 4
+    name = C.create_string_buffer(256)
+    if lib().vb200_debug_thumbnail_pages_kernel(int(width), int(page_height), int(n_pages), int(bands), int(has_alpha), int(target_width),
+                                                int(target_height or 0), SIZES[size], name, 256):
+        lib().vb200_error_clear()
+        return None
+    return name.value.decode()
+
+
 class ThumbnailPlan:
     """The batched tile pump (vb200_thumbnail_plan_* in include/vb200.h)."""
 
     def __init__(self, width, height, bands=4, target_width=512, target_height=None, size="both",
-                 has_alpha=None, linear=False):
+                 has_alpha=None, linear=False, page_height=None):
+        """height: the frame's height, a whole strip of pages of page_height rows when page_height is set (read as
+        vips_image_get_page_height does: one page unless it is below height and divides it)"""
         if has_alpha is None:
             # vips_image_hasalpha for the interpretation Image() guesses: B_W below 3 bands, sRGB from 3
             has_alpha = bands == 2 or bands >= 4
         self.width, self.height, self.bands = width, height, bands
-        self._p = lib().vb200_thumbnail_plan_new(width, height, bands, 0, int(has_alpha), target_width,
-                                                 target_height or 0, SIZES[size], int(linear))
+        if page_height is not None and 0 < page_height < height and height % page_height == 0:
+            self._p = lib().vb200_thumbnail_plan_new_pages(width, page_height, height // page_height, bands, 0, int(has_alpha),
+                                                           target_width, target_height or 0, SIZES[size], int(linear))
+        else:
+            self._p = lib().vb200_thumbnail_plan_new(width, height, bands, 0, int(has_alpha), target_width,
+                                                     target_height or 0, SIZES[size], int(linear))
         if not self._p:
             _check(-1)
         ow, oh = C.c_int(), C.c_int()
         lib().vb200_thumbnail_plan_output(self._p, C.byref(ow), C.byref(oh))
         self.out_width, self.out_height = ow.value, oh.value
+        oph = int(lib().vb200_thumbnail_plan_page_height(self._p))
+        self.out_page_height = oph if oph < self.out_height else None  # None: the output is one page
         self.in_frame_bytes = width * height * bands
         self.out_bands = bands
         self.out_frame_bytes = self.out_width * self.out_height * bands
@@ -1108,16 +1195,18 @@ class ThumbnailPlan:
                                                   self.out_frame_bytes))
         return out
 
-    def run_gif(self, streams, out_ptr=None):
-        """GIF streams, page 0 of each decoded on the device at full size and thumbnailed by this plan (made for the screen,
-        3 or 4 bands): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
+    def run_gif(self, streams, out_ptr=None, page=0, n=1):
+        """GIF streams, pages page .. page + n - 1 of each (n = -1: every page from page on) decoded on the device at full size
+        and thumbnailed by this plan (made for the screen, or with page_height = the screen height for a strip of several
+        pages; 3 or 4 bands): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
         b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
         if out_ptr is not None:
-            _check(lib().vb200_thumbnail_plan_run_gif(self._p, b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, self.out_frame_bytes))
+            _check(lib().vb200_thumbnail_plan_run_gif_pages(self._p, b.ptrs, b.lens, b.n, int(page), int(n), C.c_void_p(out_ptr), DEVICE,
+                                                            self.out_frame_bytes))
             return None
         out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
-        _check(lib().vb200_thumbnail_plan_run_gif(self._p, b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST,
-                                                  self.out_frame_bytes))
+        _check(lib().vb200_thumbnail_plan_run_gif_pages(self._p, b.ptrs, b.lens, b.n, int(page), int(n), out.ctypes.data_as(C.c_void_p),
+                                                        HOST, self.out_frame_bytes))
         return out
 
     def run_host(self, frames, embedded=None):

@@ -1017,9 +1017,12 @@ struct ThumbnailPlanImpl {
 	/* request */
 	int W = 0, H = 0, bands = 0, fmt = 0, has_alpha = 0;
 	int target_w = 0, target_h = 0, size = 0, linear = 0;
+	/* a page strip: H / page_h pages of page_h rows stacked vertically; 0 = one page */
+	int page_h = 0;
 	/* derived */
 	double hshrink = 1, vshrink = 1;
 	int OW = 0, OH = 0;
+	int out_page_h = 0; /* vips_image_get_page_height of the result: OH for one page */
 	ReduceGeom gv{}, gh{};
 	bool premul = false;
 	bool fused = false;
@@ -1756,6 +1759,45 @@ rgbx_compact_kernel(const uint8_t *__restrict__ in, size_t in_stride, uint8_t *_
 
 } // namespace
 
+/* The largest page strip a plan takes, in input bytes: every kernel a plan can pick keeps its row and byte offsets in
+ * size_t, but pixel counts (alpha_hint_kernel) and the gridDim.x of the RGB expansion in 32 bits; 2^31 - 1 bytes keeps
+ * all of them far from overflow.
+ */
+constexpr size_t kMaxStripBytes = 0x7fffffff;
+
+/* vips_thumbnail_build's shrink for a page strip (thumbnail.c:825-839): vips_thumbnail_calculate_shrink of one page, then
+ * vshrink adjusted so that every page lands on a whole number of rows.  One page: the shrink of the whole frame.
+ */
+static int
+plan_page_shrink(const char *domain, ThumbnailPlanImpl *pl)
+{
+	const int ph = pl->page_h > 0 && pl->page_h < pl->H && pl->H % pl->page_h == 0 ? pl->page_h : pl->H; /* header.c:889-901 */
+	pl->page_h = ph < pl->H ? ph : 0;
+	thumbnail_shrink(pl->W, ph, pl->target_w, pl->target_h, pl->size, &pl->hshrink, &pl->vshrink);
+	if (!pl->page_h)
+		return 0;
+	if ((size_t) pl->W * pl->H * pl->bands > kMaxStripBytes) {
+		error(domain, "page strips over 2^31 - 1 bytes (%d x %d x %d) are not on the device path", pl->W, pl->H, pl->bands);
+		return -1;
+	}
+	const int n_loaded_pages = pl->H / ph; /* thumbnail.c:238-239 */
+	const int target_page_height = (int) rint(ph / pl->vshrink);
+	pl->vshrink = (double) pl->H / ((double) target_page_height * n_loaded_pages);
+	return 0;
+}
+
+/* thumbnail.c:904-917: page-height = rint(page_height / vshrink) on a result of more than one page, read back as
+ * vips_image_get_page_height does
+ */
+static int
+plan_out_page_height(const ThumbnailPlanImpl &pl)
+{
+	if (!pl.page_h)
+		return pl.OH;
+	const int oph = (int) rint(pl.page_h / pl.vshrink);
+	return oph > 0 && oph < pl.OH && pl.OH % oph == 0 ? oph : pl.OH;
+}
+
 int
 thumbnail_plan_init(const char *domain, ThumbnailPlanImpl *pl)
 {
@@ -1763,7 +1805,8 @@ thumbnail_plan_init(const char *domain, ThumbnailPlanImpl *pl)
 		error(domain, "only uchar frames are on the batched device path");
 		return -1;
 	}
-	thumbnail_shrink(pl->W, pl->H, pl->target_w, pl->target_h, pl->size, &pl->hshrink, &pl->vshrink);
+	if (plan_page_shrink(domain, pl))
+		return -1;
 	if (pl->linear && (pl->bands < 3 || pl->hshrink < 1.0 || pl->vshrink < 1.0)) {
 		error(domain, pl->bands < 3 ? "linear thumbnails on the device path need an 8-bit image with 3+ bands"
 									: "upsizing is not on the device path yet");
@@ -2214,17 +2257,27 @@ extern "C" VB200ThumbnailPlan *
 vb200_thumbnail_plan_new(int width, int height, int bands, int band_format, int has_alpha, int target_width,
 	int target_height, int size, int linear)
 {
+	return vb200_thumbnail_plan_new_pages(width, height, 1, bands, band_format, has_alpha, target_width, target_height, size, linear);
+}
+
+/* See vb200.h: a plan for strips of n_pages pages of page_height rows (thumbnail.c:825-839, 904-917) */
+extern "C" VB200ThumbnailPlan *
+vb200_thumbnail_plan_new_pages(int width, int page_height, int n_pages, int bands, int band_format, int has_alpha, int target_width,
+	int target_height, int size, int linear)
+{
 	const char *domain = "thumbnail_plan";
 	if (ensure_init(domain))
 		return nullptr;
-	if (width <= 0 || height <= 0 || bands <= 0 || target_width <= 0) {
+	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || bands <= 0 ||
+		target_width <= 0) {
 		error(domain, "bad frame geometry");
 		return nullptr;
 	}
 	auto *plan = new VB200ThumbnailPlan();
 	ThumbnailPlanImpl &pl = plan->impl;
 	pl.W = width;
-	pl.H = height;
+	pl.H = page_height * n_pages;
+	pl.page_h = n_pages > 1 ? page_height : 0;
 	pl.bands = bands;
 	pl.fmt = band_format;
 	pl.has_alpha = has_alpha;
@@ -2237,7 +2290,14 @@ vb200_thumbnail_plan_new(int width, int height, int bands, int band_format, int 
 		delete plan;
 		return nullptr;
 	}
+	pl.out_page_h = plan_out_page_height(pl);
 	return plan;
+}
+
+extern "C" int
+vb200_thumbnail_plan_page_height(const VB200ThumbnailPlan *plan)
+{
+	return plan ? plan->impl.out_page_h : -1;
 }
 
 extern "C" void
@@ -2450,24 +2510,44 @@ stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size
 	return 0;
 }
 
+/* vips_thumbnail_buffer hands its option string to the loader (thumbnail.c:1486-1490, 1585-1590): page and n are
+ * nsgifload's; jpegload and spngload have neither, so any other value fails there
+ */
+static int
+stream_pages_check(const char *domain, StreamKind kind, int page, int n_pages)
+{
+	if (kind != STREAM_GIF && (page != 0 || n_pages != 1)) {
+		error(domain, "%s has no page or n option (page %d, n %d)", kind == STREAM_PNG ? "pngload" : "jpegload", page, n_pages);
+		return -1;
+	}
+	return 0;
+}
+
+/* page / n_pages: the GIF pages to decode (a strip of screen-height pages); JPEG and PNG take 0 / 1 */
 static int
 stream_decode(const char *domain, StreamKind kind, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *w, int *h, int *b, cudaStream_t s)
+	size_t out_frame_stride, int *w, int *h, int *b, cudaStream_t s, int page = 0, int n_pages = 1)
 {
 	switch (kind) {
 	case STREAM_PNG:
 		return dev_png_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, w, h, b, s);
 	case STREAM_GIF:
-		return dev_gif_decode_batch(domain, bufs, lens, n, 0, 1, out, out_bpl, out_frame_stride, w, h, b, s);
+		return dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, out, out_bpl, out_frame_stride, w, h, b, s);
 	default:
 		return dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, out, out_bpl, out_frame_stride, w, h, b, s);
 	}
 }
 
-/* linear: decoded at full size (thumbnail.c:496-499) and thumbnailed by vb200_thumbnail_image_linear_icc */
+static int thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size, int linear,
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, bool linear_icc, int *out_page_height);
+
+/* linear: decoded at full size (thumbnail.c:496-499) and thumbnailed by vb200_thumbnail_image_linear_icc.  A GIF's pages
+ * page .. page + n - 1 decode to a strip with nsgifload's page-height, set when more than one page loaded
+ * (nsgifload.c:279-280), and are thumbnailed as one (vb200_thumbnail_image_pages).
+ */
 static int
 thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
-	bool linear)
+	bool linear, int page = 0, int n_pages = 1, int *out_page_height = nullptr)
 {
 	const char *domain = "thumbnail_buffer";
 	if (!buf || !out) {
@@ -2477,6 +2557,14 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 	if (ensure_init(domain))
 		return -1;
 	const StreamKind kind = stream_kind(buf, len);
+	if (stream_pages_check(domain, kind, page, n_pages))
+		return -1;
+	int screen_h = 0;
+	if (kind == STREAM_GIF) {
+		int sw, sb, frames;
+		if (vb200_gif_geometry(buf, len, &sw, &screen_h, &sb, &frames))
+			return -1;
+	}
 	const bool want_profile = icc && (icc->output_profile || linear);
 	std::vector<unsigned char> embedded;
 	if ((kind == STREAM_PNG || want_profile) && stream_profile(domain, kind, (const unsigned char *) buf, len, &embedded))
@@ -2485,16 +2573,17 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 		embedded.clear();
 	cudaStream_t s = current_stream();
 	int w0, h0, b0;
-	if (stream_decode(domain, kind, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s))
+	if (stream_decode(domain, kind, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s, page, n_pages))
 		return -1;
 	const int shrink = linear || kind != STREAM_JPEG ? 1 : vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
 	int w, h, b;
-	if (stream_decode(domain, kind, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s))
+	if (stream_decode(domain, kind, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s, page, n_pages))
 		return -1;
+	const int page_height = kind == STREAM_GIF && h > screen_h ? screen_h : 0;
 	DevImage dec;
 	if (dev_image_new(domain, &dec, w, h, b, VB200_FORMAT_UCHAR, b <= 2 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, s))
 		return -1;
-	int rc = stream_decode(domain, kind, &buf, &len, 1, shrink, dec.data, dec.bpl, dec.bpl * h, nullptr, nullptr, nullptr, s);
+	int rc = stream_decode(domain, kind, &buf, &len, 1, shrink, dec.data, dec.bpl, dec.bpl * h, nullptr, nullptr, nullptr, s, page, n_pages);
 	if (!rc) {
 		VB200Image din;
 		memset(&din, 0, sizeof(din));
@@ -2510,8 +2599,8 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 		VB200Image tmp;
 		memset(&tmp, 0, sizeof(tmp));
 		tmp.where = VB200_DEVICE;
-		rc = linear ? vb200_thumbnail_image_linear_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size())
-					: vb200_thumbnail_image_icc(&din, &tmp, width, height, size, icc, embedded.data(), embedded.size());
+		rc = thumbnail_image_run(&din, page_height, &tmp, width, height, size, linear, icc, embedded.data(), embedded.size(), linear,
+			out_page_height);
 		if (!rc) {
 			/* deliver where the caller asked (allocate-or-fill) */
 			DevImage dt;
@@ -2545,13 +2634,21 @@ vb200_thumbnail_buffer_linear_icc(const void *buf, size_t len, VB200Image *out, 
 	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, true);
 }
 
+/* See vb200.h: vips_thumbnail_buffer(..., option_string = "page=..,n=..") */
+extern "C" int
+vb200_thumbnail_buffer_pages(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	int linear, int page, int n, int *out_page_height)
+{
+	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, linear != 0, page, n, out_page_height);
+}
+
 /* Decode staging feeding the plan (SURVEY 8f rank 1): compressed bytes up, decoded on the device (jpeg.cu at `shrink`,
  * png.cu and gif.cu at full size), thumbnailed by the plan's kernels -- the decoded frames never exist in host memory.  What
  * vips_thumbnail_buffer() does with the loader + vips_thumbnail_image (thumbnail.c:583-613, 848-902).
  */
 static int
 plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
-	int out_location, size_t out_frame_stride)
+	int out_location, size_t out_frame_stride, int page = 0, int n_pages = 1)
 {
 	if (!plan || !bufs || !lens || !out || n < 1) {
 		error(domain, "null argument");
@@ -2560,6 +2657,16 @@ plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, 
 	if (ensure_init(domain))
 		return -1;
 	ThumbnailPlanImpl &pl = plan->impl;
+	if (kind == STREAM_GIF) {
+		/* the decoded strip is pl.H rows only if its pages are the plan's: the screen must be one page high */
+		int sw, sh, sb, frames;
+		if (vb200_gif_geometry(bufs[0], lens[0], &sw, &sh, &sb, &frames))
+			return -1;
+		if (sh != (pl.page_h ? pl.page_h : pl.H)) {
+			error(domain, "the plan is for pages of %d rows, the streams' screen is %d rows", pl.page_h ? pl.page_h : pl.H, sh);
+			return -1;
+		}
+	}
 	cudaStream_t s = current_stream();
 	const size_t in_frame = (size_t) pl.W * pl.H * pl.bands, out_frame = (size_t) pl.OW * pl.OH * pl.out_bands();
 	if (out_frame_stride == 0)
@@ -2587,7 +2694,7 @@ plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, 
 	int rc = -1;
 	do {
 		int w, h, b;
-		if (stream_decode(domain, kind, bufs, lens, n, shrink, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, s))
+		if (stream_decode(domain, kind, bufs, lens, n, shrink, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, s, page, n_pages))
 			break;
 		if (w != pl.W || h != pl.H || b != pl.bands) {
 			error(domain, "the plan is for %d x %d x %d frames, the streams decode to %d x %d x %d", pl.W, pl.H, pl.bands, w, h, b);
@@ -2633,6 +2740,14 @@ vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bufs, 
 	size_t out_frame_stride)
 {
 	return plan_run_streams("thumbnail_plan_run_gif", STREAM_GIF, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
+}
+
+extern "C" int
+vb200_thumbnail_plan_run_gif_pages(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int page, int n_pages,
+	void *out, int out_location, size_t out_frame_stride)
+{
+	return plan_run_streams("thumbnail_plan_run_gif", STREAM_GIF, plan, bufs, lens, n, 1, out, out_location, out_frame_stride, page,
+		n_pages);
 }
 
 /* The tile pump: a ring of kStreams device staging slots; for each slice of
@@ -2715,11 +2830,12 @@ vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t 
 }
 
 /* vips_thumbnail_image, with colour management when icc sets an output profile; linear_icc: linear = TRUE with icc (may be NULL)
- * through vb200_thumbnail_plan_set_linear_icc
+ * through vb200_thumbnail_plan_set_linear_icc.  page_height: the input's page-height metadata (0: none), read as
+ * vips_image_get_page_height does; out_page_height (may be NULL) gets the result's.
  */
 static int
-thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear, const VB200ThumbnailIcc *icc,
-	const void *embedded, size_t embedded_len, bool linear_icc = false)
+thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size, int linear,
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, bool linear_icc, int *out_page_height)
 {
 	const char *domain = "thumbnail";
 	if (!in || !out) {
@@ -2760,10 +2876,13 @@ thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height
 	}
 	/* vips_image_hasalpha(): more bands than the interpretation implies (iofuncs/image.c:3113-3119) */
 	const int has_alpha = image_hasalpha(in->Type, in->Bands);
-	VB200ThumbnailPlan *plan = vb200_thumbnail_plan_new(in->Xsize, in->Ysize, in->Bands, in->BandFmt, has_alpha, width,
+	const int ph = page_height > 0 && page_height < in->Ysize && in->Ysize % page_height == 0 ? page_height : in->Ysize; /* header.c:889-901 */
+	VB200ThumbnailPlan *plan = vb200_thumbnail_plan_new_pages(in->Xsize, ph, ph > 0 ? in->Ysize / ph : 1, in->Bands, in->BandFmt, has_alpha, width,
 		height, size, linear);
 	if (!plan)
 		return -1;
+	if (out_page_height)
+		*out_page_height = plan->impl.out_page_h;
 	if (icc && (linear_icc ? vb200_thumbnail_plan_set_linear_icc(plan, icc) : vb200_thumbnail_plan_set_icc(plan, icc))) {
 		vb200_thumbnail_plan_free(plan);
 		return -1;
@@ -2802,7 +2921,7 @@ thumbnail_image_run(const VB200Image *in, VB200Image *out, int width, int height
 extern "C" int
 vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear)
 {
-	return thumbnail_image_run(in, out, width, height, size, linear, nullptr, nullptr, 0);
+	return thumbnail_image_run(in, 0, out, width, height, size, linear, nullptr, nullptr, 0, false, nullptr);
 }
 
 /* vips_thumbnail_image with "input_profile" / "output_profile" / "intent"; `embedded`: the image's ICC blob */
@@ -2810,7 +2929,16 @@ extern "C" int
 vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
 	const void *embedded, size_t embedded_len)
 {
-	return thumbnail_image_run(in, out, width, height, size, 0, icc, embedded, embedded_len);
+	return thumbnail_image_run(in, 0, out, width, height, size, 0, icc, embedded, embedded_len, false, nullptr);
+}
+
+/* See vb200.h: vips_thumbnail_image of a page strip (thumbnail.c:825-839, 904-917) */
+extern "C" int
+vb200_thumbnail_image_pages(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size,
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, int linear, int *out_page_height)
+{
+	return thumbnail_image_run(in, page_height, out, width, height, size, linear != 0, icc, embedded, embedded_len, linear != 0,
+		out_page_height);
 }
 
 /* vips_thumbnail_image(..., linear = TRUE) with "input_profile" / "output_profile" / "intent" (thumbnail.c:766-805, 929-987):
@@ -2820,7 +2948,7 @@ extern "C" int
 vb200_thumbnail_image_linear_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
 	const void *embedded, size_t embedded_len)
 {
-	return thumbnail_image_run(in, out, width, height, size, 1, icc, embedded, embedded_len, true);
+	return thumbnail_image_run(in, 0, out, width, height, size, 1, icc, embedded, embedded_len, true, nullptr);
 }
 
 /* Test hook (tests/test_thumbnail_bands.py, CPU): the tensor-pipe kernel's bands of an RGBA thumbnail plan, planned
@@ -2870,11 +2998,23 @@ extern "C" int
 vb200_debug_thumbnail_kernel(int width, int height, int bands, int has_alpha, int target_width, int target_height, int size,
 	char *name, int cap)
 {
-	if (width <= 0 || height <= 0 || bands <= 0 || target_width <= 0 || !name || cap <= 0)
+	return vb200_debug_thumbnail_pages_kernel(width, height, 1, bands, has_alpha, target_width, target_height, size, name, cap);
+}
+
+/* Test hook (tests/test_thumbnail_pages.py, CPU): vb200_debug_thumbnail_kernel for the plan vb200_thumbnail_plan_new_pages
+ * would build.  See vb200.h.
+ */
+extern "C" int
+vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, int bands, int has_alpha, int target_width,
+	int target_height, int size, char *name, int cap)
+{
+	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || bands <= 0 ||
+		target_width <= 0 || !name || cap <= 0)
 		return -1;
 	ThumbnailPlanImpl pl;
 	pl.W = width;
-	pl.H = height;
+	pl.H = page_height * n_pages;
+	pl.page_h = n_pages > 1 ? page_height : 0;
 	pl.bands = bands;
 	pl.fmt = VB200_FORMAT_UCHAR;
 	pl.has_alpha = has_alpha;
@@ -2889,5 +3029,34 @@ vb200_debug_thumbnail_kernel(int width, int height, int bands, int has_alpha, in
 	if ((int) strlen(k) >= cap)
 		return -1;
 	strcpy(name, k);
+	return 0;
+}
+
+/* Test hook (tests/test_thumbnail_pages.py, CPU): the shrinks, output size and output page height of the plan
+ * vb200_thumbnail_plan_new_pages would build, planned without a device.  See vb200.h.
+ */
+extern "C" int
+vb200_debug_thumbnail_pages_size(int width, int page_height, int n_pages, int target_width, int target_height, int size, double *hshrink,
+	double *vshrink, int *out_width, int *out_height, int *out_page_height)
+{
+	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || target_width <= 0)
+		return -1;
+	ThumbnailPlanImpl pl;
+	pl.W = width;
+	pl.H = page_height * n_pages;
+	pl.page_h = n_pages > 1 ? page_height : 0;
+	pl.bands = 1;
+	pl.fmt = VB200_FORMAT_UCHAR;
+	pl.target_w = target_width;
+	pl.target_h = target_height > 0 ? target_height : target_width;
+	pl.size = size;
+	pl.geometry_only = true;
+	if (thumbnail_plan_init("debug_thumbnail_pages_size", &pl))
+		return -1;
+	*hshrink = pl.hshrink;
+	*vshrink = pl.vshrink;
+	*out_width = pl.OW;
+	*out_height = pl.OH;
+	*out_page_height = plan_out_page_height(pl);
 	return 0;
 }
