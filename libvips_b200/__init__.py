@@ -605,28 +605,37 @@ class StreamBatch:
 JpegBatch = StreamBatch
 
 
+def _batch_geometry(fn, streams, *opts):
+    """(width, height, bands) vb200_*_decode_batch(streams, *opts) reports without an output (the streams must agree); no GPU"""
+    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(fn(b.ptrs, b.lens, b.n, *opts, None, HOST, 0, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    return w.value, h.value, bands.value
+
+
+def _decode_batch(fn, streams, opts, out_ptr, out_bpl=None, out_frame_stride=None):
+    """vb200_*_decode_batch(streams, *opts) -> uint8 [n, h, w, bands] (host), or into the device pointer out_ptr (packed
+    frames unless out_bpl / out_frame_stride say otherwise) -> (w, h, bands)"""
+    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+    w, h, bands = _batch_geometry(fn, b, *opts)
+    if out_ptr is not None:
+        bpl = out_bpl or w * bands
+        _check(fn(b.ptrs, b.lens, b.n, *opts, C.c_void_p(out_ptr), DEVICE, bpl, out_frame_stride or bpl * h, None, None, None))
+        return w, h, bands
+    out = np.empty((b.n, h, w, bands), np.uint8)
+    _check(fn(b.ptrs, b.lens, b.n, *opts, out.ctypes.data_as(C.c_void_p), HOST, w * bands, w * h * bands, None, None, None))
+    return out
+
+
 def jpeg_geometry(streams, shrink=1):
     """(width, height, bands) the streams decode to at `shrink` (they must agree); no GPU needed"""
-    b = streams if isinstance(streams, JpegBatch) else JpegBatch(streams)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_jpeg_decode_batch(b.ptrs, b.lens, b.n, int(shrink), None, HOST, 0, 0, C.byref(w), C.byref(h), C.byref(bands)))
-    return w.value, h.value, bands.value
+    return _batch_geometry(lib().vb200_jpeg_decode_batch, streams, int(shrink))
 
 
 def jpeg_decode_batch(streams, shrink=1, out_ptr=None):
     """vips_jpegload_buffer(..., shrink=shrink) of every stream on the device -> uint8 [n, h, w, bands] (host),
     or into the device pointer out_ptr (packed frames)"""
-    b = streams if isinstance(streams, JpegBatch) else JpegBatch(streams)
-    w, h, bands = jpeg_geometry(b, shrink)
-    ww, hh, bb = C.c_int(), C.c_int(), C.c_int()
-    if out_ptr is not None:
-        _check(lib().vb200_jpeg_decode_batch(b.ptrs, b.lens, b.n, int(shrink), C.c_void_p(out_ptr), DEVICE, w * bands, w * h * bands,
-                                             C.byref(ww), C.byref(hh), C.byref(bb)))
-        return w, h, bands
-    out = np.empty((b.n, h, w, bands), np.uint8)
-    _check(lib().vb200_jpeg_decode_batch(b.ptrs, b.lens, b.n, int(shrink), out.ctypes.data_as(C.c_void_p), HOST, w * bands,
-                                         w * h * bands, C.byref(ww), C.byref(hh), C.byref(bb)))
-    return out
+    return _decode_batch(lib().vb200_jpeg_decode_batch, streams, (int(shrink),), out_ptr)
 
 
 def jpeg_decode_host_twin(stream, shrink=1):
@@ -642,27 +651,13 @@ def jpeg_decode_host_twin(stream, shrink=1):
 
 def png_geometry(streams):
     """(width, height, bands) the PNG streams decode to (they must agree); no GPU needed"""
-    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, None, HOST, 0, 0, C.byref(w), C.byref(h), C.byref(bands)))
-    return w.value, h.value, bands.value
+    return _batch_geometry(lib().vb200_png_decode_batch, streams)
 
 
 def png_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None):
     """vips_pngload_buffer() of every stream on the device -> uint8 [n, h, w, bands] (host), or into the device pointer out_ptr
     (packed frames unless out_bpl / out_frame_stride say otherwise)"""
-    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
-    w, h, bands = png_geometry(b)
-    ww, hh, bb = C.c_int(), C.c_int(), C.c_int()
-    if out_ptr is not None:
-        bpl = out_bpl or w * bands
-        _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, bpl, out_frame_stride or bpl * h,
-                                            C.byref(ww), C.byref(hh), C.byref(bb)))
-        return w, h, bands
-    out = np.empty((b.n, h, w, bands), np.uint8)
-    _check(lib().vb200_png_decode_batch(b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST, w * bands, w * h * bands,
-                                        C.byref(ww), C.byref(hh), C.byref(bb)))
-    return out
+    return _decode_batch(lib().vb200_png_decode_batch, streams, (), out_ptr, out_bpl, out_frame_stride)
 
 
 def png_decode_host_twin(stream):
@@ -686,27 +681,13 @@ def gif_geometry(stream):
 
 
 def _gif_batch_geometry(b, page, n):
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), None, HOST, 0, 0, C.byref(w), C.byref(h),
-                                        C.byref(bands)))
-    return w.value, h.value, bands.value
+    return _batch_geometry(lib().vb200_gif_decode_batch, b, int(page), int(n))
 
 
 def gif_decode_batch(streams, page=0, n=1, out_ptr=None, out_bpl=None, out_frame_stride=None):
     """vips_gifload_buffer(page=page, n=n) of every stream on the device -> uint8 [streams, h * pages, w, bands] (host), or
     into the device pointer out_ptr (packed unless out_bpl / out_frame_stride say otherwise)"""
-    b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
-    w, h, bands = _gif_batch_geometry(b, page, n)
-    ww, hh, bb = C.c_int(), C.c_int(), C.c_int()
-    if out_ptr is not None:
-        bpl = out_bpl or w * bands
-        _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), C.c_void_p(out_ptr), DEVICE, bpl,
-                                            out_frame_stride or bpl * h, C.byref(ww), C.byref(hh), C.byref(bb)))
-        return w, h, bands
-    out = np.empty((b.n, h, w, bands), np.uint8)
-    _check(lib().vb200_gif_decode_batch(b.ptrs, b.lens, b.n, int(page), int(n), out.ctypes.data_as(C.c_void_p), HOST, w * bands,
-                                        w * h * bands, C.byref(ww), C.byref(hh), C.byref(bb)))
-    return out
+    return _decode_batch(lib().vb200_gif_decode_batch, streams, (int(page), int(n)), out_ptr, out_bpl, out_frame_stride)
 
 
 def gif_decode_host_twin(stream, page=0, n=1):
@@ -1027,11 +1008,7 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
     else:
         _check(lib().vb200_thumbnail_buffer_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
                                                 C.byref(icc)))
-    n = out.Ysize * out.bpl
-    a = np.frombuffer(C.string_at(out.data, n), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
-    a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
-    lib().vb200_image_free(C.byref(out))
-    return a
+    return Image._take(out).array
 
 
 def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
@@ -1048,11 +1025,7 @@ def thumbnail_buffer_linear(stream, width, height=None, size="both", output_prof
     out.where = HOST
     _check(lib().vb200_thumbnail_buffer_linear_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
                                                    C.byref(icc)))
-    n = out.Ysize * out.bpl
-    a = np.frombuffer(C.string_at(out.data, n), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
-    a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
-    lib().vb200_image_free(C.byref(out))
-    return a
+    return Image._take(out).array
 
 
 def thumbnail_jpegshrink(width, height, target_width, target_height=None, size="both"):
@@ -1170,44 +1143,30 @@ class ThumbnailPlan:
         _check(lib().vb200_thumbnail_batch_host_icc(self._p, C.c_void_p(in_ptr), self.in_frame_bytes, C.c_void_p(out_ptr),
                                                     self.out_frame_bytes, n_frames, ptrs, lens))
 
+    def _run_streams(self, fn, streams, opts, out_ptr):
+        b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
+        if out_ptr is not None:
+            _check(fn(self._p, b.ptrs, b.lens, b.n, *opts, C.c_void_p(out_ptr), DEVICE, self.out_frame_bytes))
+            return None
+        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
+        _check(fn(self._p, b.ptrs, b.lens, b.n, *opts, out.ctypes.data_as(C.c_void_p), HOST, self.out_frame_bytes))
+        return out
+
     def run_jpeg(self, streams, shrink, out_ptr=None):
         """JPEG streams decoded at `shrink` on the device and thumbnailed by this plan (made for the decoded
         geometry): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
-        b = streams if isinstance(streams, JpegBatch) else JpegBatch(streams)
-        if out_ptr is not None:
-            _check(lib().vb200_thumbnail_plan_run_jpeg(self._p, b.ptrs, b.lens, b.n, int(shrink), C.c_void_p(out_ptr), DEVICE,
-                                                       self.out_frame_bytes))
-            return None
-        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
-        _check(lib().vb200_thumbnail_plan_run_jpeg(self._p, b.ptrs, b.lens, b.n, int(shrink), out.ctypes.data_as(C.c_void_p), HOST,
-                                                   self.out_frame_bytes))
-        return out
+        return self._run_streams(lib().vb200_thumbnail_plan_run_jpeg, streams, (int(shrink),), out_ptr)
 
     def run_png(self, streams, out_ptr=None):
         """PNG streams decoded on the device at full size and thumbnailed by this plan (made for the decoded geometry):
         -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
-        b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
-        if out_ptr is not None:
-            _check(lib().vb200_thumbnail_plan_run_png(self._p, b.ptrs, b.lens, b.n, C.c_void_p(out_ptr), DEVICE, self.out_frame_bytes))
-            return None
-        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
-        _check(lib().vb200_thumbnail_plan_run_png(self._p, b.ptrs, b.lens, b.n, out.ctypes.data_as(C.c_void_p), HOST,
-                                                  self.out_frame_bytes))
-        return out
+        return self._run_streams(lib().vb200_thumbnail_plan_run_png, streams, (), out_ptr)
 
     def run_gif(self, streams, out_ptr=None, page=0, n=1):
         """GIF streams, pages page .. page + n - 1 of each (n = -1: every page from page on) decoded on the device at full size
         and thumbnailed by this plan (made for the screen, or with page_height = the screen height for a strip of several
         pages; 3 or 4 bands): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
-        b = streams if isinstance(streams, StreamBatch) else StreamBatch(streams)
-        if out_ptr is not None:
-            _check(lib().vb200_thumbnail_plan_run_gif_pages(self._p, b.ptrs, b.lens, b.n, int(page), int(n), C.c_void_p(out_ptr), DEVICE,
-                                                            self.out_frame_bytes))
-            return None
-        out = np.empty((b.n, self.out_height, self.out_width, self.out_bands), np.uint8)
-        _check(lib().vb200_thumbnail_plan_run_gif_pages(self._p, b.ptrs, b.lens, b.n, int(page), int(n), out.ctypes.data_as(C.c_void_p),
-                                                        HOST, self.out_frame_bytes))
-        return out
+        return self._run_streams(lib().vb200_thumbnail_plan_run_gif_pages, streams, (int(page), int(n)), out_ptr)
 
     def run_host(self, frames, embedded=None):
         """frames: uint8 array [n, H, W, bands] in host memory -> [n, OH, OW, out_bands]."""

@@ -43,8 +43,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <exception>
-#include <mutex>
-#include <string>
 #include <vector>
 
 #include "../../include/vb200.h"
@@ -688,12 +686,6 @@ stage_palettes(const GifInfo &G, int nf, unsigned *pals)
 	}
 }
 
-size_t
-align16(size_t v)
-{
-	return (v + 15) & ~(size_t) 15;
-}
-
 /* device bytes a stream takes in a chunk: per frame its record, table, payload and index plane */
 size_t
 stream_device_bytes(const GifInfo &G, int nf)
@@ -706,39 +698,7 @@ stream_device_bytes(const GifInfo &G, int nf)
 	return b;
 }
 
-struct GifStaging {
-	void *pinned = nullptr;
-	size_t cap = 0;
-	void release()
-	{
-		if (pinned)
-			cudaFreeHost(pinned);
-		pinned = nullptr;
-		cap = 0;
-	}
-};
-GifStaging g_staging;
-std::mutex g_staging_lock;
-
-std::string
-worker_error()
-{
-	/* the worker's thread-local "domain: reason\n", without the domain (restated with the stream's index) */
-	std::string e = vb200_error_buffer();
-	vb200_error_clear();
-	const size_t at = e.find(": ");
-	e = e.substr(at == std::string::npos ? 0 : at + 2);
-	return e.substr(0, e.find('\n'));
-}
-
 } // namespace
-
-void
-gif_staging_release()
-{
-	std::lock_guard<std::mutex> lock(g_staging_lock);
-	g_staging.release();
-}
 
 bool
 gif_signature(const void *buf, size_t len)
@@ -747,68 +707,30 @@ gif_signature(const void *buf, size_t len)
 }
 
 /* Decode n GIF streams (host memory) of one output geometry into out[n][h * pages][w][bands] on the device (out = nullptr:
- * only report the geometry; *out_h is the height of all pages).  Streams are walked on the host workers; they go up in
- * chunks bounded by png_chunk_budget(), each one pinned block (stream and frame records, tables, LZW payloads) copied to
- * the device.  Every frame of a chunk must decode clean before its pixels are composed into out.
+ * only report the geometry).  Streams are walked on the host workers; they go up in chunks bounded by
+ * decode_chunk_budget(), each one pinned block (stream and frame records, tables, LZW payloads) copied to the device.
+ * Every frame of a chunk must decode clean before its pixels are composed into out.
  */
 int
 dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int page, int npages, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *out_w, int *out_h, int *out_bands, cudaStream_t s)
+	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s)
 {
-	if (n < 1 || !bufs || !lens) {
-		error(domain, "no streams");
-		return -1;
-	}
 	std::vector<GifInfo> info(n);
 	std::vector<int> pages(n, 0);
-	std::vector<std::string> errs(n);
-	parallel_for(n, host_workers(), [&](int i) {
-		if (parse_gif(domain, (const unsigned char *) bufs[i], lens[i], &info[i]) || resolve_pages(domain, info[i], page, npages, &pages[i]))
-			errs[i] = worker_error();
-	});
-	for (int i = 0; i < n; i++)
-		if (!errs[i].empty()) {
-			error(domain, "stream %d: %s", i, errs[i].c_str());
-			return -1;
-		}
-	const int W = info[0].W, H = info[0].H, B = info[0].bands, P = pages[0];
-	for (int i = 1; i < n; i++)
-		if (info[i].W != W || info[i].H != H || info[i].bands != B || pages[i] != P) {
-			error(domain, "streams of a batch must decode to one geometry (%d x %d x %d, %d pages; stream %d: %d x %d x %d, %d pages)", W, H, B, P, i,
-				info[i].W, info[i].H, info[i].bands, pages[i]);
-			return -1;
-		}
-	if (out_w)
-		*out_w = W;
-	if (out_h)
-		*out_h = H * P;
-	if (out_bands)
-		*out_bands = B;
+	if (parse_streams(
+			domain, "stream", n,
+			[&](int i) {
+				return parse_gif(domain, (const unsigned char *) bufs[i], lens[i], &info[i]) || resolve_pages(domain, info[i], page, npages, &pages[i]) ? -1 : 0;
+			},
+			[&](int i) { return StreamGeometry{info[i].W, info[i].H, info[i].bands, pages[i]}; }, g))
+		return -1;
 	if (!out)
 		return 0;
-	if (out_bpl < (size_t) W * B || (n > 1 && out_frame_stride < out_bpl * H * P)) {
-		error(domain, "output strides too small for %d x %d x %d", W, H * P, B);
+	if (check_out_strides(domain, *g, out_bpl, out_frame_stride))
 		return -1;
-	}
-	const int nf_stream = page + P; /* frames 0 .. page + n - 1 of every stream */
-	const size_t budget = png_chunk_budget();
-	std::lock_guard<std::mutex> lock(g_staging_lock);
-	int rc = 0;
-	for (int c0 = 0; c0 < n && !rc;) {
-		size_t dev_bytes = 0;
-		int cn = 0;
-		while (c0 + cn < n && cn < kMaxBatchFrames) {
-			const size_t b = stream_device_bytes(info[c0 + cn], nf_stream);
-			if (cn > 0 && dev_bytes + b > budget)
-				break;
-			dev_bytes += b;
-			cn++;
-		}
-		if (dev_bytes > budget) {
-			error(domain, "stream %d needs %zu bytes of device memory, more than the %zu allowed", c0, dev_bytes, budget);
-			rc = -1;
-			break;
-		}
+	const int W = g->w, H = g->h, B = g->bands;
+	const int nf_stream = page + g->pages; /* frames 0 .. page + n - 1 of every stream */
+	int rc = decode_chunks(domain, "stream", n, [&](int i) { return stream_device_bytes(info[i], nf_stream); }, [&](int c0, int cn) {
 		/* records and offsets: the pinned block holds stream records, frame records, tables and payloads; the device the
 		 * same, then the index planes, counts and status words
 		 */
@@ -833,16 +755,10 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		}
 		const size_t off_fr = align16(cn * sizeof(GifStreamDev)), off_pal = off_fr + align16(nf * sizeof(GifFrameDev)),
 					 off_data = off_pal + (size_t) nf * 1024, total = off_data + data;
-		if (g_staging.cap < total) {
-			g_staging.release();
-			if (cudaMallocHost(&g_staging.pinned, total + total / 4) != cudaSuccess) {
-				rc = cuda_fail(domain, cudaGetLastError(), "cudaMallocHost (gif staging)");
-				break;
-			}
-			g_staging.cap = total + total / 4;
-		}
 		/* the previous chunk's copy out of the block has finished: its status was read after it */
-		unsigned char *hst = (unsigned char *) g_staging.pinned;
+		unsigned char *hst = (unsigned char *) decode_staging(domain, total);
+		if (!hst)
+			return -1;
 		memcpy(hst, S.data(), cn * sizeof(GifStreamDev));
 		memcpy(hst + off_fr, F.data(), nf * sizeof(GifFrameDev));
 		parallel_for(cn, host_workers(), [&](int i) {
@@ -853,10 +769,8 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		});
 		const size_t off_planes = align16(total), off_counts = off_planes + align16(planes), off_status = off_counts + align16(nf * sizeof(unsigned));
 		void *dev = nullptr;
-		if (dev_alloc(domain, &dev, off_status + nf * sizeof(int), s)) {
-			rc = -1;
-			break;
-		}
+		if (dev_alloc(domain, &dev, off_status + nf * sizeof(int), s))
+			return -1;
 		unsigned char *dv = (unsigned char *) dev;
 		const GifStreamDev *dS = (const GifStreamDev *) dv;
 		const GifFrameDev *dF = (const GifFrameDev *) (dv + off_fr);
@@ -866,6 +780,7 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		unsigned *dC = (unsigned *) (dv + off_counts);
 		int *dSt = (int *) (dv + off_status);
 		std::vector<int> st(nf, 0);
+		int rc = 0;
 		if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaMemsetAsync(dSt, 0, nf * sizeof(int), s) != cudaSuccess)
 			rc = cuda_fail(domain, cudaGetLastError(), "gif staging copy");
 		else {
@@ -890,8 +805,8 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 				rc = cuda_fail(domain, e, "gif_compose_kernel");
 		}
 		dev_free(dev, s);
-		c0 += cn;
-	}
+		return rc;
+	});
 	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
 		rc = cuda_fail(domain, cudaGetLastError(), "gif decode");
 	return rc;
@@ -978,77 +893,15 @@ extern "C" int
 vb200_gif_decode_batch(const void *const *bufs, const size_t *lens, int n, int page, int n_pages, void *out, int out_location, size_t out_bpl,
 	size_t out_frame_stride, int *width, int *height, int *bands)
 {
-	const char *domain = "gif_decode_batch";
-	int w = 0, h = 0, b = 0;
-	if (!out) {
-		if (dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, nullptr, 0, 0, &w, &h, &b, nullptr))
-			return -1;
-	}
-	else {
-		if (ensure_init(domain))
-			return -1;
-		cudaStream_t s = current_stream();
-		if (out_location == VB200_DEVICE) {
-			if (dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, out, out_bpl, out_frame_stride, &w, &h, &b, s))
-				return -1;
-		}
-		else {
-			if (dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, nullptr, 0, 0, &w, &h, &b, s))
-				return -1;
-			const size_t line = (size_t) w * b;
-			if (out_bpl < line || (n > 1 && out_frame_stride < out_bpl * h)) {
-				error(domain, "output strides too small for %d x %d x %d", w, h, b);
-				return -1;
-			}
-			/* decoded whole on the device first: a batch that fails leaves the caller's memory as it was */
-			void *dev = nullptr;
-			if (dev_alloc(domain, &dev, line * h * n, s))
-				return -1;
-			int rc = dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, dev, line, line * h, nullptr, nullptr, nullptr, s);
-			for (int i = 0; i < n && !rc; i++)
-				if (cudaMemcpy2DAsync((char *) out + (size_t) i * out_frame_stride, out_bpl, (char *) dev + (size_t) i * line * h, line, line, h,
-						cudaMemcpyDeviceToHost, s) != cudaSuccess)
-					rc = cuda_fail(domain, cudaGetLastError(), "copy to host");
-			if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, cudaGetLastError(), "gif decode");
-			dev_free(dev, s);
-			if (rc)
-				return -1;
-		}
-	}
-	if (width)
-		*width = w;
-	if (height)
-		*height = h;
-	if (bands)
-		*bands = b;
-	return 0;
+	return decode_batch_abi("gif_decode_batch", {STREAM_GIF, 1, page, n_pages}, bufs, lens, n, out, out_location, out_bpl, out_frame_stride, width,
+		height, bands);
 }
 
 /* reference: vips_gifload_buffer(buf, len, &out, "page", page, "n", n, NULL), foreign/nsgifload.c */
 extern "C" int
 vb200_gifload_buffer(const void *buf, size_t len, int page, int n, VB200Image *out)
 {
-	const char *domain = "gifload_buffer";
-	if (!buf || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	int w, h, b;
-	if (dev_gif_decode_batch(domain, &buf, &len, 1, page, n, nullptr, 0, 0, &w, &h, &b, s))
-		return -1;
-	DevImage d;
-	if (dev_image_new(domain, &d, w, h, b, VB200_FORMAT_UCHAR, VB200_INTERPRETATION_sRGB, s))
-		return -1;
-	if (dev_gif_decode_batch(domain, &buf, &len, 1, page, n, d.data, d.bpl, d.bpl * h, nullptr, nullptr, nullptr, s)) {
-		dev_image_release(&d, s);
-		return -1;
-	}
-	VB200Image like = *out;
-	return deliver(domain, &d, &like, out, s);
+	return load_abi("gifload_buffer", {STREAM_GIF, 1, page, n}, buf, len, out);
 }
 
 extern "C" int

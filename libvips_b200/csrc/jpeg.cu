@@ -1656,7 +1656,6 @@ struct FramePrep {
 	size_t coef_count = 0, plane_bytes = 0;
 	int bands = 0;
 	size_t stage_bytes = 0, stage_ints = 0; /* what the frame takes of the chunk's byte and offset pools */
-	std::string err;
 };
 
 int
@@ -2319,50 +2318,27 @@ jpeg_pump_release()
  */
 int
 dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *out_w, int *out_h, int *bands, cudaStream_t s)
+	size_t out_frame_stride, StreamGeometry *geom, cudaStream_t s)
 {
-	if (n < 1 || !bufs || !lens) {
-		error(domain, "no frames");
-		return -1;
-	}
 	const DecodeOptions o = decode_options();
 	std::vector<FramePrep> prep(n);
-	parallel_for(n, host_workers(), [&](int i) {
+	auto parse = [&](int i) {
 		if (frame_prep(domain, (const unsigned char *) bufs[i], lens[i], shrink, &prep[i]))
-			prep[i].err = vb200_error_buffer(); /* the worker's thread-local text */
-		else {
-			/* frames with one restart interval (no DRI) and a scan worth splitting decode by self-synchronising subsequences */
-			const Segment &g = prep[i].segs[0];
-			prep[i].F.sync =
-				!prep[i].F.progressive && g.S.n_intervals == 1 && o.sub_bytes > 0 && g.len >= o.sync_min_bytes && g.len / o.sub_bytes >= 8;
-		}
-	});
-	for (int i = 0; i < n; i++)
-		if (!prep[i].err.empty()) {
-			error(domain, "frame %d: %s", i, prep[i].err.c_str());
 			return -1;
-		}
+		/* frames with one restart interval (no DRI) and a scan worth splitting decode by self-synchronising subsequences */
+		const Segment &g = prep[i].segs[0];
+		prep[i].F.sync = !prep[i].F.progressive && g.S.n_intervals == 1 && o.sub_bytes > 0 && g.len >= o.sync_min_bytes && g.len / o.sub_bytes >= 8;
+		return 0;
+	};
+	if (parse_streams(domain, "frame", n, parse, [&](int i) { return StreamGeometry{prep[i].F.out_w, prep[i].F.out_h, prep[i].bands, 0}; }, geom))
+		return -1;
 	if (o.timing == '2')
 		fprintf(stderr, "[jpeg] %d headers parsed\n", n);
-	const int W = prep[0].F.out_w, Hh = prep[0].F.out_h, B = prep[0].bands;
-	for (int i = 1; i < n; i++)
-		if (prep[i].F.out_w != W || prep[i].F.out_h != Hh || prep[i].bands != B) {
-			error(domain, "frames of a batch must decode to one geometry (%d x %d x %d, frame %d: %d x %d x %d)", W, Hh, B, i,
-				prep[i].F.out_w, prep[i].F.out_h, prep[i].bands);
-			return -1;
-		}
-	if (out_w)
-		*out_w = W;
-	if (out_h)
-		*out_h = Hh;
-	if (bands)
-		*bands = B;
 	if (!out)
 		return 0;
-	if (out_bpl < (size_t) W * B || (n > 1 && out_frame_stride < out_bpl * Hh)) {
-		error(domain, "output strides too small for %d x %d x %d", W, Hh, B);
+	if (check_out_strides(domain, *geom, out_bpl, out_frame_stride))
 		return -1;
-	}
+	const int W = geom->w, Hh = geom->h;
 	static std::once_flag zz_once;
 	std::call_once(zz_once, [] { cudaMemcpyToSymbol(d_zigzag, kZigzag, 64); });
 
@@ -2545,89 +2521,15 @@ extern "C" int
 vb200_jpeg_decode_batch(const void *const *bufs, const size_t *lens, int n, int shrink, void *out, int out_location, size_t out_bpl,
 	size_t out_frame_stride, int *width, int *height, int *bands)
 {
-	const char *domain = "jpeg_decode_batch";
-	int w = 0, h = 0, b = 0;
-	if (!out) {
-		/* geometry only: no device needed */
-		if (n < 1 || !bufs || !lens) {
-			error(domain, "no frames");
-			return -1;
-		}
-		for (int i = 0; i < n; i++) {
-			int wi, hi, bi;
-			if (host_jpeg_decode(domain, bufs[i], lens[i], shrink, nullptr, 0, &wi, &hi, &bi, 0, 0, nullptr))
-				return -1;
-			if (i && (wi != w || hi != h || bi != b)) {
-				error(domain, "frames of a batch must decode to one geometry");
-				return -1;
-			}
-			w = wi, h = hi, b = bi;
-		}
-	}
-	else {
-		if (ensure_init(domain))
-			return -1;
-		cudaStream_t s = current_stream();
-		if (out_location == VB200_DEVICE) {
-			if (dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, out, out_bpl, out_frame_stride, &w, &h, &b, s))
-				return -1;
-		}
-		else {
-			if (dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, nullptr, 0, 0, &w, &h, &b, s))
-				return -1;
-			const size_t line = (size_t) w * b;
-			if (out_bpl < line || (n > 1 && out_frame_stride < out_bpl * h)) {
-				error(domain, "output strides too small for %d x %d x %d", w, h, b);
-				return -1;
-			}
-			void *dev = nullptr;
-			if (dev_alloc(domain, &dev, line * h * n, s))
-				return -1;
-			int rc = dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, dev, line, line * h, nullptr, nullptr, nullptr, s);
-			for (int i = 0; i < n && !rc; i++)
-				if (cudaMemcpy2DAsync((char *) out + (size_t) i * out_frame_stride, out_bpl, (char *) dev + (size_t) i * line * h, line, line, h,
-						cudaMemcpyDeviceToHost, s) != cudaSuccess)
-					rc = cuda_fail(domain, cudaGetLastError(), "copy to host");
-			if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, cudaGetLastError(), "jpeg decode");
-			dev_free(dev, s);
-			if (rc)
-				return -1;
-		}
-	}
-	if (width)
-		*width = w;
-	if (height)
-		*height = h;
-	if (bands)
-		*bands = b;
-	return 0;
+	return decode_batch_abi("jpeg_decode_batch", {STREAM_JPEG, shrink}, bufs, lens, n, out, out_location, out_bpl, out_frame_stride, width,
+		height, bands);
 }
 
-/* reference: vips_jpegload_buffer(buf, len, &out, "shrink", shrink, NULL), foreign/jpegload.c + jpeg2vips.c */
+/* reference: vips_jpegload_buffer(buf, len, &out, "shrink", shrink, NULL), foreign/jpeg2vips.c */
 extern "C" int
 vb200_jpegload_buffer(const void *buf, size_t len, int shrink, VB200Image *out)
 {
-	const char *domain = "jpegload_buffer";
-	if (!buf || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	int w, h, b;
-	if (dev_jpeg_decode_batch(domain, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s))
-		return -1;
-	DevImage d;
-	if (dev_image_new(domain, &d, w, h, b, VB200_FORMAT_UCHAR, b == 1 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, s))
-		return -1;
-	if (dev_jpeg_decode_batch(domain, &buf, &len, 1, shrink, d.data, d.bpl, d.bpl * h, nullptr, nullptr, nullptr, s)) {
-		dev_image_release(&d, s);
-		return -1;
-	}
-	VB200Image like = *out;
-	return deliver(domain, &d, &like, out, s);
+	return load_abi("jpegload_buffer", {STREAM_JPEG, shrink}, buf, len, out);
 }
 
 /* reference: vips_thumbnail_find_jpegshrink, resample/thumbnail.c:489-517 (linear = FALSE) */

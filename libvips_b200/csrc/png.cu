@@ -31,8 +31,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <exception>
-#include <mutex>
-#include <string>
 #include <vector>
 
 #include "../../include/vb200.h"
@@ -872,27 +870,6 @@ status_text(int st)
 	return "palette index beyond PLTE";
 }
 
-/* pinned staging, grow-only (vb200_shutdown releases it); one decode at a time uses it */
-struct PngStaging {
-	void *pinned = nullptr;
-	size_t cap = 0;
-	void release()
-	{
-		if (pinned)
-			cudaFreeHost(pinned);
-		pinned = nullptr;
-		cap = 0;
-	}
-};
-PngStaging g_staging;
-std::mutex g_staging_lock;
-
-size_t
-align16(size_t v)
-{
-	return (v + 15) & ~(size_t) 15;
-}
-
 /* device bytes a frame takes in a chunk: its staged deflate bytes and its scanlines */
 size_t
 frame_device_bytes(const PngHeader &H)
@@ -900,16 +877,7 @@ frame_device_bytes(const PngHeader &H)
 	return align16(deflate_bytes(H)) + align16(scan_bytes(H));
 }
 
-size_t g_chunk_budget = 0; /* vb200_debug_png_set_budget: device bytes per chunk, 0 = an eighth of the device (at least 1 GiB) */
-
 } // namespace
-
-void
-png_staging_release()
-{
-	std::lock_guard<std::mutex> lock(g_staging_lock);
-	g_staging.release();
-}
 
 bool
 png_signature(const void *buf, size_t len)
@@ -961,67 +929,19 @@ png_icc_profile(const char *domain, const unsigned char *d, size_t len, std::vec
  */
 int
 dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
-	int *out_w, int *out_h, int *out_bands, cudaStream_t s)
+	StreamGeometry *g, cudaStream_t s)
 {
-	if (n < 1 || !bufs || !lens) {
-		error(domain, "no frames");
-		return -1;
-	}
 	std::vector<PngHeader> hdr(n);
-	std::vector<std::string> errs(n);
-	parallel_for(n, host_workers(), [&](int i) {
-		if (parse_png(domain, (const unsigned char *) bufs[i], lens[i], &hdr[i])) {
-			/* the worker's thread-local "domain: reason\n", restated below with the frame's index */
-			std::string e = vb200_error_buffer();
-			vb200_error_clear();
-			const size_t at = e.find(": ");
-			e = e.substr(at == std::string::npos ? 0 : at + 2);
-			errs[i] = e.substr(0, e.find('\n'));
-		}
-	});
-	for (int i = 0; i < n; i++)
-		if (!errs[i].empty()) {
-			error(domain, "frame %d: %s", i, errs[i].c_str());
-			return -1;
-		}
-	const int W = hdr[0].w, Hh = hdr[0].h, B = hdr[0].bands;
-	for (int i = 1; i < n; i++)
-		if (hdr[i].w != W || hdr[i].h != Hh || hdr[i].bands != B) {
-			error(domain, "frames of a batch must decode to one geometry (%d x %d x %d, frame %d: %d x %d x %d)", W, Hh, B, i, hdr[i].w, hdr[i].h,
-				hdr[i].bands);
-			return -1;
-		}
-	if (out_w)
-		*out_w = W;
-	if (out_h)
-		*out_h = Hh;
-	if (out_bands)
-		*out_bands = B;
+	if (parse_streams(
+			domain, "frame", n, [&](int i) { return parse_png(domain, (const unsigned char *) bufs[i], lens[i], &hdr[i]); },
+			[&](int i) { return StreamGeometry{hdr[i].w, hdr[i].h, hdr[i].bands, 0}; }, g))
+		return -1;
 	if (!out)
 		return 0;
-	if (out_bpl < (size_t) W * B || (n > 1 && out_frame_stride < out_bpl * Hh)) {
-		error(domain, "output strides too small for %d x %d x %d", W, Hh, B);
+	if (check_out_strides(domain, *g, out_bpl, out_frame_stride))
 		return -1;
-	}
-	const size_t budget = png_chunk_budget();
-	std::lock_guard<std::mutex> lock(g_staging_lock);
-	int rc = 0;
-	for (int c0 = 0; c0 < n && !rc;) {
-		/* the chunk: frames while they fit the budget (at least one) */
-		size_t dev_bytes = 0;
-		int cn = 0;
-		while (c0 + cn < n && cn < kMaxBatchFrames) {
-			const size_t b = frame_device_bytes(hdr[c0 + cn]);
-			if (cn > 0 && dev_bytes + b > budget)
-				break;
-			dev_bytes += b;
-			cn++;
-		}
-		if (dev_bytes > budget) {
-			error(domain, "frame %d needs %zu bytes of device memory, more than the %zu allowed", c0, dev_bytes, budget);
-			rc = -1;
-			break;
-		}
+	const int W = g->w, Hh = g->h;
+	int rc = decode_chunks(domain, "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
 		/* the pinned block: records, palettes, deflate bytes; the device: the same, then the scanlines */
 		std::vector<PngFrameDev> F(cn);
 		size_t n_pal = 0, data = 0, scan = 0;
@@ -1036,16 +956,10 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 			scan += align16(scan_bytes(H));
 		}
 		const size_t off_pal = align16(cn * sizeof(PngFrameDev)), off_data = off_pal + n_pal * 1024, total = off_data + data;
-		if (g_staging.cap < total) {
-			g_staging.release();
-			if (cudaMallocHost(&g_staging.pinned, total + total / 4) != cudaSuccess) {
-				rc = cuda_fail(domain, cudaGetLastError(), "cudaMallocHost (png staging)");
-				break;
-			}
-			g_staging.cap = total + total / 4;
-		}
 		/* the previous chunk's copy out of the block has finished: its status was read after it */
-		unsigned char *hst = (unsigned char *) g_staging.pinned;
+		unsigned char *hst = (unsigned char *) decode_staging(domain, total);
+		if (!hst)
+			return -1;
 		memcpy(hst, F.data(), cn * sizeof(PngFrameDev));
 		parallel_for(cn, host_workers(), [&](int i) {
 			const PngHeader &H = hdr[c0 + i];
@@ -1055,19 +969,17 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		});
 		void *dev = nullptr;
 		int *status = nullptr;
-		if (dev_alloc(domain, &dev, total + scan, s)) {
-			rc = -1;
-			break;
-		}
+		if (dev_alloc(domain, &dev, total + scan, s))
+			return -1;
 		if (dev_alloc(domain, (void **) &status, cn * sizeof(int), s)) {
 			dev_free(dev, s);
-			rc = -1;
-			break;
+			return -1;
 		}
 		const PngFrameDev *dF = (const PngFrameDev *) dev;
 		const unsigned char *dP = (const unsigned char *) dev + off_pal, *dB = (const unsigned char *) dev + off_data;
 		unsigned char *dS = (unsigned char *) dev + total;
 		std::vector<int> st(cn, 0);
+		int rc = 0;
 		if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaMemsetAsync(status, 0, cn * sizeof(int), s) != cudaSuccess)
 			rc = cuda_fail(domain, cudaGetLastError(), "png staging copy");
 		else {
@@ -1107,8 +1019,8 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		}
 		dev_free(status, s);
 		dev_free(dev, s);
-		c0 += cn;
-	}
+		return rc;
+	});
 	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
 		rc = cuda_fail(domain, cudaGetLastError(), "png decode");
 	return rc;
@@ -1171,78 +1083,14 @@ extern "C" int
 vb200_png_decode_batch(const void *const *bufs, const size_t *lens, int n, void *out, int out_location, size_t out_bpl, size_t out_frame_stride,
 	int *width, int *height, int *bands)
 {
-	const char *domain = "png_decode_batch";
-	int w = 0, h = 0, b = 0;
-	if (!out) {
-		/* geometry only: the headers, no device */
-		if (dev_png_decode_batch(domain, bufs, lens, n, nullptr, 0, 0, &w, &h, &b, nullptr))
-			return -1;
-	}
-	else {
-		if (ensure_init(domain))
-			return -1;
-		cudaStream_t s = current_stream();
-		if (out_location == VB200_DEVICE) {
-			if (dev_png_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, &w, &h, &b, s))
-				return -1;
-		}
-		else {
-			if (dev_png_decode_batch(domain, bufs, lens, n, nullptr, 0, 0, &w, &h, &b, s))
-				return -1;
-			const size_t line = (size_t) w * b;
-			if (out_bpl < line || (n > 1 && out_frame_stride < out_bpl * h)) {
-				error(domain, "output strides too small for %d x %d x %d", w, h, b);
-				return -1;
-			}
-			/* decoded whole on the device first: a batch that fails leaves the caller's memory as it was */
-			void *dev = nullptr;
-			if (dev_alloc(domain, &dev, line * h * n, s))
-				return -1;
-			int rc = dev_png_decode_batch(domain, bufs, lens, n, dev, line, line * h, nullptr, nullptr, nullptr, s);
-			for (int i = 0; i < n && !rc; i++)
-				if (cudaMemcpy2DAsync((char *) out + (size_t) i * out_frame_stride, out_bpl, (char *) dev + (size_t) i * line * h, line, line, h,
-						cudaMemcpyDeviceToHost, s) != cudaSuccess)
-					rc = cuda_fail(domain, cudaGetLastError(), "copy to host");
-			if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, cudaGetLastError(), "png decode");
-			dev_free(dev, s);
-			if (rc)
-				return -1;
-		}
-	}
-	if (width)
-		*width = w;
-	if (height)
-		*height = h;
-	if (bands)
-		*bands = b;
-	return 0;
+	return decode_batch_abi("png_decode_batch", {STREAM_PNG}, bufs, lens, n, out, out_location, out_bpl, out_frame_stride, width, height, bands);
 }
 
 /* reference: vips_pngload_buffer(buf, len, &out, NULL), foreign/spngload.c */
 extern "C" int
 vb200_pngload_buffer(const void *buf, size_t len, VB200Image *out)
 {
-	const char *domain = "pngload_buffer";
-	if (!buf || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	int w, h, b;
-	if (dev_png_decode_batch(domain, &buf, &len, 1, nullptr, 0, 0, &w, &h, &b, s))
-		return -1;
-	DevImage d;
-	if (dev_image_new(domain, &d, w, h, b, VB200_FORMAT_UCHAR, b <= 2 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, s))
-		return -1;
-	if (dev_png_decode_batch(domain, &buf, &len, 1, d.data, d.bpl, d.bpl * h, nullptr, nullptr, nullptr, s)) {
-		dev_image_release(&d, s);
-		return -1;
-	}
-	VB200Image like = *out;
-	return deliver(domain, &d, &like, out, s);
+	return load_abi("pngload_buffer", {STREAM_PNG}, buf, len, out);
 }
 
 extern "C" int
@@ -1293,23 +1141,4 @@ vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *
 	if (rc)
 		error("inflate (host twin)", "%s", err == ERR_MORE ? "more output than the buffer holds" : "corrupt deflate stream");
 	return rc;
-}
-
-/* device bytes per chunk of the PNG decoder and encoder */
-size_t
-vb200::png_chunk_budget()
-{
-	size_t budget = g_chunk_budget;
-	if (!budget) {
-		size_t free_b = 0, total_b = 0;
-		cudaMemGetInfo(&free_b, &total_b);
-		budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
-	}
-	return budget;
-}
-
-extern "C" void
-vb200_debug_png_set_budget(size_t bytes)
-{
-	g_chunk_budget = bytes;
 }

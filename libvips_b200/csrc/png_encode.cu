@@ -1323,7 +1323,7 @@ dev_png_encode(const char *domain, const void *frames, int frames_location, size
 	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_last_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 4));
 	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 2));
 	const bool host_in = frames_location != VB200_DEVICE, host_out = out_location != VB200_DEVICE;
-	const size_t frame_in = g.rb * g.h, budget = png_chunk_budget(), per = frame_bytes(g, host_in, host_out);
+	const size_t frame_in = g.rb * g.h, budget = decode_chunk_budget(), per = frame_bytes(g, host_in, host_out);
 	std::vector<unsigned char> staged; /* host output: the batch's streams, packed */
 	std::vector<size_t> staged_at(n);
 	int rc = 0;

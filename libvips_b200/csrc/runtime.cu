@@ -396,8 +396,7 @@ vb200_shutdown(void)
 		cudaDeviceSynchronize();
 		resample_cache_clear();
 		jpeg_pump_release();
-		png_staging_release();
-		gif_staging_release();
+		decode_staging_release();
 	}
 	g_device.store(-1);
 }

@@ -2478,66 +2478,6 @@ vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, 
 	return vb200_thumbnail_buffer_icc(buf, len, out, width, height, size, nullptr);
 }
 
-/* The streams the thumbnail entry points take: JPEG, or PNG / GIF by their signatures.  The decoder and where the embedded
- * profile comes from are all that differ.  PNG and GIF have no load-time shrink (thumbnail.c:609-660 lists the loaders
- * that do), and a PNG with eXIf is declined: its orientation would need vips_autorot (thumbnail.c:989-996), which is not
- * built.  A GIF loads with nsgifload's defaults, page 0 and n = 1, and carries no profile.
- */
-enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF };
-
-static StreamKind
-stream_kind(const void *buf, size_t len)
-{
-	return png_signature(buf, len) ? STREAM_PNG : gif_signature(buf, len) ? STREAM_GIF : STREAM_JPEG;
-}
-
-static int
-stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size_t n, std::vector<unsigned char> *profile)
-{
-	if (kind == STREAM_GIF) {
-		profile->clear();
-		return 0;
-	}
-	if (kind == STREAM_JPEG)
-		return jpeg_icc_profile(domain, d, n, profile);
-	bool exif = false;
-	if (png_icc_profile(domain, d, n, profile, &exif))
-		return -1;
-	if (exif) {
-		error(domain, "PNG with eXIf: its orientation would need vips_autorot, which is not built");
-		return -1;
-	}
-	return 0;
-}
-
-/* vips_thumbnail_buffer hands its option string to the loader (thumbnail.c:1486-1490, 1585-1590): page and n are
- * nsgifload's; jpegload and spngload have neither, so any other value fails there
- */
-static int
-stream_pages_check(const char *domain, StreamKind kind, int page, int n_pages)
-{
-	if (kind != STREAM_GIF && (page != 0 || n_pages != 1)) {
-		error(domain, "%s has no page or n option (page %d, n %d)", kind == STREAM_PNG ? "pngload" : "jpegload", page, n_pages);
-		return -1;
-	}
-	return 0;
-}
-
-/* page / n_pages: the GIF pages to decode (a strip of screen-height pages); JPEG and PNG take 0 / 1 */
-static int
-stream_decode(const char *domain, StreamKind kind, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *w, int *h, int *b, cudaStream_t s, int page = 0, int n_pages = 1)
-{
-	switch (kind) {
-	case STREAM_PNG:
-		return dev_png_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, w, h, b, s);
-	case STREAM_GIF:
-		return dev_gif_decode_batch(domain, bufs, lens, n, page, n_pages, out, out_bpl, out_frame_stride, w, h, b, s);
-	default:
-		return dev_jpeg_decode_batch(domain, bufs, lens, n, shrink, out, out_bpl, out_frame_stride, w, h, b, s);
-	}
-}
-
 static int thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size, int linear,
 	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, bool linear_icc, int *out_page_height);
 
@@ -2556,66 +2496,54 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 	}
 	if (ensure_init(domain))
 		return -1;
-	const StreamKind kind = stream_kind(buf, len);
-	if (stream_pages_check(domain, kind, page, n_pages))
-		return -1;
-	int screen_h = 0;
-	if (kind == STREAM_GIF) {
-		int sw, sb, frames;
-		if (vb200_gif_geometry(buf, len, &sw, &screen_h, &sb, &frames))
-			return -1;
-	}
+	DecodeRequest req{stream_kind(buf, len), 1, page, n_pages};
 	const bool want_profile = icc && (icc->output_profile || linear);
 	std::vector<unsigned char> embedded;
-	if ((kind == STREAM_PNG || want_profile) && stream_profile(domain, kind, (const unsigned char *) buf, len, &embedded))
+	if ((req.kind == STREAM_PNG || want_profile) && stream_profile(domain, req.kind, (const unsigned char *) buf, len, &embedded))
 		return -1;
 	if (!want_profile)
 		embedded.clear();
 	cudaStream_t s = current_stream();
-	int w0, h0, b0;
-	if (stream_decode(domain, kind, &buf, &len, 1, 1, nullptr, 0, 0, &w0, &h0, &b0, s, page, n_pages))
-		return -1;
-	const int shrink = linear || kind != STREAM_JPEG ? 1 : vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
-	int w, h, b;
-	if (stream_decode(domain, kind, &buf, &len, 1, shrink, nullptr, 0, 0, &w, &h, &b, s, page, n_pages))
-		return -1;
-	const int page_height = kind == STREAM_GIF && h > screen_h ? screen_h : 0;
+	if (req.kind == STREAM_JPEG && !linear) {
+		int w0, h0, b0;
+		if (dev_decode_batch(domain, req, &buf, &len, 1, nullptr, 0, 0, &w0, &h0, &b0, nullptr, s))
+			return -1;
+		req.shrink = vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
+	}
 	DevImage dec;
-	if (dev_image_new(domain, &dec, w, h, b, VB200_FORMAT_UCHAR, b <= 2 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, s))
+	int page_height;
+	if (dev_load(domain, req, buf, len, &dec, &page_height, s))
 		return -1;
-	int rc = stream_decode(domain, kind, &buf, &len, 1, shrink, dec.data, dec.bpl, dec.bpl * h, nullptr, nullptr, nullptr, s, page, n_pages);
+	VB200Image din;
+	memset(&din, 0, sizeof(din));
+	din.Xsize = dec.w;
+	din.Ysize = dec.h;
+	din.Bands = dec.bands;
+	din.BandFmt = VB200_FORMAT_UCHAR;
+	din.Type = dec.type;
+	din.where = VB200_DEVICE;
+	din.data = dec.data;
+	din.bpl = dec.bpl;
+	const int where = out->where;
+	VB200Image tmp;
+	memset(&tmp, 0, sizeof(tmp));
+	tmp.where = VB200_DEVICE;
+	int rc = thumbnail_image_run(&din, page_height, &tmp, width, height, size, linear, icc, embedded.data(), embedded.size(), linear,
+		out_page_height);
 	if (!rc) {
-		VB200Image din;
-		memset(&din, 0, sizeof(din));
-		din.Xsize = w;
-		din.Ysize = h;
-		din.Bands = b;
-		din.BandFmt = VB200_FORMAT_UCHAR;
-		din.Type = dec.type;
-		din.where = VB200_DEVICE;
-		din.data = dec.data;
-		din.bpl = dec.bpl;
-		const int where = out->where;
-		VB200Image tmp;
-		memset(&tmp, 0, sizeof(tmp));
-		tmp.where = VB200_DEVICE;
-		rc = thumbnail_image_run(&din, page_height, &tmp, width, height, size, linear, icc, embedded.data(), embedded.size(), linear,
-			out_page_height);
-		if (!rc) {
-			/* deliver where the caller asked (allocate-or-fill) */
-			DevImage dt;
-			dt.w = tmp.Xsize;
-			dt.h = tmp.Ysize;
-			dt.bands = tmp.Bands;
-			dt.fmt = tmp.BandFmt;
-			dt.type = tmp.Type;
-			dt.data = tmp.data;
-			dt.bpl = tmp.bpl;
-			dt.owned = true;
-			VB200Image like = *out;
-			like.where = where;
-			rc = deliver(domain, &dt, &like, out, s);
-		}
+		/* deliver where the caller asked (allocate-or-fill) */
+		DevImage dt;
+		dt.w = tmp.Xsize;
+		dt.h = tmp.Ysize;
+		dt.bands = tmp.Bands;
+		dt.fmt = tmp.BandFmt;
+		dt.type = tmp.Type;
+		dt.data = tmp.data;
+		dt.bpl = tmp.bpl;
+		dt.owned = true;
+		VB200Image like = *out;
+		like.where = where;
+		rc = deliver(domain, &dt, &like, out, s);
 	}
 	dev_image_release(&dec, s);
 	return rc;
@@ -2647,8 +2575,8 @@ vb200_thumbnail_buffer_pages(const void *buf, size_t len, VB200Image *out, int w
  * vips_thumbnail_buffer() does with the loader + vips_thumbnail_image (thumbnail.c:583-613, 848-902).
  */
 static int
-plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
-	int out_location, size_t out_frame_stride, int page = 0, int n_pages = 1)
+plan_run_streams(const char *domain, const DecodeRequest &req, VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out,
+	int out_location, size_t out_frame_stride)
 {
 	if (!plan || !bufs || !lens || !out || n < 1) {
 		error(domain, "null argument");
@@ -2657,16 +2585,6 @@ plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, 
 	if (ensure_init(domain))
 		return -1;
 	ThumbnailPlanImpl &pl = plan->impl;
-	if (kind == STREAM_GIF) {
-		/* the decoded strip is pl.H rows only if its pages are the plan's: the screen must be one page high */
-		int sw, sh, sb, frames;
-		if (vb200_gif_geometry(bufs[0], lens[0], &sw, &sh, &sb, &frames))
-			return -1;
-		if (sh != (pl.page_h ? pl.page_h : pl.H)) {
-			error(domain, "the plan is for pages of %d rows, the streams' screen is %d rows", pl.page_h ? pl.page_h : pl.H, sh);
-			return -1;
-		}
-	}
 	cudaStream_t s = current_stream();
 	const size_t in_frame = (size_t) pl.W * pl.H * pl.bands, out_frame = (size_t) pl.OW * pl.OH * pl.out_bands();
 	if (out_frame_stride == 0)
@@ -2675,11 +2593,11 @@ plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, 
 	 * stage; PNG streams are read for eXIf either way
 	 */
 	const bool managed = pl.icc || pl.licc;
-	std::vector<std::vector<unsigned char>> profiles(managed || kind == STREAM_PNG ? n : 0);
+	std::vector<std::vector<unsigned char>> profiles(managed || req.kind == STREAM_PNG ? n : 0);
 	std::vector<const void *> emb(profiles.size());
 	std::vector<size_t> emb_len(profiles.size());
 	for (size_t i = 0; i < profiles.size(); i++) {
-		if (stream_profile(domain, kind, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
+		if (stream_profile(domain, req.kind, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
 			error(domain, "stream %d", (int) i);
 			return -1;
 		}
@@ -2693,9 +2611,14 @@ plan_run_streams(const char *domain, StreamKind kind, VB200ThumbnailPlan *plan, 
 		return -1;
 	int rc = -1;
 	do {
-		int w, h, b;
-		if (stream_decode(domain, kind, bufs, lens, n, shrink, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, s, page, n_pages))
+		int w, h, b, page_h;
+		if (dev_decode_batch(domain, req, bufs, lens, n, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, &page_h, s))
 			break;
+		/* a GIF strip is the plan's only if its pages are: the screen must be one page high */
+		if (req.kind == STREAM_GIF && (page_h ? page_h : h) != (pl.page_h ? pl.page_h : pl.H)) {
+			error(domain, "the plan is for pages of %d rows, the streams' screen is %d rows", pl.page_h ? pl.page_h : pl.H, page_h ? page_h : h);
+			break;
+		}
 		if (w != pl.W || h != pl.H || b != pl.bands) {
 			error(domain, "the plan is for %d x %d x %d frames, the streams decode to %d x %d x %d", pl.W, pl.H, pl.bands, w, h, b);
 			break;
@@ -2725,29 +2648,28 @@ extern "C" int
 vb200_thumbnail_plan_run_jpeg(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int shrink, void *out,
 	int out_location, size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_jpeg", STREAM_JPEG, plan, bufs, lens, n, shrink, out, out_location, out_frame_stride);
+	return plan_run_streams("thumbnail_plan_run_jpeg", {STREAM_JPEG, shrink}, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 extern "C" int
 vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
 	size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_png", STREAM_PNG, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
+	return plan_run_streams("thumbnail_plan_run_png", {STREAM_PNG}, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 extern "C" int
 vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
 	size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_gif", STREAM_GIF, plan, bufs, lens, n, 1, out, out_location, out_frame_stride);
+	return plan_run_streams("thumbnail_plan_run_gif", {STREAM_GIF}, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 extern "C" int
 vb200_thumbnail_plan_run_gif_pages(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int page, int n_pages,
 	void *out, int out_location, size_t out_frame_stride)
 {
-	return plan_run_streams("thumbnail_plan_run_gif", STREAM_GIF, plan, bufs, lens, n, 1, out, out_location, out_frame_stride, page,
-		n_pages);
+	return plan_run_streams("thumbnail_plan_run_gif", {STREAM_GIF, 1, page, n_pages}, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 /* The tile pump: a ring of kStreams device staging slots; for each slice of

@@ -192,9 +192,53 @@ int dev_colourspace_ext(const char *domain, const DevImage &in, DevImage *out, i
 /* Launchers of the row/column-table kernels on raw device pointers (used by
  * the generate()-shaped and scanline seams too).
  */
+/* decode.cu: the decoders' shared driver.  A stream's kind is its signature (PNG, GIF), else JPEG. */
+enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF };
+StreamKind stream_kind(const void *buf, size_t len);
+/* what to decode: shrink is JPEG's load-time shrink; page / n_pages GIF's pages (n_pages -1: to the last), 0 / 1 elsewhere */
+struct DecodeRequest {
+	StreamKind kind;
+	int shrink = 1, page = 0, n_pages = 1;
+};
+/* A batch's geometry as the decoders report it: frames of h rows, or (pages > 0) strips of `pages` pages of h rows. */
+struct StreamGeometry {
+	int w = 0, h = 0, bands = 0, pages = 0;
+	int rows() const { return h * std::max(1, pages); }
+};
+/* n streams of one geometry -> out[n][h][w][bands] on the device, out_frame_stride apart (out = nullptr: geometry only, no
+ * device call).  *page_h: the page height of a strip of more than one page, else 0.  Outputs may be null. */
+int dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl,
+	size_t out_frame_stride, int *w, int *h, int *bands, int *page_h, cudaStream_t s);
+/* the body of vb200_jpeg / png / gif_decode_batch: out in host or device memory, or null for the geometry */
+int decode_batch_abi(const char *domain, const DecodeRequest &req, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
+	size_t out_bpl, size_t out_frame_stride, int *width, int *height, int *bands);
+/* one stream into a new packed device image, B_W below 3 bands and sRGB from 3 */
+int dev_load(const char *domain, const DecodeRequest &req, const void *buf, size_t len, DevImage *out, int *page_h, cudaStream_t s);
+/* the body of vb200_jpegload / pngload / gifload_buffer: dev_load, then deliver into *out */
+int load_abi(const char *domain, const DecodeRequest &req, const void *buf, size_t len, VB200Image *out);
+/* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP; -1 for a PNG with eXIf; GIF has none */
+int stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
+/* The pieces of the per-format batch decoders.  parse_streams runs parse(i) for the n streams on the host workers (0, or -1
+ * with the reason in the worker's error buffer, restated as "<noun> i: reason") and checks that geometry(i) agrees. */
+size_t align16(size_t v);
+int parse_streams(const char *domain, const char *noun, int n, const std::function<int(int)> &parse,
+	const std::function<StreamGeometry(int)> &geometry, StreamGeometry *g);
+/* out_bpl and out_frame_stride hold frames of geometry g */
+int check_out_strides(const char *domain, const StreamGeometry &g, size_t out_bpl, size_t out_frame_stride);
+/* device bytes per chunk of the PNG and GIF decoders and the PNG encoder (vb200_debug_png_set_budget; 0: an eighth of the
+ * device, at least 1 GiB) */
+size_t decode_chunk_budget();
+/* chunk(c0, cn) for consecutive streams [c0, c0 + cn) whose device_bytes fit decode_chunk_budget() (at least one: -1 when
+ * that one alone does not), one decode at a time, so that chunk may use decode_staging() */
+int decode_chunks(const char *domain, const char *noun, int n, const std::function<size_t(int)> &device_bytes, const std::function<int(int, int)> &chunk);
+/* the pinned staging block, grow-only, at least bytes long (nullptr: cudaMallocHost failed, with the reason) */
+void *decode_staging(const char *domain, size_t bytes);
+void decode_staging_release(); /* vb200_shutdown */
+
+/* The three batch decoders dev_decode_batch switches over (n >= 1; out_frame_stride holds a frame whatever n is). */
 /* jpeg.cu: n JPEG streams of one output geometry -> out[n][h][w][bands] on the device (out = nullptr: geometry only) */
 int dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *out_w, int *out_h, int *bands, cudaStream_t s);
+	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);
 int host_jpeg_decode(const char *domain, const void *buf, size_t len, int shrink, unsigned char *out, size_t out_bpl, int *out_w,
 	int *out_h, int *bands, unsigned sub_bytes, int max_passes, int *passes_used);
 /* jpeg_encode.cu: the encoder's host twins (the per-block code on the CPU), one stream appended to out */
@@ -216,20 +260,15 @@ int jpeg_icc_profile(const char *domain, const unsigned char *d, size_t n, std::
 /* png.cu: n PNG streams of one output geometry -> out[n][h][w][bands] on the device (out = nullptr: geometry only, no
  * device call) */
 int dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
-	int *out_w, int *out_h, int *bands, cudaStream_t s);
+	StreamGeometry *g, cudaStream_t s);
 bool png_signature(const void *buf, size_t len);
 /* png.cu: the iCCP profile inflated (empty: none); *exif = whether the stream has an eXIf chunk (exif may be null) */
 int png_icc_profile(const char *domain, const unsigned char *d, size_t n, std::vector<unsigned char> *profile, bool *exif);
-void png_staging_release(); /* png.cu's pinned staging; vb200_shutdown */
-/* png.cu: device bytes per chunk of the PNG decoder and encoder (vb200_debug_png_set_budget; 0: an eighth of the device, at
- * least 1 GiB) */
-size_t png_chunk_budget();
-/* gif.cu: n GIF streams of one geometry, pages page .. page + npages - 1 (npages -1: to the last) -> out[n][h][w][bands] on
- * the device, h the height of all pages (out = nullptr: geometry only, no device call) */
+/* gif.cu: n GIF streams of one geometry, pages page .. page + npages - 1 (npages -1: to the last) -> out[n][h * pages][w][bands]
+ * on the device, g->h the screen height (out = nullptr: geometry only, no device call) */
 int dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int page, int npages, void *out, size_t out_bpl,
-	size_t out_frame_stride, int *out_w, int *out_h, int *bands, cudaStream_t s);
+	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);
 bool gif_signature(const void *buf, size_t len); /* GIF87a or GIF89a */
-void gif_staging_release(); /* gif.cu's pinned staging; vb200_shutdown */
 
 /* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
 int host_workers();
