@@ -602,7 +602,8 @@ int vb200_debug_jpeg_decode_sync(const void *buf, size_t len, int shrink, int su
  *   vb200_thumbnail_buffer: their orientation would need vips_autorot (thumbnail.c:989-996).
  * vb200_debug_png_decode / vb200_debug_inflate: test hooks, host only -- the same per-symbol, per-byte and per-pixel code
  *   on the CPU; vb200_debug_inflate takes raw deflate data and sets *out_len = cap + 1 when the output does not fit.
- * vb200_debug_png_set_budget: device bytes per chunk (0: an eighth of the device, at least 1 GiB).
+ * vb200_debug_png_set_budget: device bytes per chunk (0: an eighth of the device, at least 1 GiB); it bounds the PNG and
+ *   GIF decoders and the JPEG and PNG encoders.
  */
 int vb200_png_decode_batch(const void *const *bufs, const size_t *lens, int n, void *out, int out_location, size_t out_bpl,
 	size_t out_frame_stride, int *width, int *height, int *bands);
@@ -706,9 +707,10 @@ int vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, 
  *   2^28 pixels, a format other than uchar (vb200_pngsave_buffer).  Filters other than NONE, interlace, palette and
  *   metadata chunks other than iCCP are not written.
  * vb200_pngsave_batch: n frames of one geometry in host or device memory (frames_location); stream i at out + i *
- *   out_stride (out_location), lengths[i] bytes (host array).  A stream that does not fit out_stride returns -1 with its
- *   frame; with out in host memory nothing is written then, in device memory the frames of earlier chunks of a batch larger
- *   than one chunk (vb200_debug_png_set_budget) may be.
+ *   out_stride (out_location), lengths[i] bytes (host array, may be NULL).  A stream that does not fit out_stride returns -1
+ *   with its frame before its chunk writes anything: with out in host memory nothing is written then, in device memory the
+ *   frames of earlier chunks of a batch larger than one chunk (vb200_debug_png_set_budget) may be.  vb200_jpegsave_batch
+ *   behaves the same.
  * vb200_pngsave_buffer: one image; *out is malloc()ed, free() it.
  * vb200_debug_png_encode: test hook, host only -- the whole stream through the kernels' per-position, per-symbol and
  *   per-block code compiled for the CPU.  out = NULL only reports *len.
@@ -731,7 +733,8 @@ int vb200_debug_deflate(const void *buf, size_t n, int level, int strategy, void
  * subsample_mode says otherwise -- 0 auto, 1 on, 2 off --, baseline, standard Huffman tables, JFIF header) for n equally sized
  * 8-bit frames of 1 or 3 bands, encoded on the device (csrc/jpeg_encode.cu): the streams are libjpeg-turbo's byte for byte
  * (tests/test_jpeg_encode.py).  frames / out in host or device memory; stream i at out + i * out_stride, lengths[i] bytes
- * (host array); -1 when a stream does not fit its stride.
+ * (host array, may be NULL).  Batches run in chunks bounded by vb200_debug_png_set_budget; a stream that does not fit
+ * out_stride fails the call as in vb200_pngsave_batch.
  */
 int vb200_jpegsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands,
 	int Q, int subsample_mode, void *out, int out_location, size_t out_stride, size_t *lengths);
@@ -844,7 +847,8 @@ int vb200_debug_dz_pyramid_level(const void *pixels, size_t bpl, int width, int 
 void vb200_debug_dz_set_budget(size_t bytes);
 size_t vb200_debug_dz_pool_used(void);
 /* with env VB200_DZ_TIMING set: CUDA-event milliseconds of the calling thread's last vb200_dzsave, split into
- * ms[0] pyramid kernels, [1] gather kernels, [2] encoder calls, [3] stream compaction and device-to-host copies
+ * ms[0] pyramid kernels, [1] gather kernels, [2] encoder calls with the packed streams' device-to-host copies, [3] the
+ * host-side placement of the tiles' streams
  */
 void vb200_debug_dz_times(float *ms);
 

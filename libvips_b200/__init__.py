@@ -760,14 +760,10 @@ def flatten_host_twin(a, background=None, max_alpha=0.0, interpretation=None, x4
 _SAVE_BUFFERS = {}
 
 
-def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0,
-                   interlace=False):
-    """vips_jpegsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1 or 3) on the device -> list of bytes.
-    in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  optimize_coding: per-frame Huffman
-    tables; restart_interval: an RSTn marker every that many MCUs (0..65535, 0 for none); interlace: a progressive stream
-    (libjpeg's jpeg_simple_progression script, every scan with its own optimal tables)"""
-    mode = {"auto": 0, "on": 1, "off": 2}[subsample_mode]
-    opts = JpegSaveOptions(int(Q), mode, int(bool(optimize_coding)), int(restart_interval), int(bool(interlace)))
+def _save_batch(fn, opts, frames, in_ptr, shape, stride, extra=()):
+    """the body of jpegsave_batch / pngsave_batch: fn(src, where, bpl, frame_stride, n, w, h, bands, opts, *extra, out, HOST,
+    stride, lens) over frames on the host or at in_ptr, the streams into one reused host array -> list of bytes.  stride:
+    bytes per output slot, or a function of (w, h, bands) that gives it"""
     if in_ptr is None:
         frames = np.ascontiguousarray(frames)
         if frames.ndim == 3:
@@ -777,15 +773,25 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
     else:
         n, h, w, bands = shape
         src, where = C.c_void_p(in_ptr), DEVICE
-    stride = int(stride or (w * h * bands * 2 + 4096))
+    stride = int(stride(w, h, bands) if callable(stride) else stride)
     out = _SAVE_BUFFERS.get((n, stride))
     if out is None:
         _SAVE_BUFFERS.clear()          # one staging array, reused: a fresh quarter gigabyte per call is all page faults
         out = _SAVE_BUFFERS[(n, stride)] = np.empty((n, stride), np.uint8)
     lens = (C.c_size_t * n)()
-    _check(lib().vb200_jpegsave_batch_opts(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), out.ctypes.data_as(C.c_void_p),
-                                           HOST, stride, lens))
+    _check(fn(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), *extra, out.ctypes.data_as(C.c_void_p), HOST, stride, lens))
     return [out[i, :lens[i]].tobytes() for i in range(n)]
+
+
+def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None, stride=None, optimize_coding=False, restart_interval=0,
+                   interlace=False):
+    """vips_jpegsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1 or 3) on the device -> list of bytes.
+    in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  optimize_coding: per-frame Huffman
+    tables; restart_interval: an RSTn marker every that many MCUs (0..65535, 0 for none); interlace: a progressive stream
+    (libjpeg's jpeg_simple_progression script, every scan with its own optimal tables)"""
+    mode = {"auto": 0, "on": 1, "off": 2}[subsample_mode]
+    opts = JpegSaveOptions(int(Q), mode, int(bool(optimize_coding)), int(restart_interval), int(bool(interlace)))
+    return _save_batch(lib().vb200_jpegsave_batch_opts, opts, frames, in_ptr, shape, stride or (lambda w, h, bands: w * h * bands * 2 + 4096))
 
 
 def _png_stride(w, h, bands, profile):
@@ -798,23 +804,9 @@ def pngsave_batch(frames, compression=6, strategy="default", xres=1.0, profile=N
     """vips_pngsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1-4) on the device -> list of bytes.
     in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  compression 4-9; strategy "default"
     or "filtered"; xres in pixels per millimetre; profile: ICC bytes written as iCCP.  stride: bytes per output slot."""
-    opts = _png_options(compression, strategy, xres)
-    if in_ptr is None:
-        frames = np.ascontiguousarray(frames)
-        if frames.ndim == 3:
-            frames = frames[..., None]
-        n, h, w, bands = frames.shape
-        src, where = frames.ctypes.data_as(C.c_void_p), HOST
-    else:
-        n, h, w, bands = shape
-        src, where = C.c_void_p(in_ptr), DEVICE
     prof = bytes(profile) if profile else None
-    stride = int(stride or _png_stride(w, h, bands, prof))
-    out = np.empty((n, stride), np.uint8)
-    lens = (C.c_size_t * n)()
-    _check(lib().vb200_pngsave_batch(src, where, w * bands, w * h * bands, n, w, h, bands, C.byref(opts), prof, len(prof) if prof else 0,
-                                     out.ctypes.data_as(C.c_void_p), HOST, stride, lens))
-    return [out[i, :lens[i]].tobytes() for i in range(n)]
+    return _save_batch(lib().vb200_pngsave_batch, _png_options(compression, strategy, xres), frames, in_ptr, shape,
+                       stride or (lambda w, h, bands: _png_stride(w, h, bands, prof)), (prof, len(prof) if prof else 0))
 
 
 def pngsave_host_twin(a, compression=6, strategy="default", xres=1.0, profile=None):

@@ -91,23 +91,23 @@ check_out_strides(const char *domain, const StreamGeometry &g, size_t out_bpl, s
 	return 0;
 }
 
-/* device bytes per chunk of the PNG and GIF decoders and the PNG encoder */
+/* device bytes per chunk of the PNG and GIF decoders and the JPEG and PNG encoders */
 size_t
-decode_chunk_budget()
+chunk_budget()
 {
-	size_t budget = g_chunk_budget;
-	if (!budget) {
+	/* the device's size, asked once: cudaMemGetInfo costs more than a small encoder batch's host work */
+	static const size_t device_default = [] {
 		size_t free_b = 0, total_b = 0;
 		cudaMemGetInfo(&free_b, &total_b);
-		budget = std::max<size_t>(total_b / 8, (size_t) 1 << 30);
-	}
-	return budget;
+		return std::max<size_t>(total_b / 8, (size_t) 1 << 30);
+	}();
+	return g_chunk_budget ? g_chunk_budget : device_default;
 }
 
 int
 decode_chunks(const char *domain, const char *noun, int n, const std::function<size_t(int)> &device_bytes, const std::function<int(int, int)> &chunk)
 {
-	const size_t budget = decode_chunk_budget();
+	const size_t budget = chunk_budget();
 	std::lock_guard<std::mutex> lock(g_staging_lock);
 	for (int c0 = 0; c0 < n;) {
 		/* the chunk: streams while they fit the budget (at least one) */

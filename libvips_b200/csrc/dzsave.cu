@@ -19,9 +19,8 @@
  *                       odd-edge rule from its own size.  All levels stay in device memory: 4/3 of the input.
  *   dz_gather_kernel    the tiles of one shape (w, h), from every level, copied into one batch [n][h][w][bands], driven by
  *                       a table of source pointers built on the host
- *   the encoder         one vb200_jpegsave_batch_opts call per shape batch, device in, device out (jpeg_encode.cu)
- *   dz_compact_kernel   the streams packed end to end, so the one device-to-host copy per batch moves their bytes and
- *                       not their slots
+ *   the encoder         the encoders' batch driver per shape batch (encode.cu), device in: the streams packed end to end
+ *                       on the device, so the one device-to-host copy per chunk moves their bytes and not their slots
  * With the defaults a 16384 x 16384 image is 5 730 tiles in 45 shapes, 5 214 of them 256 x 256.
  */
 #include <algorithm>
@@ -201,16 +200,6 @@ dz_gather_kernel(const DzGatherTile *__restrict__ tiles, int row_bytes, int h, u
 		}
 		o[j] = v;
 	}
-}
-
-/* stream blockIdx.y of the batch from its slot to off[blockIdx.y] of the packed buffer; off[n] is the total */
-__global__ void __launch_bounds__(kDzThreads)
-dz_compact_kernel(const unsigned char *__restrict__ slots, size_t slot, const unsigned long long *__restrict__ off, unsigned char *__restrict__ packed)
-{
-	const unsigned long long a = off[blockIdx.y], len = off[blockIdx.y + 1] - a;
-	const unsigned char *p = slots + (size_t) blockIdx.y * slot;
-	for (unsigned long long i = blockIdx.x * kDzThreads + threadIdx.x; i < len; i += gridDim.x * kDzThreads)
-		packed[a + i] = p[i];
 }
 
 /* device scratch of one call: everything still held is freed when the call leaves, whichever way */
@@ -467,25 +456,21 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 	const size_t budget = g_budget.load() ? g_budget.load() : kDzBudget;
 	std::vector<DzGatherTile> table;
 	std::vector<size_t> lens;
-	std::vector<unsigned long long> offs;
 	for (const auto &sh : shapes) {
 		const int w = sh.first.first, h = sh.first.second;
 		const std::vector<long> &idx = sh.second;
 		const size_t frame_stride = ((size_t) w * h * bands + 15) & ~(size_t) 15;
-		/* a stream's slot, from the bound the encoder sizes its scan data by, and the device scratch the encoder takes beside */
-		size_t stream_bytes = 0, scratch_bytes = 0;
-		if (jpeg_encode_room(domain, w, h, bands, jpeg, &stream_bytes, &scratch_bytes))
+		Encoder enc;
+		if (jpeg_encoder(domain, w, h, bands, jpeg, &enc))
 			return -1;
-		const size_t slot = (stream_bytes + 15) & ~(size_t) 15;
-		const size_t per_tile = frame_stride + slot + scratch_bytes;
+		const size_t per_tile = frame_stride + enc.scratch_bytes + enc.stream_bytes;
 		if (per_tile > budget) {
 			error(domain, "a %d x %d tile takes %zu bytes of device memory, more than the %zu allowed for a batch", w, h, per_tile, budget);
 			return -1;
 		}
 		const size_t chunk = std::min<size_t>(std::min<size_t>(budget / per_tile, (size_t) kMaxBatchFrames), idx.size());
-		void *d_table = nullptr, *d_pix = nullptr, *d_slots = nullptr, *d_off = nullptr;
-		if (sc.alloc(domain, &d_table, chunk * sizeof(DzGatherTile)) || sc.alloc(domain, &d_pix, chunk * frame_stride) ||
-			sc.alloc(domain, &d_slots, chunk * slot) || sc.alloc(domain, &d_off, (chunk + 1) * sizeof(unsigned long long)))
+		void *d_table = nullptr, *d_pix = nullptr;
+		if (sc.alloc(domain, &d_table, chunk * sizeof(DzGatherTile)) || sc.alloc(domain, &d_pix, chunk * frame_stride))
 			return -1;
 		for (size_t c0 = 0; c0 < idx.size(); c0 += chunk) {
 			const int cn = (int) std::min(chunk, idx.size() - c0);
@@ -505,9 +490,10 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 			count_launch();
 			timer.end(1);
 			timer.begin();
+			EncodeDest dst;
+			dst.bytes = &P->bytes;
 			lens.assign(cn, 0);
-			if (vb200_jpegsave_batch_opts(d_pix, VB200_DEVICE, (size_t) w * bands, frame_stride, cn, w, h, bands, &jpeg, d_slots, VB200_DEVICE, slot,
-					lens.data())) {
+			if (dev_encode_batch(domain, enc, d_pix, VB200_DEVICE, (size_t) w * bands, frame_stride, cn, (size_t) w * bands, h, dst, lens.data(), s)) {
 				const DzTile &t = P->tiles[idx[c0]];
 				error(domain, "encoding the %d x %d tiles failed; frame 0 there is level %d tile %d_%d, the rest follow in index order", w, h, t.level,
 					t.x, t.y);
@@ -515,34 +501,15 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 			}
 			timer.end(2);
 			timer.begin();
-			offs.resize(cn + 1);
-			offs[0] = 0;
-			for (int i = 0; i < cn; i++)
-				offs[i + 1] = offs[i] + lens[i];
-			const size_t total = (size_t) offs[cn], base = P->bytes.size();
-			void *d_packed = nullptr;
-			if (sc.alloc(domain, &d_packed, total))
-				return -1;
-			VB200_CUDA(domain, cudaMemcpyAsync(d_off, offs.data(), (cn + 1) * sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
-			dz_compact_kernel<<<dim3(8, cn), kDzThreads, 0, s>>>((const unsigned char *) d_slots, slot, (const unsigned long long *) d_off,
-				(unsigned char *) d_packed);
-			VB200_CUDA(domain, cudaGetLastError());
-			count_launch();
-			P->bytes.resize(base + total);
-			VB200_CUDA(domain, cudaMemcpyAsync(P->bytes.data() + base, d_packed, total, cudaMemcpyDeviceToHost, s));
-			VB200_CUDA(domain, cudaStreamSynchronize(s));
-			sc.release(d_packed);
-			timer.end(3);
 			for (int i = 0; i < cn; i++) {
 				DzTile &t = P->tiles[idx[c0 + i]];
-				t.off = base + (size_t) offs[i];
+				t.off = dst.at[i];
 				t.len = lens[i];
 			}
+			timer.end(3);
 		}
 		sc.release(d_table);
 		sc.release(d_pix);
-		sc.release(d_slots);
-		sc.release(d_off);
 	}
 	if (timer.on)
 		memcpy(t_dz_ms, timer.ms, sizeof(t_dz_ms));

@@ -708,7 +708,7 @@ gif_signature(const void *buf, size_t len)
 
 /* Decode n GIF streams (host memory) of one output geometry into out[n][h * pages][w][bands] on the device (out = nullptr:
  * only report the geometry).  Streams are walked on the host workers; they go up in chunks bounded by
- * decode_chunk_budget(), each one pinned block (stream and frame records, tables, LZW payloads) copied to the device.
+ * chunk_budget(), each one pinned block (stream and frame records, tables, LZW payloads) copied to the device.
  * Every frame of a chunk must decode clean before its pixels are composed into out.
  */
 int

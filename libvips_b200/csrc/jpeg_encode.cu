@@ -1557,21 +1557,19 @@ jpeg_ffscan_kernel(const unsigned long long *__restrict__ totals, int max_chunks
 }
 
 /* stuffing, pass 3: the header, the stuffed data with the next scan's header or FF D0+((k - 1) & 7) before segment k >= 1
- * of a scan (RSTn numbering restarts with every scan; padding bytes are stuffed, markers are not), EOI, into the caller's
- * stream (a stream that does not fit is cut: the host compares lengths[frame] with the stride and reports it)
+ * of a scan (RSTn numbering restarts with every scan; padding bytes are stuffed, markers are not), EOI, into the frame's
+ * stream at out + at[frame]
  */
 template <int kInserts>
 __global__ void __launch_bounds__(128)
 jpeg_stuffcopy_kernel(const __grid_constant__ ScanScript P, const unsigned long long *__restrict__ totals, const unsigned char *__restrict__ raw,
 	size_t raw_bytes, int max_chunks, const unsigned *__restrict__ counts, const unsigned char *__restrict__ headers, size_t hdr_stride,
-	const unsigned *__restrict__ hdr_end, int hend_stride, const unsigned *__restrict__ istart, unsigned char *__restrict__ out, size_t out_stride,
-	const unsigned long long *__restrict__ lengths)
+	const unsigned *__restrict__ hdr_end, int hend_stride, const unsigned *__restrict__ istart, const unsigned long long *__restrict__ at,
+	unsigned char *__restrict__ out, const unsigned long long *__restrict__ lengths)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
-	unsigned char *o = out + (size_t) blockIdx.y * out_stride;
+	unsigned char *o = out + at[blockIdx.y];
 	const unsigned long long len = lengths[blockIdx.y];
-	if (len > out_stride)
-		return;
 	const unsigned char *hdr = headers + (size_t) blockIdx.y * hdr_stride;
 	const unsigned *hend = hdr_end + (size_t) blockIdx.y * hend_stride;
 	const unsigned h0 = hend[0];
@@ -1670,20 +1668,20 @@ make_plan(const char *domain, int w, int h, int bands, const VB200JpegSaveOption
 	return 0;
 }
 
-/* The device scratch of a call of n frames, one allocation: the buffers' offsets and the total.  Per frame: coefficients,
- * bit slots, totals, lengths, raw data, span counts, segment starts and the progressive coder's unit summaries, flushed
- * runs and deferred correction bits.  Per chunk of frames, reused by the next: symbol counts, code tables, header slots
- * and header ends (with the standard tables, the batch's header length).  Every buffer grows with n or is shared, so
- * carve(n) takes at most n times carve(1).
+/* The device scratch of a chunk of n frames, one allocation: the buffers' offsets and the total.  Per frame: coefficients,
+ * bit slots, totals, lengths, stream offsets, raw data, span counts, segment starts, the progressive coder's unit
+ * summaries, flushed runs and deferred correction bits, and with the frame's own tables its symbol counts, code tables,
+ * header slot and header ends (with the standard tables, the chunk's one header length).  Every buffer grows with n or is
+ * shared, so carve(n) takes at most n times carve(1).
  */
 struct Scratch {
-	size_t tab, hdr, coef, bits, tot, len, raw, cnt, ist, summ, runs, dslot, doff, freq, huff, slots, hend, bad, bytes;
+	size_t tab, hdr, coef, bits, tot, len, at, raw, cnt, ist, summ, runs, dslot, doff, freq, huff, slots, hend, bad, bytes;
 };
 
 Scratch
 carve(const EncodePlan &E, int n)
 {
-	const size_t nf = (size_t) n, units = E.prog ? (size_t) E.P.units : 0, nopt = E.opt ? (size_t) std::min(n, kMaxBatchFrames) : 0;
+	const size_t nf = (size_t) n, units = E.prog ? (size_t) E.P.units : 0, nopt = E.opt ? nf : 0;
 	size_t off = 0;
 	auto take = [&](size_t bytes) {
 		const size_t o = off;
@@ -1697,6 +1695,7 @@ carve(const EncodePlan &E, int n)
 	S.bits = take(nf * E.nslots * sizeof(unsigned));
 	S.tot = take(nf * sizeof(unsigned long long));
 	S.len = take(nf * sizeof(unsigned long long));
+	S.at = take(nf * sizeof(unsigned long long));
 	S.raw = take(nf * E.raw_bytes);
 	S.cnt = take(nf * E.max_chunks * sizeof(unsigned));
 	S.ist = take(E.prog || E.P.restart ? nf * E.P.nseg * sizeof(unsigned) : 0);
@@ -1722,7 +1721,7 @@ struct ChunkArgs {
 	int cn;
 	short *coef;
 	unsigned *bits, *counts, *istart, *freq, *hdr_end;
-	unsigned long long *totals, *lengths;
+	unsigned long long *totals, *lengths, *at;
 	unsigned char *raw;
 	void *huff;				   /* the frames' HuffSet<E->ntab> */
 	const unsigned char *tmpl; /* the plan's header */
@@ -1731,13 +1730,11 @@ struct ChunkArgs {
 	unsigned *runs, *dslot;
 	unsigned short *doff;
 	int *bad;
-	unsigned char *out;
-	size_t out_stride;
 };
 
-/* a sequential chunk: 7 launches with the standard tables and no restart intervals, +1 with restart intervals
- * (jpeg_segments_kernel), +2 with optimised tables (jpeg_stats_kernel, jpeg_tables_kernel); returns the launch count, -1
- * when the counts could not be cleared
+/* a sequential chunk through the lengths: 6 launches with the standard tables and no restart intervals, +1 with restart
+ * intervals (jpeg_segments_kernel), +2 with optimised tables (jpeg_stats_kernel, jpeg_tables_kernel); returns the launch
+ * count, -1 when the counts could not be cleared
  */
 template <bool kOpt, bool kRestart>
 int
@@ -1750,10 +1747,8 @@ launch_chunk(const ChunkArgs &A, cudaStream_t s)
 	const dim3 per_block((G.blocks + 127) / 128, cn), per_span((E.max_chunks + 127) / 128, cn);
 	HuffSet<4> *huff = (HuffSet<4> *) A.huff;
 	/* the frames' own headers, or the batch's for every frame */
-	const unsigned char *hdr = kOpt ? A.slots : A.tmpl;
-	const size_t hdr_stride = kOpt ? kHeaderSlot : 0;
 	const int hend_stride = kOpt ? 1 : 0;
-	int launches = 7;
+	int launches = 6;
 	jpeg_fdct_kernel<<<dim3((mcus + 127) / 128, cn), 128, 0, s>>>(G, A.T, A.frames, A.bpl, A.frame_stride, A.coef);
 	if (kOpt) {
 		if (cudaMemsetAsync(A.freq, 0, (size_t) cn * 4 * 256 * sizeof(unsigned), s) != cudaSuccess)
@@ -1774,14 +1769,12 @@ launch_chunk(const ChunkArgs &A, cudaStream_t s)
 	constexpr int kInserts = kRestart ? kRestartMarkers : kOneSegment;
 	jpeg_stuffcount_kernel<kInserts><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.istart, A.hdr_end, hend_stride, A.counts);
 	jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(A.totals, E.max_chunks, A.counts, A.hdr_end, hend_stride, A.lengths);
-	jpeg_stuffcopy_kernel<kInserts><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.counts, hdr, hdr_stride, A.hdr_end,
-		hend_stride, A.istart, A.out, A.out_stride, A.lengths);
 	return launches;
 }
 
-/* a progressive chunk: 11 launches whatever the frame count, scan count or restart interval -- FDCT, summaries, chain
- * walk, tables and headers, bit counts, bit prefix sum, segments, emit, and the three stuffing passes; -1 when the counts
- * could not be cleared
+/* a progressive chunk through the lengths: 10 launches whatever the frame count, scan count or restart interval -- FDCT,
+ * summaries, chain walk, tables and headers, bit counts, bit prefix sum, segments, emit, and the first two stuffing passes;
+ * -1 when the counts could not be cleared
  */
 int
 launch_progressive(const ChunkArgs &A, cudaStream_t s)
@@ -1805,27 +1798,35 @@ launch_progressive(const ChunkArgs &A, cudaStream_t s)
 		E.raw_bytes / 4);
 	jpeg_stuffcount_kernel<kScanHeaders><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.istart, A.hdr_end, P.nscans, A.counts);
 	jpeg_ffscan_kernel<<<cn, 1024, 0, s>>>(A.totals, E.max_chunks, A.counts, A.hdr_end, P.nscans, A.lengths);
-	jpeg_stuffcopy_kernel<kScanHeaders><<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.counts, A.slots, kProgHeaderSlot, A.hdr_end,
-		P.nscans, A.istart, A.out, A.out_stride, A.lengths);
-	return 11;
+	return 10;
 }
 
-} // namespace
+/* stuffing, pass 3, every kind of chunk: each frame's stream at out + A.at[frame] */
+void
+launch_stuffcopy(const ChunkArgs &A, unsigned char *out, cudaStream_t s)
+{
+	const EncodePlan &E = *A.E;
+	const ScanScript &P = E.P;
+	const dim3 per_span((E.max_chunks + 127) / 128, A.cn);
+	/* the frames' own headers, or the chunk's for every frame */
+	const unsigned char *hdr = E.opt ? A.slots : A.tmpl;
+	const size_t hdr_stride = E.opt ? E.slot : 0;
+	const int hend_stride = E.prog ? P.nscans : E.opt ? 1 : 0;
+	const auto copy = E.prog ? jpeg_stuffcopy_kernel<kScanHeaders> : P.restart ? jpeg_stuffcopy_kernel<kRestartMarkers> : jpeg_stuffcopy_kernel<kOneSegment>;
+	copy<<<per_span, 128, 0, s>>>(P, A.totals, A.raw, E.raw_bytes, E.max_chunks, A.counts, hdr, hdr_stride, A.hdr_end, hend_stride, A.istart, A.at, out,
+		A.lengths);
+}
 
-/* n equally sized 8-bit frames (1 or 3 bands) on the device -> n JPEG streams at out + i * out_stride (device), their
- * lengths to lengths_host[n], with vips_jpegsave's options o: sequential with the standard tables or, optimize_coding,
- * per-frame tables from the frame's symbol counts; interlace, progressive with the scan script of jpeg_simple_progression,
- * every scan with its own optimal tables; restart_interval MCUs per restart interval (0: none).  Stream-ordered on s;
- * returns after the lengths are known.
+/* cn equally sized 8-bit frames (1 or 3 bands) at src (device memory) -> their streams, with vips_jpegsave's options:
+ * sequential with the standard tables or, optimize_coding, per-frame tables from the frame's symbol counts; interlace,
+ * progressive with the scan script of jpeg_simple_progression, every scan with its own optimal tables; restart_interval
+ * MCUs per restart interval (0: none).  7 / 8 / 9 / 10 launches per chunk for a sequential stream, 11 for a progressive one.
  */
 int
-dev_jpeg_encode(const char *domain, const void *frames, size_t bpl, size_t frame_stride, int n, int w, int h, int bands, const VB200JpegSaveOptions &o,
-	void *out, size_t out_stride, size_t *lengths_host, cudaStream_t s)
+jpeg_chunk(const char *domain, const EncodePlan &E, const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place,
+	cudaStream_t s)
 {
-	EncodePlan E;
-	if (make_plan(domain, w, h, bands, o, &E))
-		return -1;
-	const Scratch S = carve(E, n);
+	const Scratch S = carve(E, cn);
 	char *scratch = nullptr;
 	if (dev_alloc(domain, (void **) &scratch, S.bytes, s))
 		return -1;
@@ -1838,7 +1839,7 @@ dev_jpeg_encode(const char *domain, const void *frames, size_t bpl, size_t frame
 		if (cudaMemcpyAsync(scratch + S.tab, &E.T, sizeof(E.T), cudaMemcpyHostToDevice, s) != cudaSuccess ||
 			cudaMemcpyAsync(scratch + S.hdr, E.header.data(), E.header.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
 			(!E.opt && cudaMemcpyAsync(scratch + S.hend, &header_len, sizeof(header_len), cudaMemcpyHostToDevice, s) != cudaSuccess) ||
-			cudaMemsetAsync(scratch + S.raw, 0, (size_t) n * E.raw_bytes, s) != cudaSuccess ||
+			cudaMemsetAsync(scratch + S.raw, 0, (size_t) cn * E.raw_bytes, s) != cudaSuccess ||
 			cudaMemsetAsync(scratch + S.bad, 0, sizeof(int), s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode setup");
 			break;
@@ -1846,84 +1847,80 @@ dev_jpeg_encode(const char *domain, const void *frames, size_t bpl, size_t frame
 		ChunkArgs A;
 		A.E = &E;
 		A.T = (const EncodeTables *) (scratch + S.tab);
+		A.frames = src;
 		A.bpl = bpl;
 		A.frame_stride = frame_stride;
+		A.cn = cn;
+		A.coef = (short *) (scratch + S.coef);
+		A.bits = (unsigned *) (scratch + S.bits);
+		A.counts = (unsigned *) (scratch + S.cnt);
+		A.istart = (unsigned *) (scratch + S.ist);
 		A.freq = (unsigned *) (scratch + S.freq);
 		A.hdr_end = (unsigned *) (scratch + S.hend);
+		A.totals = (unsigned long long *) (scratch + S.tot);
+		A.lengths = (unsigned long long *) (scratch + S.len);
+		A.at = (unsigned long long *) (scratch + S.at);
+		A.raw = (unsigned char *) (scratch + S.raw);
 		A.huff = scratch + S.huff;
 		A.tmpl = (const unsigned char *) (scratch + S.hdr);
 		A.slots = (unsigned char *) (scratch + S.slots);
+		A.summ = (unsigned char *) (scratch + S.summ);
+		A.runs = (unsigned *) (scratch + S.runs);
+		A.dslot = (unsigned *) (scratch + S.dslot);
+		A.doff = (unsigned short *) (scratch + S.doff);
 		A.bad = (int *) (scratch + S.bad);
-		A.out_stride = out_stride;
-		unsigned long long *lengths = (unsigned long long *) (scratch + S.len);
-		const size_t units = E.prog ? (size_t) E.P.units : 0;
 		const bool restart = E.P.restart > 0;
-		/* the frame is gridDim.y (or x) of every kernel: chunks of at most kMaxBatchFrames, each on its slice of the scratch */
-		cudaError_t e = cudaSuccess;
-		for (int c0 = 0; c0 < n && e == cudaSuccess; c0 += kMaxBatchFrames) {
-			const size_t f0 = (size_t) c0;
-			A.cn = std::min(kMaxBatchFrames, n - c0);
-			A.frames = (const unsigned char *) frames + f0 * frame_stride;
-			A.coef = (short *) (scratch + S.coef) + f0 * E.G.blocks * 64;
-			A.bits = (unsigned *) (scratch + S.bits) + f0 * E.nslots;
-			A.totals = (unsigned long long *) (scratch + S.tot) + f0;
-			A.lengths = lengths + f0;
-			A.raw = (unsigned char *) (scratch + S.raw) + f0 * E.raw_bytes;
-			A.counts = (unsigned *) (scratch + S.cnt) + f0 * E.max_chunks;
-			A.istart = (unsigned *) (scratch + S.ist) + f0 * E.P.nseg;
-			A.summ = (unsigned char *) (scratch + S.summ) + f0 * units;
-			A.runs = (unsigned *) (scratch + S.runs) + f0 * kProgSlotsPerUnit * units;
-			A.dslot = (unsigned *) (scratch + S.dslot) + f0 * units;
-			A.doff = (unsigned short *) (scratch + S.doff) + f0 * units;
-			A.out = (unsigned char *) out + f0 * out_stride;
-			const int launches = E.prog ? launch_progressive(A, s)
-							   : E.opt	? (restart ? launch_chunk<true, true>(A, s) : launch_chunk<true, false>(A, s))
-										: (restart ? launch_chunk<false, true>(A, s) : launch_chunk<false, false>(A, s));
-			e = cudaGetLastError();
-			if (e == cudaSuccess && launches < 0)
-				e = cudaErrorUnknown;
-			if (e == cudaSuccess)
-				count_launch(launches);
-		}
+		const int launches = E.prog ? launch_progressive(A, s)
+						   : E.opt	? (restart ? launch_chunk<true, true>(A, s) : launch_chunk<true, false>(A, s))
+									: (restart ? launch_chunk<false, true>(A, s) : launch_chunk<false, false>(A, s));
+		cudaError_t e = cudaGetLastError();
+		if (e == cudaSuccess && launches < 0)
+			e = cudaErrorUnknown;
 		if (e != cudaSuccess) {
 			cuda_fail(domain, e, "jpeg encode kernels launch");
 			break;
 		}
-		std::vector<unsigned long long> len(n);
+		count_launch(launches);
+		/* read back with the lengths: place synchronises */
 		int bad = 0;
-		if (cudaMemcpyAsync(len.data(), lengths, (size_t) n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-			cudaMemcpyAsync(&bad, scratch + S.bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
+		unsigned char *out = nullptr;
+		if (cudaMemcpyAsync(&bad, scratch + S.bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess) {
 			cuda_fail(domain, cudaGetLastError(), "jpeg encode");
 			break;
 		}
+		if (place(A.lengths, sizeof(unsigned long long), A.at, &out))
+			break;
 		if (bad) {
 			/* libjpeg's JERR_HUFF_CLEN_OVERFLOW: a symbol distribution no image of the sizes taken here produces */
 			error(domain, "optimised Huffman table: a code longer than 32 bits");
 			break;
 		}
-		rc = 0;
-		for (int i = 0; i < n; i++) {
-			if (lengths_host)
-				lengths_host[i] = (size_t) len[i];
-			if (len[i] > out_stride) {
-				error(domain, "frame %d: the stream takes %llu bytes, the output stride is %zu", i, len[i], out_stride);
-				rc = -1;
-			}
+		launch_stuffcopy(A, out, s);
+		count_launch(1);
+		if ((e = cudaGetLastError()) != cudaSuccess) {
+			cuda_fail(domain, e, "jpeg_stuffcopy_kernel");
+			break;
 		}
+		rc = 0;
 	} while (0);
 	dev_free(scratch, s);
 	return rc;
 }
 
+} // namespace
+
 int
-jpeg_encode_room(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, size_t *stream_bytes, size_t *scratch_bytes)
+jpeg_encoder(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, Encoder *enc)
 {
 	EncodePlan E;
 	if (make_plan(domain, w, h, bands, o, &E))
 		return -1;
+	enc->scratch_bytes = carve(E, 1).bytes;
 	/* the header slot, the raw data's bound, FF Dn or a scan header (counted in the slot) before each segment, EOI */
-	*stream_bytes = E.slot + E.scan_bound + 2 * (size_t) E.P.nseg + 2;
-	*scratch_bytes = carve(E, 1).bytes;
+	enc->stream_bytes = E.slot + E.scan_bound + 2 * (size_t) E.P.nseg + 2;
+	enc->chunk = [domain, E](const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place, cudaStream_t s) {
+		return jpeg_chunk(domain, E, src, bpl, frame_stride, cn, place, s);
+	};
 	return 0;
 }
 
@@ -2401,67 +2398,7 @@ vb200_jpegsave_batch_opts(const void *frames, int frames_location, size_t bpl, s
 	const VB200JpegSaveOptions *opt, void *out, int out_location, size_t out_stride, size_t *lengths)
 {
 	const char *domain = "jpegsave_batch";
-	if (!frames || !out || !opt || n < 1) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (check_restart(domain, opt->restart_interval))
-		return -1;
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	const size_t line = (size_t) width * bands;
-	if (bpl < line || (n > 1 && frame_stride < bpl * height)) {
-		error(domain, "frame strides too small for %d x %d x %d", width, height, bands);
-		return -1;
-	}
-	void *din = nullptr, *dout = nullptr;
-	int rc = -1;
-	do {
-		const void *src = frames;
-		size_t sbpl = bpl, sstride = frame_stride;
-		if (frames_location != VB200_DEVICE) {
-			if (dev_alloc(domain, &din, line * height * n, s))
-				break;
-			bool bad = false;
-			for (int i = 0; i < n && !bad; i++)
-				bad = cudaMemcpy2DAsync((char *) din + (size_t) i * line * height, line, (const char *) frames + (size_t) i * frame_stride, bpl, line,
-						  height, cudaMemcpyHostToDevice, s) != cudaSuccess;
-			if (bad) {
-				cuda_fail(domain, cudaGetLastError(), "copy to device");
-				break;
-			}
-			src = din;
-			sbpl = line;
-			sstride = line * height;
-		}
-		void *dst = out;
-		if (out_location != VB200_DEVICE) {
-			if (dev_alloc(domain, &dout, out_stride * n, s))
-				break;
-			dst = dout;
-		}
-		std::vector<size_t> len(n);
-		if (dev_jpeg_encode(domain, src, sbpl, sstride, n, width, height, bands, *opt, dst, out_stride, len.data(), s))
-			break;
-		if (lengths)
-			memcpy(lengths, len.data(), n * sizeof(size_t));
-		if (out_location != VB200_DEVICE) {
-			bool bad = false;
-			for (int i = 0; i < n && !bad; i++)
-				bad = cudaMemcpyAsync((char *) out + (size_t) i * out_stride, (char *) dout + (size_t) i * out_stride, len[i], cudaMemcpyDeviceToHost,
-						  s) != cudaSuccess;
-			if (bad || cudaStreamSynchronize(s) != cudaSuccess) {
-				cuda_fail(domain, cudaGetLastError(), "copy to host");
-				break;
-			}
-		}
-		rc = 0;
-	} while (0);
-	if (din)
-		dev_free(din, s);
-	if (dout)
-		dev_free(dout, s);
-	return rc;
+	return encode_batch_abi(domain, opt, [&](Encoder *enc) { return jpeg_encoder(domain, width, height, bands, *opt, enc); }, frames, frames_location, bpl,
+		frame_stride, n, width, height, bands, out, out_location, out_stride, lengths);
 }
 

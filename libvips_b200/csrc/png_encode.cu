@@ -1297,143 +1297,88 @@ align256(size_t v)
 	return (v + 255) & ~(size_t) 255;
 }
 
-/* device bytes one frame takes in a chunk: the encoder's scratch, its input when that comes from the host, and its stream
- * when that goes back to the host */
-size_t
-frame_bytes(const EncGeom &g, bool host_in, bool host_out)
+/* the kernels of cn frames at src (device memory): filter, deflate, then place and png_frame_kernel */
+int
+png_chunk(const char *domain, const EncGeom &g, const std::vector<unsigned char> &prefix, const unsigned char *src, size_t bpl, size_t frame_stride,
+	int cn, const EncodePlace &place, cudaStream_t s)
 {
-	return g.scan_stride + align256(4 * g.n) + align256((size_t) 2 * kWSize * g.tiles) + align256(8 * g.n) + align256(4 * g.n) +
-		align256(g.maxblk * (sizeof(BlockRec) + sizeof(DeflatePlan))) + g.zcap + sizeof(FrameOut) + sizeof(unsigned long long) +
-		(host_in ? align256(g.rb * g.h) : 0) + (host_out ? g.prefix + g.zcap + 12 * (size_t) g.maxchunks + 12 : 0);
+	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_last_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 4));
+	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 2));
+	unsigned char *dev = nullptr;
+	const size_t off_prev = align256(g.scan_stride * cn), off_last = off_prev + align256(4 * g.n * cn),
+				 off_rec = off_last + align256((size_t) 2 * kWSize * g.tiles * cn), off_sym = off_rec + align256(8 * g.n * cn),
+				 off_blk = off_sym + align256(4 * g.n * cn), off_plan = off_blk + align256(sizeof(BlockRec) * g.maxblk * cn),
+				 off_zs = off_plan + align256(sizeof(DeflatePlan) * g.maxblk * cn), off_fo = off_zs + align256(g.zcap * cn),
+				 off_at = off_fo + align256(sizeof(FrameOut) * cn), off_pre = off_at + align256(sizeof(unsigned long long) * cn),
+				 total = off_pre + align256(prefix.size());
+	if (dev_alloc(domain, (void **) &dev, total, s))
+		return -1;
+	unsigned char *scan = dev;
+	unsigned *prev = (unsigned *) (dev + off_prev), *sym = (unsigned *) (dev + off_sym), *zs = (unsigned *) (dev + off_zs);
+	unsigned short *last = (unsigned short *) (dev + off_last);
+	uint2 *rec = (uint2 *) (dev + off_rec);
+	BlockRec *blk = (BlockRec *) (dev + off_blk);
+	DeflatePlan *plans = (DeflatePlan *) (dev + off_plan);
+	FrameOut *fo = (FrameOut *) (dev + off_fo);
+	unsigned long long *at_out = (unsigned long long *) (dev + off_at);
+	unsigned char *dpre = dev + off_pre, *out = nullptr;
+	int rc = -1;
+	do {
+		if (cudaMemsetAsync(zs, 0, g.zcap * cn, s) != cudaSuccess ||
+			cudaMemcpyAsync(dpre, prefix.data(), prefix.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) {
+			cuda_fail(domain, cudaGetLastError(), "png save staging");
+			break;
+		}
+		const unsigned gx = (unsigned) std::min<size_t>((g.scan_stride + 255) / 256, 4096);
+		png_filter_kernel<<<dim3(gx, cn), 256, 0, s>>>(src, bpl, frame_stride, g, scan);
+		png_adler_kernel<<<cn, 256, 0, s>>>(scan, g, fo);
+		deflate_last_kernel<<<dim3(g.tiles, cn), 1024, kWSize * 4, s>>>(scan, g, last);
+		deflate_chain_kernel<<<dim3(g.tiles, cn), 32, kWSize * 2, s>>>(scan, g, last, prev);
+		const unsigned mx = (unsigned) std::min<size_t>((g.n + 127) / 128, 1 << 20);
+		deflate_match_kernel<<<dim3(mx, cn), 128, 0, s>>>(scan, g, prev, rec);
+		deflate_parse_kernel<<<(cn + kParseWarps - 1) / kParseWarps, kParseWarps * 32, 0, s>>>(scan, g, cn, rec, sym, blk, fo);
+		const unsigned bx = (unsigned) ((g.maxblk + kBlockWarps - 1) / kBlockWarps);
+		deflate_block_kernel<<<dim3(bx, cn), kBlockWarps * 32, 0, s>>>(g, sym, blk, plans, fo);
+		deflate_offsets_kernel<<<(cn + 127) / 128, 128, 0, s>>>(g, cn, blk, plans, zs, fo);
+		deflate_emit_kernel<<<dim3(bx, cn), kBlockWarps * 32, 0, s>>>(g, scan, sym, blk, plans, fo, zs);
+		count_launch(9);
+		cudaError_t e = cudaGetLastError();
+		if (e != cudaSuccess) {
+			cuda_fail(domain, e, "png save kernels");
+			break;
+		}
+		if (place(&fo->len, sizeof(FrameOut), at_out, &out))
+			break;
+		png_frame_kernel<<<dim3((g.maxchunks + 7) / 8, cn), 256, 0, s>>>(g, dpre, zs, fo, at_out, out);
+		count_launch(1);
+		e = cudaGetLastError();
+		if (e != cudaSuccess) {
+			cuda_fail(domain, e, "png_frame_kernel");
+			break;
+		}
+		rc = 0;
+	} while (0);
+	dev_free(dev, s);
+	return rc;
 }
 
 } // namespace
 
-/* n frames (host or device memory) -> n PNG streams at out + i * out_stride (host or device memory), lens[i] bytes.  The
- * frames go in chunks bounded by the device budget; a frame larger than the budget runs alone.  A stream longer than
- * out_stride fails the call before its chunk writes anything; streams for the host are packed on the device, copied back in
- * one piece per chunk, and placed in out only once every chunk has succeeded. */
 int
-dev_png_encode(const char *domain, const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int w, int h, int bands,
-	const VB200PngSaveOptions &o, const unsigned char *profile, size_t profile_len, void *out, int out_location, size_t out_stride, size_t *lens,
-	cudaStream_t s)
+png_encoder(const char *domain, int w, int h, int bands, const VB200PngSaveOptions &o, const unsigned char *profile, size_t profile_len,
+	Encoder *enc)
 {
+	if (check_save(domain, w, h, bands, o))
+		return -1;
 	const std::vector<unsigned char> prefix = png_prefix(w, h, bands, o, profile, profile_len);
 	const EncGeom g = enc_geom(w, h, bands, o, prefix.size());
-	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_last_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 4));
-	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 2));
-	const bool host_in = frames_location != VB200_DEVICE, host_out = out_location != VB200_DEVICE;
-	const size_t frame_in = g.rb * g.h, budget = decode_chunk_budget(), per = frame_bytes(g, host_in, host_out);
-	std::vector<unsigned char> staged; /* host output: the batch's streams, packed */
-	std::vector<size_t> staged_at(n);
-	int rc = 0;
-	for (int c0 = 0; c0 < n && !rc;) {
-		const int cn = (int) std::min<size_t>({(size_t) (n - c0), (size_t) kMaxBatchFrames, std::max<size_t>(1, budget / per)});
-		unsigned char *dev = nullptr, *packed = nullptr;
-		const size_t off_prev = align256(g.scan_stride * cn), off_last = off_prev + align256(4 * g.n * cn),
-					 off_rec = off_last + align256((size_t) 2 * kWSize * g.tiles * cn), off_sym = off_rec + align256(8 * g.n * cn),
-					 off_blk = off_sym + align256(4 * g.n * cn), off_plan = off_blk + align256(sizeof(BlockRec) * g.maxblk * cn),
-					 off_zs = off_plan + align256(sizeof(DeflatePlan) * g.maxblk * cn), off_fo = off_zs + align256(g.zcap * cn),
-					 off_at = off_fo + align256(sizeof(FrameOut) * cn), off_pre = off_at + align256(sizeof(unsigned long long) * cn),
-					 off_in = off_pre + align256(prefix.size()), total = off_in + (host_in ? align256(frame_in * cn) : 0);
-		if (dev_alloc(domain, (void **) &dev, total, s)) {
-			rc = -1;
-			break;
-		}
-		unsigned char *scan = dev;
-		unsigned *prev = (unsigned *) (dev + off_prev), *sym = (unsigned *) (dev + off_sym), *zs = (unsigned *) (dev + off_zs);
-		unsigned short *last = (unsigned short *) (dev + off_last);
-		uint2 *rec = (uint2 *) (dev + off_rec);
-		BlockRec *blk = (BlockRec *) (dev + off_blk);
-		DeflatePlan *plans = (DeflatePlan *) (dev + off_plan);
-		FrameOut *fo = (FrameOut *) (dev + off_fo);
-		unsigned long long *at_out = (unsigned long long *) (dev + off_at);
-		unsigned char *dpre = dev + off_pre;
-		std::vector<FrameOut> hfo(cn);
-		std::vector<unsigned long long> hat(cn);
-		do {
-			const unsigned char *src = (const unsigned char *) frames + (size_t) c0 * frame_stride;
-			size_t sbpl = bpl, sstride = frame_stride;
-			bool bad = cudaMemsetAsync(zs, 0, g.zcap * cn, s) != cudaSuccess ||
-				cudaMemcpyAsync(dpre, prefix.data(), prefix.size(), cudaMemcpyHostToDevice, s) != cudaSuccess;
-			if (host_in && !bad) {
-				unsigned char *din = dev + off_in;
-				if (bpl == g.rb && (cn == 1 || frame_stride == frame_in))
-					bad = cudaMemcpyAsync(din, src, frame_in * cn, cudaMemcpyHostToDevice, s) != cudaSuccess;
-				for (int i = 0; i < cn && !bad && !(bpl == g.rb && (cn == 1 || frame_stride == frame_in)); i++)
-					bad = cudaMemcpy2DAsync(din + (size_t) i * frame_in, g.rb, src + (size_t) i * frame_stride, bpl, g.rb, g.h, cudaMemcpyHostToDevice,
-							  s) != cudaSuccess;
-				src = din;
-				sbpl = g.rb;
-				sstride = frame_in;
-			}
-			if (bad) {
-				rc = cuda_fail(domain, cudaGetLastError(), "png save staging");
-				break;
-			}
-			const unsigned gx = (unsigned) std::min<size_t>((g.scan_stride + 255) / 256, 4096);
-			png_filter_kernel<<<dim3(gx, cn), 256, 0, s>>>(src, sbpl, sstride, g, scan);
-			png_adler_kernel<<<cn, 256, 0, s>>>(scan, g, fo);
-			deflate_last_kernel<<<dim3(g.tiles, cn), 1024, kWSize * 4, s>>>(scan, g, last);
-			deflate_chain_kernel<<<dim3(g.tiles, cn), 32, kWSize * 2, s>>>(scan, g, last, prev);
-			const unsigned mx = (unsigned) std::min<size_t>((g.n + 127) / 128, 1 << 20);
-			deflate_match_kernel<<<dim3(mx, cn), 128, 0, s>>>(scan, g, prev, rec);
-			deflate_parse_kernel<<<(cn + kParseWarps - 1) / kParseWarps, kParseWarps * 32, 0, s>>>(scan, g, cn, rec, sym, blk, fo);
-			const unsigned bx = (unsigned) ((g.maxblk + kBlockWarps - 1) / kBlockWarps);
-			deflate_block_kernel<<<dim3(bx, cn), kBlockWarps * 32, 0, s>>>(g, sym, blk, plans, fo);
-			deflate_offsets_kernel<<<(cn + 127) / 128, 128, 0, s>>>(g, cn, blk, plans, zs, fo);
-			deflate_emit_kernel<<<dim3(bx, cn), kBlockWarps * 32, 0, s>>>(g, scan, sym, blk, plans, fo, zs);
-			count_launch(9);
-			cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess || cudaMemcpyAsync(hfo.data(), fo, sizeof(FrameOut) * cn, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-				cudaStreamSynchronize(s) != cudaSuccess) {
-				rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "png save kernels");
-				break;
-			}
-			/* where each stream goes: packed for the host, its slot on the device */
-			unsigned long long packed_bytes = 0;
-			for (int i = 0; i < cn && !rc; i++) {
-				lens[c0 + i] = hfo[i].len;
-				if (hfo[i].len > out_stride) {
-					error(domain, "frame %d: its %llu-byte stream does not fit the %zu-byte slot", c0 + i, hfo[i].len, out_stride);
-					rc = -1;
-				}
-				hat[i] = host_out ? packed_bytes : (unsigned long long) (c0 + i) * out_stride;
-				packed_bytes += hfo[i].len;
-			}
-			if (rc)
-				break;
-			if (host_out && dev_alloc(domain, (void **) &packed, packed_bytes, s)) {
-				rc = -1;
-				break;
-			}
-			if (cudaMemcpyAsync(at_out, hat.data(), sizeof(unsigned long long) * cn, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-				rc = cuda_fail(domain, cudaGetLastError(), "png save offsets");
-				break;
-			}
-			png_frame_kernel<<<dim3((g.maxchunks + 7) / 8, cn), 256, 0, s>>>(g, dpre, zs, fo, at_out, host_out ? packed : (unsigned char *) out);
-			count_launch(1);
-			e = cudaGetLastError();
-			if (e == cudaSuccess && host_out) {
-				const size_t at = staged.size();
-				staged.resize(at + packed_bytes);
-				for (int i = 0; i < cn; i++)
-					staged_at[c0 + i] = at + hat[i];
-				if (cudaMemcpyAsync(staged.data() + at, packed, packed_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-					e = cudaGetLastError();
-			}
-			if (e != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "png_frame_kernel");
-		} while (0);
-		if (packed)
-			dev_free(packed, s);
-		dev_free(dev, s);
-		c0 += cn;
-	}
-	if (!rc && host_out)
-		for (int i = 0; i < n; i++)
-			memcpy((unsigned char *) out + (size_t) i * out_stride, staged.data() + staged_at[i], lens[i]);
-	return rc;
+	enc->scratch_bytes = g.scan_stride + align256(4 * g.n) + align256((size_t) 2 * kWSize * g.tiles) + align256(8 * g.n) + align256(4 * g.n) +
+		align256(g.maxblk * (sizeof(BlockRec) + sizeof(DeflatePlan))) + g.zcap + sizeof(FrameOut) + sizeof(unsigned long long);
+	enc->stream_bytes = g.prefix + g.zcap + 12 * (size_t) g.maxchunks + 12;
+	enc->chunk = [domain, g, prefix](const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place, cudaStream_t s) {
+		return png_chunk(domain, g, prefix, src, bpl, frame_stride, cn, place, s);
+	};
+	return 0;
 }
 
 /* the whole PNG stream on the CPU through the kernels' per-position, per-symbol and per-block code */
@@ -1466,25 +1411,9 @@ vb200_pngsave_batch(const void *frames, int frames_location, size_t bpl, size_t 
 	const VB200PngSaveOptions *options, const void *profile, size_t profile_len, void *out, int out_location, size_t out_stride, size_t *lengths)
 {
 	const char *domain = "pngsave_batch";
-	if (!frames || !out || !options || !lengths || n < 1) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (check_save(domain, width, height, bands, *options))
-		return -1;
-	const size_t line = (size_t) width * bands;
-	if (bpl < line || (n > 1 && frame_stride < bpl * height)) {
-		error(domain, "frame strides too small for %d x %d x %d", width, height, bands);
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	std::vector<size_t> len(n);
-	if (dev_png_encode(domain, frames, frames_location, bpl, frame_stride, n, width, height, bands, *options, (const unsigned char *) profile,
-			profile_len, out, out_location, out_stride, len.data(), current_stream()))
-		return -1;
-	memcpy(lengths, len.data(), n * sizeof(size_t));
-	return 0;
+	return encode_batch_abi(domain, options,
+		[&](Encoder *enc) { return png_encoder(domain, width, height, bands, *options, (const unsigned char *) profile, profile_len, enc); }, frames,
+		frames_location, bpl, frame_stride, n, width, height, bands, out, out_location, out_stride, lengths);
 }
 
 /* reference: vips_pngsave_buffer(in, &buf, &len, "compression", .., NULL), foreign/spngsave.c */
@@ -1500,21 +1429,26 @@ vb200_pngsave_buffer(const VB200Image *in, const VB200PngSaveOptions *options, c
 		error(domain, "format %d: PNG save on the device takes uchar frames (bit depth 8; 16-bit is not built)", in->BandFmt);
 		return -1;
 	}
-	if (check_save(domain, in->Xsize, in->Ysize, in->Bands, *options))
+	const size_t line = (size_t) in->Xsize * in->Bands;
+	if (in->bpl < line) {
+		error(domain, "frame strides too small for %d x %d x %d", in->Xsize, in->Ysize, in->Bands);
 		return -1;
-	const size_t line = (size_t) in->Xsize * in->Bands, n = (size_t) in->Ysize * (line + 1);
-	const size_t stride = n + n / 8 + 400 * (n / kMaxSyms + 2) + 12 * (n / kIdat + 2) + 2 * profile_len + 4096;
-	void *buf = malloc(stride);
+	}
+	Encoder enc;
+	if (png_encoder(domain, in->Xsize, in->Ysize, in->Bands, *options, (const unsigned char *) profile, profile_len, &enc) || ensure_init(domain))
+		return -1;
+	std::vector<unsigned char> bytes;
+	EncodeDest dst;
+	dst.bytes = &bytes;
+	size_t got = 0;
+	if (dev_encode_batch(domain, enc, in->data, in->where, in->bpl, in->bpl * in->Ysize, 1, line, in->Ysize, dst, &got, current_stream()))
+		return -1;
+	void *buf = malloc(got);
 	if (!buf) {
 		error(domain, "out of memory");
 		return -1;
 	}
-	size_t got = 0;
-	if (vb200_pngsave_batch(in->data, in->where, in->bpl, in->bpl * in->Ysize, 1, in->Xsize, in->Ysize, in->Bands, options, profile, profile_len, buf,
-			VB200_HOST, stride, &got)) {
-		free(buf);
-		return -1;
-	}
+	memcpy(buf, bytes.data(), got);
 	*out = buf;
 	*len = got;
 	return 0;

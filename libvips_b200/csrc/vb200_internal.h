@@ -225,10 +225,10 @@ int parse_streams(const char *domain, const char *noun, int n, const std::functi
 	const std::function<StreamGeometry(int)> &geometry, StreamGeometry *g);
 /* out_bpl and out_frame_stride hold frames of geometry g */
 int check_out_strides(const char *domain, const StreamGeometry &g, size_t out_bpl, size_t out_frame_stride);
-/* device bytes per chunk of the PNG and GIF decoders and the PNG encoder (vb200_debug_png_set_budget; 0: an eighth of the
- * device, at least 1 GiB) */
-size_t decode_chunk_budget();
-/* chunk(c0, cn) for consecutive streams [c0, c0 + cn) whose device_bytes fit decode_chunk_budget() (at least one: -1 when
+/* device bytes per chunk of the PNG and GIF decoders and the JPEG and PNG encoders (vb200_debug_png_set_budget; 0: an eighth
+ * of the device, at least 1 GiB) */
+size_t chunk_budget();
+/* chunk(c0, cn) for consecutive streams [c0, c0 + cn) whose device_bytes fit chunk_budget() (at least one: -1 when
  * that one alone does not), one decode at a time, so that chunk may use decode_staging() */
 int decode_chunks(const char *domain, const char *noun, int n, const std::function<size_t(int)> &device_bytes, const std::function<int(int, int)> &chunk);
 /* the pinned staging block, grow-only, at least bytes long (nullptr: cudaMallocHost failed, with the reason) */
@@ -246,11 +246,39 @@ int host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, i
 	int restart, std::vector<unsigned char> &out);
 int host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
 	int restart, std::vector<unsigned char> &out, unsigned long long *events);
-/* jpeg_encode.cu: the room the device encoder needs for w x h x bands frames with options o: *stream_bytes, a stream's
- * bound (its header slot, the bound its scan data is sized by, the markers between segments, EOI), and *scratch_bytes,
- * the device scratch it takes per frame of a batch
+/* encode.cu: the encoders' shared driver.  place(lengths, length_stride, at, &out), which an encoder's chunk calls once its
+ * kernels have the streams' lengths (device memory, an unsigned long long every length_stride bytes), reads them back,
+ * fails the call for a stream longer than its slot, and stores where each stream goes: stream i at out + at[i] (at: the
+ * encoder's device array of the chunk's frames).
  */
-int jpeg_encode_room(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, size_t *stream_bytes, size_t *scratch_bytes);
+using EncodePlace = std::function<int(const void *lengths, size_t length_stride, unsigned long long *at, unsigned char **out)>;
+struct Encoder {
+	size_t scratch_bytes = 0; /* device scratch per frame of a chunk */
+	size_t stream_bytes = 0;  /* a stream's bound: its device room when the streams go to the host */
+	/* cn frames on the device (bpl, frame_stride apart): the kernels through the lengths, place, then the write kernel at the
+	 * places given */
+	std::function<int(const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place, cudaStream_t s)> chunk;
+};
+/* the encoders: the option and geometry checks (0, or -1 with the reason) and, without a device call, *enc */
+int jpeg_encoder(const char *domain, int w, int h, int bands, const VB200JpegSaveOptions &o, Encoder *enc);
+int png_encoder(const char *domain, int w, int h, int bands, const VB200PngSaveOptions &o, const unsigned char *profile, size_t profile_len,
+	Encoder *enc);
+/* where the streams go: device slots (stream i at dev + i * slot), or packed host bytes appended to *bytes (stream i at
+ * (*bytes)[at[i]]).  A stream longer than slot fails the call before its chunk writes anything. */
+struct EncodeDest {
+	size_t slot = SIZE_MAX;
+	unsigned char *dev = nullptr;
+	std::vector<unsigned char> *bytes = nullptr;
+	std::vector<size_t> at;
+};
+/* n frames (host or device memory, rows of `line` bytes) -> n streams into dst, lengths[n], in chunks bounded by
+ * chunk_budget() (a frame larger than the budget runs alone); returns with the chunks' work done */
+int dev_encode_batch(const char *domain, const Encoder &enc, const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n,
+	size_t line, int h, EncodeDest &dst, size_t *lengths, cudaStream_t s);
+/* the body of vb200_jpegsave_batch_opts and vb200_pngsave_batch: every argument checked, then make(&enc), before any device
+ * call; streams for the host placed in out only once every chunk has succeeded (lengths may be null) */
+int encode_batch_abi(const char *domain, const void *options, const std::function<int(Encoder *)> &make, const void *frames, int frames_location,
+	size_t bpl, size_t frame_stride, int n, int w, int h, int bands, void *out, int out_location, size_t out_stride, size_t *lengths);
 /* min(hshrink, vshrink) of vips_thumbnail_calculate_shrink, thumbnail.c:413-487 */
 double thumbnail_common_shrink(int w, int h, int tw, int th, int size);
 void jpeg_pump_release(); /* the JPEG pump's pinned / device slots (jpeg.cu); vb200_shutdown */
