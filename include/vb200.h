@@ -703,9 +703,17 @@ int vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, 
  * compression: zlib level (:700-705, default 6); 4-9 are built, 0-3 return -1 with the reason.  strategy: 0
  *   Z_DEFAULT_STRATEGY (libpng's choice for unfiltered images), 1 Z_FILTERED.  xres: pixels per millimetre (libvips' Xres,
  *   default 1.0).
+ * filter (:714-720, :449-450): a VipsForeignPngFilter flag -- NONE 0x08, SUB 0x10, UP 0x20, AVG 0x40, PAETH 0x80 -- or 0
+ *   for NONE; every scanline is filtered with that type (PNG 2nd edition 9.2) on the raw bytes.  interlace (:707-712,
+ *   :439): non-zero writes Adam7 scanlines and IHDR interlace 1.  bitdepth (:743-748): 0 or 8, or 1 / 2 / 4 for one band,
+ *   written as grey without a palette: each sample p >> (8 - bitdepth), packed MSB first as vips_foreign_save_spng_pack
+ *   packs it (:295-324), its tail rule included (at depth 4 an odd-width row ends in v[w-2] << 4 | v[w-1]).  With all three
+ *   0 the streams are what they were before these fields existed.
  * Declined (-1 with the reason; the host keeps spngsave): compression 0-3, another strategy, bands outside 1-4, frames over
- *   2^28 pixels, a format other than uchar (vb200_pngsave_buffer).  Filters other than NONE, interlace, palette and
- *   metadata chunks other than iCCP are not written.
+ *   2^28 pixels, a format other than uchar (vb200_pngsave_buffer), unknown filter bits, more than one filter flag
+ *   (libspng's adaptive choice, ALL = 0xF8), bitdepth 16 or other than 1 / 2 / 4 / 8, bitdepth below 8 with 2 bands (no
+ *   low-bit grey + alpha in PNG) or 3-4 bands (spngsave palettises; quantisation is not built), bitdepth below 8 with a
+ *   filter other than NONE or with interlace.  Palette output and metadata chunks other than iCCP are not written.
  * vb200_pngsave_batch: n frames of one geometry in host or device memory (frames_location); stream i at out + i *
  *   out_stride (out_location), lengths[i] bytes (host array, may be NULL).  A stream that does not fit out_stride returns -1
  *   with its frame before its chunk writes anything: with out in host memory nothing is written then, in device memory the
@@ -716,11 +724,15 @@ int vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, 
  *   per-block code compiled for the CPU.  out = NULL only reports *len.
  * vb200_debug_deflate: test hook, host only -- the zlib stream (header, deflate data, Adler-32) of buf[0, n) at a level
  *   and strategy, through the same code.  out = NULL only reports *len.
+ * The struct grew by filter, interlace and bitdepth, its last members: C callers rebuild against this header.
  */
 typedef struct {
 	int compression;
 	int strategy;
 	double xres;
+	int filter;
+	int interlace;
+	int bitdepth;
 } VB200PngSaveOptions;
 int vb200_pngsave_batch(const void *frames, int frames_location, size_t bpl, size_t frame_stride, int n, int width, int height, int bands,
 	const VB200PngSaveOptions *options, const void *profile, size_t profile_len, void *out, int out_location, size_t out_stride, size_t *lengths);

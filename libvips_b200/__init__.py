@@ -121,14 +121,17 @@ class JpegSaveOptions(C.Structure):
 
 class PngSaveOptions(C.Structure):
     """VB200PngSaveOptions"""
-    _fields_ = [("compression", C.c_int), ("strategy", C.c_int), ("xres", C.c_double)]
+    _fields_ = [("compression", C.c_int), ("strategy", C.c_int), ("xres", C.c_double), ("filter", C.c_int), ("interlace", C.c_int),
+                ("bitdepth", C.c_int)]
 
 
 PNG_STRATEGIES = {"default": 0, "filtered": 1}
+PNG_FILTERS = {"none": 0x08, "sub": 0x10, "up": 0x20, "avg": 0x40, "paeth": 0x80, "all": 0xF8}   # VipsForeignPngFilter
 
 
-def _png_options(compression, strategy, xres):
-    return PngSaveOptions(int(compression), PNG_STRATEGIES.get(strategy, strategy), float(xres))
+def _png_options(compression, strategy, xres, filter="none", interlace=False, bitdepth=8):
+    return PngSaveOptions(int(compression), PNG_STRATEGIES.get(strategy, strategy), float(xres), int(PNG_FILTERS.get(filter, filter)),
+                          int(bool(interlace)), int(bitdepth))
 
 
 class DzOptions(C.Structure):
@@ -546,10 +549,11 @@ class Image:
         """vips_dzsave: the Deep Zoom / Zoomify tile pyramid of this image -> DzPyramid (see dzsave())"""
         return dzsave(self, basename, **options)
 
-    def pngsave_buffer(self, compression=6, strategy="default", xres=1.0, profile=None):
-        """vips_pngsave_buffer: this uchar image (1-4 bands) as a PNG stream (bytes), deflated on the device"""
+    def pngsave_buffer(self, compression=6, strategy="default", xres=1.0, profile=None, filter="none", interlace=False, bitdepth=8):
+        """vips_pngsave_buffer: this uchar image (1-4 bands) as a PNG stream (bytes), deflated on the device; filter, interlace
+        and bitdepth as in pngsave_batch"""
         cin = self._c()
-        opts = _png_options(compression, strategy, xres)
+        opts = _png_options(compression, strategy, xres, filter, interlace, bitdepth)
         prof = bytes(profile) if profile else None
         p, n = C.c_void_p(), C.c_size_t()
         _check(lib().vb200_pngsave_buffer(C.byref(cin), C.byref(opts), prof, len(prof) if prof else 0, C.byref(p), C.byref(n)))
@@ -794,29 +798,45 @@ def jpegsave_batch(frames, Q=75, subsample_mode="auto", in_ptr=None, shape=None,
     return _save_batch(lib().vb200_jpegsave_batch_opts, opts, frames, in_ptr, shape, stride or (lambda w, h, bands: w * h * bands * 2 + 4096))
 
 
-def _png_stride(w, h, bands, profile):
+ADAM7 = ((0, 0, 8, 8), (4, 0, 8, 8), (0, 4, 4, 8), (2, 0, 4, 4), (0, 2, 2, 4), (1, 0, 2, 2), (0, 1, 1, 2))   # (x0, y0, dx, dy)
+
+
+def _png_scan_bytes(w, h, bands, interlace=False, bitdepth=8):
+    """the scanline bytes of a frame: every non-empty pass's rows, each its filter byte and its packed samples"""
+    n = 0
+    for x0, y0, dx, dy in (ADAM7 if interlace else ((0, 0, 1, 1),)):
+        pw, ph = max(0, -(-(w - x0) // dx)), max(0, -(-(h - y0) // dy))
+        if pw and ph:
+            n += ph * ((pw * bands * bitdepth + 7) // 8 + 1)
+    return n
+
+
+def _png_stride(w, h, bands, profile, interlace=False, bitdepth=8):
     """a slot no stream of a w x h x bands frame can overflow: fixed codes cost at most 9 bits a byte"""
-    n = h * (w * bands + 1)
+    n = _png_scan_bytes(w, h, bands, interlace, bitdepth or 8)
     return n + n // 8 + 400 * (n // 16383 + 2) + 12 * (n // 8192 + 2) + 2 * len(profile or b"") + 4096
 
 
-def pngsave_batch(frames, compression=6, strategy="default", xres=1.0, profile=None, in_ptr=None, shape=None, stride=None):
+def pngsave_batch(frames, compression=6, strategy="default", xres=1.0, profile=None, in_ptr=None, shape=None, stride=None, filter="none",
+                  interlace=False, bitdepth=8):
     """vips_pngsave_buffer() of every frame of a uint8 array [n, h, w, bands] (bands 1-4) on the device -> list of bytes.
     in_ptr / shape: frames already on the device (packed), shape = (n, h, w, bands).  compression 4-9; strategy "default"
-    or "filtered"; xres in pixels per millimetre; profile: ICC bytes written as iCCP.  stride: bytes per output slot."""
+    or "filtered"; xres in pixels per millimetre; profile: ICC bytes written as iCCP.  stride: bytes per output slot.
+    filter: "none", "sub", "up", "avg" or "paeth" (or a VipsForeignPngFilter flag), every scanline filtered with it;
+    interlace: Adam7; bitdepth 1 / 2 / 4 (one band, filter none, not interlaced) or 8."""
     prof = bytes(profile) if profile else None
-    return _save_batch(lib().vb200_pngsave_batch, _png_options(compression, strategy, xres), frames, in_ptr, shape,
-                       stride or (lambda w, h, bands: _png_stride(w, h, bands, prof)), (prof, len(prof) if prof else 0))
+    return _save_batch(lib().vb200_pngsave_batch, _png_options(compression, strategy, xres, filter, interlace, bitdepth), frames, in_ptr, shape,
+                       stride or (lambda w, h, bands: _png_stride(w, h, bands, prof, interlace, bitdepth)), (prof, len(prof) if prof else 0))
 
 
-def pngsave_host_twin(a, compression=6, strategy="default", xres=1.0, profile=None):
+def pngsave_host_twin(a, compression=6, strategy="default", xres=1.0, profile=None, filter="none", interlace=False, bitdepth=8):
     """the PNG stream of one uint8 frame [h, w, bands] through the encoder's per-position, per-symbol and per-block code
     compiled for the host (vb200_debug_png_encode); no GPU"""
     a = np.ascontiguousarray(a)
     if a.ndim == 2:
         a = a[:, :, None]
     h, w, bands = a.shape
-    opts = _png_options(compression, strategy, xres)
+    opts = _png_options(compression, strategy, xres, filter, interlace, bitdepth)
     prof = bytes(profile) if profile else None
     n = C.c_size_t()
     args = (a.ctypes.data_as(C.c_void_p), a.strides[0], w, h, bands, C.byref(opts), prof, len(prof) if prof else 0)

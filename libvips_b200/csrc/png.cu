@@ -34,6 +34,7 @@
 #include <vector>
 
 #include "../../include/vb200.h"
+#include "png_common.cuh"
 #include "vb200_internal.h"
 
 #define VB_HD __host__ __device__ __forceinline__
@@ -397,15 +398,6 @@ struct PngFrameDev {
 	int pal_off, pal_n; /* into the palette pool (256 RGBA entries each), -1: none */
 	unsigned short key[3];
 };
-
-/* PNG 2nd edition 9.2: Paeth's predictor */
-VB_HD int
-paeth(int a, int b, int c)
-{
-	const int p = a + b - c;
-	const int pa = abs(p - a), pb = abs(p - b), pc = abs(p - c);
-	return (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
-}
 
 /* the reconstructed byte from the filtered one, a = left, b = up, c = up-left */
 VB_HD unsigned char

@@ -1,4 +1,4 @@
-/* png_encode.cu -- vips_pngsave_buffer's 8-bit frames on the device: filter NONE scanlines deflated by CUDA kernels.
+/* png_encode.cu -- vips_pngsave_buffer's uchar frames on the device: scanlines built and deflated by CUDA kernels.
  *
  * What the reference does (foreign/spngsave.c, libspng over zlib, defaults): compression 6 (:700-705, :768), filter NONE
  * (:714-720, :769: every scanline is its filter byte 0 and the raw row), bit depth 8 for uchar frames (:608-613), IHDR from
@@ -11,6 +11,19 @@
  * from its source here; this encoder writes IHDR, iCCP, pHYs, IDATs of at most 8192 payload bytes and IEND, and uses
  * Z_DEFAULT_STRATEGY unless asked (libpng's choice without filtering, vipspng.c:1380-1384).
  *
+ * The scanlines (scan_byte) follow the options that change them without quantisation:
+ *   filter (:449-450, SPNG_FILTER_CHOICE; VipsForeignPngFilter, include/vips/foreign.h:744-748): 0 or NONE 0x08, SUB 0x10,
+ *     UP 0x20, AVG 0x40 or PAETH 0x80 filters every scanline with that type (PNG 2nd edition 9.2) on the raw bytes: a is
+ *     the byte bpp to the left, b the byte above in the same pass, c the byte left of b, each 0 where it does not exist,
+ *     bpp the bands at 8 bits.  More than one flag (ALL = 0xF8) is libspng's adaptive choice: declined.
+ *   interlace (:707-712, :439: IHDR interlace 1): Adam7 (8.2), passes (x0, y0, dx, dy) = (0,0,8,8) (4,0,8,8) (0,4,4,8) (2,0,4,4)
+ *     (0,2,2,4) (1,0,2,2) (0,1,1,2), each ceil((w - x0) / dx) x ceil((h - y0) / dy); an empty pass has no scanlines.
+ *   bitdepth 1 / 2 / 4 on one band (:400-441, :606-653): grey without a palette, each sample p >> (8 - bitdepth) packed
+ *     MSB first by vips_foreign_save_spng_pack (:295-324), whose tail takes the last 8 / bitdepth samples and shifts them
+ *     left by 8 - (leftover << (bitdepth - 1)): right at depths 1 and 2, 0 at depth 4, so an odd-width row at depth 4 ends
+ *     in v[w-2] << 4 | v[w-1].  Only NONE, not interlaced, is built at these depths.
+ * Every scanline byte is a function of at most four raw bytes, so one thread builds each.
+ *
  * Why an exact deflate can be parallel.  Levels 4-9 run zlib's deflate_slow, which inserts every position into the hash
  * chains; the 3-byte hash (15 bits, shift 5) is a pure function of the data, so the candidates of a position -- earlier
  * positions with its hash, newest first, the first at most MAX_DIST = 32506 back and the later ones less -- do not depend
@@ -21,7 +34,7 @@
  * decision, so the parse reads answers computed ahead of it.
  *
  * Device pipeline per chunk of frames (all frames of a batch share one geometry, so one scanline count N):
- *   png_filter_kernel       frames (any bpl / frame stride) -> filter-0 scanlines in pool memory
+ *   png_scan_kernel         frames (any bpl / frame stride) -> the scanlines in pool memory, one thread per byte
  *   png_adler_kernel        one CTA per frame: per-thread sums, combined in order
  *   deflate_last_kernel     per 32 KiB tile: the last position of every hash (shared-memory atomicMax)
  *   deflate_chain_kernel    one warp per tile: the previous position of the same hash for every position, 32 positions
@@ -48,6 +61,7 @@
 #include <vector>
 
 #include "../../include/vb200.h"
+#include "png_common.cuh"
 #include "vb200_internal.h"
 
 #define VB_HD __host__ __device__ __forceinline__
@@ -718,10 +732,23 @@ crc_update(unsigned crc, const unsigned char *p, size_t n, const unsigned *tab)
 
 /* ------------------------------------------------------------------ device kernels */
 
+/* a non-empty pass: its first column and row, their steps, its size, row bytes and first scanline byte */
+struct ScanPass {
+	unsigned x0, y0, dx, dy, w, h;
+	size_t rb, off;
+};
+
+/* the scanlines of a frame: what png_scan_kernel alone reads */
+struct ScanGeom {
+	int bands, depth, filter; /* depth: bits per sample; filter: PNG filter type 0-4 */
+	int npass;		  /* non-empty passes: 1 without interlace, up to 7 with */
+	ScanPass pass[7];
+	size_t n; /* scanline bytes: every pass's rows of rb + 1 */
+};
+
 struct EncGeom {
 	int w, h, bands, level, filtered;
-	size_t rb;		/* row bytes */
-	size_t n;		/* scanline bytes of a frame: h * (rb + 1) */
+	size_t n;		/* scanline bytes of a frame (ScanGeom::n) */
 	size_t scan_stride; /* per frame in the scanline pool (n + 8, aligned) */
 	int tiles;		/* 32 KiB tiles per frame */
 	int maxblk;		/* block records per frame */
@@ -735,19 +762,58 @@ struct FrameOut {
 	unsigned adler, nblk;
 };
 
-__global__ void
-png_filter_kernel(const unsigned char *__restrict__ src, size_t bpl, size_t frame_stride, EncGeom g, unsigned char *scan)
+/* byte k of row y of pass P as spngsave hands it to libspng: the pass's samples at 8 bits, or packed MSB first at 1 / 2 / 4
+ * bits with vips_foreign_save_spng_pack's tail rule (see the top of the file).  rd(row, byte): a byte of the frame. */
+#pragma nv_exec_check_disable
+template <class Rd>
+VB_HD unsigned
+raw_byte(const ScanGeom &g, const ScanPass &P, size_t y, size_t k, Rd &rd)
 {
-	const size_t f = blockIdx.y, stride = g.rb + 1;
-	unsigned char *dst = scan + f * g.scan_stride;
-	for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < g.scan_stride; i += (size_t) gridDim.x * blockDim.x) {
-		if (i >= g.n) {
-			dst[i] = 0;
-			continue;
-		}
-		const size_t y = i / stride, x = i - y * stride;
-		dst[i] = x == 0 ? 0 : src[f * frame_stride + y * bpl + x - 1];
-	}
+	const size_t row = P.y0 + y * P.dy;
+	if (g.depth == 8)
+		return rd(row, P.dx == 1 ? k : (P.x0 + k / g.bands * P.dx) * g.bands + k % g.bands);
+	const int per = 8 / g.depth;
+	const long long e = (long long) std::min<size_t>((k + 1) * per, P.w);
+	unsigned u = 0;
+	for (int j = per; j >= 1; j--)
+		u = u << g.depth | (e - j >= 0 ? rd(row, P.x0 + (size_t) (e - j) * P.dx) >> (8 - g.depth) : 0);
+	const size_t left = P.w - k * per;
+	return left >= (size_t) per ? u : (u << (8 - ((int) left << (g.depth - 1)))) & 255;
+}
+
+/* scanline byte i of a frame: the filter type at the start of each row, then the row's bytes filtered */
+#pragma nv_exec_check_disable
+template <class Rd>
+VB_HD unsigned
+scan_byte(const ScanGeom &g, size_t i, Rd &rd)
+{
+	int p = 0;
+	while (p + 1 < g.npass && i >= g.pass[p + 1].off)
+		p++;
+	const ScanPass &P = g.pass[p];
+	const size_t q = i - P.off, y = q / (P.rb + 1), x = q - y * (P.rb + 1);
+	if (x == 0)
+		return (unsigned) g.filter;
+	const size_t k = x - 1, bpp = g.depth == 8 ? g.bands : 1;
+	const unsigned raw = raw_byte(g, P, y, k, rd);
+	if (g.filter == 0)
+		return raw;
+	const unsigned a = g.filter != 2 && k >= bpp ? raw_byte(g, P, y, k - bpp, rd) : 0;
+	const unsigned b = g.filter != 1 && y ? raw_byte(g, P, y - 1, k, rd) : 0;
+	const unsigned c = g.filter == 4 && y && k >= bpp ? raw_byte(g, P, y - 1, k - bpp, rd) : 0;
+	const unsigned pred = g.filter == 1 ? a : g.filter == 2 ? b : g.filter == 3 ? (a + b) >> 1 : (unsigned) paeth((int) a, (int) b, (int) c);
+	return (raw - pred) & 255;
+}
+
+__global__ void
+png_scan_kernel(const unsigned char *__restrict__ src, size_t bpl, size_t frame_stride, ScanGeom sg, size_t scan_stride, unsigned char *scan)
+{
+	const size_t f = blockIdx.y;
+	const unsigned char *s = src + f * frame_stride;
+	unsigned char *dst = scan + f * scan_stride;
+	auto rd = [&](size_t row, size_t col) -> unsigned { return s[row * bpl + col]; };
+	for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < scan_stride; i += (size_t) gridDim.x * blockDim.x)
+		dst[i] = i < sg.n ? (unsigned char) scan_byte(sg, i, rd) : 0;
 }
 
 __global__ void __launch_bounds__(256)
@@ -1243,7 +1309,45 @@ check_save(const char *domain, int w, int h, int bands, const VB200PngSaveOption
 		error(domain, "bad xres %g", o.xres);
 		return -1;
 	}
+	if (o.filter & ~0xF8) {
+		error(domain, "filter 0x%x: unknown flag bits (NONE 0x08, SUB 0x10, UP 0x20, AVG 0x40, PAETH 0x80)", (unsigned) o.filter);
+		return -1;
+	}
+	if (o.filter & (o.filter - 1)) {
+		error(domain, "filter 0x%x: more than one flag is libspng's adaptive filter choice, which is not built (one flag or 0)",
+			(unsigned) o.filter);
+		return -1;
+	}
+	const int depth = o.bitdepth ? o.bitdepth : 8;
+	if (depth == 16) {
+		error(domain, "bitdepth 16 is not built (uchar frames only, bit depth 1, 2, 4 or 8)");
+		return -1;
+	}
+	if (depth != 1 && depth != 2 && depth != 4 && depth != 8) {
+		error(domain, "bitdepth %d: PNG save takes bit depth 1, 2, 4 or 8", depth);
+		return -1;
+	}
+	if (depth < 8 && bands == 2) {
+		error(domain, "bitdepth %d with 2 bands: PNG has no low-bit grey + alpha", depth);
+		return -1;
+	}
+	if (depth < 8 && bands > 2) {
+		error(domain, "bitdepth %d with %d bands: spngsave writes a palette, and quantisation is not built", depth, bands);
+		return -1;
+	}
+	if (depth < 8 && ((o.filter && o.filter != 0x08) || o.interlace)) {
+		error(domain, "bitdepth %d with a filter other than NONE or with interlace is not built (libspng's sub-byte filter unit and "
+			"pass packing cannot be checked)", depth);
+		return -1;
+	}
 	return 0;
+}
+
+/* the PNG filter type of a checked filter flag */
+int
+filter_type(int flags)
+{
+	return flags == 0x10 ? 1 : flags == 0x20 ? 2 : flags == 0x40 ? 3 : flags == 0x80 ? 4 : 0;
 }
 
 /* signature, IHDR, iCCP (profile non-empty), pHYs */
@@ -1255,7 +1359,7 @@ png_prefix(int w, int h, int bands, const VB200PngSaveOptions &o, const unsigned
 	put_be32(c, (unsigned) w);
 	put_be32(c, (unsigned) h);
 	const unsigned char ct[5] = {0, 0, 4, 2, 6};
-	c.insert(c.end(), {8, ct[bands], 0, 0, 0});
+	c.insert(c.end(), {(unsigned char) (o.bitdepth ? o.bitdepth : 8), ct[bands], 0, 0, (unsigned char) (o.interlace ? 1 : 0)});
 	put_chunk(v, "IHDR", c);
 	if (profile && profile_len) {
 		c.assign({'i', 'c', 'c', 0, 0});
@@ -1274,13 +1378,39 @@ png_prefix(int w, int h, int bands, const VB200PngSaveOptions &o, const unsigned
 	return v;
 }
 
+ScanGeom
+scan_geom(int w, int h, int bands, const VB200PngSaveOptions &o)
+{
+	ScanGeom g;
+	g.bands = bands;
+	g.depth = o.bitdepth ? o.bitdepth : 8;
+	g.filter = filter_type(o.filter);
+	static const unsigned adam7[7][4] = {{0, 0, 8, 8}, {4, 0, 8, 8}, {0, 4, 4, 8}, {2, 0, 4, 4}, {0, 2, 2, 4}, {1, 0, 2, 2}, {0, 1, 1, 2}};
+	static const unsigned whole[1][4] = {{0, 0, 1, 1}};
+	const unsigned(*steps)[4] = o.interlace ? adam7 : whole;
+	g.npass = 0;
+	g.n = 0;
+	for (int p = 0; p < (o.interlace ? 7 : 1); p++) {
+		ScanPass P;
+		P.x0 = steps[p][0], P.y0 = steps[p][1], P.dx = steps[p][2], P.dy = steps[p][3];
+		P.w = (unsigned) w > P.x0 ? (w - P.x0 + P.dx - 1) / P.dx : 0;
+		P.h = (unsigned) h > P.y0 ? (h - P.y0 + P.dy - 1) / P.dy : 0;
+		if (!P.w || !P.h)
+			continue;
+		P.rb = ((size_t) P.w * bands * g.depth + 7) / 8;
+		P.off = g.n;
+		g.n += P.h * (P.rb + 1);
+		g.pass[g.npass++] = P;
+	}
+	return g;
+}
+
 EncGeom
 enc_geom(int w, int h, int bands, const VB200PngSaveOptions &o, size_t prefix)
 {
 	EncGeom g;
 	g.w = w, g.h = h, g.bands = bands, g.level = o.compression, g.filtered = o.strategy == 1;
-	g.rb = (size_t) w * bands;
-	g.n = (size_t) h * (g.rb + 1);
+	g.n = scan_geom(w, h, bands, o).n;
 	g.scan_stride = (g.n + 8 + 15) & ~(size_t) 15;
 	g.tiles = (int) ((g.n + kWSize - 1) / kWSize);
 	g.maxblk = (int) (g.n / kMaxSyms + 2);
@@ -1297,10 +1427,10 @@ align256(size_t v)
 	return (v + 255) & ~(size_t) 255;
 }
 
-/* the kernels of cn frames at src (device memory): filter, deflate, then place and png_frame_kernel */
+/* the kernels of cn frames at src (device memory): scanlines, deflate, then place and png_frame_kernel */
 int
-png_chunk(const char *domain, const EncGeom &g, const std::vector<unsigned char> &prefix, const unsigned char *src, size_t bpl, size_t frame_stride,
-	int cn, const EncodePlace &place, cudaStream_t s)
+png_chunk(const char *domain, const EncGeom &g, const ScanGeom &sg, const std::vector<unsigned char> &prefix, const unsigned char *src, size_t bpl,
+	size_t frame_stride, int cn, const EncodePlace &place, cudaStream_t s)
 {
 	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_last_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 4));
 	VB200_CUDA(domain, cudaFuncSetAttribute(deflate_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSize * 2));
@@ -1330,7 +1460,7 @@ png_chunk(const char *domain, const EncGeom &g, const std::vector<unsigned char>
 			break;
 		}
 		const unsigned gx = (unsigned) std::min<size_t>((g.scan_stride + 255) / 256, 4096);
-		png_filter_kernel<<<dim3(gx, cn), 256, 0, s>>>(src, bpl, frame_stride, g, scan);
+		png_scan_kernel<<<dim3(gx, cn), 256, 0, s>>>(src, bpl, frame_stride, sg, g.scan_stride, scan);
 		png_adler_kernel<<<cn, 256, 0, s>>>(scan, g, fo);
 		deflate_last_kernel<<<dim3(g.tiles, cn), 1024, kWSize * 4, s>>>(scan, g, last);
 		deflate_chain_kernel<<<dim3(g.tiles, cn), 32, kWSize * 2, s>>>(scan, g, last, prev);
@@ -1372,11 +1502,13 @@ png_encoder(const char *domain, int w, int h, int bands, const VB200PngSaveOptio
 		return -1;
 	const std::vector<unsigned char> prefix = png_prefix(w, h, bands, o, profile, profile_len);
 	const EncGeom g = enc_geom(w, h, bands, o, prefix.size());
+	const ScanGeom sg = scan_geom(w, h, bands, o);
 	enc->scratch_bytes = g.scan_stride + align256(4 * g.n) + align256((size_t) 2 * kWSize * g.tiles) + align256(8 * g.n) + align256(4 * g.n) +
 		align256(g.maxblk * (sizeof(BlockRec) + sizeof(DeflatePlan))) + g.zcap + sizeof(FrameOut) + sizeof(unsigned long long);
 	enc->stream_bytes = g.prefix + g.zcap + 12 * (size_t) g.maxchunks + 12;
-	enc->chunk = [domain, g, prefix](const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place, cudaStream_t s) {
-		return png_chunk(domain, g, prefix, src, bpl, frame_stride, cn, place, s);
+	enc->chunk = [domain, g, sg, prefix](const unsigned char *src, size_t bpl, size_t frame_stride, int cn, const EncodePlace &place,
+				 cudaStream_t s) {
+		return png_chunk(domain, g, sg, prefix, src, bpl, frame_stride, cn, place, s);
 	};
 	return 0;
 }
@@ -1389,11 +1521,12 @@ host_png_encode(const char *domain, const unsigned char *img, size_t bpl, int w,
 	if (check_save(domain, w, h, bands, o))
 		return -1;
 	out = png_prefix(w, h, bands, o, profile, profile_len);
-	const size_t rb = (size_t) w * bands, n = (size_t) h * (rb + 1);
-	std::vector<unsigned char> scan(n + 8, 0), z;
-	for (int y = 0; y < h; y++)
-		memcpy(&scan[(size_t) y * (rb + 1) + 1], img + (size_t) y * bpl, rb);
-	host_deflate(scan.data(), n, o.compression, o.strategy, z);
+	const ScanGeom sg = scan_geom(w, h, bands, o);
+	std::vector<unsigned char> scan(sg.n + 8, 0), z;
+	auto rd = [&](size_t row, size_t col) -> unsigned { return img[row * bpl + col]; };
+	for (size_t i = 0; i < sg.n; i++)
+		scan[i] = (unsigned char) scan_byte(sg, i, rd);
+	host_deflate(scan.data(), sg.n, o.compression, o.strategy, z);
 	for (size_t at = 0; at < z.size(); at += kIdat)
 		put_chunk(out, "IDAT", std::vector<unsigned char>(z.begin() + at, z.begin() + std::min(z.size(), at + kIdat)));
 	put_chunk(out, "IEND", {});

@@ -1,15 +1,17 @@
 """tools/bench_pngsave.py -- PNG save on the device (csrc/png_encode.cu) against zlib on the host's own threads.
 
-    python tools/bench_pngsave.py [--reps R] [--out DIR] [--small N] [--big N]
+    python tools/bench_pngsave.py [--reps R] [--out DIR] [--small N] [--big N] [--filter F] [--interlace]
 
-Workloads (frames from a seed, compression 6, filter NONE, Z_DEFAULT_STRATEGY):
+Workloads (frames from a seed, compression 6, Z_DEFAULT_STRATEGY; filter NONE and not interlaced unless --filter sub / up /
+avg / paeth or --interlace say otherwise, which then apply to every workload):
     small   N (2048) 256 x 256 RGBA and RGB frames in device memory, synthetic (smooth gradients and flat runs) and
             photo-like (noise over smooth fields)
     big     N (16) 4096 x 4096 RGB frames, the same two contents
     e2e     PNG streams -> ThumbnailPlan.run_png (to 256 pixels) -> pngsave_batch: streams in, streams out
-The baseline is zlib level 6 over the same scanlines on the machine's threads (the work libspng does); Pillow's PNG encoder
-at compress_level 6 goes beside it.  The card's name and power limit are read in the same run, and the kernel split comes
-from a separate torch.profiler pass.  One JSON line per workload; with --out, a summary in DIR/bench_pngsave.json."""
+The baseline is zlib level 6 over the same scanlines on the machine's threads, fed one scanline at a time (the work libspng
+does; the scanlines are built beforehand with numpy, filtered and interlaced as asked, and not timed); Pillow's PNG encoder at
+compress_level 6 goes beside it.  Bytes per frame are reported for the device's streams and for host zlib's.  The card's
+name and power limit are read in the same run, and the kernel split comes from a separate torch.profiler pass.  One JSON line per workload; with --out, a summary in DIR/bench_pngsave.json."""
 import argparse
 import io
 import json
@@ -56,12 +58,44 @@ def batch(kind, n, h, w, bands, distinct=8):
     return np.stack([frames[i % len(frames)] for i in range(n)])
 
 
-def host_zlib(frames, threads):
-    def one(a):
+FILTERS = {"none": 0, "sub": 1, "up": 2, "avg": 3, "paeth": 4}
+ADAM7 = ((0, 0, 8, 8), (4, 0, 8, 8), (0, 4, 4, 8), (2, 0, 4, 4), (0, 2, 2, 4), (1, 0, 2, 2), (0, 1, 1, 2))
+
+
+def scanlines(a, filter, interlace):
+    """the PNG scanlines of one 8-bit frame [h, w, bands] as a list of rows: Adam7 passes (PNG 2nd edition 8.2) or the frame,
+    every row its filter type and its bytes filtered on the raw bytes (9.2)"""
+    ft, bands, rows = FILTERS[filter], a.shape[2], []
+    for x0, y0, dx, dy in (ADAM7 if interlace else ((0, 0, 1, 1),)):
+        sub = a[y0::dy, x0::dx]
+        if not sub.size:
+            continue
+        r = sub.reshape(sub.shape[0], -1).astype(np.int16)
+        b, left, c = np.zeros_like(r), np.zeros_like(r), np.zeros_like(r)
+        b[1:], left[:, bands:], c[1:, bands:] = r[:-1], r[:, :-bands], r[:-1, :-bands]
+        if ft == 0:
+            pred = 0
+        elif ft == 1:
+            pred = left
+        elif ft == 2:
+            pred = b
+        elif ft == 3:
+            pred = (left + b) >> 1
+        else:
+            p = left + b - c
+            pa, pb, pc = np.abs(p - left), np.abs(p - b), np.abs(p - c)
+            pred = np.where((pa <= pb) & (pa <= pc), left, np.where(pb <= pc, b, c))
+        f = ((r - pred) & 255).astype(np.uint8)
+        rows += [bytes([ft]) + row.tobytes() for row in f]
+    return rows
+
+
+def host_zlib(scans, threads):
+    def one(rows):
         c = zlib.compressobj(6, zlib.DEFLATED, 15, 8, zlib.Z_DEFAULT_STRATEGY)
-        return len(b"".join(c.compress(b"\0" + r.tobytes()) for r in a) + c.flush())
+        return len(b"".join(c.compress(r) for r in rows) + c.flush())
     with ThreadPoolExecutor(threads) as ex:
-        return list(ex.map(one, frames))
+        return list(ex.map(one, scans))
 
 
 def host_pillow(frames, threads):
@@ -107,7 +141,11 @@ def main():
     ap.add_argument("--out")
     ap.add_argument("--small", type=int, default=2048)
     ap.add_argument("--big", type=int, default=16, help="large frames (0: skip that workload)")
+    ap.add_argument("--filter", default="none", choices=sorted(FILTERS), help="every scanline's filter type")
+    ap.add_argument("--interlace", action="store_true", help="Adam7 scanlines")
     args = ap.parse_args()
+    opts = dict(filter=args.filter, interlace=args.interlace)
+    tag = ("" if args.filter == "none" else "_" + args.filter) + ("_adam7" if args.interlace else "")
     import torch
     vb.init(0)
     name, power = card()
@@ -118,7 +156,7 @@ def main():
     def device_save(frames):
         t = torch.from_numpy(frames).cuda()
         n, h, w, b = frames.shape
-        return lambda: vb.pngsave_batch(None, 6, in_ptr=t.data_ptr(), shape=(n, h, w, b))
+        return lambda: vb.pngsave_batch(None, 6, in_ptr=t.data_ptr(), shape=(n, h, w, b), **opts)
 
     for label, n, (h, w) in (("small", args.small, (256, 256)), ("big", args.big, (4096, 4096))):
         if n < 1:
@@ -129,17 +167,22 @@ def main():
                 run = device_save(frames)
                 streams = run()
                 for i in range(min(n, 8 if label == "small" else 1)):  # the host twin is serial: one large frame
-                    assert streams[i] == vb.pngsave_host_twin(frames[i], 6), "device stream %d differs from the host twin" % i
+                    assert streams[i] == vb.pngsave_host_twin(frames[i], 6, **opts), "device stream %d differs from the host twin" % i
                 dev = timed(run, args.reps, sync)
                 sub = frames[:max(1, min(n, 256 if label == "small" else 4))]
-                hz = timed(lambda: host_zlib(sub, threads), 1, lambda: None) * n / len(sub)
+                scans = [scanlines(a, args.filter, args.interlace) for a in sub]
+                hz_bytes = []
+                hz = timed(lambda: hz_bytes.append(host_zlib(scans, threads)), 1, lambda: None) * n / len(sub)
                 hp = timed(lambda: host_pillow(sub, threads), 1, lambda: None) * n / len(sub)
-                r = {"workload": "%s_%s_%d" % (label, kind, bands), "frames": n, "shape": [h, w, bands], "gpu": name, "power_limit_max_sm": power,
+                r = {"workload": "%s_%s_%d%s" % (label, kind, bands, tag), "filter": args.filter, "interlace": args.interlace, "frames": n,
+                     "shape": [h, w, bands], "gpu": name, "power_limit_max_sm": power,
                      "device_s": round(dev, 4), "device_frames_per_s": round(n / dev, 1),
                      "device_MB_per_s_in": round(frames.nbytes / dev / 1e6, 1),
                      "host_zlib_s": round(hz, 4), "host_zlib_frames_per_s": round(n / hz, 1),
                      "pillow_s": round(hp, 4), "pillow_frames_per_s": round(n / hp, 1), "host_threads": threads,
                      "ratio": round(sum(len(s) for s in streams) / frames.nbytes, 4),
+                     "device_bytes_per_frame": round(sum(len(s) for s in streams) / n, 1),
+                     "host_zlib_bytes_per_frame": round(float(np.mean(hz_bytes[-1])), 1),
                      "kernels_ms": kernel_split(run)}
                 print(json.dumps(r), flush=True)
                 results.append(r)
@@ -160,12 +203,13 @@ def main():
 
     def e2e():
         plan.run_png(streams, out_ptr=out.data_ptr())
-        return vb.pngsave_batch(None, 6, in_ptr=out.data_ptr(), shape=(len(streams), oh, ow, 4))
+        return vb.pngsave_batch(None, 6, in_ptr=out.data_ptr(), shape=(len(streams), oh, ow, 4), **opts)
     got = e2e()
     th = out[:1].cpu().numpy()[0]
-    assert got[0] == vb.pngsave_host_twin(th, 6)
+    assert got[0] == vb.pngsave_host_twin(th, 6, **opts)
     t = timed(e2e, args.reps, sync)
-    r = {"workload": "e2e_png_thumbnail_png", "frames": len(streams), "in": [1024, 1024, 4], "out": [oh, ow, 4], "gpu": name,
+    r = {"workload": "e2e_png_thumbnail_png" + tag, "filter": args.filter, "interlace": args.interlace, "frames": len(streams),
+         "in": [1024, 1024, 4], "out": [oh, ow, 4], "gpu": name,
          "power_limit_max_sm": power, "device_s": round(t, 4), "frames_per_s": round(len(streams) / t, 1)}
     print(json.dumps(r), flush=True)
     results.append(r)
