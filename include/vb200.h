@@ -791,7 +791,7 @@ int vb200_debug_jpeg_optimal_table(const unsigned *freq, unsigned char *bits, un
 void vb200_debug_jpeg_times(float *huffman_ms, float *idct_ms);
 
 /* ------------------------------------------------------------------ Deep Zoom tile pyramids
- * vips_dzsave (foreign/dzsave.c) in its "dz" and "zoomify" layouts with JPEG tiles, on the device (csrc/dzsave.cu):
+ * vips_dzsave (foreign/dzsave.c) in its "dz" and "zoomify" layouts with JPEG or PNG tiles, on the device (csrc/dzsave.cu):
  * every level of the pyramid (strip_shrink :1761-1835 over region.c:1139-1156, each level the 2 x 2 rounded mean
  * (a + b + c + d + 2) >> 2 of the level above with its last column / row repeated when its size is odd,
  * level_generate_extras :1710-1754), every tile cut from it (image_strip_allocate :1106-1152) and every tile's
@@ -829,12 +829,26 @@ int vb200_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyr
  * and the encoder's host twin
  */
 int vb200_debug_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out);
+/* The save with PNG tiles: the reference with suffix ".png", where every tile is vips_image_write_to_buffer(tile, ".png")
+ * (write_image :369-402) -- spngsave with its defaults and keep NONE, so no iCCP -- and each stream is what
+ * vb200_pngsave_batch writes for it.  Images are uchar with 1 to 4 bands, Type B_W for 1-2 bands and sRGB for 3-4 (any
+ * other Type returns -1: spngsave's vips_colourspace or vips_image_hasalpha would change the pixels).  With 2 or 4 bands the
+ * last is alpha and every level is vips_region_shrink_alpha's (region.c:1444-1482): with S the sum of the four alphas, each
+ * colour band the alpha-weighted sum over S (truncated), alpha S >> 2, all 0 where S is 0 -- so an opaque RGBA image does
+ * not get the RGB pyramid.  options: as vb200_dzsave, except suffix NULL = ".png", and any other suffix must be ".png" in
+ * any case without [options]; options->jpeg is ignored.  png: the tiles' options as vb200_pngsave_batch takes them, with
+ * the same declines; NULL = spngsave's defaults (compression 6, default strategy, xres 1.0, filter NONE, no interlace,
+ * bitdepth 8).  Every decline happens before any device call.  The result is read with the vb200_dz_* calls below.
+ */
+int vb200_dzsave_png(const VB200Image *in, const VB200DzOptions *options, const VB200PngSaveOptions *png, VB200DzPyramid **out);
+/* test hook, host only: vb200_dzsave_png through the kernels' per-pixel code and the PNG encoder's host twin */
+int vb200_debug_dzsave_png(const VB200Image *in, const VB200DzOptions *options, const VB200PngSaveOptions *png, VB200DzPyramid **out);
 void vb200_dz_free(VB200DzPyramid *pyramid);
 /* levels are numbered as the reference numbers them (pyramid_build :441-577): n = 0 is the smallest */
 int vb200_dz_levels(const VB200DzPyramid *pyramid);
 int vb200_dz_level_geometry(const VB200DzPyramid *pyramid, int n, int *width, int *height, int *tiles_across, int *tiles_down);
 /* tiles in the order zoomify numbers them (tile_name :1182-1191): level 0 first, then down, then across.  left, top,
- * width, height: the tile's rect in its level; stream: its JPEG, owned by the pyramid
+ * width, height: the tile's rect in its level; stream: its JPEG or PNG, owned by the pyramid
  */
 long vb200_dz_tiles(const VB200DzPyramid *pyramid);
 int vb200_dz_tile(const VB200DzPyramid *pyramid, long i, int *level, int *x, int *y, int *left, int *top, int *width, int *height,
@@ -848,13 +862,16 @@ int vb200_dz_tile_name(const VB200DzPyramid *pyramid, long i, const char *basena
  */
 int vb200_dz_sidecar(const VB200DzPyramid *pyramid, const char *basename, char *name, size_t ncap, char *text, size_t tcap, size_t *len);
 /* The pixel pyramid alone: level n_from_top of the image (0 = the image itself, 1 = half size ...) through the same
- * kernels, into out (allocate-or-fill like every op).  -1 when the image has no such level (it stops at 1 x 1).
+ * kernels, into out (allocate-or-fill like every op).  -1 when the image has no such level (it stops at 1 x 1).  uchar,
+ * 1 to 4 bands: 2 bands (Type B_W) and 4 bands (Type sRGB) are shrunk with their alpha, as vb200_dzsave_png does.
  */
 int vb200_dz_pyramid_level(const VB200Image *in, int n_from_top, VB200Image *out);
-/* test hook, host only: vb200_dz_pyramid_level through the per-pixel code on the CPU; out: packed, caller-sized */
+/* test hook, host only: vb200_dz_pyramid_level through the per-pixel code on the CPU; out: packed, caller-sized.  It has no
+ * Type: 2 and 4 bands are alpha images */
 int vb200_debug_dz_pyramid_level(const void *pixels, size_t bpl, int width, int height, int bands, int n_from_top, void *out);
 /* test hooks: the device memory one shape batch of tiles may take (pixels, encoder scratch and stream slots; 0 = the
- * default, 1 GiB), and the bytes currently allocated from the device's stream-ordered pool
+ * default: 1 GiB for JPEG tiles, the PNG codecs' chunk budget for PNG tiles), and the bytes currently allocated from the
+ * device's stream-ordered pool
  */
 void vb200_debug_dz_set_budget(size_t bytes);
 size_t vb200_debug_dz_pool_used(void);

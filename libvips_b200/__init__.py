@@ -269,6 +269,8 @@ def lib():
         DO, PP = C.POINTER(DzOptions), C.POINTER(C.c_void_p)
         L.vb200_dzsave.argtypes = [IP, DO, PP]
         L.vb200_debug_dzsave.argtypes = [IP, DO, PP]
+        L.vb200_dzsave_png.argtypes = [IP, DO, C.POINTER(PngSaveOptions), PP]
+        L.vb200_debug_dzsave_png.argtypes = [IP, DO, C.POINTER(PngSaveOptions), PP]
         L.vb200_dz_free.argtypes = [C.c_void_p]
         L.vb200_dz_levels.argtypes = [C.c_void_p]
         L.vb200_dz_level_geometry.argtypes = [C.c_void_p, C.c_int, PI, PI, PI, PI]
@@ -548,6 +550,10 @@ class Image:
     def dzsave(self, basename=None, **options):
         """vips_dzsave: the Deep Zoom / Zoomify tile pyramid of this image -> DzPyramid (see dzsave())"""
         return dzsave(self, basename, **options)
+
+    def dzsave_png(self, basename=None, **options):
+        """vips_dzsave with suffix ".png": the tile pyramid of this image with PNG tiles -> DzPyramid (see dzsave_png())"""
+        return dzsave_png(self, basename, **options)
 
     def pngsave_buffer(self, compression=6, strategy="default", xres=1.0, profile=None, filter="none", interlace=False, bitdepth=8):
         """vips_pngsave_buffer: this uchar image (1-4 bands) as a PNG stream (bytes), deflated on the device; filter, interlace
@@ -866,7 +872,7 @@ REGION_SHRINKS = {"mean": 0, "median": 1, "mode": 2, "max": 3, "min": 4, "neares
 
 class DzTile:
     """one tile of a DzPyramid: name (path relative to the directory written in), level (0 = smallest), x, y,
-    rect = (left, top, width, height) in its level, bytes = its JPEG stream"""
+    rect = (left, top, width, height) in its level, bytes = its JPEG or PNG stream"""
     __slots__ = ("name", "level", "x", "y", "rect", "bytes")
 
     def __init__(self, name, level, x, y, rect, data):
@@ -902,7 +908,7 @@ class DzPyramid:
             L.vb200_dz_free(handle)
 
     def write(self, directory):
-        """<directory>/<basename>.dzi + <basename>_files/<level>/<x>_<y>.jpeg, or the zoomify tree"""
+        """<directory>/<basename>.dzi + <basename>_files/<level>/<x>_<y><suffix>, or the zoomify tree"""
         for name, data in [(t.name, t.bytes) for t in self.tiles] + [(self.sidecar[0], self.sidecar[1].encode())]:
             path = os.path.join(directory, name)
             os.makedirs(os.path.dirname(path), exist_ok=True)
@@ -927,7 +933,8 @@ def _dz_image(image, in_ptr, shape, bpl):
 
 
 def _dzsave(fn, image, basename, layout, tile_size, overlap, depth, Q, suffix, region_shrink, skip_blanks, container, subsample_mode,
-            optimize_coding, restart_interval, interlace, in_ptr, shape, bpl):
+            optimize_coding, restart_interval, interlace, in_ptr, shape, bpl, png=None):
+    """fn(image, DzOptions, [png,] &handle) -> DzPyramid; png: the PngSaveOptions of vb200_dzsave_png"""
     pick = lambda table, v: table[v] if v in table else int(v)
     jpeg = JpegSaveOptions(int(Q), {"auto": 0, "on": 1, "off": 2}[subsample_mode], int(bool(optimize_coding)), int(restart_interval),
                            int(bool(interlace)))
@@ -936,7 +943,7 @@ def _dzsave(fn, image, basename, layout, tile_size, overlap, depth, Q, suffix, r
                      None if suffix is None else suffix.encode(), jpeg)
     cin, keep = _dz_image(image, in_ptr, shape, bpl)
     handle = C.c_void_p()
-    _check(fn(C.byref(cin), C.byref(opts), C.byref(handle)))
+    _check(fn(C.byref(cin), C.byref(opts), *(() if png is None else (C.byref(png),)), C.byref(handle)))
     return DzPyramid(handle, basename)
 
 
@@ -958,9 +965,29 @@ def dzsave_host_twin(image, basename=None, layout="dz", tile_size=None, overlap=
                    container, subsample_mode, optimize_coding, restart_interval, interlace, None, None, None)
 
 
+def dzsave_png(image, basename=None, layout="dz", tile_size=None, overlap=None, depth=None, suffix=None, compression=6, strategy="default",
+               filter="none", interlace=False, bitdepth=8, xres=1.0, region_shrink="mean", skip_blanks=-1, container="fs", in_ptr=None, shape=None,
+               bpl=None):
+    """vips_dzsave with suffix ".png" on the device: the Deep Zoom ("dz") or Zoomify pyramid of a uint8 image of 1 to 4 bands
+    with PNG tiles, every level and every tile's deflate made by CUDA kernels -> DzPyramid.  2 and 4 bands are grey / RGB with
+    alpha, and their levels are alpha-weighted (vips_region_shrink_alpha).  suffix None is ".png"; compression, strategy,
+    filter, interlace, bitdepth and xres are pngsave_batch's.  image / in_ptr / shape / bpl and the layout options as in
+    dzsave(); what the device path does not take raises Error."""
+    return _dzsave(lib().vb200_dzsave_png, image, basename, layout, tile_size, overlap, depth, 75, suffix, region_shrink, skip_blanks, container,
+                   "auto", False, 0, False, in_ptr, shape, bpl, _png_options(compression, strategy, xres, filter, interlace, bitdepth))
+
+
+def dzsave_png_host_twin(image, basename=None, layout="dz", tile_size=None, overlap=None, depth=None, suffix=None, compression=6,
+                         strategy="default", filter="none", interlace=False, bitdepth=8, xres=1.0, region_shrink="mean", skip_blanks=-1,
+                         container="fs"):
+    """dzsave_png through the kernels' per-pixel code and the PNG encoder's host twin on the CPU (vb200_debug_dzsave_png): no GPU"""
+    return _dzsave(lib().vb200_debug_dzsave_png, image, basename, layout, tile_size, overlap, depth, 75, suffix, region_shrink, skip_blanks,
+                   container, "auto", False, 0, False, None, None, None, _png_options(compression, strategy, xres, filter, interlace, bitdepth))
+
+
 def dz_pyramid_level(image, n_from_top, in_ptr=None, shape=None, bpl=None):
     """level n_from_top of the pixel pyramid dzsave cuts its tiles from (0 = the image, 1 = half size ...), on the device ->
-    uint8 array [height, width, bands] on the host"""
+    uint8 array [height, width, bands] on the host.  2 and 4 bands are shrunk with their alpha, as dzsave_png does"""
     cin, keep = _dz_image(image, in_ptr, shape, bpl)
     cout = CImage()
     if in_ptr is not None:

@@ -1,11 +1,14 @@
-/* dzsave.cu -- vips_dzsave (foreign/dzsave.c) in its "dz" and "zoomify" layouts with JPEG tiles, on the device.
+/* dzsave.cu -- vips_dzsave (foreign/dzsave.c) in its "dz" and "zoomify" layouts with JPEG or PNG tiles, on the device.
  *
  * What the reference does: pyramid_build (:441-577) makes a chain of levels, each half the size of the one above, rounded
  * up; vips_sink_disc feeds the top level strips of rows (pyramid_strip :1942-2014); a level that has a line of tiles
  * writes them (strip_save :1653-1703, one vips_jpegsave per tile: image_strip_allocate :1106-1152, write_image :369-404)
  * and shrinks the strip into the level below (strip_shrink :1761-1835) after level_generate_extras (:1710-1754) has
  * repeated the last column / row of a level of odd size; the shrink is vips_region_shrink_uncoded_mean
- * (iofuncs/region.c:1139-1156), (p00 + p01 + p10 + p11 + 2) >> 2 per band.
+ * (iofuncs/region.c:1139-1156), (p00 + p01 + p10 + p11 + 2) >> 2 per band.  With PNG tiles (vb200_dzsave_png) the
+ * tiles are vips_image_write_to_buffer(tile, ".png") (write_image :369-402, spngsave's defaults) and an image with alpha
+ * (vips_image_hasalpha: more bands than its Type has, iofuncs/image.c:3113-3119) is shrunk by vips_region_shrink_alpha
+ * instead (region.c:1444-1482, 1551-1573, whatever region_shrink says): dz_shrink_alpha.
  *
  * Stated over whole images, which is what runs here: level k - 1 is the 2 x 2 rounded mean of level k with its last column /
  * row read twice when its width / height is odd, and tile (x, y) of a level is the rect [x * step - margin, y * step -
@@ -17,6 +20,7 @@
  *                       shared memory to levels L-1 .. L-4, so four levels cost one read of the largest; the rounding is
  *                       per level, so the levels cannot be folded into one wide box, and each level applies its own
  *                       odd-edge rule from its own size.  All levels stay in device memory: 4/3 of the input.
+ *                       With alpha (2 or 4 bands) a thread makes one output pixel from all the bands of its four.
  *   dz_gather_kernel    the tiles of one shape (w, h), from every level, copied into one batch [n][h][w][bands], driven by
  *                       a table of source pointers built on the host
  *   the encoder         the encoders' batch driver per shape batch (encode.cu), device in: the streams packed end to end
@@ -70,6 +74,34 @@ dz_mean(int a, int b, int c, int d)
 	return (a + b + c + d + 2) >> 2;
 }
 
+/* SHRINK_ALPHA_TYPE (region.c:1446-1482) for uchar, the last band alpha: in double there, a = (a1 + a2 + a3 + a4) / 4.0,
+ * each colour band (a1 p1 + a2 p2 + a3 p3 + a4 p4) / (4.0 a), alpha a, every band 0 when a == 0, each truncated to uchar.
+ * With S = a1 + a2 + a3 + a4 that is integer arithmetic: 4.0 a == S exactly, so alpha is S >> 2; the numerator is below
+ * 2^18, exact in double, and a quotient that is not an integer is at least 1 / S >= 1 / 1020 from one, far more than the
+ * division's rounding error, so truncating it is the integer quotient.
+ */
+HD void
+dz_shrink_alpha(const unsigned char *p00, const unsigned char *p01, const unsigned char *p10, const unsigned char *p11, int bands,
+	unsigned char *q)
+{
+	const unsigned a1 = p00[bands - 1], a2 = p01[bands - 1], a3 = p10[bands - 1], a4 = p11[bands - 1], S = a1 + a2 + a3 + a4;
+	if (S == 0) {
+		for (int b = 0; b < bands; b++)
+			q[b] = 0;
+		return;
+	}
+	for (int b = 0; b < bands - 1; b++)
+		q[b] = (unsigned char) ((a1 * p00[b] + a2 * p01[b] + a3 * p10[b] + a4 * p11[b]) / S);
+	q[bands - 1] = (unsigned char) (S >> 2);
+}
+
+/* vips_image_hasalpha of the images the device path takes: 2 and 4 bands are B_W / sRGB with alpha */
+HD bool
+dz_alpha(int bands)
+{
+	return bands == 2 || bands == 4;
+}
+
 /* one level from the one above, whole image: pixel (x, y) from columns 2x and 2x + 1 (2x again when that is past the
  * level's own last column: level_generate_extras), rows likewise
  */
@@ -82,8 +114,11 @@ host_shrink_level(const unsigned char *src, size_t bpl, int w, int h, int bands,
 		unsigned char *q = dst + (size_t) y * ow * bands;
 		for (int x = 0; x < ow; x++) {
 			const int c0 = 2 * x * bands, c1 = std::min(2 * x + 1, w - 1) * bands;
-			for (int b = 0; b < bands; b++)
-				q[x * bands + b] = (unsigned char) dz_mean(r0[c0 + b], r0[c1 + b], r1[c0 + b], r1[c1 + b]);
+			if (dz_alpha(bands))
+				dz_shrink_alpha(r0 + c0, r0 + c1, r1 + c0, r1 + c1, bands, q + x * bands);
+			else
+				for (int b = 0; b < bands; b++)
+					q[x * bands + b] = (unsigned char) dz_mean(r0[c0 + b], r0[c1 + b], r1[c0 + b], r1[c1 + b]);
 		}
 	}
 }
@@ -137,14 +172,25 @@ dz_pyramid_kernel(const DzPyramidArgs A)
 		for (int l = 0; l < A.n; l++) {
 			/* this level's size and this block's origin in it; the edge rule comes from the size of the level read */
 			const int ow = (fw + 1) >> 1, oh = (fh + 1) >> 1, ox0 = fx0 >> 1, oy0 = fy0 >> 1, pitch = n * BANDS;
-			for (int i = tid; i < n * pitch; i += kDzThreads) {
-				const int y = i / pitch, xb = i - y * pitch, x = xb / BANDS, b = xb - x * BANDS;
-				if (ox0 + x >= ow || oy0 + y >= oh)
-					continue;
-				const int c0 = 2 * x * BANDS + b, c1 = (2 * (ox0 + x) + 1 < fw ? 2 * x + 1 : 2 * x) * BANDS + b;
-				const int r0 = 2 * y * fpitch, r1 = (2 * (oy0 + y) + 1 < fh ? 2 * y + 1 : 2 * y) * fpitch;
-				to[i] = (unsigned char) dz_mean(from[r0 + c0], from[r0 + c1], from[r1 + c0], from[r1 + c1]);
-			}
+			if (dz_alpha(BANDS))
+				/* one thread per output pixel: the alpha weights every band of it */
+				for (int i = tid; i < n * n; i += kDzThreads) {
+					const int y = i / n, x = i - y * n;
+					if (ox0 + x >= ow || oy0 + y >= oh)
+						continue;
+					const int c0 = 2 * x * BANDS, c1 = (2 * (ox0 + x) + 1 < fw ? 2 * x + 1 : 2 * x) * BANDS;
+					const unsigned char *r0 = from + 2 * y * fpitch, *r1 = from + (2 * (oy0 + y) + 1 < fh ? 2 * y + 1 : 2 * y) * fpitch;
+					dz_shrink_alpha(r0 + c0, r0 + c1, r1 + c0, r1 + c1, BANDS, to + y * pitch + x * BANDS);
+				}
+			else
+				for (int i = tid; i < n * pitch; i += kDzThreads) {
+					const int y = i / pitch, xb = i - y * pitch, x = xb / BANDS, b = xb - x * BANDS;
+					if (ox0 + x >= ow || oy0 + y >= oh)
+						continue;
+					const int c0 = 2 * x * BANDS + b, c1 = (2 * (ox0 + x) + 1 < fw ? 2 * x + 1 : 2 * x) * BANDS + b;
+					const int r0 = 2 * y * fpitch, r1 = (2 * (oy0 + y) + 1 < fh ? 2 * y + 1 : 2 * y) * fpitch;
+					to[i] = (unsigned char) dz_mean(from[r0 + c0], from[r0 + c1], from[r1 + c0], from[r1 + c1]);
+				}
 			__syncthreads();
 			const int orows = min(n, oh - oy0), ovalid = min(n, ow - ox0) * BANDS, words = pitch / 4;
 			unsigned char *d = A.dst[l] + (size_t) oy0 * A.dst_bpl[l] + (size_t) ox0 * BANDS;
@@ -262,8 +308,12 @@ dev_pyramid(const char *domain, const unsigned char *top, size_t bpl, int w, int
 		const dim3 grid((A.w + kDzBlock - 1) / kDzBlock, std::min(A.blocks_y, kMaxGridY));
 		if (bands == 1)
 			dz_pyramid_kernel<1><<<grid, kDzThreads, 0, sc.s>>>(A);
-		else
+		else if (bands == 2)
+			dz_pyramid_kernel<2><<<grid, kDzThreads, 0, sc.s>>>(A);
+		else if (bands == 3)
 			dz_pyramid_kernel<3><<<grid, kDzThreads, 0, sc.s>>>(A);
+		else
+			dz_pyramid_kernel<4><<<grid, kDzThreads, 0, sc.s>>>(A);
 		VB200_CUDA(domain, cudaGetLastError());
 		count_launch();
 	}
@@ -272,9 +322,42 @@ dev_pyramid(const char *domain, const unsigned char *top, size_t bpl, int w, int
 
 const char *const kLayoutNames[] = {"dz", "zoomify", "google", "iiif", "iiif3"};
 
-/* options and geometry: vips_foreign_save_dz_build :2043-2113, pyramid_build :441-577, image_strip_allocate :1132-1145 */
+/* what every tile is written as: vb200_dzsave's JPEG, or vb200_dzsave_png's PNG */
+struct DzCodec {
+	bool png = false;
+	VB200JpegSaveOptions jpeg;
+	VB200PngSaveOptions pngo;
+};
+
+/* the device encoder of one tile shape (no device call) */
 int
-dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid *P, VB200JpegSaveOptions *jpeg)
+tile_encoder(const char *domain, const DzCodec &c, int w, int h, int bands, Encoder *enc)
+{
+	return c.png ? png_encoder(domain, w, h, bands, c.pngo, nullptr, 0, enc) : jpeg_encoder(domain, w, h, bands, c.jpeg, enc);
+}
+
+/* one tile's stream through the encoder's host twin, appended to out */
+int
+host_tile_encode(const char *domain, const DzCodec &c, const unsigned char *p, size_t bpl, int w, int h, int bands, std::vector<unsigned char> &out)
+{
+	if (c.png) {
+		std::vector<unsigned char> one;
+		if (host_png_encode(domain, p, bpl, w, h, bands, c.pngo, nullptr, 0, one))
+			return -1;
+		out.insert(out.end(), one.begin(), one.end());
+		return 0;
+	}
+	const VB200JpegSaveOptions &j = c.jpeg;
+	unsigned long long events[3]; /* the progressive coder's counters, a test hook of its own */
+	return j.interlace ? host_jpeg_encode_progressive(domain, p, bpl, w, h, bands, j.Q, j.subsample_mode, j.restart_interval, out, events)
+					   : host_jpeg_encode(domain, p, bpl, w, h, bands, j.Q, j.subsample_mode, j.optimize_coding != 0, j.restart_interval, out);
+}
+
+/* options and geometry: vips_foreign_save_dz_build :2043-2113, pyramid_build :441-577, image_strip_allocate :1132-1145.
+ * c->png on entry picks the tiles; png: their options (NULL: spngsave's defaults).
+ */
+int
+dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options, const VB200PngSaveOptions *png, VB200DzPyramid *P, DzCodec *c)
 {
 	if (!in || !in->data) {
 		error(domain, "no input image");
@@ -289,8 +372,21 @@ dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options,
 		error(domain, "band format %d not supported on the device path (uchar only)", in->BandFmt);
 		return -1;
 	}
-	if (in->Bands != 1 && in->Bands != 3) {
+	if (!c->png && in->Bands != 1 && in->Bands != 3) {
 		error(domain, "%d-band images not supported on the device path (1 or 3 bands: the JPEG saver would flatten or drop the others)", in->Bands);
+		return -1;
+	}
+	if (c->png && (in->Bands < 1 || in->Bands > 4)) {
+		error(domain, "%d-band images not supported on the device path (1 to 4 bands with PNG tiles)", in->Bands);
+		return -1;
+	}
+	/* spngsave runs vips_colourspace to B_W below 3 bands and to sRGB from 3 (spngsave.c:621-641), and hasalpha reads the
+	 * Type: with any other Type the pixels saved would not be these
+	 */
+	const int want_type = in->Bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB;
+	if (c->png && in->Type != want_type) {
+		error(domain, "interpretation %d with %d bands not supported on the device path (PNG tiles take B_W with 1-2 bands, sRGB with 3-4)",
+			in->Type, in->Bands);
 		return -1;
 	}
 	if (in->bpl && in->bpl < (size_t) in->Xsize * in->Bands) {
@@ -322,13 +418,18 @@ dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options,
 		return -1;
 	}
 	const bool dz = o.layout == VB200_DZ_LAYOUT_DZ;
-	P->suffix = o.suffix ? o.suffix : (dz ? ".jpeg" : ".jpg");
+	P->suffix = o.suffix ? o.suffix : c->png ? ".png" : (dz ? ".jpeg" : ".jpg");
 	if (P->suffix.find('[') != std::string::npos) {
 		error(domain, "suffix options not supported on the device path");
 		return -1;
 	}
-	if (strcasecmp(P->suffix.c_str(), ".jpg") != 0 && strcasecmp(P->suffix.c_str(), ".jpeg") != 0) {
-		error(domain, "suffix %s not supported on the device path (JPEG tiles only)", P->suffix.c_str());
+	if (c->png && strcasecmp(P->suffix.c_str(), ".png") != 0) {
+		error(domain, "suffix %s not supported on the device path (PNG tiles here; vb200_dzsave takes JPEG suffixes)", P->suffix.c_str());
+		return -1;
+	}
+	if (!c->png && strcasecmp(P->suffix.c_str(), ".jpg") != 0 && strcasecmp(P->suffix.c_str(), ".jpeg") != 0) {
+		error(domain, "suffix %s not supported on the device path (JPEG tiles only%s)", P->suffix.c_str(),
+			strcasecmp(P->suffix.c_str(), ".png") == 0 ? "; vb200_dzsave_png takes PNG tiles" : "");
 		return -1;
 	}
 	P->layout = o.layout;
@@ -385,13 +486,24 @@ dz_plan(const char *domain, const VB200Image *in, const VB200DzOptions *options,
 				P->tiles.push_back(t);
 			}
 	}
-	*jpeg = o.jpeg;
-	if (jpeg->Q == 0)
-		jpeg->Q = 75;
-	return 0;
+	if (!c->png) {
+		c->jpeg = o.jpeg;
+		if (c->jpeg.Q == 0)
+			c->jpeg.Q = 75;
+		return 0;
+	}
+	/* spngsave's defaults (spngsave.c:700-748): compression 6, filter NONE, no interlace, 8 bits, Xres 1 */
+	const VB200PngSaveOptions defaults = {6, 0, 1.0, 0, 0, 8};
+	c->pngo = png ? *png : defaults;
+	/* the encoder's own checks, once, before any device call: its geometry limit grows with the tile, so the largest shape */
+	const DzLevel &top = P->levels.back();
+	Encoder enc;
+	return png_encoder(domain, std::min(top.w, full), std::min(top.h, full), in->Bands, c->pngo, nullptr, 0, &enc);
 }
 
 std::atomic<size_t> g_budget{0};
+/* JPEG tiles' default batch bound.  PNG tiles take chunk_budget(), the PNG codecs' own: at ~20 bytes of deflate scratch a
+ * scanline byte, 1 GiB holds only ~180 RGBA tiles of 256 x 256, and the parse kernel runs one warp a tile. */
 constexpr size_t kDzBudget = (size_t) 1 << 30;
 
 struct DzTimer {
@@ -428,7 +540,7 @@ struct DzTimer {
 thread_local float t_dz_ms[4] = {-1, -1, -1, -1};
 
 int
-dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB200JpegSaveOptions &jpeg, cudaStream_t s)
+dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const DzCodec &codec, cudaStream_t s)
 {
 	DzScratch sc(s);
 	DzTimer timer(s);
@@ -453,7 +565,7 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 	std::map<std::pair<int, int>, std::vector<long>> shapes;
 	for (long i = 0; i < (long) P->tiles.size(); i++)
 		shapes[{P->tiles[i].w, P->tiles[i].h}].push_back(i);
-	const size_t budget = g_budget.load() ? g_budget.load() : kDzBudget;
+	const size_t budget = g_budget.load() ? g_budget.load() : codec.png ? chunk_budget() : kDzBudget;
 	std::vector<DzGatherTile> table;
 	std::vector<size_t> lens;
 	for (const auto &sh : shapes) {
@@ -461,7 +573,7 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 		const std::vector<long> &idx = sh.second;
 		const size_t frame_stride = ((size_t) w * h * bands + 15) & ~(size_t) 15;
 		Encoder enc;
-		if (jpeg_encoder(domain, w, h, bands, jpeg, &enc))
+		if (tile_encoder(domain, codec, w, h, bands, &enc))
 			return -1;
 		const size_t per_tile = frame_stride + enc.scratch_bytes + enc.stream_bytes;
 		if (per_tile > budget) {
@@ -517,7 +629,7 @@ dev_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB
 }
 
 int
-host_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const VB200JpegSaveOptions &jpeg)
+host_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const DzCodec &codec)
 {
 	const int bands = in->Bands, nl = (int) P->levels.size();
 	struct HostLevel {
@@ -534,14 +646,11 @@ host_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const V
 		L.push_back({store[k].data(), (size_t) l.w * bands});
 	}
 	std::vector<unsigned char> one;
-	unsigned long long events[3]; /* the progressive coder's counters, a test hook of its own */
 	for (DzTile &t : P->tiles) {
 		const HostLevel &l = L[nl - 1 - t.level];
 		const unsigned char *p = l.p + (size_t) t.top * l.bpl + (size_t) t.left * bands;
 		one.clear();
-		if (jpeg.interlace ? host_jpeg_encode_progressive(domain, p, l.bpl, t.w, t.h, bands, jpeg.Q, jpeg.subsample_mode, jpeg.restart_interval, one, events)
-						   : host_jpeg_encode(domain, p, l.bpl, t.w, t.h, bands, jpeg.Q, jpeg.subsample_mode, jpeg.optimize_coding != 0,
-								 jpeg.restart_interval, one)) {
+		if (host_tile_encode(domain, codec, p, l.bpl, t.w, t.h, bands, one)) {
 			error(domain, "level %d tile %d_%d", t.level, t.x, t.y);
 			return -1;
 		}
@@ -553,7 +662,8 @@ host_dzsave(const char *domain, const VB200Image *in, VB200DzPyramid *P, const V
 }
 
 int
-dzsave_entry(const char *domain, const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out, bool device)
+dzsave_entry(const char *domain, const VB200Image *in, const VB200DzOptions *options, bool png, const VB200PngSaveOptions *pngo,
+	VB200DzPyramid **out, bool device)
 {
 	if (!out) {
 		error(domain, "null argument");
@@ -561,17 +671,18 @@ dzsave_entry(const char *domain, const VB200Image *in, const VB200DzOptions *opt
 	}
 	*out = nullptr;
 	VB200DzPyramid *P = new VB200DzPyramid;
-	VB200JpegSaveOptions jpeg;
-	int rc = dz_plan(domain, in, options, P, &jpeg);
+	DzCodec codec;
+	codec.png = png;
+	int rc = dz_plan(domain, in, options, pngo, P, &codec);
 	if (!rc && device)
-		rc = ensure_init(domain) ? -1 : dev_dzsave(domain, in, P, jpeg, current_stream());
+		rc = ensure_init(domain) ? -1 : dev_dzsave(domain, in, P, codec, current_stream());
 	else if (!rc) {
 		if (in->where != VB200_HOST) {
 			error(domain, "the host twin takes host memory");
 			rc = -1;
 		}
 		else
-			rc = host_dzsave(domain, in, P, jpeg);
+			rc = host_dzsave(domain, in, P, codec);
 	}
 	if (rc) {
 		delete P;
@@ -612,13 +723,25 @@ using namespace vb200;
 extern "C" int
 vb200_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out)
 {
-	return dzsave_entry("dzsave", in, options, out, true);
+	return dzsave_entry("dzsave", in, options, false, nullptr, out, true);
 }
 
 extern "C" int
 vb200_debug_dzsave(const VB200Image *in, const VB200DzOptions *options, VB200DzPyramid **out)
 {
-	return dzsave_entry("dzsave", in, options, out, false);
+	return dzsave_entry("dzsave", in, options, false, nullptr, out, false);
+}
+
+extern "C" int
+vb200_dzsave_png(const VB200Image *in, const VB200DzOptions *options, const VB200PngSaveOptions *png, VB200DzPyramid **out)
+{
+	return dzsave_entry("dzsave_png", in, options, true, png, out, true);
+}
+
+extern "C" int
+vb200_debug_dzsave_png(const VB200Image *in, const VB200DzOptions *options, const VB200PngSaveOptions *png, VB200DzPyramid **out)
+{
+	return dzsave_entry("dzsave_png", in, options, true, png, out, false);
 }
 
 extern "C" void
@@ -743,8 +866,13 @@ vb200_dz_pyramid_level(const VB200Image *in, int n_from_top, VB200Image *out)
 		error(domain, "null argument");
 		return -1;
 	}
-	if (in->BandFmt != VB200_FORMAT_UCHAR || (in->Bands != 1 && in->Bands != 3) || in->Xsize < 1 || in->Ysize < 1) {
-		error(domain, "uchar images of 1 or 3 bands only");
+	if (in->BandFmt != VB200_FORMAT_UCHAR || in->Bands < 1 || in->Bands > 4 || in->Xsize < 1 || in->Ysize < 1) {
+		error(domain, "uchar images of 1 to 4 bands only");
+		return -1;
+	}
+	/* 2 and 4 bands are shrunk with alpha: that is what the reference does for B_W and sRGB (vips_image_hasalpha) */
+	if ((in->Bands == 2 && in->Type != VB200_INTERPRETATION_B_W) || (in->Bands == 4 && in->Type != VB200_INTERPRETATION_sRGB)) {
+		error(domain, "a %d-band image takes interpretation %s (its last band alpha)", in->Bands, in->Bands == 2 ? "B_W" : "sRGB");
 		return -1;
 	}
 	int w = in->Xsize, h = in->Ysize;
@@ -784,7 +912,7 @@ extern "C" int
 vb200_debug_dz_pyramid_level(const void *pixels, size_t bpl, int width, int height, int bands, int n_from_top, void *out)
 {
 	const char *domain = "dz_pyramid_level (host twin)";
-	if (!pixels || !out || width < 1 || height < 1 || (bands != 1 && bands != 3) || n_from_top < 0) {
+	if (!pixels || !out || width < 1 || height < 1 || bands < 1 || bands > 4 || n_from_top < 0) {
 		error(domain, "bad argument");
 		return -1;
 	}

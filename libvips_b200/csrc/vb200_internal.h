@@ -246,6 +246,10 @@ int host_jpeg_encode(const char *domain, const unsigned char *img, size_t bpl, i
 	int restart, std::vector<unsigned char> &out);
 int host_jpeg_encode_progressive(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, int quality, int subsample_mode,
 	int restart, std::vector<unsigned char> &out, unsigned long long *events);
+/* png_encode.cu: the PNG encoder's host twin (the kernels' per-position, per-symbol and per-block code on the CPU), the
+ * whole stream into out */
+int host_png_encode(const char *domain, const unsigned char *img, size_t bpl, int w, int h, int bands, const VB200PngSaveOptions &o,
+	const unsigned char *profile, size_t profile_len, std::vector<unsigned char> &out);
 /* encode.cu: the encoders' shared driver.  place(lengths, length_stride, at, &out), which an encoder's chunk calls once its
  * kernels have the streams' lengths (device memory, an unsigned long long every length_stride bytes), reads them back,
  * fails the call for a stream longer than its slot, and stores where each stream goes: stream i at out + at[i] (at: the
