@@ -851,16 +851,16 @@ select_input_profile(const char *domain, int frame, const VB200ThumbnailIcc &icc
 	return -1;
 }
 
-/* One launch per chunk of frames, whatever profiles they carry: frame f runs jobs[job_of[f]].  A CTA serves one frame,
+/* One launch per chunk of frames, whatever profiles they carry: frame f runs jobs[frames[f].exp].  A CTA serves one frame,
  * copies that frame's job into shared memory once and walks the frame's pixels.
  */
 __global__ void __launch_bounds__(256)
-icc_frames_kernel(const IccJob *__restrict__ jobs, const int *__restrict__ job_of, const uint8_t *__restrict__ in, size_t in_stride,
+icc_frames_kernel(const IccJob *__restrict__ jobs, const IccFrame *__restrict__ frames, const uint8_t *__restrict__ in, size_t in_stride,
 	int in_ps, uint8_t *__restrict__ out, size_t out_stride, int out_ps, size_t pixels)
 {
 	__shared__ __align__(16) unsigned char smem[sizeof(IccJob)];
 	const int f = blockIdx.y;
-	const unsigned *src = (const unsigned *) (jobs + job_of[f]);
+	const unsigned *src = (const unsigned *) (jobs + frames[f].exp);
 	for (int i = threadIdx.x; i < (int) (sizeof(IccJob) / 4); i += blockDim.x)
 		((unsigned *) smem)[i] = src[i];
 	__syncthreads();
@@ -1149,49 +1149,31 @@ select_linear(const char *domain, int frame, const VB200ThumbnailIcc &icc, int b
 } // namespace
 
 int
-icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands)
+icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, bool linear, int *out_bands)
 {
 	std::lock_guard<std::mutex> lock(st->lock);
-	stage_copy(st, icc, bands);
-	int ob = 0;
-	if (check_output_profile(domain, *st, &ob))
-		return -1;
-	st->out_bands = ob + bands - (bands < 3 ? 1 : 3);
-	/* parse the output side once now, so that a profile the evaluator declines fails here rather than per batch */
-	JobSpec sp;
-	stage_job_spec(*st, MODE_XYZ_EXPORT, IccProfileRef{nullptr, 0}, &sp);
-	IccJob J;
-	std::vector<float> pool;
-	int b, f, t;
-	if (build_job(domain, sp, VB200_FORMAT_UCHAR, bands, bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, &J, pool, &b, &f, &t))
-		return -1;
-	*out_bands = st->out_bands;
-	return 0;
-}
-
-int
-icc_stage_set_linear(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands)
-{
-	std::lock_guard<std::mutex> lock(st->lock);
-	if (bands < 3) {
+	if (linear && bands < 3) {
 		error(domain, "linear colour-managed thumbnails on the device path need 3+ band frames (sGrey / GREY16 import is not built)");
 		return -1;
 	}
 	stage_copy(st, icc, bands);
-	st->linear = true;
-	st->out_bands = bands; /* no output profile: each frame exports to its own (RGB) profile, or runs the plain path */
-	if (icc->output_profile) {
+	st->linear = linear;
+	st->out_bands = bands; /* linear without an output profile: each frame exports to its own (RGB) profile, or runs the plain path */
+	if (!linear || icc->output_profile) {
 		int ob = 0;
 		if (check_output_profile(domain, *st, &ob))
 			return -1;
-		st->out_bands = ob + bands - 3;
-		/* parse the export once now, so that a profile the evaluator declines fails here rather than per batch */
+		st->out_bands = ob + bands - (bands < 3 ? 1 : 3);
+		/* parse the export once now, so that a profile the evaluator declines fails here rather than per batch: from the float
+		 * XYZ the linear resize leaves, or from the 8-bit thumbnail
+		 */
 		JobSpec sp;
-		stage_job_spec(*st, MODE_EXPORT, IccProfileRef{st->icc.output_profile, st->icc.output_len}, &sp);
+		stage_job_spec(*st, linear ? MODE_EXPORT : MODE_XYZ_EXPORT, IccProfileRef{st->icc.output_profile, st->icc.output_len}, &sp);
 		IccJob J;
 		std::vector<float> pool;
 		int b, f, t;
-		if (build_job(domain, sp, VB200_FORMAT_FLOAT, bands, VB200_INTERPRETATION_XYZ, &J, pool, &b, &f, &t))
+		if (build_job(domain, sp, linear ? VB200_FORMAT_FLOAT : VB200_FORMAT_UCHAR, bands,
+				linear ? VB200_INTERPRETATION_XYZ : bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB, &J, pool, &b, &f, &t))
 			return -1;
 	}
 	*out_bands = st->out_bands;
@@ -1199,54 +1181,60 @@ icc_stage_set_linear(const char *domain, IccStage *st, const VB200ThumbnailIcc *
 }
 
 int
-icc_stage_run_linear(const char *domain, IccStage *st, int n, const void *const *embedded, const size_t *embedded_lens, cudaStream_t s,
-	int frame0, const std::function<int(const LinIccBatch &)> &body)
+icc_stage_batch(const char *domain, IccStage *st, int n, const void *const *embedded, const size_t *embedded_lens, cudaStream_t s,
+	int frame0, const std::function<int(const IccBatch &)> &body)
 {
 	if (n <= 0)
 		return 0;
 	std::lock_guard<std::mutex> lock(st->lock);
 	std::vector<IccCacheEntry *> used; /* distinct entries of this batch, in first-use order */
-	auto index_of = [&](IccCacheEntry *e) {
-		int k = 0;
-		while (k < (int) used.size() && used[k] != e)
-			k++;
-		if (k == (int) used.size())
-			used.push_back(e);
-		return k;
-	};
-	std::vector<LinIccFrame> frames(n);
-	for (int f = 0; f < n; f++) {
-		LinChoice c;
-		if (select_linear(domain, frame0 + f, st->icc, st->bands, embedded ? embedded[f] : nullptr, embedded && embedded_lens ? embedded_lens[f] : 0,
-				&c))
+	/* *k: the batch's index of the cached job for (mode, profile) */
+	auto job = [&](int f, int mode, const IccProfileRef &ref, int *k) {
+		IccCacheEntry *e = stage_entry(domain, *st, frame0 + f, mode, ref, used);
+		if (!e)
 			return -1;
-		frames[f] = LinIccFrame{c.branch, -1, -1};
-		if (c.branch == LIN_IMPORT) {
-			IccCacheEntry *e = stage_entry(domain, *st, frame0 + f, MODE_IMPORT, c.imp, used);
-			if (!e)
+		*k = 0;
+		while (*k < (int) used.size() && used[*k] != e)
+			++*k;
+		if (*k == (int) used.size())
+			used.push_back(e);
+		return 0;
+	};
+	std::vector<IccFrame> frames(n);
+	for (int f = 0; f < n; f++) {
+		const void *emb = embedded ? embedded[f] : nullptr;
+		const size_t emb_len = embedded && embedded_lens ? embedded_lens[f] : 0;
+		if (!st->linear) {
+			IccProfileRef ref{nullptr, 0};
+			int source = 0;
+			const int mode = select_input_profile(domain, frame0 + f, st->icc, st->bands, emb, emb_len, &ref, &source);
+			frames[f] = IccFrame{LIN_PLAIN, -1, -1};
+			if (mode < 0 || job(f, mode, ref, &frames[f].exp))
 				return -1;
-			frames[f].imp = index_of(e);
+			continue;
 		}
-		if (c.branch != LIN_PLAIN) {
-			IccCacheEntry *e = stage_entry(domain, *st, frame0 + f, MODE_EXPORT, c.exp, used);
-			if (!e)
-				return -1;
-			frames[f].exp = index_of(e);
-		}
+		LinChoice c;
+		if (select_linear(domain, frame0 + f, st->icc, st->bands, emb, emb_len, &c))
+			return -1;
+		frames[f] = IccFrame{c.branch, -1, -1};
+		if (c.branch == LIN_IMPORT && job(f, MODE_IMPORT, c.imp, &frames[f].imp))
+			return -1;
+		if (c.branch != LIN_PLAIN && job(f, MODE_EXPORT, c.exp, &frames[f].exp))
+			return -1;
 	}
 	std::vector<IccJob> jobs(used.size());
 	for (size_t k = 0; k < used.size(); k++)
 		jobs[k] = used[k]->job;
 	const size_t jobs_bytes = jobs.size() * sizeof(IccJob);
 	void *table = nullptr;
-	if (dev_alloc(domain, &table, jobs_bytes + (size_t) n * sizeof(LinIccFrame), s))
+	if (dev_alloc(domain, &table, jobs_bytes + (size_t) n * sizeof(IccFrame), s))
 		return -1;
 	int rc = 0;
 	if (cudaMemcpyAsync(table, jobs.data(), jobs_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-		cudaMemcpyAsync((char *) table + jobs_bytes, frames.data(), (size_t) n * sizeof(LinIccFrame), cudaMemcpyHostToDevice, s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "linear ICC job table upload");
+		cudaMemcpyAsync((char *) table + jobs_bytes, frames.data(), (size_t) n * sizeof(IccFrame), cudaMemcpyHostToDevice, s) != cudaSuccess)
+		rc = cuda_fail(domain, cudaGetLastError(), "ICC job table upload");
 	if (!rc) {
-		const LinIccBatch b{(const IccJob *) table, (const LinIccFrame *) ((char *) table + jobs_bytes), jobs.data(), frames.data()};
+		const IccBatch b{(const IccJob *) table, (const IccFrame *) ((char *) table + jobs_bytes), jobs.data(), frames.data()};
 		rc = body(b);
 	}
 	if (stage_hold(domain, used, s))
@@ -1283,69 +1271,35 @@ int
 icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
 	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s, int frame0)
 {
-	if (n <= 0)
-		return 0;
-	std::lock_guard<std::mutex> lock(st->lock);
-	std::vector<IccCacheEntry *> used; /* distinct entries of this batch, in first-use order */
-	std::vector<int> job_of(n);
-	for (int f = 0; f < n; f++) {
-		IccProfileRef ref{nullptr, 0};
-		int source = 0;
-		const int mode = select_input_profile(domain, frame0 + f, st->icc, st->bands, embedded ? embedded[f] : nullptr,
-			embedded && embedded_lens ? embedded_lens[f] : 0, &ref, &source);
-		if (mode < 0)
-			return -1;
-		IccCacheEntry *e = stage_entry(domain, *st, frame0 + f, mode, ref, used);
-		if (!e)
-			return -1;
-		int k = 0;
-		while (k < (int) used.size() && used[k] != e)
-			k++;
-		if (k == (int) used.size())
-			used.push_back(e);
-		job_of[f] = k;
-	}
-	std::vector<IccJob> jobs(used.size());
-	for (size_t k = 0; k < used.size(); k++)
-		jobs[k] = used[k]->job;
-	const size_t jobs_bytes = jobs.size() * sizeof(IccJob);
-	void *table = nullptr;
-	if (dev_alloc(domain, &table, jobs_bytes + (size_t) n * sizeof(int), s))
-		return -1;
-	int rc = 0;
-	if (cudaMemcpyAsync(table, jobs.data(), jobs_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-		cudaMemcpyAsync((char *) table + jobs_bytes, job_of.data(), (size_t) n * sizeof(int), cudaMemcpyHostToDevice, s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "ICC job table upload");
-	const int in_ps = st->bands, out_ps = st->out_bands;
-	/* a few CTAs per frame, each walking its share of the pixels; frames on gridDim.y, at most kMaxBatchFrames a launch */
-	const unsigned per_frame = (unsigned) std::min<size_t>((pixels + 255) / 256, 64);
-	/* VB200_ICC_TIMING: CUDA events around this call's launches, read back by vb200_debug_icc_stage_ms */
-	const bool timing = getenv("VB200_ICC_TIMING") != nullptr;
-	if (timing) {
-		for (cudaEvent_t *ev : {&g_icc_timing.start, &g_icc_timing.stop})
-			if (!*ev && cudaEventCreate(ev) != cudaSuccess)
-				rc = cuda_fail(domain, cudaGetLastError(), "ICC timing event");
-		if (!rc)
-			cudaEventRecord(g_icc_timing.start, s);
-		g_icc_timing.pending = !rc;
-	}
-	for (int f0 = 0; f0 < n && !rc; f0 += kMaxBatchFrames) {
-		const int nf = std::min(n - f0, (int) kMaxBatchFrames);
-		icc_frames_kernel<<<dim3(per_frame, nf), 256, 0, s>>>((const IccJob *) table, (const int *) ((char *) table + jobs_bytes) + f0,
-			(const uint8_t *) in + (size_t) f0 * in_stride, in_stride, in_ps, (uint8_t *) out + (size_t) f0 * out_stride, out_stride,
-			out_ps, pixels);
-		const cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-			rc = cuda_fail(domain, e, "icc_frames_kernel");
-		else
-			count_launch();
-	}
-	if (timing && g_icc_timing.pending)
-		cudaEventRecord(g_icc_timing.stop, s);
-	if (stage_hold(domain, used, s))
-		rc = -1;
-	dev_free(table, s);
-	return rc;
+	return icc_stage_batch(domain, st, n, embedded, embedded_lens, s, frame0, [&](const IccBatch &b) {
+		const int in_ps = st->bands, out_ps = st->out_bands;
+		int rc = 0;
+		/* a few CTAs per frame, each walking its share of the pixels; frames on gridDim.y, at most kMaxBatchFrames a launch */
+		const unsigned per_frame = (unsigned) std::min<size_t>((pixels + 255) / 256, 64);
+		/* VB200_ICC_TIMING: CUDA events around this call's launches, read back by vb200_debug_icc_stage_ms */
+		const bool timing = getenv("VB200_ICC_TIMING") != nullptr;
+		if (timing) {
+			for (cudaEvent_t *ev : {&g_icc_timing.start, &g_icc_timing.stop})
+				if (!*ev && cudaEventCreate(ev) != cudaSuccess)
+					rc = cuda_fail(domain, cudaGetLastError(), "ICC timing event");
+			if (!rc)
+				cudaEventRecord(g_icc_timing.start, s);
+			g_icc_timing.pending = !rc;
+		}
+		for (int f0 = 0; f0 < n && !rc; f0 += kMaxBatchFrames) {
+			const int nf = std::min(n - f0, (int) kMaxBatchFrames);
+			icc_frames_kernel<<<dim3(per_frame, nf), 256, 0, s>>>(b.d_jobs, b.d_frames + f0, (const uint8_t *) in + (size_t) f0 * in_stride,
+				in_stride, in_ps, (uint8_t *) out + (size_t) f0 * out_stride, out_stride, out_ps, pixels);
+			const cudaError_t e = cudaGetLastError();
+			if (e != cudaSuccess)
+				rc = cuda_fail(domain, e, "icc_frames_kernel");
+			else
+				count_launch();
+		}
+		if (timing && g_icc_timing.pending)
+			cudaEventRecord(g_icc_timing.stop, s);
+		return rc;
+	});
 }
 
 /* test hook: the selection of one frame, as the stage makes it */

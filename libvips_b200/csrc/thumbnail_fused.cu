@@ -1003,7 +1003,7 @@ struct LinearThumb;
 int linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const ReduceGeom &gv, const ReduceGeom &gh,
 	const AxisTable &tv, const AxisTable &th, LinearThumb **out);
 int linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_stride, void *out, size_t out_stride, int n,
-	cudaStream_t s, const LinIccBatch *icc = nullptr, int out_bands = 0);
+	cudaStream_t s, const IccBatch *icc = nullptr, int out_bands = 0);
 void linear_thumb_free(LinearThumb *lt);
 
 /* The fused kernel a plan runs, chosen once by plan_build_fused */
@@ -1068,14 +1068,13 @@ struct ThumbnailPlanImpl {
 	/* vips_sharpen appended to every batch (vb200_thumbnail_plan_set_sharpen) */
 	bool sharpen = false;
 	double sh_sigma = 0.5, sh_x1 = 2.0, sh_y2 = 10.0, sh_y3 = 20.0, sh_m1 = 0.0, sh_m2 = 3.0;
-	/* colour management between the thumbnail and the sharpen stage (vb200_thumbnail_plan_set_icc); null = off */
+	/* colour management (vb200_thumbnail_plan_set_icc / _set_linear_icc), null = off: in the stage's linear mode when the plan
+	 * is linear (import / export inside the linear thumbnail), else between the thumbnail and the sharpen stage
+	 */
 	IccStage *icc = nullptr;
 	int icc_bands = 0;			 /* output bands with the stage on */
-	/* linear = TRUE with colour management (vb200_thumbnail_plan_set_linear_icc): import / export inside the linear thumbnail */
-	IccStage *licc = nullptr;
-	int licc_bands = 0;
 	size_t stage_out_frame = 0; /* the host pump's output slots are sized for frames of this many bytes */
-	int out_bands() const { return icc ? icc_bands : licc ? licc_bands : bands; }
+	int out_bands() const { return icc ? icc_bands : bands; }
 };
 
 /* sharpen_fused.cu */
@@ -1872,12 +1871,8 @@ thumbnail_plan_init(const char *domain, ThumbnailPlanImpl *pl)
 	return 0;
 }
 
-static int thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s);
 static int thumbnail_plan_run_fused(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
 	size_t out_stride, int n, cudaStream_t s);
-static int thumbnail_plan_run_linear_icc(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s, const void *const *embedded, const size_t *embedded_lens, int frame0);
 
 double
 thumbnail_common_shrink(int w, int h, int tw, int th, int size)
@@ -1887,206 +1882,81 @@ thumbnail_common_shrink(int w, int h, int tw, int th, int size)
 	return std::min(hs, vs);
 }
 
-/* The plan's stages over a device batch: thumbnail kernel -> ICC stage (if set) -> sharpen stage (if set).  Every stage but
- * the last writes a scratch batch from the stream-ordered pool; the last writes `out`.  embedded / embedded_lens: each
- * frame's embedded ICC profile for the ICC stage (NULL: none).
- */
-int
-thumbnail_plan_run_device(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s, const void *const *embedded = nullptr, const size_t *embedded_lens = nullptr,
-	int frame0 = 0)
-{
-	if (n <= 0)
-		return 0;
-	if (pl->licc)
-		return thumbnail_plan_run_linear_icc(domain, pl, in, in_stride, out, out_stride, n, s, embedded, embedded_lens, frame0);
-	if (!pl->sharpen && !pl->icc)
-		return thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, out, out_stride, n, s);
-	const size_t frame = (size_t) pl->OW * pl->OH * pl->bands;
-	const int sb = pl->out_bands(); /* bands the sharpen stage sees */
-	const size_t sframe = (size_t) pl->OW * pl->OH * sb;
-	void *mid = nullptr, *mid2 = nullptr;
-	if (dev_alloc(domain, &mid, frame * n, s))
-		return -1;
-	if (pl->icc && pl->sharpen && dev_alloc(domain, &mid2, sframe * n, s)) {
-		dev_free(mid, s);
-		return -1;
-	}
-	int rc = thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, mid, frame, n, s);
-	const void *sin = mid;
-	if (!rc && pl->icc) {
-		rc = icc_stage_run(domain, pl->icc, mid, frame, pl->sharpen ? mid2 : out, pl->sharpen ? sframe : out_stride, n,
-			(size_t) pl->OW * pl->OH, embedded, embedded_lens, s, frame0);
-		sin = mid2;
-	}
-	if (!rc && pl->sharpen) {
-		if (sb != 3 && sb != 4) {
-			error(domain, "the sharpen stage needs 3- or 4-band frames, the output profile gives %d bands", sb);
-			rc = -1;
-		}
-		else
-			rc = dev_sharpen_fused(domain, sin, (size_t) pl->OW * sb, sframe, out, (size_t) pl->OW * sb, out_stride, n, pl->OW, pl->OH, sb,
-				pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
-		if (rc == 1) {
-			error(domain, "sharpen parameters are not on the fused path (mask too wide)");
-			rc = -1;
-		}
-	}
-	dev_free(mid, s);
-	if (mid2)
-		dev_free(mid2, s);
-	return rc;
-}
-
-/* thumbnail.c:766-806, 848-902, 971-987 for an 8-bit sRGB image without ICC profile, as the chain of leaf
- * kernels (geometries the two-kernel path declines): sRGB -> scRGB (float; alpha / 255), float premultiply
- * (max_alpha 1.0), float resize, float unpremultiply, scRGB -> sRGB.
+/* One frame through the leaf kernels (upsizing plans, 1- and 2-band plans, one-axis shrinks, and the linear geometries the
+ * two-kernel path declines): enter the working space, premultiply, vips_resize, unpremultiply, leave the working space.
+ *   uchar plan:   no working space; premultiply with the 8-bit LUT (thumbnail.c:848-902)
+ *   linear plan:  sRGB -> scRGB ... scRGB -> sRGB, float premultiply at 1.0 (thumbnail.c:766-806, 971-987)
+ *   LIN_XYZ:      sRGB -> scRGB ... scRGB -> XYZ -> the export job (:790-805, 957-970)
+ *   LIN_IMPORT:   the import job ... the export job, float premultiply at 255 on XYZ (:766-789, 929-942; header.c:195-206)
+ * fr / jobs: the frame's colour management and the batch's host job table (fr null: none).  `out` takes the last step's bands.
  */
 static int
-thumbnail_linear_chain(const char *domain, ThumbnailPlanImpl *pl, const void *in, void *out, cudaStream_t s)
-{
-	DevImage din, lin, pre, res, unpre, fin;
-	din.w = pl->W;
-	din.h = pl->H;
-	din.bands = pl->bands;
-	din.fmt = VB200_FORMAT_UCHAR;
-	din.type = VB200_INTERPRETATION_sRGB;
-	din.bpl = (size_t) pl->W * pl->bands;
-	din.data = const_cast<void *>(in);
-	int rc = dev_colourspace(domain, din, &lin, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, s);
-	const DevImage *cur = &lin;
-	if (!rc && pl->premul) {
-		rc = dev_premultiply(domain, lin, &pre, 0.0, 0, s); /* max_alpha from scRGB: 1.0 */
-		cur = &pre;
-	}
-	if (!rc)
-		rc = dev_resize(domain, *cur, &res, 1.0 / pl->hshrink, 1.0 / pl->vshrink, VB200_KERNEL_LANCZOS3, 2.0, s);
-	cur = &res;
-	if (!rc && pl->premul) {
-		rc = dev_unpremultiply(domain, res, &unpre, 0.0, 0, s);
-		cur = &unpre;
-	}
-	if (!rc)
-		rc = dev_colourspace(domain, *cur, &fin, VB200_INTERPRETATION_sRGB, VB200_INTERPRETATION_scRGB, s);
-	if (!rc) {
-		const size_t line = (size_t) fin.w * fin.bands;
-		if (cudaMemcpy2DAsync(out, line, fin.data, fin.bpl, line, fin.h, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
-			rc = cuda_fail(domain, cudaGetLastError(), "linear thumbnail copy");
-	}
-	dev_image_release(&lin, s);
-	dev_image_release(&pre, s);
-	dev_image_release(&res, s);
-	dev_image_release(&unpre, s);
-	dev_image_release(&fin, s);
-	return rc;
-}
-
-/* thumbnail.c:766-805, 848-902, 929-970 for one colour-managed frame of a linear plan, as the chain of leaf kernels (geometries the
- * two-kernel path declines, and VB200_NO_LINEAR_FUSED): LIN_IMPORT runs the import job (icc_kernel) -> float premultiply (255) ->
- * float resize -> float unpremultiply (255) -> the export job; LIN_XYZ the scRGB chain of thumbnail_linear_chain, then
- * vips_colourspace(XYZ) and the export job.  `out` takes the export's bands.
- */
-static int
-thumbnail_linear_icc_chain(const char *domain, ThumbnailPlanImpl *pl, const LinIccFrame &fr, const IccJob *jobs, const void *in,
+thumbnail_leaf_chain(const char *domain, const ThumbnailPlanImpl *pl, const IccFrame *fr, const IccJob *jobs, const void *in,
 	void *out, cudaStream_t s)
 {
+	const int kind = fr ? fr->kind : LIN_PLAIN;
 	DevImage din, lin, pre, res, unpre, xyz, fin;
 	din.w = pl->W;
 	din.h = pl->H;
 	din.bands = pl->bands;
 	din.fmt = VB200_FORMAT_UCHAR;
-	din.type = VB200_INTERPRETATION_sRGB;
+	din.type = pl->bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB;
 	din.bpl = (size_t) pl->W * pl->bands;
 	din.data = const_cast<void *>(in);
-	const bool imp = fr.kind == LIN_IMPORT;
-	const double max_alpha = imp ? 255.0 : 1.0; /* XYZ after the import, scRGB otherwise (header.c:195-206) */
-	int rc = imp ? icc_job_apply(domain, jobs, fr.imp, din, &lin, s)
-				 : dev_colourspace(domain, din, &lin, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, s);
-	const DevImage *cur = &lin;
+	const double max_alpha = pl->linear && kind != LIN_IMPORT ? 1.0 : 255.0;
+	const int uchar_mode = !pl->linear;
+	const DevImage *cur = &din;
+	int rc = 0;
+	if (kind == LIN_IMPORT)
+		rc = icc_job_apply(domain, jobs, fr->imp, din, &lin, s);
+	else if (pl->linear)
+		rc = dev_colourspace(domain, din, &lin, VB200_INTERPRETATION_scRGB, VB200_INTERPRETATION_sRGB, s);
+	if (pl->linear)
+		cur = &lin;
 	if (!rc && pl->premul) {
-		rc = dev_premultiply(domain, lin, &pre, max_alpha, 0, s);
+		rc = dev_premultiply(domain, *cur, &pre, max_alpha, uchar_mode, s);
 		cur = &pre;
 	}
 	if (!rc)
 		rc = dev_resize(domain, *cur, &res, 1.0 / pl->hshrink, 1.0 / pl->vshrink, VB200_KERNEL_LANCZOS3, 2.0, s);
 	cur = &res;
 	if (!rc && pl->premul) {
-		rc = dev_unpremultiply(domain, res, &unpre, max_alpha, 0, s);
+		rc = dev_unpremultiply(domain, res, &unpre, max_alpha, uchar_mode, s);
 		cur = &unpre;
 	}
-	if (!rc && !imp) {
-		rc = dev_colourspace(domain, *cur, &xyz, VB200_INTERPRETATION_XYZ, VB200_INTERPRETATION_scRGB, s);
+	if (!rc && pl->linear && kind != LIN_IMPORT) {
+		rc = dev_colourspace(domain, *cur, &xyz, kind == LIN_XYZ ? VB200_INTERPRETATION_XYZ : VB200_INTERPRETATION_sRGB,
+			VB200_INTERPRETATION_scRGB, s);
 		cur = &xyz;
 	}
-	if (!rc)
-		rc = icc_job_apply(domain, jobs, fr.exp, *cur, &fin, s);
+	if (!rc && kind != LIN_PLAIN) {
+		rc = icc_job_apply(domain, jobs, fr->exp, *cur, &fin, s);
+		cur = &fin;
+	}
 	if (!rc) {
-		const size_t line = (size_t) fin.w * fin.bands;
-		if (cudaMemcpy2DAsync(out, line, fin.data, fin.bpl, line, fin.h, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
-			rc = cuda_fail(domain, cudaGetLastError(), "linear ICC thumbnail copy");
+		const size_t line = (size_t) cur->w * cur->bands;
+		if (cudaMemcpy2DAsync(out, line, cur->data, cur->bpl, line, cur->h, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+			rc = cuda_fail(domain, cudaGetLastError(), "leaf thumbnail copy");
 	}
 	for (DevImage *d : {&lin, &pre, &res, &unpre, &xyz, &fin})
 		dev_image_release(d, s);
 	return rc;
 }
 
-/* A batch of a linear plan with colour management: each frame's branch and jobs from the stage, then the two-kernel path (one V and
- * one H launch per chunk of frames, whatever their branches) or, where it declines, the leaf chains frame by frame; then sharpen.
+/* The resize stage: the two-kernel linear path, the fused kernels (RGB frames expanded to RGBX around them) or, where they
+ * decline, the leaf chain frame by frame.  icc: the batch's jobs of a linear plan's colour management (null: none), which the
+ * linear path and the leaf chain run around the resize; `out` then takes the plan's output bands.
  */
 static int
-thumbnail_plan_run_linear_icc(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s, const void *const *embedded, const size_t *embedded_lens, int frame0)
-{
-	const int ob = pl->licc_bands;
-	const size_t sframe = (size_t) pl->OW * pl->OH * ob;
-	if (pl->sharpen && ob != 3 && ob != 4) {
-		error(domain, "the sharpen stage needs 3- or 4-band frames, the output profile gives %d bands", ob);
-		return -1;
-	}
-	void *mid = nullptr;
-	if (pl->sharpen && dev_alloc(domain, &mid, sframe * n, s))
-		return -1;
-	void *dst = pl->sharpen ? mid : out;
-	const size_t dst_stride = pl->sharpen ? sframe : out_stride;
-	int rc = icc_stage_run_linear(domain, pl->licc, n, embedded, embedded_lens, s, frame0, [&](const LinIccBatch &b) {
-		int r = pl->lin ? linear_thumb_run(domain, pl->lin, in, in_stride, dst, dst_stride, n, s, &b, ob) : 1;
-		for (int i = 0; r == 1 && i < n; i++) {
-			const void *fin = (const char *) in + (size_t) i * in_stride;
-			void *fout = (char *) dst + (size_t) i * dst_stride;
-			if (b.h_frames[i].kind == LIN_PLAIN ? thumbnail_linear_chain(domain, pl, fin, fout, s)
-												: thumbnail_linear_icc_chain(domain, pl, b.h_frames[i], b.h_jobs, fin, fout, s))
-				return -1;
-		}
-		return r == 1 ? 0 : r;
-	});
-	if (!rc && pl->sharpen) {
-		rc = dev_sharpen_fused(domain, mid, (size_t) pl->OW * ob, sframe, out, (size_t) pl->OW * ob, out_stride, n, pl->OW, pl->OH, ob,
-			pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
-		if (rc == 1) {
-			error(domain, "sharpen parameters are not on the fused path (mask too wide)");
-			rc = -1;
-		}
-	}
-	if (mid)
-		dev_free(mid, s);
-	return rc;
-}
-
-static int
 thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
-	size_t out_stride, int n, cudaStream_t s)
+	size_t out_stride, int n, cudaStream_t s, const IccBatch *icc)
 {
-	if (n <= 0)
-		return 0;
-	if (pl->linear) {
-		if (pl->lin)
-			return linear_thumb_run(domain, pl->lin, in, in_stride, out, out_stride, n, s);
-		for (int i = 0; i < n; i++)
-			if (thumbnail_linear_chain(domain, pl, (const char *) in + (size_t) i * in_stride, (char *) out + (size_t) i * out_stride, s))
-				return -1;
-		return 0;
+	if (pl->lin) {
+		const int rc = linear_thumb_run(domain, pl->lin, in, in_stride, out, out_stride, n, s, icc, pl->out_bands());
+		if (rc != 1)
+			return rc;
 	}
-	if (pl->fused && pl->rgb_expand && pl->bands == 3) {
+	else if (pl->fused && pl->rgb_expand && pl->bands == 3) {
 		/* sub-batches of RGBX scratch (~1 GiB): expand, fused kernel, compact */
 		if ((((uintptr_t) in) | in_stride) & 3) {
 			error(domain, "RGB frames must be 4-byte aligned for the fused path");
@@ -2127,43 +1997,66 @@ thumbnail_plan_run_thumbnail(const char *domain, ThumbnailPlanImpl *pl, const vo
 		dev_free(xout, s);
 		return rc;
 	}
-	if (pl->fused)
+	else if (pl->fused)
 		return thumbnail_plan_run_fused(domain, pl, in, in_stride, out, out_stride, n, s);
-
-	/* unfused chain of leaf kernels, frame by frame */
-	for (int i = 0; i < n; i++) {
-		DevImage d, pre, res, fin;
-		d.w = pl->W;
-		d.h = pl->H;
-		d.bands = pl->bands;
-		d.fmt = pl->fmt;
-		d.type = pl->bands < 3 ? VB200_INTERPRETATION_B_W : VB200_INTERPRETATION_sRGB;
-		d.bpl = (size_t) pl->W * pl->bands;
-		d.data = (char *) in + (size_t) i * in_stride;
-		const DevImage *src = &d;
-		if (pl->premul) {
-			if (dev_premultiply(domain, d, &pre, 255.0, 1, s))
-				return -1;
-			src = &pre;
-		}
-		if (dev_resize(domain, *src, &res, 1.0 / pl->hshrink, 1.0 / pl->vshrink, VB200_KERNEL_LANCZOS3, 2.0, s))
+	for (int i = 0; i < n; i++)
+		if (thumbnail_leaf_chain(domain, pl, icc ? &icc->h_frames[i] : nullptr, icc ? icc->h_jobs : nullptr,
+				(const char *) in + (size_t) i * in_stride, (char *) out + (size_t) i * out_stride, s))
 			return -1;
-		const DevImage *last = &res;
-		if (pl->premul) {
-			if (dev_unpremultiply(domain, res, &fin, 255.0, 1, s))
-				return -1;
-			last = &fin;
-		}
-		const size_t line = (size_t) last->w * last->bands;
-		VB200_CUDA(domain, cudaMemcpy2DAsync((char *) out + (size_t) i * out_stride, line, last->data, last->bpl, line,
-							   last->h, cudaMemcpyDeviceToDevice, s));
-		if (pl->premul) {
-			dev_image_release(&pre, s);
-			dev_image_release(&fin, s);
-		}
-		dev_image_release(&res, s);
-	}
 	return 0;
+}
+
+/* The plan's stages over a device batch: the resize stage (on a linear plan with colour management, its import and export
+ * inside it) -> the ICC stage (if set on a plan that is not linear) -> the sharpen stage (if set).  Every stage but the last
+ * writes a scratch batch from the stream-ordered pool; the last writes `out`.  embedded / embedded_lens: each frame's embedded
+ * ICC profile for colour management (NULL: none); frame0: the first frame's index in the caller's batch, for errors.
+ */
+int
+thumbnail_plan_run_device(const char *domain, ThumbnailPlanImpl *pl, const void *in, size_t in_stride, void *out,
+	size_t out_stride, int n, cudaStream_t s, const void *const *embedded = nullptr, const size_t *embedded_lens = nullptr,
+	int frame0 = 0)
+{
+	if (n <= 0)
+		return 0;
+	const int ob = pl->out_bands();
+	if (pl->sharpen && ob != 3 && ob != 4) {
+		error(domain, "the sharpen stage needs 3- or 4-band frames, the output profile gives %d bands", ob);
+		return -1;
+	}
+	const bool icc_stage = pl->icc && !pl->linear;
+	const size_t pixels = (size_t) pl->OW * pl->OH, frame = pixels * (icc_stage ? pl->bands : ob), oframe = pixels * ob;
+	void *mid = nullptr, *mid2 = nullptr; /* the resize stage's output, the ICC stage's before sharpen */
+	if ((icc_stage || pl->sharpen) && dev_alloc(domain, &mid, frame * n, s))
+		return -1;
+	if (icc_stage && pl->sharpen && dev_alloc(domain, &mid2, oframe * n, s)) {
+		dev_free(mid, s);
+		return -1;
+	}
+	void *dst = mid ? mid : out;
+	const size_t dst_stride = mid ? frame : out_stride;
+	int rc;
+	if (pl->icc && pl->linear)
+		rc = icc_stage_batch(domain, pl->icc, n, embedded, embedded_lens, s, frame0, [&](const IccBatch &b) {
+			return thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, dst, dst_stride, n, s, &b);
+		});
+	else
+		rc = thumbnail_plan_run_thumbnail(domain, pl, in, in_stride, dst, dst_stride, n, s, nullptr);
+	if (!rc && icc_stage)
+		rc = icc_stage_run(domain, pl->icc, mid, frame, mid2 ? mid2 : out, mid2 ? oframe : out_stride, n, pixels, embedded,
+			embedded_lens, s, frame0);
+	if (!rc && pl->sharpen) {
+		rc = dev_sharpen_fused(domain, mid2 ? mid2 : mid, (size_t) pl->OW * ob, oframe, out, (size_t) pl->OW * ob, out_stride, n, pl->OW,
+			pl->OH, ob, pl->sh_sigma, pl->sh_x1, pl->sh_y2, pl->sh_y3, pl->sh_m1, pl->sh_m2, s);
+		if (rc == 1) {
+			error(domain, "sharpen parameters are not on the fused path (mask too wide)");
+			rc = -1;
+		}
+	}
+	if (mid)
+		dev_free(mid, s);
+	if (mid2)
+		dev_free(mid2, s);
+	return rc;
 }
 
 /* the fused kernels over RGBA frames: the plan's kernel, but v1 when the base pointer or the frame stride of a batch
@@ -2222,8 +2115,6 @@ thumbnail_plan_destroy(ThumbnailPlanImpl *pl)
 	pl->lin = nullptr;
 	icc_stage_free(pl->icc);
 	pl->icc = nullptr;
-	icc_stage_free(pl->licc);
-	pl->licc = nullptr;
 	for (int i = 0; i < ThumbnailPlanImpl::kHintSlots; i++)
 		if (pl->hint_done[i]) {
 			cudaEventSynchronize(pl->hint_done[i]);
@@ -2253,6 +2144,28 @@ struct VB200ThumbnailPlan {
 	ThumbnailPlanImpl impl;
 };
 
+/* a plan's request: frames of n_pages pages of page_height rows, 8-bit unless the caller says otherwise; -1 for a geometry no
+ * plan takes
+ */
+static int
+plan_request(ThumbnailPlanImpl *pl, int width, int page_height, int n_pages, int bands, int has_alpha, int target_width,
+	int target_height, int size, int linear)
+{
+	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || bands <= 0 || target_width <= 0)
+		return -1;
+	pl->W = width;
+	pl->H = page_height * n_pages;
+	pl->page_h = n_pages > 1 ? page_height : 0;
+	pl->bands = bands;
+	pl->fmt = VB200_FORMAT_UCHAR;
+	pl->has_alpha = has_alpha;
+	pl->target_w = target_width;
+	pl->target_h = target_height > 0 ? target_height : target_width;
+	pl->size = size;
+	pl->linear = linear;
+	return 0;
+}
+
 extern "C" VB200ThumbnailPlan *
 vb200_thumbnail_plan_new(int width, int height, int bands, int band_format, int has_alpha, int target_width,
 	int target_height, int size, int linear)
@@ -2268,23 +2181,14 @@ vb200_thumbnail_plan_new_pages(int width, int page_height, int n_pages, int band
 	const char *domain = "thumbnail_plan";
 	if (ensure_init(domain))
 		return nullptr;
-	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || bands <= 0 ||
-		target_width <= 0) {
-		error(domain, "bad frame geometry");
-		return nullptr;
-	}
 	auto *plan = new VB200ThumbnailPlan();
 	ThumbnailPlanImpl &pl = plan->impl;
-	pl.W = width;
-	pl.H = page_height * n_pages;
-	pl.page_h = n_pages > 1 ? page_height : 0;
-	pl.bands = bands;
+	if (plan_request(&pl, width, page_height, n_pages, bands, has_alpha, target_width, target_height, size, linear)) {
+		error(domain, "bad frame geometry");
+		delete plan;
+		return nullptr;
+	}
 	pl.fmt = band_format;
-	pl.has_alpha = has_alpha;
-	pl.target_w = target_width;
-	pl.target_h = target_height > 0 ? target_height : target_width;
-	pl.size = size;
-	pl.linear = linear;
 	if (thumbnail_plan_init(domain, &pl)) {
 		thumbnail_plan_destroy(&pl);
 		delete plan;
@@ -2397,6 +2301,25 @@ vb200_thumbnail_batch_device_icc(VB200ThumbnailPlan *plan, const void *in, size_
 		current_stream(), embedded, embedded_lens);
 }
 
+/* the body of the ICC setters: the plan's stage, in the plan's mode, replaced by one for icc (NULL: off) */
+static int
+plan_set_icc(const char *domain, ThumbnailPlanImpl &pl, const VB200ThumbnailIcc *icc)
+{
+	IccStage *st = nullptr;
+	int ob = 0;
+	if (icc) {
+		st = icc_stage_new();
+		if (icc_stage_set(domain, st, icc, pl.bands, pl.linear, &ob)) {
+			icc_stage_free(st);
+			return -1;
+		}
+	}
+	icc_stage_free(pl.icc);
+	pl.icc = st;
+	pl.icc_bands = ob;
+	return 0;
+}
+
 extern "C" int
 vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *icc)
 {
@@ -2405,31 +2328,17 @@ vb200_thumbnail_plan_set_icc(VB200ThumbnailPlan *plan, const VB200ThumbnailIcc *
 		error(domain, "null plan");
 		return -1;
 	}
-	ThumbnailPlanImpl &pl = plan->impl;
-	if (!icc || !icc->output_profile) {
-		icc_stage_free(pl.icc);
-		pl.icc = nullptr;
-		return 0;
-	}
-	if (pl.linear) {
-		/* thumbnail.c:766-806, 957-970: an ICC import into the linear V kernel and an export from the H kernel, not built */
+	const bool off = !icc || !icc->output_profile;
+	if (plan->impl.linear) {
+		/* a linear plan's stage is vb200_thumbnail_plan_set_linear_icc's, and this setter's "off" leaves it alone.
+		 * thumbnail.c:766-806, 957-970: an ICC import into the linear V kernel and an export from the H kernel, not built here
+		 */
+		if (off)
+			return 0;
 		error(domain, "linear thumbnails with an output profile are not supported on the device path");
 		return -1;
 	}
-	if (pl.fmt != VB200_FORMAT_UCHAR) {
-		error(domain, "colour-managed thumbnails need 8-bit frames");
-		return -1;
-	}
-	IccStage *st = icc_stage_new();
-	int ob = 0;
-	if (icc_stage_set(domain, st, icc, pl.bands, &ob)) {
-		icc_stage_free(st);
-		return -1;
-	}
-	icc_stage_free(pl.icc);
-	pl.icc = st;
-	pl.icc_bands = ob;
-	return 0;
+	return plan_set_icc(domain, plan->impl, off ? nullptr : icc);
 }
 
 extern "C" int
@@ -2440,26 +2349,11 @@ vb200_thumbnail_plan_set_linear_icc(VB200ThumbnailPlan *plan, const VB200Thumbna
 		error(domain, "null plan");
 		return -1;
 	}
-	ThumbnailPlanImpl &pl = plan->impl;
-	if (!pl.linear) {
+	if (!plan->impl.linear) {
 		error(domain, "the plan is not linear: use vb200_thumbnail_plan_set_icc");
 		return -1;
 	}
-	if (!icc) {
-		icc_stage_free(pl.licc);
-		pl.licc = nullptr;
-		return 0;
-	}
-	IccStage *st = icc_stage_new();
-	int ob = 0;
-	if (icc_stage_set_linear(domain, st, icc, pl.bands, &ob)) {
-		icc_stage_free(st);
-		return -1;
-	}
-	icc_stage_free(pl.licc);
-	pl.licc = st;
-	pl.licc_bands = ob;
-	return 0;
+	return plan_set_icc(domain, plan->impl, icc);
 }
 
 extern "C" int
@@ -2479,7 +2373,7 @@ vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, 
 }
 
 static int thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size, int linear,
-	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, bool linear_icc, int *out_page_height);
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, int *out_page_height);
 
 /* linear: decoded at full size (thumbnail.c:496-499) and thumbnailed by vb200_thumbnail_image_linear_icc.  A GIF's pages
  * page .. page + n - 1 decode to a strip with nsgifload's page-height, set when more than one page loaded
@@ -2528,8 +2422,7 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 	VB200Image tmp;
 	memset(&tmp, 0, sizeof(tmp));
 	tmp.where = VB200_DEVICE;
-	int rc = thumbnail_image_run(&din, page_height, &tmp, width, height, size, linear, icc, embedded.data(), embedded.size(), linear,
-		out_page_height);
+	int rc = thumbnail_image_run(&din, page_height, &tmp, width, height, size, linear, icc, embedded.data(), embedded.size(), out_page_height);
 	if (!rc) {
 		/* deliver where the caller asked (allocate-or-fill) */
 		DevImage dt;
@@ -2592,7 +2485,7 @@ plan_run_streams(const char *domain, const DecodeRequest &req, VB200ThumbnailPla
 	/* with colour management on, each stream's embedded profile (jpeg2vips.c:699-799, spngload.c:244-246) goes to the ICC
 	 * stage; PNG streams are read for eXIf either way
 	 */
-	const bool managed = pl.icc || pl.licc;
+	const bool managed = pl.icc != nullptr;
 	std::vector<std::vector<unsigned char>> profiles(managed || req.kind == STREAM_PNG ? n : 0);
 	std::vector<const void *> emb(profiles.size());
 	std::vector<size_t> emb_len(profiles.size());
@@ -2751,20 +2644,20 @@ vb200_thumbnail_batch_host_icc(VB200ThumbnailPlan *plan, const void *in, size_t 
 	return 0;
 }
 
-/* vips_thumbnail_image, with colour management when icc sets an output profile; linear_icc: linear = TRUE with icc (may be NULL)
- * through vb200_thumbnail_plan_set_linear_icc.  page_height: the input's page-height metadata (0: none), read as
+/* vips_thumbnail_image, with colour management when icc sets an output profile, or with linear = TRUE when icc is set at all
+ * (vb200_thumbnail_plan_set_linear_icc).  page_height: the input's page-height metadata (0: none), read as
  * vips_image_get_page_height does; out_page_height (may be NULL) gets the result's.
  */
 static int
 thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size, int linear,
-	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, bool linear_icc, int *out_page_height)
+	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, int *out_page_height)
 {
 	const char *domain = "thumbnail";
 	if (!in || !out) {
 		error(domain, "null argument");
 		return -1;
 	}
-	if (linear_icc && icc && !(in->Type == VB200_INTERPRETATION_sRGB && in->Bands >= 3)) {
+	if (linear && icc && !(in->Type == VB200_INTERPRETATION_sRGB && in->Bands >= 3)) {
 		/* thumbnail.c:766-789 imports other interpretations with a profile of their space, and 1- / 2-band frames with sGrey:
 		 * not on the device path
 		 */
@@ -2772,11 +2665,11 @@ thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int 
 			in->Type, in->Bands);
 		return -1;
 	}
-	if (linear_icc && icc) {
+	if (linear && icc) {
 		/* the profiles are checked before any pixel moves: the stage's own checks, on the host, on a stage of its own */
 		IccStage *st = icc_stage_new();
 		int ob = 0;
-		const int rc = icc_stage_set_linear(domain, st, icc, in->Bands, &ob);
+		const int rc = icc_stage_set(domain, st, icc, in->Bands, true, &ob);
 		icc_stage_free(st);
 		if (rc)
 			return -1;
@@ -2805,14 +2698,14 @@ thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int 
 		return -1;
 	if (out_page_height)
 		*out_page_height = plan->impl.out_page_h;
-	if (icc && (linear_icc ? vb200_thumbnail_plan_set_linear_icc(plan, icc) : vb200_thumbnail_plan_set_icc(plan, icc))) {
+	if (icc && (linear ? vb200_thumbnail_plan_set_linear_icc(plan, icc) : vb200_thumbnail_plan_set_icc(plan, icc))) {
 		vb200_thumbnail_plan_free(plan);
 		return -1;
 	}
 	const int ob = plan->impl.out_bands();
 	/* icc_transform.c:374-433: the output interpretation follows the output profile's colour bands */
 	const int colour = ob - (in->Bands - (in->Bands < 3 ? 1 : 3));
-	const int otype = !plan->impl.icc && !plan->impl.licc ? in->Type
+	const int otype = !plan->impl.icc ? in->Type
 		: colour == 1				  ? VB200_INTERPRETATION_B_W
 		: colour == 3				  ? VB200_INTERPRETATION_sRGB
 									  : VB200_INTERPRETATION_CMYK;
@@ -2843,7 +2736,7 @@ thumbnail_image_run(const VB200Image *in, int page_height, VB200Image *out, int 
 extern "C" int
 vb200_thumbnail_image(const VB200Image *in, VB200Image *out, int width, int height, int size, int linear)
 {
-	return thumbnail_image_run(in, 0, out, width, height, size, linear, nullptr, nullptr, 0, false, nullptr);
+	return thumbnail_image_run(in, 0, out, width, height, size, linear, nullptr, nullptr, 0, nullptr);
 }
 
 /* vips_thumbnail_image with "input_profile" / "output_profile" / "intent"; `embedded`: the image's ICC blob */
@@ -2851,7 +2744,7 @@ extern "C" int
 vb200_thumbnail_image_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
 	const void *embedded, size_t embedded_len)
 {
-	return thumbnail_image_run(in, 0, out, width, height, size, 0, icc, embedded, embedded_len, false, nullptr);
+	return thumbnail_image_run(in, 0, out, width, height, size, 0, icc, embedded, embedded_len, nullptr);
 }
 
 /* See vb200.h: vips_thumbnail_image of a page strip (thumbnail.c:825-839, 904-917) */
@@ -2859,8 +2752,7 @@ extern "C" int
 vb200_thumbnail_image_pages(const VB200Image *in, int page_height, VB200Image *out, int width, int height, int size,
 	const VB200ThumbnailIcc *icc, const void *embedded, size_t embedded_len, int linear, int *out_page_height)
 {
-	return thumbnail_image_run(in, page_height, out, width, height, size, linear != 0, icc, embedded, embedded_len, linear != 0,
-		out_page_height);
+	return thumbnail_image_run(in, page_height, out, width, height, size, linear != 0, icc, embedded, embedded_len, out_page_height);
 }
 
 /* vips_thumbnail_image(..., linear = TRUE) with "input_profile" / "output_profile" / "intent" (thumbnail.c:766-805, 929-987):
@@ -2870,7 +2762,7 @@ extern "C" int
 vb200_thumbnail_image_linear_icc(const VB200Image *in, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
 	const void *embedded, size_t embedded_len)
 {
-	return thumbnail_image_run(in, 0, out, width, height, size, 1, icc, embedded, embedded_len, true, nullptr);
+	return thumbnail_image_run(in, 0, out, width, height, size, 1, icc, embedded, embedded_len, nullptr);
 }
 
 /* Test hook (tests/test_thumbnail_bands.py, CPU): the tensor-pipe kernel's bands of an RGBA thumbnail plan, planned
@@ -2880,16 +2772,9 @@ extern "C" int
 vb200_debug_thumbnail_bands(int width, int height, int target_width, int *out_width, int *n_bands, int *xa, int *xb,
 	int *c_lo, int *c_hi, int *seam, int cap, int *box_width, int *n_box)
 {
-	if (width <= 0 || height <= 0 || target_width <= 0 || cap <= 0)
-		return -1;
 	ThumbnailPlanImpl pl;
-	pl.W = width;
-	pl.H = height;
-	pl.bands = 4;
-	pl.fmt = VB200_FORMAT_UCHAR;
-	pl.has_alpha = 1;
-	pl.target_w = pl.target_h = target_width;
-	pl.size = VB200_SIZE_BOTH;
+	if (cap <= 0 || plan_request(&pl, width, height, 1, 4, 1, target_width, target_width, VB200_SIZE_BOTH, 0))
+		return -1;
 	pl.geometry_only = true;
 	if (thumbnail_plan_init("debug_thumbnail_bands", &pl))
 		return -1;
@@ -2930,19 +2815,9 @@ extern "C" int
 vb200_debug_thumbnail_pages_kernel(int width, int page_height, int n_pages, int bands, int has_alpha, int target_width,
 	int target_height, int size, char *name, int cap)
 {
-	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || bands <= 0 ||
-		target_width <= 0 || !name || cap <= 0)
-		return -1;
 	ThumbnailPlanImpl pl;
-	pl.W = width;
-	pl.H = page_height * n_pages;
-	pl.page_h = n_pages > 1 ? page_height : 0;
-	pl.bands = bands;
-	pl.fmt = VB200_FORMAT_UCHAR;
-	pl.has_alpha = has_alpha;
-	pl.target_w = target_width;
-	pl.target_h = target_height > 0 ? target_height : target_width;
-	pl.size = size;
+	if (!name || cap <= 0 || plan_request(&pl, width, page_height, n_pages, bands, has_alpha, target_width, target_height, size, 0))
+		return -1;
 	pl.geometry_only = true;
 	if (thumbnail_plan_init("debug_thumbnail_kernel", &pl))
 		return -1;
@@ -2961,17 +2836,9 @@ extern "C" int
 vb200_debug_thumbnail_pages_size(int width, int page_height, int n_pages, int target_width, int target_height, int size, double *hshrink,
 	double *vshrink, int *out_width, int *out_height, int *out_page_height)
 {
-	if (width <= 0 || page_height <= 0 || n_pages <= 0 || (long long) page_height * n_pages > INT_MAX || target_width <= 0)
-		return -1;
 	ThumbnailPlanImpl pl;
-	pl.W = width;
-	pl.H = page_height * n_pages;
-	pl.page_h = n_pages > 1 ? page_height : 0;
-	pl.bands = 1;
-	pl.fmt = VB200_FORMAT_UCHAR;
-	pl.target_w = target_width;
-	pl.target_h = target_height > 0 ? target_height : target_width;
-	pl.size = size;
+	if (plan_request(&pl, width, page_height, n_pages, 1, 0, target_width, target_height, size, 0))
+		return -1;
 	pl.geometry_only = true;
 	if (thumbnail_plan_init("debug_thumbnail_pages_size", &pl))
 		return -1;

@@ -63,10 +63,10 @@ struct LinVParams {
 	/* the residual-2.0 schedule (linear_v2_kernel): first[y] = f0 + 2 y, one phase, 13 taps */
 	int f0;
 	double c2[13];
-	/* colour-managed instantiations: each frame's LinIccFrame (this launch's first frame at [0]) and the batch's job table; the
+	/* colour-managed instantiations: each frame's IccFrame (this launch's first frame at [0]) and the batch's job table; the
 	 * import job and its TRC tables are staged at byte icc_off of the dynamic shared memory
 	 */
-	const LinIccFrame *iframes;
+	const IccFrame *iframes;
 	const IccJob *ijobs;
 	int icc_off;
 };
@@ -85,14 +85,14 @@ struct LinHParams {
 	/* colour-managed instantiations: as LinVParams; the export job at byte icc_off of the dynamic shared memory, out_bands
 	 * bands per output pixel, and the alpha steps of vips_colourspace(scRGB -> XYZ) for LIN_XYZ frames
 	 */
-	const LinIccFrame *iframes;
+	const IccFrame *iframes;
 	const IccJob *ijobs;
 	int icc_off, out_bands;
 	StepInfo xyz[2];
 	int n_xyz;
 };
 
-/* ---- the colour-managed frames (LinIccFrame): import in kernel V, export in kernel H, the evaluator's own code (icc_eval.cuh) */
+/* ---- the colour-managed frames (IccFrame): import in kernel V, export in kernel H, the evaluator's own code (icc_eval.cuh) */
 
 /* kernel V's per-CTA setup of an LIN_IMPORT frame: the import job, and its tabulated TRCs (matrix / TRC profiles), into shared
  * memory.  Uniform across the CTA (one frame per CTA).
@@ -100,7 +100,7 @@ struct LinHParams {
 __device__ __forceinline__ const IccJob *
 stage_import(const LinVParams &P, int frame, unsigned char *smem_raw, const float **tab)
 {
-	const LinIccFrame fr = P.iframes[frame];
+	const IccFrame fr = P.iframes[frame];
 	if (fr.kind != LIN_IMPORT)
 		return nullptr;
 	IccJob *sj = (IccJob *) (smem_raw + P.icc_off);
@@ -519,7 +519,7 @@ linear_h_kernel(const __grid_constant__ LinHParams P, uint8_t *__restrict__ out,
 	int kind = LIN_PLAIN;
 	IccJob *J = ICC ? (IccJob *) (smem_raw + P.icc_off) : nullptr;
 	if (ICC) {
-		const LinIccFrame fr = P.iframes[frame];
+		const IccFrame fr = P.iframes[frame];
 		kind = fr.kind;
 		if (kind != LIN_PLAIN) {
 			const unsigned *src = (const unsigned *) (P.ijobs + fr.exp);
@@ -857,7 +857,7 @@ thread_local LinearTiming g_linear_timing;
  */
 int
 linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_stride, void *out, size_t out_stride, int n,
-	cudaStream_t s, const LinIccBatch *icc, int out_bands)
+	cudaStream_t s, const IccBatch *icc, int out_bands)
 {
 	if (n <= 0)
 		return 0;

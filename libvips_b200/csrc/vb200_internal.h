@@ -330,44 +330,50 @@ parallel_for(int n, int threads, Fn fn)
 		t.join();
 }
 
-/* icc.cu: the colour-management stage of the thumbnail plan (vb200_thumbnail_plan_set_icc).  Frames are 8-bit, `bands`
- * bands in, *out_bands out; each frame's input profile is chosen as vips_icc_set_import does, and one launch runs a batch.
+/* icc.cu: the colour-management stage of the thumbnail plan (vb200_thumbnail_plan_set_icc / _set_linear_icc).  Frames are
+ * 8-bit, `bands` bands in, *out_bands out; each frame's input profile is chosen as vips_icc_set_import does.  The stage has
+ * two modes, fixed by icc_stage_set:
+ *   - after the thumbnail kernel (linear = false): one job per frame, the transform from its input profile or the XYZ export,
+ *     run over a batch by icc_stage_run in one launch per kMaxBatchFrames frames;
+ *   - linear (thumbnail.c:766-805, 929-987): the import runs inside the linear thumbnail's V kernel and the export inside its
+ *     H kernel (thumbnail_linear.cu), or in the leaf chain around the float resize.  Each frame takes one of:
+ *       LIN_PLAIN   sRGB -> scRGB ... scRGB -> sRGB, the linear thumbnail without a profile anywhere;
+ *       LIN_IMPORT  vips_icc_import(XYZ PCS) ... vips_icc_export from XYZ (thumbnail.c:766-789, 929-942: a profile to import with);
+ *       LIN_XYZ     sRGB -> scRGB ... scRGB -> XYZ, vips_icc_export from XYZ (:790-805, 957-970: only an output profile).
  */
 struct IccStage;
 IccStage *icc_stage_new();
 void icc_stage_free(IccStage *st);
-int icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands);
-int icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
-	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s, int frame0 = 0);
+/* the stage's profiles (copied) and mode; refuses 1- and 2-band frames in linear mode, and needs an output profile outside it */
+int icc_stage_set(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, bool linear, int *out_bands);
 int icc_debug_select(const VB200ThumbnailIcc *icc, int bands, const void *embedded, size_t embedded_len, int *source);
 int icc_debug_classify(const void *profile, size_t len, int want_bands, int intent);
 
-/* The linear mode of the stage (vb200_thumbnail_plan_set_linear_icc): the import runs inside the linear thumbnail's V kernel and
- * the export inside its H kernel (thumbnail_linear.cu), or in the leaf chain around the float resize.  Each frame takes one of:
- *   LIN_PLAIN   sRGB -> scRGB ... scRGB -> sRGB, today's linear thumbnail (no profile anywhere);
- *   LIN_IMPORT  vips_icc_import(XYZ PCS) ... vips_icc_export from XYZ (thumbnail.c:766-789, 929-942: a profile to import with);
- *   LIN_XYZ     sRGB -> scRGB ... scRGB -> XYZ, vips_icc_export from XYZ (:790-805, 957-970: only an output profile).
- * imp / exp index the batch's job table.
- */
 enum { LIN_PLAIN = 0, LIN_IMPORT = 1, LIN_XYZ = 2 };
-struct LinIccFrame {
+/* one frame's jobs, indices into the batch's job table: a linear frame's LIN_* kind and its import and export jobs (-1: none);
+ * a frame of the other mode has its one job in exp
+ */
+struct IccFrame {
 	int kind, imp, exp;
 };
 struct IccJob; /* icc_eval.cuh */
 /* one batch's resolved jobs: device copies for the kernels, host copies (device pool pointers) for the leaf chain */
-struct LinIccBatch {
+struct IccBatch {
 	const IccJob *d_jobs;
-	const LinIccFrame *d_frames;
+	const IccFrame *d_frames;
 	const IccJob *h_jobs;
-	const LinIccFrame *h_frames;
+	const IccFrame *h_frames;
 };
-int icc_stage_set_linear(const char *domain, IccStage *st, const VB200ThumbnailIcc *icc, int bands, int *out_bands);
-/* resolves the n frames' jobs (embedded / embedded_lens as icc_stage_run), uploads them on s and calls body with them, the
- * stage locked and its cache entries held until the launches body queues have been recorded.  frame0: the index of the first
- * frame in the caller's batch, for the errors that name a frame (the host pump runs a batch in slices)
+/* resolves the n frames' jobs in the stage's mode (embedded / embedded_lens: each frame's embedded profile, NULL arrays or a NULL
+ * entry: none), uploads them on s and calls body with them, the stage locked and its cache entries held until the launches body
+ * queues have been recorded.  frame0: the index of the first frame in the caller's batch, for the errors that name a frame (the
+ * host pump runs a batch in slices)
  */
-int icc_stage_run_linear(const char *domain, IccStage *st, int n, const void *const *embedded, const size_t *embedded_lens,
-	cudaStream_t s, int frame0, const std::function<int(const LinIccBatch &)> &body);
+int icc_stage_batch(const char *domain, IccStage *st, int n, const void *const *embedded, const size_t *embedded_lens,
+	cudaStream_t s, int frame0, const std::function<int(const IccBatch &)> &body);
+/* the stage after the thumbnail kernel: icc_stage_batch with icc_frames_kernel over n frames of `pixels` pixels */
+int icc_stage_run(const char *domain, IccStage *st, const void *in, size_t in_stride, void *out, size_t out_stride, int n, size_t pixels,
+	const void *const *embedded, const size_t *embedded_lens, cudaStream_t s, int frame0);
 /* the leaf chain's ICC steps: jobs[k] over a packed device image (icc_kernel, as vb200_icc_import / _export launch it) */
 int icc_job_apply(const char *domain, const IccJob *jobs, int k, const DevImage &in, DevImage *out, cudaStream_t s);
 /* test hook: one frame's linear-mode choice (*branch LIN_*, *source as icc_debug_select or -1, *export_from 0 output_profile,
