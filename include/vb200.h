@@ -157,6 +157,17 @@ size_t vb200_format_sizeof(int band_format);
  * allocates it in the same memory space (free with vb200_image_free); otherwise
  * out->data/out->bpl are used as given and must be large enough.  The rest of
  * *out is filled in.
+ *
+ * Strides and alignment (every whole-image op below, colour, convolution, ICC,
+ * flatten and morphology too): bpl = 0 means packed rows; a non-zero bpl smaller
+ * than Xsize * Bands * vb200_format_sizeof(BandFmt) is an error.  A VB200_DEVICE
+ * image is read in place, so its data and bpl must both be multiples of the
+ * element size (any byte for uchar / char, 2 for ushort / short, 4 for uint / int
+ * / float); otherwise the call fails before any launch.  Padded strides and bases
+ * off a 4- or 16-byte grid are accepted and give the same pixels: the vector
+ * kernels are used only where the layout allows them.  A caller's output buffer
+ * may have any base and stride at least a line long; one off the result's element
+ * grid is filled by a copy rather than written by the kernel.
  */
 
 /* reference: vips_shrinkv()/vips_shrinkh(), resample/shrinkv.c:474, shrinkh.c:357 */

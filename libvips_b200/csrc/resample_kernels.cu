@@ -644,11 +644,12 @@ reduceh_kernel<float>(const float *__restrict__ in, size_t in_bpl, int in_w, flo
  *   pre:   scale[i] = (int) (256 * clip(i) / max_alpha)          premultiply.c:253-259
  *   unpre: scale[i] = clip == 0 ? 0 : (int) (256 * max_alpha / clip)  unpremultiply.c:313-324
  * out = (in * scale[alpha] + 128) >> 8 stored as a byte (no clip).
+ * words: 4-band pixels as one 32-bit load and store; only when both images' bases and strides are multiples of 4.
  */
 template <bool UNPRE>
 __global__ void __launch_bounds__(256)
 premul_u8_kernel(const uint8_t *__restrict__ in, size_t in_bpl, uint8_t *__restrict__ out, size_t out_bpl, int w,
-	int h, int bands, double max_alpha)
+	int h, int bands, double max_alpha, bool words)
 {
 	__shared__ int scale[256];
 	{
@@ -666,7 +667,7 @@ premul_u8_kernel(const uint8_t *__restrict__ in, size_t in_bpl, uint8_t *__restr
 	for (int y = blockIdx.y; y < h; y += gridDim.y) {
 		const uint8_t *p = in + (size_t) y * in_bpl + (size_t) x * bands;
 		uint8_t *q = out + (size_t) y * out_bpl + (size_t) x * bands;
-		if (bands == 4) {
+		if (words) {
 			const unsigned int v = *(const unsigned int *) p;
 			const int s = scale[v >> 24];
 			const unsigned int r = (((v & 0xff) * s + 128) >> 8) & 0xff;
@@ -735,6 +736,13 @@ bool
 aligned4(const void *p, size_t bpl)
 {
 	return (((uintptr_t) p) & 3) == 0 && (bpl & 3) == 0;
+}
+
+/* premul_u8_kernel's 32-bit word path: 4 bands, both images on the word grid */
+bool
+premul_words(const DevImage &in, const DevImage &out)
+{
+	return in.bands == 4 && aligned4(in.data, in.bpl) && aligned4(out.data, out.bpl);
 }
 
 /* An AxisTable packed into one block: the AxisDev points into it (host image `host`, `total` bytes). */
@@ -1203,7 +1211,7 @@ dev_premultiply(const char *domain, const DevImage &in, DevImage *out, double ma
 #define PM(T) premul_float_kernel<T><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.h, in.bands, max_alpha)
 	if (lut)
 		premul_u8_kernel<false><<<grid, 256, 0, s>>>((const uint8_t *) in.data, in.bpl, (uint8_t *) out->data,
-			out->bpl, in.w, in.h, in.bands, max_alpha);
+			out->bpl, in.w, in.h, in.bands, max_alpha, premul_words(in, *out));
 	else
 		switch (in.fmt) {
 		case VB200_FORMAT_UCHAR: PM(uint8_t); break;
@@ -1240,7 +1248,7 @@ dev_unpremultiply(const char *domain, const DevImage &in, DevImage *out, double 
 #define UPM(T, FP) unpremul_float_kernel<T, FP><<<grid, 256, 0, s>>>((const T *) in.data, in.bpl, (float *) out->data, out->bpl, in.w, in.h, in.bands, max_alpha)
 	if (lut)
 		premul_u8_kernel<true><<<grid, 256, 0, s>>>((const uint8_t *) in.data, in.bpl, (uint8_t *) out->data,
-			out->bpl, in.w, in.h, in.bands, max_alpha);
+			out->bpl, in.w, in.h, in.bands, max_alpha, premul_words(in, *out));
 	else
 		switch (in.fmt) {
 		case VB200_FORMAT_UCHAR: UPM(uint8_t, false); break;

@@ -217,7 +217,8 @@ dev_image_new(const char *domain, DevImage *d, int w, int h, int bands, int fmt,
 	d->fmt = fmt;
 	d->type = type;
 	const size_t line = (size_t) w * bands * format_sizeof(fmt);
-	if (d->preset && d->data) {
+	const size_t es = format_sizeof(fmt);
+	if (d->preset && d->data && (uintptr_t) d->data % es == 0 && d->bpl % es == 0) {
 		/* the caller's buffer (preset_output): sized by contract for this op's result */
 		d->preset = false;
 		d->owned = false;
@@ -225,6 +226,8 @@ dev_image_new(const char *domain, DevImage *d, int w, int h, int bands, int fmt,
 			d->bpl = line;
 		return 0;
 	}
+	/* a caller's buffer off the element grid of this result is not written by the kernel: deliver() copies into it */
+	d->preset = false;
 	d->bpl = line;
 	d->owned = true;
 	return dev_alloc(domain, &d->data, d->bpl * h, s);
@@ -274,6 +277,17 @@ to_device(const char *domain, const VB200Image *in, DevImage *d, cudaStream_t s)
 		return -1;
 	}
 	const size_t bpl = in->bpl ? in->bpl : line;
+	/* checked before any copy or launch: a shorter stride makes rows overlap and the last row run past the buffer */
+	if (bpl < line) {
+		error(domain, "line stride %zu too small for %d x %d x %zu bytes", bpl, in->Xsize, in->Bands, format_sizeof(in->BandFmt));
+		return -1;
+	}
+	/* kernels read rows as arrays of the element type: a device base or stride off that grid is a misaligned load */
+	const size_t es = format_sizeof(in->BandFmt);
+	if (in->where == VB200_DEVICE && (((uintptr_t) in->data % es) != 0 || bpl % es != 0)) {
+		error(domain, "device image data %p / line stride %zu not a multiple of the %zu-byte element", in->data, bpl, es);
+		return -1;
+	}
 
 	d->w = in->Xsize;
 	d->h = in->Ysize;
