@@ -341,8 +341,9 @@ linear_v_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict_
  * (the oldest completes with tap 12 and is stored), six receive an odd tap from row B.  The seven
  * accumulators rotate through registers by unrolling seven iterations; coefficients are kernel-parameter
  * constants.  Same sums in the same order as the general kernel -- 42 instead of 93 instructions per pixel.
+ * Only RGBA frames take it, and linear_thumb_new sends a 4-band plan here only when it premultiplies.
  */
-template <bool PREMUL, int VST, bool ICC = false>
+template <int VST, bool ICC = false>
 __global__ void __launch_bounds__(kVThreads, 2)
 linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict__ in, int frame0)
 {
@@ -451,12 +452,7 @@ linear_v2_kernel(const __grid_constant__ LinVParams P, const uint8_t *__restrict
 							b = s_lin[(px >> 16) & 255];
 						}
 						const float2 an = s_aln[px >> 24];
-						float q0 = r, q1 = g, q2 = b;
-						if (PREMUL) {
-							q0 = __fmul_rn(r, an.x);
-							q1 = __fmul_rn(g, an.x);
-							q2 = __fmul_rn(b, an.x);
-						}
+						const float q0 = __fmul_rn(r, an.x), q1 = __fmul_rn(g, an.x), q2 = __fmul_rn(b, an.x);
 						sum[0] = __dadd_rn(sum[0], (double) q0);
 						sum[1] = __dadd_rn(sum[1], (double) q1);
 						sum[2] = __dadd_rn(sum[2], (double) q2);
@@ -625,7 +621,6 @@ linear_h_kernel(const __grid_constant__ LinHParams P, uint8_t *__restrict__ out,
 
 struct LinearThumb {
 	int W = 0, H = 0, OW = 0, OH = 0, bands = 0;
-	bool premul = false;
 	LinVParams v{};
 	LinHParams h{};
 	void *tables = nullptr;
@@ -682,7 +677,6 @@ linear_thumb_new(const char *domain, int W, int H, int bands, bool premul, const
 	lt->OW = OW;
 	lt->OH = OH;
 	lt->bands = bands;
-	lt->premul = premul;
 	lt->smem_v = smem_v;
 	lt->smem_h = smem_h;
 	lt->smem_v_icc = ((smem_v + 15) & ~(size_t) 15) + sizeof(IccJob) + 3 * 256 * 4;
@@ -796,42 +790,16 @@ launch_v(const char *domain, const LinearThumb *lt, const LinVParams &v, const v
 	return 0;
 }
 
+template <bool ICC = false>
 int
 launch_v2(const char *domain, const LinearThumb *lt, const LinVParams &v, const void *in, dim3 grid, cudaStream_t s)
 {
-#define LV2(PM_, VST_) \
-	do { \
-		auto kern = linear_v2_kernel<PM_, VST_>; \
-		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_v)); \
-		kern<<<grid, kVThreads, lt->smem_v, s>>>(v, (const uint8_t *) in, 0); \
-	} while (0)
-	if (lt->premul) {
-		switch (lt->vst) {
-		case 2: LV2(true, 2); break;
-		case 4: LV2(true, 4); break;
-		default: LV2(true, 8); break;
-		}
-	}
-	else {
-		switch (lt->vst) {
-		case 2: LV2(false, 2); break;
-		case 4: LV2(false, 4); break;
-		default: LV2(false, 8); break;
-		}
-	}
-#undef LV2
-	return 0;
-}
-
-/* the colour-managed linear_v2_kernel: a 4-band plan on the two-kernel path premultiplies */
-int
-launch_v2_icc(const char *domain, const LinearThumb *lt, const LinVParams &v, const void *in, dim3 grid, cudaStream_t s)
-{
+	const size_t smem = ICC ? lt->smem_v_icc : lt->smem_v;
 #define LV2(VST_) \
 	do { \
-		auto kern = linear_v2_kernel<true, VST_, true>; \
-		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_v_icc)); \
-		kern<<<grid, kVThreads, lt->smem_v_icc, s>>>(v, (const uint8_t *) in, 0); \
+		auto kern = linear_v2_kernel<VST_, ICC>; \
+		VB200_CUDA(domain, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); \
+		kern<<<grid, kVThreads, smem, s>>>(v, (const uint8_t *) in, 0); \
 	} while (0)
 	switch (lt->vst) {
 	case 2: LV2(2); break;
@@ -909,16 +877,15 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 		v.RPC = (lt->OH + splits - 1) / splits;
 		const dim3 gv(col_blocks, (lt->OH + v.RPC - 1) / v.RPC, nf);
 		const char *fin = (const char *) in + (size_t) f0 * in_stride;
+		/* a 4-band plan on this path premultiplies (linear_thumb_new), a 3-band one has no alpha */
 		if (icc)
-			rc = lt->static2 ? launch_v2_icc(domain, lt, v, fin, gv, s)
+			rc = lt->static2 ? launch_v2<true>(domain, lt, v, fin, gv, s)
 				: lt->bands == 4 ? launch_v<4, true, true>(domain, lt, v, fin, gv, 0, s)
 								 : launch_v<3, false, true>(domain, lt, v, fin, gv, 0, s);
-		else if (lt->static2)
-			rc = launch_v2(domain, lt, v, fin, gv, s);
-		else if (lt->bands == 4)
-			rc = lt->premul ? launch_v<4, true>(domain, lt, v, fin, gv, 0, s) : launch_v<4, false>(domain, lt, v, fin, gv, 0, s);
 		else
-			rc = launch_v<3, false>(domain, lt, v, fin, gv, 0, s);
+			rc = lt->static2 ? launch_v2(domain, lt, v, fin, gv, s)
+				: lt->bands == 4 ? launch_v<4, true>(domain, lt, v, fin, gv, 0, s)
+								 : launch_v<3, false>(domain, lt, v, fin, gv, 0, s);
 		cudaError_t e = cudaGetLastError();
 		if (!rc && e != cudaSuccess)
 			rc = cuda_fail(domain, e, "linear_v_kernel launch");
@@ -941,13 +908,8 @@ linear_thumb_run(const char *domain, LinearThumb *lt, const void *in, size_t in_
 			cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_h_icc);
 			kern<<<gh, 256, lt->smem_h_icc, s>>>(h, fout, 0);
 		}
-		else if (lt->bands == 4) {
-			auto kern = lt->premul ? linear_h_kernel<4, true> : linear_h_kernel<4, false>;
-			cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_h);
-			kern<<<gh, 256, lt->smem_h, s>>>(h, fout, 0);
-		}
 		else {
-			auto kern = linear_h_kernel<3, false>;
+			auto kern = lt->bands == 4 ? linear_h_kernel<4, true> : linear_h_kernel<3, false>;
 			cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lt->smem_h);
 			kern<<<gh, 256, lt->smem_h, s>>>(h, fout, 0);
 		}
