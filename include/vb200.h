@@ -656,6 +656,52 @@ int vb200_thumbnail_plan_run_gif(VB200ThumbnailPlan *plan, const void *const *bu
 int vb200_debug_gif_decode(const void *buf, size_t len, int page, int n, void *out, size_t out_bpl, int *width, int *height,
 	int *bands);
 int vb200_debug_lzw(const void *data, size_t len, int min_code_size, unsigned want, int lenient, void *out, size_t *out_len);
+/* ------------------------------------------------------------------ TIFF decode on the device
+ * vips_tiffload_buffer(buf, len, &out, "page", page, "n", n, "subifd", subifd, NULL) (foreign/tiff2vips.c over libtiff) with
+ * the strips or tiles decoded and placed on the device (csrc/tiff.cu).  Classic and BigTIFF, either byte order,
+ * PlanarConfiguration 1, FillOrder 1, 8-bit unsigned samples: MINISBLACK / MINISWHITE with 1-2 samples load as B_W (the
+ * first band of MINISWHITE inverted, rtiff_greyscale_line, tiff2vips.c:1359-1448), RGB with 3-4 as sRGB
+ * (rtiff_parse_copy, :1723-1780); ExtraSamples 0 or 2, the extra band copied.  Compression none, PackBits, LZW and deflate
+ * (8 and 32946), predictor 1 or 2; JPEG tiles, greyscale or YCbCr (to sRGB by libjpeg's YCbCr path), with or without
+ * JPEGTables (rtiff_decompress_jpeg_run, :2082-2177).  Pages page .. page + n - 1 (n = -1: to the last) stack as a strip whose pages must agree
+ * (rtiff_header_equal, :3364); subifd >= 0 loads that SubIFD of each page (rtiff_set_page, :798-846).
+ * Declined from the IFD before any device work (-1 with the reason; the host keeps tiff2vips): other depths and sample
+ * formats, PlanarConfiguration 2, FillOrder 2, palette / CIELAB / separated / LogLuv, YCbCr without JPEG, JPEG strips and
+ * RGB-photometric JPEG, associated alpha, old-style JPEG and LZW, other compressions, predictor 3, segments outside the
+ * stream, pages that differ, frames over 2^28 pixels, JPEG tiles the JPEG decoder declines ("tile k: ...").  A segment that
+ * decodes short (libtiff's "Not enough data") or corrupt, or a deflate segment whose Adler-32 trailer zlib reads and
+ * refuses, fails the batch.
+ *
+ * vb200_tiff_geometry: width, height and bands of the IFD page / subifd select, the stream's page count and the SubIFD
+ *   count of that page's main IFD; host only.
+ * vb200_tiff_decode_batch: n streams of ONE geometry -> out[n][h * pages][w][bands]; as vb200_gif_decode_batch, a stream
+ *   that fails fails the batch with "frame i:", and out = NULL only reports the geometry without a device.
+ * vb200_tiffload_buffer: one stream into a VB200Image (allocate-or-fill).
+ * vb200_tiff_icc_profile: the ICCProfile tag (34675) of the IFD page / subifd select (*profile_len = 0: none).
+ * vb200_thumbnail_plan_run_tiff: the streams' pages at subifd + the plan's thumbnail chain, frames never leave the device.
+ * vb200_thumbnail_tiff_level: host only -- the subifd (-1: none) and page vips_thumbnail_buffer loads for a thumbnail of
+ *   width / height / size: vips_thumbnail_get_tiff_pyramid_subifd (thumbnail.c:324-383) first, then
+ *   vips_thumbnail_get_pyramid_page (:262-322), and vips_thumbnail_find_pyrlevel (:519-541) over the levels found.
+ *   vb200_thumbnail_buffer (and _icc / _linear_icc) load that level; vb200_thumbnail_buffer_pages declines TIFF.
+ *   A TIFF IFD whose Orientation is not 1 is declined for thumbnails (it would need vips_autorot).
+ * vb200_debug_thumbnail_pyramid_level: test hook, host only -- the same level choice over given level geometries.
+ * vb200_debug_tiff_decode / vb200_debug_tiff_lzw: test hooks, host only -- the same per-code and per-byte code on the CPU;
+ *   vb200_debug_tiff_lzw decodes one LZW segment into exactly `want` bytes.
+ * Chunks are bounded by vb200_debug_png_set_budget, the PNG codecs' device budget.
+ */
+int vb200_tiff_geometry(const void *buf, size_t len, int page, int subifd, int *width, int *height, int *bands, int *pages, int *subifds);
+int vb200_tiff_decode_batch(const void *const *bufs, const size_t *lens, int n, int page, int n_pages, int subifd, void *out, int out_location,
+	size_t out_bpl, size_t out_frame_stride, int *width, int *height, int *bands);
+int vb200_tiffload_buffer(const void *buf, size_t len, int page, int n, int subifd, VB200Image *out);
+int vb200_tiff_icc_profile(const void *buf, size_t len, int page, int subifd, void *out, size_t cap, size_t *profile_len);
+int vb200_thumbnail_plan_run_tiff(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int page, int n_pages,
+	int subifd, void *out, int out_location, size_t out_frame_stride);
+int vb200_thumbnail_tiff_level(const void *buf, size_t len, int width, int height, int size, int *subifd, int *page);
+int vb200_debug_thumbnail_pyramid_level(int in_w, int in_h, int n_pages, const int *page_w, const int *page_h, int n_subifds,
+	const int *sub_w, const int *sub_h, int width, int height, int size, int *subifd, int *page);
+int vb200_debug_tiff_decode(const void *buf, size_t len, int page, int n, int subifd, void *out, size_t out_bpl, int *width, int *height,
+	int *bands);
+int vb200_debug_tiff_lzw(const void *data, size_t len, size_t want, void *out, size_t *out_len);
 /* ------------------------------------------------------------------ thumbnail: page strips (animated thumbnails)
  * vips_thumbnail of a multi-page image held as a strip: pages of page_height rows stacked vertically, with libvips'
  * "page-height" metadata (a GIF loaded with n = -1, a multi-page TIFF, an animated WebP).  As vips_thumbnail_build does

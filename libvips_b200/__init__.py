@@ -301,6 +301,18 @@ def lib():
                                                    C.c_size_t]
         L.vb200_debug_gif_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_lzw.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.POINTER(C.c_size_t)]
+        L.vb200_tiff_geometry.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, PI, PI, PI, PI, PI]
+        L.vb200_tiff_decode_batch.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                              C.c_int, C.c_size_t, C.c_size_t, PI, PI, PI]
+        L.vb200_tiffload_buffer.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, IP]
+        L.vb200_tiff_icc_profile.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_thumbnail_plan_run_tiff.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int,
+                                                    C.c_int, C.c_void_p, C.c_int, C.c_size_t]
+        L.vb200_thumbnail_tiff_level.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, PI, PI]
+        L.vb200_debug_thumbnail_pyramid_level.argtypes = [C.c_int, C.c_int, C.c_int, PI, PI, C.c_int, PI, PI, C.c_int, C.c_int, C.c_int,
+                                                          PI, PI]
+        L.vb200_debug_tiff_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_debug_tiff_lzw.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]
         L.vb200_thumbnail_plan_new_pages.restype = C.c_void_p
         L.vb200_thumbnail_plan_new_pages.argtypes = [C.c_int] * 10
         L.vb200_thumbnail_plan_page_height.argtypes = [C.c_void_p]
@@ -568,6 +580,20 @@ class Image:
         finally:
             C.CDLL(None).free(p)
 
+    @staticmethod
+    def tiffload_buffer(stream, page=0, n=1, subifd=-1):
+        """vips_tiffload_buffer(stream, page=page, n=n, subifd=subifd): the strips or tiles decoded on the device -> Image (uint8,
+        B_W below 3 bands, sRGB from 3), with page_height set when more than one page loaded"""
+        stream = bytes(stream)
+        out = CImage()
+        out.where = HOST
+        _check(lib().vb200_tiffload_buffer(stream, len(stream), int(page), int(n), int(subifd), C.byref(out)))
+        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
+        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
+        lib().vb200_image_free(C.byref(out))
+        page_h = tiff_geometry(stream, page, subifd)[1]
+        return Image(a, "b-w" if a.shape[2] < 3 else "srgb", page_height=page_h if a.shape[0] > page_h else None)
+
     # ---- colour
     @staticmethod
     def gifload_buffer(stream, page=0, n=1):
@@ -710,6 +736,76 @@ def gif_decode_host_twin(stream, page=0, n=1):
     _check(lib().vb200_debug_gif_decode(stream, len(stream), int(page), int(n), out.ctypes.data_as(C.c_void_p), w.value * bands.value,
                                         C.byref(w), C.byref(h), C.byref(bands)))
     return out
+
+
+def tiff_geometry(stream, page=0, subifd=-1):
+    """(width, height, bands, pages, subifds) of the TIFF IFD page / subifd select: the stream's page count and the SubIFD count
+    of that page's main IFD; no GPU needed"""
+    stream = bytes(stream)
+    v = [C.c_int() for _ in range(5)]
+    _check(lib().vb200_tiff_geometry(stream, len(stream), int(page), int(subifd), *[C.byref(x) for x in v]))
+    return tuple(x.value for x in v)
+
+
+def tiff_decode_batch(streams, page=0, n=1, subifd=-1, out_ptr=None, out_bpl=None, out_frame_stride=None):
+    """vips_tiffload_buffer(page=page, n=n, subifd=subifd) of every stream on the device -> uint8 [streams, h * pages, w, bands]
+    (host), or into the device pointer out_ptr (packed unless out_bpl / out_frame_stride say otherwise)"""
+    return _decode_batch(lib().vb200_tiff_decode_batch, streams, (int(page), int(n), int(subifd)), out_ptr, out_bpl, out_frame_stride)
+
+
+def tiff_decode_host_twin(stream, page=0, n=1, subifd=-1):
+    """the decoder's per-code / per-byte code compiled for the host (vb200_debug_tiff_decode) -> uint8 [h * pages, w, bands]"""
+    stream = bytes(stream)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_debug_tiff_decode(stream, len(stream), int(page), int(n), int(subifd), None, 0, C.byref(w), C.byref(h),
+                                         C.byref(bands)))
+    out = np.empty((h.value, w.value, bands.value), np.uint8)
+    _check(lib().vb200_debug_tiff_decode(stream, len(stream), int(page), int(n), int(subifd), out.ctypes.data_as(C.c_void_p),
+                                         w.value * bands.value, C.byref(w), C.byref(h), C.byref(bands)))
+    return out
+
+
+def tiff_icc_profile(stream, page=0, subifd=-1):
+    """the ICCProfile tag of the TIFF IFD page / subifd select (bytes, or None)"""
+    stream = bytes(stream)
+    n = C.c_size_t()
+    _check(lib().vb200_tiff_icc_profile(stream, len(stream), int(page), int(subifd), None, 0, C.byref(n)))
+    if n.value == 0:
+        return None
+    buf = C.create_string_buffer(n.value)
+    _check(lib().vb200_tiff_icc_profile(stream, len(stream), int(page), int(subifd), buf, n.value, C.byref(n)))
+    return buf.raw[:n.value]
+
+
+def tiff_lzw_host_twin(data, want):
+    """one TIFF LZW segment (libtiff's new-style codes) through the decoder's LZW on the host -> exactly `want` bytes; vb.Error
+    when libtiff would refuse it or it holds fewer"""
+    data = bytes(data)
+    out = C.create_string_buffer(max(1, int(want)))
+    n = C.c_size_t()
+    _check(lib().vb200_debug_tiff_lzw(data, len(data), int(want), out, C.byref(n)))
+    return out.raw[:n.value]
+
+
+def thumbnail_tiff_level(stream, width, height=None, size="both"):
+    """(subifd, page) vips_thumbnail_buffer loads from a TIFF for this thumbnail: a pyramid level, or (-1, 0); no GPU needed"""
+    stream = bytes(stream)
+    sub, page = C.c_int(), C.c_int()
+    _check(lib().vb200_thumbnail_tiff_level(stream, len(stream), int(width), int(height or 0), SIZES[size], C.byref(sub), C.byref(page)))
+    return sub.value, page.value
+
+
+def thumbnail_pyramid_level(input_width, input_height, pages, subifds, width, height=None, size="both"):
+    """the level choice of thumbnail_tiff_level over given geometries: pages / subifds are lists of (width, height), pages[0]
+    being the main image -> (subifd, page); no GPU needed"""
+    pw = (C.c_int * max(1, len(pages)))(*[p[0] for p in pages])
+    ph = (C.c_int * max(1, len(pages)))(*[p[1] for p in pages])
+    sw = (C.c_int * max(1, len(subifds)))(*[p[0] for p in subifds])
+    sh = (C.c_int * max(1, len(subifds)))(*[p[1] for p in subifds])
+    sub, page = C.c_int(), C.c_int()
+    _check(lib().vb200_debug_thumbnail_pyramid_level(int(input_width), int(input_height), len(pages), pw, ph, len(subifds), sw, sh,
+                                                     int(width), int(height or 0), SIZES[size], C.byref(sub), C.byref(page)))
+    return sub.value, page.value
 
 
 def lzw_host_twin(data, min_code_size, want, lenient=False):
@@ -1030,8 +1126,8 @@ def _thumbnail_buffer_pages(stream, width, height, size, icc, linear, page, n):
 
 def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                      builtin_profiles=None, page=0, n=1, return_page_height=False):
-    """vips_thumbnail_buffer() of a JPEG, PNG or GIF stream: decode (JPEG with shrink-on-load, GIF's pages page .. page + n - 1,
-    n = -1 for all from page on) + thumbnail on the device -> uint8 array; with output_profile, colour-managed with the profile
+    """vips_thumbnail_buffer() of a JPEG, PNG, GIF or TIFF stream: decode (JPEG with shrink-on-load, GIF's pages page .. page + n - 1,
+    n = -1 for all from page on, a TIFF's pyramid level as thumbnail_tiff_level picks it) + thumbnail on the device -> uint8 array; with output_profile, colour-managed with the profile
     the stream embeds (APP2 ICC_PROFILE or iCCP; GIF has none).  PNG streams with eXIf are refused: their orientation would
     need vips_autorot.  A GIF of several pages thumbnails as a page strip; return_page_height=True returns
     (array, page height) with None for a result of one page"""
@@ -1200,6 +1296,10 @@ class ThumbnailPlan:
         """PNG streams decoded on the device at full size and thumbnailed by this plan (made for the decoded geometry):
         -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
         return self._run_streams(lib().vb200_thumbnail_plan_run_png, streams, (), out_ptr)
+
+    def run_tiff(self, streams, out_ptr=None, page=0, n=1, subifd=-1):
+        """vb200_thumbnail_plan_run_tiff: the streams' pages page .. page + n - 1 at subifd through the plan"""
+        return self._run_streams(lib().vb200_thumbnail_plan_run_tiff, streams, (int(page), int(n), int(subifd)), out_ptr)
 
     def run_gif(self, streams, out_ptr=None, page=0, n=1):
         """GIF streams, pages page .. page + n - 1 of each (n = -1: every page from page on) decoded on the device at full size

@@ -1,6 +1,6 @@
-/* decode.cu -- what the JPEG, PNG and GIF decoders share around their kernels: the stream kinds and the one switch over
+/* decode.cu -- what the JPEG, PNG, GIF and TIFF decoders share around their kernels: the stream kinds and the one switch over
  * the three batch decoders, the C ABI bodies of vb200_*_decode_batch and vb200_*load_buffer, the host-worker header pass,
- * and (for PNG and GIF) the pinned staging block and the chunks bounded by the device budget.
+ * and (for PNG, GIF and TIFF) the pinned staging block and the chunks bounded by the device budget.
  */
 #include <cstdint>
 #include <cstring>
@@ -156,16 +156,28 @@ decode_staging_release()
 StreamKind
 stream_kind(const void *buf, size_t len)
 {
-	return png_signature(buf, len) ? STREAM_PNG : gif_signature(buf, len) ? STREAM_GIF : STREAM_JPEG;
+	return png_signature(buf, len) ? STREAM_PNG : gif_signature(buf, len) ? STREAM_GIF : tiff_signature(buf, len) ? STREAM_TIFF : STREAM_JPEG;
 }
 
 /* The decoder and where the embedded profile comes from are all that differ between the kinds.  PNG and GIF have no
  * load-time shrink (thumbnail.c:609-660 lists the loaders that do), and a PNG with eXIf is declined: its orientation would
- * need vips_autorot (thumbnail.c:989-996), which is not built.  A GIF carries no profile.
+ * need vips_autorot (thumbnail.c:989-996), which is not built.  The same goes for a TIFF IFD whose Orientation is not 1.
+ * A GIF carries no profile.
  */
 int
-stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size_t n, std::vector<unsigned char> *profile)
+stream_profile(const char *domain, const DecodeRequest &req, const unsigned char *d, size_t n, std::vector<unsigned char> *profile)
 {
+	const StreamKind kind = req.kind;
+	if (kind == STREAM_TIFF) {
+		int orientation = 1;
+		if (tiff_icc_profile(domain, d, n, req.page, req.n_pages, req.subifd, profile, &orientation))
+			return -1;
+		if (orientation != 1) {
+			error(domain, "TIFF with Orientation %d: it would need vips_autorot, which is not built", orientation);
+			return -1;
+		}
+		return 0;
+	}
 	if (kind == STREAM_GIF) {
 		profile->clear();
 		return 0;
@@ -189,8 +201,12 @@ dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const
 	/* vips_thumbnail_buffer hands its option string to the loader (thumbnail.c:1486-1490, 1585-1590): page and n are
 	 * nsgifload's; jpegload and spngload have neither, so any other value fails there
 	 */
-	if (req.kind != STREAM_GIF && (req.page != 0 || req.n_pages != 1)) {
+	if (req.kind != STREAM_GIF && req.kind != STREAM_TIFF && (req.page != 0 || req.n_pages != 1)) {
 		error(domain, "%s has no page or n option (page %d, n %d)", req.kind == STREAM_PNG ? "pngload" : "jpegload", req.page, req.n_pages);
+		return -1;
+	}
+	if (req.kind != STREAM_TIFF && req.subifd != -1) {
+		error(domain, "only tiffload has a subifd option (subifd %d)", req.subifd);
 		return -1;
 	}
 	if (n < 1 || !bufs || !lens) {
@@ -205,6 +221,9 @@ dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const
 		break;
 	case STREAM_GIF:
 		rc = dev_gif_decode_batch(domain, bufs, lens, n, req.page, req.n_pages, out, out_bpl, out_frame_stride, &g, s);
+		break;
+	case STREAM_TIFF:
+		rc = dev_tiff_decode_batch(domain, bufs, lens, n, req.page, req.n_pages, req.subifd, out, out_bpl, out_frame_stride, &g, s);
 		break;
 	default:
 		rc = dev_jpeg_decode_batch(domain, bufs, lens, n, req.shrink, out, out_bpl, out_frame_stride, &g, s);

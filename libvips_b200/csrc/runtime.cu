@@ -52,6 +52,13 @@ error(const char *domain, const char *fmt, ...)
 	g_error += "\n";
 }
 
+void
+error_truncate(size_t len)
+{
+	if (g_error.size() > len)
+		g_error.resize(len);
+}
+
 int
 cuda_fail(const char *domain, cudaError_t e, const char *what)
 {

@@ -2364,7 +2364,8 @@ vb200_thumbnail_plan_output_bands(const VB200ThumbnailPlan *plan)
 
 /* reference: vips_thumbnail_buffer(buf, len, &out, width, "height", height, "size", size, NULL), resample/thumbnail.c:
  * 583-613 (open with the load-time shrink vips_thumbnail_find_jpegshrink picks) then :848-902 on what was loaded.
- * JPEG, PNG or GIF streams; everything between the compressed bytes and the thumbnail stays on the device.
+ * JPEG, PNG, GIF or TIFF streams; everything between the compressed bytes and the thumbnail stays on the device.  A TIFF
+ * loads the subifd or page of a pyramid that vips_thumbnail_find_pyrlevel picks (vb200_thumbnail_tiff_level).
  */
 extern "C" int
 vb200_thumbnail_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size)
@@ -2391,9 +2392,18 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 	if (ensure_init(domain))
 		return -1;
 	DecodeRequest req{stream_kind(buf, len), 1, page, n_pages};
+	if (req.kind == STREAM_TIFF) {
+		/* the level vips_thumbnail_open picks: a subifd or page of a pyramid, else page 0 (thumbnail.c:562-581, 1552-1576) */
+		if (page != 0 || n_pages != 1) {
+			error(domain, "TIFF page strips are not thumbnailed on the device (page %d, n %d)", page, n_pages);
+			return -1;
+		}
+		if (tiff_thumbnail_level(domain, (const unsigned char *) buf, len, width, height, size, &req.subifd, &req.page))
+			return -1;
+	}
 	const bool want_profile = icc && (icc->output_profile || linear);
 	std::vector<unsigned char> embedded;
-	if ((req.kind == STREAM_PNG || want_profile) && stream_profile(domain, req.kind, (const unsigned char *) buf, len, &embedded))
+	if ((req.kind == STREAM_PNG || req.kind == STREAM_TIFF || want_profile) && stream_profile(domain, req, (const unsigned char *) buf, len, &embedded))
 		return -1;
 	if (!want_profile)
 		embedded.clear();
@@ -2460,6 +2470,10 @@ extern "C" int
 vb200_thumbnail_buffer_pages(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
 	int linear, int page, int n, int *out_page_height)
 {
+	if (buf && stream_kind(buf, len) == STREAM_TIFF) {
+		error("thumbnail_buffer", "TIFF page strips are not thumbnailed on the device: use vb200_thumbnail_buffer");
+		return -1;
+	}
 	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, linear != 0, page, n, out_page_height);
 }
 
@@ -2486,11 +2500,11 @@ plan_run_streams(const char *domain, const DecodeRequest &req, VB200ThumbnailPla
 	 * stage; PNG streams are read for eXIf either way
 	 */
 	const bool managed = pl.icc != nullptr;
-	std::vector<std::vector<unsigned char>> profiles(managed || req.kind == STREAM_PNG ? n : 0);
+	std::vector<std::vector<unsigned char>> profiles(managed || req.kind == STREAM_PNG || req.kind == STREAM_TIFF ? n : 0);
 	std::vector<const void *> emb(profiles.size());
 	std::vector<size_t> emb_len(profiles.size());
 	for (size_t i = 0; i < profiles.size(); i++) {
-		if (stream_profile(domain, req.kind, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
+		if (stream_profile(domain, req, (const unsigned char *) bufs[i], lens[i], &profiles[i])) {
 			error(domain, "stream %d", (int) i);
 			return -1;
 		}
@@ -2508,7 +2522,7 @@ plan_run_streams(const char *domain, const DecodeRequest &req, VB200ThumbnailPla
 		if (dev_decode_batch(domain, req, bufs, lens, n, dec, (size_t) pl.W * pl.bands, in_frame, &w, &h, &b, &page_h, s))
 			break;
 		/* a GIF strip is the plan's only if its pages are: the screen must be one page high */
-		if (req.kind == STREAM_GIF && (page_h ? page_h : h) != (pl.page_h ? pl.page_h : pl.H)) {
+		if ((req.kind == STREAM_GIF || req.kind == STREAM_TIFF) && (page_h ? page_h : h) != (pl.page_h ? pl.page_h : pl.H)) {
 			error(domain, "the plan is for pages of %d rows, the streams' screen is %d rows", pl.page_h ? pl.page_h : pl.H, page_h ? page_h : h);
 			break;
 		}
@@ -2563,6 +2577,16 @@ vb200_thumbnail_plan_run_gif_pages(VB200ThumbnailPlan *plan, const void *const *
 	void *out, int out_location, size_t out_frame_stride)
 {
 	return plan_run_streams("thumbnail_plan_run_gif", {STREAM_GIF, 1, page, n_pages}, plan, bufs, lens, n, out, out_location, out_frame_stride);
+}
+
+/* See vb200.h: the TIFF streams' pages page .. page + n_pages - 1 at subifd, then the plan */
+extern "C" int
+vb200_thumbnail_plan_run_tiff(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, int page, int n_pages, int subifd,
+	void *out, int out_location, size_t out_frame_stride)
+{
+	DecodeRequest req{STREAM_TIFF, 1, page, n_pages};
+	req.subifd = subifd;
+	return plan_run_streams("thumbnail_plan_run_tiff", req, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 /* The tile pump: a ring of kStreams device staging slots; for each slice of

@@ -26,6 +26,8 @@ namespace vb200 {
 
 /* vips_error(domain, fmt, ...): append to the thread-local buffer. */
 void error(const char *domain, const char *fmt, ...);
+/* drop what was appended to the thread's error buffer after its first len bytes (a probe whose failures are not errors) */
+void error_truncate(size_t len);
 int cuda_fail(const char *domain, cudaError_t e, const char *what);
 
 #define VB200_CUDA(domain, call) \
@@ -192,13 +194,15 @@ int dev_colourspace_ext(const char *domain, const DevImage &in, DevImage *out, i
 /* Launchers of the row/column-table kernels on raw device pointers (used by
  * the generate()-shaped and scanline seams too).
  */
-/* decode.cu: the decoders' shared driver.  A stream's kind is its signature (PNG, GIF), else JPEG. */
-enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF };
+/* decode.cu: the decoders' shared driver.  A stream's kind is its signature (PNG, GIF, TIFF), else JPEG. */
+enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF, STREAM_TIFF };
 StreamKind stream_kind(const void *buf, size_t len);
-/* what to decode: shrink is JPEG's load-time shrink; page / n_pages GIF's pages (n_pages -1: to the last), 0 / 1 elsewhere */
+/* what to decode: shrink is JPEG's load-time shrink; page / n_pages GIF's and TIFF's pages (n_pages -1: to the last), 0 / 1
+ * elsewhere; subifd TIFF's SubIFD of each page (-1: the page's main IFD), -1 elsewhere */
 struct DecodeRequest {
 	StreamKind kind;
 	int shrink = 1, page = 0, n_pages = 1;
+	int subifd = -1;
 };
 /* A batch's geometry as the decoders report it: frames of h rows, or (pages > 0) strips of `pages` pages of h rows. */
 struct StreamGeometry {
@@ -216,8 +220,9 @@ int decode_batch_abi(const char *domain, const DecodeRequest &req, const void *c
 int dev_load(const char *domain, const DecodeRequest &req, const void *buf, size_t len, DevImage *out, int *page_h, cudaStream_t s);
 /* the body of vb200_jpegload / pngload / gifload_buffer: dev_load, then deliver into *out */
 int load_abi(const char *domain, const DecodeRequest &req, const void *buf, size_t len, VB200Image *out);
-/* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP; -1 for a PNG with eXIf; GIF has none */
-int stream_profile(const char *domain, StreamKind kind, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
+/* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP, the ICCProfile of the TIFF IFD req selects; -1 for a
+ * PNG with eXIf or a TIFF IFD whose Orientation is not 1; GIF has none */
+int stream_profile(const char *domain, const DecodeRequest &req, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
 /* The pieces of the per-format batch decoders.  parse_streams runs parse(i) for the n streams on the host workers (0, or -1
  * with the reason in the worker's error buffer, restated as "<noun> i: reason") and checks that geometry(i) agrees. */
 size_t align16(size_t v);
@@ -301,6 +306,17 @@ int png_icc_profile(const char *domain, const unsigned char *d, size_t n, std::v
 int dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int page, int npages, void *out, size_t out_bpl,
 	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);
 bool gif_signature(const void *buf, size_t len); /* GIF87a or GIF89a */
+/* tiff.cu: n TIFF streams of one geometry, pages page .. page + npages - 1 (npages -1: to the last) at subifd (-1: each
+ * page's main IFD) -> out[n][h * pages][w][bands] on the device (out = nullptr: geometry only, no device call) */
+int dev_tiff_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int page, int npages, int subifd, void *out,
+	size_t out_bpl, size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);
+bool tiff_signature(const void *buf, size_t len); /* II*\0, MM\0*, or BigTIFF's 43 in either order */
+/* tiff.cu: the ICCProfile of the IFD page / subifd select (empty: none), and the first Orientation other than 1 among pages
+ * page .. page + n_pages - 1 (n_pages -1: to the last; orientation may be null) */
+int tiff_icc_profile(const char *domain, const unsigned char *d, size_t len, int page, int n_pages, int subifd, std::vector<unsigned char> *profile,
+	int *orientation);
+/* tiff.cu: the subifd / page vips_thumbnail_buffer loads for a thumbnail of width x height (thumbnail.c:562-581, 1552-1576) */
+int tiff_thumbnail_level(const char *domain, const unsigned char *d, size_t len, int width, int height, int size, int *subifd, int *page);
 
 /* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
 int host_workers();

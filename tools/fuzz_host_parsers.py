@@ -1,7 +1,8 @@
 """tools/fuzz_host_parsers.py -- mutation fuzzing of the host-side parsers that read untrusted bytes (the JPEG marker
 parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser, the GIF block walker + the GIF
 decoder's host twin with its LZW, the PNG chunk walker + the PNG
-decoder's host twin with its inflate, on PNG streams and on raw deflate data), meant to run against an AddressSanitizer build:
+decoder's host twin with its inflate, on PNG streams and on raw deflate data, the TIFF IFD walk + the TIFF decoder's host
+twin with its LZW and PackBits and the pyramid-level search), meant to run against an AddressSanitizer build:
 
     VB200_LIB=/tmp/asan/libvb200_asan.so LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \
         python tools/fuzz_host_parsers.py [seconds]
@@ -102,12 +103,30 @@ def gifs(rng):
     return out
 
 
+def tiffs(rng):
+    """TIFFs from the test-suite's writer (BigTIFF, both byte orders, tiles, pages, SubIFDs) and from Pillow's libtiff"""
+    import test_tiff as TT
+    out = []
+    for i in range(8):
+        a = rng.integers(0, 256, (int(rng.integers(1, 40)), int(rng.integers(1, 40)), (1, 2, 3, 4)[i % 4]), dtype=np.uint8)
+        comp = (1, 32773, 5, 8)[i % 4]
+        kw = dict(tile=(16, 16)) if i % 2 else dict(rps=int(rng.integers(1, 9)))
+        out.append(TT.make_tiff([TT.Page(a, comp=comp, pred=1 + (i % 3 == 0), subifds=[TT.Page(a[::2, ::2], comp=comp)], icc=b"icc" * 9,
+                                         **kw)] * (1 + i % 3), "<>"[i % 2], i % 3 == 1))
+    for comp in ("tiff_lzw", "packbits", "tiff_adobe_deflate"):
+        b = io.BytesIO()
+        PIL.fromarray(rng.integers(0, 256, (23, 31, 3), dtype=np.uint8)).save(b, "TIFF", compression=comp)
+        out.append(b.getvalue())
+    return out
+
+
 def main():
     budget = float(sys.argv[1]) if len(sys.argv) > 1 else 60.0
     rng = np.random.default_rng(int(time.time()))
     good = jpegs(rng)
     good_png = pngs(rng)
     good_gif = gifs(rng)
+    good_tiff = tiffs(rng)
     lzw = [g[g.index(b"\x2c") + 11:] for g in good_gif]  # from the minimum code size on: sub-block framing fed to the LZW as data
     deflate = [zlib.compress(s, int(rng.integers(0, 10)))[2:-4] for s in good_png]
     import icc_fixtures as F
@@ -143,6 +162,14 @@ def main():
         for fn in (vb.gif_decode_host_twin, lambda t: vb.gif_decode_host_twin(t, 0, -1), vb.gif_geometry):
             try:
                 fn(g)
+                ok += 1
+            except vb.Error:
+                fails += 1
+        t = mutate(rng, good_tiff[rng.integers(0, len(good_tiff))])
+        for fn in (vb.tiff_decode_host_twin, lambda t: vb.tiff_decode_host_twin(t, 0, -1, 0), lambda t: vb.tiff_geometry(t, 0, 0),
+                   vb.tiff_icc_profile, lambda t: vb.thumbnail_tiff_level(t, 5), lambda t: vb.tiff_lzw_host_twin(t[8:], 1 << 12)):
+            try:
+                fn(t)
                 ok += 1
             except vb.Error:
                 fails += 1
