@@ -457,9 +457,11 @@ int vb200_debug_rank_host(const void *in, int width, int height, int bands, int 
  * What vips_sink_memory + vips_threadpool_run (iofuncs/sinkmemory.c:324, threadpool.c:625) do for an
  * arbitrary graph of operations: a VB200Chain is a list of the operations above; vb200_chain_run_host
  * runs it over a batch of host images with upload / compute / download of consecutive images overlapped on
- * three streams, every intermediate staying on the device.  Each step is the stand-alone entry point's own
- * device function: same pixels as calling vb200_resize(), vb200_conv() ... one by one, without their
- * per-call host round trips.  in[i] / out[i] are arrays of n_images; out[i].data == NULL -> allocated
+ * three streams, every intermediate staying on the device.  vb200_chain_add_<op>() takes the arguments of
+ * vb200_<op>(), applies the same defaults and refuses what it refuses without an image (a missing or empty mask,
+ * a convsep mask that is not 1xn or nx1, a reduce factor below 1) with the same reason; the step then runs the
+ * stand-alone op's own device code: same pixels as calling vb200_resize(), vb200_conv() ... one by one, without
+ * their per-call host round trips.  in[i] / out[i] are arrays of n_images; out[i].data == NULL -> allocated
  * (vb200_image_free).  Pinned host memory (vb200_host_alloc) lets the phases overlap.
  */
 typedef struct VB200Chain VB200Chain;

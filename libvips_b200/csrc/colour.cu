@@ -597,34 +597,3 @@ dev_colourspace(const char *domain, const DevImage &in, DevImage *out, int space
 }
 
 } // namespace vb200
-
-using namespace vb200;
-
-/* reference: vips_colourspace(), colour/colourspace.c:551-617.  The source
- * space is in->Type (the reference guesses it, vips_image_guess_interpretation).
- */
-extern "C" int
-vb200_colourspace(const VB200Image *in, VB200Image *out, int space)
-{
-	const char *domain = "colourspace";
-	if (!in || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	/* colour ops keep the geometry and, but for B_W / GREY16 sources (two bands more), the band count; no output element is
-	 * wider than a float
-	 */
-	const bool grey_source = in->Type == VB200_INTERPRETATION_B_W || in->Type == VB200_INTERPRETATION_GREY16;
-	preset_output(&dout, in, out, (size_t) in->Xsize * (in->Bands + (grey_source ? 2 : 0)) * 4, in->Ysize);
-	int rc = dev_colourspace(domain, din, &dout, space, in->Type, s);
-	if (!rc)
-		rc = deliver(domain, &dout, in, out, s);
-	dev_image_release(&din, s);
-	return rc;
-}

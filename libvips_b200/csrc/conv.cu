@@ -860,10 +860,8 @@ dev_sharpen(const char *domain, const DevImage &in, DevImage *out, double sigma,
 			(const int *) dlut, labs.w, labs.h);
 		count_launch();
 		rc = dev_colourspace(domain, labs, out, in.type, VB200_INTERPRETATION_LABS, s);
-		if (!rc && out->data == labs.data) {
-			out->owned = labs.owned;
-			labs.owned = false;
-		}
+		if (!rc)
+			adopt_pass_through(&labs, out);
 	}
 	dev_image_release(&L, s);
 	dev_image_release(&blur, s);
@@ -876,83 +874,10 @@ dev_sharpen(const char *domain, const DevImage &in, DevImage *out, double sigma,
 
 using namespace vb200;
 
-namespace {
-
-template <typename Op>
-int
-run_conv_op(const char *domain, const VB200Image *in, VB200Image *out, Op op, bool direct = false)
-{
-	if (!in || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	if (direct)
-		/* convolutions keep the geometry; convf widens to float */
-		preset_output(&dout, in, out, (size_t) in->Xsize * in->Bands * std::max<size_t>(4, format_sizeof(in->BandFmt)), in->Ysize);
-	int rc = op(din, &dout, s);
-	if (!rc) {
-		if (dout.data == din.data) {
-			dout.owned = din.owned;
-			din.owned = false;
-		}
-		rc = deliver(domain, &dout, in, out, s);
-	}
-	dev_image_release(&din, s);
-	return rc;
-}
-
-} // namespace
-
 extern "C" void
 vb200_set_vector_convi(int on)
 {
 	g_vector_convi = on != 0;
-}
-
-extern "C" int
-vb200_conv(const VB200Image *in, VB200Image *out, const VB200Mask *mask, int precision)
-{
-	if (!mask || !mask->coeff) {
-		error("conv", "no mask");
-		return -1;
-	}
-	return run_conv_op("conv", in, out, [&](const DevImage &d, DevImage *o, cudaStream_t s) {
-		return dev_conv("conv", d, o, mask->coeff, mask->width, mask->height, mask->scale, mask->offset, precision, s, true);
-	}, true);
-}
-
-extern "C" int
-vb200_convsep(const VB200Image *in, VB200Image *out, const VB200Mask *mask, int precision)
-{
-	if (!mask || !mask->coeff) {
-		error("convsep", "no mask");
-		return -1;
-	}
-	/* vips_check_separable: one of the dimensions must be 1 */
-	if (mask->width != 1 && mask->height != 1) {
-		error("convsep", "mask must be 1xn or nx1 elements");
-		return -1;
-	}
-	return run_conv_op("convsep", in, out, [&](const DevImage &d, DevImage *o, cudaStream_t s) {
-		return dev_convsep("convsep", d, o, mask->coeff, mask->width, mask->height, mask->scale, mask->offset, precision, s,
-			true);
-	}, true);
-}
-
-extern "C" int
-vb200_gaussblur(const VB200Image *in, VB200Image *out, double sigma, double min_ampl, int precision)
-{
-	if (min_ampl <= 0)
-		min_ampl = 0.2; /* gaussblur.c class default */
-	return run_conv_op("gaussblur", in, out, [&](const DevImage &d, DevImage *o, cudaStream_t s) {
-		return dev_gaussblur("gaussblur", d, o, sigma, min_ampl, precision, s);
-	}, true);
 }
 
 extern "C" int
@@ -987,12 +912,4 @@ vb200_mask_free(VB200Mask *mask)
 		free((void *) mask->coeff);
 		mask->coeff = nullptr;
 	}
-}
-
-extern "C" int
-vb200_sharpen(const VB200Image *in, VB200Image *out, double sigma, double x1, double y2, double y3, double m1, double m2)
-{
-	return run_conv_op("sharpen", in, out, [&](const DevImage &d, DevImage *o, cudaStream_t s) {
-		return dev_sharpen("sharpen", d, o, sigma, x1, y2, y3, m1, m2, s);
-	});
 }

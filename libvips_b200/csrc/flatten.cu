@@ -363,30 +363,6 @@ dev_flatten(const char *domain, const DevImage &in, DevImage *out, const double 
 
 using namespace vb200;
 
-/* reference: vips_flatten(), conversion/flatten.c:605-616.  background: n = 1 or bands - 1 values (NULL: black);
- * max_alpha <= 0: the interpretation's default
- */
-extern "C" int
-vb200_flatten(const VB200Image *in, VB200Image *out, const double *background, int n, double max_alpha)
-{
-	const char *domain = "flatten";
-	if (!in || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	int rc = dev_flatten(domain, din, &dout, background, n, max_alpha, s);
-	if (!rc)
-		rc = deliver(domain, &dout, in, out, s);
-	dev_image_release(&din, s);
-	return rc;
-}
-
 /* test hook, host only: flatten.cu's per-pixel code on the CPU over packed host arrays; x4 != 0 asks for the
  * four-pixels-per-thread form (-1 if the image does not qualify)
  */

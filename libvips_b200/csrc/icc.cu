@@ -635,50 +635,42 @@ build_job(const char *domain, const JobSpec &sp, int in_fmt, int in_bands, int i
 int
 run_icc(const char *domain, const VB200Image *in, VB200Image *out, const JobSpec &sp)
 {
-	if (!in || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
 	IccJob J;
 	std::vector<float> pool;
 	int ob, of, ot;
-	if (build_job(domain, sp, in->BandFmt, in->Bands, in->Type, &J, pool, &ob, &of, &ot))
-		return -1;
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	float *dpool = nullptr;
-	int rc = 0;
-	if (!pool.empty()) {
-		rc = dev_alloc(domain, (void **) &dpool, pool.size() * sizeof(float), s);
-		if (!rc && cudaMemcpyAsync(dpool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice, s) != cudaSuccess)
-			rc = -1;
-	}
-	J.in.pool = J.out.pool = dpool;
-	preset_output(&dout, in, out, (size_t) din.w * ob * format_sizeof(of), din.h); /* the exact result extent (grey -> Lab widens 1 band to 3 floats) */
-	if (!rc)
-		rc = dev_image_new(domain, &dout, din.w, din.h, ob, of, ot, s);
-	if (!rc) {
-		const dim3 grid = row_grid(din.w, din.h);
-		(rows_loop(din.h) ? icc_kernel<true> : icc_kernel<false>)<<<grid, 256, 0, s>>>(J, (const char *) din.data, din.bpl, format_sizeof(din.fmt) * din.bands, (char *) dout.data,
-			dout.bpl, format_sizeof(of) * ob, din.w, din.h);
-		const cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-			rc = cuda_fail(domain, e, "icc_kernel");
-		else
-			count_launch();
-	}
-	if (!rc) {
-		/* the pool is read by the kernel: free it stream-ordered, after the launch */
-		rc = deliver(domain, &dout, in, out, s);
-	}
-	if (dpool)
-		dev_free(dpool, s);
-	dev_image_release(&din, s);
-	return rc;
+	return run_image(domain, in, out,
+		[&](size_t *preset_line) {
+			if (build_job(domain, sp, in->BandFmt, in->Bands, in->Type, &J, pool, &ob, &of, &ot))
+				return -1;
+			*preset_line = (size_t) in->Xsize * ob * format_sizeof(of); /* the exact result extent (grey -> Lab widens 1 band to 3 floats) */
+			return 0;
+		},
+		[&](const DevImage &din, DevImage *dout, cudaStream_t s) {
+			float *dpool = nullptr;
+			int rc = 0;
+			if (!pool.empty()) {
+				rc = dev_alloc(domain, (void **) &dpool, pool.size() * sizeof(float), s);
+				if (!rc && cudaMemcpyAsync(dpool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice, s) != cudaSuccess)
+					rc = -1;
+			}
+			J.in.pool = J.out.pool = dpool;
+			if (!rc)
+				rc = dev_image_new(domain, dout, din.w, din.h, ob, of, ot, s);
+			if (!rc) {
+				const dim3 grid = row_grid(din.w, din.h);
+				(rows_loop(din.h) ? icc_kernel<true> : icc_kernel<false>)<<<grid, 256, 0, s>>>(J, (const char *) din.data, din.bpl, format_sizeof(din.fmt) * din.bands, (char *) dout->data,
+					dout->bpl, format_sizeof(of) * ob, din.w, din.h);
+				const cudaError_t e = cudaGetLastError();
+				if (e != cudaSuccess)
+					rc = cuda_fail(domain, e, "icc_kernel");
+				else
+					count_launch();
+			}
+			/* the pool is read by the kernel: free it stream-ordered, after the launch */
+			if (dpool)
+				dev_free(dpool, s);
+			return rc;
+		});
 }
 
 /* ------------------------------------------------------------------ the ICC stage of the thumbnail plan */

@@ -121,27 +121,3 @@ dev_morph(const char *domain, const DevImage &in, DevImage *out, const double *m
 }
 
 } // namespace vb200
-
-using namespace vb200;
-
-/* reference: vips_morph(), morphology/morph.c:1030-1042.  morph: 0 = erode, 1 = dilate (VipsOperationMorphology). */
-extern "C" int
-vb200_morph(const VB200Image *in, VB200Image *out, const VB200Mask *mask, int morph)
-{
-	const char *domain = "morph";
-	if (!in || !out || !mask || !mask->coeff) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	int rc = dev_morph(domain, din, &dout, mask->coeff, mask->width, mask->height, morph, s);
-	if (!rc)
-		rc = deliver(domain, &dout, in, out, s);
-	dev_image_release(&din, s);
-	return rc;
-}

@@ -271,34 +271,6 @@ dev_rank(const char *domain, const DevImage &in, DevImage *out, int width, int h
 
 using namespace vb200;
 
-/* reference: vips_rank(), morphology/rank.c:623-635; vips_median(in, out, size) is rank(size, size, size * size / 2), :651-664 */
-extern "C" int
-vb200_rank(const VB200Image *in, VB200Image *out, int width, int height, int index)
-{
-	const char *domain = "rank";
-	if (!in || !out) {
-		error(domain, "null argument");
-		return -1;
-	}
-	if (ensure_init(domain))
-		return -1;
-	cudaStream_t s = current_stream();
-	DevImage din, dout;
-	if (to_device(domain, in, &din, s))
-		return -1;
-	int rc = dev_rank(domain, din, &dout, width, height, index, s);
-	if (!rc)
-		rc = deliver(domain, &dout, in, out, s);
-	dev_image_release(&din, s);
-	return rc;
-}
-
-extern "C" int
-vb200_median(const VB200Image *in, VB200Image *out, int size)
-{
-	return vb200_rank(in, out, size, size, (size * size) / 2);
-}
-
 /* test hook, host only: the kernel's staging and select code run tile by tile on the CPU over packed host arrays */
 extern "C" int
 vb200_debug_rank_host(const void *in, int width, int height, int bands, int band_format, int rank_width, int rank_height, int index,

@@ -316,57 +316,79 @@ to_device(const char *domain, const VB200Image *in, DevImage *d, cudaStream_t s)
 	return 0;
 }
 
+void
+adopt_pass_through(DevImage *in, DevImage *out)
+{
+	if (out->data == in->data) {
+		out->owned = in->owned;
+		in->owned = false;
+	}
+}
+
+static void
+describe(const DevImage &d, int where, VB200Image *out)
+{
+	out->Xsize = d.w;
+	out->Ysize = d.h;
+	out->Bands = d.bands;
+	out->BandFmt = d.fmt;
+	out->Type = d.type;
+	out->where = where;
+}
+
 int
-deliver(const char *domain, DevImage *d, const VB200Image *like, VB200Image *out, cudaStream_t s)
+deliver_host(const char *domain, DevImage *d, const VB200Image *like, VB200Image *out, cudaStream_t s)
 {
 	const size_t line = (size_t) d->w * d->bands * format_sizeof(d->fmt);
-	const int where = like->where;
 	void *dst = out->data;
-	size_t dst_bpl = (out->data && out->bpl) ? out->bpl : line;
-
-	out->Xsize = d->w;
-	out->Ysize = d->h;
-	out->Bands = d->bands;
-	out->BandFmt = d->fmt;
-	out->Type = d->type;
-	out->where = where;
-
-	if (where == VB200_DEVICE) {
-		if (!dst && d->owned) {
-			/* hand our buffer over */
-			out->data = d->data;
-			out->bpl = d->bpl;
-			d->owned = false;
-			return 0;
-		}
-		if (dst && dst == d->data) {
-			/* the op wrote into the caller's buffer (preset_output) */
-			out->bpl = d->bpl;
-			return 0;
-		}
-		if (!dst) {
-			if (dev_alloc(domain, &dst, line * d->h, s))
-				return -1;
-			out->data = dst;
-		}
-		out->bpl = dst_bpl;
-		VB200_CUDA(domain,
-			cudaMemcpy2DAsync(dst, dst_bpl, d->data, d->bpl, line, d->h, cudaMemcpyDeviceToDevice, s));
-		dev_image_release(d, s);
-		return 0;
-	}
-
+	const size_t dst_bpl = (out->data && out->bpl) ? out->bpl : line;
 	if (!dst) {
 		dst = malloc(line * d->h > 0 ? line * d->h : 1);
 		if (!dst) {
 			error(domain, "out of memory");
 			return -1;
 		}
+	}
+	describe(*d, like->where, out);
+	out->data = dst;
+	out->bpl = dst_bpl;
+	VB200_CUDA(domain, cudaMemcpy2DAsync(dst, dst_bpl, d->data, d->bpl, line, d->h, cudaMemcpyDeviceToHost, s));
+	dev_image_release(d, s);
+	return 0;
+}
+
+int
+deliver(const char *domain, DevImage *d, const VB200Image *like, VB200Image *out, cudaStream_t s)
+{
+	if (like->where != VB200_DEVICE) {
+		if (deliver_host(domain, d, like, out, s))
+			return -1;
+		VB200_CUDA(domain, cudaStreamSynchronize(s));
+		return 0;
+	}
+	const size_t line = (size_t) d->w * d->bands * format_sizeof(d->fmt);
+	void *dst = out->data;
+	size_t dst_bpl = (out->data && out->bpl) ? out->bpl : line;
+	describe(*d, like->where, out);
+	if (!dst && d->owned) {
+		/* hand our buffer over */
+		out->data = d->data;
+		out->bpl = d->bpl;
+		d->owned = false;
+		return 0;
+	}
+	if (dst && dst == d->data) {
+		/* the op wrote into the caller's buffer (preset_output) */
+		out->bpl = d->bpl;
+		return 0;
+	}
+	if (!dst) {
+		if (dev_alloc(domain, &dst, line * d->h, s))
+			return -1;
 		out->data = dst;
 	}
 	out->bpl = dst_bpl;
-	VB200_CUDA(domain, cudaMemcpy2DAsync(dst, dst_bpl, d->data, d->bpl, line, d->h, cudaMemcpyDeviceToHost, s));
-	VB200_CUDA(domain, cudaStreamSynchronize(s));
+	VB200_CUDA(domain, cudaMemcpy2DAsync(dst, dst_bpl, d->data, d->bpl, line, d->h, cudaMemcpyDeviceToDevice, s));
 	dev_image_release(d, s);
 	return 0;
 }

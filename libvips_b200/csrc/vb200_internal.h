@@ -87,8 +87,16 @@ bool format_is_supported(int fmt); /* the 8 real formats minus double */
 
 /* Bring a VB200Image onto the device (no copy if it already is there). */
 int to_device(const char *domain, const VB200Image *in, DevImage *d, cudaStream_t s);
-/* Deliver a device image into *out following the allocate-or-fill contract. */
+/* Deliver a device image into *out following the allocate-or-fill contract, in like's memory (host or device), and
+ * release it.  Returns once a host result has landed.
+ */
 int deliver(const char *domain, DevImage *d, const VB200Image *like, VB200Image *out, cudaStream_t s);
+/* deliver()'s host branch without the synchronise: the download is queued on s, d released in stream order */
+int deliver_host(const char *domain, DevImage *d, const VB200Image *like, VB200Image *out, cudaStream_t s);
+/* After an op that may pass its input through (out->data == in->data, out->owned false): out takes over in's ownership,
+ * so that releasing in leaves the buffer to out.
+ */
+void adopt_pass_through(DevImage *in, DevImage *out);
 /* Allocate an owned packed device image. */
 int dev_image_new(const char *domain, DevImage *d, int w, int h, int bands, int fmt, int type, cudaStream_t s);
 /* Let the op write straight into a device buffer the caller supplied (no device-to-device copy in
@@ -96,6 +104,15 @@ int dev_image_new(const char *domain, DevImage *d, int w, int h, int bands, int 
  */
 void preset_output(DevImage *dout, const VB200Image *in, const VB200Image *out, size_t out_line_bytes, int out_rows);
 void dev_image_release(DevImage *d, cudaStream_t s);
+
+/* image_ops.cu: the stand-alone form of a whole-image op (vb200_resize, vb200_conv ..., vb200_icc_import ...).  It checks
+ * in and out, runs prepare on the host (refusals that need in's descriptor; *preset_line: the bytes of a result line the
+ * op may write straight into a caller's device buffer, 0 never), brings in onto the device, runs apply, delivers the
+ * result into *out and releases in.  The whole-image ops themselves, their records and the chain pump live there too.
+ */
+using ImageApply = std::function<int(const DevImage &in, DevImage *out, cudaStream_t s)>;
+int run_image(const char *domain, const VB200Image *in, VB200Image *out, const std::function<int(size_t *preset_line)> &prepare,
+	const ImageApply &apply);
 
 /* ------------------------------------------------------------ resample host */
 
