@@ -627,6 +627,38 @@ int vb200_thumbnail_plan_run_png(VB200ThumbnailPlan *plan, const void *const *bu
 int vb200_debug_png_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
 int vb200_debug_inflate(const void *buf, size_t len, void *out, size_t cap, size_t *out_len);
 void vb200_debug_png_set_budget(size_t bytes);
+/* ------------------------------------------------------------------ WebP decode on the device
+ * vips_webpload_buffer(buf, len, &out, NULL) (foreign/webp2vips.c through webpload.c: WebPDecode in MODE_RGBA with
+ * fancy upsampling, the fourth band dropped without alpha, :600-645, 740-790) with the VP8 key frame decoded on the device
+ * (csrc/webp.cu): the VP8 chunk payloads are all that crosses PCIe.  Decoded: the simple format and VP8X without the
+ * ANIMATION and ALPHA flags, key frames up to 16383 x 16383 with every key-frame feature.  Output is uchar sRGB
+ * [n][height][width][3], pixel for pixel libwebp's.  Everything else returns -1 with its reason (the host keeps
+ * webpload): VP8L, ALPH or the ALPHA flag, ANIM / ANMF, non-key frames, a bad signature or chunk sizes that run past the
+ * RIFF or the buffer, a VP8X canvas other than the frame.  A frame libwebp refuses while decoding (a header or partition
+ * cut short, a bad partition table) fails the batch with "frame i:".
+ *
+ * vb200_webp_geometry: width, height and bands (3); host only.
+ * vb200_webp_decode_batch: n streams of ONE geometry; a stream that fails fails the batch with "frame i:" in the error,
+ *   and with out in host memory nothing is written (in device memory, frames of earlier chunks of a batch larger than one
+ *   chunk may be).  out = NULL only reports the geometry, without a device.
+ * vb200_webpload_buffer: one stream into a VB200Image (allocate-or-fill).
+ * vb200_webp_icc_profile: the ICCP chunk of a VP8X stream; as vb200_png_icc_profile.
+ * vb200_debug_webp_decode: test hook, host only -- the same per-symbol, per-block and per-pixel code on the CPU.
+ * vb200_debug_webp_tables: test hook -- the decoder's constant tables, one after another (*len bytes; copied when cap holds
+ *   them).
+ * vb200_debug_webp_times: with VB200_WEBP_TIMING set in the environment, ms[4] = the last batch's device milliseconds in the
+ *   header, token, reconstruction and RGB kernels on the calling thread (each chunk then waits for its events); -1 without.
+ * vb200_thumbnail_buffer and the other thumbnail entries refuse WebP: thumbnail.c loads it at a non-integer scale through
+ * libwebp's own rescaler, which is not built.  Chunks are bounded by vb200_debug_png_set_budget.
+ */
+int vb200_webp_geometry(const void *buf, size_t len, int *width, int *height, int *bands);
+int vb200_webp_decode_batch(const void *const *bufs, const size_t *lens, int n, void *out, int out_location, size_t out_bpl,
+	size_t out_frame_stride, int *width, int *height, int *bands);
+int vb200_webpload_buffer(const void *buf, size_t len, VB200Image *out);
+int vb200_webp_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len);
+int vb200_debug_webp_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
+int vb200_debug_webp_tables(void *out, size_t cap, size_t *len);
+void vb200_debug_webp_times(float *ms);
 /* ------------------------------------------------------------------ GIF decode on the device (SURVEY 8f rank 1)
  * vips_gifload_buffer(buf, len, &out, "page", page, "n", n, NULL) (foreign/nsgifload.c over libnsgif, fail_on = none)
  * with LZW and frame composition on the device (csrc/gif.cu): the LZW payloads, without their sub-block length bytes, and

@@ -108,6 +108,11 @@ def jpeg_icc_profile(stream):
     return _icc_blob(lib().vb200_jpeg_icc_profile, stream)
 
 
+def webp_icc_profile(stream):
+    """vips_image_get_blob(VIPS_META_ICC_NAME) of a WebP stream (its ICCP chunk): bytes, or None; no GPU"""
+    return _icc_blob(lib().vb200_webp_icc_profile, stream)
+
+
 def png_icc_profile(stream):
     """vips_image_get_blob(VIPS_META_ICC_NAME) of a PNG stream (its iCCP chunk, inflated): bytes, or None; no GPU"""
     return _icc_blob(lib().vb200_png_icc_profile, stream)
@@ -313,6 +318,14 @@ def lib():
                                                           PI, PI]
         L.vb200_debug_tiff_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_tiff_lzw.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]
+        L.vb200_webp_geometry.argtypes = [C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_webp_decode_batch.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_void_p, C.c_int, C.c_size_t,
+                                              C.c_size_t, PI, PI, PI]
+        L.vb200_webpload_buffer.argtypes = [C.c_void_p, C.c_size_t, IP]
+        L.vb200_webp_icc_profile.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_webp_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_debug_webp_tables.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.vb200_debug_webp_times.argtypes = [C.POINTER(C.c_float)]
         L.vb200_thumbnail_plan_new_pages.restype = C.c_void_p
         L.vb200_thumbnail_plan_new_pages.argtypes = [C.c_int] * 10
         L.vb200_thumbnail_plan_page_height.argtypes = [C.c_void_p]
@@ -594,6 +607,19 @@ class Image:
         page_h = tiff_geometry(stream, page, subifd)[1]
         return Image(a, "b-w" if a.shape[2] < 3 else "srgb", page_height=page_h if a.shape[0] > page_h else None)
 
+    @staticmethod
+    def webpload_buffer(stream):
+        """vips_webpload_buffer(stream) of a lossy, still, opaque WebP: the frame decoded on the device -> Image (uint8, 3 bands,
+        sRGB)"""
+        stream = bytes(stream)
+        out = CImage()
+        out.where = HOST
+        _check(lib().vb200_webpload_buffer(stream, len(stream), C.byref(out)))
+        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
+        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
+        lib().vb200_image_free(C.byref(out))
+        return Image(a, "srgb")
+
     # ---- colour
     @staticmethod
     def gifload_buffer(stream, page=0, n=1):
@@ -706,6 +732,49 @@ def png_decode_host_twin(stream):
     _check(lib().vb200_debug_png_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
                                         C.byref(h), C.byref(bands)))
     return out
+
+
+def webp_geometry(stream):
+    """(width, height, bands) a lossy, still, opaque WebP stream decodes to; no GPU needed"""
+    stream = bytes(stream)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_webp_geometry(stream, len(stream), C.byref(w), C.byref(h), C.byref(bands)))
+    return w.value, h.value, bands.value
+
+
+def webp_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None):
+    """vips_webpload_buffer() of every stream (lossy, still, opaque WebP) on the device -> uint8 [n, h, w, 3] (host), or into the
+    device pointer out_ptr (packed frames unless out_bpl / out_frame_stride say otherwise)"""
+    return _decode_batch(lib().vb200_webp_decode_batch, streams, (), out_ptr, out_bpl, out_frame_stride)
+
+
+def webp_decode_host_twin(stream):
+    """the decoder's per-symbol / per-block / per-pixel code compiled for the host (vb200_debug_webp_decode): what the CPU tests
+    pin to libwebp"""
+    stream = bytes(stream)
+    w, h, bands = C.c_int(), C.c_int(), C.c_int()
+    _check(lib().vb200_debug_webp_decode(stream, len(stream), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    out = np.empty((h.value, w.value, bands.value), np.uint8)
+    _check(lib().vb200_debug_webp_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
+                                         C.byref(h), C.byref(bands)))
+    return out
+
+
+def webp_times():
+    """{kernel: device ms} of the last WebP batch on this thread (header, tokens, recon, rgb), measured only with VB200_WEBP_TIMING
+    set in the environment; None without it"""
+    ms = (C.c_float * 4)()
+    lib().vb200_debug_webp_times(ms)
+    return None if ms[0] < 0 else dict(zip(("header", "tokens", "recon", "rgb"), [round(v, 3) for v in ms]))
+
+
+def webp_tables():
+    """the VP8 constant tables as the decoder holds them, as one bytes object (see vb200_debug_webp_tables)"""
+    n = C.c_size_t()
+    _check(lib().vb200_debug_webp_tables(None, 0, C.byref(n)))
+    buf = C.create_string_buffer(n.value)
+    _check(lib().vb200_debug_webp_tables(buf, n.value, C.byref(n)))
+    return buf.raw
 
 
 def gif_geometry(stream):

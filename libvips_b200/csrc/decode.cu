@@ -1,6 +1,6 @@
-/* decode.cu -- what the JPEG, PNG, GIF and TIFF decoders share around their kernels: the stream kinds and the one switch over
+/* decode.cu -- what the JPEG, PNG, GIF, TIFF and WebP decoders share around their kernels: the stream kinds and the one switch over
  * the three batch decoders, the C ABI bodies of vb200_*_decode_batch and vb200_*load_buffer, the host-worker header pass,
- * and (for PNG, GIF and TIFF) the pinned staging block and the chunks bounded by the device budget.
+ * and (for PNG, GIF, TIFF and WebP) the pinned staging block and the chunks bounded by the device budget.
  */
 #include <cstdint>
 #include <cstring>
@@ -156,7 +156,11 @@ decode_staging_release()
 StreamKind
 stream_kind(const void *buf, size_t len)
 {
-	return png_signature(buf, len) ? STREAM_PNG : gif_signature(buf, len) ? STREAM_GIF : tiff_signature(buf, len) ? STREAM_TIFF : STREAM_JPEG;
+	return png_signature(buf, len)	   ? STREAM_PNG
+		   : gif_signature(buf, len)  ? STREAM_GIF
+		   : tiff_signature(buf, len) ? STREAM_TIFF
+		   : webp_signature(buf, len) ? STREAM_WEBP
+									  : STREAM_JPEG;
 }
 
 /* The decoder and where the embedded profile comes from are all that differ between the kinds.  PNG and GIF have no
@@ -182,6 +186,8 @@ stream_profile(const char *domain, const DecodeRequest &req, const unsigned char
 		profile->clear();
 		return 0;
 	}
+	if (kind == STREAM_WEBP)
+		return webp_icc_profile(domain, d, n, profile);
 	if (kind == STREAM_JPEG)
 		return jpeg_icc_profile(domain, d, n, profile);
 	bool exif = false;
@@ -199,8 +205,13 @@ dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const
 	size_t out_frame_stride, int *w, int *h, int *bands, int *page_h, cudaStream_t s)
 {
 	/* vips_thumbnail_buffer hands its option string to the loader (thumbnail.c:1486-1490, 1585-1590): page and n are
-	 * nsgifload's; jpegload and spngload have neither, so any other value fails there
+	 * nsgifload's; jpegload and spngload have neither, so any other value fails there.  webpload's page and n select frames
+	 * of an animation, which is not decoded here.
 	 */
+	if (req.kind == STREAM_WEBP && (req.page != 0 || req.n_pages != 1)) {
+		error(domain, "webpload's page and n select animation frames, which are not decoded on the device (page %d, n %d)", req.page, req.n_pages);
+		return -1;
+	}
 	if (req.kind != STREAM_GIF && req.kind != STREAM_TIFF && (req.page != 0 || req.n_pages != 1)) {
 		error(domain, "%s has no page or n option (page %d, n %d)", req.kind == STREAM_PNG ? "pngload" : "jpegload", req.page, req.n_pages);
 		return -1;
@@ -224,6 +235,9 @@ dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const
 		break;
 	case STREAM_TIFF:
 		rc = dev_tiff_decode_batch(domain, bufs, lens, n, req.page, req.n_pages, req.subifd, out, out_bpl, out_frame_stride, &g, s);
+		break;
+	case STREAM_WEBP:
+		rc = dev_webp_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, &g, s);
 		break;
 	default:
 		rc = dev_jpeg_decode_batch(domain, bufs, lens, n, req.shrink, out, out_bpl, out_frame_stride, &g, s);

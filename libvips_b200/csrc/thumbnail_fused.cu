@@ -2389,9 +2389,14 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 		error(domain, "null argument");
 		return -1;
 	}
+	DecodeRequest req{stream_kind(buf, len), 1, page, n_pages};
+	if (req.kind == STREAM_WEBP) {
+		/* thumbnail.c:627-636, 1524-1532 load WebP at scale = 1 / factor: libwebp's own rescaler, not the full-size decode */
+		error(domain, "WebP shrink-on-load (libwebp's scaled decode) is not built on the device path");
+		return -1;
+	}
 	if (ensure_init(domain))
 		return -1;
-	DecodeRequest req{stream_kind(buf, len), 1, page, n_pages};
 	if (req.kind == STREAM_TIFF) {
 		/* the level vips_thumbnail_open picks: a subifd or page of a pyramid, else page 0 (thumbnail.c:562-581, 1552-1576) */
 		if (page != 0 || n_pages != 1) {

@@ -211,8 +211,8 @@ int dev_colourspace_ext(const char *domain, const DevImage &in, DevImage *out, i
 /* Launchers of the row/column-table kernels on raw device pointers (used by
  * the generate()-shaped and scanline seams too).
  */
-/* decode.cu: the decoders' shared driver.  A stream's kind is its signature (PNG, GIF, TIFF), else JPEG. */
-enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF, STREAM_TIFF };
+/* decode.cu: the decoders' shared driver.  A stream's kind is its signature (PNG, GIF, TIFF, WebP), else JPEG. */
+enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF, STREAM_TIFF, STREAM_WEBP };
 StreamKind stream_kind(const void *buf, size_t len);
 /* what to decode: shrink is JPEG's load-time shrink; page / n_pages GIF's and TIFF's pages (n_pages -1: to the last), 0 / 1
  * elsewhere; subifd TIFF's SubIFD of each page (-1: the page's main IFD), -1 elsewhere */
@@ -237,7 +237,7 @@ int decode_batch_abi(const char *domain, const DecodeRequest &req, const void *c
 int dev_load(const char *domain, const DecodeRequest &req, const void *buf, size_t len, DevImage *out, int *page_h, cudaStream_t s);
 /* the body of vb200_jpegload / pngload / gifload_buffer: dev_load, then deliver into *out */
 int load_abi(const char *domain, const DecodeRequest &req, const void *buf, size_t len, VB200Image *out);
-/* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP, the ICCProfile of the TIFF IFD req selects; -1 for a
+/* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP, the ICCProfile of the TIFF IFD req selects, WebP's ICCP; -1 for a
  * PNG with eXIf or a TIFF IFD whose Orientation is not 1; GIF has none */
 int stream_profile(const char *domain, const DecodeRequest &req, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
 /* The pieces of the per-format batch decoders.  parse_streams runs parse(i) for the n streams on the host workers (0, or -1
@@ -334,6 +334,14 @@ int tiff_icc_profile(const char *domain, const unsigned char *d, size_t len, int
 	int *orientation);
 /* tiff.cu: the subifd / page vips_thumbnail_buffer loads for a thumbnail of width x height (thumbnail.c:562-581, 1552-1576) */
 int tiff_thumbnail_level(const char *domain, const unsigned char *d, size_t len, int width, int height, int size, int *subifd, int *page);
+
+/* webp.cu: n WebP streams (lossy, still, opaque) of one geometry -> out[n][h][w][3] on the device (out = nullptr: geometry
+ * only, no device call) */
+int dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
+	StreamGeometry *g, cudaStream_t s);
+bool webp_signature(const void *buf, size_t len); /* RIFF, 4 bytes, WEBP */
+/* webp.cu: the ICCP chunk of a VP8X stream (empty: none) */
+int webp_icc_profile(const char *domain, const unsigned char *d, size_t len, std::vector<unsigned char> *profile);
 
 /* the decoders' host workers: VB200_JPEG_THREADS, else the CPUs this process may run on, at most 16 (jpeg.cu) */
 int host_workers();

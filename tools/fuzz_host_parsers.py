@@ -2,7 +2,8 @@
 parser + the decoder's host twin, the embedded-ICC-profile reader, the ICC profile parser, the GIF block walker + the GIF
 decoder's host twin with its LZW, the PNG chunk walker + the PNG
 decoder's host twin with its inflate, on PNG streams and on raw deflate data, the TIFF IFD walk + the TIFF decoder's host
-twin with its LZW and PackBits and the pyramid-level search), meant to run against an AddressSanitizer build:
+twin with its LZW and PackBits and the pyramid-level search, the WebP RIFF / VP8X / frame-tag parser + the VP8 decoder's
+host twin), meant to run against an AddressSanitizer build:
 
     VB200_LIB=/tmp/asan/libvb200_asan.so LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \
         python tools/fuzz_host_parsers.py [seconds]
@@ -120,6 +121,20 @@ def tiffs(rng):
     return out
 
 
+def webps(rng):
+    """lossy WebPs from Pillow's libwebp (simple format, and VP8X with an ICCP chunk) and the test-suite's VP8 key-frame
+    writer (2 / 4 / 8 partitions, segments, filter deltas)"""
+    import test_webp as TW
+    out = []
+    for i in range(6):
+        a = rng.integers(0, 256, (int(rng.integers(1, 40)), int(rng.integers(1, 40)), 3), dtype=np.uint8)
+        b = io.BytesIO()
+        PIL.fromarray(a).save(b, "WEBP", quality=int(rng.integers(0, 101)), **({"icc_profile": b"icc" * 9} if i % 2 else {}))
+        out.append(b.getvalue())
+    out += [TW.vp8_stream(int(rng.integers(0, 1 << 30)), h=int(rng.integers(1, 40)), w=int(rng.integers(1, 40))) for _ in range(6)]
+    return out
+
+
 def main():
     budget = float(sys.argv[1]) if len(sys.argv) > 1 else 60.0
     rng = np.random.default_rng(int(time.time()))
@@ -127,6 +142,7 @@ def main():
     good_png = pngs(rng)
     good_gif = gifs(rng)
     good_tiff = tiffs(rng)
+    good_webp = webps(rng)
     lzw = [g[g.index(b"\x2c") + 11:] for g in good_gif]  # from the minimum code size on: sub-block framing fed to the LZW as data
     deflate = [zlib.compress(s, int(rng.integers(0, 10)))[2:-4] for s in good_png]
     import icc_fixtures as F
@@ -170,6 +186,13 @@ def main():
                    vb.tiff_icc_profile, lambda t: vb.thumbnail_tiff_level(t, 5), lambda t: vb.tiff_lzw_host_twin(t[8:], 1 << 12)):
             try:
                 fn(t)
+                ok += 1
+            except vb.Error:
+                fails += 1
+        w = mutate(rng, good_webp[rng.integers(0, len(good_webp))])
+        for fn in (vb.webp_decode_host_twin, vb.webp_geometry, vb.webp_icc_profile):
+            try:
+                fn(w)
                 ok += 1
             except vb.Error:
                 fails += 1
