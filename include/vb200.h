@@ -330,9 +330,11 @@ int vb200_thumbnail_plan_is_fused(const VB200ThumbnailPlan *plan);
 size_t vb200_thumbnail_plan_bytes_per_frame(const VB200ThumbnailPlan *plan);
 /* Which kernel a batch call of this plan launches (for bench / profile labels): a
  * static string such as "thumbnail_fused_mma_kernel<VS=4,NP=6,premul,HS=4,cols=768,cpt=2>",
- * or "leaf kernels" for an unfused plan.  The plan chooses the kernel once; the one exception is a
- * batch whose base pointer, or whose frame stride (with more than one frame), is not a multiple of
- * 16 bytes: it runs thumbnail_fused_kernel (the ld.global kernel) with the same pixels.
+ * or "leaf kernels" for an unfused plan.  The template arguments are those of the instantiation
+ * that launches: "VS=0(13)" is the run-time-box form running box 13.  The plan chooses the kernel
+ * once; the one exception is a batch whose base pointer, or whose frame stride (with more than
+ * one frame), is not a multiple of 16 bytes: it runs thumbnail_fused_kernel (the ld.global kernel)
+ * with the same pixels.
  */
 const char *vb200_thumbnail_plan_kernel(const VB200ThumbnailPlan *plan);
 

@@ -2092,13 +2092,21 @@ plan_kernel_name(const ThumbnailPlanImpl &pl, char *buf, size_t cap)
 		return "linear_v_kernel + linear_h_kernel";
 	const FusedParams &fp = pl.fp;
 	const char *alpha = pl.premul ? "premul" : "plain";
+	/* v1 / v2: the box their switch instantiates (launch_ldg_vs, launch_tma_vs), else VS=0, the run-time form, and the box */
+	char vs[24];
+	const bool listed = (fp.VS >= 1 && fp.VS <= 4) || fp.VS == 8 || (pl.kernel == FusedKernel::Ldg && (fp.VS == 5 || fp.VS == 6));
+	if (listed)
+		snprintf(vs, sizeof(vs), "%d", fp.VS);
+	else
+		snprintf(vs, sizeof(vs), "0(%d)", fp.VS);
+	const int np_tma = fp.NPv == fp.NPh && (fp.NPv == 6 || fp.NPv == 7) ? fp.NPv : 0; /* launch_tma */
 	switch (pl.kernel) {
 	case FusedKernel::Mma:
 		snprintf(buf, cap, "thumbnail_fused_mma_kernel<VS=%d,NP=%d,%s,HS=%d,cols=%d,cpt=%d>", fp.VS, v4_np(fp.VS, fp.NPh, fp.HS), alpha,
 			fp.HS, kV4Cols, kV4Cpt);
 		break;
-	case FusedKernel::Tma: snprintf(buf, cap, "thumbnail_fused_tma_kernel<VS=%d,%s>", fp.VS, alpha); break;
-	case FusedKernel::Ldg: snprintf(buf, cap, "thumbnail_fused_kernel<VS=%d,%s>", fp.VS, alpha); break;
+	case FusedKernel::Tma: snprintf(buf, cap, "thumbnail_fused_tma_kernel<VS=%s,NP=%d,%s>", vs, np_tma, alpha); break;
+	case FusedKernel::Ldg: snprintf(buf, cap, "thumbnail_fused_kernel<VS=%s,%s>", vs, alpha); break;
 	}
 	return buf;
 }

@@ -55,10 +55,10 @@ CHOICES = [
     ((2048, 1536, 256, 256, "force", True), mma(3, 0, 4)),
     ((4096, 2048, 500, None, "both", True), mma(4, 7, 4)),
     ((1003, 2057, 120, None, "both", True), "thumbnail_fused_kernel<VS=8,premul>"),      # rows off 16 bytes
-    ((2560, 1280, 256, 183, "force", True), "thumbnail_fused_tma_kernel<VS=3,premul>"),  # boxes 3 / 10
+    ((2560, 1280, 256, 183, "force", True), "thumbnail_fused_tma_kernel<VS=3,NP=0,premul>"),  # boxes 3 / 10
     ((1024, 4096, 256, 256, "force", True), "thumbnail_fused_kernel<VS=8,premul>"),      # (8, 2): no v4 instantiation
-    ((1000, 1000, 400, None, "both", True), "thumbnail_fused_tma_kernel<VS=1,premul>"),  # box 1
-    ((4096, 4096, 150, None, "both", True), "thumbnail_fused_kernel<VS=13,premul>"),     # box 13
+    ((1000, 1000, 400, None, "both", True), "thumbnail_fused_tma_kernel<VS=1,NP=0,premul>"),  # box 1
+    ((4096, 4096, 150, None, "both", True), "thumbnail_fused_kernel<VS=0(13),premul>"),  # box 13: the run-time form
     ((2052, 2052, 128, None, "both", True), "thumbnail_fused_kernel<VS=8,premul>"),      # box 8 cut short at the right edge
 ]
 
@@ -97,7 +97,8 @@ def test_plan_names_only_instantiated_tensor_pipe_kernels():
                     assert key in V4_LIST, (w, h, t, th, size, name)
                     seen.add(key)
                 else:
-                    assert re.fullmatch(r"thumbnail_fused_(tma_)?kernel<VS=\d+,premul>|leaf kernels", name), name
+                    assert re.fullmatch(r"thumbnail_fused_tma_kernel<VS=([1-48]|0\(\d+\)),NP=[067],premul>|"
+                                        r"thumbnail_fused_kernel<VS=([1-68]|0\(\d+\)),premul>|leaf kernels", name), name
     assert len(seen) >= 10, seen
 
 
