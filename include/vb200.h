@@ -43,6 +43,7 @@ typedef enum {
 typedef enum {
 	VB200_INTERPRETATION_MULTIBAND = 0,
 	VB200_INTERPRETATION_B_W = 1,
+	VB200_INTERPRETATION_HISTOGRAM = 10,
 	VB200_INTERPRETATION_CMYK = 15,
 	VB200_INTERPRETATION_XYZ = 12,
 	VB200_INTERPRETATION_LAB = 13,
@@ -454,6 +455,31 @@ int vb200_median(const VB200Image *in, VB200Image *out, int size);
 int vb200_debug_rank_host(const void *in, int width, int height, int bands, int band_format, int rank_width, int rank_height,
 	int index, void *out);
 
+/* ------------------------------------------------------------ histograms
+ * reference: vips_hist_find(), arithmetic/hist_find.c:471-482 (band -1: every band; else that band alone).  uchar and
+ * ushort images (others: cast first).  The result is (mx + 1) x 1, one band per scanned band, UINT, interpretation
+ * HISTOGRAM: a uchar histogram of every band is 256 wide, every other one as wide as its largest value plus one.  Images
+ * of 2^32 or more pixels (the reference's DOUBLE histogram) are refused.  A bad band: "bandno must be -1, or less than n".
+ */
+int vb200_hist_find(const VB200Image *in, VB200Image *out, int band);
+/* reference: vips_hist_equal(), histogram/hist_equal.c:156-167: hist_find -> hist_cum -> hist_norm -> cast -> maplut, the
+ * LUT built on the device.  uchar and ushort images; band as hist_find (a one-band LUT then maps every band).
+ */
+int vb200_hist_equal(const VB200Image *in, VB200Image *out, int band);
+/* reference: vips_hist_local(), histogram/hist_local.c:417-428 (build :283-306, generate :133-250): contrast-limited local
+ * equalisation over a width x height window (max_slope > 0: CLAHE; sharp's clahe()).  uchar images; errors as the
+ * reference ("image must be uchar", "window too large"), and windows of more than 8 388 607 pixels, whose int sums
+ * overflow in the reference, are refused.
+ */
+int vb200_hist_local(const VB200Image *in, VB200Image *out, int width, int height, int max_slope);
+/* test hooks, host only: histogram.cu's hist_local staging, window update and element arithmetic run tile by tile on the
+ * CPU (packed uchar arrays; staged -1: as planned, 0 / 1: forced), and hist_equal's LUT from an n_bands x width uint32
+ * histogram (band-major) into n_bands x width entries of band_format (uchar or ushort)
+ */
+int vb200_debug_hist_local_host(const void *in, int width, int height, int bands, int window_width, int window_height,
+	int max_slope, int staged, void *out);
+int vb200_debug_hist_equal_lut_host(const unsigned *hist, int width, int n_bands, int band_format, void *lut);
+
 /* ------------------------------------------------- unfused graphs: the chain pump (SURVEY 8f rank 2)
  *
  * What vips_sink_memory + vips_threadpool_run (iofuncs/sinkmemory.c:324, threadpool.c:625) do for an
@@ -481,6 +507,9 @@ int vb200_chain_add_unpremultiply(VB200Chain *chain, double max_alpha, int uchar
 int vb200_chain_add_morph(VB200Chain *chain, const VB200Mask *mask, int morph);
 int vb200_chain_add_rank(VB200Chain *chain, int width, int height, int index);
 int vb200_chain_add_flatten(VB200Chain *chain, const double *background, int n, double max_alpha);
+int vb200_chain_add_hist_find(VB200Chain *chain, int band);
+int vb200_chain_add_hist_equal(VB200Chain *chain, int band);
+int vb200_chain_add_hist_local(VB200Chain *chain, int width, int height, int max_slope);
 int vb200_chain_run_host(VB200Chain *chain, const VB200Image *in, VB200Image *out, int n_images);
 
 /* ------------------------------------------------------------------ ICC (SURVEY 8a a20)

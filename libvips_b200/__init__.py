@@ -27,7 +27,7 @@ SIZES = {"both": 0, "up": 1, "down": 2, "force": 3}
 PRECISIONS = {"integer": 0, "float": 1, "approximate": 2}
 INTENTS = {"perceptual": 0, "relative": 1, "saturation": 2, "absolute": 3}
 PCS = {"lab": 0, "xyz": 1}
-INTERPRETATIONS = {"multiband": 0, "b-w": 1, "cmyk": 15, "xyz": 12, "lab": 13, "lch": 19, "labs": 21, "srgb": 22,
+INTERPRETATIONS = {"multiband": 0, "b-w": 1, "histogram": 10, "cmyk": 15, "xyz": 12, "lab": 13, "lch": 19, "labs": 21, "srgb": 22,
                    "yxy": 23, "rgb16": 25, "grey16": 26, "scrgb": 28, "hsv": 29}
 
 
@@ -259,6 +259,14 @@ def lib():
         L.vb200_median.argtypes = [IP, IP, C.c_int]
         L.vb200_chain_add_rank.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.vb200_debug_rank_host.argtypes = [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p]
+        L.vb200_hist_find.argtypes = [IP, IP, C.c_int]
+        L.vb200_hist_equal.argtypes = [IP, IP, C.c_int]
+        L.vb200_hist_local.argtypes = [IP, IP, C.c_int, C.c_int, C.c_int]
+        L.vb200_chain_add_hist_find.argtypes = [C.c_void_p, C.c_int]
+        L.vb200_chain_add_hist_equal.argtypes = [C.c_void_p, C.c_int]
+        L.vb200_chain_add_hist_local.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+        L.vb200_debug_hist_local_host.argtypes = [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p]
+        L.vb200_debug_hist_equal_lut_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
         L.vb200_chain_new.restype = C.c_void_p
         L.vb200_chain_free.argtypes = [C.c_void_p]
         L.vb200_chain_add_resize.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_double]
@@ -570,6 +578,20 @@ class Image:
 
     def median(self, size):
         return self._call(lib().vb200_median, int(size))
+
+    # ---- histograms
+    def hist_find(self, band=-1):
+        """vips_hist_find: the (mx + 1) x 1 uint32 histogram of every band (band=-1) or of one band, interpretation histogram"""
+        return self._call(lib().vb200_hist_find, int(band))
+
+    def hist_equal(self, band=-1):
+        """vips_hist_equal: equalise through the image's own cumulative histogram (band >= 0: that band's, for every band)"""
+        return self._call(lib().vb200_hist_equal, int(band))
+
+    def hist_local(self, width, height, max_slope=0):
+        """vips_hist_local: local equalisation over a width x height window; max_slope > 0 limits the contrast (CLAHE).  Any
+        max_slope >= 0 runs hist_local.c's arithmetic as written (the reference's argument range stops at 100)"""
+        return self._call(lib().vb200_hist_local, int(width), int(height), int(max_slope))
 
     # ---- savers
     def dzsave(self, basename=None, **options):
@@ -907,6 +929,32 @@ def rank_host_twin(a, width, height, index):
     _check(lib().vb200_debug_rank_host(a.ctypes.data_as(C.c_void_p), a.shape[1], a.shape[0], a.shape[2], FORMATS[a.dtype], int(width),
                                        int(height), int(index), out.ctypes.data_as(C.c_void_p)))
     return out
+
+
+def hist_local_host_twin(a, width, height, max_slope=0, staged=None):
+    """histogram.cu's hist_local staging, window update and element arithmetic compiled for the host
+    (vb200_debug_hist_local_host): what the CPU tests pin to hist_local.c.  staged: None as planned, else forced on / off"""
+    a = np.ascontiguousarray(a, np.uint8)
+    if a.ndim == 2:
+        a = a[:, :, None]
+    out = np.empty_like(a)
+    _check(lib().vb200_debug_hist_local_host(a.ctypes.data_as(C.c_void_p), a.shape[1], a.shape[0], a.shape[2], int(width), int(height),
+                                             int(max_slope), -1 if staged is None else int(bool(staged)),
+                                             out.ctypes.data_as(C.c_void_p)))
+    return out
+
+
+def hist_equal_lut_host_twin(hist, dtype):
+    """hist_equal's LUT from a (width, n_bands) uint32 histogram, through histogram.cu's per-entry arithmetic compiled for the
+    host (vb200_debug_hist_equal_lut_host) -> (width, n_bands) array of dtype (uint8 or uint16)"""
+    h = np.asarray(hist, np.uint32)
+    if h.ndim == 1:
+        h = h[:, None]
+    band_major = np.ascontiguousarray(h.T)
+    lut = np.empty(band_major.shape, np.dtype(dtype))
+    _check(lib().vb200_debug_hist_equal_lut_host(band_major.ctypes.data_as(C.c_void_p), h.shape[0], h.shape[1], FORMATS[np.dtype(dtype)],
+                                                 lut.ctypes.data_as(C.c_void_p)))
+    return np.ascontiguousarray(lut.T)
 
 
 def hsv_host_twin(a, to_hsv):
@@ -1440,6 +1488,18 @@ class Chain:
 
     def rank(self, width, height, index):
         _check(lib().vb200_chain_add_rank(self._p, int(width), int(height), int(index)))
+        return self
+
+    def hist_find(self, band=-1):
+        _check(lib().vb200_chain_add_hist_find(self._p, int(band)))
+        return self
+
+    def hist_equal(self, band=-1):
+        _check(lib().vb200_chain_add_hist_equal(self._p, int(band)))
+        return self
+
+    def hist_local(self, width, height, max_slope=0):
+        _check(lib().vb200_chain_add_hist_local(self._p, int(width), int(height), int(max_slope)))
         return self
 
     def gaussblur(self, sigma, min_ampl=0.2, precision="integer"):

@@ -22,7 +22,7 @@ namespace {
 
 enum ImageOpKind {
 	OP_SHRINKV, OP_SHRINKH, OP_REDUCEV, OP_REDUCEH, OP_REDUCE, OP_RESIZE, OP_PREMULTIPLY, OP_UNPREMULTIPLY, OP_CONV, OP_CONVSEP,
-	OP_GAUSSBLUR, OP_SHARPEN, OP_COLOURSPACE, OP_FLATTEN, OP_MORPH, OP_RANK
+	OP_GAUSSBLUR, OP_SHARPEN, OP_COLOURSPACE, OP_FLATTEN, OP_MORPH, OP_RANK, OP_HIST_FIND, OP_HIST_EQUAL, OP_HIST_LOCAL
 };
 
 /* One op with its arguments, defaults applied.  Each kind reads the fields named beside it. */
@@ -44,7 +44,9 @@ struct ImageOp {
 	double x1 = 0, y2 = 0, y3 = 0, m1 = 0, m2 = 0; /* sharpen */
 	int space = 0;								   /* colourspace */
 	std::vector<double> background;				   /* flatten: none if empty */
-	int width = 0, height = 0, index = 0;		   /* rank */
+	int width = 0, height = 0, index = 0;		   /* rank; hist_local's window */
+	int band = -1;								   /* hist_find, hist_equal */
+	int max_slope = 0;							   /* hist_local */
 };
 
 /* ------------------------------------------------------------------ constructors */
@@ -184,6 +186,29 @@ op_rank(int width, int height, int index)
 	return op;
 }
 
+/* hist_find and hist_equal: band -1 (every band) or the band to scan, checked against the image (vips_check_bandno) */
+ImageOp
+op_hist(ImageOpKind kind, int band)
+{
+	ImageOp op;
+	op.kind = kind;
+	op.band = band;
+	return op;
+}
+
+/* hist_local.c:283-306; the window's area is bounded so that the int sums cannot overflow */
+int
+op_hist_local(const char *domain, int width, int height, int max_slope, ImageOp *op)
+{
+	if (hist_local_check(domain, width, height, max_slope))
+		return -1;
+	op->kind = OP_HIST_LOCAL;
+	op->width = width;
+	op->height = height;
+	op->max_slope = max_slope;
+	return 0;
+}
+
 /* ------------------------------------------------------------------ dispatch */
 
 int
@@ -232,6 +257,12 @@ image_op_apply(const char *domain, const ImageOp &op, const DevImage &in, DevIma
 		return dev_morph(domain, in, out, op.mask.data(), op.mw, op.mh, op.morph, s);
 	case OP_RANK:
 		return dev_rank(domain, in, out, op.width, op.height, op.index, s);
+	case OP_HIST_FIND:
+		return dev_hist_find(domain, in, out, op.band, s);
+	case OP_HIST_EQUAL:
+		return dev_hist_equal(domain, in, out, op.band, s);
+	case OP_HIST_LOCAL:
+		return dev_hist_local(domain, in, out, op.width, op.height, op.max_slope, s);
 	}
 	return -1;
 }
@@ -268,6 +299,10 @@ run_op(const char *domain, const ImageOp &op, const VB200Image *in, VB200Image *
 	return run_image(domain, in, out,
 		[&](size_t *line) {
 			*line = preset_line(op, *in);
+			/* the histogram ops refuse a band, format or window that the descriptor rules out before the upload */
+			if (op.kind == OP_HIST_FIND || op.kind == OP_HIST_EQUAL || op.kind == OP_HIST_LOCAL)
+				return hist_refuse(domain, op.kind - OP_HIST_FIND, in->Xsize, in->Ysize, in->Bands, in->BandFmt, op.band, op.width,
+					op.height);
 			return 0;
 		},
 		[&](const DevImage &d, DevImage *o, cudaStream_t s) { return image_op_apply(domain, op, d, o, s); });
@@ -419,6 +454,28 @@ vb200_median(const VB200Image *in, VB200Image *out, int size)
 	return run_op("rank", op_rank(size, size, (size * size) / 2), in, out);
 }
 
+/* reference: vips_hist_find(), arithmetic/hist_find.c:471-482 */
+extern "C" int
+vb200_hist_find(const VB200Image *in, VB200Image *out, int band)
+{
+	return run_op("hist_find", op_hist(OP_HIST_FIND, band), in, out);
+}
+
+/* reference: vips_hist_equal(), histogram/hist_equal.c:156-167 */
+extern "C" int
+vb200_hist_equal(const VB200Image *in, VB200Image *out, int band)
+{
+	return run_op("hist_equal", op_hist(OP_HIST_EQUAL, band), in, out);
+}
+
+/* reference: vips_hist_local(), histogram/hist_local.c:417-428 */
+extern "C" int
+vb200_hist_local(const VB200Image *in, VB200Image *out, int width, int height, int max_slope)
+{
+	ImageOp op;
+	return op_hist_local("hist_local", width, height, max_slope, &op) ? -1 : run_op("hist_local", op, in, out);
+}
+
 /* ------------------------------------------------------------------ the chain pump */
 
 namespace {
@@ -539,6 +596,25 @@ extern "C" int
 vb200_chain_add_unpremultiply(VB200Chain *chain, double max_alpha, int uchar_mode)
 {
 	return chain_push(chain, op_premultiply(OP_UNPREMULTIPLY, max_alpha, uchar_mode));
+}
+
+extern "C" int
+vb200_chain_add_hist_find(VB200Chain *chain, int band)
+{
+	return chain_push(chain, op_hist(OP_HIST_FIND, band));
+}
+
+extern "C" int
+vb200_chain_add_hist_equal(VB200Chain *chain, int band)
+{
+	return chain_push(chain, op_hist(OP_HIST_EQUAL, band));
+}
+
+extern "C" int
+vb200_chain_add_hist_local(VB200Chain *chain, int width, int height, int max_slope)
+{
+	ImageOp op;
+	return op_hist_local("chain", width, height, max_slope, &op) ? -1 : chain_push(chain, std::move(op));
 }
 
 /* in[i]: host images (pinned memory lets the three phases overlap; pageable memory is correct but its

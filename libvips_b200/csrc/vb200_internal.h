@@ -199,6 +199,13 @@ int dev_flatten(const char *domain, const DevImage &in, DevImage *out, const dou
 
 /* rank.cu */
 int dev_rank(const char *domain, const DevImage &in, DevImage *out, int width, int height, int index, cudaStream_t s);
+/* histogram.cu: vips_hist_find, vips_hist_equal, vips_hist_local */
+int dev_hist_find(const char *domain, const DevImage &in, DevImage *out, int band, cudaStream_t s);
+int dev_hist_equal(const char *domain, const DevImage &in, DevImage *out, int band, cudaStream_t s);
+int dev_hist_local(const char *domain, const DevImage &in, DevImage *out, int width, int height, int max_slope, cudaStream_t s);
+int hist_local_check(const char *domain, int width, int height, int max_slope);
+/* kind 0 hist_find, 1 hist_equal, 2 hist_local: the refusals that need in's descriptor and no pixels */
+int hist_refuse(const char *domain, int kind, int w, int h, int bands, int fmt, int band, int width, int height);
 
 /* colour.cu */
 int dev_colourspace(const char *domain, const DevImage &in, DevImage *out, int space, int source_space,
