@@ -92,14 +92,14 @@ def _embedded_arrays(embedded, n):
     return keep, ptrs, lens
 
 
-def _icc_blob(fn, stream):
+def _icc_blob(fn, stream, *opts):
     stream = bytes(stream)
     n = C.c_size_t()
-    _check(fn(stream, len(stream), None, 0, C.byref(n)))
+    _check(fn(stream, len(stream), *opts, None, 0, C.byref(n)))
     if n.value == 0:
         return None
     out = C.create_string_buffer(n.value)
-    _check(fn(stream, len(stream), out, n.value, C.byref(n)))
+    _check(fn(stream, len(stream), *opts, out, n.value, C.byref(n)))
     return out.raw[:n.value]
 
 
@@ -460,12 +460,21 @@ class Image:
 
     @staticmethod
     def _take(cout):
-        n = cout.Ysize * cout.bpl
-        buf = (C.c_uint8 * n).from_address(cout.data)
-        dt = DTYPES[cout.BandFmt]
-        arr = np.frombuffer(buf, dtype=dt).reshape(cout.Ysize, cout.Xsize, cout.Bands).copy()
+        dt = np.dtype(DTYPES[cout.BandFmt])
+        buf = (C.c_uint8 * (cout.Ysize * cout.bpl)).from_address(cout.data)
+        rows = np.frombuffer(buf, np.uint8).reshape(cout.Ysize, cout.bpl)[:, :cout.Xsize * cout.Bands * dt.itemsize]
+        arr = rows.copy().view(dt).reshape(cout.Ysize, cout.Xsize, cout.Bands)
         lib().vb200_image_free(C.byref(cout))
         return Image(arr, cout.Type)
+
+    @staticmethod
+    def _load_buffer(fn, stream, *opts):
+        """fn(stream, len, *opts, &out) of a vb200_*load_buffer, delivered to host memory -> Image"""
+        stream = bytes(stream)
+        out = CImage()
+        out.where = HOST
+        _check(fn(stream, len(stream), *opts, C.byref(out)))
+        return Image._take(out)
 
     # ---- resample
     def shrinkv(self, vshrink, ceil=False):
@@ -619,28 +628,16 @@ class Image:
     def tiffload_buffer(stream, page=0, n=1, subifd=-1):
         """vips_tiffload_buffer(stream, page=page, n=n, subifd=subifd): the strips or tiles decoded on the device -> Image (uint8,
         B_W below 3 bands, sRGB from 3), with page_height set when more than one page loaded"""
-        stream = bytes(stream)
-        out = CImage()
-        out.where = HOST
-        _check(lib().vb200_tiffload_buffer(stream, len(stream), int(page), int(n), int(subifd), C.byref(out)))
-        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
-        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
-        lib().vb200_image_free(C.byref(out))
+        img = Image._load_buffer(lib().vb200_tiffload_buffer, stream, int(page), int(n), int(subifd))
         page_h = tiff_geometry(stream, page, subifd)[1]
-        return Image(a, "b-w" if a.shape[2] < 3 else "srgb", page_height=page_h if a.shape[0] > page_h else None)
+        img.page_height = page_h if img.height > page_h else None
+        return img
 
     @staticmethod
     def webpload_buffer(stream):
         """vips_webpload_buffer(stream) of a lossy, still, opaque WebP: the frame decoded on the device -> Image (uint8, 3 bands,
         sRGB)"""
-        stream = bytes(stream)
-        out = CImage()
-        out.where = HOST
-        _check(lib().vb200_webpload_buffer(stream, len(stream), C.byref(out)))
-        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
-        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
-        lib().vb200_image_free(C.byref(out))
-        return Image(a, "srgb")
+        return Image._load_buffer(lib().vb200_webpload_buffer, stream)
 
     # ---- colour
     @staticmethod
@@ -648,15 +645,10 @@ class Image:
         """vips_gifload_buffer(stream, page=page, n=n): the pages decoded on the device (n = -1: every page from `page` on),
         stacked vertically as libvips does -> Image (uint8, 3 or 4 bands), with page_height the screen height when more than
         one page loaded (nsgifload.c:279-280)"""
-        stream = bytes(stream)
-        out = CImage()
-        out.where = HOST
-        _check(lib().vb200_gifload_buffer(stream, len(stream), int(page), int(n), C.byref(out)))
-        a = np.frombuffer(C.string_at(out.data, out.Ysize * out.bpl), np.uint8).reshape(out.Ysize, out.bpl)[:, :out.Xsize * out.Bands]
-        a = a.reshape(out.Ysize, out.Xsize, out.Bands).copy()
-        lib().vb200_image_free(C.byref(out))
+        img = Image._load_buffer(lib().vb200_gifload_buffer, stream, int(page), int(n))
         screen_h = gif_geometry(stream)[1]
-        return Image(a, "srgb", page_height=screen_h if a.shape[0] > screen_h else None)
+        img.page_height = screen_h if img.height > screen_h else None
+        return img
 
     def colourspace(self, space, source_space=None):
         src = self if source_space is None else Image(self.array, source_space)
@@ -722,15 +714,20 @@ def jpeg_decode_batch(streams, shrink=1, out_ptr=None):
     return _decode_batch(lib().vb200_jpeg_decode_batch, streams, (int(shrink),), out_ptr)
 
 
-def jpeg_decode_host_twin(stream, shrink=1):
-    """the decoder's per-block code compiled for the host (vb200_debug_jpeg_decode): what the CPU tests pin to libjpeg-turbo"""
+def _host_twin(fn, stream, *opts):
+    """fn(stream, len, *opts, out, out_bpl, &w, &h, &bands) of a vb200_debug_*_decode: the geometry, then the pixels -> uint8
+    [h, w, bands]"""
     stream = bytes(stream)
     w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_debug_jpeg_decode(stream, len(stream), int(shrink), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
+    _check(fn(stream, len(stream), *opts, None, 0, C.byref(w), C.byref(h), C.byref(bands)))
     out = np.empty((h.value, w.value, bands.value), np.uint8)
-    _check(lib().vb200_debug_jpeg_decode(stream, len(stream), int(shrink), out.ctypes.data_as(C.c_void_p), w.value * bands.value,
-                                         C.byref(w), C.byref(h), C.byref(bands)))
+    _check(fn(stream, len(stream), *opts, out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w), C.byref(h), C.byref(bands)))
     return out
+
+
+def jpeg_decode_host_twin(stream, shrink=1):
+    """the decoder's per-block code compiled for the host (vb200_debug_jpeg_decode): what the CPU tests pin to libjpeg-turbo"""
+    return _host_twin(lib().vb200_debug_jpeg_decode, stream, int(shrink))
 
 
 def png_geometry(streams):
@@ -747,13 +744,7 @@ def png_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None)
 def png_decode_host_twin(stream):
     """the decoder's per-symbol / per-byte / per-pixel code compiled for the host (vb200_debug_png_decode): what the CPU tests
     pin to Pillow and zlib"""
-    stream = bytes(stream)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_debug_png_decode(stream, len(stream), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
-    out = np.empty((h.value, w.value, bands.value), np.uint8)
-    _check(lib().vb200_debug_png_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
-                                        C.byref(h), C.byref(bands)))
-    return out
+    return _host_twin(lib().vb200_debug_png_decode, stream)
 
 
 def webp_geometry(stream):
@@ -773,13 +764,7 @@ def webp_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None
 def webp_decode_host_twin(stream):
     """the decoder's per-symbol / per-block / per-pixel code compiled for the host (vb200_debug_webp_decode): what the CPU tests
     pin to libwebp"""
-    stream = bytes(stream)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_debug_webp_decode(stream, len(stream), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
-    out = np.empty((h.value, w.value, bands.value), np.uint8)
-    _check(lib().vb200_debug_webp_decode(stream, len(stream), out.ctypes.data_as(C.c_void_p), w.value * bands.value, C.byref(w),
-                                         C.byref(h), C.byref(bands)))
-    return out
+    return _host_twin(lib().vb200_debug_webp_decode, stream)
 
 
 def webp_times():
@@ -820,13 +805,7 @@ def gif_decode_batch(streams, page=0, n=1, out_ptr=None, out_bpl=None, out_frame
 def gif_decode_host_twin(stream, page=0, n=1):
     """the decoder's per-code / per-pixel code compiled for the host (vb200_debug_gif_decode): what the CPU tests pin to
     libnsgif -> uint8 [h * pages, w, bands]"""
-    stream = bytes(stream)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_debug_gif_decode(stream, len(stream), int(page), int(n), None, 0, C.byref(w), C.byref(h), C.byref(bands)))
-    out = np.empty((h.value, w.value, bands.value), np.uint8)
-    _check(lib().vb200_debug_gif_decode(stream, len(stream), int(page), int(n), out.ctypes.data_as(C.c_void_p), w.value * bands.value,
-                                        C.byref(w), C.byref(h), C.byref(bands)))
-    return out
+    return _host_twin(lib().vb200_debug_gif_decode, stream, int(page), int(n))
 
 
 def tiff_geometry(stream, page=0, subifd=-1):
@@ -846,26 +825,12 @@ def tiff_decode_batch(streams, page=0, n=1, subifd=-1, out_ptr=None, out_bpl=Non
 
 def tiff_decode_host_twin(stream, page=0, n=1, subifd=-1):
     """the decoder's per-code / per-byte code compiled for the host (vb200_debug_tiff_decode) -> uint8 [h * pages, w, bands]"""
-    stream = bytes(stream)
-    w, h, bands = C.c_int(), C.c_int(), C.c_int()
-    _check(lib().vb200_debug_tiff_decode(stream, len(stream), int(page), int(n), int(subifd), None, 0, C.byref(w), C.byref(h),
-                                         C.byref(bands)))
-    out = np.empty((h.value, w.value, bands.value), np.uint8)
-    _check(lib().vb200_debug_tiff_decode(stream, len(stream), int(page), int(n), int(subifd), out.ctypes.data_as(C.c_void_p),
-                                         w.value * bands.value, C.byref(w), C.byref(h), C.byref(bands)))
-    return out
+    return _host_twin(lib().vb200_debug_tiff_decode, stream, int(page), int(n), int(subifd))
 
 
 def tiff_icc_profile(stream, page=0, subifd=-1):
     """the ICCProfile tag of the TIFF IFD page / subifd select (bytes, or None)"""
-    stream = bytes(stream)
-    n = C.c_size_t()
-    _check(lib().vb200_tiff_icc_profile(stream, len(stream), int(page), int(subifd), None, 0, C.byref(n)))
-    if n.value == 0:
-        return None
-    buf = C.create_string_buffer(n.value)
-    _check(lib().vb200_tiff_icc_profile(stream, len(stream), int(page), int(subifd), buf, n.value, C.byref(n)))
-    return buf.raw[:n.value]
+    return _icc_blob(lib().vb200_tiff_icc_profile, stream, int(page), int(subifd))
 
 
 def tiff_lzw_host_twin(data, want):

@@ -1,9 +1,11 @@
 /* decode.cu -- what the JPEG, PNG, GIF, TIFF and WebP decoders share around their kernels: the stream kinds and the one switch over
- * the three batch decoders, the C ABI bodies of vb200_*_decode_batch and vb200_*load_buffer, the host-worker header pass,
- * and (for PNG, GIF, TIFF and WebP) the pinned staging block and the chunks bounded by the device budget.
+ * the five batch decoders, the C ABI bodies of vb200_*_decode_batch, vb200_*load_buffer, vb200_*_icc_profile and the host-twin
+ * hooks, the host-worker header pass, and (for PNG, GIF, TIFF and WebP) the pinned staging block, the chunks bounded by the
+ * device budget and the one body every such chunk runs.
  */
 #include <cstdint>
 #include <cstring>
+#include <exception>
 #include <mutex>
 #include <string>
 
@@ -91,7 +93,7 @@ check_out_strides(const char *domain, const StreamGeometry &g, size_t out_bpl, s
 	return 0;
 }
 
-/* device bytes per chunk of the PNG and GIF decoders and the JPEG and PNG encoders */
+/* device bytes per chunk of the PNG, GIF, TIFF and WebP decoders and the JPEG and PNG encoders */
 size_t
 chunk_budget()
 {
@@ -105,7 +107,8 @@ chunk_budget()
 }
 
 int
-decode_chunks(const char *domain, const char *noun, int n, const std::function<size_t(int)> &device_bytes, const std::function<int(int, int)> &chunk)
+decode_chunks(const char *domain, const char *what, const char *noun, int n, const std::function<size_t(int)> &device_bytes,
+	const std::function<int(int, int)> &chunk, cudaStream_t s)
 {
 	const size_t budget = chunk_budget();
 	std::lock_guard<std::mutex> lock(g_staging_lock);
@@ -128,7 +131,94 @@ decode_chunks(const char *domain, const char *noun, int n, const std::function<s
 			return -1;
 		c0 += cn;
 	}
+	if (cudaStreamSynchronize(s) != cudaSuccess)
+		return cuda_fail(domain, cudaGetLastError(), (std::string(what) + " decode").c_str());
 	return 0;
+}
+
+int
+decode_chunk(const char *domain, const char *what, const DecodeBlock &b, const std::function<void(unsigned char *)> &stage,
+	const std::function<int(unsigned char *, int *)> &decode, const std::function<void(int, int)> &refuse,
+	const std::function<int(unsigned char *)> &place, cudaStream_t s)
+{
+	/* the previous chunk's copy out of the pinned block has finished: its status was read after it */
+	unsigned char *hst = (unsigned char *) decode_staging(domain, b.host_bytes);
+	if (!hst)
+		return -1;
+	stage(hst);
+	const size_t off_status = align16(b.host_bytes) + align16(b.scratch_bytes);
+	unsigned char *dev = nullptr;
+	if (dev_alloc(domain, (void **) &dev, off_status + b.n_status * sizeof(int), s))
+		return -1;
+	int *status = (int *) (dev + off_status);
+	std::vector<int> st(b.n_status, 0);
+	const std::string label = what;
+	int rc = 0;
+	if (cudaMemcpyAsync(dev, hst, b.host_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+		cudaMemsetAsync(status, 0, b.n_status * sizeof(int), s) != cudaSuccess)
+		rc = cuda_fail(domain, cudaGetLastError(), (label + " staging copy").c_str());
+	else {
+		const int launched = decode(dev, status);
+		count_launch(std::max(launched, 0));
+		/* a decode that failed has its reason set; its launches still finish before the block is freed */
+		const cudaError_t e = cudaGetLastError();
+		const bool failed = e != cudaSuccess || cudaMemcpyAsync(st.data(), status, b.n_status * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+							cudaStreamSynchronize(s) != cudaSuccess;
+		if (launched < 0)
+			rc = -1;
+		else if (failed)
+			rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), (label + " decode kernels").c_str());
+	}
+	for (int k = 0; k < b.n_status && !rc; k++)
+		if (st[k]) {
+			refuse(k, st[k]);
+			rc = -1;
+		}
+	if (!rc) {
+		const int launched = place(dev);
+		count_launch(std::max(launched, 0));
+		const cudaError_t e = cudaGetLastError();
+		if (launched < 0)
+			rc = -1;
+		else if (e != cudaSuccess)
+			rc = cuda_fail(domain, e, (label + " placement").c_str());
+	}
+	dev_free(dev, s);
+	return rc;
+}
+
+int
+profile_abi(const char *domain, void *out, size_t cap, size_t *profile_len, const std::function<int(const char *, std::vector<unsigned char> *)> &fetch)
+{
+	if (!profile_len) {
+		error(domain, "null argument");
+		return -1;
+	}
+	std::vector<unsigned char> prof;
+	if (fetch(domain, &prof))
+		return -1;
+	*profile_len = prof.size();
+	if (!out)
+		return 0;
+	if (cap < prof.size()) {
+		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
+		return -1;
+	}
+	if (!prof.empty())
+		memcpy(out, prof.data(), prof.size());
+	return 0;
+}
+
+int
+host_twin_abi(const char *domain, const std::function<int(const char *)> &fn)
+{
+	try {
+		return fn(domain);
+	}
+	catch (const std::exception &e) {
+		error(domain, "%s", e.what());
+		return -1;
+	}
 }
 
 void *

@@ -730,10 +730,8 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		return -1;
 	const int W = g->w, H = g->h, B = g->bands;
 	const int nf_stream = page + g->pages; /* frames 0 .. page + n - 1 of every stream */
-	int rc = decode_chunks(domain, "stream", n, [&](int i) { return stream_device_bytes(info[i], nf_stream); }, [&](int c0, int cn) {
-		/* records and offsets: the pinned block holds stream records, frame records, tables and payloads; the device the
-		 * same, then the index planes, counts and status words
-		 */
+	return decode_chunks(domain, "gif", "stream", n, [&](int i) { return stream_device_bytes(info[i], nf_stream); }, [&](int c0, int cn) {
+		/* the block: stream records, frame records, tables and payloads staged; the index planes and counts as scratch */
 		const int nf = cn * nf_stream;
 		std::vector<GifStreamDev> S(cn);
 		std::vector<GifFrameDev> F(nf);
@@ -755,61 +753,33 @@ dev_gif_decode_batch(const char *domain, const void *const *bufs, const size_t *
 		}
 		const size_t off_fr = align16(cn * sizeof(GifStreamDev)), off_pal = off_fr + align16(nf * sizeof(GifFrameDev)),
 					 off_data = off_pal + (size_t) nf * 1024, total = off_data + data;
-		/* the previous chunk's copy out of the block has finished: its status was read after it */
-		unsigned char *hst = (unsigned char *) decode_staging(domain, total);
-		if (!hst)
-			return -1;
-		memcpy(hst, S.data(), cn * sizeof(GifStreamDev));
-		memcpy(hst + off_fr, F.data(), nf * sizeof(GifFrameDev));
-		parallel_for(cn, host_workers(), [&](int i) {
-			const GifInfo &G = info[c0 + i];
-			stage_palettes(G, nf_stream, (unsigned *) (hst + off_pal) + (size_t) S[i].f0 * 256);
-			for (int k = 0; k < nf_stream; k++)
-				stage_lzw(G, k, hst + off_data + F[S[i].f0 + k].data_off);
-		});
-		const size_t off_planes = align16(total), off_counts = off_planes + align16(planes), off_status = off_counts + align16(nf * sizeof(unsigned));
-		void *dev = nullptr;
-		if (dev_alloc(domain, &dev, off_status + nf * sizeof(int), s))
-			return -1;
-		unsigned char *dv = (unsigned char *) dev;
-		const GifStreamDev *dS = (const GifStreamDev *) dv;
-		const GifFrameDev *dF = (const GifFrameDev *) (dv + off_fr);
-		const unsigned *dP = (const unsigned *) (dv + off_pal);
-		const unsigned char *dB = dv + off_data;
-		unsigned char *dI = dv + off_planes;
-		unsigned *dC = (unsigned *) (dv + off_counts);
-		int *dSt = (int *) (dv + off_status);
-		std::vector<int> st(nf, 0);
-		int rc = 0;
-		if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaMemsetAsync(dSt, 0, nf * sizeof(int), s) != cudaSuccess)
-			rc = cuda_fail(domain, cudaGetLastError(), "gif staging copy");
-		else {
-			gif_lzw_kernel<<<std::min(nf, sm_count() * 16), 32, 0, s>>>(dF, nf, dB, dI, dC, dSt);
-			count_launch(1);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess || cudaMemcpyAsync(st.data(), dSt, nf * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-				cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "gif_lzw_kernel");
-		}
-		for (int i = 0; i < nf && !rc; i++)
-			if (st[i]) {
-				error(domain, "stream %d: frame %d: bad LZW code (libnsgif: Invalid frame data)", c0 + i / nf_stream, i % nf_stream);
-				rc = -1;
-			}
-		if (!rc) {
-			gif_compose_kernel<<<dim3((W + 255) / 256, std::min(H, kMaxGridY), cn), 256, 0, s>>>(dF, dS, dC, dI, dP, W, H, B,
-				(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
-			count_launch(1);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess)
-				rc = cuda_fail(domain, e, "gif_compose_kernel");
-		}
-		dev_free(dev, s);
-		return rc;
-	});
-	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "gif decode");
-	return rc;
+		const size_t off_planes = align16(total), off_counts = off_planes + align16(planes);
+		return decode_chunk(
+			domain, "gif", {total, align16(planes) + nf * sizeof(unsigned), nf},
+			[&](unsigned char *hst) {
+				memcpy(hst, S.data(), cn * sizeof(GifStreamDev));
+				memcpy(hst + off_fr, F.data(), nf * sizeof(GifFrameDev));
+				parallel_for(cn, host_workers(), [&](int i) {
+					const GifInfo &G = info[c0 + i];
+					stage_palettes(G, nf_stream, (unsigned *) (hst + off_pal) + (size_t) S[i].f0 * 256);
+					for (int k = 0; k < nf_stream; k++)
+						stage_lzw(G, k, hst + off_data + F[S[i].f0 + k].data_off);
+				});
+			},
+			[&](unsigned char *dev, int *status) {
+				gif_lzw_kernel<<<std::min(nf, sm_count() * 16), 32, 0, s>>>((const GifFrameDev *) (dev + off_fr), nf, dev + off_data, dev + off_planes,
+					(unsigned *) (dev + off_counts), status);
+				return 1;
+			},
+			[&](int i, int) { error(domain, "stream %d: frame %d: bad LZW code (libnsgif: Invalid frame data)", c0 + i / nf_stream, i % nf_stream); },
+			[&](unsigned char *dev) {
+				gif_compose_kernel<<<dim3((W + 255) / 256, std::min(H, kMaxGridY), cn), 256, 0, s>>>((const GifFrameDev *) (dev + off_fr),
+					(const GifStreamDev *) dev, (const unsigned *) (dev + off_counts), dev + off_planes, (const unsigned *) (dev + off_pal), W, H, B,
+					(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
+				return 1;
+			},
+			s);
+	}, s);
 }
 
 /* the same decode on the CPU through the same per-code and per-pixel code: the test-suite's host twin */
@@ -907,13 +877,8 @@ vb200_gifload_buffer(const void *buf, size_t len, int page, int n, VB200Image *o
 extern "C" int
 vb200_debug_gif_decode(const void *buf, size_t len, int page, int n, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
-	try {
-		return host_gif_decode("gif_decode (host twin)", buf, len, page, n, (unsigned char *) out, out_bpl, width, height, bands);
-	}
-	catch (const std::exception &e) {
-		error("gif_decode (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("gif_decode (host twin)",
+		[&](const char *domain) { return host_gif_decode(domain, buf, len, page, n, (unsigned char *) out, out_bpl, width, height, bands); });
 }
 
 /* LZW data (sub-blocks already joined) through the host twin's decoder: 0 and *out_len values (at most want), or -1 for

@@ -2555,13 +2555,9 @@ vb200_debug_jpeg_times(float *huffman_ms, float *idct_ms)
 extern "C" int
 vb200_debug_jpeg_decode(const void *buf, size_t len, int shrink, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
-	try {
-		return host_jpeg_decode("jpeg_decode (host twin)", buf, len, shrink, (unsigned char *) out, out_bpl, width, height, bands, 0, 0, nullptr);
-	}
-	catch (const std::exception &e) {
-		error("jpeg_decode (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("jpeg_decode (host twin)", [&](const char *domain) {
+		return host_jpeg_decode(domain, buf, len, shrink, (unsigned char *) out, out_bpl, width, height, bands, 0, 0, nullptr);
+	});
 }
 
 /* the host twin of the self-synchronising path: subsequences of sub_bytes, max_passes passes; *passes_used = the last pass
@@ -2624,22 +2620,6 @@ jpeg_icc_profile(const char *domain, const unsigned char *d, size_t len, std::ve
 extern "C" int
 vb200_jpeg_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len)
 {
-	const char *domain = "jpeg_icc_profile";
-	if (!profile_len) {
-		error(domain, "null argument");
-		return -1;
-	}
-	std::vector<unsigned char> prof;
-	if (jpeg_icc_profile(domain, (const unsigned char *) buf, len, &prof))
-		return -1;
-	*profile_len = prof.size();
-	if (!out)
-		return 0;
-	if (cap < prof.size()) {
-		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
-		return -1;
-	}
-	if (!prof.empty())
-		memcpy(out, prof.data(), prof.size());
-	return 0;
+	return profile_abi("jpeg_icc_profile", out, cap, profile_len,
+		[&](const char *domain, std::vector<unsigned char> *prof) { return jpeg_icc_profile(domain, (const unsigned char *) buf, len, prof); });
 }

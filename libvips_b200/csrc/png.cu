@@ -569,8 +569,8 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 	if (check_out_strides(domain, *g, out_bpl, out_frame_stride))
 		return -1;
 	const int W = g->w, Hh = g->h;
-	int rc = decode_chunks(domain, "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
-		/* the pinned block: records, palettes, deflate bytes; the device: the same, then the scanlines */
+	return decode_chunks(domain, "png", "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
+		/* the block: records, palettes, deflate bytes staged; the scanlines as scratch */
 		std::vector<PngFrameDev> F(cn);
 		size_t n_pal = 0, data = 0, scan = 0;
 		for (int i = 0; i < cn; i++) {
@@ -584,74 +584,45 @@ dev_png_decode_batch(const char *domain, const void *const *bufs, const size_t *
 			scan += align16(scan_bytes(H));
 		}
 		const size_t off_pal = align16(cn * sizeof(PngFrameDev)), off_data = off_pal + n_pal * 1024, total = off_data + data;
-		/* the previous chunk's copy out of the block has finished: its status was read after it */
-		unsigned char *hst = (unsigned char *) decode_staging(domain, total);
-		if (!hst)
-			return -1;
-		memcpy(hst, F.data(), cn * sizeof(PngFrameDev));
-		parallel_for(cn, host_workers(), [&](int i) {
-			const PngHeader &H = hdr[c0 + i];
-			if (F[i].pal_off >= 0)
-				memcpy(hst + off_pal + (size_t) F[i].pal_off * 1024, H.pal, 1024);
-			stage_idat(H, hst + off_data + F[i].data_off);
-		});
-		void *dev = nullptr;
-		int *status = nullptr;
-		if (dev_alloc(domain, &dev, total + scan, s))
-			return -1;
-		if (dev_alloc(domain, (void **) &status, cn * sizeof(int), s)) {
-			dev_free(dev, s);
-			return -1;
-		}
-		const PngFrameDev *dF = (const PngFrameDev *) dev;
-		const unsigned char *dP = (const unsigned char *) dev + off_pal, *dB = (const unsigned char *) dev + off_data;
-		unsigned char *dS = (unsigned char *) dev + total;
-		std::vector<int> st(cn, 0);
-		int rc = 0;
-		if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaMemsetAsync(status, 0, cn * sizeof(int), s) != cudaSuccess)
-			rc = cuda_fail(domain, cudaGetLastError(), "png staging copy");
-		else {
-			png_inflate_kernel<<<(cn + kInflateWarps - 1) / kInflateWarps, kInflateWarps * 32, 0, s>>>(dF, cn, dB, dS, status);
-			int launches = 1;
-			/* frames of one geometry may still differ in their filter unit (a palette frame's is 1 byte, an RGB frame's 3):
-			 * one launch per unit present, each skipping the others' frames
-			 */
-			bool unit[5] = {false, false, false, false, false};
-			for (const PngFrameDev &f : F)
-				unit[f.bpp] = true;
-			void (*const unfilter[5])(const PngFrameDev *, int, unsigned char *, int *) = {nullptr, png_unfilter_kernel<1>, png_unfilter_kernel<2>,
-				png_unfilter_kernel<3>, png_unfilter_kernel<4>};
-			for (int u = 1; u <= 4; u++)
-				if (unit[u]) {
-					unfilter[u]<<<cn, kUnfilterWarps * 32, 0, s>>>(dF, cn, dS, status);
-					launches++;
-				}
-			count_launch(launches);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess || cudaMemcpyAsync(st.data(), status, cn * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-				cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "png inflate / unfilter");
-		}
-		for (int i = 0; i < cn && !rc; i++)
-			if (st[i]) {
-				error(domain, "frame %d: %s", c0 + i, status_text(st[i]));
-				rc = -1;
-			}
-		if (!rc) {
-			png_expand_kernel<<<dim3((W + 255) / 256, std::min(Hh, kMaxGridY), cn), 256, 0, s>>>(dF, dS, dP,
-				(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
-			count_launch(1);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess)
-				rc = cuda_fail(domain, e, "png_expand_kernel");
-		}
-		dev_free(status, s);
-		dev_free(dev, s);
-		return rc;
-	});
-	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "png decode");
-	return rc;
+		return decode_chunk(
+			domain, "png", {total, scan, cn},
+			[&](unsigned char *hst) {
+				memcpy(hst, F.data(), cn * sizeof(PngFrameDev));
+				parallel_for(cn, host_workers(), [&](int i) {
+					const PngHeader &H = hdr[c0 + i];
+					if (F[i].pal_off >= 0)
+						memcpy(hst + off_pal + (size_t) F[i].pal_off * 1024, H.pal, 1024);
+					stage_idat(H, hst + off_data + F[i].data_off);
+				});
+			},
+			[&](unsigned char *dev, int *status) {
+				const PngFrameDev *dF = (const PngFrameDev *) dev;
+				png_inflate_kernel<<<(cn + kInflateWarps - 1) / kInflateWarps, kInflateWarps * 32, 0, s>>>(dF, cn, dev + off_data, dev + align16(total),
+					status);
+				int launches = 1;
+				/* frames of one geometry may still differ in their filter unit (a palette frame's is 1 byte, an RGB frame's 3):
+				 * one launch per unit present, each skipping the others' frames
+				 */
+				bool unit[5] = {false, false, false, false, false};
+				for (const PngFrameDev &f : F)
+					unit[f.bpp] = true;
+				void (*const unfilter[5])(const PngFrameDev *, int, unsigned char *, int *) = {nullptr, png_unfilter_kernel<1>, png_unfilter_kernel<2>,
+					png_unfilter_kernel<3>, png_unfilter_kernel<4>};
+				for (int u = 1; u <= 4; u++)
+					if (unit[u]) {
+						unfilter[u]<<<cn, kUnfilterWarps * 32, 0, s>>>(dF, cn, dev + align16(total), status);
+						launches++;
+					}
+				return launches;
+			},
+			[&](int i, int st) { error(domain, "frame %d: %s", c0 + i, status_text(st)); },
+			[&](unsigned char *dev) {
+				png_expand_kernel<<<dim3((W + 255) / 256, std::min(Hh, kMaxGridY), cn), 256, 0, s>>>((const PngFrameDev *) dev, dev + align16(total),
+					dev + off_pal, (unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
+				return 1;
+			},
+			s);
+	}, s);
 }
 
 /* the same decode on the CPU through the same per-symbol, per-byte and per-pixel code: the test-suite's host twin */
@@ -724,36 +695,15 @@ vb200_pngload_buffer(const void *buf, size_t len, VB200Image *out)
 extern "C" int
 vb200_png_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len)
 {
-	const char *domain = "png_icc_profile";
-	if (!profile_len) {
-		error(domain, "null argument");
-		return -1;
-	}
-	std::vector<unsigned char> prof;
-	if (png_icc_profile(domain, (const unsigned char *) buf, len, &prof, nullptr))
-		return -1;
-	*profile_len = prof.size();
-	if (!out)
-		return 0;
-	if (cap < prof.size()) {
-		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
-		return -1;
-	}
-	if (!prof.empty())
-		memcpy(out, prof.data(), prof.size());
-	return 0;
+	return profile_abi("png_icc_profile", out, cap, profile_len,
+		[&](const char *domain, std::vector<unsigned char> *prof) { return png_icc_profile(domain, (const unsigned char *) buf, len, prof, nullptr); });
 }
 
 extern "C" int
 vb200_debug_png_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
-	try {
-		return host_png_decode("png_decode (host twin)", buf, len, (unsigned char *) out, out_bpl, width, height, bands);
-	}
-	catch (const std::exception &e) {
-		error("png_decode (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("png_decode (host twin)",
+		[&](const char *domain) { return host_png_decode(domain, buf, len, (unsigned char *) out, out_bpl, width, height, bands); });
 }
 
 /* raw deflate data (no zlib header) through the host twin's inflate: 0 and *out_len bytes, or -1 (refused, or more than

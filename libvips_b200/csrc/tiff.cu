@@ -1231,8 +1231,8 @@ dev_tiff_decode_batch(const char *domain, const void *const *bufs, const size_t 
 			c += I.segs;
 		return c;
 	};
-	int rc = decode_chunks(
-		domain, "frame", n, [&](int i) { return ld[i].src_bytes + ld[i].dec_bytes + seg_count(i) * (sizeof(TiffSeg) + 2 * sizeof(int)); },
+	return decode_chunks(
+		domain, "tiff", "frame", n, [&](int i) { return ld[i].src_bytes + ld[i].dec_bytes + seg_count(i) * (sizeof(TiffSeg) + 2 * sizeof(int)); },
 		[&](int c0, int cn) {
 			std::vector<TiffSeg> S;
 			std::vector<const std::vector<unsigned char> *> J;
@@ -1255,114 +1255,88 @@ dev_tiff_decode_batch(const char *domain, const void *const *bufs, const size_t 
 				S[k].dec = jpg;
 				jpg += align16((size_t) S[k].dec_len);
 			}
-			/* the block: records, the kind lists, staged bytes, decoded bytes, JPEG-decoded tiles */
+			/* the block: records, the kind lists and staged bytes; decoded bytes and JPEG-decoded tiles as scratch */
 			const size_t off_list = align16(ns * sizeof(TiffSeg)), off_src = off_list + align16(ns * sizeof(int)), off_dec = off_src + src,
 						 off_jpg = off_dec + dec;
 			for (TiffSeg &r : S) {
 				r.src += off_src;
 				r.dec += r.comp == C_NONE ? off_src : r.comp == C_JPEG ? off_jpg : off_dec;
 			}
-			unsigned char *hst = (unsigned char *) decode_staging(domain, off_src + src);
-			if (!hst)
-				return -1;
-			memcpy(hst, S.data(), ns * sizeof(TiffSeg));
 			int li[4], at = 0;
 			for (int c = 1; c < 4; c++) {
 				li[c] = at;
-				if (!list[c].empty())
-					memcpy(hst + off_list + at * sizeof(int), list[c].data(), list[c].size() * sizeof(int));
 				at += (int) list[c].size();
 			}
-			parallel_for(cn, host_workers(), [&](int i) { stage_segments(ld[c0 + i], S.data() + first[i], hst); });
-			void *dev = nullptr;
-			int *status = nullptr;
-			if (dev_alloc(domain, &dev, off_jpg + jpg, s))
-				return -1;
-			if (dev_alloc(domain, (void **) &status, ns * sizeof(int), s)) {
-				dev_free(dev, s);
-				return -1;
-			}
-			unsigned char *dB = (unsigned char *) dev;
-			const TiffSeg *dS = (const TiffSeg *) dev;
-			const int *dL = (const int *) (dB + off_list);
-			std::vector<int> st(ns, 0);
-			int rc = 0;
-			if (cudaMemcpyAsync(dev, hst, off_src + src, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-				cudaMemsetAsync(status, 0, ns * sizeof(int), s) != cudaSuccess)
-				rc = cuda_fail(domain, cudaGetLastError(), "tiff staging copy");
-			else {
-				int launches = 0;
-				const int nb = std::max(1, std::min(sm_count() * 64, 1 << 20));
-				if (!list[C_DEFLATE].empty()) {
-					const int m = (int) list[C_DEFLATE].size();
-					tiff_inflate_kernel<<<std::min((m + kInflateWarps - 1) / kInflateWarps, nb), kInflateWarps * 32, 0, s>>>(dS, dL + li[C_DEFLATE], m,
-						dB, status);
-					launches++;
-				}
-				if (!list[C_LZW].empty()) {
-					const int m = (int) list[C_LZW].size();
-					tiff_lzw_kernel<<<std::min(m, nb), 32, 0, s>>>(dS, dL + li[C_LZW], m, dB, status);
-					launches++;
-				}
-				if (!list[C_PACKBITS].empty()) {
-					const int m = (int) list[C_PACKBITS].size();
-					tiff_packbits_kernel<<<std::min((m + 127) / 128, nb), 128, 0, s>>>(dS, dL + li[C_PACKBITS], m, dB, status);
-					launches++;
-				}
-				count_launch(launches);
-				/* JPEG tiles: dev_jpeg_decode_batch at shrink 1 over each run of one geometry, into their slots (no new kernel) */
-				for (size_t a = 0; a < jk.size() && !rc;) {
-					size_t b = a + 1;
-					while (b < jk.size() && S[jk[b]].seg_w == S[jk[a]].seg_w && S[jk[b]].dec_len == S[jk[a]].dec_len)
-						b++;
-					const TiffSeg &R = S[jk[a]];
-					std::vector<const void *> ptr(b - a);
-					std::vector<size_t> len(b - a);
-					for (size_t q = a; q < b; q++) {
-						ptr[q - a] = J[jk[q]]->data();
-						len[q - a] = J[jk[q]]->size();
+			return decode_chunk(
+				domain, "tiff", {off_src + src, dec + jpg, ns},
+				[&](unsigned char *hst) {
+					memcpy(hst, S.data(), ns * sizeof(TiffSeg));
+					for (int c = 1; c < 4; c++)
+						if (!list[c].empty())
+							memcpy(hst + off_list + li[c] * sizeof(int), list[c].data(), list[c].size() * sizeof(int));
+					parallel_for(cn, host_workers(), [&](int i) { stage_segments(ld[c0 + i], S.data() + first[i], hst); });
+				},
+				[&](unsigned char *dB, int *status) {
+					const TiffSeg *dS = (const TiffSeg *) dB;
+					const int *dL = (const int *) (dB + off_list);
+					int launches = 0;
+					const int nb = std::max(1, std::min(sm_count() * 64, 1 << 20));
+					if (!list[C_DEFLATE].empty()) {
+						const int m = (int) list[C_DEFLATE].size();
+						tiff_inflate_kernel<<<std::min((m + kInflateWarps - 1) / kInflateWarps, nb), kInflateWarps * 32, 0, s>>>(dS, dL + li[C_DEFLATE], m,
+							dB, status);
+						launches++;
 					}
-					const size_t before = strlen(vb200_error_buffer());
-					StreamGeometry jg;
-					if (dev_jpeg_decode_batch(domain, ptr.data(), len.data(), (int) (b - a), 1, dB + R.dec, (size_t) R.seg_w * R.spp,
-							align16((size_t) R.dec_len), &jg, s)) {
-						std::string reason;
-						const int t = jpeg_frame_error(take_errors(before), &reason);
-						if (t >= 0) {
-							const int k = jk[a + t];
-							error(domain, "frame %d: tile %d: %s", c0 + S[k].frame, k - (int) first[S[k].frame], reason.c_str());
+					if (!list[C_LZW].empty()) {
+						const int m = (int) list[C_LZW].size();
+						tiff_lzw_kernel<<<std::min(m, nb), 32, 0, s>>>(dS, dL + li[C_LZW], m, dB, status);
+						launches++;
+					}
+					if (!list[C_PACKBITS].empty()) {
+						const int m = (int) list[C_PACKBITS].size();
+						tiff_packbits_kernel<<<std::min((m + 127) / 128, nb), 128, 0, s>>>(dS, dL + li[C_PACKBITS], m, dB, status);
+						launches++;
+					}
+					/* JPEG tiles: dev_jpeg_decode_batch at shrink 1 over each run of one geometry, into their slots (no new kernel);
+					 * it counts its own launches */
+					for (size_t a = 0; a < jk.size();) {
+						size_t b = a + 1;
+						while (b < jk.size() && S[jk[b]].seg_w == S[jk[a]].seg_w && S[jk[b]].dec_len == S[jk[a]].dec_len)
+							b++;
+						const TiffSeg &R = S[jk[a]];
+						std::vector<const void *> ptr(b - a);
+						std::vector<size_t> len(b - a);
+						for (size_t q = a; q < b; q++) {
+							ptr[q - a] = J[jk[q]]->data();
+							len[q - a] = J[jk[q]]->size();
 						}
-						else
-							error(domain, "JPEG tiles: %s", reason.c_str());
-						rc = -1;
+						const size_t before = strlen(vb200_error_buffer());
+						StreamGeometry jg;
+						if (dev_jpeg_decode_batch(domain, ptr.data(), len.data(), (int) (b - a), 1, dB + R.dec, (size_t) R.seg_w * R.spp,
+								align16((size_t) R.dec_len), &jg, s)) {
+							std::string reason;
+							const int t = jpeg_frame_error(take_errors(before), &reason);
+							if (t >= 0) {
+								const int k = jk[a + t];
+								error(domain, "frame %d: tile %d: %s", c0 + S[k].frame, k - (int) first[S[k].frame], reason.c_str());
+							}
+							else
+								error(domain, "JPEG tiles: %s", reason.c_str());
+							count_launch(launches);
+							return -1;
+						}
+						a = b;
 					}
-					a = b;
-				}
-				const cudaError_t e = cudaGetLastError();
-				if (e != cudaSuccess || cudaMemcpyAsync(st.data(), status, ns * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-					cudaStreamSynchronize(s) != cudaSuccess)
-					rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "tiff segment decode");
-			}
-			for (int k = 0; k < ns && !rc; k++)
-				if (st[k]) {
-					error(domain, "frame %d: segment %d: %s", c0 + S[k].frame, k - (int) first[S[k].frame], status_text(st[k]));
-					rc = -1;
-				}
-			if (!rc) {
-				tiff_place_kernel<<<std::min(ns, 1 << 20), kPlaceWarps * 32, 0, s>>>(dS, ns, dB, (unsigned char *) out + (size_t) c0 * out_frame_stride,
-					out_bpl, out_frame_stride);
-				count_launch(1);
-				const cudaError_t e = cudaGetLastError();
-				if (e != cudaSuccess)
-					rc = cuda_fail(domain, e, "tiff_place_kernel");
-			}
-			dev_free(status, s);
-			dev_free(dev, s);
-			return rc;
-		});
-	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "tiff decode");
-	return rc;
+					return launches;
+				},
+				[&](int k, int st) { error(domain, "frame %d: segment %d: %s", c0 + S[k].frame, k - (int) first[S[k].frame], status_text(st)); },
+				[&](unsigned char *dB) {
+					tiff_place_kernel<<<std::min(ns, 1 << 20), kPlaceWarps * 32, 0, s>>>((const TiffSeg *) dB, ns, dB,
+						(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
+					return 1;
+				},
+				s);
+		}, s);
 }
 
 /* the same decode on the CPU through the same per-code and per-byte code: the test-suite's host twin */
@@ -1516,24 +1490,9 @@ vb200_tiffload_buffer(const void *buf, size_t len, int page, int n, int subifd, 
 extern "C" int
 vb200_tiff_icc_profile(const void *buf, size_t len, int page, int subifd, void *out, size_t cap, size_t *profile_len)
 {
-	const char *domain = "tiff_icc_profile";
-	if (!profile_len) {
-		error(domain, "null argument");
-		return -1;
-	}
-	std::vector<unsigned char> prof;
-	if (tiff_icc_profile(domain, (const unsigned char *) buf, len, page, 1, subifd, &prof, nullptr))
-		return -1;
-	*profile_len = prof.size();
-	if (!out)
-		return 0;
-	if (cap < prof.size()) {
-		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
-		return -1;
-	}
-	if (!prof.empty())
-		memcpy(out, prof.data(), prof.size());
-	return 0;
+	return profile_abi("tiff_icc_profile", out, cap, profile_len, [&](const char *domain, std::vector<unsigned char> *prof) {
+		return tiff_icc_profile(domain, (const unsigned char *) buf, len, page, 1, subifd, prof, nullptr);
+	});
 }
 
 /* reference: vips_thumbnail_open (thumbnail.c:562-581, 615-626) and vips_thumbnail_buffer_open's TIFF branch (:1552-1576) */
@@ -1564,13 +1523,8 @@ vb200_debug_thumbnail_pyramid_level(int in_w, int in_h, int n_pages, const int *
 extern "C" int
 vb200_debug_tiff_decode(const void *buf, size_t len, int page, int n, int subifd, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
-	try {
-		return host_tiff_decode("tiff_decode (host twin)", buf, len, page, n, subifd, (unsigned char *) out, out_bpl, width, height, bands);
-	}
-	catch (const std::exception &e) {
-		error("tiff_decode (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("tiff_decode (host twin)",
+		[&](const char *domain) { return host_tiff_decode(domain, buf, len, page, n, subifd, (unsigned char *) out, out_bpl, width, height, bands); });
 }
 
 /* one LZW segment (libtiff's new-style codes) through the decoder's LZW on the host: 0 and *out_len = want, or -1 (refused,
@@ -1578,11 +1532,6 @@ vb200_debug_tiff_decode(const void *buf, size_t len, int page, int n, int subifd
 extern "C" int
 vb200_debug_tiff_lzw(const void *data, size_t len, size_t want, void *out, size_t *out_len)
 {
-	try {
-		return debug_tiff_lzw("tiff_lzw (host twin)", (const unsigned char *) data, len, want, (unsigned char *) out, out_len);
-	}
-	catch (const std::exception &e) {
-		error("tiff_lzw (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("tiff_lzw (host twin)",
+		[&](const char *domain) { return debug_tiff_lzw(domain, (const unsigned char *) data, len, want, (unsigned char *) out, out_len); });
 }

@@ -237,13 +237,18 @@ struct StreamGeometry {
  * device call).  *page_h: the page height of a strip of more than one page, else 0.  Outputs may be null. */
 int dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl,
 	size_t out_frame_stride, int *w, int *h, int *bands, int *page_h, cudaStream_t s);
-/* the body of vb200_jpeg / png / gif_decode_batch: out in host or device memory, or null for the geometry */
+/* the body of vb200_{jpeg,png,gif,tiff,webp}_decode_batch: out in host or device memory, or null for the geometry */
 int decode_batch_abi(const char *domain, const DecodeRequest &req, const void *const *bufs, const size_t *lens, int n, void *out, int out_location,
 	size_t out_bpl, size_t out_frame_stride, int *width, int *height, int *bands);
 /* one stream into a new packed device image, B_W below 3 bands and sRGB from 3 */
 int dev_load(const char *domain, const DecodeRequest &req, const void *buf, size_t len, DevImage *out, int *page_h, cudaStream_t s);
-/* the body of vb200_jpegload / pngload / gifload_buffer: dev_load, then deliver into *out */
+/* the body of vb200_{jpeg,png,gif,tiff,webp}load_buffer: dev_load, then deliver into *out */
 int load_abi(const char *domain, const DecodeRequest &req, const void *buf, size_t len, VB200Image *out);
+/* the body of vb200_*_icc_profile: fetch(domain, &profile) (0, or -1 with the reason), *profile_len its length and, unless
+ * out is null, its bytes in out[cap] */
+int profile_abi(const char *domain, void *out, size_t cap, size_t *profile_len, const std::function<int(const char *, std::vector<unsigned char> *)> &fetch);
+/* the body of a host twin's test hook: fn(domain), an exception it throws reported as domain's error */
+int host_twin_abi(const char *domain, const std::function<int(const char *)> &fn);
 /* the profile a stream embeds (empty: none): JPEG's APP2, PNG's iCCP, the ICCProfile of the TIFF IFD req selects, WebP's ICCP; -1 for a
  * PNG with eXIf or a TIFF IFD whose Orientation is not 1; GIF has none */
 int stream_profile(const char *domain, const DecodeRequest &req, const unsigned char *d, size_t n, std::vector<unsigned char> *profile);
@@ -254,17 +259,31 @@ int parse_streams(const char *domain, const char *noun, int n, const std::functi
 	const std::function<StreamGeometry(int)> &geometry, StreamGeometry *g);
 /* out_bpl and out_frame_stride hold frames of geometry g */
 int check_out_strides(const char *domain, const StreamGeometry &g, size_t out_bpl, size_t out_frame_stride);
-/* device bytes per chunk of the PNG and GIF decoders and the JPEG and PNG encoders (vb200_debug_png_set_budget; 0: an eighth
- * of the device, at least 1 GiB) */
+/* device bytes per chunk of the PNG, GIF, TIFF and WebP decoders and the JPEG and PNG encoders (vb200_debug_png_set_budget;
+ * 0: an eighth of the device, at least 1 GiB) */
 size_t chunk_budget();
 /* chunk(c0, cn) for consecutive streams [c0, c0 + cn) whose device_bytes fit chunk_budget() (at least one: -1 when
- * that one alone does not), one decode at a time, so that chunk may use decode_staging() */
-int decode_chunks(const char *domain, const char *noun, int n, const std::function<size_t(int)> &device_bytes, const std::function<int(int, int)> &chunk);
+ * that one alone does not), one decode at a time, so that chunk may use decode_staging(); returns once s has finished the
+ * chunks' work.  what names the format in the labels of CUDA failures. */
+int decode_chunks(const char *domain, const char *what, const char *noun, int n, const std::function<size_t(int)> &device_bytes,
+	const std::function<int(int, int)> &chunk, cudaStream_t s);
 /* the pinned staging block, grow-only, at least bytes long (nullptr: cudaMallocHost failed, with the reason) */
 void *decode_staging(const char *domain, size_t bytes);
 void decode_staging_release(); /* vb200_shutdown */
+/* A chunk's one device block: [host_bytes that stage(pinned block) writes, copied up in one piece | scratch_bytes |
+ * n_status ints, zeroed], each region starting 16-aligned (the scratch at align16(host_bytes)). */
+struct DecodeBlock {
+	size_t host_bytes = 0, scratch_bytes = 0;
+	int n_status = 0;
+};
+/* One chunk of a PNG, GIF, TIFF or WebP batch on s, inside decode_chunks: the block staged and copied up, decode(dev, status)
+ * (the kernels it launched, or -1 with the reason set), then, once they have finished, refuse(k, status[k]) for the first
+ * nonzero status word (it sets the reason), else place(dev) (the kernels it launched that write the output, or -1). */
+int decode_chunk(const char *domain, const char *what, const DecodeBlock &b, const std::function<void(unsigned char *)> &stage,
+	const std::function<int(unsigned char *, int *)> &decode, const std::function<void(int, int)> &refuse,
+	const std::function<int(unsigned char *)> &place, cudaStream_t s);
 
-/* The three batch decoders dev_decode_batch switches over (n >= 1; out_frame_stride holds a frame whatever n is). */
+/* The five batch decoders dev_decode_batch switches over (n >= 1; out_frame_stride holds a frame whatever n is). */
 /* jpeg.cu: n JPEG streams of one output geometry -> out[n][h][w][bands] on the device (out = nullptr: geometry only) */
 int dev_jpeg_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, int shrink, void *out, size_t out_bpl,
 	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);

@@ -1601,7 +1601,8 @@ dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t 
 	WebpTimer timer;
 	for (float &t : t_webp_ms)
 		t = timer.on ? 0.f : -1.f;
-	int rc = decode_chunks(domain, "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
+	return decode_chunks(domain, "webp", "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
+		/* the block: records and VP8 data staged; each frame's macroblock scratch */
 		std::vector<WebpFrameDev> F(cn);
 		size_t data = 0;
 		for (int i = 0; i < cn; i++) {
@@ -1610,70 +1611,36 @@ dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t 
 			data += align16(H.len);
 		}
 		const size_t off_data = align16(cn * sizeof(WebpFrameDev)), total = off_data + data;
-		unsigned char *hst = (unsigned char *) decode_staging(domain, total);
-		if (!hst)
-			return -1;
-		memcpy(hst, F.data(), cn * sizeof(WebpFrameDev));
-		parallel_for(cn, host_workers(), [&](int i) { memcpy(hst + off_data + F[i].data_off, hdr[c0 + i].vp8, hdr[c0 + i].len); });
-		void *dev = nullptr, *scr = nullptr;
-		int *status = nullptr;
-		if (dev_alloc(domain, &dev, total, s))
-			return -1;
-		if (dev_alloc(domain, &scr, scratch_bytes * cn, s)) {
-			dev_free(dev, s);
-			return -1;
-		}
-		if (dev_alloc(domain, (void **) &status, cn * sizeof(int), s)) {
-			dev_free(scr, s);
-			dev_free(dev, s);
-			return -1;
-		}
-		const WebpFrameDev *dF = (const WebpFrameDev *) dev;
-		const unsigned char *dD = (const unsigned char *) dev + off_data;
-		unsigned char *dS = (unsigned char *) scr;
-		std::vector<int> st(cn, 0);
-		int rc = 0;
-		if (cudaMemcpyAsync(dev, hst, total, cudaMemcpyHostToDevice, s) != cudaSuccess)
-			rc = cuda_fail(domain, cudaGetLastError(), "webp staging copy");
-		else {
-			/* the diagonals of a frame hold at most min(mb_h, ceil(mb_w / 2)) macroblocks */
-			const int diag = std::min(mb_h, (mb_w + 1) / 2), threads = std::min(256, (diag + 31) / 32 * 32);
-			timer.mark(0, s);
-			webp_header_kernel<<<(cn + 63) / 64, 64, 0, s>>>(dF, cn, dD, dS, status);
-			timer.mark(1, s);
-			webp_token_kernel<<<(cn + 63) / 64, 64, 0, s>>>(dF, cn, dD, dS, status);
-			timer.mark(2, s);
-			webp_recon_kernel<<<cn, threads, 0, s>>>(dF, dS, status);
-			timer.mark(3, s);
-			count_launch(3);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess || cudaMemcpyAsync(st.data(), status, cn * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-				cudaStreamSynchronize(s) != cudaSuccess)
-				rc = cuda_fail(domain, e != cudaSuccess ? e : cudaGetLastError(), "webp header / tokens / reconstruction");
-		}
-		for (int i = 0; i < cn && !rc; i++)
-			if (st[i]) {
-				error(domain, "frame %d: %s", c0 + i, werr_text(st[i]));
-				rc = -1;
-			}
-		if (!rc) {
-			webp_rgb_kernel<<<dim3((W + 127) / 128, std::min(Hh, kMaxGridY), cn), 128, 0, s>>>(dF, dS,
-				(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
-			timer.mark(4, s);
-			timer.add();
-			count_launch(1);
-			const cudaError_t e = cudaGetLastError();
-			if (e != cudaSuccess)
-				rc = cuda_fail(domain, e, "webp_rgb_kernel");
-		}
-		dev_free(status, s);
-		dev_free(scr, s);
-		dev_free(dev, s);
-		return rc;
-	});
-	if (!rc && cudaStreamSynchronize(s) != cudaSuccess)
-		rc = cuda_fail(domain, cudaGetLastError(), "webp decode");
-	return rc;
+		return decode_chunk(
+			domain, "webp", {total, scratch_bytes * cn, cn},
+			[&](unsigned char *hst) {
+				memcpy(hst, F.data(), cn * sizeof(WebpFrameDev));
+				parallel_for(cn, host_workers(), [&](int i) { memcpy(hst + off_data + F[i].data_off, hdr[c0 + i].vp8, hdr[c0 + i].len); });
+			},
+			[&](unsigned char *dev, int *status) {
+				const WebpFrameDev *dF = (const WebpFrameDev *) dev;
+				unsigned char *dS = dev + align16(total);
+				/* the diagonals of a frame hold at most min(mb_h, ceil(mb_w / 2)) macroblocks */
+				const int diag = std::min(mb_h, (mb_w + 1) / 2), threads = std::min(256, (diag + 31) / 32 * 32);
+				timer.mark(0, s);
+				webp_header_kernel<<<(cn + 63) / 64, 64, 0, s>>>(dF, cn, dev + off_data, dS, status);
+				timer.mark(1, s);
+				webp_token_kernel<<<(cn + 63) / 64, 64, 0, s>>>(dF, cn, dev + off_data, dS, status);
+				timer.mark(2, s);
+				webp_recon_kernel<<<cn, threads, 0, s>>>(dF, dS, status);
+				timer.mark(3, s);
+				return 3;
+			},
+			[&](int i, int st) { error(domain, "frame %d: %s", c0 + i, werr_text(st)); },
+			[&](unsigned char *dev) {
+				webp_rgb_kernel<<<dim3((W + 127) / 128, std::min(Hh, kMaxGridY), cn), 128, 0, s>>>((const WebpFrameDev *) dev, dev + align16(total),
+					(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
+				timer.mark(4, s);
+				timer.add();
+				return 1;
+			},
+			s);
+	}, s);
 }
 
 /* the same decode on the CPU through the same per-symbol, per-block and per-pixel code, in raster order: the test-suite's
@@ -1770,36 +1737,15 @@ vb200_webpload_buffer(const void *buf, size_t len, VB200Image *out)
 extern "C" int
 vb200_webp_icc_profile(const void *buf, size_t len, void *out, size_t cap, size_t *profile_len)
 {
-	const char *domain = "webp_icc_profile";
-	if (!profile_len) {
-		error(domain, "null argument");
-		return -1;
-	}
-	std::vector<unsigned char> prof;
-	if (webp_icc_profile(domain, (const unsigned char *) buf, len, &prof))
-		return -1;
-	*profile_len = prof.size();
-	if (!out)
-		return 0;
-	if (cap < prof.size()) {
-		error(domain, "the profile is %zu bytes, the buffer %zu", prof.size(), cap);
-		return -1;
-	}
-	if (!prof.empty())
-		memcpy(out, prof.data(), prof.size());
-	return 0;
+	return profile_abi("webp_icc_profile", out, cap, profile_len,
+		[&](const char *domain, std::vector<unsigned char> *prof) { return webp_icc_profile(domain, (const unsigned char *) buf, len, prof); });
 }
 
 extern "C" int
 vb200_debug_webp_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
-	try {
-		return host_webp_decode("webp_decode (host twin)", buf, len, (unsigned char *) out, out_bpl, width, height, bands);
-	}
-	catch (const std::exception &e) {
-		error("webp_decode (host twin)", "%s", e.what());
-		return -1;
-	}
+	return host_twin_abi("webp_decode (host twin)",
+		[&](const char *domain) { return host_webp_decode(domain, buf, len, (unsigned char *) out, out_bpl, width, height, bands); });
 }
 
 /* ms[4]: the last batch's device milliseconds in the header, token, reconstruction and RGB kernels on this thread, with

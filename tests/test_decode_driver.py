@@ -1,5 +1,5 @@
-"""The decoders' shared driver (csrc/decode.cu): vb200_jpeg / png / gif_decode_batch and vb200_jpegload / pngload / gifload_buffer
-behave alike -- errors that name the stream, one geometry per batch, host and device delivery, batch-or-nothing into host
+"""The decoders' shared driver (csrc/decode.cu): vb200_{jpeg,png,gif,tiff,webp}_decode_batch and the matching *load_buffer
+entry points behave alike -- errors that name the stream, one geometry per batch, host and device delivery, batch-or-nothing into host
 memory, and one interpretation rule for the loaders."""
 import ctypes as C
 import io
@@ -36,14 +36,29 @@ def _gif(h, w, bands):
     return b.getvalue()
 
 
-MAKE = {"jpeg": _jpeg, "png": _png, "gif": _gif}
-BANDS = {"jpeg": (1, 3), "png": (1, 2, 3, 4), "gif": (3, 4)}
-NOUN = {"jpeg": "frame", "png": "frame", "gif": "stream"}
-DOMAIN = {"jpeg": "jpeg_decode_batch", "png": "png_decode_batch", "gif": "gif_decode_batch"}
+def _tiff(h, w, bands):
+    a = RNG.integers(0, 256, (h, w, bands), dtype=np.uint8)
+    b = io.BytesIO()
+    PIL.fromarray(a[:, :, 0] if bands == 1 else a).save(b, "TIFF", compression="tiff_lzw")
+    return b.getvalue()
+
+
+def _webp(h, w, bands):
+    a = RNG.integers(0, 256, (h, w, bands), dtype=np.uint8)
+    b = io.BytesIO()
+    PIL.fromarray(a).save(b, "WEBP", quality=80)
+    return b.getvalue()
+
+
+MAKE = {"jpeg": _jpeg, "png": _png, "gif": _gif, "tiff": _tiff, "webp": _webp}
+BANDS = {"jpeg": (1, 3), "png": (1, 2, 3, 4), "gif": (3, 4), "tiff": (1, 2, 3, 4), "webp": (3,)}
+NOUN = {"jpeg": "frame", "png": "frame", "gif": "stream", "tiff": "frame", "webp": "frame"}
+DOMAIN = {"jpeg": "jpeg_decode_batch", "png": "png_decode_batch", "gif": "gif_decode_batch", "tiff": "tiff_decode_batch",
+          "webp": "webp_decode_batch"}
 
 
 def _opts(fmt):
-    return {"jpeg": (1,), "png": (), "gif": (0, 1)}[fmt]
+    return {"jpeg": (1,), "png": (), "gif": (0, 1), "tiff": (0, 1, -1), "webp": ()}[fmt]
 
 
 def _fn(fmt):
@@ -105,7 +120,7 @@ def test_gpu_load_buffer(vb, fmt):
         out = vb.CImage()
         out.where = vb.HOST
         name = "vb200_%sload_buffer" % fmt
-        args = {"jpeg": (1,), "png": (), "gif": (0, 1)}[fmt]
+        args = _opts(fmt)
         fn = getattr(vb.lib(), name)
         fn.argtypes = [C.c_void_p, C.c_size_t] + [C.c_int] * len(args) + [C.POINTER(vb.CImage)]
         vb._check(fn(s, len(s), *args, C.byref(out)))
@@ -142,6 +157,16 @@ def _fails_in_decode(fmt):
         from test_gif import BAD, blocks, rand_pal, write_gif
         rng = np.random.default_rng(3)
         return BAD["past_table_50"], write_gif(50, 40, [dict(img=blocks(rng, 40, 50, 256))], rand_pal(rng, 256))
+    if fmt == "tiff":
+        from test_tiff import Page, img, lzw_encode, make_tiff
+        a = img(24, 32, 3, 3)
+        # an LZW segment that ends short of the strip's rows
+        return make_tiff([Page(a, comp=5, segments=[lzw_encode(a.tobytes()[:50])])]), make_tiff([Page(a, comp=5)])
+    if fmt == "webp":
+        from test_webp import _cut, pillow_or_none, vp8_payload, vp8_stream
+        good = vp8_stream(9000, h=30, w=30, parts=2)
+        # a token partition cut short where libwebp refuses it
+        return next(_cut(good, k) for k in range(len(vp8_payload(good)) - 1, 10, -1) if pillow_or_none(_cut(good, k)) is None), good
     good = MAKE[fmt](24, 32, 3)
     if fmt == "png":
         at = good.index(b"IDAT") + 4
