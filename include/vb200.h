@@ -680,7 +680,29 @@ void vb200_debug_png_set_budget(size_t bytes);
  * vb200_debug_webp_times: with VB200_WEBP_TIMING set in the environment, ms[4] = the last batch's device milliseconds in the
  *   header, token, reconstruction and RGB kernels on the calling thread (each chunk then waits for its events); -1 without.
  * vb200_thumbnail_buffer and the other thumbnail entries refuse WebP: thumbnail.c loads it at a non-integer scale through
- * libwebp's own rescaler, which is not built.  Chunks are bounded by vb200_debug_png_set_budget.
+ * libwebp's own rescaler, which only the WebP entries below take.  Chunks are bounded by vb200_debug_png_set_budget.
+ *
+ * WebP shrink-on-load: vips_webpload_buffer(buf, len, &out, "scale", scale, NULL).  scale != 1.0 is libwebp's scaled decode
+ * (webp2vips.c:513-514, 630-634): the frame becomes rint(w * scale) x rint(h * scale), refused outside 1 .. 16383 on either
+ * axis or for scale outside webpload's [0, 1024]; the loop filter is bypassed when both axes come out below three quarters
+ * (w * 3 / 4, in integers); Y, U and V each go through libwebp's WebPRescaler (area average shrinking, linear interpolation
+ * expanding, 32-bit fixed point) with no upsampler, then the same 14-bit YUV -> RGB.  Pixel for pixel libwebp's.
+ * scale == 1.0 is exactly the plain decode above.
+ *
+ * vb200_webp_decode_batch_scaled: vb200_webp_decode_batch at scale; the streams must share one source size.
+ * vb200_webpload_buffer_scaled: vb200_webpload_buffer at scale.
+ * vb200_thumbnail_webp_scale: host only -- vips_thumbnail_open's WebP factor max(1, common shrink) (thumbnail.c:627-636)
+ *   as *scale = 1 / factor and the size webpload loads at (*scaled_width / *scaled_height may be NULL).  Unlike JPEG's
+ *   shrink it applies in linear mode too.
+ * vb200_thumbnail_webp_buffer: vips_thumbnail_buffer of a WebP stream: loaded at vb200_thumbnail_webp_scale's scale on the
+ *   device, its ICCP as the embedded profile, then what vb200_thumbnail_buffer_icc (linear = 0) or
+ *   vb200_thumbnail_buffer_linear_icc (linear = 1) runs on the decode; icc NULL: no colour management.
+ * vb200_thumbnail_plan_run_webp: the streams decoded at scale + the plan's thumbnail chain, frames never leave the device;
+ *   the plan must have been made for the scaled geometry.
+ * vb200_debug_webp_decode_scaled: test hook, host only -- the scaled decode on the CPU, its rescaler streaming rows in
+ *   libwebp's order.
+ * vb200_debug_webp_rescale: test hook, host only -- one plane of src_w x src_h rescaled to dst_w x dst_h, closed_form set by
+ *   the device kernel's per-sample function, else by the host twin's row-streaming rescaler.
  */
 int vb200_webp_geometry(const void *buf, size_t len, int *width, int *height, int *bands);
 int vb200_webp_decode_batch(const void *const *bufs, const size_t *lens, int n, void *out, int out_location, size_t out_bpl,
@@ -690,6 +712,19 @@ int vb200_webp_icc_profile(const void *buf, size_t len, void *out, size_t cap, s
 int vb200_debug_webp_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands);
 int vb200_debug_webp_tables(void *out, size_t cap, size_t *len);
 void vb200_debug_webp_times(float *ms);
+int vb200_webp_decode_batch_scaled(const void *const *bufs, const size_t *lens, int n, double scale, void *out, int out_location,
+	size_t out_bpl, size_t out_frame_stride, int *width, int *height, int *bands);
+int vb200_webpload_buffer_scaled(const void *buf, size_t len, double scale, VB200Image *out);
+int vb200_thumbnail_webp_scale(int width, int height, int target_width, int target_height, int size, double *scale, int *scaled_width,
+	int *scaled_height);
+int vb200_thumbnail_webp_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
+	int linear);
+int vb200_thumbnail_plan_run_webp(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, double scale, void *out,
+	int out_location, size_t out_frame_stride);
+int vb200_debug_webp_decode_scaled(const void *buf, size_t len, double scale, void *out, size_t out_bpl, int *width, int *height,
+	int *bands);
+int vb200_debug_webp_rescale(const void *plane, size_t stride, int src_w, int src_h, int dst_w, int dst_h, int closed_form, void *out,
+	size_t out_bpl);
 /* ------------------------------------------------------------------ GIF decode on the device (SURVEY 8f rank 1)
  * vips_gifload_buffer(buf, len, &out, "page", page, "n", n, NULL) (foreign/nsgifload.c over libnsgif, fail_on = none)
  * with LZW and frame composition on the device (csrc/gif.cu): the LZW payloads, without their sub-block length bytes, and

@@ -334,6 +334,15 @@ def lib():
         L.vb200_debug_webp_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, PI, PI, PI]
         L.vb200_debug_webp_tables.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         L.vb200_debug_webp_times.argtypes = [C.POINTER(C.c_float)]
+        L.vb200_webp_decode_batch_scaled.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_double, C.c_void_p, C.c_int,
+                                                     C.c_size_t, C.c_size_t, PI, PI, PI]
+        L.vb200_webpload_buffer_scaled.argtypes = [C.c_void_p, C.c_size_t, C.c_double, IP]
+        L.vb200_debug_webp_decode_scaled.argtypes = [C.c_void_p, C.c_size_t, C.c_double, C.c_void_p, C.c_size_t, PI, PI, PI]
+        L.vb200_debug_webp_rescale.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
+        L.vb200_thumbnail_webp_scale.argtypes = [C.c_int] * 5 + [C.POINTER(C.c_double), PI, PI]
+        L.vb200_thumbnail_webp_buffer.argtypes = [C.c_void_p, C.c_size_t, IP, C.c_int, C.c_int, C.c_int, TI, C.c_int]
+        L.vb200_thumbnail_plan_run_webp.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_double, C.c_void_p,
+                                                    C.c_int, C.c_size_t]
         L.vb200_thumbnail_plan_new_pages.restype = C.c_void_p
         L.vb200_thumbnail_plan_new_pages.argtypes = [C.c_int] * 10
         L.vb200_thumbnail_plan_page_height.argtypes = [C.c_void_p]
@@ -634,10 +643,12 @@ class Image:
         return img
 
     @staticmethod
-    def webpload_buffer(stream):
-        """vips_webpload_buffer(stream) of a lossy, still, opaque WebP: the frame decoded on the device -> Image (uint8, 3 bands,
-        sRGB)"""
-        return Image._load_buffer(lib().vb200_webpload_buffer, stream)
+    def webpload_buffer(stream, scale=1.0):
+        """vips_webpload_buffer(stream, scale=scale) of a lossy, still, opaque WebP: the frame decoded on the device -> Image
+        (uint8, 3 bands, sRGB); scale != 1 is libwebp's scaled decode to rint(w * scale) x rint(h * scale)"""
+        if scale == 1.0:
+            return Image._load_buffer(lib().vb200_webpload_buffer, stream)
+        return Image._load_buffer(lib().vb200_webpload_buffer_scaled, stream, float(scale))
 
     # ---- colour
     @staticmethod
@@ -755,16 +766,31 @@ def webp_geometry(stream):
     return w.value, h.value, bands.value
 
 
-def webp_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None):
-    """vips_webpload_buffer() of every stream (lossy, still, opaque WebP) on the device -> uint8 [n, h, w, 3] (host), or into the
-    device pointer out_ptr (packed frames unless out_bpl / out_frame_stride say otherwise)"""
-    return _decode_batch(lib().vb200_webp_decode_batch, streams, (), out_ptr, out_bpl, out_frame_stride)
+def webp_decode_batch(streams, out_ptr=None, out_bpl=None, out_frame_stride=None, scale=1.0):
+    """vips_webpload_buffer(scale=scale) of every stream (lossy, still, opaque WebP) on the device -> uint8 [n, h, w, 3] (host), or
+    into the device pointer out_ptr (packed frames unless out_bpl / out_frame_stride say otherwise).  scale != 1: libwebp's
+    scaled decode, the streams sharing one source size"""
+    if scale == 1.0:
+        return _decode_batch(lib().vb200_webp_decode_batch, streams, (), out_ptr, out_bpl, out_frame_stride)
+    return _decode_batch(lib().vb200_webp_decode_batch_scaled, streams, (float(scale),), out_ptr, out_bpl, out_frame_stride)
 
 
-def webp_decode_host_twin(stream):
-    """the decoder's per-symbol / per-block / per-pixel code compiled for the host (vb200_debug_webp_decode): what the CPU tests
-    pin to libwebp"""
-    return _host_twin(lib().vb200_debug_webp_decode, stream)
+def webp_decode_host_twin(stream, scale=1.0):
+    """the decoder's per-symbol / per-block / per-pixel code compiled for the host (vb200_debug_webp_decode, or at scale != 1
+    vb200_debug_webp_decode_scaled with its row-streaming rescaler): what the CPU tests pin to libwebp"""
+    if scale == 1.0:
+        return _host_twin(lib().vb200_debug_webp_decode, stream)
+    return _host_twin(lib().vb200_debug_webp_decode_scaled, stream, float(scale))
+
+
+def webp_rescale_plane(plane, dst_w, dst_h, closed_form=True):
+    """one uint8 plane [h, w] through libwebp's rescaler to [dst_h, dst_w] on the host (vb200_debug_webp_rescale): closed_form
+    by the device kernel's per-sample function, else by the host twin's row-streaming rescaler"""
+    plane = np.ascontiguousarray(plane, np.uint8)
+    out = np.empty((dst_h, dst_w), np.uint8)
+    _check(lib().vb200_debug_webp_rescale(plane.ctypes.data_as(C.c_void_p), plane.shape[1], plane.shape[1], plane.shape[0], int(dst_w),
+                                          int(dst_h), int(closed_form), out.ctypes.data_as(C.c_void_p), int(dst_w)))
+    return out
 
 
 def webp_times():
@@ -1206,10 +1232,24 @@ def _thumbnail_buffer_pages(stream, width, height, size, icc, linear, page, n):
     return a, (oph.value if oph.value < a.shape[0] else None)
 
 
+def _is_webp(stream):
+    return len(stream) >= 12 and stream[:4] == b"RIFF" and stream[8:12] == b"WEBP"
+
+
+def _thumbnail_webp_buffer(stream, width, height, size, icc, linear):
+    """vb200_thumbnail_webp_buffer: a WebP stream loaded at vips_thumbnail's scale, then thumbnailed -> uint8 array"""
+    out = CImage()
+    out.where = HOST
+    _check(lib().vb200_thumbnail_webp_buffer(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
+                                             C.byref(icc) if icc is not None else None, int(linear)))
+    return Image._take(out).array
+
+
 def thumbnail_buffer(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                      builtin_profiles=None, page=0, n=1, return_page_height=False):
-    """vips_thumbnail_buffer() of a JPEG, PNG, GIF or TIFF stream: decode (JPEG with shrink-on-load, GIF's pages page .. page + n - 1,
-    n = -1 for all from page on, a TIFF's pyramid level as thumbnail_tiff_level picks it) + thumbnail on the device -> uint8 array; with output_profile, colour-managed with the profile
+    """vips_thumbnail_buffer() of a JPEG, PNG, GIF, TIFF or WebP stream: decode (JPEG with shrink-on-load, WebP at
+    thumbnail_webp_scale's scale, GIF's pages page .. page + n - 1, n = -1 for all from page on, a TIFF's pyramid level as
+    thumbnail_tiff_level picks it) + thumbnail on the device -> uint8 array; with output_profile, colour-managed with the profile
     the stream embeds (APP2 ICC_PROFILE or iCCP; GIF has none).  PNG streams with eXIf are refused: their orientation would
     need vips_autorot.  A GIF of several pages thumbnails as a page strip; return_page_height=True returns
     (array, page height) with None for a result of one page"""
@@ -1218,6 +1258,8 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
     if return_page_height or page != 0 or n != 1:
         a, ph = _thumbnail_buffer_pages(stream, width, height, size, icc, False, page, n)
         return (a, ph) if return_page_height else a
+    if _is_webp(stream):
+        return _thumbnail_webp_buffer(stream, width, height, size, icc, False)
     out = CImage()
     out.where = HOST
     if icc is None:
@@ -1230,7 +1272,8 @@ def thumbnail_buffer(stream, width, height=None, size="both", output_profile=Non
 
 def thumbnail_buffer_linear(stream, width, height=None, size="both", output_profile=None, input_profile=None, intent="relative",
                             builtin_profiles=None, page=0, n=1, return_page_height=False):
-    """vips_thumbnail_buffer(linear=TRUE) of a JPEG, PNG or GIF stream: full-size decode + linear-light thumbnail on the device,
+    """vips_thumbnail_buffer(linear=TRUE) of a JPEG, PNG, GIF or WebP stream: full-size decode (WebP at thumbnail_webp_scale's
+    scale, which applies in linear mode too) + linear-light thumbnail on the device,
     colour-managed with the profile the stream embeds and / or the profiles given.  PNG streams with eXIf are refused.
     page / n / return_page_height as thumbnail_buffer"""
     stream = bytes(stream)
@@ -1238,11 +1281,21 @@ def thumbnail_buffer_linear(stream, width, height=None, size="both", output_prof
     if return_page_height or page != 0 or n != 1:
         a, ph = _thumbnail_buffer_pages(stream, width, height, size, icc, True, page, n)
         return (a, ph) if return_page_height else a
+    if _is_webp(stream):
+        return _thumbnail_webp_buffer(stream, width, height, size, icc, True)
     out = CImage()
     out.where = HOST
     _check(lib().vb200_thumbnail_buffer_linear_icc(stream, len(stream), C.byref(out), int(width), int(height or 0), SIZES[size],
                                                    C.byref(icc)))
     return Image._take(out).array
+
+
+def thumbnail_webp_scale(width, height, target_width, target_height=None, size="both"):
+    """vips_thumbnail_open's WebP load (thumbnail.c:627-636): (scale, scaled width, scaled height) webpload is asked for"""
+    sc, sw, sh = C.c_double(), C.c_int(), C.c_int()
+    _check(lib().vb200_thumbnail_webp_scale(int(width), int(height), int(target_width), int(target_height or 0), SIZES[size], C.byref(sc),
+                                            C.byref(sw), C.byref(sh)))
+    return sc.value, sw.value, sh.value
 
 
 def thumbnail_jpegshrink(width, height, target_width, target_height=None, size="both"):
@@ -1373,6 +1426,11 @@ class ThumbnailPlan:
         """JPEG streams decoded at `shrink` on the device and thumbnailed by this plan (made for the decoded
         geometry): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
         return self._run_streams(lib().vb200_thumbnail_plan_run_jpeg, streams, (int(shrink),), out_ptr)
+
+    def run_webp(self, streams, scale, out_ptr=None):
+        """WebP streams decoded on the device at webpload's `scale` and thumbnailed by this plan (made for the scaled
+        geometry): -> uint8 [n, OH, OW, bands] on the host, or into the device pointer out_ptr"""
+        return self._run_streams(lib().vb200_thumbnail_plan_run_webp, streams, (float(scale),), out_ptr)
 
     def run_png(self, streams, out_ptr=None):
         """PNG streams decoded on the device at full size and thumbnailed by this plan (made for the decoded geometry):

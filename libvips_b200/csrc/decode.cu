@@ -327,7 +327,7 @@ dev_decode_batch(const char *domain, const DecodeRequest &req, const void *const
 		rc = dev_tiff_decode_batch(domain, bufs, lens, n, req.page, req.n_pages, req.subifd, out, out_bpl, out_frame_stride, &g, s);
 		break;
 	case STREAM_WEBP:
-		rc = dev_webp_decode_batch(domain, bufs, lens, n, out, out_bpl, out_frame_stride, &g, s);
+		rc = dev_webp_decode_batch(domain, bufs, lens, n, req.scale, out, out_bpl, out_frame_stride, &g, s);
 		break;
 	default:
 		rc = dev_jpeg_decode_batch(domain, bufs, lens, n, req.shrink, out, out_bpl, out_frame_stride, &g, s);

@@ -2390,7 +2390,7 @@ static int thumbnail_image_run(const VB200Image *in, int page_height, VB200Image
  */
 static int
 thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc,
-	bool linear, int page = 0, int n_pages = 1, int *out_page_height = nullptr)
+	bool linear, int page = 0, int n_pages = 1, int *out_page_height = nullptr, bool webp = false)
 {
 	const char *domain = "thumbnail_buffer";
 	if (!buf || !out) {
@@ -2398,9 +2398,13 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 		return -1;
 	}
 	DecodeRequest req{stream_kind(buf, len), 1, page, n_pages};
-	if (req.kind == STREAM_WEBP) {
+	if (req.kind == STREAM_WEBP && !webp) {
 		/* thumbnail.c:627-636, 1524-1532 load WebP at scale = 1 / factor: libwebp's own rescaler, not the full-size decode */
-		error(domain, "WebP shrink-on-load (libwebp's scaled decode) is not built on the device path");
+		error(domain, "WebP shrink-on-load (libwebp's scaled decode) is not built on the device path; vb200_thumbnail_webp_buffer takes WebP streams");
+		return -1;
+	}
+	if (webp && req.kind != STREAM_WEBP) {
+		error(domain, "not a WebP stream (no RIFF / WEBP signature)");
 		return -1;
 	}
 	if (ensure_init(domain))
@@ -2426,6 +2430,13 @@ thumbnail_buffer_run(const void *buf, size_t len, VB200Image *out, int width, in
 		if (dev_decode_batch(domain, req, &buf, &len, 1, nullptr, 0, 0, &w0, &h0, &b0, nullptr, s))
 			return -1;
 		req.shrink = vb200_thumbnail_jpegshrink(w0, h0, width, height, size);
+	}
+	if (req.kind == STREAM_WEBP) {
+		/* linear or not: only find_jpegshrink declines in linear mode (thumbnail.c:496-499) */
+		int w0, h0, b0;
+		if (dev_decode_batch(domain, req, &buf, &len, 1, nullptr, 0, 0, &w0, &h0, &b0, nullptr, s) ||
+			vb200_thumbnail_webp_scale(w0, h0, width, height, size, &req.scale, nullptr, nullptr))
+			return -1;
 	}
 	DevImage dec;
 	int page_height;
@@ -2476,6 +2487,33 @@ vb200_thumbnail_buffer_linear_icc(const void *buf, size_t len, VB200Image *out, 
 	const VB200ThumbnailIcc *icc)
 {
 	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, true);
+}
+
+/* reference: vips_thumbnail_buffer of a WebP stream: loaded at scale = 1 / vips_thumbnail_open's factor (thumbnail.c:627-636,
+ * 1524-1532) through the device's scaled decode, the stream's ICCP as the embedded profile, then thumbnail_image_run */
+extern "C" int
+vb200_thumbnail_webp_buffer(const void *buf, size_t len, VB200Image *out, int width, int height, int size, const VB200ThumbnailIcc *icc, int linear)
+{
+	return thumbnail_buffer_run(buf, len, out, width, height, size, icc, linear != 0, 0, 1, nullptr, true);
+}
+
+/* reference: vips_thumbnail_open's WebP factor, max(1, the common shrink) (thumbnail.c:627-636), as webpload's scale and the
+ * frame size it loads at (webp2vips.c:513-514) */
+extern "C" int
+vb200_thumbnail_webp_scale(int width, int height, int target_width, int target_height, int size, double *scale, int *scaled_width,
+	int *scaled_height)
+{
+	if (width < 1 || height < 1 || target_width < 1 || !scale) {
+		error("thumbnail_webp_scale", "bad arguments (%d x %d to width %d)", width, height, target_width);
+		return -1;
+	}
+	const double factor = std::max(1.0, thumbnail_common_shrink(width, height, target_width, target_height > 0 ? target_height : target_width, size));
+	*scale = 1.0 / factor;
+	if (scaled_width)
+		*scaled_width = (int) rint(width * *scale);
+	if (scaled_height)
+		*scaled_height = (int) rint(height * *scale);
+	return 0;
 }
 
 /* See vb200.h: vips_thumbnail_buffer(..., option_string = "page=..,n=..") */
@@ -2590,6 +2628,16 @@ vb200_thumbnail_plan_run_gif_pages(VB200ThumbnailPlan *plan, const void *const *
 	void *out, int out_location, size_t out_frame_stride)
 {
 	return plan_run_streams("thumbnail_plan_run_gif", {STREAM_GIF, 1, page, n_pages}, plan, bufs, lens, n, out, out_location, out_frame_stride);
+}
+
+/* See vb200.h: the WebP streams decoded at webpload's scale, then the plan (made for the scaled geometry) */
+extern "C" int
+vb200_thumbnail_plan_run_webp(VB200ThumbnailPlan *plan, const void *const *bufs, const size_t *lens, int n, double scale, void *out, int out_location,
+	size_t out_frame_stride)
+{
+	DecodeRequest req{STREAM_WEBP};
+	req.scale = scale;
+	return plan_run_streams("thumbnail_plan_run_webp", req, plan, bufs, lens, n, out, out_location, out_frame_stride);
 }
 
 /* See vb200.h: the TIFF streams' pages page .. page + n_pages - 1 at subifd, then the plan */

@@ -222,11 +222,13 @@ int dev_colourspace_ext(const char *domain, const DevImage &in, DevImage *out, i
 enum StreamKind { STREAM_JPEG, STREAM_PNG, STREAM_GIF, STREAM_TIFF, STREAM_WEBP };
 StreamKind stream_kind(const void *buf, size_t len);
 /* what to decode: shrink is JPEG's load-time shrink; page / n_pages GIF's and TIFF's pages (n_pages -1: to the last), 0 / 1
- * elsewhere; subifd TIFF's SubIFD of each page (-1: the page's main IFD), -1 elsewhere */
+ * elsewhere; subifd TIFF's SubIFD of each page (-1: the page's main IFD), -1 elsewhere; scale webpload's scale (read only
+ * for WebP: 1 is the plain decode, anything else libwebp's scaled decode) */
 struct DecodeRequest {
 	StreamKind kind;
 	int shrink = 1, page = 0, n_pages = 1;
 	int subifd = -1;
+	double scale = 1.0;
 };
 /* A batch's geometry as the decoders report it: frames of h rows, or (pages > 0) strips of `pages` pages of h rows. */
 struct StreamGeometry {
@@ -362,9 +364,9 @@ int tiff_icc_profile(const char *domain, const unsigned char *d, size_t len, int
 int tiff_thumbnail_level(const char *domain, const unsigned char *d, size_t len, int width, int height, int size, int *subifd, int *page);
 
 /* webp.cu: n WebP streams (lossy, still, opaque) of one geometry -> out[n][h][w][3] on the device (out = nullptr: geometry
- * only, no device call) */
-int dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
-	StreamGeometry *g, cudaStream_t s);
+ * only, no device call); scale != 1: libwebp's scaled decode to rint(w * scale) x rint(h * scale) */
+int dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, double scale, void *out, size_t out_bpl,
+	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s);
 bool webp_signature(const void *buf, size_t len); /* RIFF, 4 bytes, WEBP */
 /* webp.cu: the ICCP chunk of a VP8X stream (empty: none) */
 int webp_icc_profile(const char *domain, const unsigned char *d, size_t len, std::vector<unsigned char> *profile);

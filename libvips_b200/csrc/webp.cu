@@ -26,10 +26,14 @@
  *                       dependencies, the same wavefront again, in place
  *   webp_rgb_kernel     one thread per pixel, only once every frame of the chunk has decoded clean: libwebp's fancy
  *                       upsampler and its 14-bit YUV -> RGB, cropped to w x h, written at the caller's stride
+ *   webp_scaled_rgb_kernel  in its place for vips_webpload_buffer's `scale` (libwebp's scaled decode, webp2vips.c:630-634):
+ *                       one thread per output pixel, its Y, U and V samples from libwebp's rescaler in closed form, then
+ *                       the same YUV -> RGB; the reconstruction then skips the filter pass when libwebp bypasses it
  * The per-symbol, per-block and per-pixel code is __host__ __device__: vb200_debug_webp_decode runs it on the CPU in raster
  * order, so that the CPU test-suite pins it against libwebp without a GPU.
  */
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1188,6 +1192,15 @@ yuv_clip8(int v)
 	return (v & ~16383) == 0 ? v >> 6 : v < 0 ? 0 : 255;
 }
 
+/* libwebp's 14-bit fixed-point YUV -> RGB of one pixel (VP8YuvToRgb) */
+VB_HD void
+webp_yuv_rgb(int Y, int u, int v, unsigned char *dst)
+{
+	dst[0] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) + mult_hi(v, 26149) - 14234);
+	dst[1] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) - mult_hi(u, 6419) - mult_hi(v, 13320) + 8708);
+	dst[2] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) + mult_hi(u, 33050) - 17685);
+}
+
 /* Pixel (x, y) of a w x h frame: libwebp's fancy upsampler (each output row pair between two chroma rows, the (9, 3, 3, 1)
  * taps, the first and an even height's last row on one chroma row, an even width's last column on one chroma column),
  * then its 14-bit fixed-point YUV -> RGB.
@@ -1231,10 +1244,361 @@ webp_rgb_pixel(const Planes &P, int w, int h, int x, int y, unsigned char *dst)
 				uv[c] = top_line ? (d03 + t) >> 1 : (d12 + cc) >> 1;
 		}
 	}
-	const int Y = P.y[(size_t) y * P.ys + x], u = uv[0], v = uv[1];
-	dst[0] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) + mult_hi(v, 26149) - 14234);
-	dst[1] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) - mult_hi(u, 6419) - mult_hi(v, 13320) + 8708);
-	dst[2] = (unsigned char) yuv_clip8(mult_hi(Y, 19077) + mult_hi(u, 33050) - 17685);
+	webp_yuv_rgb(P.y[(size_t) y * P.ys + x], uv[0], uv[1], dst);
+}
+
+/* ------------------------------------------------------------------ libwebp's rescaler (the scaled decode)
+ *
+ * With options.use_scaling (what webpload asks for at scale != 1, webp2vips.c:630-634) libwebp skips the upsampler: three
+ * WebPRescalers take Y (W x H) and U and V ((W + 1) / 2 x (H + 1) / 2) each to sw x sh, and every output pixel is the 14-bit
+ * YUV -> RGB of its three samples.  Each axis either shrinks (src >= dst: an area average with a fractional carry into
+ * the next output) or expands (src < dst: linear interpolation), all in 32-bit fixed point.
+ *
+ * libwebp streams rows through the rescaler, but every output sample has a closed form over a window of source pixels:
+ * the horizontal carry into column x is MULT_FIX(frac, fx_scale) of one boundary pixel, the vertical carry into row y is
+ * MULT_FIX_FLOOR(frow, yscale) of one boundary row, and the sums are uint32 that wrap, so the order of additions does not
+ * matter.  RescaleTap tables hold each output index's window; rescale_sample evaluates one sample from them alone.
+ */
+
+constexpr unsigned long long RESCALER_ONE = 1ull << 32, RESCALER_ROUNDER = RESCALER_ONE >> 1;
+
+VB_HD unsigned
+mult_fix(unsigned x, unsigned y)
+{
+	return (unsigned) (((unsigned long long) x * y + RESCALER_ROUNDER) >> 32);
+}
+
+VB_HD unsigned
+mult_fix_floor(unsigned x, unsigned y)
+{
+	return (unsigned) (((unsigned long long) x * y) >> 32);
+}
+
+unsigned
+rescaler_frac(unsigned long long x, unsigned long long y)
+{
+	return (unsigned) ((x << 32) / y);
+}
+
+/* one plane's WebPRescalerInit: the increments and fixed-point scales of src_w x src_h -> dst_w x dst_h */
+struct RescaleParams {
+	int x_expand, y_expand;
+	unsigned x_add, x_sub, y_add, y_sub;
+	unsigned fx_scale, fy_scale, fxy_scale;
+	int src_w, src_h, dst_w, dst_h;
+};
+
+RescaleParams
+rescale_params(int src_w, int src_h, int dst_w, int dst_h)
+{
+	RescaleParams p{};
+	p.src_w = src_w;
+	p.src_h = src_h;
+	p.dst_w = dst_w;
+	p.dst_h = dst_h;
+	p.x_expand = src_w < dst_w;
+	p.y_expand = src_h < dst_h;
+	/* expanding, the increments are the gaps between the first and last samples: bilinear interpolation */
+	p.x_add = p.x_expand ? dst_w - 1 : src_w;
+	p.x_sub = p.x_expand ? src_w - 1 : dst_w;
+	p.y_add = p.y_expand ? src_h - 1 : src_h;
+	p.y_sub = p.y_expand ? dst_h - 1 : dst_h;
+	if (!p.x_expand)
+		p.fx_scale = rescaler_frac(1, p.x_sub);
+	if (!p.y_expand) {
+		/* dst_h / (x_add * y_add) is 1.0 only for a 1-pixel-wide source kept at its height: fxy_scale 0 marks the copy */
+		const unsigned long long ratio = (unsigned long long) dst_h * RESCALER_ONE / ((unsigned long long) p.x_add * p.y_add);
+		p.fxy_scale = ratio != (unsigned) ratio ? 0 : (unsigned) ratio;
+		p.fy_scale = rescaler_frac(1, p.y_sub);
+	}
+	else
+		p.fy_scale = rescaler_frac(1, p.x_add);
+	return p;
+}
+
+/* One output index's window on one axis:
+ *   shrink  i0 the first source index, i1 the count; w0 the carry's multiplier of source i0 - 1 (0: none), w1 the
+ *           multiplier taken off the last source (horizontally -accum, vertically yscale = fy_scale * -y_accum)
+ *   expand  horizontally i0 / i1 the left and right sources and w0 the accumulator; vertically i0 / i1 the previous and
+ *           the current row and w0 the previous row's weight B (0: the current row alone)
+ */
+struct RescaleTap {
+	int i0, i1;
+	unsigned w0, w1;
+};
+
+/* the taps of one axis, from the accumulators' walk in ImportRowShrink / ImportRowExpand (horizontal) or WebPRescalerImport
+ * and the two ExportRow forms (vertical) */
+void
+rescale_taps(const RescaleParams &p, bool vertical, RescaleTap *t)
+{
+	const int expand = vertical ? p.y_expand : p.x_expand, dst = vertical ? p.dst_h : p.dst_w, src = vertical ? p.src_h : p.src_w;
+	const int add = (int) (vertical ? p.y_add : p.x_add), sub = (int) (vertical ? p.y_sub : p.x_sub);
+	if (!expand) {
+		int accum = vertical ? add : 0, at = 0;
+		unsigned carry = 0;
+		for (int o = 0; o < dst; o++) {
+			RescaleTap &k = t[o];
+			k.i0 = at;
+			k.w0 = carry;
+			if (!vertical)
+				accum += add;
+			int n = 0;
+			while (accum > 0) {
+				accum -= sub;
+				at++;
+				n++;
+			}
+			k.i1 = n;
+			k.w1 = vertical ? p.fy_scale * (unsigned) -accum : (unsigned) -accum;
+			carry = k.w1;
+			if (vertical)
+				accum += add;
+		}
+		return;
+	}
+	if (!vertical) {
+		int accum = add, l = 0, r = src > 1 ? 1 : 0;
+		for (int o = 0; o < dst; o++) {
+			t[o] = RescaleTap{l, r, (unsigned) accum, 0};
+			accum -= sub;
+			if (accum < 0 && o + 1 < dst) {
+				l = r++;
+				accum += add;
+			}
+		}
+		return;
+	}
+	int accum = sub, prev = 0, cur = -1;
+	for (int o = 0; o < dst; o++) {
+		while (accum > 0) {
+			prev = cur < 0 ? 0 : cur;
+			cur++;
+			accum -= sub;
+		}
+		t[o] = RescaleTap{prev, cur, accum == 0 ? 0u : rescaler_frac((unsigned) -accum, (unsigned) sub), 0};
+		accum += add;
+	}
+}
+
+/* the horizontal pass of source row `row` at one output column: ImportRowExpand's interpolation or ImportRowShrink's sum
+ * times x_sub, less the fraction of the last pixel, plus the carry from the previous column */
+VB_HD unsigned
+rescale_h(const unsigned char *row, const RescaleParams &p, const RescaleTap &t)
+{
+	if (p.x_expand) {
+		const unsigned left = row[t.i0], right = row[t.i1];
+		return right * p.x_add + (left - right) * t.w0;
+	}
+	unsigned sum = t.w0 ? mult_fix(row[t.i0 - 1] * t.w0, p.fx_scale) : 0u, base = 0;
+	for (int k = 0; k < t.i1; k++) {
+		base = row[t.i0 + k];
+		sum += base;
+	}
+	return sum * p.x_sub - base * t.w1;
+}
+
+/* One rescaled sample of a plane: the vertical pass (ExportRowExpand, or ExportRowShrink with its carry) over rescale_h's
+ * rows, clipped as WebPRescalerExportRow clips. */
+VB_HD unsigned char
+rescale_sample(const unsigned char *plane, size_t stride, const RescaleParams &p, const RescaleTap &tx, const RescaleTap &ty)
+{
+	int v;
+	if (p.y_expand) {
+		const unsigned f = rescale_h(plane + (size_t) ty.i1 * stride, p, tx);
+		unsigned J = f;
+		if (ty.w0) {
+			const unsigned i = rescale_h(plane + (size_t) ty.i0 * stride, p, tx);
+			const unsigned long long I = (unsigned long long) (unsigned) (RESCALER_ONE - ty.w0) * f + (unsigned long long) ty.w0 * i;
+			J = (unsigned) ((I + RESCALER_ROUNDER) >> 32);
+		}
+		v = (int) mult_fix(J, p.fy_scale);
+	}
+	else {
+		unsigned irow = ty.w0 ? mult_fix_floor(rescale_h(plane + (size_t) (ty.i0 - 1) * stride, p, tx), ty.w0) : 0u, f = 0;
+		for (int k = 0; k < ty.i1; k++) {
+			f = rescale_h(plane + (size_t) (ty.i0 + k) * stride, p, tx);
+			irow += f;
+		}
+		if (!p.fxy_scale)
+			return (unsigned char) irow;
+		v = (int) mult_fix(ty.w1 ? irow - mult_fix_floor(f, ty.w1) : irow, p.fxy_scale);
+	}
+	return v > 255 ? 255 : (unsigned char) v;
+}
+
+/* A batch's scaled decode: its output size, whether the loop filter is bypassed, and the Y and U / V rescalers' constants and
+ * taps (taps: Y across [sw], Y down [sh], U / V across [sw], U / V down [sh], one after another). */
+struct WebpScale {
+	int sw = 0, sh = 0, bypass = 0;
+	RescaleParams y{}, uv{};
+	std::vector<RescaleTap> taps;
+};
+
+/* webpload at scale: webp2vips.c:513-514 rounds the frame to rint(w * scale) x rint(h * scale) and refuses an axis outside
+ * 1 .. 16383 (:541-552), webpload.c:189-193 limits scale to [0, 1024]; libwebp then bypasses the loop filter when both axes
+ * shrink below three quarters (WebPIoInitFromOptions) */
+int
+webp_scale_geometry(const char *domain, int w, int h, double scale, WebpScale *S)
+{
+	if (!(scale >= 0 && scale <= 1024)) {
+		error(domain, "scale %g is outside webpload's range 0 to 1024", scale);
+		return -1;
+	}
+	const double fw = rint(w * scale), fh = rint(h * scale);
+	if (fw <= 0 || fh <= 0 || fw > 0x3FFF || fh > 0x3FFF) {
+		error(domain, "bad image dimensions: %d x %d at scale %g is %.0f x %.0f", w, h, scale, fw, fh);
+		return -1;
+	}
+	S->sw = (int) fw;
+	S->sh = (int) fh;
+	S->bypass = S->sw < w * 3 / 4 && S->sh < h * 3 / 4;
+	S->y = rescale_params(w, h, S->sw, S->sh);
+	S->uv = rescale_params((w + 1) >> 1, (h + 1) >> 1, S->sw, S->sh);
+	return 0;
+}
+
+void
+webp_scale_taps(WebpScale *S)
+{
+	const int sw = S->sw, sh = S->sh;
+	S->taps.resize(2 * ((size_t) sw + sh));
+	rescale_taps(S->y, false, S->taps.data());
+	rescale_taps(S->y, true, S->taps.data() + sw);
+	rescale_taps(S->uv, false, S->taps.data() + sw + sh);
+	rescale_taps(S->uv, true, S->taps.data() + 2 * sw + sh);
+}
+
+/* libwebp's WebPRescaler as it runs, for the host twin: rows imported one at a time into frow (and summed into irow, or
+ * swapped with it when expanding), an output row exported whenever y_accum has gone to 0 or below.  Written from the
+ * streaming form, independently of the closed form above, which the test-suite checks against it. */
+struct RowRescaler {
+	RescaleParams p;
+	int y_accum, dst_y = 0;
+	std::vector<unsigned> irow, frow;
+	std::vector<unsigned char> out; /* the last exported row */
+
+	explicit RowRescaler(const RescaleParams &q) : p(q), y_accum(q.y_expand ? (int) q.y_sub : (int) q.y_add), irow(q.dst_w, 0), frow(q.dst_w, 0), out(q.dst_w)
+	{
+	}
+	bool
+	pending() const
+	{
+		return dst_y < p.dst_h && y_accum <= 0;
+	}
+	int
+	needed_lines(int max_lines) const
+	{
+		const int k = (y_accum + (int) p.y_sub - 1) / (int) p.y_sub;
+		return k > max_lines ? max_lines : k;
+	}
+	void
+	import_row(const unsigned char *src)
+	{
+		if (!p.x_expand) {
+			unsigned sum = 0;
+			int accum = 0, x_in = 0;
+			for (int x = 0; x < p.dst_w; x++) {
+				unsigned base = 0;
+				accum += (int) p.x_add;
+				while (accum > 0) {
+					accum -= (int) p.x_sub;
+					base = src[x_in++];
+					sum += base;
+				}
+				const unsigned frac = base * (unsigned) -accum;
+				frow[x] = sum * p.x_sub - frac;
+				sum = mult_fix(frac, p.fx_scale);
+			}
+			return;
+		}
+		int accum = (int) p.x_add, x_in = 0;
+		unsigned left = src[0], right = p.src_w > 1 ? src[1] : left;
+		x_in++;
+		for (int x = 0;;) {
+			frow[x] = right * p.x_add + (left - right) * (unsigned) accum;
+			if (++x >= p.dst_w)
+				break;
+			accum -= (int) p.x_sub;
+			if (accum < 0) {
+				left = right;
+				right = src[++x_in];
+				accum += (int) p.x_add;
+			}
+		}
+	}
+	/* WebPRescalerImport: up to n rows while no output is pending */
+	int
+	import(int n, const unsigned char *src, size_t stride)
+	{
+		int k = 0;
+		for (; k < n && !pending(); k++, src += stride) {
+			if (p.y_expand)
+				irow.swap(frow);
+			import_row(src);
+			if (!p.y_expand)
+				for (int x = 0; x < p.dst_w; x++)
+					irow[x] += frow[x];
+			y_accum -= (int) p.y_sub;
+		}
+		return k;
+	}
+	void
+	export_row()
+	{
+		for (int x = 0; x < p.dst_w; x++) {
+			int v;
+			if (p.y_expand) {
+				unsigned J = frow[x];
+				if (y_accum != 0) {
+					const unsigned B = rescaler_frac((unsigned) -y_accum, p.y_sub), A = (unsigned) (RESCALER_ONE - B);
+					J = (unsigned) (((unsigned long long) A * frow[x] + (unsigned long long) B * irow[x] + RESCALER_ROUNDER) >> 32);
+				}
+				v = (int) mult_fix(J, p.fy_scale);
+			}
+			else if (!p.fxy_scale) {
+				out[x] = (unsigned char) irow[x];
+				irow[x] = 0;
+				continue;
+			}
+			else {
+				const unsigned yscale = p.fy_scale * (unsigned) -y_accum;
+				const unsigned frac = yscale ? mult_fix_floor(frow[x], yscale) : 0u;
+				v = (int) mult_fix(irow[x] - frac, p.fxy_scale);
+				irow[x] = frac;
+			}
+			out[x] = v > 255 ? 255 : (unsigned char) v;
+		}
+		y_accum += (int) p.y_add;
+		dst_y++;
+	}
+};
+
+/* EmitRescaledRGB over a whole frame: Y rows in, U and V rows as the U rescaler needs them, and an RGB row out whenever Y
+ * and U both have one pending; out is sw x sh x 3 at out_bpl.  0, or -1 if the rows run out before the last output row. */
+int
+rescale_frame_rows(const Planes &P, int h, const WebpScale &S, unsigned char *out, size_t out_bpl)
+{
+	RowRescaler ry(S.y), ru(S.uv), rv(S.uv);
+	const int uv_h = (h + 1) >> 1;
+	int j = 0, uv_j = 0, y_out = 0;
+	while (j < h) {
+		j += ry.import(h - j, P.y + (size_t) j * P.ys, P.ys);
+		if (ru.needed_lines(uv_h - uv_j) > 0) {
+			const int k = ru.import(uv_h - uv_j, P.u + (size_t) uv_j * P.uvs, P.uvs);
+			rv.import(uv_h - uv_j, P.v + (size_t) uv_j * P.uvs, P.uvs);
+			uv_j += k;
+		}
+		for (; ry.pending() && ru.pending(); y_out++) {
+			ry.export_row();
+			ru.export_row();
+			rv.export_row();
+			unsigned char *o = out + (size_t) y_out * out_bpl;
+			for (int x = 0; x < S.sw; x++)
+				webp_yuv_rgb(ry.out[x], ru.out[x], rv.out[x], o + 3 * x);
+		}
+	}
+	return y_out == S.sh ? 0 : -1;
 }
 
 /* ------------------------------------------------------------------ the device pipeline */
@@ -1343,10 +1707,10 @@ webp_token_kernel(const WebpFrameDev *frames, int n, const unsigned char *data, 
 
 /* One CTA per frame.  Macroblock (x, y) needs (x - 1, y) and (x + 1, y - 1) done first, for prediction and for the filter
  * alike, so the CTA walks the diagonals x + 2y = t, one thread per macroblock of a diagonal: first reconstructing every
- * macroblock, then filtering them in place.
+ * macroblock, then filtering them in place.  bypass: the scaled decode's filter bypass, one pass only.
  */
 __global__ void __launch_bounds__(256)
-webp_recon_kernel(const WebpFrameDev *frames, unsigned char *scratch, const int *status)
+webp_recon_kernel(const WebpFrameDev *frames, unsigned char *scratch, const int *status, int bypass)
 {
 	const int i = blockIdx.x;
 	if (status[i])
@@ -1359,7 +1723,7 @@ webp_recon_kernel(const WebpFrameDev *frames, unsigned char *scratch, const int 
 	const short *coef = (const short *) (s + L.coef);
 	const Planes P = layout_planes(L, s, F.mb_w);
 	const int steps = F.mb_w + 2 * (F.mb_h - 1);
-	for (int pass = 0; pass < (H->filter_type ? 2 : 1); pass++)
+	for (int pass = 0; pass < (H->filter_type && !bypass ? 2 : 1); pass++)
 		for (int t = 0; t < steps; t++) {
 			/* y from max(0, ceil((t - mb_w + 1) / 2)) to min(mb_h - 1, t / 2) */
 			const int y0 = t >= F.mb_w ? (t - F.mb_w + 2) >> 1 : 0, y1 = min(F.mb_h - 1, t >> 1);
@@ -1386,6 +1750,35 @@ webp_rgb_kernel(const WebpFrameDev *frames, unsigned char *scratch, unsigned cha
 	unsigned char *o = out + (size_t) blockIdx.z * out_frame_stride;
 	for (int y = blockIdx.y; y < F.h; y += gridDim.y)
 		webp_rgb_pixel(P, F.w, F.h, x, y, o + (size_t) y * out_bpl + (size_t) x * 3);
+}
+
+/* the scaled decode's constants as the output kernel takes them: the two rescalers and their taps in device memory */
+struct WebpScaleDev {
+	RescaleParams y, uv;
+	const RescaleTap *yx, *yy, *uvx, *uvy;
+	int sw, sh;
+};
+
+/* The scaled decode's output, one thread per output pixel: its Y, U and V samples each in closed form from the planes
+ * (rescale_sample), then libwebp's YUV -> RGB, written straight into out. */
+__global__ void
+webp_scaled_rgb_kernel(const WebpFrameDev *frames, unsigned char *scratch, WebpScaleDev S, unsigned char *out, size_t out_bpl,
+	size_t out_frame_stride)
+{
+	const WebpFrameDev F = frames[blockIdx.z];
+	const int x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= S.sw)
+		return;
+	const Planes P = layout_planes(scratch_layout(F.mb_w, F.mb_h), scratch + F.scratch_off, F.mb_w);
+	const RescaleTap yx = S.yx[x], uvx = S.uvx[x];
+	unsigned char *o = out + (size_t) blockIdx.z * out_frame_stride + (size_t) x * 3;
+	for (int y = blockIdx.y; y < S.sh; y += gridDim.y) {
+		const RescaleTap yy = S.yy[y], uvy = S.uvy[y];
+		const int Y = rescale_sample(P.y, P.ys, S.y, yx, yy);
+		const int u = rescale_sample(P.u, P.uvs, S.uv, uvx, uvy);
+		const int v = rescale_sample(P.v, P.uvs, S.uv, uvx, uvy);
+		webp_yuv_rgb(Y, u, v, o + (size_t) y * out_bpl);
+	}
 }
 
 /* ------------------------------------------------------------------ the container, on the host */
@@ -1582,26 +1975,52 @@ webp_icc_profile(const char *domain, const unsigned char *d, size_t len, std::ve
  * geometry).  Containers and frame tags are read on the host workers; the frames go up in chunks bounded by device
  * memory, each one pinned block (frame records and VP8 data) copied to the device and decoded on s.  Every frame of a
  * chunk must decode clean before its pixels are converted into out; the call returns when they are.
+ *
+ * scale != 1 is libwebp's scaled decode at webpload's rounding: the frames must share one source size, g is the scaled
+ * size, the loop filter is bypassed when both axes shrink below three quarters, and webp_scaled_rgb_kernel writes the
+ * rescaled pixels straight into out from the planes (so a chunk still holds only VP8 data and planes), with the taps
+ * uploaded once for the batch.
  */
 int
-dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, void *out, size_t out_bpl, size_t out_frame_stride,
-	StreamGeometry *g, cudaStream_t s)
+dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t *lens, int n, double scale, void *out, size_t out_bpl,
+	size_t out_frame_stride, StreamGeometry *g, cudaStream_t s)
 {
 	std::vector<WebpHeader> hdr(n);
 	if (parse_streams(
 			domain, "frame", n, [&](int i) { return parse_webp(domain, (const unsigned char *) bufs[i], lens[i], &hdr[i]); },
 			[&](int i) { return StreamGeometry{hdr[i].w, hdr[i].h, 3, 0}; }, g))
 		return -1;
+	const int W = g->w, Hh = g->h, mb_w = (W + 15) >> 4, mb_h = (Hh + 15) >> 4;
+	const bool scaled = scale != 1.0;
+	WebpScale S;
+	if (scaled) {
+		if (webp_scale_geometry(domain, W, Hh, scale, &S))
+			return -1;
+		g->w = S.sw;
+		g->h = S.sh;
+	}
 	if (!out)
 		return 0;
 	if (check_out_strides(domain, *g, out_bpl, out_frame_stride))
 		return -1;
-	const int W = g->w, Hh = g->h, mb_w = (W + 15) >> 4, mb_h = (Hh + 15) >> 4;
+	WebpScaleDev SD{};
+	RescaleTap *taps = nullptr;
+	if (scaled) {
+		webp_scale_taps(&S);
+		const size_t bytes = S.taps.size() * sizeof(RescaleTap);
+		if (dev_alloc(domain, (void **) &taps, bytes, s))
+			return -1;
+		if (cudaMemcpyAsync(taps, S.taps.data(), bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+			dev_free(taps, s);
+			return cuda_fail(domain, cudaGetLastError(), "webp rescaler taps");
+		}
+		SD = WebpScaleDev{S.y, S.uv, taps, taps + S.sw, taps + S.sw + S.sh, taps + 2 * S.sw + S.sh, S.sw, S.sh};
+	}
 	const size_t scratch_bytes = align16(scratch_layout(mb_w, mb_h).total);
 	WebpTimer timer;
 	for (float &t : t_webp_ms)
 		t = timer.on ? 0.f : -1.f;
-	return decode_chunks(domain, "webp", "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
+	const int rc = decode_chunks(domain, "webp", "frame", n, [&](int i) { return frame_device_bytes(hdr[i]); }, [&](int c0, int cn) {
 		/* the block: records and VP8 data staged; each frame's macroblock scratch */
 		std::vector<WebpFrameDev> F(cn);
 		size_t data = 0;
@@ -1627,34 +2046,47 @@ dev_webp_decode_batch(const char *domain, const void *const *bufs, const size_t 
 				timer.mark(1, s);
 				webp_token_kernel<<<(cn + 63) / 64, 64, 0, s>>>(dF, cn, dev + off_data, dS, status);
 				timer.mark(2, s);
-				webp_recon_kernel<<<cn, threads, 0, s>>>(dF, dS, status);
+				webp_recon_kernel<<<cn, threads, 0, s>>>(dF, dS, status, S.bypass);
 				timer.mark(3, s);
 				return 3;
 			},
 			[&](int i, int st) { error(domain, "frame %d: %s", c0 + i, werr_text(st)); },
 			[&](unsigned char *dev) {
-				webp_rgb_kernel<<<dim3((W + 127) / 128, std::min(Hh, kMaxGridY), cn), 128, 0, s>>>((const WebpFrameDev *) dev, dev + align16(total),
-					(unsigned char *) out + (size_t) c0 * out_frame_stride, out_bpl, out_frame_stride);
+				unsigned char *o = (unsigned char *) out + (size_t) c0 * out_frame_stride;
+				if (scaled)
+					webp_scaled_rgb_kernel<<<dim3((S.sw + 127) / 128, std::min(S.sh, kMaxGridY), cn), 128, 0, s>>>((const WebpFrameDev *) dev,
+						dev + align16(total), SD, o, out_bpl, out_frame_stride);
+				else
+					webp_rgb_kernel<<<dim3((W + 127) / 128, std::min(Hh, kMaxGridY), cn), 128, 0, s>>>((const WebpFrameDev *) dev, dev + align16(total),
+						o, out_bpl, out_frame_stride);
 				timer.mark(4, s);
 				timer.add();
 				return 1;
 			},
 			s);
 	}, s);
+	if (taps)
+		dev_free(taps, s);
+	return rc;
 }
 
 /* the same decode on the CPU through the same per-symbol, per-block and per-pixel code, in raster order: the test-suite's
- * host twin */
+ * host twin.  At scale != 1 the planes go through RowRescaler in libwebp's row order instead of the closed form. */
 int
-host_webp_decode(const char *domain, const void *buf, size_t len, unsigned char *out, size_t out_bpl, int *out_w, int *out_h, int *out_bands)
+host_webp_decode(const char *domain, const void *buf, size_t len, double scale, unsigned char *out, size_t out_bpl, int *out_w, int *out_h,
+	int *out_bands)
 {
 	WebpHeader W;
 	if (parse_webp(domain, (const unsigned char *) buf, len, &W))
 		return -1;
+	WebpScale S;
+	const bool scaled = scale != 1.0;
+	if (scaled && webp_scale_geometry(domain, W.w, W.h, scale, &S))
+		return -1;
 	if (out_w)
-		*out_w = W.w;
+		*out_w = scaled ? S.sw : W.w;
 	if (out_h)
-		*out_h = W.h;
+		*out_h = scaled ? S.sh : W.h;
 	if (out_bands)
 		*out_bands = 3;
 	if (!out)
@@ -1698,10 +2130,17 @@ host_webp_decode(const char *domain, const void *buf, size_t len, unsigned char 
 	for (int y = 0; y < mb_h; y++)
 		for (int x = 0; x < mb_w; x++)
 			webp_recon_mb(mbs[(size_t) y * mb_w + x], &coef[((size_t) y * mb_w + x) * 384], x, y, mb_w, P);
-	if (H.filter_type)
+	if (H.filter_type && !S.bypass)
 		for (int y = 0; y < mb_h; y++)
 			for (int x = 0; x < mb_w; x++)
 				webp_filter_mb(H, mbs[(size_t) y * mb_w + x], x, y, P);
+	if (scaled) {
+		if (rescale_frame_rows(P, W.h, S, out, out_bpl)) {
+			error(domain, "the rescaler ran out of rows");
+			return -1;
+		}
+		return 0;
+	}
 	for (int y = 0; y < W.h; y++)
 		for (int x = 0; x < W.w; x++)
 			webp_rgb_pixel(P, W.w, W.h, x, y, out + (size_t) y * out_bpl + (size_t) x * 3);
@@ -1717,7 +2156,7 @@ using namespace vb200;
 extern "C" int
 vb200_webp_geometry(const void *buf, size_t len, int *width, int *height, int *bands)
 {
-	return host_webp_decode("webp_geometry", buf, len, nullptr, 0, width, height, bands);
+	return host_webp_decode("webp_geometry", buf, len, 1.0, nullptr, 0, width, height, bands);
 }
 
 extern "C" int
@@ -1727,11 +2166,78 @@ vb200_webp_decode_batch(const void *const *bufs, const size_t *lens, int n, void
 	return decode_batch_abi("webp_decode_batch", {STREAM_WEBP}, bufs, lens, n, out, out_location, out_bpl, out_frame_stride, width, height, bands);
 }
 
+static DecodeRequest
+webp_request(double scale)
+{
+	DecodeRequest req{STREAM_WEBP};
+	req.scale = scale;
+	return req;
+}
+
+extern "C" int
+vb200_webp_decode_batch_scaled(const void *const *bufs, const size_t *lens, int n, double scale, void *out, int out_location, size_t out_bpl,
+	size_t out_frame_stride, int *width, int *height, int *bands)
+{
+	return decode_batch_abi("webp_decode_batch", webp_request(scale), bufs, lens, n, out, out_location, out_bpl, out_frame_stride, width, height,
+		bands);
+}
+
 /* reference: vips_webpload_buffer(buf, len, &out, NULL), foreign/webpload.c */
 extern "C" int
 vb200_webpload_buffer(const void *buf, size_t len, VB200Image *out)
 {
 	return load_abi("webpload_buffer", {STREAM_WEBP}, buf, len, out);
+}
+
+/* reference: vips_webpload_buffer(buf, len, &out, "scale", scale, NULL) */
+extern "C" int
+vb200_webpload_buffer_scaled(const void *buf, size_t len, double scale, VB200Image *out)
+{
+	return load_abi("webpload_buffer", webp_request(scale), buf, len, out);
+}
+
+extern "C" int
+vb200_debug_webp_decode_scaled(const void *buf, size_t len, double scale, void *out, size_t out_bpl, int *width, int *height, int *bands)
+{
+	return host_twin_abi("webp_decode (host twin)",
+		[&](const char *domain) { return host_webp_decode(domain, buf, len, scale, (unsigned char *) out, out_bpl, width, height, bands); });
+}
+
+/* One plane of src_w x src_h (stride bytes a row) rescaled to dst_w x dst_h into out (out_bpl a row): closed_form set, by
+ * rescale_sample over the taps, sample by sample, as webp_scaled_rgb_kernel runs it; otherwise by RowRescaler in row order. */
+extern "C" int
+vb200_debug_webp_rescale(const void *plane, size_t stride, int src_w, int src_h, int dst_w, int dst_h, int closed_form, void *out, size_t out_bpl)
+{
+	if (!plane || !out || src_w < 1 || src_h < 1 || dst_w < 1 || dst_h < 1 || stride < (size_t) src_w || out_bpl < (size_t) dst_w) {
+		error("debug_webp_rescale", "bad arguments");
+		return -1;
+	}
+	const unsigned char *src = (const unsigned char *) plane;
+	unsigned char *dst = (unsigned char *) out;
+	const RescaleParams p = rescale_params(src_w, src_h, dst_w, dst_h);
+	if (closed_form) {
+		std::vector<RescaleTap> tx(dst_w), ty(dst_h);
+		rescale_taps(p, false, tx.data());
+		rescale_taps(p, true, ty.data());
+		for (int y = 0; y < dst_h; y++)
+			for (int x = 0; x < dst_w; x++)
+				dst[(size_t) y * out_bpl + x] = rescale_sample(src, stride, p, tx[x], ty[y]);
+		return 0;
+	}
+	RowRescaler r(p);
+	int j = 0;
+	while (r.dst_y < dst_h) {
+		j += r.import(src_h - j, src + (size_t) j * stride, stride);
+		if (!r.pending()) {
+			error("debug_webp_rescale", "the rescaler ran out of rows");
+			return -1;
+		}
+		while (r.pending()) {
+			r.export_row();
+			memcpy(dst + (size_t) (r.dst_y - 1) * out_bpl, r.out.data(), dst_w);
+		}
+	}
+	return 0;
 }
 
 extern "C" int
@@ -1745,7 +2251,7 @@ extern "C" int
 vb200_debug_webp_decode(const void *buf, size_t len, void *out, size_t out_bpl, int *width, int *height, int *bands)
 {
 	return host_twin_abi("webp_decode (host twin)",
-		[&](const char *domain) { return host_webp_decode(domain, buf, len, (unsigned char *) out, out_bpl, width, height, bands); });
+		[&](const char *domain) { return host_webp_decode(domain, buf, len, 1.0, (unsigned char *) out, out_bpl, width, height, bands); });
 }
 
 /* ms[4]: the last batch's device milliseconds in the header, token, reconstruction and RGB kernels on this thread, with
